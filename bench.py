@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- env-steps/s of the batched RAMP cluster simulator hot path on B200.
+"""bench.py -- env-steps/s of the batched RAMP cluster simulator hot path on one or more GPUs.
 
     python bench.py --gpus N --steps K --warmup W            # product arm (CUDA kernels through the C ABI)
     python bench.py --impl reference --gpus N --steps K ...   # CPU arm: the unmodified Python reference (oracle/_ref), one
@@ -11,7 +11,9 @@ One bench "step" = one batched env-step: every one of the B episodes takes one a
 all episodes are reset (which clears the per-episode memo tables like RCE:269-275), so the timed region
 contains resets, memo misses (lookaheads executed) and memo hits in the proportion a real rollout has.
 
-Prints ONE JSON line (rank 0).  See README / DESIGN.md for the field definitions.
+Prints ONE JSON line (rank 0).  See README / DESIGN.md for the field definitions.  --dump-outputs DIR also writes what the
+timed path returned in its last timed step (step statistics, cluster steps, episode state) as DIR/<name>.npy, so that two
+builds run with the same arguments -- hence the same seeded inputs -- can be compared output for output.
 """
 import argparse
 import json
@@ -66,6 +68,9 @@ def parse_args():
     ap.add_argument('--gather-every', type=int, default=0,
                     help='all-gather the episode metrics every this many steps (0 = once per scripted segment, i.e. per batch of rollouts)')
     ap.add_argument('--no-batched-env', action='store_true', help='skip the BatchedRampJobPartitioningEnvironment secondary figure')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step as DIR/<name>.npy (float64; at most 64 MB, a seeded sample of '
+                         'episodes beyond that)')
     return ap.parse_args()
 
 
@@ -111,8 +116,7 @@ def workload_config(args, cfg, templates, world, B):
 
 # ---------------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """Samples SM clocks / throttle reasons during the timed region (B200_PROFILING.md recipe): NVML when importable,
-    else the nvidia-smi query line."""
+    """Samples SM clocks / throttle reasons during the timed region: NVML when importable, else the nvidia-smi query line."""
 
     Q = ('clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
          'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
@@ -178,22 +182,41 @@ def measured_peaks():
             return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'data sheet (H100 SXM HBM3, 3.35 TB/s at 700 W), not a measurement'
 
 
-def ncu_profile_summary():
-    """STATIC figures from the committed ncu capture of this bench command (profiles/r2_ncu_thread_summary.json, written by
-    scripts/ncu_summary.py): DRAM bytes per lookahead launch and warp instructions per lookahead.  Not measured in this run --
-    counters need ncu, and a number taken under a profiler is never a bench value -- so they carry their source."""
-    p = os.path.join(ROOT, 'profiles', 'r2_ncu_thread_summary.json')
-    if os.path.exists(p):
-        try:
-            d = json.load(open(p))
-            return {'dram_bytes_per_launch': d.get('dram_bytes_per_launch'), 'warp_inst_per_lookahead': d.get('warp_inst_per_lookahead'),
-                    'source': 'static, from profiles/r2_ncu_thread_summary.json'}
-        except Exception:
-            pass
-    return {'source': 'no committed ncu summary'}
+def device_info(index):
+    """Which card the numbers of this line were measured on: name, SM count and the power limit it was set to."""
+    import torch
+    p = torch.cuda.get_device_properties(index)
+    info = {'name': p.name, 'sm_count': p.multi_processor_count, 'total_memory_gb': round(p.total_memory / 1e9, 1)}
+    try:
+        out = subprocess.run(['nvidia-smi', '--query-gpu=power.limit,clocks.max.sm', '--format=csv,noheader,nounits', '-i', str(index)],
+                             capture_output=True, text=True, timeout=10).stdout.strip()
+        lim, mx = [x.strip() for x in out.split(',')]
+        info.update(power_limit_w=float(lim), sm_max_mhz=float(mx))
+    except Exception:
+        info.update(power_limit_w=None, sm_max_mhz=None)
+    return info
+
+
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(directory, arrays, seed, suffix=''):
+    """Writes each [B, ...] array as <directory>/<name><suffix>.npy in float64.  Over DUMP_MAX_BYTES in all, the same seeded
+    sample of episode rows is taken from every array (and written as episode_index) so that the dump stays comparable."""
+    os.makedirs(directory, exist_ok=True)
+    arrays = {k: np.ascontiguousarray(v, dtype=np.float64) for k, v in arrays.items()}
+    B = len(next(iter(arrays.values())))
+    row_bytes = sum(v.nbytes // max(len(v), 1) for v in arrays.values())
+    if B * row_bytes > DUMP_MAX_BYTES:
+        keep = max(1, (DUMP_MAX_BYTES - 8 * B) // (row_bytes + 8))
+        rows = np.sort(np.random.default_rng(seed).choice(B, size=keep, replace=False))
+        arrays = {k: v[rows] for k, v in arrays.items()}
+        arrays['episode_index'] = rows.astype(np.float64)
+    for k, v in arrays.items():
+        np.save(os.path.join(directory, f'{k}{suffix}.npy'), v)
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -460,6 +483,15 @@ def run_b200_arm(args, rank, world, local_rank):
     fold_memo()
     memo = dict(memo_acc)
     eng.check_status()
+    if args.dump_outputs:
+        # what step_device handed its caller in the last timed step, plus the episode state it leaves (read before the
+        # e2e leg below resets the episodes)
+        ep_last = torch.empty((B, engine.EP_LEN), dtype=torch.float64, device='cuda')
+        eng.export_episode_state_to(ep_last.data_ptr())
+        eng.sync()
+        dump_outputs(args.dump_outputs, {'step_stats': stats_dev.cpu().numpy(), 'n_cluster_steps': ncs_dev.cpu().numpy(),
+                                         'episode_state': ep_last.cpu().numpy()},
+                     seed=args.seed, suffix='' if rank == 0 else f'_rank{rank}')
     # the episode resets inside the loop synchronise the stream, so wall time ~ device time; use the larger
     elapsed_ms = max(dev_ms, 0.0)
     el = torch.tensor([elapsed_ms, t_wall * 1e3], dtype=torch.float64, device='cuda')
@@ -630,9 +662,7 @@ def run_b200_arm(args, rank, world, local_rank):
         peak, peak_src = measured_peaks()
         la_ms = kt['total_ms']
         achieved = (kt['algorithmic_bytes'] / 1e9) / (la_ms / 1e3) if la_ms > 0 else 0.0
-        prof = ncu_profile_summary()
         n_launch = max(kt['launches'], 1)
-        sm_mhz = (clocks or {}).get('sm_mhz') or 1965.0
         roofline = {
             'bound': 'hbm', 'kernel': 'ramp_lookahead_thread_kernel', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s',
             'frac': achieved / peak if peak else None, 'peak_source': peak_src,
@@ -641,18 +671,9 @@ def run_b200_arm(args, rank, world, local_rank):
             # what the kernel really touches: the symmetry quotient of each job (ramp_quotient.cpp), same formula on its sizes
             'achieved_on_quotient': (kt.get('quotient_bytes', 0) / 1e9) / (la_ms / 1e3) if la_ms > 0 else 0.0,
             'quotient_bytes_per_launch': kt.get('quotient_bytes', 0) / n_launch,
-            'traffic': prof.get('dram_bytes_per_launch'), 'traffic_source': prof.get('source'),
             'kernel_ms_per_launch': la_ms / n_launch, 'kernel_launches': kt['launches'],
             'lookaheads': kt['work_items'], 'kernel_share_of_step': la_ms / elapsed_ms if elapsed_ms else None,
-            'algorithmic_bytes_per_launch': kt['algorithmic_bytes'] / n_launch,
-            # the kernel is bound by the latency of dependent instructions of ONE thread per lookahead, not by bandwidth:
-            # warp instructions issued per second against the SM sub-partitions' issue slots (148 x 4 per cycle)
-            'issue_slots': {'warp_inst_per_lookahead': prof.get('warp_inst_per_lookahead'),
-                            'achieved_warp_inst_per_s': (prof.get('warp_inst_per_lookahead') or 0) * kt['work_items'] / 32.0 / (la_ms / 1e3) if la_ms > 0 else None,
-                            'peak_warp_inst_per_s': 148 * 4 * sm_mhz * 1e6, 'source': prof.get('source'),
-                            'note': '32 lookaheads share one warp: warp instructions = per-lookahead instructions x lookaheads / 32'}}
-        if roofline['issue_slots']['achieved_warp_inst_per_s']:
-            roofline['issue_slots']['frac'] = roofline['issue_slots']['achieved_warp_inst_per_s'] / roofline['issue_slots']['peak_warp_inst_per_s']
+            'algorithmic_bytes_per_launch': kt['algorithmic_bytes'] / n_launch}
         # end to end = the call a user makes.  Preferred: the batched gym-like surface on the device
         # (DeviceRampJobPartitioningEnvironment.step(actions[B]) -> obs, reward, done: actions host -> device, observation / reward /
         # done device -> host through page-locked arrays every step, placement + lowering lookup + rewards + observation inside).
@@ -671,7 +692,7 @@ def run_b200_arm(args, rank, world, local_rank):
         line = {
             'metric': METRIC, 'value': value, 'unit': UNIT, 'n_gpus': world, 'steps': K, 'warmup': W,
             'ms_per_step': elapsed_ms / K, 'higher_is_better': True, 'scaling': args.scaling, 'vs_baseline': None,
-            'dtype': 'f64', 'data': 'synthetic',
+            'dtype': 'f64', 'data': 'synthetic', 'device': device_info(local_rank),
             'config': workload_config(args, cfg, wl.templates, world, B),
             'trace_mb_per_step': _trace_mb(kt), 'gather_every_steps': gather_every if world > 1 else None,
             'e2e': e2e_line,

@@ -1,4 +1,4 @@
-"""Builds ddls_b200/libramp_b200.so (the C-ABI shared library) with nvcc for sm_100a, in-tree."""
+"""Builds ddls_b200/libramp_b200.so (the C-ABI shared library) with nvcc for sm_90a, in-tree."""
 import os
 import shutil
 import subprocess
@@ -11,7 +11,7 @@ DEPS = SOURCES + [os.path.join(HERE, 'csrc', 'ramp_kernels.cuh'), os.path.join(H
                   os.path.join(HERE, 'csrc', 'ramp_lookahead_thread.cuh'), os.path.join(HERE, 'csrc', 'ramp_env.cuh'),
                   os.path.join(os.path.dirname(HERE), 'include', 'ramp_b200.h')]
 
-NVCC_FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo',
+NVCC_FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo',
               '-fmad=false',            # no FMA contraction: f64 results must equal CPython's
               '-Xcompiler', '-fPIC', '-Xcompiler', '-ffp-contract=off', '-shared', '-cudart', 'static']
 

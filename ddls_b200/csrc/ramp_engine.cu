@@ -134,8 +134,7 @@ struct ramp_engine {
     int debug = 0;               // RAMP_DEBUG=1 prints the per-step launch decisions to stderr
     int mode = 0;                // 0 auto, 1 warp-per-lookahead, 2 CTA-per-lookahead (RAMP_LOOKAHEAD_MODE)
     int32_t* h_n_work = nullptr; // pinned [4]
-    int64_t big_threshold = 60000;   // N + E from which one CTA per lookahead beats one warp (RAMP_BIG_THRESHOLD); measured
-                                     // on B200: N+E=35k 3.4 vs 3.8 ms, N+E=137k 8.4 vs 4.5 ms (profiles/r1_latency_by_degree.txt)
+    int64_t big_threshold = 60000;   // N + E from which one CTA per lookahead beats one warp (RAMP_BIG_THRESHOLD)
     WorkItem* d_items_big = nullptr;
     cudaStream_t stream2 = nullptr;  // big lookaheads run concurrently with the small ones
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -230,7 +229,7 @@ int ensure_scratch(ramp_engine* e) {
         CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, e->nt, smem));
         if (occ < 1) occ = 1;
         if (e->max_ctas_per_sm > 0 && occ > e->max_ctas_per_sm) occ = e->max_ctas_per_sm;
-        e->grid = e->sm_count * occ;     // persistent CTAs: a whole number of waves (148 SMs x resident CTAs per SM)
+        e->grid = e->sm_count * occ;     // persistent CTAs: a whole number of waves (SMs x resident CTAs per SM)
         e->smem_bytes = smem;
         // beside a CTA kernel the small lookaheads run in 2-warp CTAs: they fill the registers and shared memory the CTA
         // kernel leaves on every SM at a finer grain (the block scheduler spreads both kernels over all SMs)
@@ -301,8 +300,6 @@ LookaheadArgs make_lookahead_args(ramp_engine* e, const WorkItem* items, Counter
 // Launches ONE lookahead kernel for n_items work items of a standalone run (ramp_run_lookaheads): one CTA per lookahead
 // when there are big lookaheads among them and the items fit in about one wave of CTAs (latency-bound regime), one warp
 // per lookahead otherwise (small lookaheads are fastest on one warp; many lookaheads need the warp kernel's density).
-// Measured on B200 (ResNet-50-like job): degree 16 alone 2.7 ms on a 128-thread CTA, 4.0 ms on a 64-thread CTA, 4.5-5 ms on
-// one warp; degree 2: 1.8 / 1.8 / 1.5 ms.
 void launch_lookahead(ramp_engine* e, const LookaheadArgs& a, int n_items, int n_big, cudaStream_t st) {
     int cta_nt = 0;
     if (e->mode == 2) cta_nt = e->cta_nt ? e->cta_nt : (n_items <= e->cta_grid ? 128 : 64);

@@ -1,4 +1,4 @@
-// ramp_kernels.cuh -- device-side data layout and kernels of the B200-native RAMP simulator hot path.
+// ramp_kernels.cuh -- device-side data layout and kernels of the GPU-native (H100, sm_90a) RAMP simulator hot path.
 //
 // Reference semantics (cwfparsonson/ddls @ 9e0b5ba; RCE = ddls/environments/ramp_cluster/
 // ramp_cluster_environment.py, JOB = ddls/demands/jobs/job.py):
@@ -273,7 +273,7 @@ __device__ __forceinline__ double util_sum(const double* term, int n_rec) {
 //      the non-flow list as one flattened, coalesced copy (first ticked next tick == the RCE:429 snapshot). (RCE:691-716)
 //   I,J lane 0 accumulates t / comm / comp and the trace in tick order                              (RCE:442-445, 777-791)
 #ifndef RAMP_U
-#define RAMP_U 2            // batch depth: independent loads in flight per lane per phase (2 measured best on B200: 4 -1.2 %, 8 -7 %)
+#define RAMP_U 2            // batch depth: independent loads in flight per lane per phase
 #endif
 #ifndef RAMP_OPS_CAP
 #define RAMP_OPS_CAP 48     // op-frontier records kept in shared memory per buffer (overflow goes to HBM)

@@ -201,9 +201,9 @@ struct LaneNF {
 
 // Remaining times are non-negative doubles (validated and canonicalised to +0 at registration): their u64 bit patterns order like
 // the values, so every comparison of the tick loop -- winners' minimum, tick = min(t_comm, t_op), "did it complete" -- is a 64-bit
-// INTEGER comparison (two ISETP) instead of an FP64 one.  On sm_100a DSETP / DADD results come back through the long scoreboard
-// (profiles/r2_ncu_thread_source.md: 20 % of all stall samples sat on four DSETP after tick_down); only the subtraction of the
-// survivors and the three accumulators stay FP64, off the control path.
+// INTEGER comparison (two ISETP) instead of an FP64 one: DSETP / DADD results come back through the long scoreboard, so FP64
+// compares on the control path stall the tick loop; only the subtraction of the survivors and the three accumulators stay FP64,
+// off the control path.
 //   x -= min(tick, x) == 0  (JOB:555-556, 561-562)  <=>  x <= tick   (x > tick >= 0 gives x - tick > 0: no underflow to zero)
 typedef unsigned long long u64_t;
 __device__ __forceinline__ u64_t rem_bits(const int4& r) { return ((u64_t)(uint32_t)r.y << 32) | (u64_t)(uint32_t)r.x; }

@@ -370,7 +370,7 @@ struct ramp_policy {
     float* d_emb = nullptr;               // [n_models][out_node]
     float* d_gstatic = nullptr;           // [n_models][6]
     bool weights_set = false, emb_valid = false;
-    int sm_count = 148;
+    int sm_count = 132;
     size_t head_smem = 0;
     // outputs of the last act / forward
     int32_t cap = 0;

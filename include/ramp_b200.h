@@ -1,5 +1,5 @@
 /*
- * ramp_b200 -- C ABI of the B200-native RAMP cluster simulator hot path.
+ * ramp_b200 -- C ABI of the GPU-native (H100, sm_90a) RAMP cluster simulator hot path.
  *
  * The reference (cwfparsonson/ddls @ 9e0b5ba) is pure Python and has no FFI; the interface this
  * library sits behind is the Python class surface of

@@ -2,8 +2,7 @@
 
     python scripts/ncu_summary.py gpurun_out/prof_bench.ncu-rep "<what>" [out.json] [lookaheads per launch]
 
-Writes profiles/ncu_lookahead_summary.json by default; round 2 writes profiles/r2_ncu_thread_summary.json, which bench.py reads for
-the STATIC `roofline.traffic` / `roofline.issue_slots` figures (labelled with this file as their source)."""
+Writes profiles/ncu_lookahead_summary.json by default."""
 import csv, json, subprocess, sys, os
 
 rep = sys.argv[1]

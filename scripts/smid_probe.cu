@@ -1,5 +1,5 @@
-// Probe used for DESIGN.md section 4 (launch policy): nvcc -O2 -gencode arch=compute_100a,code=sm_100a -o smid_probe scripts/smid_probe.cu
-// prints how many blocks of two concurrent kernels each SM received (B200: breadth-first over all SMs).
+// Probe used for DESIGN.md section 4 (launch policy): nvcc -O2 -gencode arch=compute_90a,code=sm_90a -o smid_probe scripts/smid_probe.cu
+// prints how many blocks of two concurrent kernels each SM received.
 // how does the block scheduler spread two concurrent kernels over the SMs?
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -27,7 +27,8 @@ int main(int argc, char** argv) {
     for (int x : ha) if (x >= 0 && x < 160) ca[x]++;
     for (int x : hb) if (x >= 0 && x < 160) cb[x]++;
     printf("per-SM (A,B) block counts over the whole run:\n");
-    for (int i = 0; i < 148; ++i) printf("%d:%d,%d ", i, ca[i], cb[i]);
+    int n_sm = 0; cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, 0);
+    for (int i = 0; i < n_sm && i < 160; ++i) printf("%d:%d,%d ", i, ca[i], cb[i]);
     printf("\nfirst 20 A blocks -> SM: "); for (int i = 0; i < 20; ++i) printf("%d ", ha[i]);
     printf("\n");
     return 0;

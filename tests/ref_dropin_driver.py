@@ -3,10 +3,12 @@
 RJPE:199-206), on one of the seeded golden episodes, and prints what the reference itself recorded for that episode
 (tests/golden/<case>.npz) next to what this run produced.
 
-    PYTHONHASHSEED=0 python tests/ref_dropin_driver.py <case> [--fake-engine]
+    PYTHONHASHSEED=0 python tests/ref_dropin_driver.py <case> [--fake-engine] [--reference-cluster [--record]]
 
 --fake-engine answers the engine calls with the CPU oracle (tests/fake_engine.py) so the host logic can be checked
-without a GPU; without it the CUDA engine is used (needs cuda:0)."""
+without a GPU; without it the CUDA engine is used (needs cuda:0).  --reference-cluster runs the reference's own cluster
+environment instead of the drop-in; with --record its result is stored as tests/golden/<case>_reference_cluster.json, the
+run the drop-in is compared with in tests/test_reference_dropin.py."""
 import json
 import os
 import random
@@ -124,6 +126,10 @@ def main():
     out['last_step_stats'] = {k: float(cluster.step_stats[k]) for k in ('num_jobs_blocked', 'num_jobs_completed', 'num_jobs_arrived', 'step_end_time')}
     out['init_details_memo_keys'] = sorted([str(m), int(p)] for m in memo for p in memo[m])
     print('RESULT ' + json.dumps(out), flush=True)
+    if '--record' in sys.argv:
+        assert use_reference_cluster, '--record stores the reference cluster environment\'s run'
+        with open(os.path.join(HERE, 'golden', f'{case}_reference_cluster.json'), 'w') as f:
+            json.dump(out, f)
 
 
 if __name__ == '__main__':

@@ -80,7 +80,7 @@ def _check(case, out):
 @pytest.mark.parametrize('case', CASES)
 def test_dropin_inside_the_reference_host_logic(case):
     if not _reference_available():
-        pytest.skip('reference not available (neither the build container checkout nor oracle/_ref)')
+        pytest.skip("needs the reference's own environment: no reference checkout, nothing staged at oracle/_ref")
     out = _run(case, fake=True)
     _check(case, out)
 
@@ -94,8 +94,15 @@ def test_dropin_inside_the_reference_on_cuda(case):
     _check(case, out)
 
 
+def _reference_cluster_run(case):
+    """The reference's own cluster environment on the same seeds, as recorded by
+    ``PYTHONHASHSEED=0 python tests/ref_dropin_driver.py <case> --reference-cluster --record``."""
+    with open(os.path.join(ROOT, 'tests', 'golden', f'{case}_reference_cluster.json')) as f:
+        return json.load(f)
+
+
 def _check_live(mine, ref):
-    """Drop-in vs the reference's own cluster environment run live on the same seeds."""
+    """Drop-in vs the reference's own cluster environment on the same seeds."""
     assert mine['is_dropin'] and not ref['is_dropin']
     for k in ('num_jobs_arrived', 'num_jobs_completed', 'num_jobs_blocked', 'n_env_steps', 'n_cluster_steps', 'actions',
               'completed_job_idxs'):
@@ -120,9 +127,9 @@ def test_per_tick_utilisation_lists_equal_the_reference(case):
     """step_stats['mean_mounted_worker_utilisation_frac'] / ['mean_cluster_worker_utilisation_frac'] stay per-tick lists in the
     reference (RCE:989-994); the drop-in returns the engine's own per-iteration entries (every event ends the reference's step --
     RCE:1003-1044 -- so a list has one entry unless rounding keeps an event from firing; the engine records however many there are)."""
-    if not os.path.isdir('/root/' + 'reference'):
-        pytest.skip('needs the build container: runs the reference live for comparison')
-    ref = _run(case, fake=True, reference_cluster=True)
+    if not _reference_available():
+        pytest.skip("needs the reference's own environment: no reference checkout, nothing staged at oracle/_ref")
+    ref = _reference_cluster_run(case)
     mine = _run(case, fake=True)
     assert all(len(step) >= 1 for step in ref['tick_lists']['mean_mounted_worker_utilisation_frac'])
     _check_live(mine, ref)
@@ -132,9 +139,9 @@ def test_per_tick_utilisation_lists_equal_the_reference(case):
 def test_dropin_with_a_generator_that_never_runs_dry(case):
     """'remove_and_repeat' sampling: len(jobs_generator) never reaches 0, the episode ends on max_simulation_run_time and jobs
     keep arriving until then -- the drop-in streams arrivals one ahead instead of fixing their number at reset."""
-    if not os.path.isdir('/root/' + 'reference'):
-        pytest.skip('needs the build container: runs the reference live for comparison')
-    ref = _run(case, fake=True, reference_cluster=True)
+    if not _reference_available():
+        pytest.skip("needs the reference's own environment: no reference checkout, nothing staged at oracle/_ref")
+    ref = _reference_cluster_run(case)
     mine = _run(case, fake=True)
     assert ref['num_jobs_arrived'] > 6            # more arrivals than the 3 / 2 distinct jobs the generator holds
     _check_live(mine, ref)
@@ -145,6 +152,6 @@ def test_dropin_with_a_generator_that_never_runs_dry(case):
 def test_dropin_with_a_generator_that_never_runs_dry_on_cuda(case):
     if not _reference_available():
         pytest.skip('reference not staged at oracle/_ref')
-    ref = _run(case, fake=True, reference_cluster=True)
+    ref = _reference_cluster_run(case)
     mine = _run(case, fake=False)
     _check_live(mine, ref)
