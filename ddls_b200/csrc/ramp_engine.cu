@@ -439,12 +439,14 @@ int ensure_thread_scratch(ramp_engine* e) {
         CUDA_TRY(cudaFuncSetAttribute(ramp_lookahead_thread_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         CUDA_TRY(cudaFuncSetAttribute(ramp_lookahead_thread_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
         int occ = 0;
-        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ramp_lookahead_thread_kernel, 32, smem));
+        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ramp_lookahead_thread_kernel, RAMP_THREAD_CTA, smem));
         if (occ < 1) occ = 1;
         // one chunk = up to 32 lookaheads; enough resident CTAs for every episode to miss at once, at most 2 per SM
         const int want = (e->cfg.n_episodes + 31) / 32 + 8;
         e->res_grid = std::max(1, std::min(std::min(e->sm_count * occ, e->sm_count * 2), want));
         e->res_smem = smem;
+        if (e->debug) fprintf(stderr, "[ramp] thread kernel: %zu B dynamic shared memory, %d CTAs of %d threads per SM fit, grid %d\n",
+                              smem, occ, RAMP_THREAD_CTA, e->res_grid);
     }
     const uint64_t stride = thread_scratch_bytes(e->res_spill_ops, e->res_spill_deps, e->cfg.trace_cap);
     if (stride != e->res_scratch_stride || e->res_grid != e->res_scratch_grid || !e->d_res_scratch) {
@@ -877,7 +879,7 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
             ramp_bucket_kernel<<<1, 1024, 0, st>>>(ba);
             ThreadArgs ta = make_thread_args(e, e->d_chunks, &e->d_counters->n_chunks, &e->d_counters->chunk_cursor, e->d_chunk_items,
                                              e->res, e->pool, e->d_stats);
-            ramp_lookahead_thread_kernel<<<e->res_grid, 32, e->res_smem, st>>>(ta);
+            ramp_lookahead_thread_kernel<<<e->res_grid, RAMP_THREAD_CTA, e->res_smem, st>>>(ta);
             e->launches += 2;
         }
         if (e->n_nonresident > 0) {
@@ -1158,7 +1160,7 @@ int ramp_run_lookaheads(ramp_engine_t* e, const int32_t* template_ids, int32_t n
         ThreadArgs ta = make_thread_args(e, e->sa_chunks, &e->sa_counters->n_chunks, &e->sa_counters->chunk_cursor, e->sa_chunk_items,
                                          e->sa_res, tp, nullptr);
         const int g = std::max(1, std::min(e->res_grid, (int)chunks.size()));
-        ramp_lookahead_thread_kernel<<<g, 32, e->res_smem, st>>>(ta);
+        ramp_lookahead_thread_kernel<<<g, RAMP_THREAD_CTA, e->res_smem, st>>>(ta);
         e->launches++;
     }
     if (!old_idx.empty()) {

@@ -5,9 +5,9 @@
 // tick.  There is nothing left for a warp to share, so each lookahead runs on ONE lane, scalar, with no shuffles,
 // ballots, atomics or barriers in the tick loop:
 //
-//   * a CTA is one warp; it pulls CHUNKS of up to 32 work items that use the same template (ramp_bucket_kernel groups the
-//     step's memo misses by template), so its lanes run the same instruction stream over the same template -- no
-//     divergence, and every template read is a shared-memory broadcast;
+//   * a CTA is a sim warp and a ledger warp (below); it pulls CHUNKS of up to 32 work items that use the same template
+//     (ramp_bucket_kernel groups the step's memo misses by template), so the sim lanes run the same instruction stream over
+//     the same template -- no divergence, and every template read is a shared-memory broadcast;
 //   * the template blob (header + op records + rows + thresholds + packed dep words + run times) is copied into shared
 //     memory ONCE per chunk with a bulk async copy (cp.async.bulk -> UBLKCP, completion on an mbarrier), so a tick never
 //     waits for L2;
@@ -24,7 +24,13 @@
 //   H    every ready flow: rem -= min(tick, rem); == 0 -> its child class's counter += entry size; the class is readied
 //        when the counter passes through its threshold (n_parents x class size)                 (RCE:733-775, JOB:525-536)
 //   G    winning op classes tick; == 0 -> completed, their out-entries become ready (first ticked next tick, RCE:429)
-//   I,J  t / comm / comp and the trace, f64, tick order                                           (RCE:442-445, 777-791)
+//   I,J  t / comm / comp, the utilisation term and the trace, f64, tick order                    (RCE:442-445, 777-791, 830-832)
+//
+// Only E..H and the frontier updates feed the next tick; I and J are accounting.  They run on a second warp: a CTA is two
+// warps, and lane k of warp 0 (the SIM lane) and lane k of warp 1 (the LEDGER lane) share work item chunk * 32 + k.  The sim
+// lane appends one record per tick {tick, n_active, flows ticked} to its ring in shared memory and publishes its record count
+// every RAMP_T_PUB ticks; the ledger lane replays the records with the same f64 operations in the same order (bit-identical
+// results), writes the trace, and runs the epilogue.  The sim warp's tick loop keeps no FP64 but the survivors' subtraction.
 #pragma once
 
 namespace ramp {
@@ -43,6 +49,10 @@ namespace ramp {
 #endif
 #define RAMP_T_WCAP 8       // worker groups / channel groups with a per-lane winner table (more: pairwise comparison)
 #define RAMP_T_CCAP 32
+#define RAMP_T_RING 32      // tick records per lane in the sim -> ledger ring (a power of two)
+#define RAMP_T_PUB 8        // the sim lane publishes its record count every this many ticks (a power of two, <= RAMP_T_RING)
+#define RAMP_T_DONE 0x80000000u   // set in the published count with the sim lane's last record
+#define RAMP_THREAD_CTA 64  // threads of a thread-kernel CTA: the sim warp and the ledger warp
 
 // header of a resident template blob (the blob is what the bulk copy moves: 16-byte aligned, size a multiple of 16)
 struct ResHeader {
@@ -56,6 +66,8 @@ struct ResHeader {
 static_assert(sizeof(ResHeader) == 96, "resident header is 96 bytes");
 
 struct ChunkDesc { int32_t template_id, count; };      // up to 32 work items of one template; items at [chunk * 32 + lane]
+static_assert((RAMP_T_RING & (RAMP_T_RING - 1)) == 0 && (RAMP_T_PUB & (RAMP_T_PUB - 1)) == 0 && RAMP_T_PUB <= RAMP_T_RING,
+              "ring and publish interval are powers of two");
 
 // recorded by the first lookahead of a template that completes (deterministic per template): lets later ones write their trace
 // in place and keep every list in shared memory
@@ -83,7 +95,7 @@ struct ThreadArgs {
 };
 
 __host__ __device__ inline size_t thread_smem_bytes(int tmpl_cap, int n_cap) {
-    size_t per_lane = (size_t)RAMP_T_FCAP * 16 + (size_t)RAMP_T_OCAP * 20 + (size_t)RAMP_T_NFCAP * 4
+    size_t per_lane = (size_t)RAMP_T_RING * 16 + (size_t)RAMP_T_FCAP * 16 + (size_t)RAMP_T_OCAP * 20 + (size_t)RAMP_T_NFCAP * 4
                       + (size_t)(RAMP_T_WCAP + RAMP_T_CCAP) * 4 + (size_t)n_cap * 2;
     return (size_t)tmpl_cap + 32 * per_lane + 64;
 }
@@ -208,23 +220,55 @@ struct LaneNF {
 typedef unsigned long long u64_t;
 __device__ __forceinline__ u64_t rem_bits(const int4& r) { return ((u64_t)(uint32_t)r.y << 32) | (u64_t)(uint32_t)r.x; }
 
-struct LaneCtx {                      // what one lane's lookahead works on
+// ---------------------------------------------------------------------------------------------------
+// sim -> ledger ring: per lane, RAMP_T_RING records {tick.lo, tick.hi, n_active, flows ticked} at ring[slot * 32 + lane]; the
+// sim lane publishes how many it has written (release), the ledger lane how many it has consumed (acquire / release pairs)
+__device__ __forceinline__ void st_release_cta(uint32_t* p, uint32_t v) {
+    asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_acquire_cta(const uint32_t* p) {
+    uint32_t v;
+    asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory");
+    return v;
+}
+
+struct SimFinal { int status, tick_no, max_o, max_f, max_nf; };   // what the sim lane hands over with its last record
+
+struct LedgerFeed {                   // the sim lane's end of its ring
+    int4* ring; uint32_t* head; const uint32_t* tail; SimFinal* fin; int lane;
+    uint32_t n, room;                 // records written; the first record number that has no free slot yet
+    __device__ __forceinline__ void put(const u64_t tick_b, const int n_active, const bool flows) {
+        if (n == room) {              // ring full: publish everything, then wait for the ledger lane to free a slot
+            st_release_cta(head, n);
+            uint32_t t;
+            do { t = ld_acquire_cta(tail); } while (n - t >= RAMP_T_RING);
+            room = t + RAMP_T_RING;
+        }
+        ring[(n & (RAMP_T_RING - 1)) * 32 + lane] = make_int4((int)(uint32_t)tick_b, (int)(uint32_t)(tick_b >> 32), n_active, flows ? 1 : 0);
+        ++n;
+        if ((n & (RAMP_T_PUB - 1)) == 0u) st_release_cta(head, n);
+    }
+    __device__ __forceinline__ void finish(const SimFinal& f) {
+        *fin = f;
+        st_release_cta(head, n | RAMP_T_DONE);
+    }
+};
+
+struct LaneCtx {                      // what one sim lane's lookahead works on
     const unsigned char* tm;         // template blob in shared memory
     int4* f_sm; int4* o_sm; uint32_t* nf_sm; int32_t* oi_sm; uint32_t* wk_sm; uint32_t* ck_sm; uint16_t* cnt_sm;
     int4* f_gl; int4* o_gl; uint32_t* nf_gl; int32_t* oi_gl;
-    int32_t* tr_n; double* tr_tick;  // trace destination: element k at [k * tr_stride]
-    int tr_stride, tr_cap;
+    int4* ring; uint32_t* head; const uint32_t* tail; SimFinal* fin;   // this lane's ledger feed
+    int tr_cap;                      // ticks the trace can hold: one more is RAMP_ST_TRACE_OVERFLOW and ends the lookahead
     int lane, n_cap;
-    double util_jct, util_dn;        // != 0: accumulate sum (n_active / util_dn) * (tick / util_jct) in tick order (RCE:830-832)
 };
 
-struct LaneResult { double t, comm, comp, util; int tick_no, status, max_o, max_f, max_nf; };
-
-// _run_lookahead for one lane.  SPILL = false: every frontier fits its shared-memory capacity (TemplateHints);
-// SIMPLE = true: one worker group and at most one channel group (the usual quotient of a partitioned job): the winner is the
-// largest key, no tables.
+// _run_lookahead for one sim lane: the tick loop (A-H, K, L); every tick goes to the ledger lane as one ring record, and the
+// final status, tick count and largest frontiers follow the last one.  SPILL = false: every frontier fits its shared-memory
+// capacity (TemplateHints); SIMPLE = true: one worker group and at most one channel group (the usual quotient of a
+// partitioned job): the winner is the largest key, no tables.
 template <bool SPILL, bool SIMPLE>
-__device__ __forceinline__ LaneResult thread_lookahead(const LaneCtx& x) {
+__device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
     const int lane = x.lane;
     const ResHeader& H = *reinterpret_cast<const ResHeader*>(x.tm);
     const int4* op_rec = reinterpret_cast<const int4*>(x.tm + sizeof(ResHeader));                  // {cost.lo, cost.hi, key, worker | weight << 16}
@@ -248,19 +292,11 @@ __device__ __forceinline__ LaneResult thread_lookahead(const LaneCtx& x) {
     for (int i = 0; i < N && i < x.n_cap; ++i) cnt[i * 32] = 0;
     int nO = H.n_src, nF = 0, nNF = 0;
     for (int k = 0; k < nO; ++k) { const int op = src_ops[k]; ops.put(k, op_rec[op], op); }       // RCE:1334
-    LaneResult R;
-    R.t = 0.0; R.comm = 0.0; R.comp = 0.0; R.util = 0.0; R.tick_no = 0; R.max_o = nO; R.max_f = 0; R.max_nf = 0;
+    SimFinal R;
+    R.tick_no = 0; R.max_o = nO; R.max_f = 0; R.max_nf = 0;
     R.status = (N <= x.n_cap) ? RAMP_ST_OK : RAMP_ST_TABLE_FULL;                                    // cannot happen (eligibility)
     int to_complete = N + E;              // ops and deps still to complete (JOB:549-551)
-    const bool do_util = x.util_jct != 0.0;
-    int util_last_n = -1;
-    double util_last_q = 0.0;
-    // the term of one tick (RCE:830-832); a tick with no active worker or no length adds +0.0 and is skipped (see the epilogue)
-    auto add_util = [&](const int n_active, const double tick) {
-        if (n_active != util_last_n) { util_last_n = n_active; util_last_q = __ddiv_rn((double)n_active, x.util_dn); }
-        R.util = __dadd_rn(R.util, __dmul_rn(util_last_q, __ddiv_rn(tick, x.util_jct)));
-    };
-    int tr_idx = 0;                       // trace element k lives at [k * tr_stride]
+    LedgerFeed feed{x.ring, x.head, x.tail, x.fin, lane, 0u, (uint32_t)RAMP_T_RING};
 
     if (R.status == RAMP_ST_OK) for (;;) {       // left through ONE combined exit test per tick
         if (nF <= RAMP_T_FASTF && nO <= 2) {
@@ -299,15 +335,12 @@ __device__ __forceinline__ LaneResult thread_lookahead(const LaneCtx& x) {
                 cnt[child * 32] = (uint16_t)neu;
                 if (old < thr && thr <= neu) { ops.put(tailO, op_rec[child], child); ++tailO; }     // JOB:531 for every member
             };
-            // E, I, J: the tick, the three accumulators, the utilisation term and the trace entry
+            // E: the tick; its record goes to the ledger lane (I, J)
             auto take_tick = [&](const u64_t t_comm, const bool ticked_flows) {
                 tick_b = (t_comm < t_op) ? t_comm : t_op;
                 tick = __longlong_as_double((long long)tick_b);
-                if (ticked_flows) R.comm = __dadd_rn(R.comm, tick);                                  // RCE:434-439, 777-791
-                if (n_active > 0) { R.comp = __dadd_rn(R.comp, tick); if (do_util && tick_b != 0ull) add_util(n_active, tick); }
-                R.t = __dadd_rn(R.t, tick);
-                if (R.tick_no < x.tr_cap) { x.tr_n[tr_idx] = n_active; x.tr_tick[tr_idx] = tick; tr_idx += x.tr_stride; }
-                else R.status = RAMP_ST_TRACE_OVERFLOW;
+                feed.put(tick_b, n_active, ticked_flows);
+                if (R.tick_no >= x.tr_cap) R.status = RAMP_ST_TRACE_OVERFLOW;
                 ++R.tick_no;
             };
             auto flow_tick = [&](auto nf_tag) {
@@ -508,17 +541,12 @@ __device__ __forceinline__ LaneResult thread_lookahead(const LaneCtx& x) {
                 }
             }
         }
-        // ---- E, I, J ----
+        // ---- E (I, J on the ledger lane) ----
         const u64_t tick_b = (t_comm < t_op) ? t_comm : t_op;
         const double tick = __longlong_as_double((long long)tick_b);
-        {
-            if ((!any_nf) && (nF > 0)) R.comm = __dadd_rn(R.comm, tick);                             // RCE:434-439, 777-791
-            if (n_active > 0) { R.comp = __dadd_rn(R.comp, tick); if (do_util && tick_b != 0ull) add_util(n_active, tick); }
-            R.t = __dadd_rn(R.t, tick);
-            if (R.tick_no < x.tr_cap) { x.tr_n[tr_idx] = n_active; x.tr_tick[tr_idx] = tick; tr_idx += x.tr_stride; }
-            else R.status = RAMP_ST_TRACE_OVERFLOW;
-            ++R.tick_no;
-        }
+        feed.put(tick_b, n_active, (!any_nf) && (nF > 0));
+        if (R.tick_no >= x.tr_cap) R.status = RAMP_ST_TRACE_OVERFLOW;
+        ++R.tick_no;
         // ---- H ----
         int tailO = nO;                       // ops readied in this tick are appended behind the current frontier
         auto complete_dep = [&](const uint32_t hi) {                                                // JOB:525-536
@@ -594,17 +622,75 @@ __device__ __forceinline__ LaneResult thread_lookahead(const LaneCtx& x) {
             break;
         }
     }
-    return R;
+    feed.finish(R);
 }
 
-__global__ void __launch_bounds__(32) ramp_lookahead_thread_kernel(const ThreadArgs a) {
+// ---------------------------------------------------------------------------------------------------
+// The ledger lane: replays its sim lane's ticks in tick order -- t / comm / comp (RCE:434-445, 777-791), the utilisation term
+// (RCE:830-832) and the trace element -- with the f64 operations the tick loop used to do itself, in the same order.
+struct LedgerCtx {
+    const int4* ring; const uint32_t* head; uint32_t* tail; int lane;
+    int32_t* tr_n; double* tr_tick;  // trace destination: element k at [k * tr_stride]
+    int tr_stride, tr_cap;
+    double util_jct, util_dn;        // != 0: accumulate sum (n_active / util_dn) * (tick / util_jct) in tick order (RCE:830-832)
+};
+struct LedgerSums { double t, comm, comp, util; };
+
+__device__ __forceinline__ LedgerSums ledger_run(const LedgerCtx& y) {
+    LedgerSums S;
+    S.t = 0.0; S.comm = 0.0; S.comp = 0.0; S.util = 0.0;
+    const bool do_util = y.util_jct != 0.0;
+    int util_last_n = -1;
+    double util_last_q = 0.0;
+    int tr_idx = 0;
+    uint32_t k = 0;                       // records consumed
+    for (;;) {
+        const uint32_t h = ld_acquire_cta(y.head);
+        const uint32_t end = h & ~RAMP_T_DONE;
+        if (k == end) {
+            if (h & RAMP_T_DONE) break;
+            __nanosleep(64);              // the sim lane publishes every RAMP_T_PUB ticks (several microseconds): poll gently
+            continue;
+        }
+        _Pragma("unroll 1")
+        for (; k != end; ++k) {
+            const int4 r = y.ring[(k & (RAMP_T_RING - 1)) * 32 + y.lane];
+            const u64_t tick_b = rem_bits(r);
+            const double tick = __longlong_as_double((long long)tick_b);
+            const int n_active = r.z;
+            if (r.w) S.comm = __dadd_rn(S.comm, tick);
+            if (n_active > 0) {
+                S.comp = __dadd_rn(S.comp, tick);
+                // a tick with no active worker or no length adds +0.0 and is skipped (see the epilogue)
+                if (do_util && tick_b != 0ull) {
+                    if (n_active != util_last_n) { util_last_n = n_active; util_last_q = __ddiv_rn((double)n_active, y.util_dn); }
+                    S.util = __dadd_rn(S.util, __dmul_rn(util_last_q, __ddiv_rn(tick, y.util_jct)));
+                }
+            }
+            S.t = __dadd_rn(S.t, tick);
+            if ((int)k < y.tr_cap) { y.tr_n[tr_idx] = n_active; y.tr_tick[tr_idx] = tick; tr_idx += y.tr_stride; }
+        }
+        st_release_cta(y.tail, k);
+    }
+    return S;
+}
+
+__global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(const ThreadArgs a) {
     extern __shared__ __align__(128) unsigned char smem_thr[];
     __shared__ __align__(8) unsigned long long mbar;
-    const int lane = threadIdx.x;
+    __shared__ uint32_t s_head[32], s_tail[32];     // per lane: ring records the sim lane published / the ledger lane consumed
+    __shared__ SimFinal s_fin[32];                   // per lane: the sim lane's status, tick count and largest frontiers
+    __shared__ int32_t s_tr_cap[32];                 // per lane: ticks its trace holds (the ledger lane places the trace)
+    __shared__ int4 s_chunk;                         // {chunk, template (-1: none left), count, -}
+    __shared__ int4 s_hint;                          // TemplateHints of the chunk's template
+    __shared__ double s_hint_jct;
+    const int lane = threadIdx.x & 31;
+    const bool is_sim = threadIdx.x < 32;           // warp 0: tick loops; warp 1: ledger lanes
     unsigned char* st = smem_thr + a.tmpl_cap;                      // per-lane state, by decreasing alignment
+    int4* ring = reinterpret_cast<int4*>(st);                                            // [RING][32]
     LaneCtx x;
     x.tm = smem_thr;                                                // template blob
-    x.f_sm = reinterpret_cast<int4*>(st);                                                // [FCAP][32]
+    x.f_sm = ring + RAMP_T_RING * 32;                                                    // [FCAP][32]
     x.o_sm = x.f_sm + RAMP_T_FCAP * 32;                                                  // [OCAP][32]
     x.nf_sm = reinterpret_cast<uint32_t*>(x.o_sm + RAMP_T_OCAP * 32);                    // [NFCAP][32]
     x.oi_sm = reinterpret_cast<int32_t*>(x.nf_sm + RAMP_T_NFCAP * 32);                   // [OCAP][32]
@@ -618,29 +704,45 @@ __global__ void __launch_bounds__(32) ramp_lookahead_thread_kernel(const ThreadA
     x.nf_gl = reinterpret_cast<uint32_t*>(tmp_tick + (size_t)a.trace_cap * 32);          // [spill_deps][32]
     x.oi_gl = reinterpret_cast<int32_t*>(x.nf_gl + (size_t)a.spill_deps * 32);           // [spill_ops][32]
     int32_t* tmp_n = x.oi_gl + (size_t)a.spill_ops * 32;                                 // [trace_cap][32]
+    x.ring = ring; x.head = &s_head[lane]; x.tail = &s_tail[lane]; x.fin = &s_fin[lane];
     x.lane = lane; x.n_cap = a.n_cap;
 
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&mbar)));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    __syncwarp();
+    __syncthreads();
     uint32_t phase = 0;
     int loaded = -1;
 
     for (;;) {
-        int c = 0;
-        if (lane == 0) c = atomicAdd(a.cursor, 1);
-        c = __shfl_sync(0xffffffffu, c, 0);
-        if (c >= *a.n_chunks) break;
-        const ChunkDesc ch = a.chunks[c];
-        const TemplateDev& TD = a.templates[ch.template_id];
-        if (ch.template_id != loaded) {
-            // every lane is done with the previous template (convergence point above); order those generic-proxy accesses
-            // before the async-proxy writes of the bulk copy
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) {
+        // both warps are done with the previous chunk (the barrier below): order their generic-proxy accesses to the blob
+        // before the async-proxy writes of a bulk copy into it
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        if (threadIdx.x == 0) {
+            // the chunk, and what an earlier lookahead of its template recorded (number of ticks, largest frontiers,
+            // completion time: deterministic per template), read ONCE so that both warps take the same path
+            int4 cd = make_int4(0, -1, 0, 0), hv = make_int4(0, 0, 0, 0);
+            double hj = 0.0;
+            const int c = atomicAdd(a.cursor, 1);
+            if (c < *a.n_chunks) {
+                const ChunkDesc ch = a.chunks[c];
+                cd = make_int4(c, ch.template_id, ch.count, 0);
+                hv = __ldcg(reinterpret_cast<const int4*>(&a.hints[ch.template_id]));
+                hj = __ldcg(&a.hint_jct[ch.template_id]);
+            }
+            s_chunk = cd; s_hint = hv; s_hint_jct = hj;
+        }
+        __syncthreads();
+        const int4 cd = s_chunk;
+        if (cd.y < 0) break;
+        const int c = cd.x, tmpl = cd.y, count = cd.z;
+        TemplateHints hint;
+        { const int4 hv = s_hint; hint.n_ticks = hv.x; hint.max_o = hv.y; hint.max_f = hv.z; hint.max_nf = hv.w; }
+        const double hj = s_hint_jct;
+        const TemplateDev& TD = a.templates[tmpl];
+        if (tmpl != loaded) {
+            if (threadIdx.x == 0) {
                 const uint32_t bytes = (uint32_t)TD.res_bytes;
                 asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&mbar)), "r"(bytes) : "memory");
                 asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -656,100 +758,115 @@ __global__ void __launch_bounds__(32) ramp_lookahead_thread_kernel(const ThreadA
                 "RAMP_DONE_%=:\n"
                 "}\n" ::"r"(smem_u32(&mbar)), "r"(phase) : "memory");
             phase ^= 1u;
-            loaded = ch.template_id;
+            loaded = tmpl;
         }
-        // what an earlier lookahead of this template recorded: number of ticks and the largest frontiers (deterministic per
-        // template).  With it the trace goes straight to an exactly-sized pool allocation and no list can leave shared memory.
-        TemplateHints hint;
-        { const int4 hv = __ldcg(reinterpret_cast<const int4*>(&a.hints[ch.template_id])); hint.n_ticks = hv.x; hint.max_o = hv.y; hint.max_f = hv.z; hint.max_nf = hv.w; }
+        // with the hints the trace goes straight to an exactly-sized pool allocation and no list can leave shared memory
         const bool fast = hint.n_ticks > 0 && hint.n_ticks <= a.trace_cap && hint.max_o <= RAMP_T_OCAP && hint.max_f <= RAMP_T_FCAP
                           && hint.max_nf <= RAMP_T_NFCAP;
-        if (lane < ch.count) {
-            const WorkItem item = a.items[(size_t)c * 32 + lane];
-            const ResHeader& H = *reinterpret_cast<const ResHeader*>(x.tm);
-            const bool simple = (H.n_workers == 1) && (H.n_channels <= 1);
-            long long off = -1;
-            int status0 = RAMP_ST_OK;
-            const bool direct = fast && a.pool.top != nullptr;          // trace written in place
-            if (direct) {
-                const unsigned long long o = atomicAdd(a.pool.top, (unsigned long long)hint.n_ticks);
-                if (o + (unsigned long long)hint.n_ticks <= a.pool.len) off = (long long)o; else status0 = RAMP_ST_TRACE_OVERFLOW;
-            }
-            if (off >= 0) { x.tr_n = a.pool.n_active + off; x.tr_tick = a.pool.tick + off; x.tr_stride = 1; x.tr_cap = hint.n_ticks; }
-            else { x.tr_n = tmp_n + lane; x.tr_tick = tmp_tick + lane; x.tr_stride = 32; x.tr_cap = a.trace_cap; }
-            // utilisation inside the tick loop when an earlier lookahead of the template left its completion time
-            const int nmw = item.n_mounted_workers > 0 ? item.n_mounted_workers : H.orig_workers;
-            double hj = 0.0;
-            if (fast) hj = __ldcg(&a.hint_jct[ch.template_id]);
-            x.util_jct = (hj > 0.0 && !isinf(hj)) ? hj : 0.0;
-            {   // keep the conversion out of the tick loop (the compiler re-materialised it there: one I2F.F64 per tick)
-                double dn = (double)nmw;
-                asm volatile("" : "+d"(dn));
-                x.util_dn = dn;
-            }
-            LaneResult R;
-            if (fast) R = simple ? thread_lookahead<false, true>(x) : thread_lookahead<false, false>(x);
-            else R = simple ? thread_lookahead<true, true>(x) : thread_lookahead<true, false>(x);
-            int status = (R.status == RAMP_ST_OK) ? status0 : R.status;
-            if (direct && status == RAMP_ST_OK && R.tick_no != hint.n_ticks) status = RAMP_ST_TRACE_OVERFLOW;   // cannot happen
-            if (!fast && status == RAMP_ST_OK) {                      // every lane of the chunk writes the same values
-                *reinterpret_cast<int4*>(&a.hints[ch.template_id]) = make_int4(R.tick_no, R.max_o, R.max_f, R.max_nf);
-                a.hint_jct[ch.template_id] = __dmul_rn(R.t, (double)H.num_training_steps);
-            }
+        const ResHeader& H = *reinterpret_cast<const ResHeader*>(x.tm);
+        const bool active = lane < count;
 
-            // ---- results (RCE:450-452) ----
-            const int n_rec = R.tick_no < x.tr_cap ? R.tick_no : x.tr_cap;
-            const double steps = (double)H.num_training_steps;
-            const double jct = __dmul_rn(R.t, steps);
-            const bool can_util = (status == RAMP_ST_OK);
-            // the in-loop sum divided by the recorded completion time: valid when this lookahead found the very same one
-            const bool util_done = can_util && x.util_jct != 0.0 && jct == x.util_jct;
-            if (!direct && a.pool.top != nullptr) {
-                const unsigned long long o = atomicAdd(a.pool.top, (unsigned long long)n_rec);
-                if (o + (unsigned long long)n_rec <= a.pool.len) off = (long long)o;
-                else if (status == RAMP_ST_OK) status = RAMP_ST_TRACE_OVERFLOW;
-            }
-            double util = util_done ? R.util : 0.0;
-            if (!(util_done && (direct || off < 0))) {
-                if (util_done) util = 0.0;                 // the loop below recomputes it while it copies the trace
-                // RCE:830-832: util = sum over ticks, in tick order, of (n_active / n_mounted_workers) * (tick / jct).  A term
-                // with n_active == 0 or tick == 0 is +0.0 (jct > 0 finite) and adding +0.0 leaves the non-negative sum as it
-                // is, so those ticks are skipped (about two thirds of them); n_active / n_mounted_workers is re-used while
-                // n_active repeats.  Same f64 operations on the same values for every term that can change the sum.
-                const double dn = (double)nmw;
-                const bool copy = (!direct) && off >= 0;
-                int32_t* pn = copy ? a.pool.n_active + off : nullptr;
-                double* pt = copy ? a.pool.tick + off : nullptr;
-                const int32_t* sn = x.tr_n; const double* stt = x.tr_tick; const int sstr = x.tr_stride;
-                const bool skip_zero = can_util && (jct > 0.0) && !isinf(jct);
-                int last_n = -1;
-                double last_q = 0.0;
-#pragma unroll 4
-                for (int k = 0; k < n_rec; ++k) {
-                    const int nk = sn[(size_t)k * sstr];
-                    const double tk = stt[(size_t)k * sstr];
-                    if (copy) { pn[k] = nk; pt[k] = tk; }
-                    if (!can_util) continue;
-                    if (skip_zero && (nk == 0 || tk == 0.0)) continue;
-                    if (nk != last_n) { last_n = nk; last_q = __ddiv_rn((double)nk, dn); }
-                    util = __dadd_rn(util, __dmul_rn(last_q, __ddiv_rn(tk, jct)));
+        // ---- ledger lane, before the tick loop: trace destination and utilisation inputs ----
+        LedgerCtx y;
+        WorkItem item;
+        long long off = -1;
+        int status0 = RAMP_ST_OK, nmw = 0, num_training_steps = 0, n_ops = 0, n_deps = 0;
+        const bool direct = fast && a.pool.top != nullptr;              // trace written in place
+        if (!is_sim) {
+            s_head[lane] = 0u; s_tail[lane] = 0u;
+            if (active) {
+                item = a.items[(size_t)c * 32 + lane];
+                num_training_steps = H.num_training_steps; n_ops = H.n_ops; n_deps = H.n_deps;   // header fields the epilogue needs
+                if (direct) {
+                    const unsigned long long o = atomicAdd(a.pool.top, (unsigned long long)hint.n_ticks);
+                    if (o + (unsigned long long)hint.n_ticks <= a.pool.len) off = (long long)o; else status0 = RAMP_ST_TRACE_OVERFLOW;
+                }
+                y.ring = ring; y.head = &s_head[lane]; y.tail = &s_tail[lane]; y.lane = lane;
+                if (off >= 0) { y.tr_n = a.pool.n_active + off; y.tr_tick = a.pool.tick + off; y.tr_stride = 1; y.tr_cap = hint.n_ticks; }
+                else { y.tr_n = tmp_n + lane; y.tr_tick = tmp_tick + lane; y.tr_stride = 32; y.tr_cap = a.trace_cap; }
+                s_tr_cap[lane] = y.tr_cap;
+                // utilisation inside the tick loop when an earlier lookahead of the template left its completion time
+                nmw = item.n_mounted_workers > 0 ? item.n_mounted_workers : H.orig_workers;
+                y.util_jct = (fast && hj > 0.0 && !isinf(hj)) ? hj : 0.0;
+                {   // keep the conversion out of the loop (the compiler re-materialised it there: one I2F.F64 per tick)
+                    double dn = (double)nmw;
+                    asm volatile("" : "+d"(dn));
+                    y.util_dn = dn;
                 }
             }
-            a.res.jct[item.slot] = jct;
-            a.res.comm[item.slot] = __dmul_rn(R.comm, steps);
-            a.res.comp[item.slot] = __dmul_rn(R.comp, steps);
-            a.res.n_ticks[item.slot] = R.tick_no;
-            a.res.util[item.slot] = can_util ? util : 0.0;
-            a.res.util_nmw[item.slot] = can_util ? nmw : -1;
-            a.res.trace_off[item.slot] = off;
-            a.res.status[item.slot] = status;
-            if (a.stats) {
-                atomicAdd(&a.stats->lookaheads, 1ull);
-                atomicAdd(&a.stats->alg_bytes, (unsigned long long)(TD.algorithmic_bytes_static + 12ull * (unsigned long long)R.tick_no));
-                atomicAdd(&a.stats->quotient_bytes, (unsigned long long)(20ull * H.n_ops + 19ull * H.n_deps + 24ull + 12ull * (unsigned long long)R.tick_no));
+        }
+        __syncthreads();              // ring counters reset and s_tr_cap set; every thread has read s_chunk / s_hint
+
+        if (is_sim) {
+            if (active) {
+                x.tr_cap = s_tr_cap[lane];
+                const bool simple = (H.n_workers == 1) && (H.n_channels <= 1);
+                if (fast) { if (simple) thread_lookahead<false, true>(x); else thread_lookahead<false, false>(x); }
+                else { if (simple) thread_lookahead<true, true>(x); else thread_lookahead<true, false>(x); }
+            }
+            continue;
+        }
+        if (!active) continue;
+        const LedgerSums S = ledger_run(y);
+        const SimFinal R = s_fin[lane];           // written before the DONE count ledger_run acquired
+        int status = (R.status == RAMP_ST_OK) ? status0 : R.status;
+        if (direct && status == RAMP_ST_OK && R.tick_no != hint.n_ticks) status = RAMP_ST_TRACE_OVERFLOW;   // cannot happen
+        if (!fast && status == RAMP_ST_OK) {                      // every lane of the chunk writes the same values
+            *reinterpret_cast<int4*>(&a.hints[tmpl]) = make_int4(R.tick_no, R.max_o, R.max_f, R.max_nf);
+            a.hint_jct[tmpl] = __dmul_rn(S.t, (double)num_training_steps);
+        }
+
+        // ---- results (RCE:450-452) ----
+        const int n_rec = R.tick_no < y.tr_cap ? R.tick_no : y.tr_cap;
+        const double steps = (double)num_training_steps;
+        const double jct = __dmul_rn(S.t, steps);
+        const bool can_util = (status == RAMP_ST_OK);
+        // the in-loop sum divided by the recorded completion time: valid when this lookahead found the very same one
+        const bool util_done = can_util && y.util_jct != 0.0 && jct == y.util_jct;
+        if (!direct && a.pool.top != nullptr) {
+            const unsigned long long o = atomicAdd(a.pool.top, (unsigned long long)n_rec);
+            if (o + (unsigned long long)n_rec <= a.pool.len) off = (long long)o;
+            else if (status == RAMP_ST_OK) status = RAMP_ST_TRACE_OVERFLOW;
+        }
+        double util = util_done ? S.util : 0.0;
+        if (!(util_done && (direct || off < 0))) {
+            if (util_done) util = 0.0;                 // the loop below recomputes it while it copies the trace
+            // RCE:830-832: util = sum over ticks, in tick order, of (n_active / n_mounted_workers) * (tick / jct).  A term
+            // with n_active == 0 or tick == 0 is +0.0 (jct > 0 finite) and adding +0.0 leaves the non-negative sum as it
+            // is, so those ticks are skipped (about two thirds of them); n_active / n_mounted_workers is re-used while
+            // n_active repeats.  Same f64 operations on the same values for every term that can change the sum.
+            const double dn = (double)nmw;
+            const bool copy = (!direct) && off >= 0;
+            int32_t* pn = copy ? a.pool.n_active + off : nullptr;
+            double* pt = copy ? a.pool.tick + off : nullptr;
+            const int32_t* sn = y.tr_n; const double* stt = y.tr_tick; const int sstr = y.tr_stride;
+            const bool skip_zero = can_util && (jct > 0.0) && !isinf(jct);
+            int last_n = -1;
+            double last_q = 0.0;
+#pragma unroll 4
+            for (int k = 0; k < n_rec; ++k) {
+                const int nk = sn[(size_t)k * sstr];
+                const double tk = stt[(size_t)k * sstr];
+                if (copy) { pn[k] = nk; pt[k] = tk; }
+                if (!can_util) continue;
+                if (skip_zero && (nk == 0 || tk == 0.0)) continue;
+                if (nk != last_n) { last_n = nk; last_q = __ddiv_rn((double)nk, dn); }
+                util = __dadd_rn(util, __dmul_rn(last_q, __ddiv_rn(tk, jct)));
             }
         }
-        __syncwarp();
+        a.res.jct[item.slot] = jct;
+        a.res.comm[item.slot] = __dmul_rn(S.comm, steps);
+        a.res.comp[item.slot] = __dmul_rn(S.comp, steps);
+        a.res.n_ticks[item.slot] = R.tick_no;
+        a.res.util[item.slot] = can_util ? util : 0.0;
+        a.res.util_nmw[item.slot] = can_util ? nmw : -1;
+        a.res.trace_off[item.slot] = off;
+        a.res.status[item.slot] = status;
+        if (a.stats) {
+            atomicAdd(&a.stats->lookaheads, 1ull);
+            atomicAdd(&a.stats->alg_bytes, (unsigned long long)(TD.algorithmic_bytes_static + 12ull * (unsigned long long)R.tick_no));
+            atomicAdd(&a.stats->quotient_bytes, (unsigned long long)(20ull * n_ops + 19ull * n_deps + 24ull + 12ull * (unsigned long long)R.tick_no));
+        }
     }
 }
 
