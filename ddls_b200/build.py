@@ -23,21 +23,23 @@ def nvcc_path():
     return p
 
 
-def is_stale():
-    if not os.path.exists(LIB_PATH):
+def is_stale(out=LIB_PATH):
+    if not os.path.exists(out):
         return True
-    t = os.path.getmtime(LIB_PATH)
+    t = os.path.getmtime(out)
     return any(os.path.getmtime(d) > t for d in DEPS)
 
 
-def build(force=False, verbose=False, extra_flags=()):
-    if not force and not is_stale():
-        return LIB_PATH
-    cmd = [nvcc_path()] + NVCC_FLAGS + list(extra_flags) + ['-o', LIB_PATH] + SOURCES
+def build(force=False, verbose=False, extra_flags=(), out=LIB_PATH):
+    """out: where the library goes; measurement variants (extra -D flags) are built elsewhere than LIB_PATH."""
+    if not force and not is_stale(out):
+        return out
+    os.makedirs(os.path.dirname(os.path.abspath(out)), exist_ok=True)
+    cmd = [nvcc_path()] + NVCC_FLAGS + list(extra_flags) + ['-o', out] + SOURCES
     if verbose:
         print(' '.join(cmd))
     subprocess.check_call(cmd)
-    return LIB_PATH
+    return out
 
 
 if __name__ == '__main__':

@@ -374,8 +374,7 @@ bool build_resident_blob(const ramp_lowered_job_t* j, const ramp_quotient_t& q, 
     const size_t off_rec = off;                 off += align_up((uint64_t)N * 16, 16);
     h.off_op_row = (int32_t)off;                off += align_up((uint64_t)N * 8, 16);
     h.off_op_thr = (int32_t)off;                off += align_up((uint64_t)N * 4, 16);
-    h.off_dep_kd = (int32_t)off;                off += align_up((uint64_t)std::max(E, 1) * 8, 16);
-    h.off_dep_rt = (int32_t)off;                off += align_up((uint64_t)std::max(E, 1) * 8, 16);
+    h.off_out = (int32_t)off;                   off += align_up((uint64_t)std::max(E, 1) * 16, 16);
     h.off_src = (int32_t)off;                   off += align_up((uint64_t)std::max<size_t>(src.size(), 1) * 4, 16);
     if (off > (size_t)max_bytes) return false;
     h.total_bytes = (int32_t)off;
@@ -385,18 +384,26 @@ bool build_resident_blob(const ramp_lowered_job_t* j, const ramp_quotient_t& q, 
     OpRec* rec = reinterpret_cast<OpRec*>(blob.data() + off_rec);
     int32_t* row = reinterpret_cast<int32_t*>(blob.data() + h.off_op_row);
     uint32_t* thr = reinterpret_cast<uint32_t*>(blob.data() + h.off_op_thr);
-    unsigned long long* kd = reinterpret_cast<unsigned long long*>(blob.data() + h.off_dep_kd);
-    double* rt = reinterpret_cast<double*>(blob.data() + h.off_dep_rt);
+    struct OutRec { double run_time; uint32_t lo, hi; };      // = the ready-flow frontier entry the kernel copies it to
+    static_assert(sizeof(OutRec) == 16, "out-entry record is 16 bytes");
+    OutRec* out = reinterpret_cast<OutRec*>(blob.data() + h.off_out);
     for (int32_t c = 0; c < N; ++c) {
         rec[c] = OpRec{q.op_cost[c] + 0.0, q.op_key[c], q.op_worker[c] | (q.op_weight[c] << 16)};
-        row[2 * c] = q.row_ptr[c]; row[2 * c + 1] = q.row_ptr[c + 1] - q.row_ptr[c];
         thr[c] = q.op_threshold[c];
-    }
-    for (int32_t k = 0; k < E; ++k) {
-        const uint32_t lo = dense_key[k] | (uint32_t)(q.dep_group_mask[k] << h.cshift);
-        const uint32_t hi = (q.dep_is_flow[k] ? 1u : 0u) | (q.dep_inc[k] << h.ishift) | ((uint32_t)q.dep_dst[k] << h.dshift);
-        kd[k] = (unsigned long long)lo | ((unsigned long long)hi << 32);
-        rt[k] = q.dep_run_time[k] + 0.0;
+        // the class's out-entries, flows first, each group in entry order: completing the class appends them to the ready-flow
+        // and ready-non-flow lists in the same order as a walk over the entries would
+        int32_t pos = q.row_ptr[c], n_fl = 0;
+        for (int pass = 0; pass < 2; ++pass)
+            for (int32_t k = q.row_ptr[c]; k < q.row_ptr[c + 1]; ++k) {
+                if ((q.dep_is_flow[k] != 0) != (pass == 0)) continue;
+                const uint32_t lo = dense_key[k] | (uint32_t)(q.dep_group_mask[k] << h.cshift);
+                const uint32_t hi = (q.dep_is_flow[k] ? 1u : 0u) | (q.dep_inc[k] << h.ishift) | ((uint32_t)q.dep_dst[k] << h.dshift);
+                out[pos++] = OutRec{q.dep_run_time[k] + 0.0, lo, hi};
+                n_fl += pass == 0;
+            }
+        const int32_t n_nf = q.row_ptr[c + 1] - q.row_ptr[c] - n_fl;
+        if (n_fl > 0xFFFF || n_nf > 0x7FFF) return false;
+        row[2 * c] = q.row_ptr[c]; row[2 * c + 1] = n_fl | (n_nf << 16);
     }
     if (!src.empty()) memcpy(blob.data() + h.off_src, src.data(), sizeof(int32_t) * src.size());
     return true;
@@ -482,6 +489,22 @@ void ramp_internal_count_launches(ramp_engine_t* e, int n) { e->launches += n; }
 extern "C" {
 
 const char* ramp_last_error(void) { return g_last_error.c_str(); }
+
+#ifdef RAMP_TICK_CLOCKS
+// measurement builds only (scripts/tick_cycles.py): the thread kernel's cycle ledger summed over CTAs into
+// out[RAMP_TC_SHAPES][RAMP_TC_PHASES + 1] (cycles per phase, then ticks), on the current device; reset = 1 zeroes it after
+int ramp_debug_tick_clocks(unsigned long long* out, int reset) {
+    static unsigned long long h[RAMP_TC_MAX_CTAS][RAMP_TC_SHAPES][RAMP_TC_PHASES + 1];
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemcpyFromSymbol(h, ramp::ramp_tick_clocks, sizeof(h)));
+    memset(out, 0, sizeof(h[0]));
+    for (int b = 0; b < RAMP_TC_MAX_CTAS; ++b)
+        for (int s = 0; s < RAMP_TC_SHAPES; ++s)
+            for (int i = 0; i <= RAMP_TC_PHASES; ++i) out[s * (RAMP_TC_PHASES + 1) + i] += h[b][s][i];
+    if (reset) { memset(h, 0, sizeof(h)); CUDA_TRY(cudaMemcpyToSymbol(ramp::ramp_tick_clocks, h, sizeof(h))); }
+    return RAMP_OK;
+}
+#endif
 
 int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     if (!cfg_in || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");

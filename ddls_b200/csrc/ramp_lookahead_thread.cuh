@@ -8,7 +8,7 @@
 //   * a CTA is a sim warp and a ledger warp (below); it pulls CHUNKS of up to 32 work items that use the same template
 //     (ramp_bucket_kernel groups the step's memo misses by template), so the sim lanes run the same instruction stream over
 //     the same template -- no divergence, and every template read is a shared-memory broadcast;
-//   * the template blob (header + op records + rows + thresholds + packed dep words + run times) is copied into shared
+//   * the template blob (header + op records + rows + thresholds + out-entry records) is copied into shared
 //     memory ONCE per chunk with a bulk async copy (cp.async.bulk -> UBLKCP, completion on an mbarrier), so a tick never
 //     waits for L2;
 //   * per-lane state is lane-interleaved in shared memory ([slot][lane]: conflict-free): u16 parent counters per op
@@ -60,8 +60,8 @@ struct ResHeader {
     int32_t n_src, num_training_steps, orig_workers, _pad0;
     uint32_t kmask, cmask, imask, _pad1;               // dep word lo: key | SET of channel groups << cshift (empty: no channel);
     int32_t cshift, fshift, ishift, dshift;            // dep word hi: flow | inc << 1 | child << dshift  (fshift = 0, ishift = 1)
-    int32_t off_op_row, off_op_thr, off_dep_kd, off_dep_rt;   // byte offsets from the blob start (op records follow the header)
-    int32_t off_src, total_bytes, _pad2, _pad3;
+    int32_t off_op_row, off_op_thr, off_out, off_src;  // byte offsets from the blob start (op records follow the header)
+    int32_t total_bytes, _pad2, _pad3, _pad4;
 };
 static_assert(sizeof(ResHeader) == 96, "resident header is 96 bytes");
 
@@ -232,6 +232,43 @@ __device__ __forceinline__ uint32_t ld_acquire_cta(const uint32_t* p) {
     return v;
 }
 
+#ifdef RAMP_TICK_CLOCKS
+// Cycle ledger of the sim lane, for measurement builds only (scripts/tick_cycles.py builds them; the library built without
+// the switch has no trace of it).  Every sim lane reads clock() at the phase boundaries of each tick -- all lanes, so the
+// warp stays converged -- and lane 0 adds the deltas to its CTA's row of ramp_tick_clocks, keyed by the tick's frontier
+// shape.  A tick runs from its first stamp to the next tick's first stamp (or the loop's exit), so the phases add up to
+// the tick loop's time.  The atomics are fire-and-forget reductions issued at the start of the next tick.
+#define RAMP_TC_SHAPES 64       // ready op classes {0, 1, 2, >2} x ready flow entries {0..6, >6} x non-flow tick or not
+#define RAMP_TC_PHASES 5        // A/B | D, E and the ring record | H | G | compaction, exit test and the loop's back edge
+#define RAMP_TC_MAX_CTAS 1024
+__device__ unsigned long long ramp_tick_clocks[RAMP_TC_MAX_CTAS][RAMP_TC_SHAPES][RAMP_TC_PHASES + 1];   // deltas, then ticks
+
+struct TickClocks {
+    uint32_t c[RAMP_TC_PHASES];
+    int shape = -1;
+    int lane;
+    __device__ __forceinline__ void flush(uint32_t now) {
+        if (shape >= 0 && lane == 0 && blockIdx.x < RAMP_TC_MAX_CTAS) {
+            unsigned long long* t = ramp_tick_clocks[blockIdx.x][shape];
+#pragma unroll
+            for (int i = 0; i < RAMP_TC_PHASES; ++i) atomicAdd(t + i, (unsigned long long)(((i + 1 < RAMP_TC_PHASES) ? c[i + 1] : now) - c[i]));
+            atomicAdd(t + RAMP_TC_PHASES, 1ull);
+        }
+    }
+    __device__ __forceinline__ void begin(int nO, int nF, bool nf) {
+        const uint32_t now = (uint32_t)clock();
+        flush(now);
+        shape = ((nO > 2 ? 3 : nO) * 8 + (nF > 6 ? 7 : nF)) * 2 + (nf ? 1 : 0);
+        c[0] = now;
+    }
+    __device__ __forceinline__ void stamp(int i) { c[i] = (uint32_t)clock(); }
+    __device__ __forceinline__ void finish() { flush((uint32_t)clock()); }
+};
+#define RAMP_TC(...) __VA_ARGS__
+#else
+#define RAMP_TC(...)
+#endif
+
 struct SimFinal { int status, tick_no, max_o, max_f, max_nf; };   // what the sim lane hands over with its last record
 
 struct LedgerFeed {                   // the sim lane's end of its ring
@@ -272,10 +309,9 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
     const int lane = x.lane;
     const ResHeader& H = *reinterpret_cast<const ResHeader*>(x.tm);
     const int4* op_rec = reinterpret_cast<const int4*>(x.tm + sizeof(ResHeader));                  // {cost.lo, cost.hi, key, worker | weight << 16}
-    const int2* op_row = reinterpret_cast<const int2*>(x.tm + H.off_op_row);
+    const int2* op_row = reinterpret_cast<const int2*>(x.tm + H.off_op_row);                        // {first, n flows | n non-flows << 16}
     const uint32_t* op_thr = reinterpret_cast<const uint32_t*>(x.tm + H.off_op_thr);
-    const uint2* dep_kd = reinterpret_cast<const uint2*>(x.tm + H.off_dep_kd);
-    const double* dep_rt = reinterpret_cast<const double*>(x.tm + H.off_dep_rt);
+    const int4* out_rec = reinterpret_cast<const int4*>(x.tm + H.off_out);                          // ready-flow entries, as appended
     const int32_t* src_ops = reinterpret_cast<const int32_t*>(x.tm + H.off_src);
     const int N = H.n_ops, E = H.n_deps, W = H.n_workers, C = H.n_channels;
     const uint32_t kmask = H.kmask, imask = H.imask;
@@ -291,14 +327,26 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
 
     for (int i = 0; i < N && i < x.n_cap; ++i) cnt[i * 32] = 0;
     int nO = H.n_src, nF = 0, nNF = 0;
+    // JOB:496-506: a completed class's out-entries become ready.  The blob stores them as ready-made frontier entries, flows
+    // first (ramp_engine.cu, build_resident_blob): straight copies, no per-entry flow test or second load
+    auto complete_op = [&](const int op) {
+        const int2 row = op_row[op];
+        const int e_nf = row.x + (row.y & 0xffff), e_end = e_nf + (row.y >> 16);
+        _Pragma("unroll 1")
+        for (int e = row.x; e < e_nf; ++e) { flows.put(nF, out_rec[e]); ++nF; }
+        _Pragma("unroll 1")
+        for (int e = e_nf; e < e_end; ++e) { nfs.put(nNF, (uint32_t)out_rec[e].w); ++nNF; }
+    };
     for (int k = 0; k < nO; ++k) { const int op = src_ops[k]; ops.put(k, op_rec[op], op); }       // RCE:1334
     SimFinal R;
     R.tick_no = 0; R.max_o = nO; R.max_f = 0; R.max_nf = 0;
     R.status = (N <= x.n_cap) ? RAMP_ST_OK : RAMP_ST_TABLE_FULL;                                    // cannot happen (eligibility)
     int to_complete = N + E;              // ops and deps still to complete (JOB:549-551)
     LedgerFeed feed{x.ring, x.head, x.tail, x.fin, lane, 0u, (uint32_t)RAMP_T_RING};
+    RAMP_TC(TickClocks tc; tc.lane = lane;)
 
     if (R.status == RAMP_ST_OK) for (;;) {       // left through ONE combined exit test per tick
+        RAMP_TC(tc.begin(nO, nF, nNF > 0);)
         if (nF <= RAMP_T_FASTF && nO <= 2) {
             // ======== small frontiers (the usual case on a quotient): every ready item is loaded ONCE into registers and each
             // phase runs code specialised for the exact number of ready ops (0-2) and flows (0-4): winners by pairwise
@@ -321,6 +369,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                 }
                 if (ow0) { const u64_t r0 = rem_bits(orr[0]); t_op = (r0 < t_op) ? r0 : t_op; n_active += (int)((uint32_t)orr[0].w >> 16); }
             }
+            RAMP_TC(tc.stamp(1);)
             // ---- C, D, E, I, J, H: dispatched ONCE on the number of ready flow entries; each case is straight-line code ----
             const bool any_nf = nNF > 0;
             u64_t tick_b = 0ull;
@@ -342,6 +391,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                 feed.put(tick_b, n_active, ticked_flows);
                 if (R.tick_no >= x.tr_cap) R.status = RAMP_ST_TRACE_OVERFLOW;
                 ++R.tick_no;
+                RAMP_TC(tc.stamp(2);)
             };
             auto flow_tick = [&](auto nf_tag) {
                 constexpr int NF = decltype(nf_tag)::value;
@@ -392,6 +442,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                 else if (opaque(nF) == 5) flow_tick(std::integral_constant<int, 5>{});
                 else flow_tick(std::integral_constant<int, 6>{});
             }
+            RAMP_TC(tc.stamp(3);)
             // ---- G ----
             int p = 0;
             auto tick_op = [&](int4 r, const int op, const bool win) {
@@ -399,16 +450,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                     const u64_t rb = rem_bits(r);
                     if (rb <= tick_b) {                                                             // JOB:555-556
                         --to_complete;
-                        const int2 row = op_row[op];
-                        _Pragma("unroll 1")
-                        for (int e = row.x; e < row.x + row.y; ++e) {                               // JOB:496-506
-                            const uint2 kd = dep_kd[e];
-                            if (kd.y & 1u) {
-                                const double rt = dep_rt[e];
-                                flows.put(nF, make_int4(__double2loint(rt), __double2hiint(rt), (int)kd.x, (int)kd.y));
-                                ++nF;
-                            } else { nfs.put(nNF, kd.y); ++nNF; }
-                        }
+                        complete_op(op);
                         return;
                     }
                     const double rem = __dsub_rn(__longlong_as_double((long long)rb), tick);
@@ -420,6 +462,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                 tick_op(orr[0], oi[0], ow0);
                 if (nO == 2) tick_op(orr[1], oi[1], ow1);
             }
+            RAMP_TC(tc.stamp(4);)
             if (tailO != nO) {
                 _Pragma("unroll 1")
                 for (int k = nO; k < tailO; ++k, ++p) { if (p != k) ops.put(p, ops.rec(k), ops.idx(k)); }
@@ -487,6 +530,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                 }
             }
         }
+        RAMP_TC(tc.stamp(1);)
         // ---- C, D ----
         const bool any_nf = nNF > 0;
         u64_t t_comm = 0ull;
@@ -547,6 +591,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
         feed.put(tick_b, n_active, (!any_nf) && (nF > 0));
         if (R.tick_no >= x.tr_cap) R.status = RAMP_ST_TRACE_OVERFLOW;
         ++R.tick_no;
+        RAMP_TC(tc.stamp(2);)
         // ---- H ----
         int tailO = nO;                       // ops readied in this tick are appended behind the current frontier
         auto complete_dep = [&](const uint32_t hi) {                                                // JOB:525-536
@@ -577,6 +622,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
             }
             nF = p;
         }
+        RAMP_TC(tc.stamp(3);)
         // ---- G ----
         int p = 0;
         _Pragma("unroll 1")
@@ -591,16 +637,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                 const u64_t rb = rem_bits(r);
                 if (rb <= tick_b) {                                                                 // JOB:555-556
                     --to_complete;
-                    const int2 row = op_row[op];
-                    _Pragma("unroll 1")
-                    for (int e = row.x; e < row.x + row.y; ++e) {                                   // JOB:496-506
-                        const uint2 kd = dep_kd[e];
-                        if (kd.y & 1u) {
-                            const double rt = dep_rt[e];
-                            flows.put(nF, make_int4(__double2loint(rt), __double2hiint(rt), (int)kd.x, (int)kd.y));
-                            ++nF;
-                        } else { nfs.put(nNF, kd.y); ++nNF; }
-                    }
+                    complete_op(op);
                     continue;
                 }
                 const double rem = __dsub_rn(__longlong_as_double((long long)rb), tick);
@@ -608,6 +645,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
             }
             ops.put(p, r, op); ++p;
         }
+        RAMP_TC(tc.stamp(4);)
         _Pragma("unroll 1")
         for (int k = nO; k < tailO; ++k, ++p) { if (p != k) ops.put(p, ops.rec(k), ops.idx(k)); }
         nO = p;
@@ -622,6 +660,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
             break;
         }
     }
+    RAMP_TC(tc.finish();)
     feed.finish(R);
 }
 
@@ -801,8 +840,14 @@ __global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(
             if (active) {
                 x.tr_cap = s_tr_cap[lane];
                 const bool simple = (H.n_workers == 1) && (H.n_channels <= 1);
-                if (fast) { if (simple) thread_lookahead<false, true>(x); else thread_lookahead<false, false>(x); }
-                else { if (simple) thread_lookahead<true, true>(x); else thread_lookahead<true, false>(x); }
+                // one instantiation per line: scripts/tick_cycles.py finds each one's SASS by the line it is inlined at
+                if (fast) {
+                    if (simple) thread_lookahead<false, true>(x);
+                    else thread_lookahead<false, false>(x);
+                } else {
+                    if (simple) thread_lookahead<true, true>(x);
+                    else thread_lookahead<true, false>(x);
+                }
             }
             continue;
         }
