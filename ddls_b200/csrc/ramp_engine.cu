@@ -1103,6 +1103,22 @@ int ramp_get_last_lookahead(ramp_engine_t* e, int32_t episode, ramp_lookahead_re
     return RAMP_OK;
 }
 
+int ramp_debug_template_info(ramp_engine_t* e, int32_t template_id, int32_t out[7], double* hint_jct) {
+    if (!e || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (template_id < 0 || template_id >= (int32_t)e->templates.size()) return set_error(RAMP_ERR_BAD_ARG, "template id %d is not registered", template_id);
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    const TemplateDev& d = e->templates[template_id].dev;
+    TemplateHints h{};
+    double hj = 0.0;
+    CUDA_TRY(cudaMemcpy(&h, e->d_hints + template_id, sizeof(TemplateHints), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&hj, e->d_hint_jct + template_id, sizeof(double), cudaMemcpyDeviceToHost));
+    out[0] = d.size_class; out[1] = d.res_n_ops; out[2] = d.res_n_deps;
+    out[3] = h.n_ticks; out[4] = h.max_o; out[5] = h.max_f; out[6] = h.max_nf;
+    if (hint_jct) *hint_jct = hj;
+    return RAMP_OK;
+}
+
 int ramp_run_lookaheads(ramp_engine_t* e, const int32_t* template_ids, int32_t n, ramp_lookahead_result_t* results,
                         int32_t* trace_n, double* trace_tick, int32_t trace_cap, float* kernel_ms_out) {
     if (!e || !template_ids || !results || n < 0) return set_error(RAMP_ERR_BAD_ARG, "bad argument");

@@ -49,8 +49,17 @@ namespace ramp {
 #endif
 #define RAMP_T_WCAP 8       // worker groups / channel groups with a per-lane winner table (more: pairwise comparison)
 #define RAMP_T_CCAP 32
+#ifndef RAMP_T_RING
 #define RAMP_T_RING 32      // tick records per lane in the sim -> ledger ring (a power of two)
+#endif
+#ifndef RAMP_T_PUB
 #define RAMP_T_PUB 8        // the sim lane publishes its record count every this many ticks (a power of two, <= RAMP_T_RING)
+#endif
+// the small-frontier path reads the first RAMP_T_FASTF flow entries and 2 op classes straight from shared memory, and every
+// list keeps at least one entry there
+static_assert(RAMP_T_FCAP >= RAMP_T_FASTF && RAMP_T_OCAP >= 2 && RAMP_T_NFCAP >= 1, "shared-memory capacities below the small-frontier path");
+// RAMP_T_LEDGER_NS (off in the normal build): the ledger lane sleeps that many nanoseconds per record it consumes, so it stays
+// behind its sim lane and the sim lane's ring-full wait runs on every template with enough ticks (tests/test_gpu_thread_kernel.py)
 #define RAMP_T_DONE 0x80000000u   // set in the published count with the sim lane's last record
 #define RAMP_THREAD_CTA 64  // threads of a thread-kernel CTA: the sim warp and the ledger warp
 
@@ -708,6 +717,9 @@ __device__ __forceinline__ LedgerSums ledger_run(const LedgerCtx& y) {
             }
             S.t = __dadd_rn(S.t, tick);
             if ((int)k < y.tr_cap) { y.tr_n[tr_idx] = n_active; y.tr_tick[tr_idx] = tick; tr_idx += y.tr_stride; }
+#ifdef RAMP_T_LEDGER_NS
+            __nanosleep(RAMP_T_LEDGER_NS);
+#endif
         }
         st_release_cta(y.tail, k);
     }

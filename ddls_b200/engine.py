@@ -104,6 +104,7 @@ def load_library():
     L.ramp_get_last_lookahead.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
     L.ramp_run_lookaheads.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_int32, C.POINTER(C.c_float)]
+    L.ramp_debug_template_info.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_double)]
     L.ramp_launch_count.restype = C.c_int64
     L.ramp_launch_count.argtypes = [C.c_void_p]
     L.ramp_get_lookahead_kernel_time.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64),
@@ -111,7 +112,8 @@ def load_library():
     for name in ('ramp_engine_create', 'ramp_engine_destroy', 'ramp_register_template', 'ramp_template_count',
                  'ramp_reset', 'ramp_set_arrivals', 'ramp_step_host', 'ramp_step_device', 'ramp_sync', 'ramp_check_status',
                  'ramp_get_job_records', 'ramp_get_episode_state', 'ramp_episode_state_device', 'ramp_export_episode_state_to',
-                 'ramp_get_memo_stats', 'ramp_get_memo_stats_ex', 'ramp_get_last_lookahead', 'ramp_run_lookaheads', 'ramp_get_lookahead_kernel_time'):
+                 'ramp_get_memo_stats', 'ramp_get_memo_stats_ex', 'ramp_get_last_lookahead', 'ramp_run_lookaheads',
+                 'ramp_debug_template_info', 'ramp_get_lookahead_kernel_time'):
         getattr(L, name).restype = C.c_int
     _lib = L
     return L
@@ -122,7 +124,7 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_step_device', 'ramp_sync', 'ramp_check_status', 'ramp_get_job_records',
                     'ramp_get_episode_state', 'ramp_episode_state_device', 'ramp_export_episode_state_to',
                     'ramp_get_memo_stats', 'ramp_get_memo_stats_ex',
-                    'ramp_get_last_lookahead', 'ramp_run_lookaheads', 'ramp_launch_count',
+                    'ramp_get_last_lookahead', 'ramp_run_lookaheads', 'ramp_debug_template_info', 'ramp_launch_count',
                     'ramp_get_lookahead_kernel_time', 'ramp_expand_template', 'ramp_free_expanded_job', 'ramp_free_expanded_aux', 'ramp_first_fit_place',
                     'ramp_quotient_template', 'ramp_free_quotient', 'ramp_get_quotient_bytes', 'ramp_set_job_count',
                     'ramp_set_limits', 'ramp_first_fit_place_many', 'ramp_env_create', 'ramp_env_set_template',
@@ -308,6 +310,16 @@ class RampEngine:
         if want_trace:
             return res, ms.value, tn, tt
         return res, ms.value
+
+    def template_info(self, template_id):
+        """How a registered template runs: size_class (2 = resident, on the thread-per-lookahead kernel), the resident
+        quotient's n_ops / n_deps, and the TemplateHints its first completed lookahead recorded (n_ticks, max_o, max_f,
+        max_nf; 0 before) with hint_jct."""
+        out = (C.c_int32 * 7)()
+        hj = C.c_double(0.0)
+        _check(self._L.ramp_debug_template_info(self._h, int(template_id), out, C.byref(hj)))
+        return dict(size_class=out[0], res_n_ops=out[1], res_n_deps=out[2], n_ticks=out[3], max_o=out[4], max_f=out[5],
+                    max_nf=out[6], hint_jct=hj.value)
 
     @property
     def launch_count(self):

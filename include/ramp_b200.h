@@ -222,6 +222,12 @@ int ramp_get_last_lookahead(ramp_engine_t* eng, int32_t episode, ramp_lookahead_
 int ramp_run_lookaheads(ramp_engine_t* eng, const int32_t* template_ids, int32_t n,
                         ramp_lookahead_result_t* results, int32_t* trace_n_active, double* trace_tick,
                         int32_t trace_cap, float* kernel_ms_out);
+/* How a registered template runs, for tests and diagnostics: out[0] size class (2 = resident: the thread-per-lookahead
+ * kernel on its quotient, 0 / 1 = the warp / CTA kernels), out[1..2] the resident quotient's classes and dep entries
+ * (0 when not resident), out[3..6] what the first completed lookahead of the template recorded for the later ones
+ * (ticks, largest ready-op / ready-flow / ready-non-flow frontiers; all 0 before), *hint_jct (may be NULL) its job
+ * completion time.  Waits for the engine stream. */
+int ramp_debug_template_info(ramp_engine_t* eng, int32_t template_id, int32_t out[7], double* hint_jct);
 
 /* kernel launch counter (gpu_launches in bench.py) and device time spent in the lookahead kernel inside
  * ramp_step_* since the last call (CUDA events on the engine stream) */

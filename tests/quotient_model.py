@@ -196,6 +196,9 @@ def run_lookahead_quotient(q):
     ops_completed = deps_completed = 0
     INF = math.inf
     finished = False
+    # the frontier peaks the thread kernel records in TemplateHints: ready op classes counted with the classes readied in the
+    # tick (the kernel appends them behind the frontier before it compacts it), ready flow / non-flow entries after the tick
+    max_o, max_f, max_nf = len(ops), 0, 0
     while True:
         wkey = {}
         for op, rem in ops:
@@ -249,6 +252,7 @@ def run_lookahead_quotient(q):
                     deps_completed += 1
                 else:
                     survivors.append([e, r2])
+        max_o = max(max_o, len(ops) + len(ops_next))
         win_set = {op for op, _ in winners}
         arrivals = []
         for op, rem in ops:
@@ -267,10 +271,31 @@ def run_lookahead_quotient(q):
                 nf.append(e)
         flows = survivors
         ops = ops_next
+        max_f, max_nf = max(max_f, len(flows)), max(max_nf, len(nf))
         finished = ops_completed == N and deps_completed == E
         if finished or math.isinf(tick):
             break
     steps = float(q.num_training_steps)
     return dict(jct=t * steps, comm=comm * steps, comp=comp * steps, n_ticks=len(trace_tick),
                 trace_n_active=np.array(trace_n, dtype=np.int32), trace_tick=np.array(trace_tick, dtype=np.float64),
-                finished=finished)
+                finished=finished, max_o=max_o, max_f=max_f, max_nf=max_nf)
+
+
+def identity_quotient(job):
+    """Every op its own class (ramp_engine.cu identity_quotient): what RAMP_LOOKAHEAD_MODE=thread_unfolded simulates."""
+    from ddls_b200.quotient import QuotientJob
+    job.canonicalise()
+    N, E, C = job.n_ops, job.n_deps, job.n_channels
+    chan = job.dep_channel.astype(np.int64)
+    has_ch = chan != 0xFFFF
+    masks_valid = C <= 64
+    mask = np.array([(1 << int(c)) if (h and masks_valid) else 0 for c, h in zip(chan, has_ch)], dtype=np.uint64)
+    return QuotientJob(n_ops=N, n_deps=E, n_workers=job.n_workers, n_channels=C, num_training_steps=job.num_training_steps,
+                       op_cost=job.op_cost + 0.0, op_key=np.array(rank_keys(job.op_prio), dtype=np.int64),
+                       op_worker=job.op_worker.astype(np.int64), op_weight=np.ones(N, dtype=np.int64),
+                       op_threshold=job.op_n_parents.astype(np.int64), row_ptr=job.row_ptr.astype(np.int64),
+                       dep_dst=job.dep_dst.astype(np.int64), dep_run_time=job.dep_run_time + 0.0,
+                       dep_key=np.array(rank_keys(job.dep_prio), dtype=np.int64),
+                       dep_channel=np.where(has_ch, chan, 0xFFFFFFFF), dep_is_flow=job.dep_is_flow.astype(np.uint8),
+                       dep_inc=np.ones(E, dtype=np.int64), op_class=np.arange(N, dtype=np.int64),
+                       dep_entry=np.arange(E, dtype=np.int64), dep_group_mask=mask, merged=0, masks_valid=int(masks_valid))

@@ -30,27 +30,42 @@ def eng_mod():
 # every lookahead kernel: one THREAD per lookahead on the symmetry quotient (the default whenever the quotient fits shared
 # memory), the same kernel on the unfolded job, one warp per lookahead, one CTA per lookahead
 MODES = ['thread', 'thread_unfolded', 'warp', 'cta']
+THREAD_MODES = ['thread', 'thread_unfolded']
+# every mode on a template's first launch, and the thread kernel's second route too: a later launch of a template reads the
+# TemplateHints the first one recorded, keeps every list in shared memory, writes its trace in place and sums the utilisation
+# inside the tick loop (the warp / CTA kernels keep no hints)
+MODE_LAUNCHES = [pytest.param(m, 'first', id=m) for m in MODES] + [pytest.param(m, 'hinted', id=f'{m}-hinted') for m in THREAD_MODES]
 
 
-def _run_all_templates(engine, templates, n_cluster_workers=64, repeat=1, mode='auto'):
+def _run_all_templates(engine, templates, n_cluster_workers=64, repeat=1, mode='auto', launch='first', trace_cap=1 << 16,
+                       want_info=False):
+    """launch='first': one run_lookaheads (every template's first run); 'hinted': the same run once without a trace, which
+    records the hints, then again with the trace -- the second run's results.  want_info: also each template's
+    engine.template_info after the runs."""
     import os
     os.environ['RAMP_LOOKAHEAD_MODE'] = mode
     try:
-        eng = engine.RampEngine(n_episodes=1, n_cluster_workers=n_cluster_workers, max_jobs=1, trace_cap=1 << 16)
+        eng = engine.RampEngine(n_episodes=1, n_cluster_workers=n_cluster_workers, max_jobs=1, trace_cap=trace_cap)
     finally:
         os.environ.pop('RAMP_LOOKAHEAD_MODE', None)
     tids = [eng.register_template(t) for t in templates]
-    res, ms, tn, tt = eng.run_lookaheads(np.repeat(tids, repeat), want_trace=True)
+    ids = np.repeat(tids, repeat)
+    if launch == 'hinted':
+        eng.run_lookaheads(ids)
+    else:
+        assert launch == 'first', launch
+    res, ms, tn, tt = eng.run_lookaheads(ids, want_trace=True)
+    info = [eng.template_info(t) for t in tids] if want_info else None
     eng.close()
-    return res, tn, tt
+    return (res, tn, tt, info) if want_info else (res, tn, tt)
 
 
-@pytest.mark.parametrize('mode', MODES)
+@pytest.mark.parametrize('mode,launch', MODE_LAUNCHES)
 @pytest.mark.parametrize('fname', FILES)
-def test_lookahead_vs_reference_golden(fname, mode, eng_mod):
+def test_lookahead_vs_reference_golden(fname, mode, launch, eng_mod):
     """_run_lookahead RCE:379-467: (jct, comm, comp) and the whole tick trace equal the reference's, bit for bit."""
     g = Golden(fname)
-    res, tn, tt = _run_all_templates(eng_mod, g.templates, g.n_cluster_workers, mode=mode)
+    res, tn, tt = _run_all_templates(eng_mod, g.templates, g.n_cluster_workers, mode=mode, launch=launch)
     assert (res['status'] == 0).all()
     for i in range(g.n_lookaheads):
         la = g.lookahead(i)
@@ -62,12 +77,12 @@ def test_lookahead_vs_reference_golden(fname, mode, eng_mod):
         assert res['jct'][k] == la['jct'] and res['comm'][k] == la['comm'] and res['comp'][k] == la['comp']
 
 
-@pytest.mark.parametrize('mode', MODES)
+@pytest.mark.parametrize('mode,launch', MODE_LAUNCHES)
 @pytest.mark.parametrize('fname', FILES)
-def test_lookahead_vs_oracle_all_templates(fname, mode, eng_mod, oracle_lib):
+def test_lookahead_vs_oracle_all_templates(fname, mode, launch, eng_mod, oracle_lib):
     """Every lowered Action in the fixtures (not only the un-memoised ones) against the CPU oracle."""
     g = Golden(fname)
-    res, tn, tt = _run_all_templates(eng_mod, g.templates, g.n_cluster_workers, repeat=3, mode=mode)
+    res, tn, tt = _run_all_templates(eng_mod, g.templates, g.n_cluster_workers, repeat=3, mode=mode, launch=launch)
     for k, t in enumerate(g.templates):
         o = oracle_lib.run_lookahead(t)
         for rep in range(3):
@@ -224,15 +239,29 @@ def test_fused_empty_steps_match_separate_steps(eng_mod):
     e1.close(); e2.close()
 
 
-@pytest.mark.parametrize('mode', MODES)
-def test_random_templates_vs_oracle(mode, eng_mod, oracle_lib):
+def zero_jct_template():
+    """Every op zero-cost and every flow zero-time: jct == 0, so hint_jct == 0 and a hinted launch sums no utilisation
+    in its tick loop (the reference would divide by zero computing it, RCE:832; only the lookahead is run here)."""
+    from ddls_b200.lowered import LoweredJob, MountScalars
+    # op 0 -> op 1 (flow on channel 0, run time 0) and op 0 -> op 2 (non-flow), op 1 -> op 2 (flow); two workers
+    return LoweredJob(n_ops=3, n_deps=3, n_workers=2, n_channels=1, num_training_steps=2, model_id=0, degree=1,
+                      op_cost=np.zeros(3), op_prio=np.array([2, 1, 0]), op_worker=np.array([0, 1, 0]),
+                      op_n_parents=np.array([0, 1, 2]), row_ptr=np.array([0, 2, 3, 3]), dep_dst=np.array([1, 2, 2]),
+                      dep_run_time=np.zeros(3), dep_prio=np.array([0, 1, 2]), dep_channel=np.array([0, 0xFFFF, 0]),
+                      dep_is_flow=np.array([1, 0, 1]), mount=MountScalars(n_mounted_workers=2)).canonicalise()
+
+
+@pytest.mark.parametrize('mode,launch', MODE_LAUNCHES)
+def test_random_templates_vs_oracle(mode, launch, eng_mod, oracle_lib):
     """Adversarial random lowered jobs: priority ties, zero-cost ops, zero-time flows, flows without a channel,
-    mutual edges, deadlocks (status INFINITE_TICK must match too)."""
+    mutual edges, deadlocks (status INFINITE_TICK must match too), and a job whose completion time is 0."""
     from ddls_b200.template_builder import random_dag_template
     rng = np.random.default_rng(1234)
     templates = [random_dag_template(rng, int(n), n_workers=int(w)) for n, w in
                  zip(rng.integers(2, 400, size=60), rng.integers(1, 9, size=60))]
-    res, tn, tt = _run_all_templates(eng_mod, templates, mode=mode)
+    templates.append(zero_jct_template())
+    res, tn, tt = _run_all_templates(eng_mod, templates, mode=mode, launch=launch)
+    assert res['jct'][-1] == 0.0 and res['status'][-1] == 0
     n_err = 0
     for k, t in enumerate(templates):
         o = oracle_lib.run_lookahead(t)
@@ -247,15 +276,15 @@ def test_random_templates_vs_oracle(mode, eng_mod, oracle_lib):
     assert n_err < len(templates)
 
 
-@pytest.mark.parametrize('mode', MODES)
-@pytest.mark.parametrize('degree', [2, 8, 16])
-def test_baseline_sized_template_vs_oracle(degree, mode, eng_mod, oracle_lib):
+@pytest.mark.parametrize('mode,launch', MODE_LAUNCHES)
+@pytest.mark.parametrize('degree', [2, 4, 8, 16])
+def test_baseline_sized_template_vs_oracle(degree, mode, launch, eng_mod, oracle_lib):
     """BASELINE.json config 2/3 shape: ResNet-50-like job partitioned to `degree` on a 64-worker RAMP."""
     from ddls_b200 import synth
     from ddls_b200.template_builder import build_template, RampShape
     t = build_template(synth.resnet_like_graph(), degree, RampShape(4, 4, 4))
     o = oracle_lib.run_lookahead(t)
-    res, tn, tt = _run_all_templates(eng_mod, [t], repeat=8, mode=mode)
+    res, tn, tt = _run_all_templates(eng_mod, [t], repeat=8, mode=mode, launch=launch)
     for rep in range(8):
         assert res['status'][rep] == 0 and res['n_ticks'][rep] == o['n_ticks']
         assert res['jct'][rep] == o['jct'] and res['comm'][rep] == o['comm'] and res['comp'][rep] == o['comp']
@@ -379,10 +408,13 @@ def _fan_template(M, W, seed):
                       mount=MountScalars(n_mounted_workers=W)).canonicalise()
 
 
-@pytest.mark.parametrize('mode,cta_threads', [('warp', '0'), ('cta', '64'), ('cta', '128'), ('cta', '256'), ('thread', '0'),
-                                               ('thread_unfolded', '0')])
+@pytest.mark.parametrize('mode,cta_threads,launch',
+                         [pytest.param(m, c, 'first', id=f'{m}-{c}') for m, c in
+                          [('warp', '0'), ('cta', '64'), ('cta', '128'), ('cta', '256'), ('thread', '0'), ('thread_unfolded', '0')]]
+                         + [pytest.param(m, '0', 'hinted', id=f'{m}-0-hinted') for m in THREAD_MODES])
 @pytest.mark.parametrize('M,W', [(200, 4), (3000, 6)])
-def test_wide_fan_overflows_every_shared_memory_list(M, W, mode, cta_threads, eng_mod, oracle_lib):
+def test_wide_fan_overflows_every_shared_memory_list(M, W, mode, cta_threads, launch, eng_mod, oracle_lib):
+    """Frontiers far beyond shared memory.  Hinted: the recorded frontiers do not fit, so the second launch must spill too."""
     import os
     t = _fan_template(M, W, seed=M)
     want = oracle_lib.run_lookahead(t)
@@ -395,6 +427,12 @@ def test_wide_fan_overflows_every_shared_memory_list(M, W, mode, cta_threads, en
         os.environ.pop('RAMP_LOOKAHEAD_MODE', None)
         os.environ.pop('RAMP_LOOKAHEAD_CTA_THREADS', None)
     tid = eng.register_template(t)
+    if launch == 'hinted':
+        eng.run_lookaheads(np.full(5, tid, dtype=np.int32))
+        h = eng.template_info(tid)
+        assert (h['size_class'] == 2) == (M == 200)             # M = 3000: the quotient blob exceeds 96 KB (warp kernel)
+        if M == 200:
+            assert h['n_ticks'] == want['n_ticks'] and h['max_f'] > 16
     res, _, tn, tt = eng.run_lookaheads(np.full(5, tid, dtype=np.int32), want_trace=True)
     assert (res['status'] == 0).all() and (res['n_ticks'] == want['n_ticks']).all()
     for i in range(5):
