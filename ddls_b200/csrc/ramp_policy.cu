@@ -372,12 +372,13 @@ struct ramp_policy {
     bool weights_set = false, emb_valid = false;
     int sm_count = 132;
     size_t head_smem = 0;
-    // outputs of the last act / forward
-    int32_t cap = 0;
+    // outputs of the last act, for ramp_policy_read and ramp_policy_trajectory_record; act_n: its environment's episodes (-1: none yet)
+    int32_t cap = 0, act_n = -1;
     float* d_logits = nullptr; float* d_value = nullptr; float* d_logp = nullptr;
-    // staging for ramp_policy_forward
+    // inputs and outputs of ramp_policy_forward / ramp_policy_decide, apart from act's
     int32_t fcap = 0;
     int32_t* f_model = nullptr; float* f_gf = nullptr; uint8_t* f_mask = nullptr; int32_t* f_actions = nullptr;
+    float* f_logits = nullptr; float* f_value = nullptr; float* f_logp = nullptr;
     unsigned long long act_calls = 0;
     // trajectory of a rollout segment (ramp_policy_trajectory_*): [horizon][B] per field, on the device until read
     int32_t traj_h = 0, traj_b = 0, traj_a = 0;
@@ -462,6 +463,46 @@ int launch_head(ramp_policy* p, const HeadArgs& a, cudaStream_t st) {
     return RAMP_OK;
 }
 
+// the read-out on host inputs (ramp_policy_forward / ramp_policy_decide), in buffers of its own: what the last act left for
+// ramp_policy_read and the trajectory stays as it was
+int head_on_host(ramp_policy* p, int32_t n, const int32_t* model, const float* graph_features, const uint8_t* action_mask, int32_t sample,
+                 uint64_t seed, float* logits_out, float* value_out, float* logp_out, int32_t* actions_out) {
+    if (!p || !model || !graph_features || !action_mask) return perr(RAMP_ERR_BAD_ARG, "null argument");
+    if (n < 1) return RAMP_OK;
+    const ramp_policy_config_t& c = p->P.c;
+    PCUDA(cudaSetDevice(p->device));
+    int rc;
+    if (!p->emb_valid && (rc = launch_embed(p, 0)) != RAMP_OK) return rc;
+    if (n > p->fcap) {
+        cudaFree(p->f_model); cudaFree(p->f_gf); cudaFree(p->f_mask); cudaFree(p->f_actions);
+        cudaFree(p->f_logits); cudaFree(p->f_value); cudaFree(p->f_logp);
+        p->f_model = nullptr; p->f_gf = nullptr; p->f_mask = nullptr; p->f_actions = nullptr;
+        p->f_logits = p->f_value = p->f_logp = nullptr; p->fcap = 0;
+        PCUDA(cudaMalloc(&p->f_model, sizeof(int32_t) * (size_t)n));
+        PCUDA(cudaMalloc(&p->f_gf, sizeof(float) * (size_t)n * c.in_features_graph));
+        PCUDA(cudaMalloc(&p->f_mask, (size_t)n * c.n_actions));
+        PCUDA(cudaMalloc(&p->f_actions, sizeof(int32_t) * (size_t)n));
+        PCUDA(cudaMalloc(&p->f_logits, sizeof(float) * (size_t)n * c.n_actions));
+        PCUDA(cudaMalloc(&p->f_value, sizeof(float) * (size_t)n));
+        PCUDA(cudaMalloc(&p->f_logp, sizeof(float) * (size_t)n));
+        p->fcap = n;
+    }
+    PCUDA(cudaMemcpy(p->f_model, model, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice));
+    PCUDA(cudaMemcpy(p->f_gf, graph_features, sizeof(float) * (size_t)n * c.in_features_graph, cudaMemcpyHostToDevice));
+    PCUDA(cudaMemcpy(p->f_mask, action_mask, (size_t)n * c.n_actions, cudaMemcpyHostToDevice));
+    HeadArgs a{};
+    a.n = n; a.graph_features = p->f_gf; a.model = p->f_model; a.mask = p->f_mask; a.emb = p->d_emb; a.graph_static = p->d_gstatic;
+    a.logits = p->f_logits; a.value = p->f_value; a.logp = p->f_logp; a.actions = p->f_actions;
+    a.sample = sample; a.seed = seed;
+    if ((rc = launch_head(p, a, 0)) != RAMP_OK) return rc;
+    PCUDA(cudaStreamSynchronize(0));
+    if (logits_out) PCUDA(cudaMemcpy(logits_out, p->f_logits, sizeof(float) * (size_t)n * c.n_actions, cudaMemcpyDeviceToHost));
+    if (value_out) PCUDA(cudaMemcpy(value_out, p->f_value, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    if (logp_out) PCUDA(cudaMemcpy(logp_out, p->f_logp, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    if (actions_out) PCUDA(cudaMemcpy(actions_out, p->f_actions, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -507,6 +548,7 @@ void ramp_policy_destroy(ramp_policy_t* p) {
     cudaFree(p->d_w); cudaFree(p->d_models); cudaFree(p->d_emb); cudaFree(p->d_gstatic);
     cudaFree(p->d_logits); cudaFree(p->d_value); cudaFree(p->d_logp);
     cudaFree(p->f_model); cudaFree(p->f_gf); cudaFree(p->f_mask); cudaFree(p->f_actions);
+    cudaFree(p->f_logits); cudaFree(p->f_value); cudaFree(p->f_logp);
     cudaFree(p->t_obs); cudaFree(p->t_model); cudaFree(p->t_mask); cudaFree(p->t_action); cudaFree(p->t_logp); cudaFree(p->t_value);
     cudaFree(p->t_reward); cudaFree(p->t_done);
     delete p;
@@ -584,33 +626,12 @@ int ramp_policy_embed(ramp_policy_t* p, float* embeddings_out) {
 
 int ramp_policy_forward(ramp_policy_t* p, int32_t n, const int32_t* model, const float* graph_features, const uint8_t* action_mask,
                         float* logits_out, float* value_out) {
-    if (!p || !model || !graph_features || !action_mask) return perr(RAMP_ERR_BAD_ARG, "null argument");
-    if (n < 1) return RAMP_OK;
-    const ramp_policy_config_t& c = p->P.c;
-    PCUDA(cudaSetDevice(p->device));
-    int rc;
-    if (!p->emb_valid && (rc = launch_embed(p, 0)) != RAMP_OK) return rc;
-    if ((rc = ensure_outputs(p, n)) != RAMP_OK) return rc;
-    if (n > p->fcap) {
-        cudaFree(p->f_model); cudaFree(p->f_gf); cudaFree(p->f_mask); cudaFree(p->f_actions);
-        p->f_model = nullptr; p->f_gf = nullptr; p->f_mask = nullptr; p->f_actions = nullptr; p->fcap = 0;
-        PCUDA(cudaMalloc(&p->f_model, sizeof(int32_t) * (size_t)n));
-        PCUDA(cudaMalloc(&p->f_gf, sizeof(float) * (size_t)n * c.in_features_graph));
-        PCUDA(cudaMalloc(&p->f_mask, (size_t)n * c.n_actions));
-        PCUDA(cudaMalloc(&p->f_actions, sizeof(int32_t) * (size_t)n));
-        p->fcap = n;
-    }
-    PCUDA(cudaMemcpy(p->f_model, model, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice));
-    PCUDA(cudaMemcpy(p->f_gf, graph_features, sizeof(float) * (size_t)n * c.in_features_graph, cudaMemcpyHostToDevice));
-    PCUDA(cudaMemcpy(p->f_mask, action_mask, (size_t)n * c.n_actions, cudaMemcpyHostToDevice));
-    HeadArgs a{};
-    a.n = n; a.graph_features = p->f_gf; a.model = p->f_model; a.mask = p->f_mask; a.emb = p->d_emb; a.graph_static = p->d_gstatic;
-    a.logits = p->d_logits; a.value = p->d_value; a.logp = p->d_logp; a.actions = p->f_actions;
-    if ((rc = launch_head(p, a, 0)) != RAMP_OK) return rc;
-    PCUDA(cudaStreamSynchronize(0));
-    if (logits_out) PCUDA(cudaMemcpy(logits_out, p->d_logits, sizeof(float) * (size_t)n * c.n_actions, cudaMemcpyDeviceToHost));
-    if (value_out) PCUDA(cudaMemcpy(value_out, p->d_value, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
-    return RAMP_OK;
+    return head_on_host(p, n, model, graph_features, action_mask, 0, 0, logits_out, value_out, nullptr, nullptr);
+}
+
+int ramp_policy_decide(ramp_policy_t* p, int32_t n, const int32_t* model, const float* graph_features, const uint8_t* action_mask,
+                       int32_t sample, uint64_t seed, float* logits_out, float* value_out, float* logp_out, int32_t* actions_out) {
+    return head_on_host(p, n, model, graph_features, action_mask, sample, seed, logits_out, value_out, logp_out, actions_out);
 }
 
 int ramp_policy_act(ramp_policy_t* p, ramp_engine_t* eng, int32_t sample, uint64_t seed) {
@@ -633,6 +654,7 @@ int ramp_policy_act(ramp_policy_t* p, ramp_engine_t* eng, int32_t sample, uint64
     a.mask = eb.action_mask; a.emb = p->d_emb; a.logits = p->d_logits; a.value = p->d_value; a.logp = p->d_logp; a.actions = eb.actions;
     a.sample = sample; a.seed = seed ^ (0x9E3779B97F4A7C15ull * (++p->act_calls));
     if ((rc = launch_head(p, a, st)) != RAMP_OK) return rc;
+    p->act_n = eb.n_episodes;
     ramp_internal_count_launches(eng, launches);
     return RAMP_OK;
 }
@@ -642,7 +664,7 @@ int ramp_policy_read(ramp_policy_t* p, ramp_engine_t* eng, float* logits_out, fl
     ramp_env_buffers_t eb{};
     int rc = ramp_env_buffers(eng, &eb);
     if (rc != RAMP_OK) return rc;
-    if (eb.n_episodes > p->cap) return perr(RAMP_ERR_BAD_ARG, "policy: nothing to read (ramp_policy_act was not called)");
+    if (eb.n_episodes != p->act_n) return perr(RAMP_ERR_BAD_ARG, "policy: nothing to read (ramp_policy_act was not called for this environment)");
     cudaStream_t st = ramp_internal_stream(eng);
     const size_t B = (size_t)eb.n_episodes;
     if (logits_out) PCUDA(cudaMemcpyAsync(logits_out, p->d_logits, sizeof(float) * B * p->P.c.n_actions, cudaMemcpyDeviceToHost, st));
@@ -692,7 +714,7 @@ int ramp_policy_trajectory_record(ramp_policy_t* p, ramp_engine_t* eng, int32_t 
     ramp_env_buffers_t eb{};
     int rc = ramp_env_buffers(eng, &eb);
     if (rc != RAMP_OK) return rc;
-    if (eb.n_episodes != p->traj_b || eb.n_actions != p->traj_a || eb.n_episodes > p->cap)
+    if (eb.n_episodes != p->traj_b || eb.n_actions != p->traj_a || eb.n_episodes != p->act_n)
         return perr(RAMP_ERR_BAD_ARG, "policy: the trajectory was set up for another environment, or ramp_policy_act was not called");
     cudaStream_t st = ramp_internal_stream(eng);
     const size_t B = (size_t)eb.n_episodes, o = (size_t)t * B;

@@ -32,6 +32,22 @@ class _Config(C.Structure):
                                           'aggregator_activation', 'fcnet_activation', 'apply_action_mask', 'n_models')]
 
 
+def c_config(config: Dict, n_actions: int, n_models: int) -> _Config:
+    """ramp_policy_config_t of a gnn.yaml-style configuration (one read-out hidden layer)"""
+    c = config
+    return _Config(c['in_features_node'], c['in_features_edge'], c['in_features_graph'], int(n_actions), c['out_features_msg'],
+                   c['out_features_hidden'], c['out_features_node'], c['out_features_graph'], c['num_rounds'],
+                   tuple(c['fcnet_hiddens'])[0], ACTIVATIONS[c['aggregator_activation']], ACTIVATIONS[c['fcnet_activation']],
+                   1 if c['apply_action_mask'] else 0, int(n_models))
+
+
+def _shaped(name, a, shape):
+    """a, refusing any other shape: the library reads exactly that many elements through the raw pointer"""
+    if a.shape != tuple(shape):
+        raise ValueError(f'{name}: shape {a.shape}, expected {tuple(shape)}')
+    return a
+
+
 def _bind(L):
     if getattr(L, '_policy_bound', False):
         return
@@ -49,6 +65,8 @@ def _bind(L):
     L.ramp_policy_embed.argtypes = [C.c_void_p, C.c_void_p]
     L.ramp_policy_forward.restype = C.c_int
     L.ramp_policy_forward.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 5
+    L.ramp_policy_decide.restype = C.c_int
+    L.ramp_policy_decide.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 3 + [C.c_int32, C.c_uint64] + [C.c_void_p] * 4
     L.ramp_policy_act.restype = C.c_int
     L.ramp_policy_act.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_uint64]
     L.ramp_policy_read.restype = C.c_int
@@ -148,11 +166,7 @@ class DeviceGNNPolicy:
         L = _engine.load_library()
         _bind(L)
         self._L = L
-        c = self.config
-        self._cfg = _Config(c['in_features_node'], c['in_features_edge'], c['in_features_graph'], self.n_actions, c['out_features_msg'],
-                            c['out_features_hidden'], c['out_features_node'], c['out_features_graph'], c['num_rounds'],
-                            tuple(c['fcnet_hiddens'])[0], ACTIVATIONS[c['aggregator_activation']], ACTIVATIONS[c['fcnet_activation']],
-                            1 if c['apply_action_mask'] else 0, self.n_models)
+        self._cfg = c_config(self.config, self.n_actions, self.n_models)
         self._h = C.c_void_p()
         _engine._check(L.ramp_policy_create(device, C.byref(self._cfg), C.byref(self._h)))
         self.static = [static_observation(g) for g in graphs]
@@ -173,11 +187,15 @@ class DeviceGNNPolicy:
             pass
 
     def set_model(self, m, node_features, edge_features, edges_src, edges_dst, graph_static):
+        c = self.config
         nf = np.ascontiguousarray(node_features, dtype=np.float32)
-        ef = np.ascontiguousarray(edge_features, dtype=np.float32)
         src = np.ascontiguousarray(edges_src, dtype=np.int32)
-        dst = np.ascontiguousarray(edges_dst, dtype=np.int32)
-        gs = np.ascontiguousarray(graph_static, dtype=np.float32)
+        N, E = (len(nf) if nf.ndim == 2 else -1), (len(src) if src.ndim == 1 else -1)
+        _shaped('node_features', nf, (N, c['in_features_node']))
+        _shaped('edges_src', src, (E,))
+        dst = _shaped('edges_dst', np.ascontiguousarray(edges_dst, dtype=np.int32), (E,))
+        ef = _shaped('edge_features', np.ascontiguousarray(edge_features, dtype=np.float32), (E, c['in_features_edge']))
+        gs = _shaped('graph_static', np.ascontiguousarray(graph_static, dtype=np.float32), (6,))
         _engine._check(self._L.ramp_policy_set_model(self._h, int(m), len(nf), len(ef), nf.ctypes.data, ef.ctypes.data, src.ctypes.data,
                                                      dst.ctypes.data, gs.ctypes.data))
 
@@ -194,15 +212,34 @@ class DeviceGNNPolicy:
     def forward(self, model, graph_features, action_mask):
         """logits [n, |A|], value [n] for host inputs: model [n], graph_features [n, in_features_graph] (the observation's
         graph_features without the mask), action_mask [n, |A|]."""
-        model = np.ascontiguousarray(model, dtype=np.int32)
-        gf = np.ascontiguousarray(graph_features, dtype=np.float32)
-        mask = np.ascontiguousarray(action_mask, dtype=np.uint8)
+        model, gf, mask = self._host_inputs(model, graph_features, action_mask)
         n = len(model)
         logits = np.zeros((n, self.n_actions), dtype=np.float32)
         value = np.zeros(n, dtype=np.float32)
         _engine._check(self._L.ramp_policy_forward(self._h, n, model.ctypes.data, gf.ctypes.data, mask.ctypes.data, logits.ctypes.data,
                                                    value.ctypes.data))
         return logits, value
+
+    def decide(self, model, graph_features, action_mask, sample: bool = False, seed: int = 0):
+        """forward() plus act()'s action selection on host inputs: logits [n, |A|], value [n], logp [n] (of the chosen action),
+        action [n].  Row b draws with the key (seed, b), the seed used as given.  Rows whose model is outside [0, n_models) get
+        zeros and action 0."""
+        model, gf, mask = self._host_inputs(model, graph_features, action_mask)
+        n = len(model)
+        logits = np.zeros((n, self.n_actions), dtype=np.float32)
+        value, logp, action = np.zeros(n, dtype=np.float32), np.zeros(n, dtype=np.float32), np.zeros(n, dtype=np.int32)
+        _engine._check(self._L.ramp_policy_decide(self._h, n, model.ctypes.data, gf.ctypes.data, mask.ctypes.data, 1 if sample else 0,
+                                                  C.c_uint64(seed & (2 ** 64 - 1)), logits.ctypes.data, value.ctypes.data,
+                                                  logp.ctypes.data, action.ctypes.data))
+        return logits, value, logp, action
+
+    def _host_inputs(self, model, graph_features, action_mask):
+        model = np.ascontiguousarray(model, dtype=np.int32)
+        n = len(model) if model.ndim == 1 else -1
+        _shaped('model', model, (n,))
+        gf = _shaped('graph_features', np.ascontiguousarray(graph_features, dtype=np.float32), (n, self.config['in_features_graph']))
+        mask = _shaped('action_mask', np.ascontiguousarray(action_mask, dtype=np.uint8), (n, self.n_actions))
+        return model, gf, mask
 
     def act(self, env, sample: bool = False, seed: int = 0):
         """One decision per episode of a DeviceRampJobPartitioningEnvironment, written into its device action buffer; follow with

@@ -436,14 +436,21 @@ int ramp_policy_set_model(ramp_policy_t* p, int32_t model, int32_t n_nodes, int3
 /* message passing + node mean of every registered model; embeddings_out: HOST [n_models][out_features_node] or NULL */
 int ramp_policy_embed(ramp_policy_t* p, float* embeddings_out);
 /* read-out on HOST inputs (tests, host-side policies): model [n], graph_features [n][in_features_graph], action_mask
- * [n][n_actions] -> logits [n][n_actions], value [n] (either may be NULL) */
+ * [n][n_actions] -> logits [n][n_actions], value [n] (either may be NULL).  Uses buffers of its own: what the last
+ * ramp_policy_act left for ramp_policy_read / ramp_policy_trajectory_record is not touched. */
 int ramp_policy_forward(ramp_policy_t* p, int32_t n, const int32_t* model, const float* graph_features, const uint8_t* action_mask,
                         float* logits_out, float* value_out);
+/* ramp_policy_forward plus the action selection of ramp_policy_act on HOST inputs: log-probability of the chosen action [n] and the
+ * action [n] (any output may be NULL).  Row b draws with the key (seed, b); `seed` is used as given (act mixes in its call count).
+ * Rows whose model is outside [0, n_models) get zero logits, value and log-probability and action 0. */
+int ramp_policy_decide(ramp_policy_t* p, int32_t n, const int32_t* model, const float* graph_features, const uint8_t* action_mask,
+                       int32_t sample, uint64_t seed, float* logits_out, float* value_out, float* logp_out, int32_t* actions_out);
 /* one decision for every episode of `eng`'s environment on the engine's stream: reads queued_model / obs_dynamic / action_mask,
  * writes ramp_env_buffers_t.actions (greedy: the first maximal logit; sample: categorical over softmax(logits) from a counter-based
  * generator keyed by (seed, episode)); finished episodes get action 0.  No host transfer. */
 int ramp_policy_act(ramp_policy_t* p, ramp_engine_t* eng, int32_t sample, uint64_t seed);
-/* HOST copies of the last ramp_policy_act: logits [B][n_actions], value [B], log-probability of the chosen action [B], actions [B] (any may be NULL) */
+/* HOST copies of the last ramp_policy_act: logits [B][n_actions], value [B], log-probability of the chosen action [B], actions [B] (any may be NULL);
+ * RAMP_ERR_BAD_ARG unless that act ran for an environment of `eng`'s size */
 int ramp_policy_read(ramp_policy_t* p, ramp_engine_t* eng, float* logits_out, float* value_out, float* logp_out, int32_t* actions_out);
 
 /* A rollout segment recorded on the device, for a trainer: ramp_policy_trajectory_begin sizes [horizon][n_episodes] slots;
