@@ -42,22 +42,21 @@ int set_error(int code, const char* fmt, ...) {
 constexpr int MAX_EVENT_PAIRS = 64;
 constexpr int RAMP_SMEM_CARVEOUT = 100;   // percent of the unified L1/shared array given to shared memory
 
-// The lookahead kernel is instantiated for several CTA sizes; small CTAs (1-2 warps) keep more lookaheads
-// resident per SM and waste fewer lanes on the small per-tick frontiers, large CTAs finish one lookahead sooner.
+// Templates whose quotient blob does not fit shared memory run on the warp kernel (one lookahead per warp) or the CTA kernel
+// (one lookahead per CTA).  The warp kernel runs in 4-warp CTAs, or in 1-warp CTAs beside a CTA kernel: they fill the
+// registers and shared memory the CTA kernel leaves on every SM at a finer grain.
 using LookaheadKernel = void (*)(const LookaheadArgs);
-LookaheadKernel lookahead_kernel_for(int nt) {   // nt = threads per CTA = 32 x (independent lookahead warps per CTA)
-    switch (nt) {
-        case 32: return ramp_lookahead_kernel<1>;
-        case 64: return ramp_lookahead_kernel<2>;
-        case 128: return ramp_lookahead_kernel<4>;
-        case 256: return ramp_lookahead_kernel<8>;
-        default: return nullptr;
-    }
-}
+constexpr int WARP_NT = 128, SPLIT_WARP_NT = 32;    // threads per CTA of the warp kernel alone / beside a CTA kernel
+LookaheadKernel warp_kernel() { return ramp_lookahead_kernel<WARP_NT / 32>; }
+LookaheadKernel split_warp_kernel() { return ramp_lookahead_kernel<SPLIT_WARP_NT / 32>; }
 
 // the dense shape of the warp kernel: smaller shared-memory frontiers, 16 instead of 12 lookahead warps per SM
 constexpr int DENSE_F_CAP = 256, DENSE_OPS_CAP = 32, DENSE_NT = 128;
 LookaheadKernel lookahead_dense_kernel() { return ramp_lookahead_kernel<DENSE_NT / 32, DENSE_F_CAP, DENSE_OPS_CAP>; }
+
+constexpr int64_t BIG_THRESHOLD = 60000;          // N + E from which one CTA per lookahead beats one warp (size class 1)
+constexpr double SPLIT_ALPHA = 1.3;               // 64-thread-CTA split while 2 n_big + n_small <= SPLIT_ALPHA x register slots
+constexpr int32_t RESIDENT_MAX_BYTES = 96 * 1024; // largest quotient blob that goes resident on the thread kernel
 
 LookaheadKernel lookahead_cta_kernel_for(int nt) {   // one CTA of nt threads per lookahead
     switch (nt) {
@@ -113,9 +112,7 @@ struct ramp_engine {
     unsigned char* d_scratch = nullptr;
     uint64_t scratch_stride = 0;
     int scratch_grid = 0;
-    int grid = 0;
-    int nt = 128;                // threads per lookahead CTA = 32 x warps, one lookahead per warp (RAMP_LOOKAHEAD_THREADS overrides)
-    int max_ctas_per_sm = 0;     // optional cap (RAMP_LOOKAHEAD_CTAS_PER_SM)
+    int grid = 0;                // resident CTAs of the warp kernel's 4-warp shape
     size_t smem_bytes = 0;
     // CTA-per-lookahead variant (lower latency; used when a launch has fewer work items than warp slots)
     int cta_nt = 0;              // 0 = pick 128 or 64 threads per launch; RAMP_LOOKAHEAD_CTA_THREADS forces one
@@ -127,21 +124,15 @@ struct ramp_engine {
     int cta256_grid = 0;         // resident CTAs of the 256-thread variant
     int cta_grid_for(int nt) const { return nt == 256 ? cta256_grid : nt == 128 ? cta_grid : cta64_grid; }
     size_t cta_smem_bytes = 0;
-    int split_warp_nt = 32;      // threads per CTA of the warp kernel when it runs beside a CTA kernel
-    size_t smem2_bytes = 0;      // dynamic shared memory of the 2-warp CTAs used beside a CTA kernel
-    int use_cta256 = 1;          // RAMP_USE_CTA256=0 turns off: 256-thread CTAs for the big lookaheads when 8 n_big + n_small fit the warp slots
-    double split_alpha = 1.3;    // 64-thread-CTA split while 2 n_big + n_small <= split_alpha x resident warp slots
-    int debug = 0;               // RAMP_DEBUG=1 prints the per-step launch decisions to stderr
-    int mode = 0;                // 0 auto, 1 warp-per-lookahead, 2 CTA-per-lookahead (RAMP_LOOKAHEAD_MODE)
+    size_t smem2_bytes = 0;      // dynamic shared memory of the 1-warp CTAs used beside a CTA kernel
+    int debug = 0;               // RAMP_DEBUG=1 prints the launch decisions to stderr
+    int mode = 0;                // 0 auto, 1 warp-per-lookahead, 2 CTA-per-lookahead (RAMP_LOOKAHEAD_MODE); 1 and 2 make nothing resident
     int32_t* h_n_work = nullptr; // pinned [4]
-    int64_t big_threshold = 60000;   // N + E from which one CTA per lookahead beats one warp (RAMP_BIG_THRESHOLD)
     WorkItem* d_items_big = nullptr;
     cudaStream_t stream2 = nullptr;  // big lookaheads run concurrently with the small ones
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     // resident (quotient) templates: thread-per-lookahead kernel
-    int use_resident = 1;        // RAMP_RESIDENT=0: register every template for the warp / CTA kernels only
-    int use_quotient = 1;        // RAMP_QUOTIENT=0: resident blobs are built from the unfolded job (identity quotient)
-    int32_t res_max_bytes = 96 * 1024;   // largest quotient blob that goes resident (RAMP_RESIDENT_MAX_KB)
+    int use_quotient = 1;        // 0 (RAMP_LOOKAHEAD_MODE=thread_unfolded): resident blobs are built from the unfolded job (identity quotient)
     int n_resident = 0, n_nonresident = 0;
     int32_t res_tmpl_cap = 0, res_n_cap = 0, res_spill_ops = 0, res_spill_deps = 0;
     int res_grid = 0;
@@ -169,7 +160,8 @@ struct ramp_engine {
     ChunkDesc* sa_chunks = nullptr;
     ResultSlots sa_res{};
     int32_t sa_cap = 0;
-    WorkItem* sa_items = nullptr;
+    WorkItem* sa_items = nullptr;        // [n]: the small, big and resident work lists, one after the other
+    int32_t* sa_rank = nullptr;          // [n] ramp_bucket_kernel scratch
     Counters* sa_counters = nullptr;
     // instrumentation
     int64_t launches = 0;
@@ -216,25 +208,23 @@ int resolve_events(ramp_engine* e) {
 int ensure_scratch(ramp_engine* e) {
     const uint64_t trace_bytes = align_up((uint64_t)e->cfg.trace_cap * 12, 16);
     const uint64_t stride = align_up(std::max<uint64_t>(e->max_scratch, 16), 256) + align_up(trace_bytes, 256);
-    const size_t smem = lookahead_smem_per_warp(e->max_w, e->max_c, e->par_cap) * (size_t)(e->nt / 32);
+    const size_t smem = lookahead_smem_per_warp(e->max_w, e->max_c, e->par_cap) * (size_t)(WARP_NT / 32);
     if (smem > 200 * 1024)
         return set_error(RAMP_ERR_CAPACITY, "a template needs %zu B of shared memory for its worker/channel key arrays (max 200 KiB)", smem);
     if (smem != e->smem_bytes || e->grid == 0) {
-        LookaheadKernel kern = lookahead_kernel_for(e->nt);
+        LookaheadKernel kern = warp_kernel();
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         // all lookahead kernels ask for the same L1/shared split: kernels with different carve-outs cannot share an SM,
         // which would serialise the CTA kernel and the warp kernel when they are launched side by side
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
         int occ = 0;
-        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, e->nt, smem));
+        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, WARP_NT, smem));
         if (occ < 1) occ = 1;
-        if (e->max_ctas_per_sm > 0 && occ > e->max_ctas_per_sm) occ = e->max_ctas_per_sm;
         e->grid = e->sm_count * occ;     // persistent CTAs: a whole number of waves (SMs x resident CTAs per SM)
         e->smem_bytes = smem;
-        // beside a CTA kernel the small lookaheads run in 2-warp CTAs: they fill the registers and shared memory the CTA
-        // kernel leaves on every SM at a finer grain (the block scheduler spreads both kernels over all SMs)
-        const size_t smem2 = lookahead_smem_per_warp(e->max_w, e->max_c, e->par_cap) * (size_t)(e->split_warp_nt / 32);
-        LookaheadKernel kern2 = lookahead_kernel_for(e->split_warp_nt);
+        // the block scheduler spreads the 1-warp CTAs used beside a CTA kernel and the CTA kernel's over all SMs
+        const size_t smem2 = lookahead_smem_per_warp(e->max_w, e->max_c, e->par_cap) * (size_t)(SPLIT_WARP_NT / 32);
+        LookaheadKernel kern2 = split_warp_kernel();
         CUDA_TRY(cudaFuncSetAttribute(kern2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
         CUDA_TRY(cudaFuncSetAttribute(kern2, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
         e->smem2_bytes = smem2;
@@ -263,7 +253,7 @@ int ensure_scratch(ramp_engine* e) {
         e->cta_smem_bytes = cta_smem;
     }
     // one slab per lookahead in flight; the warp kernel and one of the CTA kernels may run side by side
-    const int n_slabs = std::max(e->grid * (e->nt / 32) + std::max(e->cta_grid, e->cta64_grid), e->dense_grid * (DENSE_NT / 32));
+    const int n_slabs = std::max(e->grid * (WARP_NT / 32) + std::max(e->cta_grid, e->cta64_grid), e->dense_grid * (DENSE_NT / 32));
     if (stride != e->scratch_stride || n_slabs != e->scratch_grid || e->d_scratch == nullptr) {
         CUDA_TRY(cudaStreamSynchronize(e->stream));
         if (e->d_scratch) cudaFree(e->d_scratch);
@@ -276,7 +266,7 @@ int ensure_scratch(ramp_engine* e) {
 }
 
 LookaheadArgs make_lookahead_args(ramp_engine* e, const WorkItem* items, Counters* counters, const ResultSlots& res,
-                                  bool use_pool, MemoStats* stats) {
+                                  const TracePool& pool, MemoStats* stats) {
     LookaheadArgs a{};
     a.templates = e->d_templates;
     a.items = items;
@@ -287,35 +277,13 @@ LookaheadArgs make_lookahead_args(ramp_engine* e, const WorkItem* items, Counter
     a.scratch = e->d_scratch;
     a.scratch_stride = e->scratch_stride;
     a.res = res;
-    a.pool = e->pool;
-    if (!use_pool) a.pool.top = nullptr;
+    a.pool = pool;
     a.trace_cap = e->cfg.trace_cap;
     a.w_cap = e->max_w;
     a.c_cap = e->max_c;
     a.par_cap = e->par_cap;
     a.stats = stats;
     return a;
-}
-
-// Launches ONE lookahead kernel for n_items work items of a standalone run (ramp_run_lookaheads): one CTA per lookahead
-// when there are big lookaheads among them and the items fit in about one wave of CTAs (latency-bound regime), one warp
-// per lookahead otherwise (small lookaheads are fastest on one warp; many lookaheads need the warp kernel's density).
-void launch_lookahead(ramp_engine* e, const LookaheadArgs& a, int n_items, int n_big, cudaStream_t st) {
-    int cta_nt = 0;
-    if (e->mode == 2) cta_nt = e->cta_nt ? e->cta_nt : (n_items <= e->cta_grid ? 128 : 64);
-    else if (e->mode != 1 && n_big > 0) {
-        if (e->cta_nt) { if (n_items <= e->cta_grid_for(e->cta_nt)) cta_nt = e->cta_nt; }
-        else if (n_items <= e->cta_grid) cta_nt = 128;
-        else if (n_items <= e->cta64_grid) cta_nt = 64;
-    }
-    if (cta_nt) {
-        const int grid = std::max(1, std::min(e->cta_grid_for(cta_nt), n_items));
-        lookahead_cta_kernel_for(cta_nt)<<<grid, cta_nt, e->cta_smem_bytes, st>>>(a);
-    } else {
-        const int wpb = e->nt / 32;
-        const int grid = std::max(1, std::min(e->grid, (n_items + wpb - 1) / wpb));
-        lookahead_kernel_for(e->nt)<<<grid, e->nt, e->smem_bytes, st>>>(a);
-    }
 }
 
 uint64_t fnv1a(const unsigned char* p, size_t n) {
@@ -409,7 +377,8 @@ bool build_resident_blob(const ramp_lowered_job_t* j, const ramp_quotient_t& q, 
     return true;
 }
 
-// the identity quotient: every op its own class (RAMP_QUOTIENT=0; lets the tests run the thread kernel on unfolded jobs)
+// the identity quotient: every op its own class (RAMP_LOOKAHEAD_MODE=thread_unfolded; lets the tests run the thread kernel
+// on unfolded jobs)
 int identity_quotient(const ramp_lowered_job_t* j, ramp_quotient_t* q) {
     memset(q, 0, sizeof(*q));
     const int32_t N = j->n_ops, E = j->n_deps;
@@ -467,15 +436,105 @@ int ensure_thread_scratch(ramp_engine* e) {
     return RAMP_OK;
 }
 
-ThreadArgs make_thread_args(ramp_engine* e, const ChunkDesc* chunks, const int32_t* n_chunks, int32_t* cursor, const WorkItem* items,
+ThreadArgs make_thread_args(ramp_engine* e, const ChunkDesc* chunks, const WorkItem* chunk_items, Counters* c,
                             const ResultSlots& res, const TracePool& pool, MemoStats* stats) {
     ThreadArgs a{};
-    a.templates = e->d_templates; a.chunks = chunks; a.n_chunks = n_chunks; a.cursor = cursor; a.items = items;
+    a.templates = e->d_templates; a.chunks = chunks; a.n_chunks = &c->n_chunks; a.cursor = &c->chunk_cursor; a.items = chunk_items;
     a.scratch = e->d_res_scratch; a.scratch_stride = e->res_scratch_stride;
     a.res = res; a.pool = pool; a.trace_cap = e->cfg.trace_cap;
     a.tmpl_cap = e->res_tmpl_cap; a.n_cap = e->res_n_cap; a.spill_ops = e->res_spill_ops; a.spill_deps = e->res_spill_deps;
     a.stats = stats; a.hints = e->d_hints; a.hint_jct = e->d_hint_jct;
     return a;
+}
+
+// groups the resident work items (list 2 of `c`) by template into chunks of <= 32 for the thread kernel, on the device
+void bucket_resident(ramp_engine* e, const WorkItem* items, Counters* c, WorkItem* chunk_items, ChunkDesc* chunks, int32_t* rank,
+                     cudaStream_t st) {
+    BucketArgs ba{};
+    ba.items = items; ba.n_items = &c->n_work_res; ba.n_templates = (int32_t)e->templates.size();
+    ba.tcount = e->d_tcount; ba.tbase = e->d_tbase; ba.chunk_items = chunk_items; ba.chunks = chunks;
+    ba.n_chunks = &c->n_chunks; ba.cursor = &c->chunk_cursor; ba.rank = rank;
+    ramp_bucket_kernel<<<1, 1024, 0, st>>>(ba);
+    e->launches++;
+}
+
+// Launches the lookaheads of a step or of a standalone run (ramp_run_lookaheads), so both pick kernels by the same rule.
+// The resident ones, already bucketed into chunks, run on the thread kernel over thread_grid CTAs (0: there are none).  The
+// others come as two work lists whose sizes the host knows: small (list 0 of `c`) and big (list 1).
+int launch_lookaheads(ramp_engine* e, const ChunkDesc* chunks, const WorkItem* chunk_items, int thread_grid,
+                      const WorkItem* items, int n_small, const WorkItem* items_big, int n_big, Counters* c,
+                      const ResultSlots& res, const TracePool& pool, MemoStats* stats, cudaStream_t st) {
+    if (thread_grid > 0) {
+        ThreadArgs ta = make_thread_args(e, chunks, chunk_items, c, res, pool, stats);
+        ramp_lookahead_thread_kernel<<<thread_grid, RAMP_THREAD_CTA, e->res_smem, st>>>(ta);
+        e->launches++;
+    }
+    if (n_small + n_big == 0) return RAMP_OK;
+    LookaheadArgs a = make_lookahead_args(e, items, c, res, pool, stats);
+    LookaheadArgs ab = a;
+    ab.items = items_big; ab.n_work = &c->n_work_big; ab.cursor = &c->work_cursor_big;
+    const int wpb = WARP_NT / 32;
+    const int warp_slots = e->grid * wpb;
+    // The big lookaheads set the latency, the small ones the load.  While everything fits the SMs' warp slots at once
+    // (registers cap every mix at cta_grid x 4 warps) each big lookahead gets a 256-thread CTA if 8 warps per big one still
+    // fit (2.4 ms instead of 2.9 ms for the bench job), else a 128-thread CTA; while the big ones still fit as 64-thread CTAs
+    // and the small ones need at most a short second wave they get those; beyond that everything goes through the warp
+    // kernel, the big list first (longest-processing-time-first keeps the tail short).  The CTA kernel runs on a second
+    // stream beside the warp kernel for the small list.
+    const int reg_slots = e->cta_grid * 4;
+    int split_nt = 0;
+    if (e->mode != 1 && n_big > 0) {
+        if (n_big <= e->cta256_grid && 8 * n_big + n_small <= reg_slots) split_nt = 256;
+        else if (n_big <= e->cta_grid && 4 * n_big + n_small <= reg_slots) split_nt = 128;
+        else if (n_big <= e->cta64_grid && 2 * n_big + n_small <= (int)(SPLIT_ALPHA * reg_slots)) split_nt = 64;
+    }
+    const bool split = split_nt != 0;
+    if (e->debug) fprintf(stderr, "[ramp] lookaheads: small=%d big=%d warp_slots=%d reg_slots=%d -> %s %d\n", n_small, n_big,
+                          warp_slots, reg_slots, split ? "split (CTA || warp), CTA threads" : "single warp kernel, big first", split_nt);
+    if (split) {
+        // the second stream starts after all that is queued on `st`: a standalone run's uploads and bucket kernel, the
+        // thread kernel
+        CUDA_TRY(cudaEventRecord(e->ev_fork, st));
+        CUDA_TRY(cudaStreamWaitEvent(e->stream2, e->ev_fork, 0));
+        const int grid = std::min(n_big, e->cta_grid_for(split_nt));
+        lookahead_cta_kernel_for(split_nt)<<<grid, split_nt, e->cta_smem_bytes, e->stream2>>>(ab);
+        CUDA_TRY(cudaEventRecord(e->ev_join, e->stream2));
+        e->launches++;
+        if (n_small > 0) {
+            LookaheadArgs as = a;
+            as.scratch = a.scratch + (uint64_t)std::max(e->cta_grid, e->cta64_grid) * a.scratch_stride;   // slabs past the CTA kernel's
+            const int wpb2 = SPLIT_WARP_NT / 32;
+            const int g2 = std::max(1, std::min(e->grid * wpb / wpb2, (n_small + wpb2 - 1) / wpb2));   // never more warps than slabs
+            split_warp_kernel()<<<g2, SPLIT_WARP_NT, e->smem2_bytes, st>>>(as);
+            e->launches++;
+        }
+        CUDA_TRY(cudaStreamWaitEvent(st, e->ev_join, 0));
+    } else if (e->mode == 2) {
+        // each list on a CTA kernel of its own: RAMP_LOOKAHEAD_CTA_THREADS threads per CTA, else 128 while the list fits
+        // one wave of them and 64 beyond
+        auto cta_list = [&](const LookaheadArgs& l, int n) {
+            const int nt = e->cta_nt ? e->cta_nt : (n <= e->cta_grid ? 128 : 64);
+            lookahead_cta_kernel_for(nt)<<<std::min(e->cta_grid_for(nt), n), nt, e->cta_smem_bytes, st>>>(l);
+            e->launches++;
+        };
+        if (n_big > 0) cta_list(ab, n_big);
+        if (n_small > 0) cta_list(a, n_small);
+    } else {
+        LookaheadArgs all = ab;                      // list A = big, list B = small, one cursor
+        all.items_b = items; all.n_work_b = &c->n_work;
+        const int n_all = n_small + n_big;
+        if (e->mode == 0 && e->dense_grid * (DENSE_NT / 32) > warp_slots && n_all > (int)(e->dense_factor * warp_slots)) {
+            // far more lookaheads than slots: throughput matters, not the latency of one -> 16 warps per SM
+            const int wd = DENSE_NT / 32;
+            const int g = std::max(1, std::min(e->dense_grid, (n_all + wd - 1) / wd));
+            lookahead_dense_kernel()<<<g, DENSE_NT, e->dense_smem_bytes, st>>>(all);
+        } else {
+            const int g = std::max(1, std::min(e->grid, (n_all + wpb - 1) / wpb));
+            warp_kernel()<<<g, WARP_NT, e->smem_bytes, st>>>(all);
+        }
+        e->launches++;
+    }
+    return RAMP_OK;
 }
 
 }  // namespace
@@ -524,12 +583,6 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     CUDA_TRY(cudaSetDevice(cfg.device));
     ramp_engine* e = new ramp_engine();
     e->cfg = cfg;
-    if (const char* v = getenv("RAMP_LOOKAHEAD_THREADS")) {
-        const int nt = atoi(v);
-        if (lookahead_kernel_for(nt) == nullptr) { delete e; return set_error(RAMP_ERR_BAD_ARG, "RAMP_LOOKAHEAD_THREADS must be 32, 64, 128 or 256"); }
-        e->nt = nt;
-    }
-    if (const char* v = getenv("RAMP_LOOKAHEAD_CTAS_PER_SM")) e->max_ctas_per_sm = atoi(v);
     if (const char* v = getenv("RAMP_LOOKAHEAD_CTA_THREADS")) {
         const int nt = atoi(v);
         if (lookahead_cta_kernel_for(nt) == nullptr) { delete e; return set_error(RAMP_ERR_BAD_ARG, "RAMP_LOOKAHEAD_CTA_THREADS must be 64, 128 or 256"); }
@@ -539,22 +592,10 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
         // warp / cta: every template goes to that kernel (no resident quotient blobs); thread_unfolded: the thread kernel on
         // the unfolded job (identity quotient); anything else: automatic (resident whenever the quotient blob fits)
         e->mode = !strcmp(v, "warp") ? 1 : !strcmp(v, "cta") ? 2 : 0;
-        if (e->mode != 0) e->use_resident = 0;
         if (!strcmp(v, "thread_unfolded")) e->use_quotient = 0;
     }
-    if (const char* v = getenv("RAMP_BIG_THRESHOLD")) e->big_threshold = atoll(v);
     if (const char* v = getenv("RAMP_DEBUG")) e->debug = atoi(v);
-    if (const char* v = getenv("RAMP_RESIDENT")) e->use_resident = atoi(v);
-    if (const char* v = getenv("RAMP_QUOTIENT")) e->use_quotient = atoi(v);
-    if (const char* v = getenv("RAMP_RESIDENT_MAX_KB")) e->res_max_bytes = atoi(v) * 1024;
-    if (const char* v = getenv("RAMP_SPLIT_ALPHA")) e->split_alpha = atof(v);
-    if (const char* v = getenv("RAMP_USE_CTA256")) e->use_cta256 = atoi(v);
     if (const char* v = getenv("RAMP_DENSE_FACTOR")) e->dense_factor = atof(v);
-    if (const char* v = getenv("RAMP_SPLIT_WARP_THREADS")) {
-        const int nt = atoi(v);
-        if (lookahead_kernel_for(nt) == nullptr) { delete e; return set_error(RAMP_ERR_BAD_ARG, "RAMP_SPLIT_WARP_THREADS must be 32, 64, 128 or 256"); }
-        e->split_warp_nt = nt;
-    }
     cudaDeviceProp prop{};
     CUDA_TRY(cudaGetDeviceProperties(&prop, cfg.device));
     e->sm_count = prop.multiProcessorCount;
@@ -644,7 +685,7 @@ int ramp_engine_destroy(ramp_engine_t* e) {
     if (e->env_h_need) cudaFreeHost(e->env_h_need);
     if (e->env_h_mirror) cudaFreeHost(e->env_h_mirror);
     cudaFree(e->d_items_res); cudaFree(e->d_chunk_items); cudaFree(e->d_chunks); cudaFree(e->d_tcount); cudaFree(e->d_tbase); cudaFree(e->d_rank); cudaFree(e->d_hints); cudaFree(e->d_hint_jct);
-    cudaFree(e->d_res_scratch); cudaFree(e->sa_chunk_items); cudaFree(e->sa_chunks);
+    cudaFree(e->d_res_scratch); cudaFree(e->sa_chunk_items); cudaFree(e->sa_chunks); cudaFree(e->sa_rank);
     cudaFree(e->d_templates); cudaFree(e->d_memo_keys); cudaFree(e->d_memo_vals); cudaFree(e->d_memo_keys2);
     free_result_slots(e->res); free_result_slots(e->sa_res);
     cudaFree(e->pool.n_active); cudaFree(e->pool.tick); cudaFree(e->pool.top);
@@ -761,7 +802,7 @@ int ramp_register_template(ramp_engine_t* e, const ramp_lowered_job_t* j, int32_
     d.n_ops = N; d.n_deps = E; d.n_workers = W; d.n_channels = C;
     d.num_training_steps = j->num_training_steps; d.model_id = j->model_id; d.degree = j->degree;
     d.n_src = (int32_t)src.size(); d.canon_id = canon;
-    d.size_class = ((int64_t)N + (int64_t)E >= e->big_threshold) ? 1 : 0;
+    d.size_class = ((int64_t)N + (int64_t)E >= BIG_THRESHOLD) ? 1 : 0;
     d.par_in_smem = par_in_smem ? 1 : 0;
     d._pad0 = 0;
     d.op_rec = (const int4*)(base + segs[0].off); d.op_n_parents = (const uint16_t*)(base + segs[1].off);
@@ -772,12 +813,12 @@ int ramp_register_template(ramp_engine_t* e, const ramp_lowered_job_t* j, int32_
     d.algorithmic_bytes_static = 20ull * (uint64_t)N + 19ull * (uint64_t)E + 24ull;
     // ---- symmetry quotient -> resident blob for the thread-per-lookahead kernel ----
     d.res_blob = nullptr; d.res_bytes = 0; d.res_n_ops = 0; d.res_n_deps = 0; d._pad2 = 0;
-    if (e->use_resident) {
+    if (e->mode == 0) {
         ramp_quotient_t q{};
         const int qrc = e->use_quotient ? ramp_quotient_template(j, &q) : identity_quotient(j, &q);
         if (qrc != RAMP_OK) { cudaFree(ht.blob); return set_error(qrc, "ramp_quotient_template failed (%d)", qrc); }
         std::vector<unsigned char> rblob;
-        if (build_resident_blob(j, q, e->res_max_bytes, rblob)) {
+        if (build_resident_blob(j, q, RESIDENT_MAX_BYTES, rblob)) {
             cudaError_t ce = cudaMalloc(&ht.res_blob, rblob.size());
             if (ce == cudaSuccess) ce = cudaMemcpy(ht.res_blob, rblob.data(), rblob.size(), cudaMemcpyHostToDevice);
             if (ce != cudaSuccess) { ramp_free_quotient(&q); cudaFree(ht.blob); return set_error(RAMP_ERR_CUDA, "resident blob upload failed: %s", cudaGetErrorString(ce)); }
@@ -872,9 +913,6 @@ int ramp_set_limits(ramp_engine_t* e, double max_sim_time, int32_t queue_capacit
 int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t fuse, double* d_stats_out, int32_t* d_ncs_out) {
     if (!e || !d_actions) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     if (e->ep.n_jobs < 1) return set_error(RAMP_ERR_BAD_ARG, "ramp_reset must be called before ramp_step");
-    if (e->templates.empty()) {
-        // allowed: every action must then be Action(); still need a scratch-less plan
-    }
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     if (e->n_nonresident > 0) { int rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
     if (e->n_resident > 0) { int rc = ensure_thread_scratch(e); if (rc != RAMP_OK) return rc; }
@@ -892,84 +930,20 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
     if (!e->templates.empty()) {
         if (e->ev_pending >= MAX_EVENT_PAIRS) { CUDA_TRY(cudaStreamSynchronize(st)); int rc = resolve_events(e); if (rc) return rc; }
         CUDA_TRY(cudaEventRecord(e->ev_a[e->ev_pending], st));
-        if (e->n_resident > 0) {
-            // memo misses on resident templates: grouped by template into chunks of <= 32, one THREAD per lookahead.  No
-            // host read-back: the counts stay on the device, idle CTAs find the chunk cursor exhausted and exit.
-            BucketArgs ba{};
-            ba.items = e->d_items_res; ba.n_items = &e->d_counters->n_work_res; ba.n_templates = (int32_t)e->templates.size();
-            ba.tcount = e->d_tcount; ba.tbase = e->d_tbase; ba.chunk_items = e->d_chunk_items; ba.chunks = e->d_chunks;
-            ba.n_chunks = &e->d_counters->n_chunks; ba.cursor = &e->d_counters->chunk_cursor; ba.rank = e->d_rank;
-            ramp_bucket_kernel<<<1, 1024, 0, st>>>(ba);
-            ThreadArgs ta = make_thread_args(e, e->d_chunks, &e->d_counters->n_chunks, &e->d_counters->chunk_cursor, e->d_chunk_items,
-                                             e->res, e->pool, e->d_stats);
-            ramp_lookahead_thread_kernel<<<e->res_grid, RAMP_THREAD_CTA, e->res_smem, st>>>(ta);
-            e->launches += 2;
-        }
+        // memo misses on resident templates: one THREAD per lookahead, grouped on the device.  Their count stays there: idle
+        // CTAs find the chunk cursor exhausted and exit.
+        if (e->n_resident > 0) bucket_resident(e, e->d_items_res, e->d_counters, e->d_chunk_items, e->d_chunks, e->d_rank, st);
+        int n_small = 0, n_big = 0;
         if (e->n_nonresident > 0) {
-        // the number of memo misses of each size class decides the kernel shapes: a 16-byte read-back (~10 us) against
-        // multi-ms kernels
-        CUDA_TRY(cudaMemcpyAsync(e->h_n_work, &e->d_counters->n_work, sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        const int n_small = e->h_n_work[0], n_big = e->h_n_work[2];
-        if (n_small + n_big > 0) {
-            LookaheadArgs a = make_lookahead_args(e, e->d_items, e->d_counters, e->res, true, e->d_stats);
-            LookaheadArgs ab = a;
-            ab.items = e->d_items_big; ab.n_work = &e->d_counters->n_work_big; ab.cursor = &e->d_counters->work_cursor_big;
-            const int wpb = e->nt / 32;
-            const int warp_slots = e->grid * wpb;
-            // The big lookaheads set the step's latency, the small ones its load.  While everything fits the SMs' warp slots
-            // at once (registers cap every mix at cta_grid x 4 warps) each big lookahead gets a 256-thread CTA if 8 warps per
-            // big one still fit (2.4 ms instead of 2.9 ms for the bench job), else a 128-thread CTA; while the big
-            // ones still fit as 64-thread CTAs and the small ones need at most a short second wave they get those; beyond
-            // that everything goes through the warp kernel, the big list first (longest-processing-time-first keeps the
-            // tail short).  The CTA kernel runs on a second stream beside the warp kernel for the small list.
-            const int reg_slots = e->cta_grid * 4;
-            int split_nt = 0;
-            if (e->mode != 1 && n_big > 0) {
-                if (e->use_cta256 && n_big <= e->cta256_grid && 8 * n_big + n_small <= reg_slots) split_nt = 256;
-                else if (n_big <= e->cta_grid && 4 * n_big + n_small <= reg_slots) split_nt = 128;
-                else if (n_big <= e->cta64_grid && 2 * n_big + n_small <= (int)(e->split_alpha * reg_slots)) split_nt = 64;
-            }
-            const bool split = split_nt != 0;
-            if (e->debug) fprintf(stderr, "[ramp] step lookaheads: small=%d big=%d warp_slots=%d reg_slots=%d -> %s %d\n", n_small, n_big,
-                                  warp_slots, reg_slots, split ? "split (CTA || warp), CTA threads" : "single warp kernel, big first", split_nt);
-            if (split) {
-                const int cgrid = e->cta_grid_for(split_nt);
-                const int grid = std::min(n_big, cgrid);
-                // `st` is idle here (synchronised for the read-back above), so the second stream needs no fork event and the
-                // CTA kernel's blocks are always placed before the warp kernel's
-                lookahead_cta_kernel_for(split_nt)<<<grid, split_nt, e->cta_smem_bytes, e->stream2>>>(ab);
-                CUDA_TRY(cudaEventRecord(e->ev_join, e->stream2));
-                e->launches++;
-                if (n_small > 0) {
-                    LookaheadArgs as = a;
-                    as.scratch = a.scratch + (uint64_t)std::max(e->cta_grid, e->cta64_grid) * a.scratch_stride;   // slabs past the CTA kernel's
-                    const int wpb2 = e->split_warp_nt / 32;
-                    const int g2 = std::max(1, std::min(e->grid * wpb / wpb2, (n_small + wpb2 - 1) / wpb2));   // never more warps than slabs
-                    lookahead_kernel_for(e->split_warp_nt)<<<g2, e->split_warp_nt, e->smem2_bytes, st>>>(as);
-                    e->launches++;
-                }
-                CUDA_TRY(cudaStreamWaitEvent(st, e->ev_join, 0));
-            } else if (e->mode == 2) {
-                if (n_big > 0) { launch_lookahead(e, ab, n_big, n_big, st); e->launches++; }
-                if (n_small > 0) { launch_lookahead(e, a, n_small, 0, st); e->launches++; }
-            } else {
-                LookaheadArgs all = ab;                      // list A = big, list B = small, one cursor
-                all.items_b = e->d_items; all.n_work_b = &e->d_counters->n_work;
-                const int n_all = n_small + n_big;
-                if (e->mode == 0 && e->dense_grid * (DENSE_NT / 32) > warp_slots && n_all > (int)(e->dense_factor * warp_slots)) {
-                    // far more lookaheads than slots: throughput matters, not the latency of one -> 16 warps per SM
-                    const int wd = DENSE_NT / 32;
-                    const int g = std::max(1, std::min(e->dense_grid, (n_all + wd - 1) / wd));
-                    lookahead_dense_kernel()<<<g, DENSE_NT, e->dense_smem_bytes, st>>>(all);
-                } else {
-                    const int g = std::max(1, std::min(e->grid, (n_all + wpb - 1) / wpb));
-                    lookahead_kernel_for(e->nt)<<<g, e->nt, e->smem_bytes, st>>>(all);
-                }
-                e->launches++;
-            }
+            // the number of memo misses of each size class decides the kernel shapes: a 16-byte read-back (~10 us) against
+            // multi-ms kernels
+            CUDA_TRY(cudaMemcpyAsync(e->h_n_work, &e->d_counters->n_work, sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaStreamSynchronize(st));
+            n_small = e->h_n_work[0]; n_big = e->h_n_work[2];
         }
-        }
+        int rc = launch_lookaheads(e, e->d_chunks, e->d_chunk_items, e->n_resident > 0 ? e->res_grid : 0, e->d_items, n_small,
+                                   e->d_items_big, n_big, e->d_counters, e->res, e->pool, e->d_stats, st);
+        if (rc != RAMP_OK) return rc;
         CUDA_TRY(cudaEventRecord(e->ev_b[e->ev_pending], st));
         e->ev_pending++;
     }
@@ -1127,55 +1101,42 @@ int ramp_run_lookaheads(ramp_engine_t* e, const int32_t* template_ids, int32_t n
     for (int32_t k = 0; k < n; ++k)
         if (template_ids[k] < 0 || template_ids[k] >= (int32_t)e->templates.size())
             return set_error(RAMP_ERR_BAD_ARG, "template id %d at %d is not registered", template_ids[k], k);
-    std::vector<int32_t> res_idx, old_idx;
-    for (int32_t k = 0; k < n; ++k) (e->templates[template_ids[k]].dev.size_class == 2 ? res_idx : old_idx).push_back(k);
+    // the step's three work lists, by size class: small and big (warp / CTA kernels), resident (thread kernel), each in item order
+    std::vector<WorkItem> lists[3];
+    std::vector<int32_t> per_template(e->templates.size(), 0);
+    for (int32_t k = 0; k < n; ++k) {
+        const int32_t t = template_ids[k], size_class = e->templates[t].dev.size_class;
+        lists[size_class].push_back(WorkItem{t, k, -1, 0});
+        if (size_class == 2) per_template[t]++;
+    }
+    const int n_small = (int)lists[0].size(), n_big = (int)lists[1].size(), n_res = (int)lists[2].size();
+    int n_chunks = 0;                   // what ramp_bucket_kernel will make of the resident list
+    for (int32_t m : per_template) n_chunks += (m + 31) / 32;
     int rc = RAMP_OK;
-    if (!old_idx.empty()) { rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
-    if (!res_idx.empty()) { rc = ensure_thread_scratch(e); if (rc != RAMP_OK) return rc; }
+    if (n_small + n_big > 0) { rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
+    if (n_res > 0) { rc = ensure_thread_scratch(e); if (rc != RAMP_OK) return rc; }
     cudaStream_t st = e->stream;
     if (n > e->sa_cap) {
         CUDA_TRY(cudaStreamSynchronize(st));
-        free_result_slots(e->sa_res); cudaFree(e->sa_items); cudaFree(e->sa_chunk_items); cudaFree(e->sa_chunks);
+        free_result_slots(e->sa_res); cudaFree(e->sa_items); cudaFree(e->sa_rank); cudaFree(e->sa_chunk_items); cudaFree(e->sa_chunks);
         if (alloc_result_slots(e->sa_res, n) != RAMP_OK) return RAMP_ERR_CUDA;
         CUDA_TRY(cudaMalloc(&e->sa_items, sizeof(WorkItem) * n));
+        CUDA_TRY(cudaMalloc(&e->sa_rank, sizeof(int32_t) * n));
         CUDA_TRY(cudaMalloc(&e->sa_chunk_items, sizeof(WorkItem) * (size_t)n * 32));
         CUDA_TRY(cudaMalloc(&e->sa_chunks, sizeof(ChunkDesc) * n));
         e->sa_cap = n;
     }
     if (!e->sa_counters) CUDA_TRY(cudaMalloc(&e->sa_counters, sizeof(Counters)));
-    std::vector<WorkItem> items(old_idx.size());
-    for (size_t q = 0; q < old_idx.size(); ++q) {
-        const int32_t k = old_idx[q];
-        items[q].template_id = template_ids[k]; items[q].slot = k; items[q].episode = -1; items[q].n_mounted_workers = 0;
-    }
-    // resident templates: chunks of <= 32 items of one template, built here (the step path builds them on the device)
-    std::vector<ChunkDesc> chunks;
-    std::vector<WorkItem> chunk_items;
-    {
-        std::vector<int32_t> order(res_idx);
-        std::stable_sort(order.begin(), order.end(), [&](int32_t x, int32_t y) { return template_ids[x] < template_ids[y]; });
-        for (size_t q = 0; q < order.size();) {
-            const int32_t t = template_ids[order[q]];
-            size_t r = q;
-            while (r < order.size() && template_ids[order[r]] == t && r - q < 32) ++r;
-            ChunkDesc cd; cd.template_id = t; cd.count = (int32_t)(r - q);
-            chunks.push_back(cd);
-            const size_t base = chunk_items.size();
-            chunk_items.resize(base + 32);
-            for (size_t x = q; x < r; ++x) {
-                WorkItem& it = chunk_items[base + (x - q)];
-                it.template_id = t; it.slot = order[x]; it.episode = -1; it.n_mounted_workers = 0;
-            }
-            q = r;
-        }
-    }
-    Counters c{}; c.n_work = (int32_t)old_idx.size(); c.n_chunks = (int32_t)chunks.size();
-    if (!items.empty()) CUDA_TRY(cudaMemcpyAsync(e->sa_items, items.data(), sizeof(WorkItem) * items.size(), cudaMemcpyHostToDevice, st));
-    if (!chunks.empty()) {
-        CUDA_TRY(cudaMemcpyAsync(e->sa_chunks, chunks.data(), sizeof(ChunkDesc) * chunks.size(), cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(e->sa_chunk_items, chunk_items.data(), sizeof(WorkItem) * chunk_items.size(), cudaMemcpyHostToDevice, st));
-    }
+    std::vector<WorkItem> items;
+    items.reserve(n);
+    for (const auto& l : lists) items.insert(items.end(), l.begin(), l.end());
+    WorkItem* const d_small = e->sa_items;
+    WorkItem* const d_big = d_small + n_small;
+    WorkItem* const d_res = d_big + n_big;
+    Counters c{}; c.n_work = n_small; c.n_work_big = n_big; c.n_work_res = n_res;
+    CUDA_TRY(cudaMemcpyAsync(e->sa_items, items.data(), sizeof(WorkItem) * n, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(e->sa_counters, &c, sizeof(Counters), cudaMemcpyHostToDevice, st));
+    if (n_res > 0) bucket_resident(e, d_res, e->sa_counters, e->sa_chunk_items, e->sa_chunks, e->sa_rank, st);
     // traces of standalone runs go to a private pool sized n x trace_cap when requested
     TracePool priv{};
     const bool want_trace = trace_n && trace_tick && trace_cap > 0;
@@ -1188,26 +1149,14 @@ int ramp_run_lookaheads(ramp_engine_t* e, const int32_t* template_ids, int32_t n
         CUDA_TRY(cudaMemsetAsync(d_top, 0, sizeof(unsigned long long), st));
         priv.top = d_top;
     }
-    LookaheadArgs a = make_lookahead_args(e, e->sa_items, e->sa_counters, e->sa_res, false, nullptr);
-    if (want_trace) a.pool = priv;
+    TracePool pool = want_trace ? priv : e->pool;
+    if (!want_trace) pool.top = nullptr;
     cudaEvent_t ea = e->ev_a[MAX_EVENT_PAIRS - 1], eb = e->ev_b[MAX_EVENT_PAIRS - 1];
     if (e->ev_pending >= MAX_EVENT_PAIRS - 1) { CUDA_TRY(cudaStreamSynchronize(st)); rc = resolve_events(e); if (rc) return rc; }
     CUDA_TRY(cudaEventRecord(ea, st));
-    if (!chunks.empty()) {
-        TracePool tp = want_trace ? priv : e->pool;
-        if (!want_trace) tp.top = nullptr;
-        ThreadArgs ta = make_thread_args(e, e->sa_chunks, &e->sa_counters->n_chunks, &e->sa_counters->chunk_cursor, e->sa_chunk_items,
-                                         e->sa_res, tp, nullptr);
-        const int g = std::max(1, std::min(e->res_grid, (int)chunks.size()));
-        ramp_lookahead_thread_kernel<<<g, RAMP_THREAD_CTA, e->res_smem, st>>>(ta);
-        e->launches++;
-    }
-    if (!old_idx.empty()) {
-        int n_big = 0;
-        for (int32_t k : old_idx) n_big += e->templates[template_ids[k]].dev.size_class == 1 ? 1 : 0;
-        launch_lookahead(e, a, (int)old_idx.size(), n_big, st);
-        e->launches++;
-    }
+    rc = launch_lookaheads(e, e->sa_chunks, e->sa_chunk_items, n_res > 0 ? std::min(e->res_grid, n_chunks) : 0, d_small, n_small,
+                           d_big, n_big, e->sa_counters, e->sa_res, pool, nullptr, st);
+    if (rc != RAMP_OK) return rc;
     CUDA_TRY(cudaEventRecord(eb, st));
     CUDA_TRY(cudaGetLastError());
     std::vector<double> jct(n), comm(n), comp(n);

@@ -9,9 +9,11 @@
  *     RampClusterEnvironment.step      RCE:894-1179 -> ramp_step_host / ramp_step_device
  *       _place_ops/_schedule_ops/_place_deps/_schedule_deps RCE:1305-1415 -> ramp_register_template (+ per-step mount rows)
  *       _perform_lookahead_job_completion_time + memo dicts RCE:469-518, RCE:269-275 -> memo hash table inside the step
- *       _run_lookahead                  RCE:379-467  -> ramp_lookahead_kernel (also callable alone: ramp_run_lookaheads)
- *       _register_completed_lookahead   RCE:793-888  -> ramp_register_kernel
- *       outer event loop + stats        RCE:942-1167 -> ramp_advance_kernel
+ *       _run_lookahead                  RCE:379-467  -> ramp_lookahead_thread_kernel, or ramp_lookahead_kernel /
+ *                                                       ramp_lookahead_cta_kernel for jobs too large for it
+ *                                                       (also callable alone: ramp_run_lookaheads)
+ *       _register_completed_lookahead   RCE:793-888  -> ramp_step_kernel
+ *       outer event loop + stats        RCE:942-1167 -> ramp_step_kernel
  *     RampClusterEnvironment.is_done   RCE:1542-1557 -> stats[RAMP_SS_DONE]
  * batched over `n_episodes` independent cluster instances (one per RL rollout) that advance in lock step.
  * ddls_b200/engine.py is the ctypes binding; INTEGRATION.md shows the stub a reference maintainer would add.
@@ -215,10 +217,12 @@ int ramp_get_memo_stats_ex(ramp_engine_t* eng, int64_t out[4]);
 int ramp_get_last_lookahead(ramp_engine_t* eng, int32_t episode, ramp_lookahead_result_t* res,
                             int32_t* trace_n_active, double* trace_tick, int32_t trace_cap);
 
-/* ---- the lookahead kernel on its own ------------------------------------------------------------ */
+/* ---- the lookahead kernels on their own --------------------------------------------------------- */
 /* Runs _run_lookahead (RCE:379-467) for n work items; item k uses template template_ids[k] (HOST array).
+ * The items go to the lookahead kernels by the rule a step uses for its memo misses.
  * results: HOST [n].  trace_n_active / trace_tick: HOST [n][trace_cap] or NULL.  kernel_ms_out (may be
- * NULL) receives the CUDA-event duration of the kernel alone. */
+ * NULL) receives the CUDA-event duration of the lookahead kernels, without the uploads and the grouping of
+ * the resident items by template. */
 int ramp_run_lookaheads(ramp_engine_t* eng, const int32_t* template_ids, int32_t n,
                         ramp_lookahead_result_t* results, int32_t* trace_n_active, double* trace_tick,
                         int32_t trace_cap, float* kernel_ms_out);
