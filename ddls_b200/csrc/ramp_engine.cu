@@ -308,10 +308,11 @@ int bits_for_u64(uint64_t max_value) { int b = 1; while ((max_value >> b) != 0) 
 
 // Packs a quotient job (ramp_quotient.cpp) into the blob the thread-per-lookahead kernel bulk-copies into shared memory
 // (layout: ResHeader, ramp_lookahead_thread.cuh).  Returns false when the job is not eligible: blob larger than
-// max_bytes, class sizes / counters beyond 16 bits, or a dep word wider than 64 bits.
+// max_bytes, more channel groups than the kernel's winner table holds (RAMP_T_CCAP), class sizes / counters beyond 16
+// bits, or a dep word wider than 64 bits.
 bool build_resident_blob(const ramp_lowered_job_t* j, const ramp_quotient_t& q, int32_t max_bytes, std::vector<unsigned char>& blob) {
     const int32_t N = q.n_ops, E = q.n_deps;
-    if (N < 1 || q.n_workers > 0xFFFF || q.n_channels >= 0xFFFF) return false;
+    if (N < 1 || q.n_workers > 0xFFFF || q.n_channels > RAMP_T_CCAP) return false;
     if (!q.masks_valid) return false;
     std::vector<uint64_t> in_total(N, 0);
     uint32_t max_inc = 1;

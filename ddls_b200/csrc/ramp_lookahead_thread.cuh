@@ -47,8 +47,8 @@ namespace ramp {
 #ifndef RAMP_T_NFCAP
 #define RAMP_T_NFCAP 8      // ready non-flow entries kept in shared memory per lane
 #endif
-#define RAMP_T_WCAP 8       // worker groups / channel groups with a per-lane winner table (more: pairwise comparison)
-#define RAMP_T_CCAP 32
+#define RAMP_T_WCAP 8       // worker groups with a per-lane winner table (more: pairwise comparison)
+#define RAMP_T_CCAP 32      // channel groups with a per-lane winner table: the most a resident template may have
 #ifndef RAMP_T_RING
 #define RAMP_T_RING 32      // tick records per lane in the sim -> ledger ring (a power of two)
 #endif
@@ -311,9 +311,10 @@ struct LaneCtx {                      // what one sim lane's lookahead works on
 
 // _run_lookahead for one sim lane: the tick loop (A-H, K, L); every tick goes to the ledger lane as one ring record, and the
 // final status, tick count and largest frontiers follow the last one.  SPILL = false: every frontier fits its shared-memory
-// capacity (TemplateHints); SIMPLE = true: one worker group and at most one channel group (the usual quotient of a
-// partitioned job): the winner is the largest key, no tables.
-template <bool SPILL, bool SIMPLE>
+// capacity (TemplateHints).  A tick with at most 2 ready op classes and RAMP_T_FASTF ready flow entries (every tick of the
+// usual quotient of a partitioned job) runs the small-frontier half; any other tick runs the general half, whose winners come
+// from per-group tables.  Both halves share the steps defined ahead of the loop and the end of the tick.
+template <bool SPILL>
 __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
     const int lane = x.lane;
     const ResHeader& H = *reinterpret_cast<const ResHeader*>(x.tm);
@@ -325,7 +326,7 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
     const int N = H.n_ops, E = H.n_deps, W = H.n_workers, C = H.n_channels;
     const uint32_t kmask = H.kmask, imask = H.imask;
     const int csh = H.cshift, dsh = H.dshift;
-    const bool tab_w = (W <= RAMP_T_WCAP), tab_c = (C <= RAMP_T_CCAP);
+    const bool tab_w = (W <= RAMP_T_WCAP);
     const LaneOps<SPILL> ops{x.o_sm, x.oi_sm, x.o_gl, x.oi_gl, lane};
     const LaneFlows<SPILL> flows{x.f_sm, x.f_gl, lane};
     const LaneNF<SPILL> nfs{x.nf_sm, x.nf_gl, lane};
@@ -353,19 +354,45 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
     int to_complete = N + E;              // ops and deps still to complete (JOB:549-551)
     LedgerFeed feed{x.ring, x.head, x.tail, x.fin, lane, 0u, (uint32_t)RAMP_T_RING};
     RAMP_TC(TickClocks tc; tc.lane = lane;)
+    // the tick's state: t_op = smallest remaining time of the op winners and n_active = their class sizes (A, B), the tick
+    // (E), and tailO, the end of the op-class frontier: classes readied in the tick are appended behind it (H, G)
+    u64_t t_op = RAMP_INF_BITS, tick_b = 0ull;
+    double tick = 0.0;
+    int n_active = 0, tailO = nO;
+    auto complete_dep = [&](const uint32_t hi) {                                                    // JOB:525-536
+        const int child = (int)(hi >> dsh);
+        const uint32_t inc = (hi >> 1) & imask;
+        const uint32_t old = cnt[child * 32];
+        const uint32_t thr = op_thr[child];
+        const uint32_t neu = old + inc;
+        cnt[child * 32] = (uint16_t)neu;
+        if (old < thr && thr <= neu) { ops.put(tailO, op_rec[child], child); ++tailO; }             // JOB:531 for every member
+    };
+    // ---- E: the tick; its record goes to the ledger lane (I, J) ----
+    auto take_tick = [&](const u64_t t_comm, const bool ticked_flows) {
+        tick_b = (t_comm < t_op) ? t_comm : t_op;
+        tick = __longlong_as_double((long long)tick_b);
+        feed.put(tick_b, n_active, ticked_flows);
+        if (R.tick_no >= x.tr_cap) R.status = RAMP_ST_TRACE_OVERFLOW;
+        ++R.tick_no;
+        RAMP_TC(tc.stamp(2);)
+    };
 
     if (R.status == RAMP_ST_OK) for (;;) {       // left through ONE combined exit test per tick
         RAMP_TC(tc.begin(nO, nF, nNF > 0);)
+        t_op = RAMP_INF_BITS;
+        n_active = 0;
+        tailO = nO;
+        const bool any_nf = nNF > 0;
+        int p = 0;                               // op classes left after G
         if (nF <= RAMP_T_FASTF && nO <= 2) {
             // ======== small frontiers (the usual case on a quotient): every ready item is loaded ONCE into registers and each
-            // phase runs code specialised for the exact number of ready ops (0-2) and flows (0-4): winners by pairwise
+            // phase runs code specialised for the exact number of ready ops (0-2) and flows (0-6): winners by pairwise
             // comparison (no tables, any number of worker / channel groups), no loop or predication overhead ========
             static_assert(RAMP_T_FASTF == 6, "the dispatch below has cases for up to 6 ready flow entries");
             int4 fr[RAMP_T_FASTF], orr[2];
             int oi[2];
             bool ow0 = false, ow1 = false;
-            u64_t t_op = RAMP_INF_BITS;
-            int n_active = 0;
             // ---- A, B ----
             if (nO >= 1) {
                 orr[0] = x.o_sm[lane]; oi[0] = x.oi_sm[lane];
@@ -380,28 +407,6 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
             }
             RAMP_TC(tc.stamp(1);)
             // ---- C, D, E, I, J, H: dispatched ONCE on the number of ready flow entries; each case is straight-line code ----
-            const bool any_nf = nNF > 0;
-            u64_t tick_b = 0ull;
-            double tick = 0.0;
-            int tailO = nO;
-            auto complete_dep = [&](const uint32_t hi) {                                            // JOB:525-536
-                const int child = (int)(hi >> dsh);
-                const uint32_t inc = (hi >> 1) & imask;
-                const uint32_t old = cnt[child * 32];
-                const uint32_t thr = op_thr[child];
-                const uint32_t neu = old + inc;
-                cnt[child * 32] = (uint16_t)neu;
-                if (old < thr && thr <= neu) { ops.put(tailO, op_rec[child], child); ++tailO; }     // JOB:531 for every member
-            };
-            // E: the tick; its record goes to the ledger lane (I, J)
-            auto take_tick = [&](const u64_t t_comm, const bool ticked_flows) {
-                tick_b = (t_comm < t_op) ? t_comm : t_op;
-                tick = __longlong_as_double((long long)tick_b);
-                feed.put(tick_b, n_active, ticked_flows);
-                if (R.tick_no >= x.tr_cap) R.status = RAMP_ST_TRACE_OVERFLOW;
-                ++R.tick_no;
-                RAMP_TC(tc.stamp(2);)
-            };
             auto flow_tick = [&](auto nf_tag) {
                 constexpr int NF = decltype(nf_tag)::value;
                 uint32_t gm[NF], key[NF];
@@ -420,17 +425,17 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                     if (open_groups) { const u64_t rem = rem_bits(fr[k]); t_comm = (rem < t_comm) ? rem : t_comm; }
                 }
                 take_tick(t_comm, true);
-                int p = 0;
+                int pf = 0;
 #pragma unroll
                 for (int k = 0; k < NF; ++k) {
                     const u64_t rb = rem_bits(fr[k]);
                     if (rb <= tick_b) { complete_dep((uint32_t)fr[k].w); --to_complete; }        // JOB:561-562
                     else {
                         const double r2 = __dsub_rn(__longlong_as_double((long long)rb), tick);
-                        fr[k].x = __double2loint(r2); fr[k].y = __double2hiint(r2); x.f_sm[p * 32 + lane] = fr[k]; ++p;
+                        fr[k].x = __double2loint(r2); fr[k].y = __double2hiint(r2); x.f_sm[pf * 32 + lane] = fr[k]; ++pf;
                     }
                 }
-                nF = p;
+                nF = pf;
             };
             // by frequency on the quotient of a partitioned job: one ready flow entry, a non-flow tick, none, two, ...
             if (any_nf) {                                           // zero-length tick that completes the ready non-flow deps
@@ -453,7 +458,6 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
             }
             RAMP_TC(tc.stamp(3);)
             // ---- G ----
-            int p = 0;
             auto tick_op = [&](int4 r, const int op, const bool win) {
                 if (win) {                                                                          // this tick's winner
                     const u64_t rb = rem_bits(r);
@@ -471,94 +475,57 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                 tick_op(orr[0], oi[0], ow0);
                 if (nO == 2) tick_op(orr[1], oi[1], ow1);
             }
-            RAMP_TC(tc.stamp(4);)
-            if (tailO != nO) {
-                _Pragma("unroll 1")
-                for (int k = nO; k < tailO; ++k, ++p) { if (p != k) ops.put(p, ops.rec(k), ops.idx(k)); }
-            }
-            nO = p;
-            if (SPILL) {
-                R.max_o = (tailO > R.max_o) ? tailO : R.max_o;
-                R.max_f = (nF > R.max_f) ? nF : R.max_f;
-                R.max_nf = (nNF > R.max_nf) ? nNF : R.max_nf;
-            }
-            if ((to_complete == 0) | ((uint32_t)(tick_b >> 32) == 0x7FF00000u) | (R.status != RAMP_ST_OK)) {
-                if (to_complete != 0 && (uint32_t)(tick_b >> 32) == 0x7FF00000u) R.status = RAMP_ST_INFINITE_TICK;   // JOB:549-551 first, then RCE:462
-                break;
-            }
-            continue;
-        }
-        // ---- A, B: winners per worker group: largest key; t_op = min of their remaining times ----
-        u64_t t_op = RAMP_INF_BITS;
-        int n_active = 0;
-        uint32_t best_w = 0u;                 // SIMPLE: the winner's key
-        if (nO > 0) {
-            if (SIMPLE) {
-                _Pragma("unroll 1")
-                for (int k = 0; k < nO; ++k) {
-                    const int4 r = ops.rec(k);
-                    if ((uint32_t)r.z > best_w) { best_w = (uint32_t)r.z; t_op = rem_bits(r); n_active = (int)((uint32_t)r.w >> 16); }
-                }
-            } else if (tab_w) {
-                _Pragma("unroll 1")
-                for (int w = 0; w < W; ++w) wk[w * 32] = 0u;
-                _Pragma("unroll 1")
-                for (int k = 0; k < nO; ++k) {
-                    const int4 r = ops.rec(k);
-                    const int w = r.w & 0xffff;
-                    if ((uint32_t)r.z > wk[w * 32]) wk[w * 32] = (uint32_t)r.z;
-                }
-                _Pragma("unroll 1")
-                for (int k = 0; k < nO; ++k) {
-                    const int4 r = ops.rec(k);
-                    if (wk[(r.w & 0xffff) * 32] == (uint32_t)r.z) {
-                        const u64_t rem = rem_bits(r);
-                        t_op = (rem < t_op) ? rem : t_op;
-                        n_active += (int)((uint32_t)r.w >> 16);
-                    }
-                }
-            } else {
-                // more worker groups than table slots: pairwise comparison; the winners are marked in bit 31 of the key
-                // (keys are ranks <= N < 2^31) for phase G, which clears the mark
-                _Pragma("unroll 1")
-                for (int k = 0; k < nO; ++k) {
-                    int4 r = ops.rec(k);
-                    bool win = true;
+        } else {
+            // ---- A, B: winners per worker group: largest key; t_op = min of their remaining times ----
+            if (nO > 0) {
+                if (tab_w) {
                     _Pragma("unroll 1")
-                    for (int j = 0; j < nO && win; ++j) {
-                        const int4 r2 = ops.rec(j);
-                        if ((r2.w & 0xffff) == (r.w & 0xffff) && ((uint32_t)r2.z & 0x7fffffffu) > (uint32_t)r.z) win = false;
+                    for (int w = 0; w < W; ++w) wk[w * 32] = 0u;
+                    _Pragma("unroll 1")
+                    for (int k = 0; k < nO; ++k) {
+                        const int4 r = ops.rec(k);
+                        const int w = r.w & 0xffff;
+                        if ((uint32_t)r.z > wk[w * 32]) wk[w * 32] = (uint32_t)r.z;
                     }
-                    if (win) {
-                        const u64_t rem = rem_bits(r);
-                        t_op = (rem < t_op) ? rem : t_op;
-                        n_active += (int)((uint32_t)r.w >> 16);
-                        r.z = (int)((uint32_t)r.z | 0x80000000u);
-                        ops.put(k, r, ops.idx(k));
+                    _Pragma("unroll 1")
+                    for (int k = 0; k < nO; ++k) {
+                        const int4 r = ops.rec(k);
+                        if (wk[(r.w & 0xffff) * 32] == (uint32_t)r.z) {
+                            const u64_t rem = rem_bits(r);
+                            t_op = (rem < t_op) ? rem : t_op;
+                            n_active += (int)((uint32_t)r.w >> 16);
+                        }
+                    }
+                } else {
+                    // more worker groups than table slots: pairwise comparison; the winners are marked in bit 31 of the key
+                    // (keys are ranks <= N < 2^31) for phase G, which clears the mark
+                    _Pragma("unroll 1")
+                    for (int k = 0; k < nO; ++k) {
+                        int4 r = ops.rec(k);
+                        bool win = true;
+                        _Pragma("unroll 1")
+                        for (int j = 0; j < nO && win; ++j) {
+                            const int4 r2 = ops.rec(j);
+                            if ((r2.w & 0xffff) == (r.w & 0xffff) && ((uint32_t)r2.z & 0x7fffffffu) > (uint32_t)r.z) win = false;
+                        }
+                        if (win) {
+                            const u64_t rem = rem_bits(r);
+                            t_op = (rem < t_op) ? rem : t_op;
+                            n_active += (int)((uint32_t)r.w >> 16);
+                            r.z = (int)((uint32_t)r.z | 0x80000000u);
+                            ops.put(k, r, ops.idx(k));
+                        }
                     }
                 }
             }
-        }
-        RAMP_TC(tc.stamp(1);)
-        // ---- C, D ----
-        const bool any_nf = nNF > 0;
-        u64_t t_comm = 0ull;
-        if (!any_nf) {
-            t_comm = RAMP_INF_BITS;
-            if (nF > 0) {
-                if (SIMPLE) {
-                    uint32_t best = 0u;
-                    _Pragma("unroll 1")
-                    for (int k = 0; k < nF; ++k) {
-                        const int4 f = flows.get(k);
-                        if (((uint32_t)f.z >> csh) == 0u) continue;                                  // no channel: ticks, never a winner
-                        const uint32_t key = (uint32_t)f.z & kmask;
-                        const u64_t rem = rem_bits(f);
-                        if (key > best) { best = key; t_comm = rem; }
-                        else if (key == best) t_comm = (rem < t_comm) ? rem : t_comm;
-                    }
-                } else if (tab_c) {
-                    // per-group table: largest key among the ready entries whose set contains the group
+            RAMP_TC(tc.stamp(1);)
+            // ---- C, D ----
+            u64_t t_comm = 0ull;
+            if (!any_nf) {
+                t_comm = RAMP_INF_BITS;
+                if (nF > 0) {
+                    // per-group table: largest key among the ready entries whose set contains the group (a resident template
+                    // has at most RAMP_T_CCAP channel groups: build_resident_blob)
                     _Pragma("unroll 1")
                     for (int q = 0; q < C; ++q) ck[q * 32] = 0u;
                     _Pragma("unroll 1")
@@ -577,88 +544,59 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                         while (m && !win) { const int q = __ffs((int)m) - 1; m &= m - 1u; win = ck[q * 32] == key; }
                         if (win) { const u64_t rem = rem_bits(f); t_comm = (rem < t_comm) ? rem : t_comm; }
                     }
-                } else {
-                    _Pragma("unroll 1")
-                    for (int k = 0; k < nF; ++k) {
-                        const int4 f = flows.get(k);
-                        uint32_t open_groups = (uint32_t)f.z >> csh;
-                        if (open_groups == 0u) continue;
-                        const uint32_t key = (uint32_t)f.z & kmask;
-                        _Pragma("unroll 1")
-                        for (int j = 0; j < nF && open_groups; ++j) {
-                            const uint32_t lo2 = (uint32_t)flows.get(j).z;
-                            if ((lo2 & kmask) > key) open_groups &= ~(lo2 >> csh);
-                        }
-                        if (open_groups) { const u64_t rem = rem_bits(f); t_comm = (rem < t_comm) ? rem : t_comm; }
+                }
+            }
+            take_tick(t_comm, (!any_nf) && (nF > 0));
+            // ---- H ----
+            if (any_nf) {
+                _Pragma("unroll 1")
+                for (int k = 0; k < nNF; ++k) complete_dep(nfs.get(k));
+                to_complete -= nNF;
+                nNF = 0;
+            } else {
+                int pf = 0;
+                _Pragma("unroll 1")
+                for (int k = 0; k < nF; ++k) {
+                    int4 f = flows.get(k);
+                    const u64_t rb = rem_bits(f);
+                    if (rb <= tick_b) { complete_dep((uint32_t)f.w); --to_complete; }            // JOB:561-562
+                    else {
+                        const double r2 = __dsub_rn(__longlong_as_double((long long)rb), tick);
+                        f.x = __double2loint(r2); f.y = __double2hiint(r2); flows.put(pf, f); ++pf;
                     }
                 }
+                nF = pf;
             }
-        }
-        // ---- E (I, J on the ledger lane) ----
-        const u64_t tick_b = (t_comm < t_op) ? t_comm : t_op;
-        const double tick = __longlong_as_double((long long)tick_b);
-        feed.put(tick_b, n_active, (!any_nf) && (nF > 0));
-        if (R.tick_no >= x.tr_cap) R.status = RAMP_ST_TRACE_OVERFLOW;
-        ++R.tick_no;
-        RAMP_TC(tc.stamp(2);)
-        // ---- H ----
-        int tailO = nO;                       // ops readied in this tick are appended behind the current frontier
-        auto complete_dep = [&](const uint32_t hi) {                                                // JOB:525-536
-            const int child = (int)(hi >> dsh);
-            const uint32_t inc = (hi >> 1) & imask;
-            const uint32_t old = cnt[child * 32];
-            const uint32_t thr = op_thr[child];
-            const uint32_t neu = old + inc;
-            cnt[child * 32] = (uint16_t)neu;
-            if (old < thr && thr <= neu) { ops.put(tailO, op_rec[child], child); ++tailO; }         // JOB:531 for every member
-        };
-        if (any_nf) {
+            RAMP_TC(tc.stamp(3);)
+            // ---- G ----
             _Pragma("unroll 1")
-            for (int k = 0; k < nNF; ++k) complete_dep(nfs.get(k));
-            to_complete -= nNF;
-            nNF = 0;
-        } else {
-            int p = 0;
-            _Pragma("unroll 1")
-            for (int k = 0; k < nF; ++k) {
-                int4 f = flows.get(k);
-                const u64_t rb = rem_bits(f);
-                if (rb <= tick_b) { complete_dep((uint32_t)f.w); --to_complete; }                // JOB:561-562
-                else {
-                    const double r2 = __dsub_rn(__longlong_as_double((long long)rb), tick);
-                    f.x = __double2loint(r2); f.y = __double2hiint(r2); flows.put(p, f); ++p;
+            for (int k = 0; k < nO; ++k) {
+                int4 r = ops.rec(k);
+                const int op = ops.idx(k);
+                bool win;
+                if (tab_w) win = wk[(r.w & 0xffff) * 32] == (uint32_t)r.z;
+                else { win = r.z < 0; r.z &= 0x7fffffff; }
+                if (win) {                                                                          // this tick's winner
+                    const u64_t rb = rem_bits(r);
+                    if (rb <= tick_b) {                                                             // JOB:555-556
+                        --to_complete;
+                        complete_op(op);
+                        continue;
+                    }
+                    const double rem = __dsub_rn(__longlong_as_double((long long)rb), tick);
+                    r.x = __double2loint(rem); r.y = __double2hiint(rem);
                 }
+                ops.put(p, r, op); ++p;
             }
-            nF = p;
-        }
-        RAMP_TC(tc.stamp(3);)
-        // ---- G ----
-        int p = 0;
-        _Pragma("unroll 1")
-        for (int k = 0; k < nO; ++k) {
-            int4 r = ops.rec(k);
-            const int op = ops.idx(k);
-            bool win;
-            if (SIMPLE) win = (uint32_t)r.z == best_w;
-            else if (tab_w) win = wk[(r.w & 0xffff) * 32] == (uint32_t)r.z;
-            else { win = r.z < 0; r.z &= 0x7fffffff; }
-            if (win) {                                                                              // this tick's winner
-                const u64_t rb = rem_bits(r);
-                if (rb <= tick_b) {                                                                 // JOB:555-556
-                    --to_complete;
-                    complete_op(op);
-                    continue;
-                }
-                const double rem = __dsub_rn(__longlong_as_double((long long)rb), tick);
-                r.x = __double2loint(rem); r.y = __double2hiint(rem);
-            }
-            ops.put(p, r, op); ++p;
         }
         RAMP_TC(tc.stamp(4);)
-        _Pragma("unroll 1")
-        for (int k = nO; k < tailO; ++k, ++p) { if (p != k) ops.put(p, ops.rec(k), ops.idx(k)); }
+        // the classes readied in this tick go behind the p that are left
+        if (tailO != nO) {
+            _Pragma("unroll 1")
+            for (int k = nO; k < tailO; ++k, ++p) { if (p != k) ops.put(p, ops.rec(k), ops.idx(k)); }
+        }
         nO = p;
-        if (SPILL) {                          // the sizes the fast path relies on next time (TemplateHints)
+        if (SPILL) {                              // the sizes the fast path relies on next time (TemplateHints)
             R.max_o = (tailO > R.max_o) ? tailO : R.max_o;
             R.max_f = (nF > R.max_f) ? nF : R.max_f;
             R.max_nf = (nNF > R.max_nf) ? nNF : R.max_nf;
@@ -851,15 +789,9 @@ __global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(
         if (is_sim) {
             if (active) {
                 x.tr_cap = s_tr_cap[lane];
-                const bool simple = (H.n_workers == 1) && (H.n_channels <= 1);
                 // one instantiation per line: scripts/tick_cycles.py finds each one's SASS by the line it is inlined at
-                if (fast) {
-                    if (simple) thread_lookahead<false, true>(x);
-                    else thread_lookahead<false, false>(x);
-                } else {
-                    if (simple) thread_lookahead<true, true>(x);
-                    else thread_lookahead<true, false>(x);
-                }
+                if (fast) thread_lookahead<false>(x);
+                else thread_lookahead<true>(x);
             }
             continue;
         }

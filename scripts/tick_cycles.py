@@ -7,8 +7,9 @@ quotient templates (ResNet-50-like job at degrees 2 / 4 / 8 / 16, 4x4x4 RAMP, li
 four mixed, n lookaheads, then each degree alone, n / 4 lookaheads.  For each run it prints lane 0's cycles per tick by
 phase and by frontier shape (ready op classes O, ready flow entries F, non-flow tick nf) with each shape's share of the
 ticks.  Beside it: microseconds per tick of the instrumented build and of the normal build (the clock() reads cost a
-little), and the static side from the normal build's SASS -- instructions of the kernel, of thread_lookahead<false, true>
-(the instantiation the bench's templates run), of its tick loop and of its small-frontier path.
+little), and the static side from the normal build's SASS -- instructions of the kernel, of thread_lookahead<false>
+(the hinted instantiation, which every lookahead after a template's first runs), of its tick loop and of its small-frontier
+half.
 """
 import argparse
 import ctypes as C
@@ -115,7 +116,7 @@ def static_side(lib, tmp):
     src = open(CUH).read().splitlines()
     def line_of(pat):
         return next(i + 1 for i, l in enumerate(src) if pat in l)
-    call = line_of('if (simple) thread_lookahead<false, true>(x);')
+    call = line_of('if (fast) thread_lookahead<false>(x);')
     loop0, loop1 = line_of('for (;;) {       // left through ONE'), line_of('feed.finish(R);')
     fast0, fast1 = line_of('if (nF <= RAMP_T_FASTF && nO <= 2) {'), line_of('// ---- A, B: winners per worker group')
     subprocess.run([cuda_tool('cuobjdump'), '-xelf', 'all', os.path.abspath(lib)], check=True, cwd=tmp, capture_output=True)
@@ -176,8 +177,8 @@ def main():
     with tempfile.TemporaryDirectory() as tmp:
         st = static_side(normal_lib, tmp)
     print(f'GPU: {gpu_line()}')
-    print(f'thread_lookahead<false, true> in the normal build: {st["instantiation"]} instructions ({st["instantiation"] * 16} B), '
-          f'tick loop {st["tick_loop"]}, small-frontier path {st["small_frontier_path"]}; whole kernel {st["kernel"]} '
+    print(f'thread_lookahead<false> in the normal build: {st["instantiation"]} instructions ({st["instantiation"] * 16} B), '
+          f'tick loop {st["tick_loop"]}, small-frontier half {st["small_frontier_path"]}; whole kernel {st["kernel"]} '
           f'({st["kernel"] * 16} B)')
     normal = sub(normal_lib, args, False)
     inst = sub(variant, args, True)

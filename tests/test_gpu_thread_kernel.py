@@ -25,7 +25,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FILES = golden_files()
 THREAD_MODES = ['thread', 'thread_unfolded']
 MODES = THREAD_MODES + ['warp', 'cta']
-OCAP, FASTF, FCAP, NFCAP, WCAP = 8, 6, 16, 8, 8        # RAMP_T_* of the normal build
+OCAP, FASTF, FCAP, NFCAP, WCAP, CCAP = 8, 6, 16, 8, 8, 32    # RAMP_T_* of the normal build
 RES_MAX_BYTES = 96 * 1024                                 # ramp_engine.cu res_max_bytes
 MODEL_MAX_WORK = 20_000_000                               # (classes + entries) x ticks the Python model is run for
 
@@ -117,9 +117,9 @@ def model_peaks(job, mode):
 
 def resident_rule(job, q):
     """ramp_engine.cu build_resident_blob's eligibility, restated: the quotient fits the 96 KB blob, its counters 16 bits,
-    and a dep word's key + one bit per channel group fit 32 bits."""
+    it has at most RAMP_T_CCAP channel groups, and a dep word's key + one bit per channel group fit 32 bits."""
     N, E = q.n_ops, q.n_deps
-    if N < 1 or not q.masks_valid:
+    if N < 1 or not q.masks_valid or q.n_channels > CCAP:
         return False
     bits = lambda v: max(1, int(v).bit_length())
     in_total = np.bincount(q.dep_dst, weights=q.dep_inc, minlength=N) if E else np.zeros(N)
@@ -161,8 +161,9 @@ def test_model_peaks_match_the_oracle_traces(oracle_lib):
 
 @pytest.mark.parametrize('n_groups', [32, 40])
 def test_32_channel_groups_are_never_resident(n_groups):
-    """A resident dep word holds the key and one bit per channel group in 32 bits, so a resident template has at most 31
-    channel groups and the thread kernel's pairwise channel-winner branch (more than RAMP_T_CCAP = 32 groups) is unreachable."""
+    """A resident template has at most RAMP_T_CCAP = 32 channel groups, the size of the thread kernel's per-channel-group
+    winner table, which is its only channel-winner path.  A resident dep word also holds the key and one bit per channel
+    group in 32 bits, so in fact 32 groups are already too many."""
     job = channel_groups_template(n_groups)
     q = native_quotient(job)
     assert q.n_channels == n_groups
