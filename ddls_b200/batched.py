@@ -133,6 +133,8 @@ class BatchedRampJobPartitioningEnvironment:
         self.queued = np.zeros(B, dtype=np.int64)                 # RCE:280-281: job 0 is queued
         self.done = np.zeros(B, dtype=bool)
         self.n_running = np.zeros(B, dtype=np.int64)
+        self.job_template = np.full((B, J), -1, dtype=np.int32)    # template each accepted job was mounted with
+        self.episode_return = np.zeros(B, dtype=np.float64)        # sum of the rewards since the reset
         self.step_counter = 0
         return self._observe()
 
@@ -291,6 +293,8 @@ class BatchedRampJobPartitioningEnvironment:
         # ---- occupancy: servers of the jobs that are running now ----
         acc = np.nonzero(accepted)[0]
         self.job_mask[acc, qq[acc]] = mask_words[acc]
+        self.job_template[acc, qq[acc]] = tid[acc]
+        self.episode_return += reward
         running = (status == _engine.JS_RUNNING)
         self.busy = np.bitwise_or.reduce(np.where(running[:, :, None], self.job_mask, np.uint64(0)), axis=1)
         self.n_running = running.sum(axis=1)
@@ -301,6 +305,63 @@ class BatchedRampJobPartitioningEnvironment:
         self.step_counter += 1
         info = {'template_id': tid, 'cluster_steps': ncs, 'accepted': accepted}
         return self._observe(), reward, self.done.copy(), info
+
+    # ---- EvalLoop's episode statistics ----------------------------------------------------------------------------
+    def _episode_tables(self):
+        return self.job_template, self.episode_return
+
+    def episode_stats(self):
+        """RampClusterEnvironment.episode_stats of every episode, keyed by the reference's names (RCE:1086-1167, 1466-1540), plus
+        EvalLoop's ``return`` (loops/eval_loop.py:26-134).  Every scalar is an array [B] (``engine.ES_FIELDS``: the finalised
+        episode means over every cluster step, fused ones included; episodes that are not done hold the same formulas over the
+        episode so far).  The per-job lists are lists of B arrays in completion order (event order): ``job_completion_time``,
+        ``job_completion_time_speedup``, ``job_communication_overhead_time``, ``job_computation_overhead_time``,
+        ``jobs_completed_mean_mounted_worker_utilisation_frac``, ``jobs_completed_num_mounted_workers`` / ``_channels``,
+        ``jobs_completed_max_acceptable_job_completion_time``, ``jobs_blocked_max_acceptable_job_completion_time``, with the job
+        indices in ``completed_job_idxs`` / ``blocked_job_idxs``.  Reads the [B][J] tables back once: call it when episodes end."""
+        ES = _engine.ES
+        rows = self.eng.episode_stats()
+        job_template, ret = self._episode_tables()
+        rec = self.eng.job_records()
+        out = {}
+        for k in _engine.ES_FIELDS:
+            col = rows[:, ES[k]]
+            out[k] = col.astype(np.int64) if k in _engine.ES_COUNTS else col.astype(bool) if k == 'done' else col.copy()
+        out['return'] = np.array(ret, dtype=np.float64)
+        mounts = self._mount_arrays()
+        if not len(mounts):
+            mounts = np.zeros((1, 6))
+        seq = np.array([m.seq_time for m in self.models], dtype=np.float64)
+        # every [B][J] table in each episode's event order
+        order = np.argsort(rec['event_seq'], axis=1, kind='stable')
+        r = np.take_along_axis(rec, order, axis=1)
+        tid = np.take_along_axis(job_template, order, axis=1)
+        model_of = np.take_along_axis(self.model_of, order, axis=1)
+        # the job's max acceptable JCT as the action row carried it: the override, else frac x the sequential time of the template
+        # it was mounted with (of its model when it was never mounted)
+        macc = np.take_along_axis(self.frac, order, axis=1) * np.where(tid >= 0, mounts[np.maximum(tid, 0), 0], seq[model_of])
+        if self.macc_override is not None:
+            ov = np.take_along_axis(self.macc_override, order, axis=1)
+            macc = np.where(np.isnan(ov), macc, ov)
+        comp, blk = r['status'] == _engine.JS_COMPLETED, r['status'] == _engine.JS_BLOCKED
+
+        def per_episode(mask, values):
+            return np.split(values[mask], np.cumsum(mask.sum(axis=1))[:-1])
+        jct = r['time_completed'] - r['time_arrived']
+        mt = mounts[np.maximum(tid, 0)]
+        with np.errstate(divide='ignore', invalid='ignore'):
+            speedup = seq[model_of] / jct
+        lists = {'job_completion_time': per_episode(comp, jct), 'job_completion_time_speedup': per_episode(comp, speedup),
+                 'job_communication_overhead_time': per_episode(comp, r['comm']),
+                 'job_computation_overhead_time': per_episode(comp, r['comp']),
+                 'jobs_completed_mean_mounted_worker_utilisation_frac': per_episode(comp, r['util']),
+                 'jobs_completed_num_mounted_workers': per_episode(comp, mt[..., 4].astype(np.int64)),
+                 'jobs_completed_num_mounted_channels': per_episode(comp, mt[..., 5].astype(np.int64)),
+                 'jobs_completed_max_acceptable_job_completion_time': per_episode(comp, macc),
+                 'jobs_blocked_max_acceptable_job_completion_time': per_episode(blk, macc),
+                 'completed_job_idxs': per_episode(comp, order.astype(np.int64)), 'blocked_job_idxs': per_episode(blk, order.astype(np.int64))}
+        out.update(lists)
+        return out
 
     # ---- observations ---------------------------------------------------------------------------------------------
     def jobs_params(self):
@@ -596,6 +657,16 @@ class DeviceRampJobPartitioningEnvironment(BatchedRampJobPartitioningEnvironment
         L.ramp_env_read_state.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _engine._check(L.ramp_env_read_state(self.eng._h, None, None, out.ctypes.data))
         return out
+
+    def _episode_tables(self):
+        import ctypes as C
+        job_template = np.zeros((self.B, self.J), dtype=np.int32)
+        ret = np.zeros(self.B, dtype=np.float64)
+        L = self.eng._L
+        L.ramp_env_read_episode.restype = C.c_int
+        L.ramp_env_read_episode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _engine._check(L.ramp_env_read_episode(self.eng._h, job_template.ctypes.data, ret.ctypes.data))
+        return job_template, ret
 
     def _decide_on_host(self, episodes, actions):
         """Episodes the device tables could not decide: full native placer + expansion, then patch the rows (and remember the

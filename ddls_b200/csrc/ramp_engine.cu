@@ -104,6 +104,7 @@ struct ramp_engine {
     double* d_step_stats = nullptr;
     int32_t* d_n_cluster_steps = nullptr;
     double* d_ep_export = nullptr;
+    double* d_es_export = nullptr;   // [B][RAMP_ES_LEN] ramp_get_episode_stats
     // episode state
     EpisodeState ep{};
     ramp_arrival_t* d_arrivals = nullptr;
@@ -155,6 +156,7 @@ struct ramp_engine {
     int32_t* env_h_need = nullptr;       // pinned: [0] = count, [1] = error flag; [2], [3]: the same, read by ramp_env_read; [4] engine error episode
     void* env_h_mirror = nullptr;        // pinned host arrays (ramp_env_host_mirror)
     bool env_unchecked_decide = false;   // a ramp_env_decide without need_host_out has not been looked at yet
+    bool env_agents_set = false;         // ramp_env_set_agents ran
     // standalone lookahead buffers
     WorkItem* sa_chunk_items = nullptr;
     ChunkDesc* sa_chunks = nullptr;
@@ -648,6 +650,7 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     CUDA_TRY(cudaMalloc(&e->d_step_stats, sizeof(double) * RAMP_STEP_STATS_LEN * B));
     CUDA_TRY(cudaMalloc(&e->d_n_cluster_steps, sizeof(int32_t) * B));
     CUDA_TRY(cudaMalloc(&e->d_ep_export, sizeof(double) * RAMP_EP_LEN * B));
+    CUDA_TRY(cudaMalloc(&e->d_es_export, sizeof(double) * RAMP_ES_LEN * B));
     CUDA_TRY(cudaMallocHost(&e->h_n_work, sizeof(int32_t) * 4));
 
     EpisodeState& ep = e->ep;
@@ -691,7 +694,7 @@ int ramp_engine_destroy(ramp_engine_t* e) {
     free_result_slots(e->res); free_result_slots(e->sa_res);
     cudaFree(e->pool.n_active); cudaFree(e->pool.tick); cudaFree(e->pool.top);
     cudaFree(e->d_items); cudaFree(e->d_items_big); cudaStreamDestroy(e->stream2); cudaEventDestroy(e->ev_fork); cudaEventDestroy(e->ev_join); cudaFree(e->d_counters); cudaFree(e->d_stats); cudaFree(e->d_actions);
-    cudaFree(e->d_step_stats); cudaFree(e->d_n_cluster_steps); cudaFree(e->d_ep_export);
+    cudaFree(e->d_step_stats); cudaFree(e->d_n_cluster_steps); cudaFree(e->d_ep_export); cudaFree(e->d_es_export);
     cudaFree(e->ep.ef); cudaFree(e->ep.ei); cudaFree(e->ep.rf); cudaFree(e->ep.ri); cudaFree(e->ep.rec);
     cudaFree(e->d_arrivals); cudaFree(e->d_n_jobs_ep); cudaFree(e->d_scratch); cudaFree(e->sa_items); cudaFree(e->sa_counters); cudaFreeHost(e->h_n_work);
     for (int k = 0; k < MAX_EVENT_PAIRS; ++k) { cudaEventDestroy(e->ev_a[k]); cudaEventDestroy(e->ev_b[k]); }
@@ -1268,6 +1271,10 @@ int ramp_env_create(ramp_engine_t* e, const ramp_env_config_t* c) {
     if ((rc = env_upload<int32_t>(e, &v.tid, nullptr, (size_t)B))) return rc;
     if ((rc = env_upload<int32_t>(e, &v.decided_job, nullptr, (size_t)B))) return rc;
     if ((rc = env_upload<int32_t>(e, &v.n_decided, nullptr, (size_t)B))) return rc;
+    if ((rc = env_upload<int32_t>(e, &v.job_tmpl, nullptr, (size_t)B * J))) return rc;
+    if ((rc = env_upload<double>(e, &v.ret, nullptr, (size_t)B))) return rc;
+    if ((rc = env_upload<int32_t>(e, &v.agent_kind, nullptr, (size_t)B))) return rc;
+    if ((rc = env_upload<int32_t>(e, &v.agent_param, nullptr, (size_t)B))) return rc;
     if ((rc = env_upload<int32_t>(e, &v.actions, nullptr, (size_t)B))) return rc;
     if ((rc = env_upload<double>(e, &v.reward, nullptr, (size_t)B))) return rc;
     if ((rc = env_upload<uint8_t>(e, &v.done, nullptr, (size_t)B))) return rc;
@@ -1305,6 +1312,8 @@ int ramp_env_reset(ramp_engine_t* e, const int32_t* model_of, const double* frac
     CUDA_TRY(cudaMemsetAsync(v.job_mask, 0, sizeof(unsigned long long) * n * v.n_words, e->stream));
     CUDA_TRY(cudaMemsetAsync(v.done, 0, (size_t)v.B, e->stream));
     CUDA_TRY(cudaMemsetAsync(v.n_decided, 0, sizeof(int32_t) * (size_t)v.B, e->stream));
+    CUDA_TRY(cudaMemsetAsync(v.job_tmpl, 0xFF, sizeof(int32_t) * n, e->stream));          // -1
+    CUDA_TRY(cudaMemsetAsync(v.ret, 0, sizeof(double) * (size_t)v.B, e->stream));
     CUDA_TRY(cudaMemsetAsync(v.err, 0, sizeof(int32_t), e->stream));
     int rc = ramp_reset(e, arrivals, v.J);
     if (rc != RAMP_OK) return rc;
@@ -1489,6 +1498,50 @@ int ramp_env_read_state(ramp_engine_t* e, uint64_t* busy_out, int32_t* actions_o
     if (actions_out) CUDA_TRY(cudaMemcpyAsync(actions_out, v.actions, sizeof(int32_t) * v.B, cudaMemcpyDeviceToHost, e->stream));
     if (n_decided_out) CUDA_TRY(cudaMemcpyAsync(n_decided_out, v.n_decided, sizeof(int32_t) * v.B, cudaMemcpyDeviceToHost, e->stream));
     return ramp_sync(e);
+}
+
+int ramp_env_read_episode(ramp_engine_t* e, int32_t* job_template_out, double* return_out) {
+    if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
+    const EnvDev& v = e->env;
+    if (job_template_out)
+        CUDA_TRY(cudaMemcpyAsync(job_template_out, v.job_tmpl, sizeof(int32_t) * (size_t)v.B * v.J, cudaMemcpyDeviceToHost, e->stream));
+    if (return_out) CUDA_TRY(cudaMemcpyAsync(return_out, v.ret, sizeof(double) * v.B, cudaMemcpyDeviceToHost, e->stream));
+    return ramp_sync(e);
+}
+
+int ramp_get_episode_stats(ramp_engine_t* e, double* out) {
+    if (!e || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    const int B = e->cfg.n_episodes;
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    ramp_episode_stats_kernel<<<(B + 127) / 128, 128, 0, e->stream>>>(e->ep, e->d_es_export);
+    e->launches++;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(out, e->d_es_export, sizeof(double) * RAMP_ES_LEN * B, cudaMemcpyDeviceToHost, e->stream));
+    return ramp_sync(e);
+}
+
+int ramp_env_set_agents(ramp_engine_t* e, const int32_t* kind, const int32_t* param) {
+    if (!e || !e->has_env || !kind) return set_error(RAMP_ERR_BAD_ARG, "no environment or no agent kinds");
+    EnvDev& v = e->env;
+    for (int b = 0; b < v.B; ++b)
+        if (kind[b] < 0 || kind[b] >= RAMP_AGENT_COUNT) return set_error(RAMP_ERR_BAD_ARG, "episode %d: unknown agent kind %d", b, kind[b]);
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    CUDA_TRY(cudaMemcpy(v.agent_kind, kind, sizeof(int32_t) * v.B, cudaMemcpyHostToDevice));
+    if (param) CUDA_TRY(cudaMemcpy(v.agent_param, param, sizeof(int32_t) * v.B, cudaMemcpyHostToDevice));
+    else CUDA_TRY(cudaMemset(v.agent_param, 0, sizeof(int32_t) * v.B));
+    e->env_agents_set = true;
+    return RAMP_OK;
+}
+
+int ramp_env_agent_act(ramp_engine_t* e, uint64_t seed) {
+    if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
+    if (!e->env_agents_set) return set_error(RAMP_ERR_BAD_ARG, "no agents: call ramp_env_set_agents first");
+    const EnvDev& v = e->env;
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    ramp_env_agent_kernel<<<(v.B + 127) / 128, 128, 0, e->stream>>>(v, e->ep, (unsigned long long)seed);
+    e->launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
 }
 
 }  // extern "C"

@@ -6,7 +6,10 @@
 //                           order) with no busy server; template by (model, degree, geometry); action row for the engine
 //   ramp_env_update_kernel  after the cluster step: reward (rewards/job_acceptance.py), servers of the accepted job, occupancy =
 //                           OR over the running jobs, and the next queued job's dynamic graph features + action mask
-//                           (observations/ramp_job_partitioning_observation.py:80-131, 358-498)
+//                           (observations/ramp_job_partitioning_observation.py:80-131, 358-498); the template id of the
+//                           accepted job and the episode's return (EvalLoop's episode_stats['return'], loops/eval_loop.py:26-134)
+//   ramp_env_agent_kernel   the reference's six heuristic agents (ddls/environments/ramp_job_partitioning/agents/*.py), one per
+//                           episode, writing `actions`
 #pragma once
 
 namespace ramp {
@@ -30,6 +33,10 @@ struct EnvDev {
     int32_t* tid;                   // [B]
     int32_t* decided_job;           // [B] job idx the decision was for
     int32_t* n_decided;             // [B] decisions taken since the reset (env-steps of the episode)
+    int32_t* job_tmpl;              // [B][J] template the job was mounted with when it was accepted (-1 otherwise)
+    double* ret;                    // [B] sum of the rewards since the reset
+    int32_t* agent_kind;            // [B] RAMP_AGENT_* (ramp_env_set_agents)
+    int32_t* agent_param;           // [B] SiPML's max_partitions_per_op (<= 0: None)
     // i/o
     int32_t* actions; double* reward; uint8_t* done; int32_t* queued_model; float* obs_dyn; uint8_t* action_mask;
     int32_t* need_host; int32_t* n_need_host;
@@ -130,7 +137,11 @@ __global__ void ramp_env_update_kernel(const EnvDev v, const EpisodeState ep, co
         } else {
             v.reward[b] = was_live ? v.fail_reward : 0.0;
         }
-        if (accepted) for (int w = 0; w < nw; ++w) v.job_mask[((size_t)b * J + q) * nw + w] = v.placed[(size_t)b * nw + w];
+        v.ret[b] = __dadd_rn(v.ret[b], v.reward[b]);
+        if (accepted) {
+            for (int w = 0; w < nw; ++w) v.job_mask[((size_t)b * J + q) * nw + w] = v.placed[(size_t)b * nw + w];
+            v.job_tmpl[(size_t)b * J + q] = v.tid[b];
+        }
     }
     // ---- occupancy: servers of the jobs that are running now (one job per worker, ramp_rules.py:6-39) ----
     int n_running = 0;
@@ -165,6 +176,72 @@ __global__ void ramp_env_update_kernel(const EnvDev v, const EpisodeState ep, co
     }
     o[9] = (float)((double)(v.n_workers - free_workers) / (double)v.n_workers);
     o[10] = (float)((double)n_running / (double)v.n_workers);
+}
+
+// The reference's heuristic agents (ddls/environments/ramp_job_partitioning/agents/*.py), restated line for line on the action
+// mask ramp_env_update_kernel left: valid_actions = action_set[action_mask] in ascending order.  With one valid action
+// MinParallelism and NoParallelism return 0, the others valid_actions[0].  Otherwise:
+//   Random          np.random.choice(valid_actions[1:]) (random.py:8-16): uniform over the valid actions after the first,
+//                   drawn from splitmix64 keyed by (seed, episode, decisions taken so far) -- the policy's construction
+//                   (ramp_policy.cu); it does not reproduce numpy's stream
+//   SiPML           min(param, valid_actions[-1]), param <= 0 = None: valid_actions[-1] (sip_ml.py:13-25); not re-checked
+//                   against the mask
+//   AcceptableJCT   target = ceil(seq / max_acceptable_jct) in f64; the first valid action >= target, 0 included, else
+//                   valid_actions[-1] (acceptable_jct.py:21-44)
+//   MaxParallelism  valid_actions[1:][-1] (max_parallelism.py:5-13)
+//   MinParallelism  2 when more than two actions are valid, even if 2 is masked; 1 when two are (min_parallelism.py:5-17)
+//   NoParallelism   1 (no_parallelism.py:5-13)
+// Finished episodes get 0.
+__global__ void ramp_env_agent_kernel(const EnvDev v, const EpisodeState ep, unsigned long long seed) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= v.B) return;
+    if (v.done[b]) { v.actions[b] = 0; return; }
+    const uint8_t* am = v.action_mask + (size_t)b * (v.max_degree + 1);
+    int n_valid = 0, first = 0, last = 0;
+    for (int a = 0; a <= v.max_degree; ++a) {
+        if (am[a]) { if (n_valid == 0) first = a; last = a; ++n_valid; }
+    }
+    const int kind = v.agent_kind[b];
+    int action = first;
+    if (kind == RAMP_AGENT_MIN_PARALLELISM) {
+        action = n_valid > 2 ? 2 : n_valid == 2 ? 1 : 0;
+    } else if (kind == RAMP_AGENT_NO_PARALLELISM) {
+        action = n_valid > 1 ? 1 : 0;
+    } else if (n_valid > 1) {
+        switch (kind) {
+            case RAMP_AGENT_RANDOM: {
+                const unsigned long long key = seed ^ (0x9E3779B97F4A7C15ull * (unsigned long long)v.n_decided[b]);
+                const unsigned long long r = splitmix64(key ^ ((unsigned long long)b * 0xD1342543DE82EF95ull));
+                const int k = (int)(((r >> 32) * (unsigned long long)(n_valid - 1)) >> 32);   // valid_actions[1 + k]
+                int seen = -1;
+                for (int a = 0; a <= v.max_degree; ++a) {
+                    if (am[a] && seen++ == k) { action = a; break; }
+                }
+                break;
+            }
+            case RAMP_AGENT_SIPML: {
+                const int p = v.agent_param[b];
+                action = (p > 0 && p < last) ? p : last;
+                break;
+            }
+            case RAMP_AGENT_ACCEPTABLE_JCT: {
+                const int q = ep.ei[EI_QUEUED * v.B + b];
+                const int m = v.queued_model[b];
+                const double seq = v.model_params[(size_t)m * 5];
+                const double ov = v.macc[(size_t)b * v.J + q];
+                const double macc = isnan(ov) ? __dmul_rn(v.frac[(size_t)b * v.J + q], seq) : ov;
+                const double target = ceil(__ddiv_rn(seq, macc));
+                action = last;
+                for (int a = 0; a <= v.max_degree; ++a) {
+                    if (am[a] && (double)a >= target) { action = a; break; }
+                }
+                break;
+            }
+            case RAMP_AGENT_MAX_PARALLELISM: action = last; break;
+            default: action = 0; break;
+        }
+    }
+    v.actions[b] = action;
 }
 
 }  // namespace ramp

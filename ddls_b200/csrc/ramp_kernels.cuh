@@ -105,7 +105,12 @@ enum { RF_JCT = 0, RF_STARTED, RF_COMM, RF_COMP, RF_UTIL, RF_PART_OP_MEM, RF_PAR
 enum { RI_JOB_IDX = 0, RI_N_WORKERS, RI_N_CHANNELS, RI_COUNT };
 
 // per-episode scalars (SoA: [field][episode])
-enum { EF_NOW = 0, EF_NEXT_ARRIVAL, EF_LAST_ARRIVAL, EF_LOAD_SUM, EF_COUNT };
+// EF_ACC_*: the episode_stats accumulators (RCE:1086-1106), every cluster step's values summed in cluster-step order --
+// the seven *_info_processed in RAMP_SS_COMPUTE_INFO_PROCESSED order, the four step means RCE:1099-1102, the sums and length
+// of the per-tick utilisation lists (RCE:1103-1104) and the number of cluster steps; ramp_episode_stats_kernel finalises them
+enum { EF_NOW = 0, EF_NEXT_ARRIVAL, EF_LAST_ARRIVAL, EF_LOAD_SUM,
+       EF_ACC_INFO, EF_ACC_COMP_FRAC = EF_ACC_INFO + 7, EF_ACC_COMM_FRAC, EF_ACC_JOBS_RUNNING, EF_ACC_MOUNTED_WORKERS,
+       EF_ACC_UTIL_MOUNTED, EF_ACC_UTIL_CLUSTER, EF_ACC_TICKS, EF_ACC_STEPS, EF_COUNT };
 enum { EI_NUM_ARRIVED = 0, EI_NUM_COMPLETED, EI_NUM_BLOCKED, EI_QUEUED, EI_N_RUNNING, EI_STEP_COUNTER, EI_EVENT_SEQ,
        EI_LOAD_N, EI_STATUS, EI_DONE, EI_LAST_SLOT, EI_PLAN_SLOT, EI_PLAN_RAN, EI_COUNT };
 
@@ -1083,6 +1088,22 @@ __global__ void ramp_step_kernel(const StepArgs s) {
             st[RAMP_SS_NUM_TICKS] = (double)n_iter;
             if (ep.tick_util) ep.tick_util_n[b] = n_iter;
             st[RAMP_SS_JOB_QUEUE_LENGTH] = EI(EI_QUEUED) >= 0 ? 1.0 : 0.0;                       // RCE:1082
+            // RCE:1086-1106: this cluster step's contribution to episode_stats.  The addresses come from the kernel parameter, not
+            // from EF()'s `ef`: the kernel sits at 254 registers, and through `ef` ptxas spilled 8 bytes
+            {
+                double* acc = s.ep.ef + b;
+                const size_t Bs = (size_t)s.ep.B;
+#pragma unroll
+                for (int k = 0; k < 7; ++k) acc[(EF_ACC_INFO + k) * Bs] = __dadd_rn(acc[(EF_ACC_INFO + k) * Bs], st[RAMP_SS_COMPUTE_INFO_PROCESSED + k]);
+                acc[EF_ACC_COMP_FRAC * Bs] = __dadd_rn(acc[EF_ACC_COMP_FRAC * Bs], st[RAMP_SS_MEAN_COMPUTE_OVERHEAD_FRAC]);
+                acc[EF_ACC_COMM_FRAC * Bs] = __dadd_rn(acc[EF_ACC_COMM_FRAC * Bs], st[RAMP_SS_MEAN_COMMUNICATION_OVERHEAD_FRAC]);
+                acc[EF_ACC_JOBS_RUNNING * Bs] = __dadd_rn(acc[EF_ACC_JOBS_RUNNING * Bs], st[RAMP_SS_MEAN_NUM_JOBS_RUNNING]);
+                acc[EF_ACC_MOUNTED_WORKERS * Bs] = __dadd_rn(acc[EF_ACC_MOUNTED_WORKERS * Bs], st[RAMP_SS_MEAN_NUM_MOUNTED_WORKERS]);
+                acc[EF_ACC_UTIL_MOUNTED * Bs] = __dadd_rn(acc[EF_ACC_UTIL_MOUNTED * Bs], st[RAMP_SS_UTIL_MOUNTED_SUM]);
+                acc[EF_ACC_UTIL_CLUSTER * Bs] = __dadd_rn(acc[EF_ACC_UTIL_CLUSTER * Bs], st[RAMP_SS_UTIL_CLUSTER_SUM]);
+                acc[EF_ACC_TICKS * Bs] = __dadd_rn(acc[EF_ACC_TICKS * Bs], st[RAMP_SS_NUM_TICKS]);
+                acc[EF_ACC_STEPS * Bs] = __dadd_rn(acc[EF_ACC_STEPS * Bs], 1.0);
+            }
             EI(EI_STEP_COUNTER)++;                                                                // RCE:1109
             const bool done = step_is_done(ep, b);
             if (done) {                                                                           // RCE:1111-1121
@@ -1147,6 +1168,40 @@ __global__ void ramp_export_episode_state_kernel(const EpisodeState ep, double* 
     o[RAMP_EP_NUM_RUNNING] = EI(EI_N_RUNNING); o[RAMP_EP_STEP_COUNTER] = EI(EI_STEP_COUNTER);
     o[RAMP_EP_LOAD_RATE_SUM] = EF(EF_LOAD_SUM); o[RAMP_EP_LOAD_RATE_N] = EI(EI_LOAD_N);
     o[RAMP_EP_DONE] = EI(EI_DONE); o[RAMP_EP_STATUS] = EI(EI_STATUS);
+}
+
+// the episode-end finalisation RCE:1123-1167 applied to the EF_ACC_* accumulators: [B][RAMP_ES_LEN].  An episode that is not
+// done gets the same formulas over the episode so far.
+__global__ void ramp_episode_stats_kernel(const EpisodeState ep, double* out) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    const int B = ep.B;
+    if (b >= B) return;
+    const double* ef = ep.ef; const int32_t* ei = ep.ei;
+    double* o = out + (size_t)b * RAMP_ES_LEN;
+    const double t = EF(EF_NOW);                                                  // RCE:1125-1127 (episode_start_time = 0)
+    o[RAMP_ES_EPISODE_START_TIME] = 0.0; o[RAMP_ES_EPISODE_END_TIME] = t; o[RAMP_ES_EPISODE_TIME] = t;
+    const int n_arr = EI(EI_NUM_ARRIVED), n_comp = EI(EI_NUM_COMPLETED), n_blk = EI(EI_NUM_BLOCKED);
+    o[RAMP_ES_NUM_JOBS_ARRIVED] = n_arr; o[RAMP_ES_NUM_JOBS_COMPLETED] = n_comp; o[RAMP_ES_NUM_JOBS_BLOCKED] = n_blk;
+    o[RAMP_ES_MEAN_LOAD_RATE] = EI(EI_LOAD_N) > 0 ? __ddiv_rn(EF(EF_LOAD_SUM), (double)EI(EI_LOAD_N)) : 0.0;   // RCE:1129
+    o[RAMP_ES_BLOCKING_RATE] = n_arr > 0 ? __ddiv_rn((double)n_blk, (double)n_arr) : 0.0;                       // RCE:1131-1134
+    o[RAMP_ES_ACCEPTANCE_RATE] = n_arr > 0 ? __ddiv_rn((double)n_comp, (double)n_arr) : 0.0;                    // RCE:1135-1138
+    for (int k = 0; k < 7; ++k) {                                                                                // RCE:1140-1154
+        const double info = EF(EF_ACC_INFO + k);
+        o[RAMP_ES_COMPUTE_INFO_PROCESSED + k] = info;
+        o[RAMP_ES_MEAN_COMPUTE_THROUGHPUT + k] = (info != 0.0 && t != 0.0) ? __ddiv_rn(info, t) : 0.0;
+    }
+    const double n_steps = EF(EF_ACC_STEPS), n_ticks = EF(EF_ACC_TICKS);                                        // RCE:1156-1167
+    const bool live = t != 0.0;
+#define RAMP_MEAN(sum, n) ((live && (n) > 0.0) ? __ddiv_rn((sum), (n)) : 0.0)
+    o[RAMP_ES_MEAN_COMPUTE_OVERHEAD_FRAC] = RAMP_MEAN(EF(EF_ACC_COMP_FRAC), n_steps);
+    o[RAMP_ES_MEAN_COMMUNICATION_OVERHEAD_FRAC] = RAMP_MEAN(EF(EF_ACC_COMM_FRAC), n_steps);
+    o[RAMP_ES_MEAN_NUM_JOBS_RUNNING] = RAMP_MEAN(EF(EF_ACC_JOBS_RUNNING), n_steps);
+    o[RAMP_ES_MEAN_NUM_MOUNTED_WORKERS] = RAMP_MEAN(EF(EF_ACC_MOUNTED_WORKERS), n_steps);
+    o[RAMP_ES_MEAN_MOUNTED_WORKER_UTILISATION_FRAC] = RAMP_MEAN(EF(EF_ACC_UTIL_MOUNTED), n_ticks);
+    o[RAMP_ES_MEAN_CLUSTER_WORKER_UTILISATION_FRAC] = RAMP_MEAN(EF(EF_ACC_UTIL_CLUSTER), n_ticks);
+#undef RAMP_MEAN
+    o[RAMP_ES_NUM_CLUSTER_STEPS] = n_steps; o[RAMP_ES_NUM_TICKS] = n_ticks;
+    o[RAMP_ES_DONE] = EI(EI_DONE);
 }
 
 #undef EF

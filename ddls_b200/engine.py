@@ -36,6 +36,20 @@ EP_FIELDS = ['time', 'next_arrival', 'num_arrived', 'num_completed', 'num_blocke
 EP = {k: i for i, k in enumerate(EP_FIELDS)}
 EP_LEN = len(EP_FIELDS)
 
+# RampClusterEnvironment.episode_stats' scalars (RCE:1123-1167), include/ramp_b200.h RAMP_ES_*: the reference's names, plus the
+# number of cluster steps and ticks the means run over and the done flag
+ES_FIELDS = ['episode_start_time', 'episode_end_time', 'episode_time', 'num_jobs_arrived', 'num_jobs_completed', 'num_jobs_blocked',
+             'mean_load_rate', 'blocking_rate', 'acceptance_rate',
+             'compute_info_processed', 'dep_info_processed', 'flow_info_processed', 'cluster_info_processed',
+             'demand_compute_info_processed', 'demand_dep_info_processed', 'demand_total_info_processed',
+             'mean_compute_throughput', 'mean_dep_throughput', 'mean_flow_throughput', 'mean_cluster_throughput',
+             'mean_demand_compute_throughput', 'mean_demand_dep_throughput', 'mean_demand_total_throughput',
+             'mean_compute_overhead_frac', 'mean_communication_overhead_frac', 'mean_num_jobs_running', 'mean_num_mounted_workers',
+             'mean_mounted_worker_utilisation_frac', 'mean_cluster_worker_utilisation_frac', 'num_cluster_steps', 'num_ticks', 'done']
+ES = {k: i for i, k in enumerate(ES_FIELDS)}
+ES_LEN = len(ES_FIELDS)
+ES_COUNTS = ('num_jobs_arrived', 'num_jobs_completed', 'num_jobs_blocked', 'num_cluster_steps', 'num_ticks')
+
 JS_NOT_ARRIVED, JS_QUEUED, JS_RUNNING, JS_COMPLETED, JS_BLOCKED = range(5)
 
 ACTION_DTYPE = np.dtype([('max_acceptable_jct', np.float64), ('part_op_mem', np.float64), ('part_dep_size', np.float64),
@@ -99,6 +113,7 @@ def load_library():
     L.ramp_get_episode_state.argtypes = [C.c_void_p, C.c_void_p]
     L.ramp_episode_state_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
     L.ramp_export_episode_state_to.argtypes = [C.c_void_p, C.c_void_p]
+    L.ramp_get_episode_stats.argtypes = [C.c_void_p, C.c_void_p]
     L.ramp_get_memo_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.ramp_get_memo_stats_ex.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     L.ramp_get_last_lookahead.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
@@ -112,7 +127,7 @@ def load_library():
     for name in ('ramp_engine_create', 'ramp_engine_destroy', 'ramp_register_template', 'ramp_template_count',
                  'ramp_reset', 'ramp_set_arrivals', 'ramp_step_host', 'ramp_step_device', 'ramp_sync', 'ramp_check_status',
                  'ramp_get_job_records', 'ramp_get_episode_state', 'ramp_episode_state_device', 'ramp_export_episode_state_to',
-                 'ramp_get_memo_stats', 'ramp_get_memo_stats_ex', 'ramp_get_last_lookahead', 'ramp_run_lookaheads',
+                 'ramp_get_episode_stats', 'ramp_get_memo_stats', 'ramp_get_memo_stats_ex', 'ramp_get_last_lookahead', 'ramp_run_lookaheads',
                  'ramp_debug_template_info', 'ramp_get_lookahead_kernel_time'):
         getattr(L, name).restype = C.c_int
     _lib = L
@@ -122,7 +137,7 @@ def load_library():
 EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destroy', 'ramp_engine_stream',
                     'ramp_register_template', 'ramp_template_count', 'ramp_reset', 'ramp_set_arrivals', 'ramp_step_host',
                     'ramp_step_device', 'ramp_sync', 'ramp_check_status', 'ramp_get_job_records',
-                    'ramp_get_episode_state', 'ramp_episode_state_device', 'ramp_export_episode_state_to',
+                    'ramp_get_episode_state', 'ramp_episode_state_device', 'ramp_export_episode_state_to', 'ramp_get_episode_stats',
                     'ramp_get_memo_stats', 'ramp_get_memo_stats_ex',
                     'ramp_get_last_lookahead', 'ramp_run_lookaheads', 'ramp_debug_template_info', 'ramp_launch_count',
                     'ramp_get_lookahead_kernel_time', 'ramp_expand_template', 'ramp_free_expanded_job', 'ramp_free_expanded_aux', 'ramp_first_fit_place',
@@ -131,7 +146,8 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_env_reset', 'ramp_env_buffers', 'ramp_env_host_mirror', 'ramp_env_decide', 'ramp_env_patch', 'ramp_env_advance', 'ramp_env_read', 'ramp_get_last_step_stats', 'ramp_env_read_state',
                     'ramp_enable_tick_lists', 'ramp_get_tick_lists', 'ramp_policy_weight_count', 'ramp_policy_create', 'ramp_policy_destroy', 'ramp_policy_set_weights', 'ramp_policy_set_model',
                     'ramp_policy_embed', 'ramp_policy_forward', 'ramp_policy_decide', 'ramp_policy_act', 'ramp_policy_read',
-                    'ramp_pinned_alloc', 'ramp_pinned_free', 'ramp_policy_trajectory_begin', 'ramp_policy_trajectory_record', 'ramp_policy_trajectory_read']
+                    'ramp_pinned_alloc', 'ramp_pinned_free', 'ramp_policy_trajectory_begin', 'ramp_policy_trajectory_record', 'ramp_policy_trajectory_read',
+                    'ramp_env_read_episode', 'ramp_env_set_agents', 'ramp_env_agent_act']
 
 
 def _check(rc):
@@ -262,6 +278,13 @@ class RampEngine:
     def episode_state(self):
         out = np.empty((self.n_episodes, EP_LEN), dtype=np.float64)
         _check(self._L.ramp_get_episode_state(self._h, out.ctypes.data))
+        return out
+
+    def episode_stats(self):
+        """[n_episodes, ES_LEN] f64: RampClusterEnvironment.episode_stats' scalars (RCE:1123-1167) from every cluster step since the
+        reset; rows of episodes that are not done hold the same formulas over the episode so far (include/ramp_b200.h)."""
+        out = np.empty((self.n_episodes, ES_LEN), dtype=np.float64)
+        _check(self._L.ramp_get_episode_stats(self._h, out.ctypes.data))
         return out
 
     def episode_state_device_ptr(self):

@@ -208,6 +208,29 @@ int ramp_episode_state_device(ramp_engine_t* eng, double** d_out);
 /* writes the table into a caller-owned DEVICE buffer [n_episodes][RAMP_EP_LEN] (asynchronous on the engine stream),
  * e.g. a torch tensor that is then all-gathered over NCCL */
 int ramp_export_episode_state_to(ramp_engine_t* eng, double* d_dst);
+/* RampClusterEnvironment.episode_stats' scalars (RCE:1086-1106 appends, RCE:1123-1167 finalises): double[n_episodes][RAMP_ES_LEN].
+ * The step kernel adds every cluster step's values to per-episode accumulators (including the empty steps RJPE:394-395 fuses),
+ * in cluster-step order; this applies the finalisation to them:
+ *   blocking / acceptance rate      0 when no job arrived
+ *   *_throughput                    *_info_processed / episode_time unless either is 0 (then 0)
+ *   the four step means             sum of the per-cluster-step means / number of cluster steps; 0 when episode_time == 0
+ *   the two utilisation means       the mean over every per-tick entry of the episode (sum of the per-step list sums / the
+ *                                   number of ticks), 0 when episode_time == 0.  The reference's np.mean over its list of
+ *                                   per-step lists is not defined when the lists are ragged; this is the definition of the
+ *                                   drop-in class (ddls_b200/host/cluster.py), which flattens them.
+ * Rows of episodes that are not done (RAMP_ES_DONE = 0) hold the same formulas over the episode so far.  Waits for the engine
+ * stream. */
+enum { RAMP_ES_EPISODE_START_TIME = 0, RAMP_ES_EPISODE_END_TIME, RAMP_ES_EPISODE_TIME,
+       RAMP_ES_NUM_JOBS_ARRIVED, RAMP_ES_NUM_JOBS_COMPLETED, RAMP_ES_NUM_JOBS_BLOCKED,
+       RAMP_ES_MEAN_LOAD_RATE, RAMP_ES_BLOCKING_RATE, RAMP_ES_ACCEPTANCE_RATE,
+       RAMP_ES_COMPUTE_INFO_PROCESSED, RAMP_ES_DEP_INFO_PROCESSED, RAMP_ES_FLOW_INFO_PROCESSED, RAMP_ES_CLUSTER_INFO_PROCESSED,
+       RAMP_ES_DEMAND_COMPUTE_INFO_PROCESSED, RAMP_ES_DEMAND_DEP_INFO_PROCESSED, RAMP_ES_DEMAND_TOTAL_INFO_PROCESSED,
+       RAMP_ES_MEAN_COMPUTE_THROUGHPUT, RAMP_ES_MEAN_DEP_THROUGHPUT, RAMP_ES_MEAN_FLOW_THROUGHPUT, RAMP_ES_MEAN_CLUSTER_THROUGHPUT,
+       RAMP_ES_MEAN_DEMAND_COMPUTE_THROUGHPUT, RAMP_ES_MEAN_DEMAND_DEP_THROUGHPUT, RAMP_ES_MEAN_DEMAND_TOTAL_THROUGHPUT,
+       RAMP_ES_MEAN_COMPUTE_OVERHEAD_FRAC, RAMP_ES_MEAN_COMMUNICATION_OVERHEAD_FRAC, RAMP_ES_MEAN_NUM_JOBS_RUNNING,
+       RAMP_ES_MEAN_NUM_MOUNTED_WORKERS, RAMP_ES_MEAN_MOUNTED_WORKER_UTILISATION_FRAC, RAMP_ES_MEAN_CLUSTER_WORKER_UTILISATION_FRAC,
+       RAMP_ES_NUM_CLUSTER_STEPS, RAMP_ES_NUM_TICKS, RAMP_ES_DONE, RAMP_ES_LEN };
+int ramp_get_episode_stats(ramp_engine_t* eng, double* out /* HOST [n_episodes][RAMP_ES_LEN] */);
 /* memo statistics since the last reset: lookups, hits, lookaheads executed */
 int ramp_get_memo_stats(ramp_engine_t* eng, int64_t* lookups, int64_t* hits, int64_t* lookaheads);
 /* {lookups, per-episode hits, batch-wide (shared) hits, lookaheads executed} since the last reset */
@@ -399,6 +422,22 @@ int ramp_get_last_step_stats(ramp_engine_t* eng, double* stats_out, int32_t* n_c
 /* HOST copies of the occupancy [n_episodes][n_words], of the actions the device holds, and of the number of decisions every episode
  * has taken since ramp_env_reset (= its env-steps; a finished episode takes none) -- any may be NULL */
 int ramp_env_read_state(ramp_engine_t* eng, uint64_t* busy_out, int32_t* actions_out, int32_t* n_decided_out);
+/* What the per-job lists of episode_stats need beyond the job records, as HOST copies (either may be NULL): the template every
+ * accepted job was mounted with ([n_episodes][jobs_per_episode], -1 for the others) and every episode's return, the sum of its
+ * rewards since ramp_env_reset (EvalLoop's episode_stats['return'], loops/eval_loop.py:26-134). */
+int ramp_env_read_episode(ramp_engine_t* eng, int32_t* job_template_out, double* return_out);
+
+/* The reference's heuristic agents (ddls/environments/ramp_job_partitioning/agents/*.py) on the device.  ramp_env_set_agents
+ * uploads one agent per episode (kind: HOST [n_episodes] RAMP_AGENT_*; param: HOST [n_episodes], SiPML's max_partitions_per_op,
+ * <= 0 = None, ignored by the others, may be NULL), so that one batch can run different agents side by side.
+ * ramp_env_agent_act writes ramp_env_buffers_t.actions from the current action mask, queued model, max acceptable JCT and
+ * model_params, one thread per episode on the engine stream, with no host transfer; finished episodes get 0.  Random draws
+ * from splitmix64 keyed by (seed, episode, decisions the episode has taken), not numpy's stream.  See ramp_env.cuh for each
+ * agent's rule. */
+enum { RAMP_AGENT_RANDOM = 0, RAMP_AGENT_SIPML, RAMP_AGENT_ACCEPTABLE_JCT, RAMP_AGENT_MAX_PARALLELISM, RAMP_AGENT_MIN_PARALLELISM,
+       RAMP_AGENT_NO_PARALLELISM, RAMP_AGENT_COUNT };
+int ramp_env_set_agents(ramp_engine_t* eng, const int32_t* kind, const int32_t* param);
+int ramp_env_agent_act(ramp_engine_t* eng, uint64_t seed);
 /* also raises what ramp_check_status would (RAMP_ERR_SIM) -- one synchronisation per step for a host-side policy */
 int ramp_env_read(ramp_engine_t* eng, double* reward, uint8_t* done, int32_t* queued_model, float* obs_dynamic, uint8_t* action_mask);
 
