@@ -9,8 +9,11 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
+#include <mutex>
 #include <numeric>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "ramp_kernels.cuh"
@@ -189,6 +192,24 @@ int alloc_result_slots(ResultSlots& r, int32_t n) {
     return RAMP_OK;
 }
 
+// A kernel's dynamic shared memory limit (cudaFuncAttributeMaxDynamicSharedMemorySize) belongs to the kernel in the device's
+// context, not to an engine: every engine of the process shares it.  Lowering it to what one engine needs would make another
+// engine's launches that need more fail, so it only ever rises.  Each engine still launches with, and sizes its grid for, its own
+// dynamic shared memory.
+cudaError_t reserve_dynamic_smem(const void* kern, size_t bytes) {
+    static std::mutex mu;
+    static std::map<std::pair<int, const void*>, size_t> reserved;
+    int dev = 0;
+    cudaError_t err = cudaGetDevice(&dev);
+    if (err != cudaSuccess) return err;
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& cur = reserved[{dev, kern}];
+    if (bytes <= cur) return cudaSuccess;
+    err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (err == cudaSuccess) cur = bytes;
+    return err;
+}
+
 void free_result_slots(ResultSlots& r) {
     cudaFree(r.jct); cudaFree(r.comm); cudaFree(r.comp); cudaFree(r.n_ticks); cudaFree(r.status); cudaFree(r.trace_off);
     cudaFree(r.util); cudaFree(r.util_nmw);
@@ -215,7 +236,7 @@ int ensure_scratch(ramp_engine* e) {
         return set_error(RAMP_ERR_CAPACITY, "a template needs %zu B of shared memory for its worker/channel key arrays (max 200 KiB)", smem);
     if (smem != e->smem_bytes || e->grid == 0) {
         LookaheadKernel kern = warp_kernel();
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(reserve_dynamic_smem((const void*)kern, smem));
         // all lookahead kernels ask for the same L1/shared split: kernels with different carve-outs cannot share an SM,
         // which would serialise the CTA kernel and the warp kernel when they are launched side by side
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
@@ -227,12 +248,12 @@ int ensure_scratch(ramp_engine* e) {
         // the block scheduler spreads the 1-warp CTAs used beside a CTA kernel and the CTA kernel's over all SMs
         const size_t smem2 = lookahead_smem_per_warp(e->max_w, e->max_c, e->par_cap) * (size_t)(SPLIT_WARP_NT / 32);
         LookaheadKernel kern2 = split_warp_kernel();
-        CUDA_TRY(cudaFuncSetAttribute(kern2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+        CUDA_TRY(reserve_dynamic_smem((const void*)kern2, smem2));
         CUDA_TRY(cudaFuncSetAttribute(kern2, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
         e->smem2_bytes = smem2;
         const size_t smem_d = lookahead_smem_per_warp(e->max_w, e->max_c, e->par_cap, DENSE_F_CAP, DENSE_OPS_CAP) * (size_t)(DENSE_NT / 32);
         LookaheadKernel kern_d = lookahead_dense_kernel();
-        CUDA_TRY(cudaFuncSetAttribute(kern_d, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_d));
+        CUDA_TRY(reserve_dynamic_smem((const void*)kern_d, smem_d));
         CUDA_TRY(cudaFuncSetAttribute(kern_d, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
         int occ_d = 0;
         CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_d, kern_d, DENSE_NT, smem_d));
@@ -245,7 +266,7 @@ int ensure_scratch(ramp_engine* e) {
     if (cta_smem != e->cta_smem_bytes || e->cta_grid == 0) {
         for (int nt : {256, 128, 64}) {
             LookaheadKernel kern = lookahead_cta_kernel_for(nt);
-            CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cta_smem));
+            CUDA_TRY(reserve_dynamic_smem((const void*)kern, cta_smem));
             CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
             int occ = 0;
             CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, nt, cta_smem));
@@ -415,7 +436,7 @@ int ensure_thread_scratch(ramp_engine* e) {
     const size_t smem = thread_smem_bytes(e->res_tmpl_cap, e->res_n_cap);
     if (smem > 220 * 1024) return set_error(RAMP_ERR_CAPACITY, "resident templates need %zu B of shared memory (max 220 KiB)", smem);
     if (smem != e->res_smem || e->res_grid == 0) {
-        CUDA_TRY(cudaFuncSetAttribute(ramp_lookahead_thread_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(reserve_dynamic_smem((const void*)ramp_lookahead_thread_kernel, smem));
         CUDA_TRY(cudaFuncSetAttribute(ramp_lookahead_thread_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
         int occ = 0;
         CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ramp_lookahead_thread_kernel, RAMP_THREAD_CTA, smem));

@@ -27,6 +27,12 @@ STEP_STATS_LEN = len(STEP_STATS)
 JS_NOT_ARRIVED, JS_QUEUED, JS_RUNNING, JS_COMPLETED, JS_BLOCKED = range(5)
 ORC_OK, ORC_ERR_INFINITE_TICK, ORC_ERR_TRACE_OVERFLOW = 0, 1, 2
 
+# the episode-state row (ramp_oracle.h ORC_EP_*, the product's RAMP_EP_* layout)
+EP_FIELDS = ['time', 'next_arrival', 'num_arrived', 'num_completed', 'num_blocked', 'queued_job', 'num_running',
+             'step_counter', 'load_rate_sum', 'load_rate_n', 'done', 'status']
+EP = {k: i for i, k in enumerate(EP_FIELDS)}
+EP_LEN = len(EP_FIELDS)
+
 
 class CLoweredJob(C.Structure):
     _fields_ = [('n_ops', C.c_int32), ('n_deps', C.c_int32), ('n_workers', C.c_int32), ('n_channels', C.c_int32),
@@ -121,6 +127,12 @@ def lib():
                                              C.c_void_p, C.c_void_p, C.c_int32]
         L.orc_run_scripted_rjpe_batch.restype = C.c_int
         L.orc_run_scripted_rjpe_batch.argtypes = L.orc_run_scripted_batch.argtypes
+        L.orc_run_scripted_rjpe_full_batch.restype = C.c_int
+        L.orc_run_scripted_rjpe_full_batch.argtypes = ([C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                                         C.c_void_p, C.c_int32, C.c_double, C.c_int32, C.c_int32, C.c_int32]
+                                                        + [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 3 + [C.c_int32])
+        L.orc_env_episode_state.restype = None
+        L.orc_env_episode_state.argtypes = [C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -153,6 +165,39 @@ def run_lookahead(job, trace_cap=None):
     T = min(res.n_ticks, cap)
     return dict(jct=res.jct, comm=res.comm, comp=res.comp, n_ticks=res.n_ticks, status=res.status,
                 trace_n_active=tn[:T].copy(), trace_tick=tt[:T].copy())
+
+
+def run_scripted_episodes(templates, script_tid, script_mount, arrivals, n_cluster_workers, memo_models,
+                          max_sim_time=float('inf'), memo_degrees=1025, cs_cap=None, n_threads=None):
+    """RampJobPartitioningEnvironment.step per scripted decision for B independent episodes (orc_run_scripted_rjpe_full_batch).
+
+    script_tid [B, L] indexes `templates` (-1 = action 0); script_mount [B, L] MOUNT_DTYPE; arrivals [B, J] ARRIVAL_DTYPE.
+    A done episode is not stepped again.  Returns a dict of numpy arrays:
+      stats [B, L, STEP_STATS_LEN]   each env-step's action-step row, done taken after the whole env-step
+      n_cluster_steps [B, L]         cluster steps per env-step (0 once done)
+      cluster_stats [B, cs_cap, STEP_STATS_LEN], n_cluster_stats [B]   every cluster step's row, in order
+      records [B, J] JOB_RECORD_DTYPE, episode_state [B, EP_LEN]
+    """
+    B, L = script_tid.shape
+    arr = np.ascontiguousarray(arrivals, dtype=ARRIVAL_DTYPE)
+    assert arr.ndim == 2 and arr.shape[0] == B
+    J = arr.shape[1]
+    tid = np.ascontiguousarray(script_tid, dtype=np.int32)
+    mount = np.ascontiguousarray(script_mount, dtype=MOUNT_DTYPE)
+    assert mount.shape == (B, L)
+    cap = int(cs_cap or 4 * L + 4)
+    out = dict(stats=np.zeros((B, L, STEP_STATS_LEN)), n_cluster_steps=np.zeros((B, L), np.int32),
+               cluster_stats=np.zeros((B, cap, STEP_STATS_LEN)), n_cluster_stats=np.zeros(B, np.int32),
+               records=np.zeros((B, J), JOB_RECORD_DTYPE), episode_state=np.zeros((B, EP_LEN)))
+    ctemps = (CLoweredJob * max(len(templates), 1))(*[to_c(t) for t in templates])
+    rc = lib().orc_run_scripted_rjpe_full_batch(
+        ctemps, len(templates), B, L, tid.ctypes.data, mount.ctypes.data, arr.ctypes.data, J, float(max_sim_time),
+        n_cluster_workers, memo_models, memo_degrees, out['stats'].ctypes.data, out['n_cluster_steps'].ctypes.data,
+        out['cluster_stats'].ctypes.data, cap, out['n_cluster_stats'].ctypes.data, out['records'].ctypes.data,
+        out['episode_state'].ctypes.data, int(n_threads or os.cpu_count() or 1))
+    if rc != ORC_OK:
+        raise Exception(f'orc_run_scripted_rjpe_full_batch failed with status {rc}')
+    return out
 
 
 def utilisation(trace_n_active, trace_tick, n_mounted_workers, jct):
@@ -220,6 +265,12 @@ class OracleEnv:
     @property
     def mean_load_rate(self):
         return lib().orc_env_mean_load_rate(self._h)
+
+    def episode_state(self):
+        """[EP_LEN] f64: the episode scalars in the product's episode-state layout (EP_FIELDS)."""
+        out = np.zeros(EP_LEN)
+        lib().orc_env_episode_state(self._h, out.ctypes.data)
+        return out
 
     def job_records(self):
         ptr = lib().orc_env_job_records(self._h)

@@ -521,6 +521,14 @@ int32_t orc_env_tick_lists(const orc_env_t* env, double* mounted_out, double* cl
 }
 double orc_env_mean_load_rate(const orc_env_t* env) { return env->load_rate_n > 0 ? env->load_rate_sum / (double)env->load_rate_n : 0.0; }
 const orc_job_record_t* orc_env_job_records(const orc_env_t* env) { return env->records; }
+void orc_env_episode_state(const orc_env_t* env, double* out) {
+    out[ORC_EP_TIME] = env->now; out[ORC_EP_NEXT_ARRIVAL] = env->next_arrival;
+    out[ORC_EP_NUM_ARRIVED] = env->num_arrived; out[ORC_EP_NUM_COMPLETED] = env->num_completed;
+    out[ORC_EP_NUM_BLOCKED] = env->num_blocked; out[ORC_EP_QUEUED_JOB] = env->queued_job;
+    out[ORC_EP_NUM_RUNNING] = env->n_running; out[ORC_EP_STEP_COUNTER] = env->step_counter;
+    out[ORC_EP_LOAD_RATE_SUM] = env->load_rate_sum; out[ORC_EP_LOAD_RATE_N] = env->load_rate_n;
+    out[ORC_EP_DONE] = is_done(env) ? 1.0 : 0.0; out[ORC_EP_STATUS] = ORC_OK;
+}
 int32_t orc_env_last_trace(const orc_env_t* env, const int32_t** n_active, const double** tick) {
     if (!env->last_memo) return 0;
     *n_active = env->last_memo->trace_n; *tick = env->last_memo->trace_tick;

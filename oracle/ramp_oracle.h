@@ -184,6 +184,42 @@ const orc_job_record_t* orc_env_job_records(const orc_env_t* env);
 /* last lookahead trace run or looked up by the env (for parity checks) */
 int32_t orc_env_last_trace(const orc_env_t* env, const int32_t** n_active, const double** tick);
 
+/* the episode scalars in the layout of the product's episode-state row (include/ramp_b200.h RAMP_EP_*) */
+enum { ORC_EP_TIME = 0, ORC_EP_NEXT_ARRIVAL, ORC_EP_NUM_ARRIVED, ORC_EP_NUM_COMPLETED, ORC_EP_NUM_BLOCKED, ORC_EP_QUEUED_JOB,
+       ORC_EP_NUM_RUNNING, ORC_EP_STEP_COUNTER, ORC_EP_LOAD_RATE_SUM, ORC_EP_LOAD_RATE_N, ORC_EP_DONE, ORC_EP_STATUS, ORC_EP_LEN };
+void orc_env_episode_state(const orc_env_t* env, double* out /* [ORC_EP_LEN] */);
+
+/* ------------------------------------------------------------------------- */
+/* batched drivers (ramp_oracle_batch.c): one orc_env_t per episode, episodes spread over n_threads host threads.
+ * script_tid / script_mount: [n_episodes][n_steps], tid -1 = Action(); arrivals: [n_episodes][n_jobs]. */
+int orc_run_lookahead_batch(const orc_lowered_job_t* const* jobs, int32_t n, orc_lookahead_result_t* results, int32_t n_threads);
+/* n_steps cluster steps per episode; stats_out [n_episodes][n_steps][ORC_STEP_STATS_LEN] may be NULL */
+int orc_run_scripted_batch(const orc_lowered_job_t* templates, int32_t n_templates, int32_t n_episodes, int32_t n_steps,
+                           const int32_t* script_tid, const orc_mount_t* script_mount, const orc_arrival_t* arrivals, int32_t n_jobs,
+                           double max_sim_time, int32_t n_cluster_workers, int32_t memo_models, int32_t memo_degrees,
+                           double* stats_out, orc_job_record_t* records_out, int32_t n_threads);
+/* n_steps RampJobPartitioningEnvironment.step calls per episode (the action step, then Action() until a job is queued or the
+ * episode is done); stats_out rows are the action steps' with SS_DONE taken after the whole env-step */
+int orc_run_scripted_rjpe_batch(const orc_lowered_job_t* templates, int32_t n_templates, int32_t n_episodes, int32_t n_steps,
+                                const int32_t* script_tid, const orc_mount_t* script_mount, const orc_arrival_t* arrivals, int32_t n_jobs,
+                                double max_sim_time, int32_t n_cluster_workers, int32_t memo_models, int32_t memo_degrees,
+                                double* stats_out, orc_job_record_t* records_out, int32_t n_threads);
+/* The same env-steps with everything the product's step path hands back.  An episode that is done is not stepped again: its
+ * later env-steps run no cluster step, and their stats_out rows are zero but for SS_STEP_COUNTER, SS_JOB_QUEUE_LENGTH and
+ * SS_DONE, as the product writes them for a finished episode.  Outputs (each may be NULL):
+ *   stats_out       [n_episodes][n_steps][ORC_STEP_STATS_LEN]   as orc_run_scripted_rjpe_batch
+ *   ncs_out         [n_episodes][n_steps]                        cluster steps of each env-step
+ *   cs_stats_out    [n_episodes][cs_cap][ORC_STEP_STATS_LEN]     every cluster step's row in order, fused Action() steps included
+ *   cs_total_out    [n_episodes]                                 rows written to cs_stats_out
+ *   records_out     [n_episodes][n_jobs]
+ *   ep_out          [n_episodes][ORC_EP_LEN]                     orc_env_episode_state after the last env-step
+ * Returns ORC_ERR_TRACE_OVERFLOW if an episode runs more than cs_cap cluster steps (cs_stats_out != NULL). */
+int orc_run_scripted_rjpe_full_batch(const orc_lowered_job_t* templates, int32_t n_templates, int32_t n_episodes, int32_t n_steps,
+                                     const int32_t* script_tid, const orc_mount_t* script_mount, const orc_arrival_t* arrivals,
+                                     int32_t n_jobs, double max_sim_time, int32_t n_cluster_workers, int32_t memo_models,
+                                     int32_t memo_degrees, double* stats_out, int32_t* ncs_out, double* cs_stats_out, int32_t cs_cap,
+                                     int32_t* cs_total_out, orc_job_record_t* records_out, double* ep_out, int32_t n_threads);
+
 #ifdef __cplusplus
 }
 #endif
