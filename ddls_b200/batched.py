@@ -31,7 +31,7 @@ import numpy as np
 
 from . import engine as _engine
 from .expand import expand_template
-from .observation import PARAM_KEYS, _block_shapes_exist
+from .observation import PARAM_KEYS, _block_shapes_exist, job_arrays
 from .synth import ForwardGraph
 from .template_builder import RampShape, original_job_totals
 
@@ -47,13 +47,50 @@ class _Model:
         self.n = g.n
         self.mem = [a + p for a, p in zip(g.act, g.par)]
         self.op_mem_total, self.dep_size_total = original_job_totals(g)
+        self.n_ops, self.n_deps = 2 * g.n, 2 * len(g.edges) + 1       # the mirrored job's nodes and edges (the join edge n -> n+1)
         self.quantum = quantum
-        # the mirrored job graph's node order: forward 1..n then backward 2n..n+1 is NOT the reference's dict order; the static
-        # observation only needs multiset statistics and per-op arrays in any fixed order, so forward-then-backward is used
-        self.seq_time = float(sum(g.fwd) + sum(g.bwd)) * num_training_steps
+        # summed in the mirrored job's node order (JOB:224-235), as the reference's job details hold it
+        self.seq_time = job_arrays(g, num_training_steps)['sequential_completion_time']
 
     def splits(self, degree: int) -> List[int]:
         return [int(max(1, min(math.ceil(math.ceil(c / self.quantum) / 2) * 2, degree))) for c in self.graph.fwd]   # RJPE:336
+
+
+def jobs_params(models: Sequence[_Model], frac: Tuple[float, float], num_training_steps: int, max_partitions_per_op_in_observation: int = 1):
+    """(min, max) per PARAM_KEYS, by JobsGenerator._init_jobs_params' rules (jobs_generator.py:276-333) over one job of each model:
+
+      * job_total_num_ops: max = int(max * max_partitions_per_op_in_observation)
+      * job_total_num_deps: max = int(max / 2 * P * 2) forward + twice that backward (3 * max at P = 1)
+      * job_total_dep_sizes: max = max * int(N (N - 1) / 2), N = the largest op count * P (the job made fully connected)
+      * every other key: min and max of the values.
+
+    RampJobPartitioningEnvironment never sets max_partitions_per_op_in_observation, so P = 1.  The reference takes the two
+    max-acceptable-JCT keys over the max_acceptable_job_completion_time_frac of every job of its sampled pool; that pool is not
+    modelled here, so they span the frac distribution's bounds frac = (lo, hi): [lo, hi] and [lo * seq, hi * seq] over the
+    models.  Pass the reference's own jobs_params to the environment (``jobs_params=``) to observe exactly what it observes."""
+    P = max_partitions_per_op_in_observation
+    lo, hi = frac[0], frac[1]
+    n_ops, n_deps = [m.n_ops for m in models], [m.n_deps for m in models]
+    fwd_deps = int((max(n_deps) / 2) * P * 2)
+    max_nodes = max(n_ops) * P
+    dep = [m.dep_size_total for m in models]
+    seq = [m.seq_time for m in models]
+    opm = [m.op_mem_total for m in models]
+    macc = [f * s for s in seq for f in (lo, hi)]
+    table = {
+        'job_total_num_ops': (min(n_ops), int(max(n_ops) * P)),
+        'job_total_num_deps': (min(n_deps), fwd_deps + int(fwd_deps * 2)),
+        'job_sequential_completion_times': (min(seq), max(seq)),
+        'max_acceptable_job_completion_times': (min(macc), max(macc)),
+        'max_acceptable_job_completion_time_fracs': (lo, hi),
+        'job_total_op_memory_costs': (min(opm), max(opm)),
+        'job_total_dep_sizes': (min(dep), max(dep) * int(max_nodes * (max_nodes - 1) / 2)),
+        'job_num_training_steps': (num_training_steps, num_training_steps),
+    }
+    return [(float(table[k][0]), float(table[k][1])) for k in PARAM_KEYS]
+
+
+_default_jobs_params = jobs_params              # the environment's constructor argument of the same name shadows it
 
 
 class BatchedRampJobPartitioningEnvironment:
@@ -62,7 +99,11 @@ class BatchedRampJobPartitioningEnvironment:
                  interarrival=('fixed', 1000.0), frac=(0.1, 1.0, 2), max_simulation_run_time: float = float('inf'),
                  fail_reward: float = -1, success_reward: float = 1, device: int = 0, seed: int = 0,
                  run_times: str = 'reference', apply_action_mask: bool = True, script: Optional[dict] = None,
-                 memo_mode: int = _engine.MEMO_REFERENCE):
+                 memo_mode: int = _engine.MEMO_REFERENCE, jobs_params: Optional[dict] = None, machine_epsilon: float = 1e-7):
+        """jobs_params: the normalisers of the observation's job features, as the reference's ``JobsGenerator.jobs_params`` holds
+        them (``min_<key>`` / ``max_<key>`` for the keys of observation.PARAM_KEYS); the keys it gives replace the defaults of
+        ``jobs_params(models, ...)``.  machine_epsilon: added to a normalised feature that comes out negative (observation.py:441-444,
+        493-496), as RampJobPartitioningObservation does."""
         self.shape = RampShape(*shape)
         self.W = self.shape.n_workers
         self.B, self.J = int(n_episodes), int(jobs_per_episode)
@@ -91,7 +132,11 @@ class BatchedRampJobPartitioningEnvironment:
         self._t_mount: List[tuple] = []                      # per template id: (seq_time, part_op_mem, part_dep, flow, n_workers, n_channels)
         self._t_arrays = None
         self.stats = {'placer_calls': 0, 'expansions': 0, 'placement_hits': 0}
-        self._jobs_params = None
+        self.machine_epsilon = float(machine_epsilon)
+        self._jobs_params = _default_jobs_params(self.models, frac, num_training_steps)
+        for i, k in enumerate(PARAM_KEYS):
+            if jobs_params is not None and f'min_{k}' in jobs_params and f'max_{k}' in jobs_params:
+                self._jobs_params[i] = (float(jobs_params[f'min_{k}']), float(jobs_params[f'max_{k}']))
 
     # ---- arrival streams ------------------------------------------------------------------------------------------
     def _draw_streams(self):
@@ -365,20 +410,8 @@ class BatchedRampJobPartitioningEnvironment:
 
     # ---- observations ---------------------------------------------------------------------------------------------
     def jobs_params(self):
-        """(min, max) per PARAM_KEYS over the job types, as JobsGenerator.jobs_params holds them (jobs_generator.py:278-333)."""
-        if self._jobs_params is None:
-            lo, hi, _ = self.frac_dist
-            vals = {
-                'job_total_num_ops': [2 * m.n for m in self.models],
-                'job_total_num_deps': [2 * len(m.graph.edges) + 1 for m in self.models],
-                'job_sequential_completion_times': [m.seq_time for m in self.models],
-                'max_acceptable_job_completion_times': [f * m.seq_time for m in self.models for f in (lo, hi)],
-                'max_acceptable_job_completion_time_fracs': [lo, hi],
-                'job_total_op_memory_costs': [m.op_mem_total for m in self.models],
-                'job_total_dep_sizes': [m.dep_size_total for m in self.models],
-                'job_num_training_steps': [self.num_training_steps],
-            }
-            self._jobs_params = [(min(vals[k]), max(vals[k])) for k in PARAM_KEYS]
+        """(min, max) per PARAM_KEYS: the normalisers of the observation's job features (``jobs_params(models, ...)`` or the
+        reference's table given to the constructor)."""
         return self._jobs_params
 
     def _observe(self):
@@ -386,14 +419,14 @@ class BatchedRampJobPartitioningEnvironment:
         qq = np.clip(self.queued, 0, self.J - 1)
         m_of = self.model_of[np.arange(B), qq]
         fr = self.frac[np.arange(B), qq]
-        P = self.jobs_params()
+        P = self._jobs_params
 
         def norm(x, k):
             lo, hi = P[PARAM_KEYS.index(k)]
             return (x - lo) / (hi - lo) if hi - lo != 0 else np.ones_like(x, dtype=np.float64)
         seq = np.array([m.seq_time for m in self.models])[m_of]
-        n_ops = np.array([2.0 * m.n for m in self.models])[m_of]
-        n_deps = np.array([2.0 * len(m.graph.edges) + 1 for m in self.models])[m_of]
+        n_ops = np.array([float(m.n_ops) for m in self.models])[m_of]
+        n_deps = np.array([float(m.n_deps) for m in self.models])[m_of]
         opm = np.array([m.op_mem_total for m in self.models])[m_of]
         dps = np.array([m.dep_size_total for m in self.models])[m_of]
         mounted = self.W - self._free_count()
@@ -402,7 +435,8 @@ class BatchedRampJobPartitioningEnvironment:
                         norm(fr, 'max_acceptable_job_completion_time_fracs'), fr, norm(opm, 'job_total_op_memory_costs'),
                         norm(dps, 'job_total_dep_sizes'),
                         norm(np.full(B, float(self.num_training_steps)), 'job_num_training_steps'),
-                        mounted / self.W, self.n_running / self.W], axis=1).astype(np.float32)
+                        mounted / self.W, self.n_running / self.W], axis=1)
+        dyn = np.where(dyn < 0, dyn + self.machine_epsilon, dyn).astype(np.float32)     # observation.py:441-444, 493-496
         mask = self.action_mask()
         return {'model': m_of.astype(np.int32), 'graph_features_dynamic': dyn, 'action_set': self.action_set,
                 'action_mask': mask.astype(np.int16), 'queued_job': self.queued.copy(), 'done': self.done.copy()}
@@ -460,9 +494,8 @@ class DeviceRampJobPartitioningEnvironment(BatchedRampJobPartitioningEnvironment
                         and sum(model.mem) <= d * A100_MEMORY:
                     uniform[m, d] = 1
         self._uniform = uniform
-        P = self.jobs_params()
-        mp = np.array([[mo.seq_time, 2.0 * mo.n, 2.0 * len(mo.graph.edges) + 1, mo.op_mem_total, mo.dep_size_total] for mo in self.models],
-                      dtype=np.float64)
+        P = self._jobs_params
+        mp = np.array([[mo.seq_time, mo.n_ops, mo.n_deps, mo.op_mem_total, mo.dep_size_total] for mo in self.models], dtype=np.float64)
         keep = dict(cand_ptr=np.ascontiguousarray(cand_ptr, dtype=np.int32),
                     cand_mask=np.ascontiguousarray(cand_mask, dtype=np.uint64).reshape(-1, nw),
                     cand_geom=np.ascontiguousarray(cand_geom, dtype=np.int32), uniform=np.ascontiguousarray(uniform),
@@ -473,10 +506,12 @@ class DeviceRampJobPartitioningEnvironment(BatchedRampJobPartitioningEnvironment
             _fields_ = [('shape', C.c_int32 * 3), ('n_models', C.c_int32), ('max_degree', C.c_int32), ('n_geoms', C.c_int32),
                         ('jobs_per_episode', C.c_int32), ('n_words', C.c_int32), ('apply_action_mask', C.c_int32),
                         ('num_training_steps', C.c_int32), ('fail_reward', C.c_double), ('success_reward', C.c_double),
+                        ('machine_epsilon', C.c_double),
                         ('cand_ptr', C.c_void_p), ('cand_mask', C.c_void_p), ('cand_geom', C.c_void_p), ('uniform', C.c_void_p),
                         ('shape_ok', C.c_void_p), ('model_params', C.c_void_p), ('jobs_params', C.c_void_p)]
         cfg = _Cfg((C.c_int32 * 3)(*shape), M, D, self._n_geoms, self.J, nw, 1 if self.apply_action_mask else 0, self.num_training_steps,
-                   float(self.fail_reward), float(self.success_reward), keep['cand_ptr'].ctypes.data, keep['cand_mask'].ctypes.data,
+                   float(self.fail_reward), float(self.success_reward), self.machine_epsilon,
+                   keep['cand_ptr'].ctypes.data, keep['cand_mask'].ctypes.data,
                    keep['cand_geom'].ctypes.data, keep['uniform'].ctypes.data, keep['shape_ok'].ctypes.data, keep['mp'].ctypes.data,
                    keep['jp'].ctypes.data)
         L = self.eng._L

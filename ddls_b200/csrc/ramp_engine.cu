@@ -1266,6 +1266,7 @@ int ramp_env_create(ramp_engine_t* e, const ramp_env_config_t* c) {
     v.B = B; v.J = J; v.n_words = nw; v.n_models = M; v.max_degree = D; v.n_geoms = G; v.n_workers = n_workers;
     v.apply_mask = c->apply_action_mask; v.fail_reward = c->fail_reward; v.success_reward = c->success_reward;
     v.num_training_steps = (double)c->num_training_steps;
+    v.machine_epsilon = c->machine_epsilon;
     const int n_cand = c->cand_ptr[D + 1];
     int rc;
     int32_t* cand_ptr; unsigned long long* cand_mask; int32_t* cand_geom; uint8_t* uniform; uint8_t* shape_ok; double* mp; double* jp;

@@ -16,7 +16,7 @@ namespace ramp {
 
 struct EnvDev {
     int32_t B, J, n_words, n_models, max_degree, n_geoms, n_workers, apply_mask;
-    double fail_reward, success_reward, num_training_steps;
+    double fail_reward, success_reward, num_training_steps, machine_epsilon;
     // tables
     const int32_t* cand_ptr; const unsigned long long* cand_mask; const int32_t* cand_geom;
     const uint8_t* uniform; const uint8_t* shape_ok;
@@ -114,9 +114,15 @@ __global__ void ramp_env_decide_kernel(const EnvDev v, const EpisodeState ep, ra
     rows[b] = row;
 }
 
-__device__ __forceinline__ float env_norm(double x, const double* jp, int k) {
+// a graph feature as the reference stores it: a negative value gets machine_epsilon added (observation.py:441-444, 493-496), in
+// double, before the float32 observation
+__device__ __forceinline__ float env_feature(double x, double eps) {
+    return (float)(x < 0.0 ? x + eps : x);
+}
+
+__device__ __forceinline__ float env_norm(double x, const double* jp, int k, double eps) {
     const double lo = jp[2 * k], hi = jp[2 * k + 1];
-    return (float)((hi - lo != 0.0) ? (x - lo) / (hi - lo) : 1.0);               // observation.py _norm
+    return env_feature((hi - lo != 0.0) ? (x - lo) / (hi - lo) : 1.0, eps);     // observation.py _norm
 }
 
 __global__ void ramp_env_update_kernel(const EnvDev v, const EpisodeState ep, const int32_t* n_cluster_steps, int first) {
@@ -167,15 +173,16 @@ __global__ void ramp_env_update_kernel(const EnvDev v, const EpisodeState ep, co
         const double* mp = v.model_params + (size_t)m * 5;
         const double fr = v.frac[(size_t)b * J + q2];
         const double* jp = v.jobs_params;
-        o[0] = env_norm(mp[1], jp, 0); o[1] = env_norm(mp[2], jp, 1); o[2] = env_norm(mp[0], jp, 2);
-        o[3] = env_norm(__dmul_rn(fr, mp[0]), jp, 3); o[4] = env_norm(fr, jp, 4); o[5] = (float)fr;
-        o[6] = env_norm(mp[3], jp, 5); o[7] = env_norm(mp[4], jp, 6); o[8] = env_norm(v.num_training_steps, jp, 7);
+        const double eps = v.machine_epsilon;
+        o[0] = env_norm(mp[1], jp, 0, eps); o[1] = env_norm(mp[2], jp, 1, eps); o[2] = env_norm(mp[0], jp, 2, eps);
+        o[3] = env_norm(__dmul_rn(fr, mp[0]), jp, 3, eps); o[4] = env_norm(fr, jp, 4, eps); o[5] = env_feature(fr, eps);
+        o[6] = env_norm(mp[3], jp, 5, eps); o[7] = env_norm(mp[4], jp, 6, eps); o[8] = env_norm(v.num_training_steps, jp, 7, eps);
     } else {
         v.queued_model[b] = -1;
         for (int k = 0; k < 9; ++k) o[k] = 0.f;
     }
-    o[9] = (float)((double)(v.n_workers - free_workers) / (double)v.n_workers);
-    o[10] = (float)((double)n_running / (double)v.n_workers);
+    o[9] = env_feature((double)(v.n_workers - free_workers) / (double)v.n_workers, v.machine_epsilon);
+    o[10] = env_feature((double)n_running / (double)v.n_workers, v.machine_epsilon);
 }
 
 // The reference's heuristic agents (ddls/environments/ramp_job_partitioning/agents/*.py), restated line for line on the action

@@ -29,6 +29,7 @@ from typing import Dict, List, Tuple
 import numpy as np
 
 from .lowered import LoweredJob, MountScalars, NO_CHANNEL
+from .observation import job_arrays
 from .synth import ForwardGraph
 
 
@@ -339,16 +340,11 @@ def build_template(fwd: ForwardGraph, degree: int, shape: RampShape, block_start
 
 
 def original_job_totals(fwd: ForwardGraph):
-    """(job_total_op_memory_cost, job_total_dep_size) of the un-partitioned mirrored job (JOB:237-248)."""
-    n = fwd.n
-    mem = [fwd.act[i] + fwd.par[i] for i in range(n)]
-    op_mem = 2.0 * sum(mem)
-    dep = 0.0
-    for (u, v) in fwd.edges:
-        dep += mem[u - 1]            # forward edge: size = mem(src)
-        dep += mem[v - 1]            # mirrored backward edge 2n-(v-1) -> 2n-(u-1): src is the mirror of v
-    dep += mem[n - 1]                # join edge
-    return op_mem, dep
+    """(job_total_op_memory_cost, job_total_dep_size) of the un-partitioned mirrored job (JOB:237-248): the ops' memory costs
+    (activation + parameters) and the deps' sizes (the source op's activation, utils.py:394-396) summed in the job graph's node /
+    edge iteration order -- ``observation.job_arrays``' totals, so the arrival rows carry the reference's values bit for bit."""
+    a = job_arrays(fwd)
+    return a['total_op_memory'], a['total_dep_size']
 
 
 def random_dag_template(rng: np.random.Generator, n_ops: int, avg_out: float = 3.0, n_workers: int = 4,

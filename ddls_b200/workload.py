@@ -19,7 +19,7 @@ import numpy as np
 
 from . import synth
 from .lowered import LoweredJob
-from .template_builder import RampShape, build_template, original_job_totals
+from .template_builder import RampShape, build_template
 
 ARRIVAL_DTYPE = np.dtype([('interarrival', np.float64), ('orig_op_mem', np.float64), ('orig_dep_size', np.float64)])
 ACTION_DTYPE = np.dtype([('max_acceptable_jct', np.float64), ('part_op_mem', np.float64), ('part_dep_size', np.float64),
@@ -39,6 +39,21 @@ CONFIGS = {
     'cfg5-mix-128w': dict(shape=(8, 4, 4), graphs=[('resnet', {}), ('gpt2', {})], degrees=(2, 4, 8, 16), n_episodes=16384,
                           exponential=True),
 }
+
+
+def scripted_job_totals(g: synth.ForwardGraph):
+    """(orig_op_mem, orig_dep_size) the scripted arrival rows carry for a job of graph g: twice the ops' memory (activation +
+    parameters), and every dep of the mirrored job sized by its source op's memory.  These rows are an input of the workload
+    (the load rate and the demand_* sums of every step read them), fixed so that every version of the simulator is measured on
+    the same workload and its outputs stay comparable; both arms read the same rows.  They are not the reference's job totals
+    (``template_builder.original_job_totals`` is, and the batched environments use it): the dep sizes there are activations only."""
+    mem = [a + p for a, p in zip(g.act, g.par)]
+    dep = 0.0
+    for (u, v) in g.edges:
+        dep += mem[u - 1]            # forward edge: the source op
+        dep += mem[v - 1]            # mirrored backward edge 2n-(v-1) -> 2n-(u-1): its source mirrors v
+    dep += mem[g.n - 1]              # join edge n -> n+1
+    return 2.0 * sum(mem), dep
 
 
 def make_graph(kind, **kw):
@@ -122,7 +137,7 @@ def generate(config: str, jct_of_template: Callable[[Sequence[LoweredJob]], Sequ
     rng = np.random.default_rng(seed)
     jct = np.asarray(jct_of_template(templates), dtype=np.float64)
     n_models = len(graphs)
-    totals = [original_job_totals(g) for g in graphs]
+    totals = [scripted_job_totals(g) for g in graphs]
     by_model = [[t for t in range(len(templates)) if t_model[t] == m] for m in range(n_models)]
 
     # arrival streams (JobsGenerator stand-in): model per job, inter-arrival gaps, max-acceptable fraction

@@ -371,7 +371,8 @@ typedef struct {
     int32_t apply_action_mask;    /* 1: an invalid action is an error (RJPE:317-319); 0: it becomes action 0       */
     int32_t num_training_steps;
     double  fail_reward, success_reward;
-    const int32_t*  cand_ptr;     /* [max_degree + 2] candidates of degree d are [cand_ptr[d], cand_ptr[d + 1])    */
+    double  machine_epsilon;      /* added to a normalised observation feature that is negative (observation.py:441-444, 493-496) */
+    const int32_t*  cand_ptr;    /* [max_degree + 2] candidates of degree d are [cand_ptr[d], cand_ptr[d + 1])    */
     const uint64_t* cand_mask;    /* [n_cand][n_words] servers of the block (bit set)                              */
     const int32_t*  cand_geom;    /* [n_cand] geometry index of the block (what the lowered job depends on)        */
     const uint8_t*  uniform;      /* [n_models][max_degree + 1] 1: every op of the model takes `degree` sub-ops and the job fits

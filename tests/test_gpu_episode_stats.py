@@ -23,7 +23,9 @@ LISTS = ['job_completion_time', 'job_completion_time_speedup', 'job_communicatio
 def golden_env(names, where, max_partitions_per_op=16):
     """The environment replaying golden episodes `names` side by side (tests/test_gpu_batched_env.py's set-up), with every job's
     max acceptable JCT as the reference computed it: from the recorded mount rows for mounted jobs, from the recorded
-    episode_stats for the blocked ones that never mounted.  Returns (env, goldens, per-episode decisions)."""
+    episode_stats for the blocked ones that never mounted.  The arrival rows are the environment's own: the load rates (RCE:364)
+    and the demand_* sums read the original job's total op memory and dep size from them.  Returns (env, goldens, per-episode
+    decisions)."""
     from ddls_b200 import batched
     from ddls_b200.template_builder import original_job_totals
     cls = batched.BatchedRampJobPartitioningEnvironment if where == 'host' else batched.DeviceRampJobPartitioningEnvironment
@@ -54,17 +56,6 @@ def golden_env(names, where, max_partitions_per_op=16):
     env = cls(SHAPES[goldens[0].n_cluster_workers], graphs, n_episodes=B, jobs_per_episode=J, max_partitions_per_op=max_partitions_per_op,
               max_simulation_run_time=goldens[0].max_sim_time, script={'model': model, 'gap': gap, 'max_acceptable_jct': macc},
               apply_action_mask=False)
-    # the arrival rows as the reference recorded them: the load rates (RCE:364) and the demand_* sums read the original job's
-    # total op memory and dep size, and the environment's own dep-size total of a model is not the reference's
-    draw = env._draw_streams
-
-    def recorded_streams():
-        arr = draw()
-        for b, g in enumerate(goldens):
-            a = g.d['arrivals']
-            arr['orig_op_mem'][b, :len(a)], arr['orig_dep_size'][b, :len(a)] = a[:, 1], a[:, 2]
-        return arr
-    env._draw_streams = recorded_streams
     return env, goldens, decisions
 
 
