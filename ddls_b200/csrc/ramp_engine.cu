@@ -5,42 +5,22 @@
 //   plan (memo) -> lookahead (persistent CTAs, one lookahead per CTA at a time) -> step (one thread per episode).
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <map>
 #include <mutex>
 #include <numeric>
-#include <string>
 #include <utility>
 #include <vector>
 
 #include "ramp_kernels.cuh"
 #include "ramp_env.cuh"
+#include "ramp_owned.cuh"
 
 using namespace ramp;
 
 namespace {
-
-thread_local std::string g_last_error;
-
-int set_error(int code, const char* fmt, ...) {
-    char buf[1024];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof(buf), fmt, ap);
-    va_end(ap);
-    g_last_error = buf;
-    return code;
-}
-
-#define CUDA_TRY(expr)                                                                                   \
-    do {                                                                                                 \
-        cudaError_t _e = (expr);                                                                         \
-        if (_e != cudaSuccess)                                                                           \
-            return set_error(RAMP_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-    } while (0)
 
 constexpr int MAX_EVENT_PAIRS = 64;
 constexpr int RAMP_SMEM_CARVEOUT = 100;   // percent of the unified L1/shared array given to shared memory
@@ -72,10 +52,29 @@ LookaheadKernel lookahead_cta_kernel_for(int nt) {   // one CTA of nt threads pe
 
 struct HostTemplate {
     TemplateDev dev;             // copy of what sits in the device array
-    void* blob = nullptr;        // single device allocation holding all arrays
+    DeviceArray<unsigned char> blob;   // single device allocation holding all arrays
     std::vector<unsigned char> bytes;  // canonical host bytes for exact-duplicate detection
     uint64_t hash = 0;
-    void* res_blob = nullptr;    // device copy of the quotient blob (thread-per-lookahead kernel), null if not resident
+    DeviceArray<unsigned char> res_blob;   // device copy of the quotient blob (thread-per-lookahead kernel), empty if not resident
+};
+
+struct ResultArrays {
+    DeviceArray<double> jct, comm, comp, util;
+    DeviceArray<int32_t> n_ticks, status, util_nmw;
+    DeviceArray<int64_t> trace_off;
+    cudaError_t alloc(size_t n) { return alloc_each(n, jct, comm, comp, util, n_ticks, status, util_nmw, trace_off); }
+    ResultSlots view() const { return {jct.get(), comm.get(), comp.get(), n_ticks.get(), status.get(), trace_off.get(), util.get(), util_nmw.get()}; }
+};
+
+struct TraceArrays {
+    DeviceArray<int32_t> n_active;
+    DeviceArray<double> tick;
+    DeviceArray<unsigned long long> top;
+    cudaError_t alloc(uint64_t len) {
+        const cudaError_t err = alloc_each(len, n_active, tick);
+        return err == cudaSuccess ? top.alloc(1) : err;
+    }
+    TracePool view() const { return TracePool{n_active.get(), tick.get(), top.get(), (uint64_t)n_active.size()}; }
 };
 
 }  // namespace
@@ -83,39 +82,39 @@ struct HostTemplate {
 struct ramp_engine {
     ramp_config_t cfg{};
     int sm_count = 0;
-    cudaStream_t stream = nullptr;
+    Stream stream;
     // templates
     std::vector<HostTemplate> templates;
-    TemplateDev* d_templates = nullptr;
+    DeviceArray<TemplateDev> d_templates;
     uint64_t max_scratch = 0;
     int32_t max_w = 1, max_c = 1;
     int32_t par_cap = 0;         // bytes of shared-memory parent counters per lookahead
     // memo + results
     uint32_t memo_cap = 0;
-    unsigned long long* d_memo_keys = nullptr;
-    int32_t* d_memo_vals = nullptr;
-    unsigned long long* d_memo_keys2 = nullptr;
+    DeviceArray<unsigned long long> d_memo_keys;
+    DeviceArray<int32_t> d_memo_vals;
+    DeviceArray<unsigned long long> d_memo_keys2;
     uint32_t memo_cap2 = 0;
-    ResultSlots res{};
+    ResultArrays res;
     int32_t n_slots = 0;
-    TracePool pool{};
+    TraceArrays pool;
     // per-step
-    WorkItem* d_items = nullptr;
-    Counters* d_counters = nullptr;
-    MemoStats* d_stats = nullptr;
-    ramp_action_t* d_actions = nullptr;
-    double* d_step_stats = nullptr;
-    int32_t* d_n_cluster_steps = nullptr;
-    double* d_ep_export = nullptr;
-    double* d_es_export = nullptr;   // [B][RAMP_ES_LEN] ramp_get_episode_stats
-    // episode state
+    DeviceArray<WorkItem> d_items;
+    DeviceArray<Counters> d_counters;
+    DeviceArray<MemoStats> d_stats;
+    DeviceArray<ramp_action_t> d_actions;
+    DeviceArray<double> d_step_stats;
+    DeviceArray<int32_t> d_n_cluster_steps;
+    DeviceArray<double> d_ep_export;
+    DeviceArray<double> d_es_export;     // [B][RAMP_ES_LEN] ramp_get_episode_stats
+    // episode state: the view the kernels take, and its arrays
     EpisodeState ep{};
-    ramp_arrival_t* d_arrivals = nullptr;
-    int32_t* d_n_jobs_ep = nullptr;
+    DeviceArray<double> ep_ef, ep_rf, tick_util; DeviceArray<int32_t> ep_ei, ep_ri, tick_util_n; DeviceArray<ramp_job_record_t> ep_rec;
+    DeviceArray<ramp_arrival_t> d_arrivals;
+    DeviceArray<int32_t> d_n_jobs_ep;
     // lookahead scratch
-    unsigned char* d_scratch = nullptr;
+    DeviceArray<unsigned char> d_scratch;
     uint64_t scratch_stride = 0;
-    int scratch_grid = 0;
     int grid = 0;                // resident CTAs of the warp kernel's 4-warp shape
     size_t smem_bytes = 0;
     // CTA-per-lookahead variant (lower latency; used when a launch has fewer work items than warp slots)
@@ -131,46 +130,45 @@ struct ramp_engine {
     size_t smem2_bytes = 0;      // dynamic shared memory of the 1-warp CTAs used beside a CTA kernel
     int debug = 0;               // RAMP_DEBUG=1 prints the launch decisions to stderr
     int mode = 0;                // 0 auto, 1 warp-per-lookahead, 2 CTA-per-lookahead (RAMP_LOOKAHEAD_MODE); 1 and 2 make nothing resident
-    int32_t* h_n_work = nullptr; // pinned [4]
-    WorkItem* d_items_big = nullptr;
-    cudaStream_t stream2 = nullptr;  // big lookaheads run concurrently with the small ones
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+    PinnedArray<int32_t> h_n_work;   // [4]
+    DeviceArray<WorkItem> d_items_big;
+    Stream stream2;              // big lookaheads run concurrently with the small ones
+    Event ev_fork, ev_join;
     // resident (quotient) templates: thread-per-lookahead kernel
     int use_quotient = 1;        // 0 (RAMP_LOOKAHEAD_MODE=thread_unfolded): resident blobs are built from the unfolded job (identity quotient)
     int n_resident = 0, n_nonresident = 0;
     int32_t res_tmpl_cap = 0, res_n_cap = 0, res_spill_ops = 0, res_spill_deps = 0;
     int res_grid = 0;
     size_t res_smem = 0;
-    unsigned char* d_res_scratch = nullptr;
+    DeviceArray<unsigned char> d_res_scratch;
     uint64_t res_scratch_stride = 0;
-    int res_scratch_grid = 0;
-    WorkItem* d_items_res = nullptr;
-    WorkItem* d_chunk_items = nullptr;   // [B][32]
-    ChunkDesc* d_chunks = nullptr;       // [B]
-    int32_t* d_tcount = nullptr;         // [max_templates + 1]
-    int32_t* d_tbase = nullptr;
-    int32_t* d_rank = nullptr;           // [B]
-    TemplateHints* d_hints = nullptr;    // [max_templates]
-    double* d_hint_jct = nullptr;        // [max_templates]
+    DeviceArray<WorkItem> d_items_res;
+    DeviceArray<WorkItem> d_chunk_items;   // [B][32]
+    DeviceArray<ChunkDesc> d_chunks;       // [B]
+    DeviceArray<int32_t> d_tcount;         // [max_templates + 1]
+    DeviceArray<int32_t> d_tbase;
+    DeviceArray<int32_t> d_rank;           // [B]
+    DeviceArray<TemplateHints> d_hints;    // [max_templates]
+    DeviceArray<double> d_hint_jct;        // [max_templates]
     // device-resident rollouts (ramp_env_*)
     bool has_env = false;
     EnvDev env{};
-    std::vector<void*> env_allocs;
-    int32_t* env_h_need = nullptr;       // pinned: [0] = count, [1] = error flag; [2], [3]: the same, read by ramp_env_read; [4] engine error episode
-    void* env_h_mirror = nullptr;        // pinned host arrays (ramp_env_host_mirror)
+    std::vector<DeviceArray<unsigned char>> env_allocs;
+    PinnedArray<int32_t> env_h_need;     // [0] = count, [1] = error flag; [2], [3]: the same, read by ramp_env_read; [4] engine error episode
+    PinnedArray<unsigned char> env_h_mirror;   // host arrays of ramp_env_host_mirror
     bool env_unchecked_decide = false;   // a ramp_env_decide without need_host_out has not been looked at yet
     bool env_agents_set = false;         // ramp_env_set_agents ran
     // standalone lookahead buffers
-    WorkItem* sa_chunk_items = nullptr;
-    ChunkDesc* sa_chunks = nullptr;
-    ResultSlots sa_res{};
+    DeviceArray<WorkItem> sa_chunk_items;
+    DeviceArray<ChunkDesc> sa_chunks;
+    ResultArrays sa_res;
     int32_t sa_cap = 0;
-    WorkItem* sa_items = nullptr;        // [n]: the small, big and resident work lists, one after the other
-    int32_t* sa_rank = nullptr;          // [n] ramp_bucket_kernel scratch
-    Counters* sa_counters = nullptr;
+    DeviceArray<WorkItem> sa_items;      // [n]: the small, big and resident work lists, one after the other
+    DeviceArray<int32_t> sa_rank;        // [n] ramp_bucket_kernel scratch
+    DeviceArray<Counters> sa_counters;
     // instrumentation
     int64_t launches = 0;
-    cudaEvent_t ev_a[MAX_EVENT_PAIRS]{}, ev_b[MAX_EVENT_PAIRS]{};
+    Event ev_a[MAX_EVENT_PAIRS], ev_b[MAX_EVENT_PAIRS];
     int ev_pending = 0;
     double la_ms_total = 0.0;
     int64_t la_launches = 0;
@@ -178,25 +176,11 @@ struct ramp_engine {
     MemoStats memo_base{};       // device counters at the last ramp_reset (memo statistics are reported since the reset)
 };
 
-namespace {
-
-int alloc_result_slots(ResultSlots& r, int32_t n) {
-    CUDA_TRY(cudaMalloc(&r.jct, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc(&r.comm, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc(&r.comp, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc(&r.n_ticks, sizeof(int32_t) * n));
-    CUDA_TRY(cudaMalloc(&r.status, sizeof(int32_t) * n));
-    CUDA_TRY(cudaMalloc(&r.trace_off, sizeof(int64_t) * n));
-    CUDA_TRY(cudaMalloc(&r.util, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc(&r.util_nmw, sizeof(int32_t) * n));
-    return RAMP_OK;
-}
-
 // A kernel's dynamic shared memory limit (cudaFuncAttributeMaxDynamicSharedMemorySize) belongs to the kernel in the device's
 // context, not to an engine: every engine of the process shares it.  Lowering it to what one engine needs would make another
 // engine's launches that need more fail, so it only ever rises.  Each engine still launches with, and sizes its grid for, its own
 // dynamic shared memory.
-cudaError_t reserve_dynamic_smem(const void* kern, size_t bytes) {
+cudaError_t ramp::reserve_dynamic_smem(const void* kern, size_t bytes) {
     static std::mutex mu;
     static std::map<std::pair<int, const void*>, size_t> reserved;
     int dev = 0;
@@ -210,16 +194,12 @@ cudaError_t reserve_dynamic_smem(const void* kern, size_t bytes) {
     return err;
 }
 
-void free_result_slots(ResultSlots& r) {
-    cudaFree(r.jct); cudaFree(r.comm); cudaFree(r.comp); cudaFree(r.n_ticks); cudaFree(r.status); cudaFree(r.trace_off);
-    cudaFree(r.util); cudaFree(r.util_nmw);
-    r = ResultSlots{};
-}
+namespace {
 
 int resolve_events(ramp_engine* e) {
     for (int k = 0; k < e->ev_pending; ++k) {
         float ms = 0.f;
-        CUDA_TRY(cudaEventElapsedTime(&ms, e->ev_a[k], e->ev_b[k]));
+        CUDA_TRY(cudaEventElapsedTime(&ms, e->ev_a[k].get(), e->ev_b[k].get()));
         e->la_ms_total += ms;
         e->la_launches++;
     }
@@ -277,13 +257,10 @@ int ensure_scratch(ramp_engine* e) {
     }
     // one slab per lookahead in flight; the warp kernel and one of the CTA kernels may run side by side
     const int n_slabs = std::max(e->grid * (WARP_NT / 32) + std::max(e->cta_grid, e->cta64_grid), e->dense_grid * (DENSE_NT / 32));
-    if (stride != e->scratch_stride || n_slabs != e->scratch_grid || e->d_scratch == nullptr) {
-        CUDA_TRY(cudaStreamSynchronize(e->stream));
-        if (e->d_scratch) cudaFree(e->d_scratch);
-        e->d_scratch = nullptr;
-        CUDA_TRY(cudaMalloc(&e->d_scratch, stride * (uint64_t)n_slabs));
+    if (stride != e->scratch_stride || stride * (uint64_t)n_slabs != e->d_scratch.size()) {
+        CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
+        CUDA_TRY(e->d_scratch.alloc(stride * (uint64_t)n_slabs));
         e->scratch_stride = stride;
-        e->scratch_grid = n_slabs;
     }
     return RAMP_OK;
 }
@@ -291,13 +268,13 @@ int ensure_scratch(ramp_engine* e) {
 LookaheadArgs make_lookahead_args(ramp_engine* e, const WorkItem* items, Counters* counters, const ResultSlots& res,
                                   const TracePool& pool, MemoStats* stats) {
     LookaheadArgs a{};
-    a.templates = e->d_templates;
+    a.templates = e->d_templates.get();
     a.items = items;
     a.n_work = &counters->n_work;
     a.items_b = nullptr;
     a.n_work_b = nullptr;
     a.cursor = &counters->work_cursor;
-    a.scratch = e->d_scratch;
+    a.scratch = e->d_scratch.get();
     a.scratch_stride = e->scratch_stride;
     a.res = res;
     a.pool = pool;
@@ -449,13 +426,10 @@ int ensure_thread_scratch(ramp_engine* e) {
                               smem, occ, RAMP_THREAD_CTA, e->res_grid);
     }
     const uint64_t stride = thread_scratch_bytes(e->res_spill_ops, e->res_spill_deps, e->cfg.trace_cap);
-    if (stride != e->res_scratch_stride || e->res_grid != e->res_scratch_grid || !e->d_res_scratch) {
-        CUDA_TRY(cudaStreamSynchronize(e->stream));
-        if (e->d_res_scratch) cudaFree(e->d_res_scratch);
-        e->d_res_scratch = nullptr;
-        CUDA_TRY(cudaMalloc(&e->d_res_scratch, stride * (uint64_t)e->res_grid));
+    if (stride != e->res_scratch_stride || stride * (uint64_t)e->res_grid != e->d_res_scratch.size()) {
+        CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
+        CUDA_TRY(e->d_res_scratch.alloc(stride * (uint64_t)e->res_grid));
         e->res_scratch_stride = stride;
-        e->res_scratch_grid = e->res_grid;
     }
     return RAMP_OK;
 }
@@ -463,11 +437,11 @@ int ensure_thread_scratch(ramp_engine* e) {
 ThreadArgs make_thread_args(ramp_engine* e, const ChunkDesc* chunks, const WorkItem* chunk_items, Counters* c,
                             const ResultSlots& res, const TracePool& pool, MemoStats* stats) {
     ThreadArgs a{};
-    a.templates = e->d_templates; a.chunks = chunks; a.n_chunks = &c->n_chunks; a.cursor = &c->chunk_cursor; a.items = chunk_items;
-    a.scratch = e->d_res_scratch; a.scratch_stride = e->res_scratch_stride;
+    a.templates = e->d_templates.get(); a.chunks = chunks; a.n_chunks = &c->n_chunks; a.cursor = &c->chunk_cursor; a.items = chunk_items;
+    a.scratch = e->d_res_scratch.get(); a.scratch_stride = e->res_scratch_stride;
     a.res = res; a.pool = pool; a.trace_cap = e->cfg.trace_cap;
     a.tmpl_cap = e->res_tmpl_cap; a.n_cap = e->res_n_cap; a.spill_ops = e->res_spill_ops; a.spill_deps = e->res_spill_deps;
-    a.stats = stats; a.hints = e->d_hints; a.hint_jct = e->d_hint_jct;
+    a.stats = stats; a.hints = e->d_hints.get(); a.hint_jct = e->d_hint_jct.get();
     return a;
 }
 
@@ -476,7 +450,7 @@ void bucket_resident(ramp_engine* e, const WorkItem* items, Counters* c, WorkIte
                      cudaStream_t st) {
     BucketArgs ba{};
     ba.items = items; ba.n_items = &c->n_work_res; ba.n_templates = (int32_t)e->templates.size();
-    ba.tcount = e->d_tcount; ba.tbase = e->d_tbase; ba.chunk_items = chunk_items; ba.chunks = chunks;
+    ba.tcount = e->d_tcount.get(); ba.tbase = e->d_tbase.get(); ba.chunk_items = chunk_items; ba.chunks = chunks;
     ba.n_chunks = &c->n_chunks; ba.cursor = &c->chunk_cursor; ba.rank = rank;
     ramp_bucket_kernel<<<1, 1024, 0, st>>>(ba);
     e->launches++;
@@ -518,11 +492,11 @@ int launch_lookaheads(ramp_engine* e, const ChunkDesc* chunks, const WorkItem* c
     if (split) {
         // the second stream starts after all that is queued on `st`: a standalone run's uploads and bucket kernel, the
         // thread kernel
-        CUDA_TRY(cudaEventRecord(e->ev_fork, st));
-        CUDA_TRY(cudaStreamWaitEvent(e->stream2, e->ev_fork, 0));
+        CUDA_TRY(cudaEventRecord(e->ev_fork.get(), st));
+        CUDA_TRY(cudaStreamWaitEvent(e->stream2.get(), e->ev_fork.get(), 0));
         const int grid = std::min(n_big, e->cta_grid_for(split_nt));
-        lookahead_cta_kernel_for(split_nt)<<<grid, split_nt, e->cta_smem_bytes, e->stream2>>>(ab);
-        CUDA_TRY(cudaEventRecord(e->ev_join, e->stream2));
+        lookahead_cta_kernel_for(split_nt)<<<grid, split_nt, e->cta_smem_bytes, e->stream2.get()>>>(ab);
+        CUDA_TRY(cudaEventRecord(e->ev_join.get(), e->stream2.get()));
         e->launches++;
         if (n_small > 0) {
             LookaheadArgs as = a;
@@ -532,7 +506,7 @@ int launch_lookaheads(ramp_engine* e, const ChunkDesc* chunks, const WorkItem* c
             split_warp_kernel()<<<g2, SPLIT_WARP_NT, e->smem2_bytes, st>>>(as);
             e->launches++;
         }
-        CUDA_TRY(cudaStreamWaitEvent(st, e->ev_join, 0));
+        CUDA_TRY(cudaStreamWaitEvent(st, e->ev_join.get(), 0));
     } else if (e->mode == 2) {
         // each list on a CTA kernel of its own: RAMP_LOOKAHEAD_CTA_THREADS threads per CTA, else 128 while the list fits
         // one wave of them and 64 beyond
@@ -561,11 +535,21 @@ int launch_lookaheads(ramp_engine* e, const ChunkDesc* chunks, const WorkItem* c
     return RAMP_OK;
 }
 
+// one array of the device environment (EnvDev), owned by the engine: n elements of T from `src`, or zeros
+template <class T> int env_upload(ramp_engine* e, T** dst, const void* src, size_t n) {
+    e->env_allocs.emplace_back();
+    CUDA_TRY(e->env_allocs.back().alloc(sizeof(T) * std::max<size_t>(n, 1)));
+    *dst = reinterpret_cast<T*>(e->env_allocs.back().get());
+    if (src && n) CUDA_TRY(cudaMemcpy(e->env_allocs.back().get(), src, sizeof(T) * n, cudaMemcpyHostToDevice));
+    else CUDA_TRY(cudaMemset(e->env_allocs.back().get(), 0, sizeof(T) * std::max<size_t>(n, 1)));
+    return RAMP_OK;
+}
+
 }  // namespace
 
 // hooks for the other translation units of the library (ramp_policy.cu); not part of the C ABI
 int ramp_internal_set_error(int code, const char* msg) { g_last_error = msg; return code; }
-cudaStream_t ramp_internal_stream(ramp_engine_t* e) { return e->stream; }
+cudaStream_t ramp_internal_stream(ramp_engine_t* e) { return e->stream.get(); }
 int ramp_internal_device(ramp_engine_t* e) { return e->cfg.device; }
 void ramp_internal_count_launches(ramp_engine_t* e, int n) { e->launches += n; }
 
@@ -605,11 +589,11 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
         cfg.memo_capacity_log2 = lg;
     }
     CUDA_TRY(cudaSetDevice(cfg.device));
-    ramp_engine* e = new ramp_engine();
+    std::unique_ptr<ramp_engine> e(new ramp_engine());     // frees whatever was allocated when a step below fails
     e->cfg = cfg;
     if (const char* v = getenv("RAMP_LOOKAHEAD_CTA_THREADS")) {
         const int nt = atoi(v);
-        if (lookahead_cta_kernel_for(nt) == nullptr) { delete e; return set_error(RAMP_ERR_BAD_ARG, "RAMP_LOOKAHEAD_CTA_THREADS must be 64, 128 or 256"); }
+        if (lookahead_cta_kernel_for(nt) == nullptr) return set_error(RAMP_ERR_BAD_ARG, "RAMP_LOOKAHEAD_CTA_THREADS must be 64, 128 or 256");
         e->cta_nt = nt;
     }
     if (const char* v = getenv("RAMP_LOOKAHEAD_MODE")) {
@@ -623,108 +607,82 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     cudaDeviceProp prop{};
     CUDA_TRY(cudaGetDeviceProperties(&prop, cfg.device));
     e->sm_count = prop.multiProcessorCount;
-    CUDA_TRY(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+    CUDA_TRY(create(e->stream, cudaStreamNonBlocking));
     const int B = cfg.n_episodes;
 
-    CUDA_TRY(cudaMalloc(&e->d_templates, sizeof(TemplateDev) * cfg.max_templates));
+    CUDA_TRY(e->d_templates.alloc(cfg.max_templates));
     e->memo_cap = 1u << cfg.memo_capacity_log2;
-    CUDA_TRY(cudaMalloc(&e->d_memo_keys, sizeof(unsigned long long) * e->memo_cap));
-    CUDA_TRY(cudaMemset(e->d_memo_keys, 0, sizeof(unsigned long long) * e->memo_cap));
-    CUDA_TRY(cudaMalloc(&e->d_memo_vals, sizeof(int32_t) * e->memo_cap));
+    CUDA_TRY(e->d_memo_keys.alloc(e->memo_cap));
+    CUDA_TRY(cudaMemset(e->d_memo_keys.get(), 0, sizeof(unsigned long long) * e->memo_cap));
+    CUDA_TRY(e->d_memo_vals.alloc(e->memo_cap));
     e->memo_cap2 = 1;
     while (e->memo_cap2 < (uint32_t)cfg.max_templates * 2u) e->memo_cap2 <<= 1;
-    CUDA_TRY(cudaMalloc(&e->d_memo_keys2, sizeof(unsigned long long) * e->memo_cap2));
-    CUDA_TRY(cudaMemset(e->d_memo_keys2, 0, sizeof(unsigned long long) * e->memo_cap2));
+    CUDA_TRY(e->d_memo_keys2.alloc(e->memo_cap2));
+    CUDA_TRY(cudaMemset(e->d_memo_keys2.get(), 0, sizeof(unsigned long long) * e->memo_cap2));
     e->n_slots = (int32_t)e->memo_cap + B + (int32_t)e->memo_cap2;
-    if (alloc_result_slots(e->res, e->n_slots) != RAMP_OK) return RAMP_ERR_CUDA;
-    CUDA_TRY(cudaMemset(e->res.status, 0, sizeof(int32_t) * e->n_slots));
+    CUDA_TRY(e->res.alloc(e->n_slots));
+    CUDA_TRY(cudaMemset(e->res.status.get(), 0, sizeof(int32_t) * e->n_slots));
 
     // trace pool: exact-size allocations; 4 Mi entries at least, else enough for 8 un-memoised lookaheads of 2,048 ticks per
     // episode between two resets (the pool is reset with the memo)
-    e->pool.len = std::max<uint64_t>(4ull << 20, (uint64_t)B * 8ull * 2048ull);      // B=1: 48 MiB; B=4096: 805 MiB
-    CUDA_TRY(cudaMalloc(&e->pool.n_active, sizeof(int32_t) * e->pool.len));
-    CUDA_TRY(cudaMalloc(&e->pool.tick, sizeof(double) * e->pool.len));
-    CUDA_TRY(cudaMalloc(&e->pool.top, sizeof(unsigned long long)));
-    CUDA_TRY(cudaMemset(e->pool.top, 0, sizeof(unsigned long long)));
+    CUDA_TRY(e->pool.alloc(std::max<uint64_t>(4ull << 20, (uint64_t)B * 8ull * 2048ull)));      // B=1: 48 MiB; B=4096: 805 MiB
+    CUDA_TRY(cudaMemset(e->pool.top.get(), 0, sizeof(unsigned long long)));
 
-    CUDA_TRY(cudaMalloc(&e->d_items, sizeof(WorkItem) * B));
-    CUDA_TRY(cudaMalloc(&e->d_items_big, sizeof(WorkItem) * B));
-    CUDA_TRY(cudaMalloc(&e->d_items_res, sizeof(WorkItem) * B));
-    CUDA_TRY(cudaMalloc(&e->d_chunk_items, sizeof(WorkItem) * (size_t)B * 32));
-    CUDA_TRY(cudaMalloc(&e->d_chunks, sizeof(ChunkDesc) * B));
-    CUDA_TRY(cudaMalloc(&e->d_tcount, sizeof(int32_t) * ((size_t)cfg.max_templates + 1)));
-    CUDA_TRY(cudaMemset(e->d_tcount, 0, sizeof(int32_t) * ((size_t)cfg.max_templates + 1)));
-    CUDA_TRY(cudaMalloc(&e->d_tbase, sizeof(int32_t) * ((size_t)cfg.max_templates + 1)));
-    CUDA_TRY(cudaMalloc(&e->d_rank, sizeof(int32_t) * B));
-    CUDA_TRY(cudaMalloc(&e->d_hints, sizeof(TemplateHints) * (size_t)cfg.max_templates));
-    CUDA_TRY(cudaMemset(e->d_hints, 0, sizeof(TemplateHints) * (size_t)cfg.max_templates));
-    CUDA_TRY(cudaMalloc(&e->d_hint_jct, sizeof(double) * (size_t)cfg.max_templates));
-    CUDA_TRY(cudaMemset(e->d_hint_jct, 0, sizeof(double) * (size_t)cfg.max_templates));
-    CUDA_TRY(cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking));
-    CUDA_TRY(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
-    CUDA_TRY(cudaMalloc(&e->d_counters, sizeof(Counters)));
-    CUDA_TRY(cudaMemset(e->d_counters, 0, sizeof(Counters)));
-    CUDA_TRY(cudaMalloc(&e->d_stats, sizeof(MemoStats)));
-    CUDA_TRY(cudaMemset(e->d_stats, 0, sizeof(MemoStats)));
-    CUDA_TRY(cudaMalloc(&e->d_actions, sizeof(ramp_action_t) * B));
-    CUDA_TRY(cudaMalloc(&e->d_step_stats, sizeof(double) * RAMP_STEP_STATS_LEN * B));
-    CUDA_TRY(cudaMalloc(&e->d_n_cluster_steps, sizeof(int32_t) * B));
-    CUDA_TRY(cudaMalloc(&e->d_ep_export, sizeof(double) * RAMP_EP_LEN * B));
-    CUDA_TRY(cudaMalloc(&e->d_es_export, sizeof(double) * RAMP_ES_LEN * B));
-    CUDA_TRY(cudaMallocHost(&e->h_n_work, sizeof(int32_t) * 4));
+    CUDA_TRY(alloc_each(B, e->d_items, e->d_items_big, e->d_items_res, e->d_chunks, e->d_rank, e->d_actions, e->d_n_cluster_steps));
+    CUDA_TRY(e->d_chunk_items.alloc((size_t)B * 32));
+    CUDA_TRY(alloc_each((size_t)cfg.max_templates + 1, e->d_tcount, e->d_tbase));
+    CUDA_TRY(cudaMemset(e->d_tcount.get(), 0, sizeof(int32_t) * ((size_t)cfg.max_templates + 1)));
+    CUDA_TRY(e->d_hints.alloc(cfg.max_templates));
+    CUDA_TRY(cudaMemset(e->d_hints.get(), 0, sizeof(TemplateHints) * (size_t)cfg.max_templates));
+    CUDA_TRY(e->d_hint_jct.alloc(cfg.max_templates));
+    CUDA_TRY(cudaMemset(e->d_hint_jct.get(), 0, sizeof(double) * (size_t)cfg.max_templates));
+    CUDA_TRY(create(e->stream2, cudaStreamNonBlocking));
+    CUDA_TRY(create(e->ev_fork, cudaEventDisableTiming));
+    CUDA_TRY(create(e->ev_join, cudaEventDisableTiming));
+    CUDA_TRY(alloc_each(1, e->d_counters, e->d_stats));
+    CUDA_TRY(cudaMemset(e->d_counters.get(), 0, sizeof(Counters)));
+    CUDA_TRY(cudaMemset(e->d_stats.get(), 0, sizeof(MemoStats)));
+    CUDA_TRY(e->d_step_stats.alloc((size_t)RAMP_STEP_STATS_LEN * B));
+    CUDA_TRY(e->d_ep_export.alloc((size_t)RAMP_EP_LEN * B));
+    CUDA_TRY(e->d_es_export.alloc((size_t)RAMP_ES_LEN * B));
+    CUDA_TRY(e->h_n_work.alloc(4));
 
     EpisodeState& ep = e->ep;
     ep.B = B; ep.max_running = cfg.max_running; ep.max_jobs = cfg.max_jobs; ep.n_jobs = 0;
     ep.n_cluster_workers = cfg.n_cluster_workers; ep.queue_capacity = cfg.job_queue_capacity;
     ep.eps = cfg.machine_epsilon; ep.max_sim_time = cfg.max_simulation_run_time;
-    CUDA_TRY(cudaMalloc(&ep.ef, sizeof(double) * EF_COUNT * B));
-    CUDA_TRY(cudaMalloc(&ep.ei, sizeof(int32_t) * EI_COUNT * B));
-    CUDA_TRY(cudaMalloc(&ep.rf, sizeof(double) * RF_COUNT * (size_t)cfg.max_running * B));
-    CUDA_TRY(cudaMalloc(&ep.ri, sizeof(int32_t) * RI_COUNT * (size_t)cfg.max_running * B));
-    CUDA_TRY(cudaMalloc(&ep.rec, sizeof(ramp_job_record_t) * (size_t)cfg.max_jobs * B));
-    CUDA_TRY(cudaMalloc(&e->d_arrivals, sizeof(ramp_arrival_t) * (size_t)cfg.max_jobs * B));
+    CUDA_TRY(e->ep_ef.alloc((size_t)EF_COUNT * B));
+    CUDA_TRY(e->ep_ei.alloc((size_t)EI_COUNT * B));
+    CUDA_TRY(e->ep_rf.alloc((size_t)RF_COUNT * cfg.max_running * B));
+    CUDA_TRY(e->ep_ri.alloc((size_t)RI_COUNT * cfg.max_running * B));
+    CUDA_TRY(e->ep_rec.alloc((size_t)cfg.max_jobs * B));
+    CUDA_TRY(e->d_arrivals.alloc((size_t)cfg.max_jobs * B));
+    ep.ef = e->ep_ef.get(); ep.ei = e->ep_ei.get(); ep.rf = e->ep_rf.get(); ep.ri = e->ep_ri.get(); ep.rec = e->ep_rec.get();
     CUDA_TRY(cudaMemset(ep.ef, 0, sizeof(double) * EF_COUNT * B));
     CUDA_TRY(cudaMemset(ep.ei, 0, sizeof(int32_t) * EI_COUNT * B));
     CUDA_TRY(cudaMemset(ep.rec, 0, sizeof(ramp_job_record_t) * (size_t)cfg.max_jobs * B));
-    ep.arr = e->d_arrivals;
-    CUDA_TRY(cudaMalloc(&e->d_n_jobs_ep, sizeof(int32_t) * B));
-    CUDA_TRY(cudaMemset(e->d_n_jobs_ep, 0, sizeof(int32_t) * B));
-    ep.n_jobs_ep = e->d_n_jobs_ep;
+    ep.arr = e->d_arrivals.get();
+    CUDA_TRY(e->d_n_jobs_ep.alloc(B));
+    CUDA_TRY(cudaMemset(e->d_n_jobs_ep.get(), 0, sizeof(int32_t) * B));
+    ep.n_jobs_ep = e->d_n_jobs_ep.get();
 
     for (int k = 0; k < MAX_EVENT_PAIRS; ++k) {
-        CUDA_TRY(cudaEventCreate(&e->ev_a[k]));
-        CUDA_TRY(cudaEventCreate(&e->ev_b[k]));
+        CUDA_TRY(create(e->ev_a[k], cudaEventDefault));
+        CUDA_TRY(create(e->ev_b[k], cudaEventDefault));
     }
-    *out = e;
+    *out = e.release();
     return RAMP_OK;
 }
 
 int ramp_engine_destroy(ramp_engine_t* e) {
     if (!e) return RAMP_OK;
     cudaSetDevice(e->cfg.device);
-    cudaStreamSynchronize(e->stream);
-    for (auto& t : e->templates) { cudaFree(t.blob); cudaFree(t.res_blob); }
-    for (void* pa : e->env_allocs) cudaFree(pa);
-    cudaFree(e->ep.tick_util); cudaFree(e->ep.tick_util_n);
-    if (e->env_h_need) cudaFreeHost(e->env_h_need);
-    if (e->env_h_mirror) cudaFreeHost(e->env_h_mirror);
-    cudaFree(e->d_items_res); cudaFree(e->d_chunk_items); cudaFree(e->d_chunks); cudaFree(e->d_tcount); cudaFree(e->d_tbase); cudaFree(e->d_rank); cudaFree(e->d_hints); cudaFree(e->d_hint_jct);
-    cudaFree(e->d_res_scratch); cudaFree(e->sa_chunk_items); cudaFree(e->sa_chunks); cudaFree(e->sa_rank);
-    cudaFree(e->d_templates); cudaFree(e->d_memo_keys); cudaFree(e->d_memo_vals); cudaFree(e->d_memo_keys2);
-    free_result_slots(e->res); free_result_slots(e->sa_res);
-    cudaFree(e->pool.n_active); cudaFree(e->pool.tick); cudaFree(e->pool.top);
-    cudaFree(e->d_items); cudaFree(e->d_items_big); cudaStreamDestroy(e->stream2); cudaEventDestroy(e->ev_fork); cudaEventDestroy(e->ev_join); cudaFree(e->d_counters); cudaFree(e->d_stats); cudaFree(e->d_actions);
-    cudaFree(e->d_step_stats); cudaFree(e->d_n_cluster_steps); cudaFree(e->d_ep_export); cudaFree(e->d_es_export);
-    cudaFree(e->ep.ef); cudaFree(e->ep.ei); cudaFree(e->ep.rf); cudaFree(e->ep.ri); cudaFree(e->ep.rec);
-    cudaFree(e->d_arrivals); cudaFree(e->d_n_jobs_ep); cudaFree(e->d_scratch); cudaFree(e->sa_items); cudaFree(e->sa_counters); cudaFreeHost(e->h_n_work);
-    for (int k = 0; k < MAX_EVENT_PAIRS; ++k) { cudaEventDestroy(e->ev_a[k]); cudaEventDestroy(e->ev_b[k]); }
-    cudaStreamDestroy(e->stream);
+    cudaStreamSynchronize(e->stream.get());
     delete e;
     return RAMP_OK;
 }
 
-void* ramp_engine_stream(ramp_engine_t* e) { return e ? (void*)e->stream : nullptr; }
+void* ramp_engine_stream(ramp_engine_t* e) { return e ? (void*)e->stream.get() : nullptr; }
 
 int ramp_template_count(ramp_engine_t* e) { return e ? (int)e->templates.size() : 0; }
 
@@ -820,9 +778,9 @@ int ramp_register_template(ramp_engine_t* e, const ramp_lowered_job_t* j, int32_
         if (e->templates[t].hash == ht.hash && e->templates[t].bytes == ht.bytes) { canon = e->templates[t].dev.canon_id; break; }
 
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    CUDA_TRY(cudaMalloc(&ht.blob, total));
-    CUDA_TRY(cudaMemcpy(ht.blob, ht.bytes.data(), total, cudaMemcpyHostToDevice));
-    unsigned char* base = (unsigned char*)ht.blob;
+    CUDA_TRY(ht.blob.alloc(total));
+    CUDA_TRY(cudaMemcpy(ht.blob.get(), ht.bytes.data(), total, cudaMemcpyHostToDevice));
+    unsigned char* base = ht.blob.get();
     TemplateDev& d = ht.dev;
     d.n_ops = N; d.n_deps = E; d.n_workers = W; d.n_channels = C;
     d.num_training_steps = j->num_training_steps; d.model_id = j->model_id; d.degree = j->degree;
@@ -841,13 +799,13 @@ int ramp_register_template(ramp_engine_t* e, const ramp_lowered_job_t* j, int32_
     if (e->mode == 0) {
         ramp_quotient_t q{};
         const int qrc = e->use_quotient ? ramp_quotient_template(j, &q) : identity_quotient(j, &q);
-        if (qrc != RAMP_OK) { cudaFree(ht.blob); return set_error(qrc, "ramp_quotient_template failed (%d)", qrc); }
+        if (qrc != RAMP_OK) return set_error(qrc, "ramp_quotient_template failed (%d)", qrc);
         std::vector<unsigned char> rblob;
         if (build_resident_blob(j, q, RESIDENT_MAX_BYTES, rblob)) {
-            cudaError_t ce = cudaMalloc(&ht.res_blob, rblob.size());
-            if (ce == cudaSuccess) ce = cudaMemcpy(ht.res_blob, rblob.data(), rblob.size(), cudaMemcpyHostToDevice);
-            if (ce != cudaSuccess) { ramp_free_quotient(&q); cudaFree(ht.blob); return set_error(RAMP_ERR_CUDA, "resident blob upload failed: %s", cudaGetErrorString(ce)); }
-            d.res_blob = (const unsigned char*)ht.res_blob; d.res_bytes = (int32_t)rblob.size();
+            cudaError_t ce = ht.res_blob.alloc(rblob.size());
+            if (ce == cudaSuccess) ce = cudaMemcpy(ht.res_blob.get(), rblob.data(), rblob.size(), cudaMemcpyHostToDevice);
+            if (ce != cudaSuccess) { ramp_free_quotient(&q); return set_error(RAMP_ERR_CUDA, "resident blob upload failed: %s", cudaGetErrorString(ce)); }
+            d.res_blob = ht.res_blob.get(); d.res_bytes = (int32_t)rblob.size();
             d.res_n_ops = q.n_ops; d.res_n_deps = q.n_deps;
             d.size_class = 2;
             e->res_tmpl_cap = std::max(e->res_tmpl_cap, (int32_t)align_up((uint64_t)rblob.size(), 128));
@@ -859,9 +817,9 @@ int ramp_register_template(ramp_engine_t* e, const ramp_lowered_job_t* j, int32_
                               N, E, W, C, q.n_ops, q.n_deps, q.n_workers, q.n_channels, d.res_blob ? "resident" : "not resident", rblob.size());
         ramp_free_quotient(&q);
     }
-    if (d.size_class == 2) e->n_resident++; else e->n_nonresident++;
     const int32_t id = (int32_t)e->templates.size();
-    CUDA_TRY(cudaMemcpy(e->d_templates + id, &d, sizeof(TemplateDev), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(e->d_templates.get() + id, &d, sizeof(TemplateDev), cudaMemcpyHostToDevice));
+    if (d.size_class == 2) e->n_resident++; else e->n_nonresident++;
     if (d.size_class != 2) {       // the warp / CTA kernels' slabs and shared-memory tables are sized by the jobs that use them
         e->max_scratch = std::max(e->max_scratch, d.scratch_bytes);
         e->max_w = std::max(e->max_w, W);
@@ -879,29 +837,29 @@ int ramp_reset(ramp_engine_t* e, const ramp_arrival_t* arrivals, int32_t n_jobs)
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     const int B = e->cfg.n_episodes;
     if (n_jobs == e->cfg.max_jobs) {
-        CUDA_TRY(cudaMemcpyAsync(e->d_arrivals, arrivals, sizeof(ramp_arrival_t) * (size_t)n_jobs * B, cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(e->d_arrivals.get(), arrivals, sizeof(ramp_arrival_t) * (size_t)n_jobs * B, cudaMemcpyHostToDevice, e->stream.get()));
     } else {
-        CUDA_TRY(cudaMemcpy2DAsync(e->d_arrivals, sizeof(ramp_arrival_t) * (size_t)e->cfg.max_jobs, arrivals,
+        CUDA_TRY(cudaMemcpy2DAsync(e->d_arrivals.get(), sizeof(ramp_arrival_t) * (size_t)e->cfg.max_jobs, arrivals,
                                    sizeof(ramp_arrival_t) * (size_t)n_jobs, sizeof(ramp_arrival_t) * (size_t)n_jobs, B,
-                                   cudaMemcpyHostToDevice, e->stream));
+                                   cudaMemcpyHostToDevice, e->stream.get()));
     }
     e->ep.n_jobs = n_jobs;
     {
         std::vector<int32_t> nj(B, n_jobs);
-        CUDA_TRY(cudaMemcpyAsync(e->d_n_jobs_ep, nj.data(), sizeof(int32_t) * B, cudaMemcpyHostToDevice, e->stream));
-        CUDA_TRY(cudaStreamSynchronize(e->stream));     // nj goes out of scope
+        CUDA_TRY(cudaMemcpyAsync(e->d_n_jobs_ep.get(), nj.data(), sizeof(int32_t) * B, cudaMemcpyHostToDevice, e->stream.get()));
+        CUDA_TRY(cudaStreamSynchronize(e->stream.get()));     // nj goes out of scope
     }
     // memo is per env instance per episode: cleared on reset (RCE:269-275)
-    CUDA_TRY(cudaMemsetAsync(e->d_memo_keys, 0, sizeof(unsigned long long) * e->memo_cap, e->stream));
+    CUDA_TRY(cudaMemsetAsync(e->d_memo_keys.get(), 0, sizeof(unsigned long long) * e->memo_cap, e->stream.get()));
     // the batch-wide cache of RAMP_MEMO_SHARED (level-2 keys, its result slots and traces) is a pure function of the
     // lowered job and survives the reset; every other mode starts from an empty trace pool
-    if (e->cfg.memo_mode != RAMP_MEMO_SHARED) CUDA_TRY(cudaMemsetAsync(e->pool.top, 0, sizeof(unsigned long long), e->stream));
-    CUDA_TRY(cudaMemcpyAsync(&e->memo_base, e->d_stats, sizeof(MemoStats), cudaMemcpyDeviceToHost, e->stream));   // counters stay cumulative
-    CUDA_TRY(cudaMemsetAsync(e->d_counters, 0, sizeof(Counters), e->stream));
-    ramp_reset_kernel<<<(B + 127) / 128, 128, 0, e->stream>>>(e->ep);
+    if (e->cfg.memo_mode != RAMP_MEMO_SHARED) CUDA_TRY(cudaMemsetAsync(e->pool.top.get(), 0, sizeof(unsigned long long), e->stream.get()));
+    CUDA_TRY(cudaMemcpyAsync(&e->memo_base, e->d_stats.get(), sizeof(MemoStats), cudaMemcpyDeviceToHost, e->stream.get()));   // counters stay cumulative
+    CUDA_TRY(cudaMemsetAsync(e->d_counters.get(), 0, sizeof(Counters), e->stream.get()));
+    ramp_reset_kernel<<<(B + 127) / 128, 128, 0, e->stream.get()>>>(e->ep);
     e->launches++;
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     return RAMP_OK;
 }
 
@@ -910,9 +868,9 @@ int ramp_set_arrivals(ramp_engine_t* e, int32_t episode, int32_t first_job, cons
     if (episode < 0 || episode >= e->cfg.n_episodes || first_job < 0 || n < 0 || first_job + n > e->cfg.max_jobs)
         return set_error(RAMP_ERR_BAD_ARG, "arrival rows [%d, %d) of episode %d out of range (max_jobs=%d)", first_job, first_job + n, episode, e->cfg.max_jobs);
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    CUDA_TRY(cudaMemcpyAsync(e->d_arrivals + (size_t)episode * e->cfg.max_jobs + first_job, rows, sizeof(ramp_arrival_t) * (size_t)n,
-                             cudaMemcpyHostToDevice, e->stream));
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaMemcpyAsync(e->d_arrivals.get() + (size_t)episode * e->cfg.max_jobs + first_job, rows, sizeof(ramp_arrival_t) * (size_t)n,
+                             cudaMemcpyHostToDevice, e->stream.get()));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     return RAMP_OK;
 }
 
@@ -922,8 +880,8 @@ int ramp_set_job_count(ramp_engine_t* e, int32_t episode, int32_t n_jobs) {
         return set_error(n_jobs > e->cfg.max_jobs ? RAMP_ERR_CAPACITY : RAMP_ERR_BAD_ARG,
                          "job count %d of episode %d out of range (max_jobs=%d)", n_jobs, episode, e->cfg.max_jobs);
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    CUDA_TRY(cudaMemcpyAsync(e->d_n_jobs_ep + episode, &n_jobs, sizeof(int32_t), cudaMemcpyHostToDevice, e->stream));
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaMemcpyAsync(e->d_n_jobs_ep.get() + episode, &n_jobs, sizeof(int32_t), cudaMemcpyHostToDevice, e->stream.get()));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     return RAMP_OK;
 }
 
@@ -942,38 +900,38 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
     if (e->n_nonresident > 0) { int rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
     if (e->n_resident > 0) { int rc = ensure_thread_scratch(e); if (rc != RAMP_OK) return rc; }
     const int B = e->cfg.n_episodes;
-    cudaStream_t st = e->stream;
-    CUDA_TRY(cudaMemsetAsync(e->d_counters, 0, 4 * sizeof(int32_t), st));   // both work lists' counts and cursors
+    cudaStream_t st = e->stream.get();
+    CUDA_TRY(cudaMemsetAsync(e->d_counters.get(), 0, 4 * sizeof(int32_t), st));   // both work lists' counts and cursors
     PlanArgs p{};
-    p.actions = d_actions; p.templates = e->d_templates; p.n_templates = (int32_t)e->templates.size();
-    p.ep = e->ep; p.memo.keys = e->d_memo_keys; p.memo.mask = e->memo_cap - 1; p.memo.mode = e->cfg.memo_mode;
-    p.memo.vals = e->d_memo_vals; p.memo.keys2 = e->d_memo_keys2; p.memo.mask2 = e->memo_cap2 - 1;
+    p.actions = d_actions; p.templates = e->d_templates.get(); p.n_templates = (int32_t)e->templates.size();
+    p.ep = e->ep; p.memo.keys = e->d_memo_keys.get(); p.memo.mask = e->memo_cap - 1; p.memo.mode = e->cfg.memo_mode;
+    p.memo.vals = e->d_memo_vals.get(); p.memo.keys2 = e->d_memo_keys2.get(); p.memo.mask2 = e->memo_cap2 - 1;
     p.memo.slot2_base = (int32_t)e->memo_cap + e->cfg.n_episodes;
-    p.items = e->d_items; p.items_big = e->d_items_big; p.items_res = e->d_items_res; p.counters = e->d_counters; p.stats = e->d_stats;
+    p.items = e->d_items.get(); p.items_big = e->d_items_big.get(); p.items_res = e->d_items_res.get(); p.counters = e->d_counters.get(); p.stats = e->d_stats.get();
     ramp_plan_kernel<<<(B + 127) / 128, 128, 0, st>>>(p);
     e->launches++;
     if (!e->templates.empty()) {
         if (e->ev_pending >= MAX_EVENT_PAIRS) { CUDA_TRY(cudaStreamSynchronize(st)); int rc = resolve_events(e); if (rc) return rc; }
-        CUDA_TRY(cudaEventRecord(e->ev_a[e->ev_pending], st));
+        CUDA_TRY(cudaEventRecord(e->ev_a[e->ev_pending].get(), st));
         // memo misses on resident templates: one THREAD per lookahead, grouped on the device.  Their count stays there: idle
         // CTAs find the chunk cursor exhausted and exit.
-        if (e->n_resident > 0) bucket_resident(e, e->d_items_res, e->d_counters, e->d_chunk_items, e->d_chunks, e->d_rank, st);
+        if (e->n_resident > 0) bucket_resident(e, e->d_items_res.get(), e->d_counters.get(), e->d_chunk_items.get(), e->d_chunks.get(), e->d_rank.get(), st);
         int n_small = 0, n_big = 0;
         if (e->n_nonresident > 0) {
             // the number of memo misses of each size class decides the kernel shapes: a 16-byte read-back (~10 us) against
             // multi-ms kernels
-            CUDA_TRY(cudaMemcpyAsync(e->h_n_work, &e->d_counters->n_work, sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(e->h_n_work.get(), &e->d_counters.get()->n_work, sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));
-            n_small = e->h_n_work[0]; n_big = e->h_n_work[2];
+            n_small = e->h_n_work.get()[0]; n_big = e->h_n_work.get()[2];
         }
-        int rc = launch_lookaheads(e, e->d_chunks, e->d_chunk_items, e->n_resident > 0 ? e->res_grid : 0, e->d_items, n_small,
-                                   e->d_items_big, n_big, e->d_counters, e->res, e->pool, e->d_stats, st);
+        int rc = launch_lookaheads(e, e->d_chunks.get(), e->d_chunk_items.get(), e->n_resident > 0 ? e->res_grid : 0, e->d_items.get(), n_small,
+                                   e->d_items_big.get(), n_big, e->d_counters.get(), e->res.view(), e->pool.view(), e->d_stats.get(), st);
         if (rc != RAMP_OK) return rc;
-        CUDA_TRY(cudaEventRecord(e->ev_b[e->ev_pending], st));
+        CUDA_TRY(cudaEventRecord(e->ev_b[e->ev_pending].get(), st));
         e->ev_pending++;
     }
     StepArgs s{};
-    s.actions = d_actions; s.ep = e->ep; s.res = e->res; s.pool = e->pool; s.counters = e->d_counters;
+    s.actions = d_actions; s.ep = e->ep; s.res = e->res.view(); s.pool = e->pool.view(); s.counters = e->d_counters.get();
     s.stats_out = d_stats_out; s.n_cluster_steps_out = d_ncs_out; s.fuse_empty_steps = fuse;
     ramp_step_kernel<<<(B + 63) / 64, 64, 0, st>>>(s);
     e->launches++;
@@ -983,7 +941,7 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
 
 int ramp_sync(ramp_engine_t* e) {
     if (!e) return set_error(RAMP_ERR_BAD_ARG, "null engine");
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     return resolve_events(e);
 }
 
@@ -991,26 +949,26 @@ int ramp_step_host(ramp_engine_t* e, const ramp_action_t* actions, int32_t fuse,
     if (!e || !actions) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     const int B = e->cfg.n_episodes;
-    CUDA_TRY(cudaMemcpyAsync(e->d_actions, actions, sizeof(ramp_action_t) * B, cudaMemcpyHostToDevice, e->stream));
-    int rc = ramp_step_device(e, e->d_actions, fuse, stats_out ? e->d_step_stats : nullptr, ncs_out ? e->d_n_cluster_steps : nullptr);
+    CUDA_TRY(cudaMemcpyAsync(e->d_actions.get(), actions, sizeof(ramp_action_t) * B, cudaMemcpyHostToDevice, e->stream.get()));
+    int rc = ramp_step_device(e, e->d_actions.get(), fuse, stats_out ? e->d_step_stats.get() : nullptr, ncs_out ? e->d_n_cluster_steps.get() : nullptr);
     if (rc != RAMP_OK) return rc;
     if (stats_out)
-        CUDA_TRY(cudaMemcpyAsync(stats_out, e->d_step_stats, sizeof(double) * RAMP_STEP_STATS_LEN * B, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(stats_out, e->d_step_stats.get(), sizeof(double) * RAMP_STEP_STATS_LEN * B, cudaMemcpyDeviceToHost, e->stream.get()));
     if (ncs_out)
-        CUDA_TRY(cudaMemcpyAsync(ncs_out, e->d_n_cluster_steps, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(ncs_out, e->d_n_cluster_steps.get(), sizeof(int32_t) * B, cudaMemcpyDeviceToHost, e->stream.get()));
     return ramp_sync(e);
 }
 
 int ramp_check_status(ramp_engine_t* e, int32_t* ep_out, int32_t* st_out) {
     if (!e) return set_error(RAMP_ERR_BAD_ARG, "null engine");
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     Counters c{};
-    CUDA_TRY(cudaMemcpy(&c, e->d_counters, sizeof(Counters), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&c, e->d_counters.get(), sizeof(Counters), cudaMemcpyDeviceToHost));
     if (c.err_episode == 0) { if (ep_out) *ep_out = -1; if (st_out) *st_out = 0; return RAMP_OK; }
     const int b = c.err_episode - 1;
     int32_t st = 0;
     CUDA_TRY(cudaMemcpy(&st, e->ep.ei + (size_t)EI_STATUS * e->cfg.n_episodes + b, sizeof(int32_t), cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemset(&e->d_counters->err_episode, 0, sizeof(int32_t)));
+    CUDA_TRY(cudaMemset(&e->d_counters.get()->err_episode, 0, sizeof(int32_t)));
     if (ep_out) *ep_out = b;
     if (st_out) *st_out = st;
     const char* what = st == RAMP_ST_INFINITE_TICK ? "ERROR: Last tick was infinite, a bug has occurred somewhere."
@@ -1024,7 +982,7 @@ int ramp_check_status(ramp_engine_t* e, int32_t* ep_out, int32_t* st_out) {
 
 int ramp_get_job_records(ramp_engine_t* e, ramp_job_record_t* out) {
     if (!e || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     CUDA_TRY(cudaMemcpy(out, e->ep.rec, sizeof(ramp_job_record_t) * (size_t)e->cfg.max_jobs * e->cfg.n_episodes, cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
@@ -1032,17 +990,17 @@ int ramp_get_job_records(ramp_engine_t* e, ramp_job_record_t* out) {
 int ramp_episode_state_device(ramp_engine_t* e, double** d_out) {
     if (!e || !d_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     const int B = e->cfg.n_episodes;
-    ramp_export_episode_state_kernel<<<(B + 127) / 128, 128, 0, e->stream>>>(e->ep, e->d_ep_export);
+    ramp_export_episode_state_kernel<<<(B + 127) / 128, 128, 0, e->stream.get()>>>(e->ep, e->d_ep_export.get());
     e->launches++;
     CUDA_TRY(cudaGetLastError());
-    *d_out = e->d_ep_export;
+    *d_out = e->d_ep_export.get();
     return RAMP_OK;
 }
 
 int ramp_export_episode_state_to(ramp_engine_t* e, double* d_dst) {
     if (!e || !d_dst) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     const int B = e->cfg.n_episodes;
-    ramp_export_episode_state_kernel<<<(B + 127) / 128, 128, 0, e->stream>>>(e->ep, d_dst);
+    ramp_export_episode_state_kernel<<<(B + 127) / 128, 128, 0, e->stream.get()>>>(e->ep, d_dst);
     e->launches++;
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
@@ -1052,16 +1010,16 @@ int ramp_get_episode_state(ramp_engine_t* e, double* out) {
     double* d = nullptr;
     int rc = ramp_episode_state_device(e, &d);
     if (rc != RAMP_OK) return rc;
-    CUDA_TRY(cudaMemcpyAsync(out, d, sizeof(double) * RAMP_EP_LEN * e->cfg.n_episodes, cudaMemcpyDeviceToHost, e->stream));
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaMemcpyAsync(out, d, sizeof(double) * RAMP_EP_LEN * e->cfg.n_episodes, cudaMemcpyDeviceToHost, e->stream.get()));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     return RAMP_OK;
 }
 
 int ramp_get_memo_stats(ramp_engine_t* e, int64_t* lookups, int64_t* hits, int64_t* lookaheads) {
     if (!e) return set_error(RAMP_ERR_BAD_ARG, "null engine");
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     MemoStats s{};
-    CUDA_TRY(cudaMemcpy(&s, e->d_stats, sizeof(MemoStats), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&s, e->d_stats.get(), sizeof(MemoStats), cudaMemcpyDeviceToHost));
     if (lookups) *lookups = (int64_t)(s.lookups - e->memo_base.lookups);
     if (hits) *hits = (int64_t)(s.hits - e->memo_base.hits);
     if (lookaheads) *lookaheads = (int64_t)(s.lookaheads - e->memo_base.lookaheads);
@@ -1070,9 +1028,9 @@ int ramp_get_memo_stats(ramp_engine_t* e, int64_t* lookups, int64_t* hits, int64
 
 int ramp_get_memo_stats_ex(ramp_engine_t* e, int64_t out[4]) {
     if (!e || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     MemoStats s{};
-    CUDA_TRY(cudaMemcpy(&s, e->d_stats, sizeof(MemoStats), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&s, e->d_stats.get(), sizeof(MemoStats), cudaMemcpyDeviceToHost));
     out[0] = (int64_t)(s.lookups - e->memo_base.lookups);
     out[1] = (int64_t)(s.hits - e->memo_base.hits);
     out[2] = (int64_t)(s.shared_hits - e->memo_base.shared_hits);
@@ -1083,21 +1041,21 @@ int ramp_get_memo_stats_ex(ramp_engine_t* e, int64_t out[4]) {
 int ramp_get_last_lookahead(ramp_engine_t* e, int32_t episode, ramp_lookahead_result_t* res, int32_t* tn, double* tt, int32_t cap) {
     if (!e || !res) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     if (episode < 0 || episode >= e->cfg.n_episodes) return set_error(RAMP_ERR_BAD_ARG, "episode out of range");
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     int32_t slot = -1;
     CUDA_TRY(cudaMemcpy(&slot, e->ep.ei + (size_t)EI_LAST_SLOT * e->cfg.n_episodes + episode, sizeof(int32_t), cudaMemcpyDeviceToHost));
     if (slot < 0) return set_error(RAMP_ERR_BAD_ARG, "episode %d has not mounted a job yet", episode);
     int64_t off = -1;
-    CUDA_TRY(cudaMemcpy(&res->jct, e->res.jct + slot, sizeof(double), cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&res->comm, e->res.comm + slot, sizeof(double), cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&res->comp, e->res.comp + slot, sizeof(double), cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&res->n_ticks, e->res.n_ticks + slot, sizeof(int32_t), cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&res->status, e->res.status + slot, sizeof(int32_t), cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&off, e->res.trace_off + slot, sizeof(int64_t), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&res->jct, e->res.jct.get() + slot, sizeof(double), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&res->comm, e->res.comm.get() + slot, sizeof(double), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&res->comp, e->res.comp.get() + slot, sizeof(double), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&res->n_ticks, e->res.n_ticks.get() + slot, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&res->status, e->res.status.get() + slot, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&off, e->res.trace_off.get() + slot, sizeof(int64_t), cudaMemcpyDeviceToHost));
     if (tn && tt && off >= 0) {
         const int32_t n = std::min(std::min(res->n_ticks, cap), e->cfg.trace_cap);
-        CUDA_TRY(cudaMemcpy(tn, e->pool.n_active + off, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
-        CUDA_TRY(cudaMemcpy(tt, e->pool.tick + off, sizeof(double) * n, cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(tn, e->pool.n_active.get() + off, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(tt, e->pool.tick.get() + off, sizeof(double) * n, cudaMemcpyDeviceToHost));
     }
     return RAMP_OK;
 }
@@ -1106,12 +1064,12 @@ int ramp_debug_template_info(ramp_engine_t* e, int32_t template_id, int32_t out[
     if (!e || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     if (template_id < 0 || template_id >= (int32_t)e->templates.size()) return set_error(RAMP_ERR_BAD_ARG, "template id %d is not registered", template_id);
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     const TemplateDev& d = e->templates[template_id].dev;
     TemplateHints h{};
     double hj = 0.0;
-    CUDA_TRY(cudaMemcpy(&h, e->d_hints + template_id, sizeof(TemplateHints), cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&hj, e->d_hint_jct + template_id, sizeof(double), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&h, e->d_hints.get() + template_id, sizeof(TemplateHints), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&hj, e->d_hint_jct.get() + template_id, sizeof(double), cudaMemcpyDeviceToHost));
     out[0] = d.size_class; out[1] = d.res_n_ops; out[2] = d.res_n_deps;
     out[3] = h.n_ticks; out[4] = h.max_o; out[5] = h.max_f; out[6] = h.max_nf;
     if (hint_jct) *hint_jct = hj;
@@ -1140,59 +1098,52 @@ int ramp_run_lookaheads(ramp_engine_t* e, const int32_t* template_ids, int32_t n
     int rc = RAMP_OK;
     if (n_small + n_big > 0) { rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
     if (n_res > 0) { rc = ensure_thread_scratch(e); if (rc != RAMP_OK) return rc; }
-    cudaStream_t st = e->stream;
+    cudaStream_t st = e->stream.get();
     if (n > e->sa_cap) {
         CUDA_TRY(cudaStreamSynchronize(st));
-        free_result_slots(e->sa_res); cudaFree(e->sa_items); cudaFree(e->sa_rank); cudaFree(e->sa_chunk_items); cudaFree(e->sa_chunks);
-        if (alloc_result_slots(e->sa_res, n) != RAMP_OK) return RAMP_ERR_CUDA;
-        CUDA_TRY(cudaMalloc(&e->sa_items, sizeof(WorkItem) * n));
-        CUDA_TRY(cudaMalloc(&e->sa_rank, sizeof(int32_t) * n));
-        CUDA_TRY(cudaMalloc(&e->sa_chunk_items, sizeof(WorkItem) * (size_t)n * 32));
-        CUDA_TRY(cudaMalloc(&e->sa_chunks, sizeof(ChunkDesc) * n));
+        e->sa_cap = 0;                  // until every buffer has the new size
+        CUDA_TRY(alloc_each(n, e->sa_res, e->sa_items, e->sa_rank, e->sa_chunks));
+        CUDA_TRY(e->sa_chunk_items.alloc((size_t)n * 32));
         e->sa_cap = n;
     }
-    if (!e->sa_counters) CUDA_TRY(cudaMalloc(&e->sa_counters, sizeof(Counters)));
+    if (!e->sa_counters.get()) CUDA_TRY(e->sa_counters.alloc(1));
     std::vector<WorkItem> items;
     items.reserve(n);
     for (const auto& l : lists) items.insert(items.end(), l.begin(), l.end());
-    WorkItem* const d_small = e->sa_items;
+    WorkItem* const d_small = e->sa_items.get();
     WorkItem* const d_big = d_small + n_small;
     WorkItem* const d_res = d_big + n_big;
     Counters c{}; c.n_work = n_small; c.n_work_big = n_big; c.n_work_res = n_res;
-    CUDA_TRY(cudaMemcpyAsync(e->sa_items, items.data(), sizeof(WorkItem) * n, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(e->sa_counters, &c, sizeof(Counters), cudaMemcpyHostToDevice, st));
-    if (n_res > 0) bucket_resident(e, d_res, e->sa_counters, e->sa_chunk_items, e->sa_chunks, e->sa_rank, st);
+    CUDA_TRY(cudaMemcpyAsync(e->sa_items.get(), items.data(), sizeof(WorkItem) * n, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(e->sa_counters.get(), &c, sizeof(Counters), cudaMemcpyHostToDevice, st));
+    if (n_res > 0) bucket_resident(e, d_res, e->sa_counters.get(), e->sa_chunk_items.get(), e->sa_chunks.get(), e->sa_rank.get(), st);
     // traces of standalone runs go to a private pool sized n x trace_cap when requested
-    TracePool priv{};
+    TraceArrays priv;
     const bool want_trace = trace_n && trace_tick && trace_cap > 0;
-    unsigned long long* d_top = nullptr;
     if (want_trace) {
-        priv.len = (uint64_t)n * (uint64_t)e->cfg.trace_cap;      // the kernels allocate n_ticks entries per lookahead; truncated on copy-out
-        CUDA_TRY(cudaMalloc(&priv.n_active, sizeof(int32_t) * priv.len));
-        CUDA_TRY(cudaMalloc(&priv.tick, sizeof(double) * priv.len));
-        CUDA_TRY(cudaMalloc(&d_top, sizeof(unsigned long long)));
-        CUDA_TRY(cudaMemsetAsync(d_top, 0, sizeof(unsigned long long), st));
-        priv.top = d_top;
+        // the kernels allocate n_ticks entries per lookahead; truncated on copy-out
+        CUDA_TRY(priv.alloc((uint64_t)n * (uint64_t)e->cfg.trace_cap));
+        CUDA_TRY(cudaMemsetAsync(priv.top.get(), 0, sizeof(unsigned long long), st));
     }
-    TracePool pool = want_trace ? priv : e->pool;
+    TracePool pool = want_trace ? priv.view() : e->pool.view();
     if (!want_trace) pool.top = nullptr;
-    cudaEvent_t ea = e->ev_a[MAX_EVENT_PAIRS - 1], eb = e->ev_b[MAX_EVENT_PAIRS - 1];
+    cudaEvent_t ea = e->ev_a[MAX_EVENT_PAIRS - 1].get(), eb = e->ev_b[MAX_EVENT_PAIRS - 1].get();
     if (e->ev_pending >= MAX_EVENT_PAIRS - 1) { CUDA_TRY(cudaStreamSynchronize(st)); rc = resolve_events(e); if (rc) return rc; }
     CUDA_TRY(cudaEventRecord(ea, st));
-    rc = launch_lookaheads(e, e->sa_chunks, e->sa_chunk_items, n_res > 0 ? std::min(e->res_grid, n_chunks) : 0, d_small, n_small,
-                           d_big, n_big, e->sa_counters, e->sa_res, pool, nullptr, st);
+    rc = launch_lookaheads(e, e->sa_chunks.get(), e->sa_chunk_items.get(), n_res > 0 ? std::min(e->res_grid, n_chunks) : 0, d_small, n_small,
+                           d_big, n_big, e->sa_counters.get(), e->sa_res.view(), pool, nullptr, st);
     if (rc != RAMP_OK) return rc;
     CUDA_TRY(cudaEventRecord(eb, st));
     CUDA_TRY(cudaGetLastError());
     std::vector<double> jct(n), comm(n), comp(n);
     std::vector<int32_t> nt(n), stt(n);
     std::vector<int64_t> off(n);
-    CUDA_TRY(cudaMemcpyAsync(jct.data(), e->sa_res.jct, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(comm.data(), e->sa_res.comm, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(comp.data(), e->sa_res.comp, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(nt.data(), e->sa_res.n_ticks, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(stt.data(), e->sa_res.status, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(off.data(), e->sa_res.trace_off, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(jct.data(), e->sa_res.jct.get(), sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(comm.data(), e->sa_res.comm.get(), sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(comp.data(), e->sa_res.comp.get(), sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(nt.data(), e->sa_res.n_ticks.get(), sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(stt.data(), e->sa_res.status.get(), sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(off.data(), e->sa_res.trace_off.get(), sizeof(int64_t) * n, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     if (kernel_ms_out) CUDA_TRY(cudaEventElapsedTime(kernel_ms_out, ea, eb));
     for (int32_t k = 0; k < n; ++k) {
@@ -1203,24 +1154,29 @@ int ramp_run_lookaheads(ramp_engine_t* e, const int32_t* template_ids, int32_t n
         for (int32_t k = 0; k < n; ++k) {
             if (off[k] < 0) continue;
             const int32_t m = std::min(std::min(nt[k], trace_cap), e->cfg.trace_cap);
-            CUDA_TRY(cudaMemcpy(trace_n + (size_t)k * trace_cap, priv.n_active + off[k], sizeof(int32_t) * m, cudaMemcpyDeviceToHost));
-            CUDA_TRY(cudaMemcpy(trace_tick + (size_t)k * trace_cap, priv.tick + off[k], sizeof(double) * m, cudaMemcpyDeviceToHost));
+            CUDA_TRY(cudaMemcpy(trace_n + (size_t)k * trace_cap, priv.n_active.get() + off[k], sizeof(int32_t) * m, cudaMemcpyDeviceToHost));
+            CUDA_TRY(cudaMemcpy(trace_tick + (size_t)k * trace_cap, priv.tick.get() + off[k], sizeof(double) * m, cudaMemcpyDeviceToHost));
         }
-        cudaFree(priv.n_active); cudaFree(priv.tick); cudaFree(d_top);
     }
     return RAMP_OK;
 }
 
 int64_t ramp_launch_count(ramp_engine_t* e) { return e ? e->launches : 0; }
 
+int ramp_debug_device_bytes(int64_t* device_bytes, int64_t* pinned_bytes) {
+    if (device_bytes) *device_bytes = g_device_bytes.load();
+    if (pinned_bytes) *pinned_bytes = g_pinned_bytes.load();
+    return RAMP_OK;
+}
+
 int ramp_get_lookahead_kernel_time(ramp_engine_t* e, double* total_ms, int64_t* launches, int64_t* work_items,
                                    int64_t* alg_bytes, int32_t reset) {
     if (!e) return set_error(RAMP_ERR_BAD_ARG, "null engine");
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     int rc = resolve_events(e);
     if (rc) return rc;
     MemoStats s{};
-    CUDA_TRY(cudaMemcpy(&s, e->d_stats, sizeof(MemoStats), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&s, e->d_stats.get(), sizeof(MemoStats), cudaMemcpyDeviceToHost));
     if (total_ms) *total_ms = e->la_ms_total;
     if (launches) *launches = e->la_launches;
     if (work_items) *work_items = (int64_t)(s.lookaheads - e->la_items_base);
@@ -1232,26 +1188,15 @@ int ramp_get_lookahead_kernel_time(ramp_engine_t* e, double* total_ms, int64_t* 
 
 int ramp_get_quotient_bytes(ramp_engine_t* e, int64_t* quotient_bytes) {
     if (!e || !quotient_bytes) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     MemoStats s{};
-    CUDA_TRY(cudaMemcpy(&s, e->d_stats, sizeof(MemoStats), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&s, e->d_stats.get(), sizeof(MemoStats), cudaMemcpyDeviceToHost));
     *quotient_bytes = (int64_t)(s.quotient_bytes - e->la_qbytes_base);
     return RAMP_OK;
 }
 
 
 // ---- device-resident rollouts ---------------------------------------------------------------------------------------
-extern "C++" {
-namespace {
-template <class T> int env_upload(ramp_engine* e, T** dst, const T* src, size_t n) {
-    CUDA_TRY(cudaMalloc(dst, sizeof(T) * std::max<size_t>(n, 1)));
-    e->env_allocs.push_back(*dst);
-    if (src && n) CUDA_TRY(cudaMemcpy(*dst, src, sizeof(T) * n, cudaMemcpyHostToDevice));
-    else CUDA_TRY(cudaMemset(*dst, 0, sizeof(T) * std::max<size_t>(n, 1)));
-    return RAMP_OK;
-}
-}  // namespace
-}  // extern "C++"
 
 int ramp_env_create(ramp_engine_t* e, const ramp_env_config_t* c) {
     if (!e || !c) return set_error(RAMP_ERR_BAD_ARG, "null argument");
@@ -1269,24 +1214,19 @@ int ramp_env_create(ramp_engine_t* e, const ramp_env_config_t* c) {
     v.machine_epsilon = c->machine_epsilon;
     const int n_cand = c->cand_ptr[D + 1];
     int rc;
-    int32_t* cand_ptr; unsigned long long* cand_mask; int32_t* cand_geom; uint8_t* uniform; uint8_t* shape_ok; double* mp; double* jp;
-    if ((rc = env_upload(e, &cand_ptr, c->cand_ptr, (size_t)D + 2))) return rc;
-    if ((rc = env_upload(e, &cand_mask, (const unsigned long long*)c->cand_mask, (size_t)n_cand * nw))) return rc;
-    if ((rc = env_upload(e, &cand_geom, c->cand_geom, (size_t)n_cand))) return rc;
-    if ((rc = env_upload(e, &uniform, c->uniform, (size_t)M * (D + 1)))) return rc;
-    if ((rc = env_upload(e, &shape_ok, c->shape_ok, (size_t)D + 1))) return rc;
-    if ((rc = env_upload(e, &mp, c->model_params, (size_t)M * 5))) return rc;
-    if ((rc = env_upload(e, &jp, c->jobs_params, (size_t)16))) return rc;
-    v.cand_ptr = cand_ptr; v.cand_mask = cand_mask; v.cand_geom = cand_geom; v.uniform = uniform; v.shape_ok = shape_ok;
-    v.model_params = mp; v.jobs_params = jp;
+    if ((rc = env_upload(e, &v.cand_ptr, c->cand_ptr, (size_t)D + 2))) return rc;
+    if ((rc = env_upload(e, &v.cand_mask, c->cand_mask, (size_t)n_cand * nw))) return rc;
+    if ((rc = env_upload(e, &v.cand_geom, c->cand_geom, (size_t)n_cand))) return rc;
+    if ((rc = env_upload(e, &v.uniform, c->uniform, (size_t)M * (D + 1)))) return rc;
+    if ((rc = env_upload(e, &v.shape_ok, c->shape_ok, (size_t)D + 1))) return rc;
+    if ((rc = env_upload(e, &v.model_params, c->model_params, (size_t)M * 5))) return rc;
+    if ((rc = env_upload(e, &v.jobs_params, c->jobs_params, (size_t)16))) return rc;
     std::vector<int32_t> minus1((size_t)M * (D + 1) * G, -1);
     if ((rc = env_upload(e, &v.tmpl_of, minus1.data(), minus1.size()))) return rc;
     if ((rc = env_upload<double>(e, &v.tmpl_mount, nullptr, (size_t)e->cfg.max_templates * 6))) return rc;
-    int32_t* model_of; double* frac; double* macc;
-    if ((rc = env_upload<int32_t>(e, &model_of, nullptr, (size_t)B * J))) return rc;
-    if ((rc = env_upload<double>(e, &frac, nullptr, (size_t)B * J))) return rc;
-    if ((rc = env_upload<double>(e, &macc, nullptr, (size_t)B * J))) return rc;
-    v.model_of = model_of; v.frac = frac; v.macc = macc;
+    if ((rc = env_upload(e, &v.model_of, nullptr, (size_t)B * J))) return rc;
+    if ((rc = env_upload(e, &v.frac, nullptr, (size_t)B * J))) return rc;
+    if ((rc = env_upload(e, &v.macc, nullptr, (size_t)B * J))) return rc;
     if ((rc = env_upload<unsigned long long>(e, &v.busy, nullptr, (size_t)B * nw))) return rc;
     if ((rc = env_upload<unsigned long long>(e, &v.job_mask, nullptr, (size_t)B * J * nw))) return rc;
     if ((rc = env_upload<unsigned long long>(e, &v.placed, nullptr, (size_t)B * nw))) return rc;
@@ -1306,7 +1246,7 @@ int ramp_env_create(ramp_engine_t* e, const ramp_env_config_t* c) {
     if ((rc = env_upload<int32_t>(e, &v.need_host, nullptr, (size_t)B))) return rc;
     if ((rc = env_upload<int32_t>(e, &v.n_need_host, nullptr, 1))) return rc;
     if ((rc = env_upload<int32_t>(e, &v.err, nullptr, 1))) return rc;
-    CUDA_TRY(cudaMallocHost(&e->env_h_need, sizeof(int32_t) * 8));
+    CUDA_TRY(e->env_h_need.alloc(8));
     e->has_env = true;
     return RAMP_OK;
 }
@@ -1328,21 +1268,21 @@ int ramp_env_reset(ramp_engine_t* e, const int32_t* model_of, const double* frac
     EnvDev& v = e->env;
     const size_t n = (size_t)v.B * v.J;
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    CUDA_TRY(cudaMemcpyAsync((void*)v.model_of, model_of, sizeof(int32_t) * n, cudaMemcpyHostToDevice, e->stream));
-    CUDA_TRY(cudaMemcpyAsync((void*)v.frac, frac, sizeof(double) * n, cudaMemcpyHostToDevice, e->stream));
-    CUDA_TRY(cudaMemcpyAsync((void*)v.macc, macc, sizeof(double) * n, cudaMemcpyHostToDevice, e->stream));
-    CUDA_TRY(cudaMemsetAsync(v.job_mask, 0, sizeof(unsigned long long) * n * v.n_words, e->stream));
-    CUDA_TRY(cudaMemsetAsync(v.done, 0, (size_t)v.B, e->stream));
-    CUDA_TRY(cudaMemsetAsync(v.n_decided, 0, sizeof(int32_t) * (size_t)v.B, e->stream));
-    CUDA_TRY(cudaMemsetAsync(v.job_tmpl, 0xFF, sizeof(int32_t) * n, e->stream));          // -1
-    CUDA_TRY(cudaMemsetAsync(v.ret, 0, sizeof(double) * (size_t)v.B, e->stream));
-    CUDA_TRY(cudaMemsetAsync(v.err, 0, sizeof(int32_t), e->stream));
+    CUDA_TRY(cudaMemcpyAsync((void*)v.model_of, model_of, sizeof(int32_t) * n, cudaMemcpyHostToDevice, e->stream.get()));
+    CUDA_TRY(cudaMemcpyAsync((void*)v.frac, frac, sizeof(double) * n, cudaMemcpyHostToDevice, e->stream.get()));
+    CUDA_TRY(cudaMemcpyAsync((void*)v.macc, macc, sizeof(double) * n, cudaMemcpyHostToDevice, e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(v.job_mask, 0, sizeof(unsigned long long) * n * v.n_words, e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(v.done, 0, (size_t)v.B, e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(v.n_decided, 0, sizeof(int32_t) * (size_t)v.B, e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(v.job_tmpl, 0xFF, sizeof(int32_t) * n, e->stream.get()));          // -1
+    CUDA_TRY(cudaMemsetAsync(v.ret, 0, sizeof(double) * (size_t)v.B, e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(v.err, 0, sizeof(int32_t), e->stream.get()));
     int rc = ramp_reset(e, arrivals, v.J);
     if (rc != RAMP_OK) return rc;
-    ramp_env_update_kernel<<<(v.B + 127) / 128, 128, 0, e->stream>>>(v, e->ep, nullptr, 1);
+    ramp_env_update_kernel<<<(v.B + 127) / 128, 128, 0, e->stream.get()>>>(v, e->ep, nullptr, 1);
     e->launches++;
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     return RAMP_OK;
 }
 
@@ -1360,12 +1300,12 @@ int ramp_env_host_mirror(ramp_engine_t* e, ramp_env_buffers_t* out) {
     const EnvDev& v = e->env;
     const size_t B = (size_t)v.B, A = (size_t)v.max_degree + 1;
     const size_t o_reward = 0, o_obs = o_reward + 8 * B, o_act = o_obs + 44 * B, o_qm = o_act + 4 * B, o_done = o_qm + 4 * B, o_mask = o_done + B;
-    if (!e->env_h_mirror) {
+    if (!e->env_h_mirror.get()) {
         CUDA_TRY(cudaSetDevice(e->cfg.device));
-        CUDA_TRY(cudaMallocHost(&e->env_h_mirror, o_mask + B * A + 64));
-        memset(e->env_h_mirror, 0, o_mask + B * A + 64);
+        CUDA_TRY(e->env_h_mirror.alloc(o_mask + B * A + 64));
+        memset(e->env_h_mirror.get(), 0, o_mask + B * A + 64);
     }
-    unsigned char* m = (unsigned char*)e->env_h_mirror;
+    unsigned char* m = e->env_h_mirror.get();
     memset(out, 0, sizeof(*out));
     out->reward = (double*)(m + o_reward); out->obs_dynamic = (float*)(m + o_obs); out->actions = (int32_t*)(m + o_act);
     out->queued_model = (int32_t*)(m + o_qm); out->done = m + o_done; out->action_mask = m + o_mask;
@@ -1377,23 +1317,23 @@ int ramp_env_decide(ramp_engine_t* e, const int32_t* actions, int32_t* n_need_ho
     if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
     EnvDev& v = e->env;
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    cudaStream_t st = e->stream;
+    cudaStream_t st = e->stream.get();
     if (actions) CUDA_TRY(cudaMemcpyAsync(v.actions, actions, sizeof(int32_t) * v.B, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemsetAsync(v.n_need_host, 0, sizeof(int32_t), st));
-    ramp_env_decide_kernel<<<(v.B + 127) / 128, 128, 0, st>>>(v, e->ep, e->d_actions);
+    ramp_env_decide_kernel<<<(v.B + 127) / 128, 128, 0, st>>>(v, e->ep, e->d_actions.get());
     e->launches++;
     CUDA_TRY(cudaGetLastError());
     if (n_need_host_out) {
-        CUDA_TRY(cudaMemcpyAsync(e->env_h_need, v.n_need_host, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(e->env_h_need + 1, v.err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get(), v.n_need_host, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 1, v.err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
-        if (e->env_h_need[1] != 0) {
+        if (e->env_h_need.get()[1] != 0) {
             CUDA_TRY(cudaMemset(v.err, 0, sizeof(int32_t)));
-            return set_error(RAMP_ERR_BAD_ARG, "episode %d: the action is invalid given its action mask (RJPE:314-319)", e->env_h_need[1] - 1);
+            return set_error(RAMP_ERR_BAD_ARG, "episode %d: the action is invalid given its action mask (RJPE:314-319)", e->env_h_need.get()[1] - 1);
         }
-        *n_need_host_out = e->env_h_need[0];
-        if (need_host_out && e->env_h_need[0] > 0)
-            CUDA_TRY(cudaMemcpy(need_host_out, v.need_host, sizeof(int32_t) * e->env_h_need[0], cudaMemcpyDeviceToHost));
+        *n_need_host_out = e->env_h_need.get()[0];
+        if (need_host_out && e->env_h_need.get()[0] > 0)
+            CUDA_TRY(cudaMemcpy(need_host_out, v.need_host, sizeof(int32_t) * e->env_h_need.get()[0], cudaMemcpyDeviceToHost));
     } else {
         e->env_unchecked_decide = true;      // looked at by the next ramp_env_read
     }
@@ -1405,7 +1345,7 @@ int ramp_env_patch(ramp_engine_t* e, int32_t episode, int32_t template_id, const
     EnvDev& v = e->env;
     if (episode < 0 || episode >= v.B || template_id >= (int32_t)e->templates.size()) return set_error(RAMP_ERR_BAD_ARG, "bad patch");
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     int32_t q = -1;
     CUDA_TRY(cudaMemcpy(&q, v.decided_job + episode, sizeof(int32_t), cudaMemcpyDeviceToHost));
     ramp_action_t row{};
@@ -1420,7 +1360,7 @@ int ramp_env_patch(ramp_engine_t* e, int32_t episode, int32_t template_id, const
     } else {
         row.template_id = -1;
     }
-    CUDA_TRY(cudaMemcpy(e->d_actions + episode, &row, sizeof(row), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(e->d_actions.get() + episode, &row, sizeof(row), cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(v.tid + episode, &row.template_id, sizeof(int32_t), cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(v.placed + (size_t)episode * v.n_words, server_mask, sizeof(uint64_t) * v.n_words, cudaMemcpyHostToDevice));
     return RAMP_OK;
@@ -1429,9 +1369,9 @@ int ramp_env_patch(ramp_engine_t* e, int32_t episode, int32_t template_id, const
 int ramp_env_advance(ramp_engine_t* e) {
     if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
     EnvDev& v = e->env;
-    int rc = ramp_step_device(e, e->d_actions, 1, e->d_step_stats, e->d_n_cluster_steps);
+    int rc = ramp_step_device(e, e->d_actions.get(), 1, e->d_step_stats.get(), e->d_n_cluster_steps.get());
     if (rc != RAMP_OK) return rc;
-    ramp_env_update_kernel<<<(v.B + 127) / 128, 128, 0, e->stream>>>(v, e->ep, e->d_n_cluster_steps, 0);
+    ramp_env_update_kernel<<<(v.B + 127) / 128, 128, 0, e->stream.get()>>>(v, e->ep, e->d_n_cluster_steps.get(), 0);
     e->launches++;
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
@@ -1440,47 +1380,47 @@ int ramp_env_advance(ramp_engine_t* e) {
 int ramp_env_read(ramp_engine_t* e, double* reward, uint8_t* done, int32_t* queued_model, float* obs_dynamic, uint8_t* action_mask) {
     if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
     const EnvDev& v = e->env;
-    cudaStream_t st = e->stream;
+    cudaStream_t st = e->stream.get();
     if (reward) CUDA_TRY(cudaMemcpyAsync(reward, v.reward, sizeof(double) * v.B, cudaMemcpyDeviceToHost, st));
     if (done) CUDA_TRY(cudaMemcpyAsync(done, v.done, (size_t)v.B, cudaMemcpyDeviceToHost, st));
     if (queued_model) CUDA_TRY(cudaMemcpyAsync(queued_model, v.queued_model, sizeof(int32_t) * v.B, cudaMemcpyDeviceToHost, st));
     if (obs_dynamic) CUDA_TRY(cudaMemcpyAsync(obs_dynamic, v.obs_dyn, sizeof(float) * 11 * v.B, cudaMemcpyDeviceToHost, st));
     if (action_mask) CUDA_TRY(cudaMemcpyAsync(action_mask, v.action_mask, (size_t)v.B * (v.max_degree + 1), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(e->env_h_need + 4, &e->d_counters->err_episode, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 4, &e->d_counters.get()->err_episode, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     if (e->env_unchecked_decide) {
         // decisions taken without the host looking (a device-resident policy): an invalid action under apply_action_mask is sticky
         // in `err`; episodes the tables could not decide were left unplaced, which only the LAST decide's count can show
-        CUDA_TRY(cudaMemcpyAsync(e->env_h_need + 2, v.n_need_host, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(e->env_h_need + 3, v.err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 2, v.n_need_host, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 3, v.err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         int rc = ramp_sync(e);
         if (rc != RAMP_OK) return rc;
         e->env_unchecked_decide = false;
-        if (e->env_h_need[3] != 0) {
+        if (e->env_h_need.get()[3] != 0) {
             CUDA_TRY(cudaMemset(v.err, 0, sizeof(int32_t)));
-            return set_error(RAMP_ERR_BAD_ARG, "episode %d: the action is invalid given its action mask (RJPE:314-319)", e->env_h_need[3] - 1);
+            return set_error(RAMP_ERR_BAD_ARG, "episode %d: the action is invalid given its action mask (RJPE:314-319)", e->env_h_need.get()[3] - 1);
         }
-        if (e->env_h_need[2] != 0)
-            return set_error(RAMP_ERR_BAD_ARG, "%d episodes needed the host's placer but ramp_env_decide was called without need_host_out", e->env_h_need[2]);
-        return e->env_h_need[4] != 0 ? ramp_check_status(e, nullptr, nullptr) : RAMP_OK;
+        if (e->env_h_need.get()[2] != 0)
+            return set_error(RAMP_ERR_BAD_ARG, "%d episodes needed the host's placer but ramp_env_decide was called without need_host_out", e->env_h_need.get()[2]);
+        return e->env_h_need.get()[4] != 0 ? ramp_check_status(e, nullptr, nullptr) : RAMP_OK;
     }
     {
         int rc = ramp_sync(e);
         if (rc != RAMP_OK) return rc;
     }
-    return e->env_h_need[4] != 0 ? ramp_check_status(e, nullptr, nullptr) : RAMP_OK;
+    return e->env_h_need.get()[4] != 0 ? ramp_check_status(e, nullptr, nullptr) : RAMP_OK;
 }
 
 
 int ramp_enable_tick_lists(ramp_engine_t* e, int32_t cap) {
     if (!e || cap < 1) return set_error(RAMP_ERR_BAD_ARG, "ramp_enable_tick_lists: cap must be >= 1");
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
-    if (e->ep.tick_util) { cudaFree(e->ep.tick_util); cudaFree(e->ep.tick_util_n); e->ep.tick_util = nullptr; e->ep.tick_util_n = nullptr; }
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
+    e->ep.tick_util = nullptr; e->ep.tick_util_n = nullptr;     // no lists until both arrays are there
     const size_t B = (size_t)e->cfg.n_episodes;
-    CUDA_TRY(cudaMalloc(&e->ep.tick_util, sizeof(double) * B * (size_t)cap * 2));
-    CUDA_TRY(cudaMalloc(&e->ep.tick_util_n, sizeof(int32_t) * B));
-    CUDA_TRY(cudaMemset(e->ep.tick_util_n, 0, sizeof(int32_t) * B));
-    e->ep.tick_util_cap = cap;
+    CUDA_TRY(e->tick_util.alloc(B * (size_t)cap * 2));
+    CUDA_TRY(e->tick_util_n.alloc(B));
+    CUDA_TRY(cudaMemset(e->tick_util_n.get(), 0, sizeof(int32_t) * B));
+    e->ep.tick_util = e->tick_util.get(); e->ep.tick_util_n = e->tick_util_n.get(); e->ep.tick_util_cap = cap;
     return RAMP_OK;
 }
 
@@ -1489,7 +1429,7 @@ int ramp_get_tick_lists(ramp_engine_t* e, int32_t episode, double* mounted_out, 
     if (!e->ep.tick_util) return set_error(RAMP_ERR_BAD_ARG, "per-tick lists are not recorded (ramp_enable_tick_lists)");
     if (episode < 0 || episode >= e->cfg.n_episodes) return set_error(RAMP_ERR_BAD_ARG, "bad episode %d", episode);
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     int32_t n = 0;
     CUDA_TRY(cudaMemcpy(&n, e->ep.tick_util_n + episode, sizeof(int32_t), cudaMemcpyDeviceToHost));
     *n_out = n;
@@ -1507,8 +1447,8 @@ int ramp_get_tick_lists(ramp_engine_t* e, int32_t episode, double* mounted_out, 
 int ramp_get_last_step_stats(ramp_engine_t* e, double* stats_out, int32_t* n_cluster_steps_out) {
     if (!e) return set_error(RAMP_ERR_BAD_ARG, "null engine");
     const int B = e->cfg.n_episodes;
-    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, e->d_step_stats, sizeof(double) * RAMP_STEP_STATS_LEN * B, cudaMemcpyDeviceToHost, e->stream));
-    if (n_cluster_steps_out) CUDA_TRY(cudaMemcpyAsync(n_cluster_steps_out, e->d_n_cluster_steps, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, e->stream));
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, e->d_step_stats.get(), sizeof(double) * RAMP_STEP_STATS_LEN * B, cudaMemcpyDeviceToHost, e->stream.get()));
+    if (n_cluster_steps_out) CUDA_TRY(cudaMemcpyAsync(n_cluster_steps_out, e->d_n_cluster_steps.get(), sizeof(int32_t) * B, cudaMemcpyDeviceToHost, e->stream.get()));
     return ramp_sync(e);
 }
 
@@ -1516,9 +1456,9 @@ int ramp_get_last_step_stats(ramp_engine_t* e, double* stats_out, int32_t* n_clu
 int ramp_env_read_state(ramp_engine_t* e, uint64_t* busy_out, int32_t* actions_out, int32_t* n_decided_out) {
     if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
     const EnvDev& v = e->env;
-    if (busy_out) CUDA_TRY(cudaMemcpyAsync(busy_out, v.busy, sizeof(uint64_t) * (size_t)v.B * v.n_words, cudaMemcpyDeviceToHost, e->stream));
-    if (actions_out) CUDA_TRY(cudaMemcpyAsync(actions_out, v.actions, sizeof(int32_t) * v.B, cudaMemcpyDeviceToHost, e->stream));
-    if (n_decided_out) CUDA_TRY(cudaMemcpyAsync(n_decided_out, v.n_decided, sizeof(int32_t) * v.B, cudaMemcpyDeviceToHost, e->stream));
+    if (busy_out) CUDA_TRY(cudaMemcpyAsync(busy_out, v.busy, sizeof(uint64_t) * (size_t)v.B * v.n_words, cudaMemcpyDeviceToHost, e->stream.get()));
+    if (actions_out) CUDA_TRY(cudaMemcpyAsync(actions_out, v.actions, sizeof(int32_t) * v.B, cudaMemcpyDeviceToHost, e->stream.get()));
+    if (n_decided_out) CUDA_TRY(cudaMemcpyAsync(n_decided_out, v.n_decided, sizeof(int32_t) * v.B, cudaMemcpyDeviceToHost, e->stream.get()));
     return ramp_sync(e);
 }
 
@@ -1526,8 +1466,8 @@ int ramp_env_read_episode(ramp_engine_t* e, int32_t* job_template_out, double* r
     if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
     const EnvDev& v = e->env;
     if (job_template_out)
-        CUDA_TRY(cudaMemcpyAsync(job_template_out, v.job_tmpl, sizeof(int32_t) * (size_t)v.B * v.J, cudaMemcpyDeviceToHost, e->stream));
-    if (return_out) CUDA_TRY(cudaMemcpyAsync(return_out, v.ret, sizeof(double) * v.B, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(job_template_out, v.job_tmpl, sizeof(int32_t) * (size_t)v.B * v.J, cudaMemcpyDeviceToHost, e->stream.get()));
+    if (return_out) CUDA_TRY(cudaMemcpyAsync(return_out, v.ret, sizeof(double) * v.B, cudaMemcpyDeviceToHost, e->stream.get()));
     return ramp_sync(e);
 }
 
@@ -1535,10 +1475,10 @@ int ramp_get_episode_stats(ramp_engine_t* e, double* out) {
     if (!e || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     const int B = e->cfg.n_episodes;
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    ramp_episode_stats_kernel<<<(B + 127) / 128, 128, 0, e->stream>>>(e->ep, e->d_es_export);
+    ramp_episode_stats_kernel<<<(B + 127) / 128, 128, 0, e->stream.get()>>>(e->ep, e->d_es_export.get());
     e->launches++;
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaMemcpyAsync(out, e->d_es_export, sizeof(double) * RAMP_ES_LEN * B, cudaMemcpyDeviceToHost, e->stream));
+    CUDA_TRY(cudaMemcpyAsync(out, e->d_es_export.get(), sizeof(double) * RAMP_ES_LEN * B, cudaMemcpyDeviceToHost, e->stream.get()));
     return ramp_sync(e);
 }
 
@@ -1560,7 +1500,7 @@ int ramp_env_agent_act(ramp_engine_t* e, uint64_t seed) {
     if (!e->env_agents_set) return set_error(RAMP_ERR_BAD_ARG, "no agents: call ramp_env_set_agents first");
     const EnvDev& v = e->env;
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    ramp_env_agent_kernel<<<(v.B + 127) / 128, 128, 0, e->stream>>>(v, e->ep, (unsigned long long)seed);
+    ramp_env_agent_kernel<<<(v.B + 127) / 128, 128, 0, e->stream.get()>>>(v, e->ep, (unsigned long long)seed);
     e->launches++;
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;

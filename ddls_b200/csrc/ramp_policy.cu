@@ -16,19 +16,13 @@
 //                           environment's action buffer.  All read-out weights are staged once per CTA in shared memory, laid
 //                           out so that lanes read consecutive words.
 #include <cfloat>
-#include <cstdarg>
 #include <cmath>
 #include <cstdint>
-#include <cstdio>
 #include <cstring>
-#include <string>
 #include <vector>
 
-#include <cuda_runtime.h>
+#include "ramp_owned.cuh"
 
-#include "../../include/ramp_b200.h"
-
-int ramp_internal_set_error(int code, const char* msg);
 cudaStream_t ramp_internal_stream(ramp_engine_t* e);
 int ramp_internal_device(ramp_engine_t* e);
 void ramp_internal_count_launches(ramp_engine_t* e, int n);
@@ -39,21 +33,6 @@ constexpr int POL_MAX_ROUNDS = 8;
 constexpr int POL_MAX_DIM = 128;        // node / message / embedding widths
 constexpr int POL_MAX_HPL = 16;         // read-out hidden units per lane (hidden <= 512)
 constexpr float LN_EPS = 1e-5f;         // torch.nn.LayerNorm default
-
-static int perr(int code, const char* fmt, ...) {
-    char buf[512];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof(buf), fmt, ap);
-    va_end(ap);
-    return ramp_internal_set_error(code, buf);
-}
-
-#define PCUDA(expr)                                                                                              \
-    do {                                                                                                         \
-        cudaError_t _e = (expr);                                                                                 \
-        if (_e != cudaSuccess) return perr(RAMP_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-    } while (0)
 
 struct RoundW {                          // offsets (in floats) into the weight blob
     int32_t in, out;
@@ -356,7 +335,7 @@ using namespace ramp;
 
 struct HostModel {
     ModelDev d{};
-    std::vector<void*> allocs;
+    std::vector<DeviceArray<unsigned char>> allocs;
     bool set = false;
 };
 
@@ -364,26 +343,25 @@ struct ramp_policy {
     int device = 0;
     PolicyDev P{};
     int64_t n_weights = 0;
-    float* d_w = nullptr;
+    DeviceArray<float> d_w;
     std::vector<HostModel> models;
-    ModelDev* d_models = nullptr;
-    float* d_emb = nullptr;               // [n_models][out_node]
-    float* d_gstatic = nullptr;           // [n_models][6]
+    DeviceArray<ModelDev> d_models;
+    DeviceArray<float> d_emb;             // [n_models][out_node]
+    DeviceArray<float> d_gstatic;         // [n_models][6]
     bool weights_set = false, emb_valid = false;
     int sm_count = 132;
     size_t head_smem = 0;
     // outputs of the last act, for ramp_policy_read and ramp_policy_trajectory_record; act_n: its environment's episodes (-1: none yet)
     int32_t cap = 0, act_n = -1;
-    float* d_logits = nullptr; float* d_value = nullptr; float* d_logp = nullptr;
+    DeviceArray<float> d_logits, d_value, d_logp;
     // inputs and outputs of ramp_policy_forward / ramp_policy_decide, apart from act's
     int32_t fcap = 0;
-    int32_t* f_model = nullptr; float* f_gf = nullptr; uint8_t* f_mask = nullptr; int32_t* f_actions = nullptr;
-    float* f_logits = nullptr; float* f_value = nullptr; float* f_logp = nullptr;
+    DeviceArray<int32_t> f_model, f_actions; DeviceArray<float> f_gf, f_logits, f_value, f_logp; DeviceArray<uint8_t> f_mask;
     unsigned long long act_calls = 0;
     // trajectory of a rollout segment (ramp_policy_trajectory_*): [horizon][B] per field, on the device until read
     int32_t traj_h = 0, traj_b = 0, traj_a = 0;
-    float* t_obs = nullptr; int32_t* t_model = nullptr; uint8_t* t_mask = nullptr; int32_t* t_action = nullptr;
-    float* t_logp = nullptr; float* t_value = nullptr; double* t_reward = nullptr; uint8_t* t_done = nullptr;
+    DeviceArray<float> t_obs, t_logp, t_value; DeviceArray<int32_t> t_model, t_action;
+    DeviceArray<uint8_t> t_mask, t_done; DeviceArray<double> t_reward;
 };
 
 namespace {
@@ -414,41 +392,39 @@ int64_t layout(const ramp_policy_config_t& c, PolicyDev* P) {
 int check_config(const ramp_policy_config_t& c) {
     auto in = [](int v, int lo, int hi) { return v >= lo && v <= hi; };
     if (!in(c.in_features_node, 1, POL_MAX_DIM) || !in(c.in_features_edge, 1, POL_MAX_DIM) || !in(c.in_features_graph, 1, POL_MAX_DIM - 32))
-        return perr(RAMP_ERR_BAD_ARG, "policy: feature widths must be in [1, %d]", POL_MAX_DIM);
+        return set_error(RAMP_ERR_BAD_ARG, "policy: feature widths must be in [1, %d]", POL_MAX_DIM);
     if (!in(c.out_features_msg, 2, POL_MAX_DIM) || (c.out_features_msg & 1) || !in(c.out_features_hidden, 1, POL_MAX_DIM) || !in(c.out_features_node, 1, POL_MAX_DIM - 32))
-        return perr(RAMP_ERR_BAD_ARG, "policy: out_features_msg must be even and every width <= %d", POL_MAX_DIM);
+        return set_error(RAMP_ERR_BAD_ARG, "policy: out_features_msg must be even and every width <= %d", POL_MAX_DIM);
     if (!in(c.out_features_graph, 1, 32) || !in(c.n_actions, 1, 32) || c.in_features_graph + c.n_actions > POL_MAX_DIM)
-        return perr(RAMP_ERR_BAD_ARG, "policy: out_features_graph and n_actions must be <= 32");
-    if (c.num_rounds < 2 || c.num_rounds > POL_MAX_ROUNDS) return perr(RAMP_ERR_BAD_ARG, "policy: num_rounds must be in [2, %d] (gnn.py:40-41)", POL_MAX_ROUNDS);
+        return set_error(RAMP_ERR_BAD_ARG, "policy: out_features_graph and n_actions must be <= 32");
+    if (c.num_rounds < 2 || c.num_rounds > POL_MAX_ROUNDS) return set_error(RAMP_ERR_BAD_ARG, "policy: num_rounds must be in [2, %d] (gnn.py:40-41)", POL_MAX_ROUNDS);
     if (c.fcnet_hidden < 32 || c.fcnet_hidden % 32 || c.fcnet_hidden > 32 * POL_MAX_HPL)
-        return perr(RAMP_ERR_BAD_ARG, "policy: fcnet_hidden must be a multiple of 32 in [32, %d]", 32 * POL_MAX_HPL);
+        return set_error(RAMP_ERR_BAD_ARG, "policy: fcnet_hidden must be a multiple of 32 in [32, %d]", 32 * POL_MAX_HPL);
     if (!in(c.aggregator_activation, 0, 1) || !(c.fcnet_activation == 0 || c.fcnet_activation == 2))
-        return perr(RAMP_ERR_BAD_ARG, "policy: unsupported activation");
-    if (c.n_models < 1) return perr(RAMP_ERR_BAD_ARG, "policy: n_models must be >= 1");
+        return set_error(RAMP_ERR_BAD_ARG, "policy: unsupported activation");
+    if (c.n_models < 1) return set_error(RAMP_ERR_BAD_ARG, "policy: n_models must be >= 1");
     return RAMP_OK;
 }
 
 int ensure_outputs(ramp_policy* p, int32_t n) {
     if (n <= p->cap) return RAMP_OK;
-    cudaFree(p->d_logits); cudaFree(p->d_value); cudaFree(p->d_logp);
-    p->d_logits = p->d_value = p->d_logp = nullptr; p->cap = 0;
-    PCUDA(cudaMalloc(&p->d_logits, sizeof(float) * (size_t)n * p->P.c.n_actions));
-    PCUDA(cudaMalloc(&p->d_value, sizeof(float) * (size_t)n));
-    PCUDA(cudaMalloc(&p->d_logp, sizeof(float) * (size_t)n));
+    p->cap = 0;                           // until every buffer has the new size
+    CUDA_TRY(p->d_logits.alloc((size_t)n * p->P.c.n_actions));
+    CUDA_TRY(alloc_each(n, p->d_value, p->d_logp));
     p->cap = n;
     return RAMP_OK;
 }
 
 int launch_embed(ramp_policy* p, cudaStream_t st) {
     for (size_t m = 0; m < p->models.size(); ++m)
-        if (!p->models[m].set) return perr(RAMP_ERR_BAD_ARG, "policy: model %zu was never registered (ramp_policy_set_model)", m);
-    if (!p->weights_set) return perr(RAMP_ERR_BAD_ARG, "policy: no weights (ramp_policy_set_weights)");
+        if (!p->models[m].set) return set_error(RAMP_ERR_BAD_ARG, "policy: model %zu was never registered (ramp_policy_set_model)", m);
+    if (!p->weights_set) return set_error(RAMP_ERR_BAD_ARG, "policy: no weights (ramp_policy_set_weights)");
     std::vector<ModelDev> h(p->models.size());
     for (size_t m = 0; m < h.size(); ++m) h[m] = p->models[m].d;
-    PCUDA(cudaMemcpyAsync(p->d_models, h.data(), sizeof(ModelDev) * h.size(), cudaMemcpyHostToDevice, st));
-    PCUDA(cudaStreamSynchronize(st));                                  // `h` is pageable
-    ramp_gnn_embed_kernel<<<(unsigned)h.size(), 256, 0, st>>>(p->P, p->d_models, p->d_emb);
-    PCUDA(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(p->d_models.get(), h.data(), sizeof(ModelDev) * h.size(), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));                                  // `h` is pageable
+    ramp_gnn_embed_kernel<<<(unsigned)h.size(), 256, 0, st>>>(p->P, p->d_models.get(), p->d_emb.get());
+    CUDA_TRY(cudaGetLastError());
     p->emb_valid = true;
     return RAMP_OK;
 }
@@ -459,7 +435,7 @@ int launch_head(ramp_policy* p, const HeadArgs& a, cudaStream_t st) {
     if (grid > p->sm_count * 2) grid = p->sm_count * 2;
     if (grid < 1) grid = 1;
     ramp_policy_head_kernel<<<grid, wpc * 32, p->head_smem, st>>>(p->P, a);
-    PCUDA(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
 }
 
@@ -467,39 +443,32 @@ int launch_head(ramp_policy* p, const HeadArgs& a, cudaStream_t st) {
 // ramp_policy_read and the trajectory stays as it was
 int head_on_host(ramp_policy* p, int32_t n, const int32_t* model, const float* graph_features, const uint8_t* action_mask, int32_t sample,
                  uint64_t seed, float* logits_out, float* value_out, float* logp_out, int32_t* actions_out) {
-    if (!p || !model || !graph_features || !action_mask) return perr(RAMP_ERR_BAD_ARG, "null argument");
+    if (!p || !model || !graph_features || !action_mask) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     if (n < 1) return RAMP_OK;
     const ramp_policy_config_t& c = p->P.c;
-    PCUDA(cudaSetDevice(p->device));
+    CUDA_TRY(cudaSetDevice(p->device));
     int rc;
     if (!p->emb_valid && (rc = launch_embed(p, 0)) != RAMP_OK) return rc;
     if (n > p->fcap) {
-        cudaFree(p->f_model); cudaFree(p->f_gf); cudaFree(p->f_mask); cudaFree(p->f_actions);
-        cudaFree(p->f_logits); cudaFree(p->f_value); cudaFree(p->f_logp);
-        p->f_model = nullptr; p->f_gf = nullptr; p->f_mask = nullptr; p->f_actions = nullptr;
-        p->f_logits = p->f_value = p->f_logp = nullptr; p->fcap = 0;
-        PCUDA(cudaMalloc(&p->f_model, sizeof(int32_t) * (size_t)n));
-        PCUDA(cudaMalloc(&p->f_gf, sizeof(float) * (size_t)n * c.in_features_graph));
-        PCUDA(cudaMalloc(&p->f_mask, (size_t)n * c.n_actions));
-        PCUDA(cudaMalloc(&p->f_actions, sizeof(int32_t) * (size_t)n));
-        PCUDA(cudaMalloc(&p->f_logits, sizeof(float) * (size_t)n * c.n_actions));
-        PCUDA(cudaMalloc(&p->f_value, sizeof(float) * (size_t)n));
-        PCUDA(cudaMalloc(&p->f_logp, sizeof(float) * (size_t)n));
+        p->fcap = 0;                      // until every buffer has the new size
+        CUDA_TRY(alloc_each(n, p->f_model, p->f_actions, p->f_value, p->f_logp));
+        CUDA_TRY(p->f_gf.alloc((size_t)n * c.in_features_graph));
+        CUDA_TRY(alloc_each((size_t)n * c.n_actions, p->f_mask, p->f_logits));
         p->fcap = n;
     }
-    PCUDA(cudaMemcpy(p->f_model, model, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice));
-    PCUDA(cudaMemcpy(p->f_gf, graph_features, sizeof(float) * (size_t)n * c.in_features_graph, cudaMemcpyHostToDevice));
-    PCUDA(cudaMemcpy(p->f_mask, action_mask, (size_t)n * c.n_actions, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->f_model.get(), model, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->f_gf.get(), graph_features, sizeof(float) * (size_t)n * c.in_features_graph, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->f_mask.get(), action_mask, (size_t)n * c.n_actions, cudaMemcpyHostToDevice));
     HeadArgs a{};
-    a.n = n; a.graph_features = p->f_gf; a.model = p->f_model; a.mask = p->f_mask; a.emb = p->d_emb; a.graph_static = p->d_gstatic;
-    a.logits = p->f_logits; a.value = p->f_value; a.logp = p->f_logp; a.actions = p->f_actions;
+    a.n = n; a.graph_features = p->f_gf.get(); a.model = p->f_model.get(); a.mask = p->f_mask.get(); a.emb = p->d_emb.get(); a.graph_static = p->d_gstatic.get();
+    a.logits = p->f_logits.get(); a.value = p->f_value.get(); a.logp = p->f_logp.get(); a.actions = p->f_actions.get();
     a.sample = sample; a.seed = seed;
     if ((rc = launch_head(p, a, 0)) != RAMP_OK) return rc;
-    PCUDA(cudaStreamSynchronize(0));
-    if (logits_out) PCUDA(cudaMemcpy(logits_out, p->f_logits, sizeof(float) * (size_t)n * c.n_actions, cudaMemcpyDeviceToHost));
-    if (value_out) PCUDA(cudaMemcpy(value_out, p->f_value, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
-    if (logp_out) PCUDA(cudaMemcpy(logp_out, p->f_logp, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
-    if (actions_out) PCUDA(cudaMemcpy(actions_out, p->f_actions, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaStreamSynchronize(0));
+    if (logits_out) CUDA_TRY(cudaMemcpy(logits_out, p->f_logits.get(), sizeof(float) * (size_t)n * c.n_actions, cudaMemcpyDeviceToHost));
+    if (value_out) CUDA_TRY(cudaMemcpy(value_out, p->f_value.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    if (logp_out) CUDA_TRY(cudaMemcpy(logp_out, p->f_logp.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    if (actions_out) CUDA_TRY(cudaMemcpy(actions_out, p->f_actions.get(), sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
 
@@ -513,11 +482,11 @@ int64_t ramp_policy_weight_count(const ramp_policy_config_t* cfg) {
 }
 
 int ramp_policy_create(int device, const ramp_policy_config_t* cfg, ramp_policy_t** out) {
-    if (!cfg || !out) return perr(RAMP_ERR_BAD_ARG, "null argument");
+    if (!cfg || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     int rc = check_config(*cfg);
     if (rc != RAMP_OK) return rc;
-    PCUDA(cudaSetDevice(device));
-    ramp_policy* p = new ramp_policy();
+    CUDA_TRY(cudaSetDevice(device));
+    std::unique_ptr<ramp_policy> p(new ramp_policy());
     p->device = device;
     p->P.c = *cfg;
     p->n_weights = layout(*cfg, &p->P);
@@ -525,41 +494,31 @@ int ramp_policy_create(int device, const ramp_policy_config_t* cfg, ramp_policy_
     cudaDeviceProp prop{};
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) p->sm_count = prop.multiProcessorCount;
     p->head_smem = head_smem_floats(*cfg, 8) * sizeof(float);
-    auto fail = [&](int code) { ramp_policy_destroy(p); return code; };
-    if (p->head_smem > 200 * 1024) return fail(perr(RAMP_ERR_CAPACITY, "policy: the read-out needs %zu B of shared memory (max 200 KiB)", p->head_smem));
-    if (cudaFuncSetAttribute(ramp_policy_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->head_smem) != cudaSuccess)
-        return fail(perr(RAMP_ERR_CUDA, "policy: cannot reserve %zu B of shared memory", p->head_smem));
-    if (cudaMalloc(&p->d_w, sizeof(float) * p->n_weights) != cudaSuccess ||
-        cudaMalloc(&p->d_models, sizeof(ModelDev) * cfg->n_models) != cudaSuccess ||
-        cudaMalloc(&p->d_emb, sizeof(float) * (size_t)cfg->n_models * cfg->out_features_node) != cudaSuccess ||
-        cudaMalloc(&p->d_gstatic, sizeof(float) * (size_t)cfg->n_models * 6) != cudaSuccess)
-        return fail(perr(RAMP_ERR_CUDA, "policy: out of device memory"));
-    cudaMemset(p->d_emb, 0, sizeof(float) * (size_t)cfg->n_models * cfg->out_features_node);
-    cudaMemset(p->d_gstatic, 0, sizeof(float) * (size_t)cfg->n_models * 6);
-    p->P.w = p->d_w;
-    *out = p;
+    if (p->head_smem > 200 * 1024) return set_error(RAMP_ERR_CAPACITY, "policy: the read-out needs %zu B of shared memory (max 200 KiB)", p->head_smem);
+    CUDA_TRY(reserve_dynamic_smem((const void*)ramp_policy_head_kernel, p->head_smem));
+    CUDA_TRY(p->d_w.alloc(p->n_weights));
+    CUDA_TRY(p->d_models.alloc(cfg->n_models));
+    CUDA_TRY(p->d_emb.alloc((size_t)cfg->n_models * cfg->out_features_node));
+    CUDA_TRY(p->d_gstatic.alloc((size_t)cfg->n_models * 6));
+    cudaMemset(p->d_emb.get(), 0, sizeof(float) * (size_t)cfg->n_models * cfg->out_features_node);
+    cudaMemset(p->d_gstatic.get(), 0, sizeof(float) * (size_t)cfg->n_models * 6);
+    p->P.w = p->d_w.get();
+    *out = p.release();
     return RAMP_OK;
 }
 
 void ramp_policy_destroy(ramp_policy_t* p) {
     if (!p) return;
     cudaSetDevice(p->device);
-    for (auto& m : p->models) for (void* a : m.allocs) cudaFree(a);
-    cudaFree(p->d_w); cudaFree(p->d_models); cudaFree(p->d_emb); cudaFree(p->d_gstatic);
-    cudaFree(p->d_logits); cudaFree(p->d_value); cudaFree(p->d_logp);
-    cudaFree(p->f_model); cudaFree(p->f_gf); cudaFree(p->f_mask); cudaFree(p->f_actions);
-    cudaFree(p->f_logits); cudaFree(p->f_value); cudaFree(p->f_logp);
-    cudaFree(p->t_obs); cudaFree(p->t_model); cudaFree(p->t_mask); cudaFree(p->t_action); cudaFree(p->t_logp); cudaFree(p->t_value);
-    cudaFree(p->t_reward); cudaFree(p->t_done);
     delete p;
 }
 
 int ramp_policy_set_weights(ramp_policy_t* p, const float* weights, int64_t n) {
-    if (!p || !weights) return perr(RAMP_ERR_BAD_ARG, "null argument");
-    if (n != p->n_weights) return perr(RAMP_ERR_BAD_ARG, "policy: %lld weights given, the configuration has %lld", (long long)n, (long long)p->n_weights);
-    PCUDA(cudaSetDevice(p->device));
-    PCUDA(cudaDeviceSynchronize());                                    // a running rollout may still read the old set
-    PCUDA(cudaMemcpy(p->d_w, weights, sizeof(float) * n, cudaMemcpyHostToDevice));
+    if (!p || !weights) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (n != p->n_weights) return set_error(RAMP_ERR_BAD_ARG, "policy: %lld weights given, the configuration has %lld", (long long)n, (long long)p->n_weights);
+    CUDA_TRY(cudaSetDevice(p->device));
+    CUDA_TRY(cudaDeviceSynchronize());                                    // a running rollout may still read the old set
+    CUDA_TRY(cudaMemcpy(p->d_w.get(), weights, sizeof(float) * n, cudaMemcpyHostToDevice));
     p->weights_set = true;
     p->emb_valid = false;
     return RAMP_OK;
@@ -568,15 +527,14 @@ int ramp_policy_set_weights(ramp_policy_t* p, const float* weights, int64_t n) {
 int ramp_policy_set_model(ramp_policy_t* p, int32_t model, int32_t n_nodes, int32_t n_edges, const float* node_features,
                           const float* edge_features, const int32_t* edges_src, const int32_t* edges_dst, const float* graph_static) {
     if (!p || !node_features || !graph_static || (n_edges > 0 && (!edge_features || !edges_src || !edges_dst)))
-        return perr(RAMP_ERR_BAD_ARG, "null argument");
+        return set_error(RAMP_ERR_BAD_ARG, "null argument");
     const ramp_policy_config_t& c = p->P.c;
-    if (model < 0 || model >= c.n_models || n_nodes < 1 || n_edges < 0) return perr(RAMP_ERR_BAD_ARG, "policy: bad model %d (%d nodes, %d edges)", model, n_nodes, n_edges);
+    if (model < 0 || model >= c.n_models || n_nodes < 1 || n_edges < 0) return set_error(RAMP_ERR_BAD_ARG, "policy: bad model %d (%d nodes, %d edges)", model, n_nodes, n_edges);
     for (int e = 0; e < n_edges; ++e)
         if (edges_src[e] < 0 || edges_src[e] >= n_nodes || edges_dst[e] < 0 || edges_dst[e] >= n_nodes)
-            return perr(RAMP_ERR_BAD_ARG, "policy: edge %d of model %d names node %d -> %d of %d", e, model, edges_src[e], edges_dst[e], n_nodes);
-    PCUDA(cudaSetDevice(p->device));
+            return set_error(RAMP_ERR_BAD_ARG, "policy: edge %d of model %d names node %d -> %d of %d", e, model, edges_src[e], edges_dst[e], n_nodes);
+    CUDA_TRY(cudaSetDevice(p->device));
     HostModel& hm = p->models[model];
-    for (void* a : hm.allocs) cudaFree(a);
     hm.allocs.clear();
     hm.set = false;
     // incoming-edge lists by destination, in edge order (the order DGL delivers a node's mailbox is not observable through a mean)
@@ -587,10 +545,10 @@ int ramp_policy_set_model(ramp_policy_t* p, int32_t model, int32_t n_nodes, int3
     for (int e = 0; e < n_edges; ++e) { const int at = cur[edges_dst[e]]++; ine[at] = e; ins[at] = edges_src[e]; }
     const int half = c.out_features_msg / 2;
     auto up = [&](const void* src, size_t bytes, const void** dst) -> int {
-        void* d = nullptr;
-        PCUDA(cudaMalloc(&d, bytes ? bytes : 4));
-        hm.allocs.push_back(d);
-        if (src && bytes) PCUDA(cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
+        hm.allocs.emplace_back();
+        CUDA_TRY(hm.allocs.back().alloc(bytes ? bytes : 4));
+        void* d = hm.allocs.back().get();
+        if (src && bytes) CUDA_TRY(cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
         *dst = d;
         return RAMP_OK;
     };
@@ -606,7 +564,7 @@ int ramp_policy_set_model(ramp_policy_t* p, int32_t model, int32_t n_nodes, int3
     if ((rc = up(nullptr, sizeof(float) * (size_t)n_nodes * POL_MAX_DIM, (const void**)&d.z1))) return rc;
     if ((rc = up(nullptr, sizeof(float) * (size_t)n_nodes * half, (const void**)&d.hn))) return rc;
     if ((rc = up(nullptr, sizeof(float) * (size_t)n_edges * half, (const void**)&d.he))) return rc;
-    PCUDA(cudaMemcpy(p->d_gstatic + (size_t)model * 6, graph_static, sizeof(float) * 6, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->d_gstatic.get() + (size_t)model * 6, graph_static, sizeof(float) * 6, cudaMemcpyHostToDevice));
     hm.d = d;
     hm.set = true;
     p->emb_valid = false;
@@ -614,13 +572,13 @@ int ramp_policy_set_model(ramp_policy_t* p, int32_t model, int32_t n_nodes, int3
 }
 
 int ramp_policy_embed(ramp_policy_t* p, float* embeddings_out) {
-    if (!p) return perr(RAMP_ERR_BAD_ARG, "null policy");
-    PCUDA(cudaSetDevice(p->device));
+    if (!p) return set_error(RAMP_ERR_BAD_ARG, "null policy");
+    CUDA_TRY(cudaSetDevice(p->device));
     int rc = launch_embed(p, 0);
     if (rc != RAMP_OK) return rc;
-    PCUDA(cudaStreamSynchronize(0));
+    CUDA_TRY(cudaStreamSynchronize(0));
     if (embeddings_out)
-        PCUDA(cudaMemcpy(embeddings_out, p->d_emb, sizeof(float) * (size_t)p->P.c.n_models * p->P.c.out_features_node, cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(embeddings_out, p->d_emb.get(), sizeof(float) * (size_t)p->P.c.n_models * p->P.c.out_features_node, cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
 
@@ -635,23 +593,23 @@ int ramp_policy_decide(ramp_policy_t* p, int32_t n, const int32_t* model, const 
 }
 
 int ramp_policy_act(ramp_policy_t* p, ramp_engine_t* eng, int32_t sample, uint64_t seed) {
-    if (!p || !eng) return perr(RAMP_ERR_BAD_ARG, "null argument");
+    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     ramp_env_buffers_t eb{};
     int rc = ramp_env_buffers(eng, &eb);
     if (rc != RAMP_OK) return rc;
     const ramp_policy_config_t& c = p->P.c;
-    if (ramp_internal_device(eng) != p->device) return perr(RAMP_ERR_BAD_ARG, "policy and engine live on different devices");
-    if (eb.n_actions != c.n_actions) return perr(RAMP_ERR_BAD_ARG, "policy has %d actions, the environment %d", c.n_actions, eb.n_actions);
-    if (c.in_features_graph != 17) return perr(RAMP_ERR_BAD_ARG, "the environment emits 17 graph features, the policy expects %d", c.in_features_graph);
-    if (eb.n_models > c.n_models) return perr(RAMP_ERR_BAD_ARG, "the environment has %d job types, the policy %d", eb.n_models, c.n_models);
-    PCUDA(cudaSetDevice(p->device));
+    if (ramp_internal_device(eng) != p->device) return set_error(RAMP_ERR_BAD_ARG, "policy and engine live on different devices");
+    if (eb.n_actions != c.n_actions) return set_error(RAMP_ERR_BAD_ARG, "policy has %d actions, the environment %d", c.n_actions, eb.n_actions);
+    if (c.in_features_graph != 17) return set_error(RAMP_ERR_BAD_ARG, "the environment emits 17 graph features, the policy expects %d", c.in_features_graph);
+    if (eb.n_models > c.n_models) return set_error(RAMP_ERR_BAD_ARG, "the environment has %d job types, the policy %d", eb.n_models, c.n_models);
+    CUDA_TRY(cudaSetDevice(p->device));
     cudaStream_t st = ramp_internal_stream(eng);
     int launches = 1;
     if (!p->emb_valid) { if ((rc = launch_embed(p, st)) != RAMP_OK) return rc; ++launches; }
     if ((rc = ensure_outputs(p, eb.n_episodes)) != RAMP_OK) return rc;
     HeadArgs a{};
-    a.n = eb.n_episodes; a.obs_dyn = eb.obs_dynamic; a.graph_static = p->d_gstatic; a.model = eb.queued_model; a.done = eb.done;
-    a.mask = eb.action_mask; a.emb = p->d_emb; a.logits = p->d_logits; a.value = p->d_value; a.logp = p->d_logp; a.actions = eb.actions;
+    a.n = eb.n_episodes; a.obs_dyn = eb.obs_dynamic; a.graph_static = p->d_gstatic.get(); a.model = eb.queued_model; a.done = eb.done;
+    a.mask = eb.action_mask; a.emb = p->d_emb.get(); a.logits = p->d_logits.get(); a.value = p->d_value.get(); a.logp = p->d_logp.get(); a.actions = eb.actions;
     a.sample = sample; a.seed = seed ^ (0x9E3779B97F4A7C15ull * (++p->act_calls));
     if ((rc = launch_head(p, a, st)) != RAMP_OK) return rc;
     p->act_n = eb.n_episodes;
@@ -660,74 +618,66 @@ int ramp_policy_act(ramp_policy_t* p, ramp_engine_t* eng, int32_t sample, uint64
 }
 
 int ramp_policy_read(ramp_policy_t* p, ramp_engine_t* eng, float* logits_out, float* value_out, float* logp_out, int32_t* actions_out) {
-    if (!p || !eng) return perr(RAMP_ERR_BAD_ARG, "null argument");
+    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     ramp_env_buffers_t eb{};
     int rc = ramp_env_buffers(eng, &eb);
     if (rc != RAMP_OK) return rc;
-    if (eb.n_episodes != p->act_n) return perr(RAMP_ERR_BAD_ARG, "policy: nothing to read (ramp_policy_act was not called for this environment)");
+    if (eb.n_episodes != p->act_n) return set_error(RAMP_ERR_BAD_ARG, "policy: nothing to read (ramp_policy_act was not called for this environment)");
     cudaStream_t st = ramp_internal_stream(eng);
     const size_t B = (size_t)eb.n_episodes;
-    if (logits_out) PCUDA(cudaMemcpyAsync(logits_out, p->d_logits, sizeof(float) * B * p->P.c.n_actions, cudaMemcpyDeviceToHost, st));
-    if (value_out) PCUDA(cudaMemcpyAsync(value_out, p->d_value, sizeof(float) * B, cudaMemcpyDeviceToHost, st));
-    if (logp_out) PCUDA(cudaMemcpyAsync(logp_out, p->d_logp, sizeof(float) * B, cudaMemcpyDeviceToHost, st));
-    if (actions_out) PCUDA(cudaMemcpyAsync(actions_out, eb.actions, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, st));
-    PCUDA(cudaStreamSynchronize(st));
+    if (logits_out) CUDA_TRY(cudaMemcpyAsync(logits_out, p->d_logits.get(), sizeof(float) * B * p->P.c.n_actions, cudaMemcpyDeviceToHost, st));
+    if (value_out) CUDA_TRY(cudaMemcpyAsync(value_out, p->d_value.get(), sizeof(float) * B, cudaMemcpyDeviceToHost, st));
+    if (logp_out) CUDA_TRY(cudaMemcpyAsync(logp_out, p->d_logp.get(), sizeof(float) * B, cudaMemcpyDeviceToHost, st));
+    if (actions_out) CUDA_TRY(cudaMemcpyAsync(actions_out, eb.actions, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     return RAMP_OK;
 }
 
 void* ramp_pinned_alloc(size_t bytes) {
     void* ptr = nullptr;
-    if (cudaMallocHost(&ptr, bytes ? bytes : 1) != cudaSuccess) { perr(RAMP_ERR_CUDA, "cudaMallocHost(%zu) failed", bytes); return nullptr; }
+    if (cudaMallocHost(&ptr, bytes ? bytes : 1) != cudaSuccess) { set_error(RAMP_ERR_CUDA, "cudaMallocHost(%zu) failed", bytes); return nullptr; }
     return ptr;
 }
 
 void ramp_pinned_free(void* ptr) { if (ptr) cudaFreeHost(ptr); }
 
 int ramp_policy_trajectory_begin(ramp_policy_t* p, ramp_engine_t* eng, int32_t horizon) {
-    if (!p || !eng || horizon < 1) return perr(RAMP_ERR_BAD_ARG, "policy: bad trajectory horizon");
+    if (!p || !eng || horizon < 1) return set_error(RAMP_ERR_BAD_ARG, "policy: bad trajectory horizon");
     ramp_env_buffers_t eb{};
     int rc = ramp_env_buffers(eng, &eb);
     if (rc != RAMP_OK) return rc;
-    PCUDA(cudaSetDevice(p->device));
+    CUDA_TRY(cudaSetDevice(p->device));
     if (horizon == p->traj_h && eb.n_episodes == p->traj_b && eb.n_actions == p->traj_a) return RAMP_OK;
-    PCUDA(cudaStreamSynchronize(ramp_internal_stream(eng)));
-    cudaFree(p->t_obs); cudaFree(p->t_model); cudaFree(p->t_mask); cudaFree(p->t_action); cudaFree(p->t_logp); cudaFree(p->t_value);
-    cudaFree(p->t_reward); cudaFree(p->t_done);
-    p->t_obs = nullptr; p->t_model = nullptr; p->t_mask = nullptr; p->t_action = nullptr; p->t_logp = nullptr; p->t_value = nullptr;
-    p->t_reward = nullptr; p->t_done = nullptr; p->traj_h = 0;
+    CUDA_TRY(cudaStreamSynchronize(ramp_internal_stream(eng)));
+    p->traj_h = 0;                        // until every buffer has the new size
     const size_t n = (size_t)horizon * (size_t)eb.n_episodes;
-    PCUDA(cudaMalloc(&p->t_obs, sizeof(float) * 11 * n));
-    PCUDA(cudaMalloc(&p->t_model, sizeof(int32_t) * n));
-    PCUDA(cudaMalloc(&p->t_mask, (size_t)eb.n_actions * n));
-    PCUDA(cudaMalloc(&p->t_action, sizeof(int32_t) * n));
-    PCUDA(cudaMalloc(&p->t_logp, sizeof(float) * n));
-    PCUDA(cudaMalloc(&p->t_value, sizeof(float) * n));
-    PCUDA(cudaMalloc(&p->t_reward, sizeof(double) * n));
-    PCUDA(cudaMalloc(&p->t_done, n));
+    CUDA_TRY(alloc_each(n, p->t_model, p->t_action, p->t_logp, p->t_value, p->t_reward, p->t_done));
+    CUDA_TRY(p->t_obs.alloc(11 * n));
+    CUDA_TRY(p->t_mask.alloc((size_t)eb.n_actions * n));
     p->traj_h = horizon; p->traj_b = eb.n_episodes; p->traj_a = eb.n_actions;
     return RAMP_OK;
 }
 
 int ramp_policy_trajectory_record(ramp_policy_t* p, ramp_engine_t* eng, int32_t t, int32_t phase) {
-    if (!p || !eng) return perr(RAMP_ERR_BAD_ARG, "null argument");
-    if (p->traj_h < 1 || t < 0 || t >= p->traj_h) return perr(RAMP_ERR_BAD_ARG, "policy: trajectory slot %d outside [0, %d)", t, p->traj_h);
+    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (p->traj_h < 1 || t < 0 || t >= p->traj_h) return set_error(RAMP_ERR_BAD_ARG, "policy: trajectory slot %d outside [0, %d)", t, p->traj_h);
     ramp_env_buffers_t eb{};
     int rc = ramp_env_buffers(eng, &eb);
     if (rc != RAMP_OK) return rc;
     if (eb.n_episodes != p->traj_b || eb.n_actions != p->traj_a || eb.n_episodes != p->act_n)
-        return perr(RAMP_ERR_BAD_ARG, "policy: the trajectory was set up for another environment, or ramp_policy_act was not called");
+        return set_error(RAMP_ERR_BAD_ARG, "policy: the trajectory was set up for another environment, or ramp_policy_act was not called");
     cudaStream_t st = ramp_internal_stream(eng);
     const size_t B = (size_t)eb.n_episodes, o = (size_t)t * B;
     // phase 0: after ramp_policy_act, before the environment steps -- what the policy saw and decided;
     // phase 1: after the environment stepped -- what came back
     TrajArgs a{};
     a.B = eb.n_episodes; a.A = p->traj_a; a.phase = phase;
-    a.obs = eb.obs_dynamic; a.model = eb.queued_model; a.mask = eb.action_mask; a.action = eb.actions; a.logp = p->d_logp; a.value = p->d_value;
+    a.obs = eb.obs_dynamic; a.model = eb.queued_model; a.mask = eb.action_mask; a.action = eb.actions; a.logp = p->d_logp.get(); a.value = p->d_value.get();
     a.reward = eb.reward; a.done = eb.done;
-    a.t_obs = p->t_obs + o * 11; a.t_model = p->t_model + o; a.t_mask = p->t_mask + o * p->traj_a; a.t_action = p->t_action + o;
-    a.t_logp = p->t_logp + o; a.t_value = p->t_value + o; a.t_reward = p->t_reward + o; a.t_done = p->t_done + o;
+    a.t_obs = p->t_obs.get() + o * 11; a.t_model = p->t_model.get() + o; a.t_mask = p->t_mask.get() + o * p->traj_a; a.t_action = p->t_action.get() + o;
+    a.t_logp = p->t_logp.get() + o; a.t_value = p->t_value.get() + o; a.t_reward = p->t_reward.get() + o; a.t_done = p->t_done.get() + o;
     ramp_trajectory_record_kernel<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(a);
-    PCUDA(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     ramp_internal_count_launches(eng, 1);
     return RAMP_OK;
 }
@@ -735,19 +685,19 @@ int ramp_policy_trajectory_record(ramp_policy_t* p, ramp_engine_t* eng, int32_t 
 int ramp_policy_trajectory_read(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, float* obs_dynamic_out, int32_t* model_out,
                                 uint8_t* action_mask_out, int32_t* action_out, float* logp_out, float* value_out, double* reward_out,
                                 uint8_t* done_out) {
-    if (!p || !eng) return perr(RAMP_ERR_BAD_ARG, "null argument");
-    if (n_steps < 1 || n_steps > p->traj_h) return perr(RAMP_ERR_BAD_ARG, "policy: %d steps asked of a trajectory of %d", n_steps, p->traj_h);
+    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (n_steps < 1 || n_steps > p->traj_h) return set_error(RAMP_ERR_BAD_ARG, "policy: %d steps asked of a trajectory of %d", n_steps, p->traj_h);
     cudaStream_t st = ramp_internal_stream(eng);
     const size_t n = (size_t)n_steps * (size_t)p->traj_b;
-    if (obs_dynamic_out) PCUDA(cudaMemcpyAsync(obs_dynamic_out, p->t_obs, sizeof(float) * 11 * n, cudaMemcpyDeviceToHost, st));
-    if (model_out) PCUDA(cudaMemcpyAsync(model_out, p->t_model, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
-    if (action_mask_out) PCUDA(cudaMemcpyAsync(action_mask_out, p->t_mask, (size_t)p->traj_a * n, cudaMemcpyDeviceToHost, st));
-    if (action_out) PCUDA(cudaMemcpyAsync(action_out, p->t_action, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
-    if (logp_out) PCUDA(cudaMemcpyAsync(logp_out, p->t_logp, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
-    if (value_out) PCUDA(cudaMemcpyAsync(value_out, p->t_value, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
-    if (reward_out) PCUDA(cudaMemcpyAsync(reward_out, p->t_reward, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    if (done_out) PCUDA(cudaMemcpyAsync(done_out, p->t_done, n, cudaMemcpyDeviceToHost, st));
-    PCUDA(cudaStreamSynchronize(st));
+    if (obs_dynamic_out) CUDA_TRY(cudaMemcpyAsync(obs_dynamic_out, p->t_obs.get(), sizeof(float) * 11 * n, cudaMemcpyDeviceToHost, st));
+    if (model_out) CUDA_TRY(cudaMemcpyAsync(model_out, p->t_model.get(), sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
+    if (action_mask_out) CUDA_TRY(cudaMemcpyAsync(action_mask_out, p->t_mask.get(), (size_t)p->traj_a * n, cudaMemcpyDeviceToHost, st));
+    if (action_out) CUDA_TRY(cudaMemcpyAsync(action_out, p->t_action.get(), sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
+    if (logp_out) CUDA_TRY(cudaMemcpyAsync(logp_out, p->t_logp.get(), sizeof(float) * n, cudaMemcpyDeviceToHost, st));
+    if (value_out) CUDA_TRY(cudaMemcpyAsync(value_out, p->t_value.get(), sizeof(float) * n, cudaMemcpyDeviceToHost, st));
+    if (reward_out) CUDA_TRY(cudaMemcpyAsync(reward_out, p->t_reward.get(), sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    if (done_out) CUDA_TRY(cudaMemcpyAsync(done_out, p->t_done.get(), n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     return RAMP_OK;
 }
 

@@ -122,13 +122,14 @@ def load_library():
     L.ramp_debug_template_info.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_double)]
     L.ramp_launch_count.restype = C.c_int64
     L.ramp_launch_count.argtypes = [C.c_void_p]
+    L.ramp_debug_device_bytes.argtypes = [C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.ramp_get_lookahead_kernel_time.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64),
                                                  C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32]
     for name in ('ramp_engine_create', 'ramp_engine_destroy', 'ramp_register_template', 'ramp_template_count',
                  'ramp_reset', 'ramp_set_arrivals', 'ramp_step_host', 'ramp_step_device', 'ramp_sync', 'ramp_check_status',
                  'ramp_get_job_records', 'ramp_get_episode_state', 'ramp_episode_state_device', 'ramp_export_episode_state_to',
                  'ramp_get_episode_stats', 'ramp_get_memo_stats', 'ramp_get_memo_stats_ex', 'ramp_get_last_lookahead', 'ramp_run_lookaheads',
-                 'ramp_debug_template_info', 'ramp_get_lookahead_kernel_time'):
+                 'ramp_debug_template_info', 'ramp_debug_device_bytes', 'ramp_get_lookahead_kernel_time'):
         getattr(L, name).restype = C.c_int
     _lib = L
     return L
@@ -139,7 +140,7 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_step_device', 'ramp_sync', 'ramp_check_status', 'ramp_get_job_records',
                     'ramp_get_episode_state', 'ramp_episode_state_device', 'ramp_export_episode_state_to', 'ramp_get_episode_stats',
                     'ramp_get_memo_stats', 'ramp_get_memo_stats_ex',
-                    'ramp_get_last_lookahead', 'ramp_run_lookaheads', 'ramp_debug_template_info', 'ramp_launch_count',
+                    'ramp_get_last_lookahead', 'ramp_run_lookaheads', 'ramp_debug_template_info', 'ramp_launch_count', 'ramp_debug_device_bytes',
                     'ramp_get_lookahead_kernel_time', 'ramp_expand_template', 'ramp_free_expanded_job', 'ramp_free_expanded_aux', 'ramp_first_fit_place',
                     'ramp_quotient_template', 'ramp_free_quotient', 'ramp_get_quotient_bytes', 'ramp_set_job_count',
                     'ramp_set_limits', 'ramp_first_fit_place_many', 'ramp_env_create', 'ramp_env_set_template',
@@ -148,6 +149,14 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_policy_embed', 'ramp_policy_forward', 'ramp_policy_decide', 'ramp_policy_act', 'ramp_policy_read',
                     'ramp_pinned_alloc', 'ramp_pinned_free', 'ramp_policy_trajectory_begin', 'ramp_policy_trajectory_record', 'ramp_policy_trajectory_read',
                     'ramp_env_read_episode', 'ramp_env_set_agents', 'ramp_env_agent_act']
+
+
+def device_bytes():
+    """(device bytes, page-locked host bytes) that the library's engines and policies hold right now, over the whole process.
+    Unlike cudaMemGetInfo it does not move with other processes on the same GPU."""
+    dev, pinned = C.c_int64(), C.c_int64()
+    _check(load_library().ramp_debug_device_bytes(C.byref(dev), C.byref(pinned)))
+    return dev.value, pinned.value
 
 
 def _check(rc):

@@ -259,6 +259,9 @@ int ramp_debug_template_info(ramp_engine_t* eng, int32_t template_id, int32_t ou
 /* kernel launch counter (gpu_launches in bench.py) and device time spent in the lookahead kernel inside
  * ramp_step_* since the last call (CUDA events on the engine stream) */
 int64_t ramp_launch_count(ramp_engine_t* eng);
+/* Bytes of device memory and of page-locked host memory the library's engines and policies hold right now, over the whole
+ * process (either pointer may be NULL).  Memory ramp_pinned_alloc hands to the caller is not counted. */
+int ramp_debug_device_bytes(int64_t* device_bytes, int64_t* pinned_bytes);
 int ramp_get_lookahead_kernel_time(ramp_engine_t* eng, double* total_ms, int64_t* launches, int64_t* work_items,
                                    int64_t* algorithmic_bytes, int32_t reset);
 /* the same 20 N + 19 E + 12 T + 24 accounting on the sizes of the symmetry quotients the thread-per-lookahead kernel really
