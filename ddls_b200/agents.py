@@ -6,7 +6,8 @@ ddls_b200/csrc/ramp_env.cuh): ``Random``, ``SiPML``, ``AcceptableJCT``, ``MaxPar
 ``DeviceRampJobPartitioningEnvironment``, deciding from the action mask and queued job the environment left on the device.
 
 ``evaluate`` is EvalLoop (ddls/loops/eval_loop.py:26-134, "use for validating heuristics") for all the episodes at once: reset,
-then actor -> ``step_device()`` until every episode is done, then the episodes' ``episode_stats``.
+then actor -> ``step_device()`` until every episode is done, then the episodes' ``episode_stats`` and, on request, EvalLoop's
+per-env-step ``step_stats``.
 """
 from __future__ import annotations
 
@@ -55,13 +56,20 @@ class DeviceHeuristicAgents:
         _engine._check(self.env.eng._L.ramp_env_agent_act(self.env.eng._h, C.c_uint64(int(seed) & (2 ** 64 - 1))))
 
 
-def evaluate(env, actor, seed: int = 0, sample: bool = False):
+def evaluate(env, actor, seed: int = 0, sample: bool = False, step_stats: bool = False):
     """EvalLoop.run (loops/eval_loop.py:26-134) for every episode of a DeviceRampJobPartitioningEnvironment at once: reset, then
     ``jobs_per_episode`` rounds of actor -> ``env.step_device()`` (an env-step consumes the one queued job, so no episode takes
     more), then ``env.episode_stats()``.  actor: a DeviceHeuristicAgents, or a DeviceGNNPolicy (greedy unless ``sample``).  The
-    loop does not synchronise when ``prewarm()`` lets the device decide every placement.  Raises if an episode is not done."""
+    loop does not synchronise when ``prewarm()`` lets the device decide every placement.  Raises if an episode is not done.
+
+    step_stats=False returns ``env.episode_stats()``.  step_stats=True returns EvalLoop.run's ``{'step_stats': ...,
+    'episode_stats': ...}``: the device records every env-step's action, reward and reduced steps_log row while the loop runs
+    (``env.record_steps``), still without synchronising, and ``step_stats`` is ``env.recorded_steps()`` -- per key a list of B
+    arrays, one entry per env-step of the episode."""
     from .policy import DeviceGNNPolicy
     env.reset()
+    if step_stats:
+        env.record_steps(env.J)
     for t in range(env.J):
         if isinstance(actor, DeviceGNNPolicy):
             actor.act(env, sample=sample, seed=seed + t)
@@ -71,4 +79,8 @@ def evaluate(env, actor, seed: int = 0, sample: bool = False):
     _, _, done = env.read()                                # raises what a step would have raised
     if not done.all():
         raise Exception(f'{int((~done).sum())} of {env.B} episodes are not done after {env.J} env-steps')
-    return env.episode_stats()
+    if not step_stats:
+        return env.episode_stats()
+    steps = env.recorded_steps()
+    env.record_steps(0)
+    return {'step_stats': steps, 'episode_stats': env.episode_stats()}

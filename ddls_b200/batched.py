@@ -118,7 +118,8 @@ class BatchedRampJobPartitioningEnvironment:
         self.rng = np.random.default_rng(seed)
         self.script = script
         self.eng = _engine.RampEngine(n_episodes=self.B, n_cluster_workers=self.W, max_jobs=self.J, device=device,
-                                      memo_mode=memo_mode, trace_cap=8192, max_simulation_run_time=self.max_simulation_run_time)
+                                      memo_mode=memo_mode, trace_cap=8192, max_simulation_run_time=self.max_simulation_run_time,
+                                      env_step_stats=True)
         self.n_words = (self.W + 63) // 64
         self._servers = [(c, r, s) for c in range(self.shape.c) for r in range(self.shape.r) for s in range(self.shape.s)]
         self._server_index = {sv: i for i, sv in enumerate(self._servers)}
@@ -408,6 +409,14 @@ class BatchedRampJobPartitioningEnvironment:
         out.update(lists)
         return out
 
+    def env_step_stats(self):
+        """EvalLoop's results['step_stats'] entries for every episode's last env-step (loops/eval_loop.py:50-100), as [B] arrays keyed
+        by the cluster's steps_log names in its order (``engine.ENV_STEP_STATS``): every key reduced by the step kernel over the
+        cluster steps of the env-step, the fused empty ones included -- step_start_time the first value, step_end_time and
+        step_counter the last, 'mean' keys the mean, the others the sum; the per-tick utilisation lists the mean over every entry.
+        A finished episode keeps its last env-step's row.  ``step()``'s return value does not carry it."""
+        return _engine.env_step_columns(self.eng.env_step_stats())
+
     # ---- observations ---------------------------------------------------------------------------------------------
     def jobs_params(self):
         """(min, max) per PARAM_KEYS: the normalisers of the observation's job features (``jobs_params(models, ...)`` or the
@@ -691,6 +700,39 @@ class DeviceRampJobPartitioningEnvironment(BatchedRampJobPartitioningEnvironment
         L.ramp_env_read_state.restype = C.c_int
         L.ramp_env_read_state.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _engine._check(L.ramp_env_read_state(self.eng._h, None, None, out.ctypes.data))
+        return out
+
+    def record_steps(self, horizon: int):
+        """Keeps EvalLoop's results['step_stats'] on the device from now on (ramp_env_steplog_begin): every env-step's row, action
+        and reward for up to `horizon` env-steps per episode, written by each step without a synchronisation.  0 stops recording and
+        frees the record.  ``recorded_steps()`` reads it back."""
+        import ctypes as C
+        L = self.eng._L
+        L.ramp_env_steplog_begin.restype = C.c_int
+        L.ramp_env_steplog_begin.argtypes = [C.c_void_p, C.c_int32]
+        _engine._check(L.ramp_env_steplog_begin(self.eng._h, int(horizon)))
+        self._log_horizon = int(horizon)
+
+    def recorded_steps(self):
+        """EvalLoop's results['step_stats'] (loops/eval_loop.py:44-100) of every episode since ``record_steps``: ``action``,
+        ``reward`` and the ``engine.ENV_STEP_STATS`` keys, each a list of B arrays with one entry per env-step the episode took.
+        One copy back."""
+        import ctypes as C
+        H, B, K = getattr(self, '_log_horizon', 0), self.B, _engine.ENV_STEP_STATS_LEN
+        if H <= 0:
+            raise Exception('no env-step record: call record_steps(horizon) first')
+        stats, rewards = np.zeros((H, K, B)), np.zeros((H, B))
+        actions, n = np.zeros((H, B), dtype=np.int32), np.zeros(B, dtype=np.int32)
+        L = self.eng._L
+        L.ramp_env_steplog_read.restype = C.c_int
+        L.ramp_env_steplog_read.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 4
+        _engine._check(L.ramp_env_steplog_read(self.eng._h, H, stats.ctypes.data, actions.ctypes.data, rewards.ctypes.data, n.ctypes.data))
+        if (n > H).any():
+            raise Exception(f'an episode took {int(n.max())} env-steps, the record holds {H}')
+        cols = _engine.env_step_columns(stats.transpose(2, 0, 1))       # [B][H] per key
+        out = {'action': [actions[:n[b], b].astype(np.int64) for b in range(B)], 'reward': [rewards[:n[b], b].copy() for b in range(B)]}
+        for k in _engine.ENV_STEP_STATS:
+            out[k] = [cols[k][b, :n[b]] for b in range(B)]
         return out
 
     def _episode_tables(self):

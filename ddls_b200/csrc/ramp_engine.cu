@@ -109,7 +109,7 @@ struct ramp_engine {
     DeviceArray<double> d_es_export;     // [B][RAMP_ES_LEN] ramp_get_episode_stats
     // episode state: the view the kernels take, and its arrays
     EpisodeState ep{};
-    DeviceArray<double> ep_ef, ep_rf, tick_util; DeviceArray<int32_t> ep_ei, ep_ri, tick_util_n; DeviceArray<ramp_job_record_t> ep_rec;
+    DeviceArray<double> ep_ef, ep_es, ep_rf, tick_util; DeviceArray<int32_t> ep_ei, ep_ri, tick_util_n; DeviceArray<ramp_job_record_t> ep_rec;
     DeviceArray<ramp_arrival_t> d_arrivals;
     DeviceArray<int32_t> d_n_jobs_ep;
     // lookahead scratch
@@ -158,6 +158,8 @@ struct ramp_engine {
     PinnedArray<unsigned char> env_h_mirror;   // host arrays of ramp_env_host_mirror
     bool env_unchecked_decide = false;   // a ramp_env_decide without need_host_out has not been looked at yet
     bool env_agents_set = false;         // ramp_env_set_agents ran
+    DeviceArray<double> steplog_stats, steplog_rewards;   // ramp_env_steplog_begin: [horizon][RAMP_ENV_STEP_STATS_LEN][B], [horizon][B]
+    DeviceArray<int32_t> steplog_actions;                 // [horizon][B]
     // standalone lookahead buffers
     DeviceArray<WorkItem> sa_chunk_items;
     DeviceArray<ChunkDesc> sa_chunks;
@@ -1452,6 +1454,68 @@ int ramp_get_last_step_stats(ramp_engine_t* e, double* stats_out, int32_t* n_clu
     return ramp_sync(e);
 }
 
+
+int ramp_enable_env_step_stats(ramp_engine_t* e) {
+    if (!e) return set_error(RAMP_ERR_BAD_ARG, "null engine");
+    if (e->ep.es) return RAMP_OK;
+    const size_t B = (size_t)e->cfg.n_episodes;
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
+    CUDA_TRY(e->ep_es.alloc((size_t)ES_STRIDE * B));
+    CUDA_TRY(cudaMemset(e->ep_es.get(), 0, sizeof(double) * ES_STRIDE * B));
+    e->ep.es = e->ep_es.get();
+    return RAMP_OK;
+}
+
+// eval_loop.py:50-100: the rows the step kernel closed, the first RAMP_ENV_STEP_STATS_LEN of every episode's ES_STRIDE
+int ramp_get_env_step_stats(ramp_engine_t* e, double* out) {
+    if (!e || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (!e->ep.es) return set_error(RAMP_ERR_BAD_ARG, "env-step statistics are not kept (ramp_enable_env_step_stats)");
+    const size_t B = (size_t)e->cfg.n_episodes, K = RAMP_ENV_STEP_STATS_LEN;
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    CUDA_TRY(cudaMemcpy2DAsync(out, sizeof(double) * K, e->ep.es, sizeof(double) * ES_STRIDE, sizeof(double) * K, B,
+                               cudaMemcpyDeviceToHost, e->stream.get()));
+    return ramp_sync(e);
+}
+
+// eval_loop.py:44-100: results['step_stats'] of every episode, one row per env-step, written by ramp_env_update_kernel
+int ramp_env_steplog_begin(ramp_engine_t* e, int32_t horizon) {
+    if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
+    if (horizon < 0) return set_error(RAMP_ERR_BAD_ARG, "horizon %d < 0", horizon);
+    if (horizon > 0 && !e->ep.es) return set_error(RAMP_ERR_BAD_ARG, "env-step statistics are not kept (ramp_enable_env_step_stats)");
+    EnvDev& v = e->env;
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));      // no queued ramp_env_advance still writes the old record
+    v.log_horizon = 0; v.log_stats = nullptr; v.log_actions = nullptr; v.log_rewards = nullptr;
+    e->steplog_stats = {}; e->steplog_actions = {}; e->steplog_rewards = {};
+    if (horizon == 0) return RAMP_OK;
+    const size_t n = (size_t)horizon * v.B;
+    CUDA_TRY(e->steplog_stats.alloc(n * RAMP_ENV_STEP_STATS_LEN));
+    CUDA_TRY(alloc_each(n, e->steplog_rewards));
+    CUDA_TRY(alloc_each(n, e->steplog_actions));
+    CUDA_TRY(cudaMemsetAsync(e->steplog_stats.get(), 0, sizeof(double) * n * RAMP_ENV_STEP_STATS_LEN, e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(e->steplog_rewards.get(), 0, sizeof(double) * n, e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(e->steplog_actions.get(), 0, sizeof(int32_t) * n, e->stream.get()));
+    v.log_stats = e->steplog_stats.get(); v.log_actions = e->steplog_actions.get(); v.log_rewards = e->steplog_rewards.get();
+    v.log_horizon = horizon;
+    return RAMP_OK;
+}
+
+int ramp_env_steplog_read(ramp_engine_t* e, int32_t horizon, double* stats_out, int32_t* actions_out, double* rewards_out,
+                          int32_t* n_steps_out) {
+    if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
+    const EnvDev& v = e->env;
+    if (v.log_horizon <= 0) return set_error(RAMP_ERR_BAD_ARG, "no env-step record: call ramp_env_steplog_begin first");
+    if (horizon != v.log_horizon) return set_error(RAMP_ERR_BAD_ARG, "horizon %d != the record's %d", horizon, v.log_horizon);
+    const size_t n = (size_t)horizon * v.B;
+    cudaStream_t st = e->stream.get();
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, v.log_stats, sizeof(double) * n * RAMP_ENV_STEP_STATS_LEN, cudaMemcpyDeviceToHost, st));
+    if (actions_out) CUDA_TRY(cudaMemcpyAsync(actions_out, v.log_actions, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
+    if (rewards_out) CUDA_TRY(cudaMemcpyAsync(rewards_out, v.log_rewards, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    if (n_steps_out) CUDA_TRY(cudaMemcpyAsync(n_steps_out, v.n_decided, sizeof(int32_t) * v.B, cudaMemcpyDeviceToHost, st));
+    return ramp_sync(e);
+}
 
 int ramp_env_read_state(ramp_engine_t* e, uint64_t* busy_out, int32_t* actions_out, int32_t* n_decided_out) {
     if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");

@@ -41,6 +41,11 @@ struct EnvDev {
     int32_t* actions; double* reward; uint8_t* done; int32_t* queued_model; float* obs_dyn; uint8_t* action_mask;
     int32_t* need_host; int32_t* n_need_host;
     int32_t* err;                   // first episode with an invalid action (+1)
+    // EvalLoop's results['step_stats'] (ramp_env_steplog_begin; null / 0 when not recording)
+    double* log_stats;              // [log_horizon][RAMP_ENV_STEP_STATS_LEN][B]
+    int32_t* log_actions;           // [log_horizon][B]
+    double* log_rewards;            // [log_horizon][B]
+    int32_t log_horizon;
 };
 
 __device__ __forceinline__ int env_free_workers(const EnvDev& v, int b) {
@@ -144,6 +149,15 @@ __global__ void ramp_env_update_kernel(const EnvDev v, const EpisodeState ep, co
             v.reward[b] = was_live ? v.fail_reward : 0.0;
         }
         v.ret[b] = __dadd_rn(v.ret[b], v.reward[b]);
+        // eval_loop.py:44-100: env-step n_decided - 1 of a live episode -- its action, reward and the row the step kernel closed
+        const int row = v.n_decided[b] - 1;
+        if (was_live && row >= 0 && row < v.log_horizon) {
+            const size_t r = (size_t)row * B + b;
+            v.log_actions[r] = v.actions[b];
+            v.log_rewards[r] = v.reward[b];
+            for (int k = 0; k < RAMP_ENV_STEP_STATS_LEN; ++k)
+                v.log_stats[((size_t)row * RAMP_ENV_STEP_STATS_LEN + k) * B + b] = ep.es[(size_t)b * ES_STRIDE + k];
+        }
         if (accepted) {
             for (int w = 0; w < nw; ++w) v.job_mask[((size_t)b * J + q) * nw + w] = v.placed[(size_t)b * nw + w];
             v.job_tmpl[(size_t)b * J + q] = v.tid[b];

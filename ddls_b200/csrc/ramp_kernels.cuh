@@ -111,6 +111,11 @@ enum { RI_JOB_IDX = 0, RI_N_WORKERS, RI_N_CHANNELS, RI_COUNT };
 enum { EF_NOW = 0, EF_NEXT_ARRIVAL, EF_LAST_ARRIVAL, EF_LOAD_SUM,
        EF_ACC_INFO, EF_ACC_COMP_FRAC = EF_ACC_INFO + 7, EF_ACC_COMM_FRAC, EF_ACC_JOBS_RUNNING, EF_ACC_MOUNTED_WORKERS,
        EF_ACC_UTIL_MOUNTED, EF_ACC_UTIL_CLUSTER, EF_ACC_TICKS, EF_ACC_STEPS, EF_COUNT };
+// the env-step accumulators of EvalLoop's results['step_stats'] (eval_loop.py:50-100), next to the episode ones: RAMP_ESS_* and the
+// env-step's tick count, opened by the action step, folded over every cluster step of the env-step in cluster-step order and closed
+// into the env-step's row when it ends.  [B][ES_STRIDE]: one base address per episode, so that the fold adds no live registers to
+// the step kernel (with the [field][B] layout of ef, ptxas keeps one address per field and spills)
+enum { ES_TICKS = RAMP_ENV_STEP_STATS_LEN, ES_STRIDE };
 enum { EI_NUM_ARRIVED = 0, EI_NUM_COMPLETED, EI_NUM_BLOCKED, EI_QUEUED, EI_N_RUNNING, EI_STEP_COUNTER, EI_EVENT_SEQ,
        EI_LOAD_N, EI_STATUS, EI_DONE, EI_LAST_SLOT, EI_PLAN_SLOT, EI_PLAN_RAN, EI_COUNT };
 
@@ -119,6 +124,8 @@ struct EpisodeState {
     int32_t n_cluster_workers, queue_capacity;
     double eps, max_sim_time;
     double*  ef;                // [EF_COUNT][B]
+    double*  es;                // [B][ES_STRIDE] env-step accumulators; between env-steps the last env-step's row.  Null until
+                                //     ramp_enable_env_step_stats: the step kernel then skips them
     int32_t* ei;                // [EI_COUNT][B]
     double*  rf;                // [RF_COUNT][max_running][B]
     int32_t* ri;                // [RI_COUNT][max_running][B]
@@ -1088,6 +1095,39 @@ __global__ void ramp_step_kernel(const StepArgs s) {
             st[RAMP_SS_NUM_TICKS] = (double)n_iter;
             if (ep.tick_util) ep.tick_util_n[b] = n_iter;
             st[RAMP_SS_JOB_QUEUE_LENGTH] = EI(EI_QUEUED) >= 0 ? 1.0 : 0.0;                       // RCE:1082
+            if (s.ep.es) {
+                // eval_loop.py:50-97: this cluster step into the env-step's row, in cluster-step order; the action step (cs 0) opens
+                // it.  The end-of-episode blocks below come after RCE:1084 logged the step, so they are not in it
+                double* es = s.ep.es + (size_t)b * ES_STRIDE;
+                const bool open = cs == 0;
+#define RAMP_ES_ADD(e, src) es[e] = __dadd_rn(open ? 0.0 : es[e], st[src])
+                es[RAMP_ESS_STEP_COUNTER] = st[RAMP_SS_STEP_COUNTER];                               // eval_loop.py:96-97 last
+                if (open) es[RAMP_ESS_STEP_START_TIME] = st[RAMP_SS_STEP_START_TIME];                   // :66-68 first
+                es[RAMP_ESS_STEP_END_TIME] = st[RAMP_SS_STEP_END_TIME];                             // :70-72 last
+                RAMP_ES_ADD(RAMP_ESS_MEAN_NUM_MOUNTED_WORKERS, RAMP_SS_MEAN_NUM_MOUNTED_WORKERS);            // :74-83 'mean': sum here,
+                RAMP_ES_ADD(RAMP_ESS_MEAN_NUM_MOUNTED_CHANNELS, RAMP_SS_MEAN_NUM_MOUNTED_CHANNELS);          //   / cluster steps at the end
+                RAMP_ES_ADD(RAMP_ESS_MEAN_COMPUTE_THROUGHPUT, RAMP_SS_MEAN_COMPUTE_THROUGHPUT);
+                RAMP_ES_ADD(RAMP_ESS_MEAN_DEP_THROUGHPUT, RAMP_SS_MEAN_DEP_THROUGHPUT);
+                RAMP_ES_ADD(RAMP_ESS_MEAN_CLUSTER_THROUGHPUT, RAMP_SS_MEAN_CLUSTER_THROUGHPUT);
+                RAMP_ES_ADD(RAMP_ESS_MEAN_DEMAND_COMPUTE_THROUGHPUT, RAMP_SS_MEAN_DEMAND_COMPUTE_THROUGHPUT);
+                RAMP_ES_ADD(RAMP_ESS_MEAN_DEMAND_DEP_THROUGHPUT, RAMP_SS_MEAN_DEMAND_DEP_THROUGHPUT);
+                RAMP_ES_ADD(RAMP_ESS_MEAN_DEMAND_TOTAL_THROUGHPUT, RAMP_SS_MEAN_DEMAND_TOTAL_THROUGHPUT);
+                RAMP_ES_ADD(RAMP_ESS_MEAN_COMPUTE_OVERHEAD_FRAC, RAMP_SS_MEAN_COMPUTE_OVERHEAD_FRAC);
+                RAMP_ES_ADD(RAMP_ESS_MEAN_COMMUNICATION_OVERHEAD_FRAC, RAMP_SS_MEAN_COMMUNICATION_OVERHEAD_FRAC);
+                RAMP_ES_ADD(RAMP_ESS_MEAN_NUM_JOBS_RUNNING, RAMP_SS_MEAN_NUM_JOBS_RUNNING);
+                RAMP_ES_ADD(RAMP_ESS_MEAN_FLOW_THROUGHPUT, RAMP_SS_MEAN_FLOW_THROUGHPUT);
+                RAMP_ES_ADD(RAMP_ESS_NUM_JOBS_COMPLETED, RAMP_SS_NUM_JOBS_COMPLETED);                    // :85-94 the rest: np.sum
+                RAMP_ES_ADD(RAMP_ESS_NUM_JOBS_ARRIVED, RAMP_SS_NUM_JOBS_ARRIVED);
+                RAMP_ES_ADD(RAMP_ESS_NUM_JOBS_BLOCKED, RAMP_SS_NUM_JOBS_BLOCKED);
+#pragma unroll
+                for (int k = 0; k < 7; ++k) RAMP_ES_ADD(RAMP_ESS_COMPUTE_INFO_PROCESSED + k, RAMP_SS_COMPUTE_INFO_PROCESSED + k);
+                RAMP_ES_ADD(RAMP_ESS_STEP_TIME, RAMP_SS_STEP_TIME);
+                RAMP_ES_ADD(RAMP_ESS_JOB_QUEUE_LENGTH, RAMP_SS_JOB_QUEUE_LENGTH);
+                RAMP_ES_ADD(RAMP_ESS_MEAN_MOUNTED_WORKER_UTILISATION_FRAC, RAMP_SS_UTIL_MOUNTED_SUM);        // per-tick lists: sums
+                RAMP_ES_ADD(RAMP_ESS_MEAN_CLUSTER_WORKER_UTILISATION_FRAC, RAMP_SS_UTIL_CLUSTER_SUM);        //   and their length
+                RAMP_ES_ADD(ES_TICKS, RAMP_SS_NUM_TICKS);
+#undef RAMP_ES_ADD
+            }
             // RCE:1086-1106: this cluster step's contribution to episode_stats.  The addresses come from the kernel parameter, not
             // from EF()'s `ef`: the kernel sits at 254 registers, and through `ef` ptxas spilled 8 bytes
             {
@@ -1121,6 +1161,23 @@ __global__ void ramp_step_kernel(const StepArgs s) {
             }
             // RJPE:394-395: while len(job_queue) == 0 and not is_done(): step(Action())
             if (!s.fuse_empty_steps || done || EI(EI_QUEUED) >= 0) break;
+        }
+        if (s.ep.es) {
+            // the env-step ends: its row (eval_loop.py:74-83).  np.mean over the cluster steps is their sum (in order) / their number;
+            // the per-tick lists' mean is over every entry of the env-step
+            double* es = s.ep.es + (size_t)b * ES_STRIDE;
+            const double n = (double)n_cluster_steps;
+#define RAMP_ES_MEAN(e) es[e] = __ddiv_rn(es[e], n)
+            RAMP_ES_MEAN(RAMP_ESS_MEAN_NUM_MOUNTED_WORKERS); RAMP_ES_MEAN(RAMP_ESS_MEAN_NUM_MOUNTED_CHANNELS);
+            RAMP_ES_MEAN(RAMP_ESS_MEAN_COMPUTE_THROUGHPUT); RAMP_ES_MEAN(RAMP_ESS_MEAN_DEP_THROUGHPUT);
+            RAMP_ES_MEAN(RAMP_ESS_MEAN_CLUSTER_THROUGHPUT); RAMP_ES_MEAN(RAMP_ESS_MEAN_DEMAND_COMPUTE_THROUGHPUT);
+            RAMP_ES_MEAN(RAMP_ESS_MEAN_DEMAND_DEP_THROUGHPUT); RAMP_ES_MEAN(RAMP_ESS_MEAN_DEMAND_TOTAL_THROUGHPUT);
+            RAMP_ES_MEAN(RAMP_ESS_MEAN_COMPUTE_OVERHEAD_FRAC); RAMP_ES_MEAN(RAMP_ESS_MEAN_COMMUNICATION_OVERHEAD_FRAC);
+            RAMP_ES_MEAN(RAMP_ESS_MEAN_NUM_JOBS_RUNNING); RAMP_ES_MEAN(RAMP_ESS_MEAN_FLOW_THROUGHPUT);
+#undef RAMP_ES_MEAN
+            const double ticks = es[ES_TICKS];                     // >= 1: every cluster step ticks at least once
+            es[RAMP_ESS_MEAN_MOUNTED_WORKER_UTILISATION_FRAC] = __ddiv_rn(es[RAMP_ESS_MEAN_MOUNTED_WORKER_UTILISATION_FRAC], ticks);
+            es[RAMP_ESS_MEAN_CLUSTER_WORKER_UTILISATION_FRAC] = __ddiv_rn(es[RAMP_ESS_MEAN_CLUSTER_WORKER_UTILISATION_FRAC], ticks);
         }
         if (s.fuse_empty_steps) st0[RAMP_SS_DONE] = EI(EI_DONE) ? 1.0 : 0.0;
     } else {

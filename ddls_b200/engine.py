@@ -50,6 +50,23 @@ ES = {k: i for i, k in enumerate(ES_FIELDS)}
 ES_LEN = len(ES_FIELDS)
 ES_COUNTS = ('num_jobs_arrived', 'num_jobs_completed', 'num_jobs_blocked', 'num_cluster_steps', 'num_ticks')
 
+# EvalLoop's results['step_stats'] row of one env-step (loops/eval_loop.py:50-100), include/ramp_b200.h RAMP_ESS_*: the keys of the
+# cluster's steps_log in the order it first sees them; ENV_STEP_COUNTS are integers in the reference
+ENV_STEP_STATS = ['step_counter', 'step_start_time', 'mean_num_mounted_workers', 'mean_num_mounted_channels', 'mean_compute_throughput',
+                  'mean_dep_throughput', 'mean_cluster_throughput', 'mean_demand_compute_throughput', 'mean_demand_dep_throughput',
+                  'mean_demand_total_throughput', 'mean_compute_overhead_frac', 'mean_communication_overhead_frac',
+                  'mean_mounted_worker_utilisation_frac', 'mean_cluster_worker_utilisation_frac', 'num_jobs_completed',
+                  'mean_num_jobs_running', 'num_jobs_arrived', 'num_jobs_blocked', 'compute_info_processed', 'dep_info_processed',
+                  'flow_info_processed', 'cluster_info_processed', 'demand_compute_info_processed', 'demand_dep_info_processed',
+                  'demand_total_info_processed', 'step_end_time', 'step_time', 'mean_flow_throughput', 'job_queue_length']
+ENV_STEP_STATS_LEN = len(ENV_STEP_STATS)
+ENV_STEP_COUNTS = ('step_counter', 'num_jobs_completed', 'num_jobs_arrived', 'num_jobs_blocked', 'job_queue_length')
+
+
+def env_step_columns(rows):
+    """{name: rows[..., i]} for the RAMP_ESS_* columns of `rows` (last axis ENV_STEP_STATS_LEN), the counts as int64."""
+    return {k: rows[..., i].astype(np.int64) if k in ENV_STEP_COUNTS else rows[..., i].copy() for i, k in enumerate(ENV_STEP_STATS)}
+
 JS_NOT_ARRIVED, JS_QUEUED, JS_RUNNING, JS_COMPLETED, JS_BLOCKED = range(5)
 
 ACTION_DTYPE = np.dtype([('max_acceptable_jct', np.float64), ('part_op_mem', np.float64), ('part_dep_size', np.float64),
@@ -145,6 +162,7 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_quotient_template', 'ramp_free_quotient', 'ramp_get_quotient_bytes', 'ramp_set_job_count',
                     'ramp_set_limits', 'ramp_first_fit_place_many', 'ramp_env_create', 'ramp_env_set_template',
                     'ramp_env_reset', 'ramp_env_buffers', 'ramp_env_host_mirror', 'ramp_env_decide', 'ramp_env_patch', 'ramp_env_advance', 'ramp_env_read', 'ramp_get_last_step_stats', 'ramp_env_read_state',
+                    'ramp_enable_env_step_stats', 'ramp_get_env_step_stats', 'ramp_env_steplog_begin', 'ramp_env_steplog_read',
                     'ramp_enable_tick_lists', 'ramp_get_tick_lists', 'ramp_policy_weight_count', 'ramp_policy_create', 'ramp_policy_destroy', 'ramp_policy_set_weights', 'ramp_policy_set_model',
                     'ramp_policy_embed', 'ramp_policy_forward', 'ramp_policy_decide', 'ramp_policy_act', 'ramp_policy_read',
                     'ramp_pinned_alloc', 'ramp_pinned_free', 'ramp_policy_trajectory_begin', 'ramp_policy_trajectory_record', 'ramp_policy_trajectory_read',
@@ -175,7 +193,9 @@ class RampEngine:
 
     def __init__(self, n_episodes, n_cluster_workers, max_jobs, max_running=0, device=0, memo_mode=MEMO_REFERENCE,
                  trace_cap=0, max_templates=0, memo_capacity_log2=0, job_queue_capacity=10, machine_epsilon=1e-7,
-                 max_simulation_run_time=float('inf')):
+                 max_simulation_run_time=float('inf'), env_step_stats=False):
+        """env_step_stats: keep EvalLoop's per-env-step rows (``env_step_stats()``, ramp_enable_env_step_stats); the step kernel
+        skips them otherwise."""
         L = load_library()
         self._L = L
         cfg = _Config(device, n_episodes, n_cluster_workers, max_jobs, max_running, max_templates, memo_mode,
@@ -188,6 +208,10 @@ class RampEngine:
         self.trace_cap = trace_cap if trace_cap > 0 else 16384
         self.device = device
         self._templates = []
+        if env_step_stats:
+            L.ramp_enable_env_step_stats.restype = C.c_int
+            L.ramp_enable_env_step_stats.argtypes = [C.c_void_p]
+            _check(L.ramp_enable_env_step_stats(self._h))
 
     def close(self):
         if getattr(self, '_h', None):
@@ -294,6 +318,15 @@ class RampEngine:
         reset; rows of episodes that are not done hold the same formulas over the episode so far (include/ramp_b200.h)."""
         out = np.empty((self.n_episodes, ES_LEN), dtype=np.float64)
         _check(self._L.ramp_get_episode_stats(self._h, out.ctypes.data))
+        return out
+
+    def env_step_stats(self):
+        """[n_episodes, ENV_STEP_STATS_LEN] f64: every episode's last env-step row as the step kernel closed it (EvalLoop's
+        reduction over the cluster steps of the env-step, loops/eval_loop.py:50-100; include/ramp_b200.h RAMP_ESS_*)."""
+        out = np.empty((self.n_episodes, ENV_STEP_STATS_LEN), dtype=np.float64)
+        self._L.ramp_get_env_step_stats.restype = C.c_int
+        self._L.ramp_get_env_step_stats.argtypes = [C.c_void_p, C.c_void_p]
+        _check(self._L.ramp_get_env_step_stats(self._h, out.ctypes.data))
         return out
 
     def episode_state_device_ptr(self):

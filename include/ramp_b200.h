@@ -145,6 +145,25 @@ enum {
     RAMP_STEP_STATS_LEN
 };
 
+/* env-step statistics: EvalLoop's results['step_stats'] row of one env-step (loops/eval_loop.py:50-100), double[RAMP_ENV_STEP_STATS_LEN]
+ * per episode, in the order the cluster's steps_log first sees the keys (RCE:306-338, the outer loop RCE:962-982 when a job runs in
+ * the episode's first cluster step, RCE:1046-1084).  Every key is reduced over the cluster steps of the env-step, the fused empty
+ * steps after the action step included (RJPE:394-395): step_start_time takes the first value, step_end_time and step_counter the
+ * last, keys containing 'mean' the mean, the others the sum.  The two per-tick utilisation lists are reduced by the mean over every
+ * entry of the env-step. */
+enum {
+    RAMP_ESS_STEP_COUNTER = 0, RAMP_ESS_STEP_START_TIME, RAMP_ESS_MEAN_NUM_MOUNTED_WORKERS, RAMP_ESS_MEAN_NUM_MOUNTED_CHANNELS,
+    RAMP_ESS_MEAN_COMPUTE_THROUGHPUT, RAMP_ESS_MEAN_DEP_THROUGHPUT, RAMP_ESS_MEAN_CLUSTER_THROUGHPUT,
+    RAMP_ESS_MEAN_DEMAND_COMPUTE_THROUGHPUT, RAMP_ESS_MEAN_DEMAND_DEP_THROUGHPUT, RAMP_ESS_MEAN_DEMAND_TOTAL_THROUGHPUT,
+    RAMP_ESS_MEAN_COMPUTE_OVERHEAD_FRAC, RAMP_ESS_MEAN_COMMUNICATION_OVERHEAD_FRAC,
+    RAMP_ESS_MEAN_MOUNTED_WORKER_UTILISATION_FRAC, RAMP_ESS_MEAN_CLUSTER_WORKER_UTILISATION_FRAC,
+    RAMP_ESS_NUM_JOBS_COMPLETED, RAMP_ESS_MEAN_NUM_JOBS_RUNNING, RAMP_ESS_NUM_JOBS_ARRIVED, RAMP_ESS_NUM_JOBS_BLOCKED,
+    RAMP_ESS_COMPUTE_INFO_PROCESSED, RAMP_ESS_DEP_INFO_PROCESSED, RAMP_ESS_FLOW_INFO_PROCESSED, RAMP_ESS_CLUSTER_INFO_PROCESSED,
+    RAMP_ESS_DEMAND_COMPUTE_INFO_PROCESSED, RAMP_ESS_DEMAND_DEP_INFO_PROCESSED, RAMP_ESS_DEMAND_TOTAL_INFO_PROCESSED,
+    RAMP_ESS_STEP_END_TIME, RAMP_ESS_STEP_TIME, RAMP_ESS_MEAN_FLOW_THROUGHPUT, RAMP_ESS_JOB_QUEUE_LENGTH,
+    RAMP_ENV_STEP_STATS_LEN
+};
+
 /* job record table: one row per (episode, job idx) */
 enum { RAMP_JS_NOT_ARRIVED = 0, RAMP_JS_QUEUED = 1, RAMP_JS_RUNNING = 2, RAMP_JS_COMPLETED = 3, RAMP_JS_BLOCKED = 4 };
 typedef struct {
@@ -423,6 +442,22 @@ int ramp_enable_tick_lists(ramp_engine_t* eng, int32_t cap);
 int ramp_get_tick_lists(ramp_engine_t* eng, int32_t episode, double* mounted_out, double* cluster_out, int32_t cap, int32_t* n_out);
 /* step statistics / cluster-step counts of the last ramp_env_advance (the engine's own buffers): HOST [n_episodes][RAMP_STEP_STATS_LEN], [n_episodes] */
 int ramp_get_last_step_stats(ramp_engine_t* eng, double* stats_out, int32_t* n_cluster_steps_out);
+/* ramp_enable_env_step_stats makes the step kernel keep EvalLoop's per-env-step rows (both batched environments enable it; the
+ * engine alone does not pay for them).  The env-step row (RAMP_ESS_*) of every episode's last env-step -- the last step call with fuse_empty_steps, ramp_env_advance or
+ * ramp_step_host -- as the step kernel closed it: HOST [n_episodes][RAMP_ENV_STEP_STATS_LEN] (EvalLoop's reduction of one env-step,
+ * loops/eval_loop.py:50-100).  A finished episode keeps its last row. */
+int ramp_enable_env_step_stats(ramp_engine_t* eng);
+int ramp_get_env_step_stats(ramp_engine_t* eng, double* out);
+/* EvalLoop's results['step_stats'] for every episode, kept on the device (loops/eval_loop.py:44-100).  ramp_env_steplog_begin
+ * allocates room for `horizon` env-steps per episode ([horizon][RAMP_ENV_STEP_STATS_LEN][n_episodes] f64, actions and rewards
+ * [horizon][n_episodes]) and clears it; horizon 0 frees it.  From then on every ramp_env_advance writes, for every episode that was
+ * not done, env-step n_decided - 1's row, its action (as the agent chose it, before apply_action_mask=False turns an invalid one
+ * into 0, eval_loop.py:44-47) and its reward, on the engine stream without synchronising.  ramp_env_steplog_read copies the
+ * record back once: HOST stats [horizon][RAMP_ENV_STEP_STATS_LEN][n_episodes], actions / rewards [horizon][n_episodes], and
+ * n_steps [n_episodes], the env-steps each episode took (rows beyond `horizon` are not kept; any pointer may be NULL). */
+int ramp_env_steplog_begin(ramp_engine_t* eng, int32_t horizon);
+int ramp_env_steplog_read(ramp_engine_t* eng, int32_t horizon, double* stats_out, int32_t* actions_out, double* rewards_out,
+                          int32_t* n_steps_out);
 /* HOST copies of the occupancy [n_episodes][n_words], of the actions the device holds, and of the number of decisions every episode
  * has taken since ramp_env_reset (= its env-steps; a finished episode takes none) -- any may be NULL */
 int ramp_env_read_state(ramp_engine_t* eng, uint64_t* busy_out, int32_t* actions_out, int32_t* n_decided_out);

@@ -2,9 +2,10 @@
 reference's heuristic agents, on bench.py's config 3 (4,096 episodes of a 64-worker RAMP, the ResNet-50-like job, every block
 geometry prewarmed so that the loop never waits for the host).  Prints one line per agent: env-steps per second (live
 episodes' decisions over the wall time of evaluate(), which ends in a synchronise), and the episodes' mean acceptance rate,
-with the card's name and power limit.
+with the card's name and power limit.  --step-stats times evaluate(step_stats=True): the device also records every env-step's
+EvalLoop row, action and reward, and the timed window includes reading the record back.
 
-    python scripts/eval_rollouts.py [--episodes 4096] [--jobs 8] [--repeats 3]
+    python scripts/eval_rollouts.py [--episodes 4096] [--jobs 8] [--repeats 3] [--step-stats]
 """
 import argparse
 import json
@@ -33,6 +34,7 @@ def main():
     ap.add_argument('--jobs', type=int, default=8)
     ap.add_argument('--repeats', type=int, default=3)
     ap.add_argument('--seed', type=int, default=0)
+    ap.add_argument('--step-stats', action='store_true', help="evaluate(step_stats=True): EvalLoop's per-env-step record as well")
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -48,14 +50,16 @@ def main():
     name, power = card()
     for kind in AGENTS:
         agents = DeviceHeuristicAgents(env, kind)            # SiPML without a maximum: the largest valid degree
-        evaluate(env, agents, seed=args.seed)                # warm-up: memo, lookahead hints, module loads
+        evaluate(env, agents, seed=args.seed, step_stats=args.step_stats)     # warm-up: memo, lookahead hints, module loads
         rates = []
         for r in range(args.repeats):
             t0 = time.perf_counter()
-            es = evaluate(env, agents, seed=args.seed + r)
+            es = evaluate(env, agents, seed=args.seed + r, step_stats=args.step_stats)
             dt = time.perf_counter() - t0
+            if args.step_stats:
+                es = es['episode_stats']
             rates.append(float(env.decisions().sum()) / dt)
-        print(json.dumps({'agent': kind, 'episodes': args.episodes, 'jobs_per_episode': args.jobs,
+        print(json.dumps({'agent': kind, 'step_stats': args.step_stats, 'episodes': args.episodes, 'jobs_per_episode': args.jobs,
                           'env_steps_per_s': [round(x, 1) for x in rates], 'acceptance_rate': round(float(np.mean(es['acceptance_rate'])), 4),
                           'mean_return': round(float(np.mean(es['return'])), 4), 'card': name, 'power_limit': power}), flush=True)
     env.close()
