@@ -331,12 +331,17 @@ __global__ void ramp_trajectory_record_kernel(const TrajArgs a) {
 
 }  // namespace ramp
 
+#include "ramp_policy_learn.cuh"
+
 using namespace ramp;
 
 struct HostModel {
     ModelDev d{};
     std::vector<DeviceArray<unsigned char>> allocs;
     bool set = false;
+    GradModelDev g{};                     // the out-edge CSR (with `allocs`) and the learner's scratch (`lallocs`, made on first use)
+    std::vector<DeviceArray<unsigned char>> lallocs;
+    bool grad_ready = false;
 };
 
 struct ramp_policy {
@@ -360,8 +365,26 @@ struct ramp_policy {
     unsigned long long act_calls = 0;
     // trajectory of a rollout segment (ramp_policy_trajectory_*): [horizon][B] per field, on the device until read
     int32_t traj_h = 0, traj_b = 0, traj_a = 0;
+    int32_t traj_n = 0;                   // slots recorded in order, both phases, since ramp_policy_trajectory_begin
     DeviceArray<float> t_obs, t_logp, t_value; DeviceArray<int32_t> t_model, t_action;
     DeviceArray<uint8_t> t_mask, t_done; DeviceArray<double> t_reward;
+    // learner (ramp_policy_backward / ramp_ppo_loss_grad / ramp_policy_learn): gradient, Adam's moments and step count, per job type
+    // gradients, norm partials; per-row scratch for `lcap` rows, the head segments for `seg_n` rows
+    bool learner_ready = false, gmodels_ready = false;
+    int32_t adam_parity = 0, lcap = 0, seg_n = 0;
+    int64_t seg_total = 0;
+    DeviceArray<float> l_grad, l_adam_m, l_adam_v, l_gpart, l_rec, l_row_stats;
+    DeviceArray<int32_t> l_n_rows, l_step, l_row_model;
+    DeviceArray<double> l_norm_part, l_stats, l_mb_stats;
+    DeviceArray<Seg> l_segs;
+    DeviceArray<GradModelDev> d_gmodels;
+    // host-input batches of ramp_policy_backward / ramp_ppo_loss_grad
+    int32_t hcap = 0;
+    DeviceArray<int32_t> h_model, h_action; DeviceArray<float> h_gf, h_gl, h_gv, h_old, h_adv, h_vt; DeviceArray<uint8_t> h_mask;
+    // ramp_policy_learn's train batch ([horizon * B] rows, live rows first, t-major) and bootstrap values ([B])
+    int32_t bcap = 0, boot_cap = 0, b_rows = 0;
+    DeviceArray<float> b_obs, b_logp, b_logp_old, b_adv, b_vt, b_old, b_value, b_lpx, l_boot;
+    DeviceArray<int32_t> b_model, b_action, b_actx, l_boot_act; DeviceArray<uint8_t> b_mask; DeviceArray<double> b_adv64;
 };
 
 namespace {
@@ -472,6 +495,176 @@ int head_on_host(ramp_policy* p, int32_t n, const int32_t* model, const float* g
     return RAMP_OK;
 }
 
+// ---- the learner ----
+
+uint64_t mix64(uint64_t x) {              // splitmix64, as the kernels' splitmix64
+    x += 0x9E3779B97F4A7C15ull;
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+    return x ^ (x >> 31);
+}
+
+int64_t gnn_weight_count(const ramp_policy* p) { return p->P.gln_w; }     // the rounds come first in the blob
+
+int ensure_learner(ramp_policy* p) {
+    if (p->learner_ready) return RAMP_OK;
+    const size_t nw = (size_t)p->n_weights;
+    CUDA_TRY(alloc_each(nw, p->l_grad, p->l_adam_m, p->l_adam_v));
+    CUDA_TRY(p->l_gpart.alloc((size_t)p->P.c.n_models * gnn_weight_count(p)));
+    CUDA_TRY(p->l_n_rows.alloc(2));                                  // [0] learn's train batch, [1] a host batch
+    CUDA_TRY(p->l_step.alloc(2));
+    CUDA_TRY(p->l_norm_part.alloc(LRN_GRID));
+    CUDA_TRY(p->l_stats.alloc(RAMP_PPO_STATS_LEN));
+    CUDA_TRY(p->l_segs.alloc(HEAD_SEGS));
+    CUDA_TRY(p->d_gmodels.alloc(p->P.c.n_models));
+    CUDA_TRY(cudaMemset(p->l_adam_m.get(), 0, sizeof(float) * nw));
+    CUDA_TRY(cudaMemset(p->l_adam_v.get(), 0, sizeof(float) * nw));
+    CUDA_TRY(cudaMemset(p->l_step.get(), 0, sizeof(int32_t) * 2));
+    p->adam_parity = 0;
+    p->learner_ready = true;
+    return RAMP_OK;
+}
+
+// every job type's forward states and records for the embedding backward, sized by its graph
+int ensure_gmodels(ramp_policy* p) {
+    if (p->gmodels_ready) return RAMP_OK;
+    const ramp_policy_config_t& c = p->P.c;
+    const GnnDims D = gnn_dims(c);
+    const size_t half = c.out_features_msg / 2, R = c.num_rounds;
+    std::vector<GradModelDev> h(p->models.size());
+    for (size_t m = 0; m < h.size(); ++m) {
+        HostModel& hm = p->models[m];
+        if (!hm.set) return set_error(RAMP_ERR_BAD_ARG, "policy: model %zu was never registered (ramp_policy_set_model)", m);
+        if (!hm.grad_ready) {
+            hm.lallocs.clear();
+            const size_t N = hm.d.n_nodes, E = hm.d.n_edges;
+            auto take = [&](size_t floats, float** dst) -> int {
+                hm.lallocs.emplace_back();
+                CUDA_TRY(hm.lallocs.back().alloc(sizeof(float) * floats));
+                *dst = (float*)hm.lallocs.back().get();
+                return RAMP_OK;
+            };
+            GradModelDev& g = hm.g;
+            int rc;
+            if ((rc = take(R * N * D.zs, &g.z)) || (rc = take(R * N * half, &g.hn)) || (rc = take(R * E * half, &g.he)) ||
+                (rc = take(N * D.zs, &g.dz)) || (rc = take(N * D.zs, &g.dz2)) || (rc = take(N * half, &g.dhn)) ||
+                (rc = take(N * D.nrs, &g.nrec)) || (rc = take(E * D.ers, &g.erec)) || (rc = take((N + E) * D.mrs, &g.mrec)) ||
+                (rc = take((N + E) * c.out_features_msg, &g.mdx)))
+                return rc;
+            hm.grad_ready = true;
+        }
+        h[m] = hm.g;
+    }
+    CUDA_TRY(cudaMemcpy(p->d_gmodels.get(), h.data(), sizeof(GradModelDev) * h.size(), cudaMemcpyHostToDevice));
+    p->gmodels_ready = true;
+    return RAMP_OK;
+}
+
+// per-row scratch for minibatches of n rows, and the head segments summing exactly n rows
+int ensure_rows(ramp_policy* p, int32_t n) {
+    if (n > p->lcap) {
+        p->lcap = 0;
+        p->seg_n = 0;
+        CUDA_TRY(p->l_rec.alloc((size_t)n * head_rec(p->P.c).stride));
+        CUDA_TRY(p->l_row_stats.alloc((size_t)n * RS_N));
+        CUDA_TRY(p->l_row_model.alloc(n));
+        p->lcap = n;
+    }
+    if (n != p->seg_n) {
+        Seg s[HEAD_SEGS];
+        head_segs(p->P, p->l_rec.get(), n, s);
+        p->seg_total = 0;
+        for (const Seg& x : s) p->seg_total += seg_size(x);
+        CUDA_TRY(cudaMemcpy(p->l_segs.get(), s, sizeof(s), cudaMemcpyHostToDevice));
+        p->seg_n = n;
+    }
+    return RAMP_OK;
+}
+
+int prepare_learner(ramp_policy* p, cudaStream_t st) {
+    int rc;
+    if ((rc = ensure_learner(p)) != RAMP_OK || (rc = ensure_gmodels(p)) != RAMP_OK) return rc;
+    if (!p->emb_valid && (rc = launch_embed(p, st)) != RAMP_OK) return rc;
+    return RAMP_OK;
+}
+
+// the MeanPool rounds of every job type, kept for the backward (and the embeddings when `emb` is given); nothing for a minibatch
+// starting at `start` past the end of a batch of *n_rows rows (n_rows may be nullptr)
+int launch_states(ramp_policy* p, cudaStream_t st, const int32_t* n_rows, int32_t start, float* emb) {
+    EmbGradArgs eg{};
+    eg.n_rows = n_rows; eg.start = start; eg.emb = emb;
+    ramp_gnn_embed_grad_kernel<EMB_FORWARD><<<p->P.c.n_models, 256, 0, st>>>(p->P, p->d_models.get(), p->d_gmodels.get(), eg);
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
+}
+
+// head gradient -> head reduction -> embedding gradient (from launch_states' states) -> per-job-type sum and norm partials:
+// the gradient in l_grad
+int launch_grad(ramp_policy* p, GradArgs ga, cudaStream_t st) {
+    ga.rec = p->l_rec.get(); ga.row_model = p->l_row_model.get(); ga.row_stats = p->l_row_stats.get();
+    ga.emb = p->d_emb.get(); ga.graph_static = p->d_gstatic.get();
+    ramp_policy_head_grad_kernel<<<(ga.mb + LRN_WARPS - 1) / LRN_WARPS, LRN_WARPS * 32, 0, st>>>(p->P, ga);
+    int64_t grid = (p->seg_total + 255) / 256;
+    if (grid > 4 * p->sm_count) grid = 4 * p->sm_count;
+    ramp_policy_head_reduce_kernel<<<(unsigned)grid, 256, 0, st>>>(p->P, p->l_segs.get(), HEAD_SEGS, p->seg_total, p->l_grad.get());
+    EmbGradArgs eg{};
+    eg.rec = p->l_rec.get(); eg.row_model = p->l_row_model.get(); eg.rows = ga.mb; eg.gpart = p->l_gpart.get(); eg.n_gnn = gnn_weight_count(p);
+    ramp_gnn_embed_grad_kernel<EMB_BACKWARD><<<p->P.c.n_models, 256, 0, st>>>(p->P, p->d_models.get(), p->d_gmodels.get(), eg);
+    ramp_grad_finish_kernel<<<LRN_GRID, 256, 0, st>>>(p->l_gpart.get(), p->P.c.n_models, gnn_weight_count(p), p->n_weights,
+                                                       p->l_grad.get(), p->l_norm_part.get());
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
+}
+
+int check_ppo_config(const ramp_ppo_config_t* cfg) {
+    if (!cfg) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (cfg->sgd_minibatch_size < 1 || cfg->num_sgd_iter < 0) return set_error(RAMP_ERR_BAD_ARG, "ppo: sgd_minibatch_size must be >= 1, num_sgd_iter >= 0");
+    if (!(cfg->clip_param > 0) || !(cfg->vf_clip_param > 0) || !(cfg->lr >= 0) || !(cfg->adam_eps > 0))
+        return set_error(RAMP_ERR_BAD_ARG, "ppo: clip_param, vf_clip_param and adam_eps must be > 0, lr >= 0");
+    return RAMP_OK;
+}
+
+void ppo_terms(GradArgs& ga, const ramp_ppo_config_t& cfg) {
+    ga.clip = (float)cfg.clip_param; ga.vf_clip = (float)cfg.vf_clip_param; ga.vf_coeff = (float)cfg.vf_loss_coeff;
+    ga.ent_coeff = (float)cfg.entropy_coeff; ga.kl_coeff = (float)cfg.kl_coeff;
+}
+
+// the host inputs of ramp_policy_backward / ramp_ppo_loss_grad on the device (any pointer may be NULL: not copied)
+int upload_host_batch(ramp_policy* p, int32_t n, const int32_t* model, const float* gf, const uint8_t* mask, const float* gl,
+                      const float* gv, const int32_t* action, const float* old_logits, const float* adv, const float* vt) {
+    const ramp_policy_config_t& c = p->P.c;
+    const size_t A = c.n_actions;
+    if (n > p->hcap) {
+        p->hcap = 0;
+        CUDA_TRY(alloc_each(n, p->h_model, p->h_action, p->h_gv, p->h_adv, p->h_vt));
+        CUDA_TRY(p->h_gf.alloc((size_t)n * c.in_features_graph));
+        CUDA_TRY(alloc_each((size_t)n * A, p->h_gl, p->h_old, p->h_mask));
+        p->hcap = n;
+    }
+    auto put = [&](void* dst, const void* src, size_t bytes) -> int {
+        if (src) CUDA_TRY(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
+        return RAMP_OK;
+    };
+    int rc;
+    if ((rc = put(p->h_model.get(), model, 4 * (size_t)n)) || (rc = put(p->h_gf.get(), gf, 4 * (size_t)n * c.in_features_graph)) ||
+        (rc = put(p->h_mask.get(), mask, (size_t)n * A)) || (rc = put(p->h_gl.get(), gl, 4 * (size_t)n * A)) ||
+        (rc = put(p->h_gv.get(), gv, 4 * (size_t)n)) || (rc = put(p->h_action.get(), action, 4 * (size_t)n)) ||
+        (rc = put(p->h_old.get(), old_logits, 4 * (size_t)n * A)) || (rc = put(p->h_adv.get(), adv, 4 * (size_t)n)) ||
+        (rc = put(p->h_vt.get(), vt, 4 * (size_t)n)) || (rc = put(p->l_n_rows.get() + 1, &n, 4)))
+        return rc;
+    for (int32_t b = 0; b < n; ++b)
+        if (action && model[b] >= 0 && model[b] < c.n_models && (action[b] < 0 || action[b] >= c.n_actions))
+            return set_error(RAMP_ERR_BAD_ARG, "ppo: action %d of row %d outside [0, %d)", action[b], b, c.n_actions);
+    return RAMP_OK;
+}
+
+GradArgs host_batch_args(ramp_policy* p, int32_t n) {
+    GradArgs ga{};
+    ga.mb = n; ga.start = 0; ga.n_rows = p->l_n_rows.get() + 1;
+    ga.graph_features = p->h_gf.get(); ga.model = p->h_model.get(); ga.mask = p->h_mask.get();
+    return ga;
+}
+
 }  // namespace
 
 extern "C" {
@@ -536,7 +729,8 @@ int ramp_policy_set_model(ramp_policy_t* p, int32_t model, int32_t n_nodes, int3
     CUDA_TRY(cudaSetDevice(p->device));
     HostModel& hm = p->models[model];
     hm.allocs.clear();
-    hm.set = false;
+    hm.lallocs.clear();
+    hm.set = hm.grad_ready = p->gmodels_ready = false;
     // incoming-edge lists by destination, in edge order (the order DGL delivers a node's mailbox is not observable through a mean)
     std::vector<int32_t> ptr(n_nodes + 1, 0), ine(n_edges), ins(n_edges);
     for (int e = 0; e < n_edges; ++e) ptr[edges_dst[e] + 1]++;
@@ -564,7 +758,17 @@ int ramp_policy_set_model(ramp_policy_t* p, int32_t model, int32_t n_nodes, int3
     if ((rc = up(nullptr, sizeof(float) * (size_t)n_nodes * POL_MAX_DIM, (const void**)&d.z1))) return rc;
     if ((rc = up(nullptr, sizeof(float) * (size_t)n_nodes * half, (const void**)&d.hn))) return rc;
     if ((rc = up(nullptr, sizeof(float) * (size_t)n_edges * half, (const void**)&d.he))) return rc;
+    // outgoing-edge lists by source, in edge order: the backward gathers a node's message gradients through them
+    std::vector<int32_t> optr(n_nodes + 1, 0), oute(n_edges);
+    for (int e = 0; e < n_edges; ++e) optr[edges_src[e] + 1]++;
+    for (int v = 0; v < n_nodes; ++v) optr[v + 1] += optr[v];
+    std::vector<int32_t> ocur(optr.begin(), optr.end() - 1);
+    for (int e = 0; e < n_edges; ++e) oute[ocur[edges_src[e]]++] = e;
+    GradModelDev g{};
+    if ((rc = up(optr.data(), sizeof(int32_t) * optr.size(), (const void**)&g.out_ptr))) return rc;
+    if ((rc = up(oute.data(), sizeof(int32_t) * oute.size(), (const void**)&g.out_edge))) return rc;
     CUDA_TRY(cudaMemcpy(p->d_gstatic.get() + (size_t)model * 6, graph_static, sizeof(float) * 6, cudaMemcpyHostToDevice));
+    hm.g = g;
     hm.d = d;
     hm.set = true;
     p->emb_valid = false;
@@ -647,6 +851,7 @@ int ramp_policy_trajectory_begin(ramp_policy_t* p, ramp_engine_t* eng, int32_t h
     int rc = ramp_env_buffers(eng, &eb);
     if (rc != RAMP_OK) return rc;
     CUDA_TRY(cudaSetDevice(p->device));
+    p->traj_n = 0;
     if (horizon == p->traj_h && eb.n_episodes == p->traj_b && eb.n_actions == p->traj_a) return RAMP_OK;
     CUDA_TRY(cudaStreamSynchronize(ramp_internal_stream(eng)));
     p->traj_h = 0;                        // until every buffer has the new size
@@ -678,6 +883,7 @@ int ramp_policy_trajectory_record(ramp_policy_t* p, ramp_engine_t* eng, int32_t 
     a.t_logp = p->t_logp.get() + o; a.t_value = p->t_value.get() + o; a.t_reward = p->t_reward.get() + o; a.t_done = p->t_done.get() + o;
     ramp_trajectory_record_kernel<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(a);
     CUDA_TRY(cudaGetLastError());
+    if (phase == 1 && t == p->traj_n) p->traj_n = t + 1;
     ramp_internal_count_launches(eng, 1);
     return RAMP_OK;
 }
@@ -698,6 +904,200 @@ int ramp_policy_trajectory_read(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_
     if (reward_out) CUDA_TRY(cudaMemcpyAsync(reward_out, p->t_reward.get(), sizeof(double) * n, cudaMemcpyDeviceToHost, st));
     if (done_out) CUDA_TRY(cudaMemcpyAsync(done_out, p->t_done.get(), n, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
+    return RAMP_OK;
+}
+
+int ramp_policy_get_weights(ramp_policy_t* p, float* out) {
+    if (!p || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (!p->weights_set) return set_error(RAMP_ERR_BAD_ARG, "policy: no weights (ramp_policy_set_weights)");
+    CUDA_TRY(cudaSetDevice(p->device));
+    CUDA_TRY(cudaDeviceSynchronize());                                    // a learn call may still be updating them
+    CUDA_TRY(cudaMemcpy(out, p->d_w.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
+int ramp_policy_backward(ramp_policy_t* p, int32_t n, const int32_t* model, const float* graph_features, const uint8_t* action_mask,
+                         const float* grad_logits, const float* grad_value, float* grad_weights_out) {
+    if (!p || !model || !graph_features || !action_mask || !grad_logits || !grad_value || !grad_weights_out)
+        return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "policy: backward of %d rows", n);
+    CUDA_TRY(cudaSetDevice(p->device));
+    int rc;
+    if ((rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n)) ||
+        (rc = upload_host_batch(p, n, model, graph_features, action_mask, grad_logits, grad_value, nullptr, nullptr, nullptr, nullptr)))
+        return rc;
+    GradArgs ga = host_batch_args(p, n);
+    ga.grad_logits = p->h_gl.get(); ga.grad_value = p->h_gv.get();
+    if ((rc = launch_states(p, 0, nullptr, 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, 0)) != RAMP_OK) return rc;
+    CUDA_TRY(cudaStreamSynchronize(0));
+    CUDA_TRY(cudaMemcpy(grad_weights_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
+int ramp_ppo_loss_grad(ramp_policy_t* p, const ramp_ppo_config_t* cfg, int32_t n, const int32_t* model, const float* graph_features,
+                       const uint8_t* action_mask, const int32_t* action, const float* old_logits, const float* advantage,
+                       const float* value_target, float* grad_out, double* stats_out) {
+    if (!p || !model || !graph_features || !action_mask || !action || !old_logits || !advantage || !value_target)
+        return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = check_ppo_config(cfg);
+    if (rc != RAMP_OK) return rc;
+    if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "ppo: loss of %d rows", n);
+    CUDA_TRY(cudaSetDevice(p->device));
+    if ((rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n)) ||
+        (rc = upload_host_batch(p, n, model, graph_features, action_mask, nullptr, nullptr, action, old_logits, advantage, value_target)))
+        return rc;
+    GradArgs ga = host_batch_args(p, n);
+    ga.action = p->h_action.get(); ga.old_logits = p->h_old.get(); ga.adv = p->h_adv.get(); ga.vt = p->h_vt.get();
+    ppo_terms(ga, *cfg);
+    if ((rc = launch_states(p, 0, nullptr, 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, 0)) != RAMP_OK) return rc;
+    ramp_ppo_minibatch_stats_kernel<<<1, 1>>>(p->l_row_stats.get(), n, ga.vf_coeff, ga.ent_coeff, ga.kl_coeff, p->l_norm_part.get(), p->l_stats.get());
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(0));
+    if (grad_out) CUDA_TRY(cudaMemcpy(grad_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    if (stats_out) CUDA_TRY(cudaMemcpy(stats_out, p->l_stats.get(), sizeof(double) * RAMP_PPO_STATS_LEN, cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
+int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_ppo_config_t* cfg, double* stats_out) {
+    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = check_ppo_config(cfg);
+    if (rc != RAMP_OK) return rc;
+    ramp_env_buffers_t eb{};
+    if ((rc = ramp_env_buffers(eng, &eb)) != RAMP_OK) return rc;
+    if (n_steps < 1 || n_steps > p->traj_n)
+        return set_error(RAMP_ERR_BAD_ARG, "ppo: %d steps asked of a trajectory with %d recorded", n_steps, p->traj_n);
+    if (eb.n_episodes != p->traj_b || eb.n_actions != p->traj_a)
+        return set_error(RAMP_ERR_BAD_ARG, "ppo: the trajectory was recorded from another environment");
+    const ramp_policy_config_t& c = p->P.c;
+    CUDA_TRY(cudaSetDevice(p->device));
+    cudaStream_t st = ramp_internal_stream(eng);
+    const int32_t B = eb.n_episodes, rows = n_steps * B, mb = cfg->sgd_minibatch_size, n_mb = (rows + mb - 1) / mb;
+    if ((rc = prepare_learner(p, st)) || (rc = ensure_rows(p, mb))) return rc;
+    if (rows > p->bcap) {
+        p->bcap = 0;
+        CUDA_TRY(alloc_each(rows, p->b_logp, p->b_logp_old, p->b_adv, p->b_vt, p->b_value, p->b_lpx, p->b_model, p->b_action, p->b_actx, p->b_adv64));
+        CUDA_TRY(p->b_obs.alloc((size_t)rows * 11));
+        CUDA_TRY(alloc_each((size_t)rows * c.n_actions, p->b_mask, p->b_old));
+        p->bcap = rows;
+    }
+    if (B > p->boot_cap) {
+        p->boot_cap = 0;
+        CUDA_TRY(alloc_each(B, p->l_boot, p->l_boot_act));
+        p->boot_cap = B;
+    }
+    if ((size_t)n_mb * RAMP_PPO_STATS_LEN > p->l_mb_stats.size()) CUDA_TRY(p->l_mb_stats.alloc((size_t)n_mb * RAMP_PPO_STATS_LEN));
+    int launches = 2;                                                   // GAE, old logits
+    // 1. the value of the state after the last step (RLlib's truncate_episodes bootstrap): when the trajectory goes on, the value
+    //    act recorded in slot n_steps; after its last recorded slot, the environment's current state, by the head kernel on its
+    //    buffers -- not through ramp_policy_act, which mixes its call count into the seed and writes the action buffer
+    const float* boot = p->t_value.get() + (size_t)n_steps * B;
+    if (n_steps == p->traj_n) {
+        HeadArgs hb{};
+        hb.n = B; hb.obs_dyn = eb.obs_dynamic; hb.graph_static = p->d_gstatic.get(); hb.model = eb.queued_model; hb.done = eb.done;
+        hb.mask = eb.action_mask; hb.emb = p->d_emb.get(); hb.value = p->l_boot.get(); hb.actions = p->l_boot_act.get();
+        if ((rc = launch_head(p, hb, st)) != RAMP_OK) return rc;
+        boot = p->l_boot.get();
+        ++launches;
+    }
+    // 2. GAE, the live rows t-major, standardised advantages
+    GaeArgs ge{};
+    ge.T = n_steps; ge.B = B; ge.A = c.n_actions; ge.n_models = c.n_models; ge.standardize = cfg->standardize_advantages;
+    ge.gamma = cfg->gamma; ge.lambda = cfg->lambda;
+    ge.t_obs = p->t_obs.get(); ge.t_model = p->t_model.get(); ge.t_mask = p->t_mask.get(); ge.t_action = p->t_action.get();
+    ge.t_logp = p->t_logp.get(); ge.t_value = p->t_value.get(); ge.t_reward = p->t_reward.get(); ge.t_done = p->t_done.get();
+    ge.boot = boot; ge.adv64 = p->b_adv64.get();
+    ge.obs = p->b_obs.get(); ge.model = p->b_model.get(); ge.mask = p->b_mask.get(); ge.action = p->b_action.get(); ge.logp = p->b_logp.get();
+    ge.adv = p->b_adv.get(); ge.vt = p->b_vt.get(); ge.n_rows = p->l_n_rows.get();
+    ramp_ppo_gae_kernel<<<1, 1024, 0, st>>>(ge);
+    CUDA_TRY(cudaGetLastError());
+    // 3. the collection weights' logits of every row: the head kernel again, so they are act's bits
+    HeadArgs ho{};
+    ho.n = rows; ho.obs_dyn = p->b_obs.get(); ho.graph_static = p->d_gstatic.get(); ho.model = p->b_model.get(); ho.mask = p->b_mask.get();
+    ho.emb = p->d_emb.get(); ho.logits = p->b_old.get(); ho.value = p->b_value.get(); ho.logp = p->b_lpx.get(); ho.actions = p->b_actx.get();
+    if ((rc = launch_head(p, ho, st)) != RAMP_OK) return rc;
+    // 4. num_sgd_iter shuffled passes of minibatch updates; a minibatch past the batch's end (its size is on the device) is a no-op
+    GradArgs ga{};
+    ga.mb = mb; ga.n_rows = p->l_n_rows.get(); ga.shuffle = 1; ga.obs_dyn = p->b_obs.get(); ga.model = p->b_model.get();
+    ga.mask = p->b_mask.get(); ga.action = p->b_action.get(); ga.old_logits = p->b_old.get(); ga.adv = p->b_adv.get(); ga.vt = p->b_vt.get();
+    ppo_terms(ga, *cfg);
+    AdamArgs aa{};
+    aa.lr = cfg->lr; aa.beta1 = cfg->adam_beta1; aa.beta2 = cfg->adam_beta2;
+    aa.beta2_f = (float)cfg->adam_beta2; aa.one_m_beta1 = (float)(1.0 - cfg->adam_beta1); aa.one_m_beta2 = (float)(1.0 - cfg->adam_beta2);
+    aa.eps = (float)cfg->adam_eps;
+    aa.max_norm = (float)cfg->grad_clip; aa.n_rows = p->l_n_rows.get(); aa.mb = mb; aa.step = p->l_step.get();
+    aa.m = p->l_adam_m.get(); aa.v = p->l_adam_v.get(); aa.grad = p->l_grad.get(); aa.norm_part = p->l_norm_part.get(); aa.w = p->d_w.get();
+    aa.row_stats = p->l_row_stats.get(); aa.vf_coeff = ga.vf_coeff; aa.ent_coeff = ga.ent_coeff; aa.kl_coeff = ga.kl_coeff;
+    for (int pass = 0; pass < cfg->num_sgd_iter; ++pass) {
+        ga.key = mix64(cfg->seed ^ mix64((uint64_t)pass + 1));
+        ga.logp_old = pass == 0 ? p->b_logp_old.get() : nullptr;
+        for (int k = 0; k < n_mb; ++k) {
+            // the rounds at the current weights, kept for the backward; from the second minibatch on also the embeddings, which
+            // the previous update made stale (the first uses those the old logits were computed with)
+            ga.start = aa.start = k * mb;
+            if ((rc = launch_states(p, st, p->l_n_rows.get(), ga.start, pass || k ? p->d_emb.get() : nullptr)) != RAMP_OK ||
+                (rc = launch_grad(p, ga, st)) != RAMP_OK)
+                return rc;
+            aa.parity = p->adam_parity; p->adam_parity ^= 1;
+            aa.stats = p->l_mb_stats.get() + (size_t)k * RAMP_PPO_STATS_LEN;
+            ramp_adam_kernel<<<LRN_GRID, 256, 0, st>>>(aa, p->n_weights);
+            CUDA_TRY(cudaGetLastError());
+            launches += 6;
+        }
+    }
+    if (cfg->num_sgd_iter > 0) p->emb_valid = false;
+    p->b_rows = rows;
+    // 5. the last pass's statistics and the adapted KL coefficient: the call's one read-back
+    ramp_ppo_learn_stats_kernel<<<1, 1, 0, st>>>(p->l_mb_stats.get(), cfg->num_sgd_iter > 0 ? n_mb : 0, (float)cfg->kl_coeff,
+                                                 (float)cfg->kl_target, p->l_n_rows.get(), p->l_stats.get());
+    CUDA_TRY(cudaGetLastError());
+    ramp_internal_count_launches(eng, launches + 1);
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, p->l_stats.get(), sizeof(double) * RAMP_PPO_STATS_LEN, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return RAMP_OK;
+}
+
+int ramp_policy_train_batch_read(ramp_policy_t* p, ramp_engine_t* eng, int32_t* n_out, int32_t* model_out, int32_t* action_out,
+                                 float* logp_out, float* logp_old_out, float* advantage_out, float* value_target_out) {
+    if (!p || !eng || !n_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (p->b_rows < 1) return set_error(RAMP_ERR_BAD_ARG, "ppo: no train batch (ramp_policy_learn)");
+    cudaStream_t st = ramp_internal_stream(eng);
+    CUDA_TRY(cudaMemcpyAsync(n_out, p->l_n_rows.get(), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    const size_t n = (size_t)*n_out;
+    if (model_out) CUDA_TRY(cudaMemcpyAsync(model_out, p->b_model.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (action_out) CUDA_TRY(cudaMemcpyAsync(action_out, p->b_action.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (logp_out) CUDA_TRY(cudaMemcpyAsync(logp_out, p->b_logp.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (logp_old_out) CUDA_TRY(cudaMemcpyAsync(logp_old_out, p->b_logp_old.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (advantage_out) CUDA_TRY(cudaMemcpyAsync(advantage_out, p->b_adv.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (value_target_out) CUDA_TRY(cudaMemcpyAsync(value_target_out, p->b_vt.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return RAMP_OK;
+}
+
+int ramp_policy_learner_state(ramp_policy_t* p, float* exp_avg_out, float* exp_avg_sq_out, int32_t* step_out) {
+    if (!p) return set_error(RAMP_ERR_BAD_ARG, "null policy");
+    CUDA_TRY(cudaSetDevice(p->device));
+    if (!p->learner_ready) {
+        if (exp_avg_out) memset(exp_avg_out, 0, sizeof(float) * p->n_weights);
+        if (exp_avg_sq_out) memset(exp_avg_sq_out, 0, sizeof(float) * p->n_weights);
+        if (step_out) *step_out = 0;
+        return RAMP_OK;
+    }
+    CUDA_TRY(cudaDeviceSynchronize());                                    // a learn call may still be updating them
+    if (exp_avg_out) CUDA_TRY(cudaMemcpy(exp_avg_out, p->l_adam_m.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    if (exp_avg_sq_out) CUDA_TRY(cudaMemcpy(exp_avg_sq_out, p->l_adam_v.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    if (step_out) CUDA_TRY(cudaMemcpy(step_out, p->l_step.get() + p->adam_parity, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
+int ramp_policy_learner_reset(ramp_policy_t* p) {
+    if (!p) return set_error(RAMP_ERR_BAD_ARG, "null policy");
+    CUDA_TRY(cudaSetDevice(p->device));
+    if (!p->learner_ready) return RAMP_OK;
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemset(p->l_adam_m.get(), 0, sizeof(float) * p->n_weights));
+    CUDA_TRY(cudaMemset(p->l_adam_v.get(), 0, sizeof(float) * p->n_weights));
+    CUDA_TRY(cudaMemset(p->l_step.get(), 0, sizeof(int32_t) * 2));
     return RAMP_OK;
 }
 

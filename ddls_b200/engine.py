@@ -166,7 +166,9 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_enable_tick_lists', 'ramp_get_tick_lists', 'ramp_policy_weight_count', 'ramp_policy_create', 'ramp_policy_destroy', 'ramp_policy_set_weights', 'ramp_policy_set_model',
                     'ramp_policy_embed', 'ramp_policy_forward', 'ramp_policy_decide', 'ramp_policy_act', 'ramp_policy_read',
                     'ramp_pinned_alloc', 'ramp_pinned_free', 'ramp_policy_trajectory_begin', 'ramp_policy_trajectory_record', 'ramp_policy_trajectory_read',
-                    'ramp_env_read_episode', 'ramp_env_set_agents', 'ramp_env_agent_act']
+                    'ramp_env_read_episode', 'ramp_env_set_agents', 'ramp_env_agent_act', 'ramp_policy_get_weights',
+                    'ramp_policy_backward', 'ramp_ppo_loss_grad', 'ramp_policy_learn', 'ramp_policy_train_batch_read',
+                    'ramp_policy_learner_state', 'ramp_policy_learner_reset']
 
 
 def device_bytes():

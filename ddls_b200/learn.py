@@ -1,0 +1,151 @@
+"""RLlib's PPO learner step for the device GNN policy (include/ramp_b200.h: ramp_ppo_loss_grad, ramp_policy_learn).
+
+``DevicePPOLearner(policy, config).learn(env, horizon)`` learns from the rollout segment the policy's last ``collect(env, ...)``
+recorded (``collect_and_learn`` does both) without moving the batch to the host: GAE and advantage standardisation, ``num_sgd_iter`` shuffled passes of minibatch PPO loss
+gradients, global-norm clipping and Adam, all on the device.  ``PPOConfig``'s defaults are the reference's tuned PPO settings
+(scripts/ramp_job_partitioning_configs/algo/ppo.yaml; lambda is RLlib's default 1.0).
+
+The loss, GAE and the KL-coefficient update restate RLlib's PPO (ppo_torch_policy.py, postprocessing.compute_advantages,
+PPO.update_kl) as published for the ray the reference pins; RLlib itself is not installed, so they are pinned against a float64
+restatement (tests/test_ppo_model.py, tests/test_gpu_policy_learn.py), not against RLlib.
+
+There is no CPU fallback: the CUDA library is required."""
+from __future__ import annotations
+
+import ctypes as C
+import dataclasses
+import time
+from typing import Dict
+
+import numpy as np
+
+from . import engine as _engine
+
+STATS = ('total_loss', 'policy_loss', 'vf_loss', 'entropy', 'kl', 'clip_frac', 'grad_gnorm', 'kl_coeff', 'rows')
+
+
+@dataclasses.dataclass
+class PPOConfig:
+    gamma: float = 0.997
+    lambda_: float = 1.0
+    clip_param: float = 0.18
+    vf_clip_param: float = 128.8
+    vf_loss_coeff: float = 0.5
+    entropy_coeff: float = 0.003
+    kl_coeff: float = 0.01
+    kl_target: float = 0.001
+    grad_clip: float = 1.5            # <= 0: no clipping
+    lr: float = 2.785e-4
+    sgd_minibatch_size: int = 128
+    num_sgd_iter: int = 50
+    adam_beta1: float = 0.9
+    adam_beta2: float = 0.999
+    adam_eps: float = 1e-8
+    standardize_advantages: bool = True
+    seed: int = 0
+
+
+class _CConfig(C.Structure):
+    _fields_ = [('seed', C.c_uint64)] + [(n, C.c_double) for n in (
+        'gamma', 'lambda_', 'clip_param', 'vf_clip_param', 'vf_loss_coeff', 'entropy_coeff', 'kl_coeff', 'kl_target', 'grad_clip', 'lr',
+        'adam_beta1', 'adam_beta2', 'adam_eps')] + [('sgd_minibatch_size', C.c_int32), ('num_sgd_iter', C.c_int32),
+                                                    ('standardize_advantages', C.c_int32)]
+
+
+def c_config(cfg: PPOConfig) -> _CConfig:
+    c = _CConfig()
+    for f in _CConfig._fields_:
+        v = getattr(cfg, f[0])
+        setattr(c, f[0], int(v) & (2 ** 64 - 1) if f[0] == 'seed' else (int(v) if f[1] is C.c_int32 else float(v)))
+    return c
+
+
+def _bind(L):
+    if getattr(L, '_learn_bound', False):
+        return
+    L.ramp_ppo_loss_grad.restype = C.c_int
+    L.ramp_ppo_loss_grad.argtypes = [C.c_void_p, C.POINTER(_CConfig), C.c_int32] + [C.c_void_p] * 9
+    L.ramp_policy_learn.restype = C.c_int
+    L.ramp_policy_learn.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CConfig), C.c_void_p]
+    L.ramp_policy_train_batch_read.restype = C.c_int
+    L.ramp_policy_train_batch_read.argtypes = [C.c_void_p, C.c_void_p] + [C.c_void_p] * 7
+    L.ramp_policy_learner_state.restype = C.c_int
+    L.ramp_policy_learner_state.argtypes = [C.c_void_p] * 4
+    L.ramp_policy_learner_reset.restype = C.c_int
+    L.ramp_policy_learner_reset.argtypes = [C.c_void_p]
+    L._learn_bound = True
+
+
+def _stats(raw) -> Dict[str, float]:
+    return {k: float(v) for k, v in zip(STATS, raw)}
+
+
+class DevicePPOLearner:
+    def __init__(self, policy, config: PPOConfig = None):
+        """policy: a DeviceGNNPolicy, whose weights the learner updates in place (Adam's state lives with the policy)."""
+        self.policy = policy
+        self.config = dataclasses.replace(config) if config is not None else PPOConfig()
+        self._L = policy._L
+        _bind(self._L)
+        self._calls = 0
+
+    def collect_and_learn(self, env, horizon: int, seed: int = 0) -> Dict[str, float]:
+        """policy.collect(env, horizon) then learn(); also returns the wall time of each (seconds) and the segment's trajectory."""
+        t0 = time.perf_counter()
+        traj = self.policy.collect(env, horizon, sample=True, seed=seed)
+        t1 = time.perf_counter()
+        stats = self.learn(env, horizon)
+        stats['collect_s'], stats['learn_s'] = t1 - t0, time.perf_counter() - t1
+        return stats, traj
+
+    def learn(self, env, horizon: int) -> Dict[str, float]:
+        """One PPO learner step on the first ``horizon`` steps of the segment the policy's last collect(env, ...) recorded (a shorter
+        horizon bootstraps its advantages with the value recorded at the next step): the statistics averaged over the
+        last pass's minibatches (STATS); kl_coeff is the adapted coefficient, which this learner uses from the next call on.
+        Call k of this learner shuffles with the seed config.seed + k."""
+        cfg = dataclasses.replace(self.config, seed=self.config.seed + self._calls)
+        out = np.zeros(len(STATS), dtype=np.float64)
+        _engine._check(self._L.ramp_policy_learn(self.policy._h, env.eng._h, int(horizon), C.byref(c_config(cfg)), out.ctypes.data))
+        self._calls += 1
+        stats = _stats(out)
+        self.config.kl_coeff = stats['kl_coeff']
+        return stats
+
+    def train_batch(self, env) -> Dict[str, np.ndarray]:
+        """the last learn()'s train batch: per live row, t-major, the job type, action, collected log-probability, the one
+        recomputed from the collection weights, the advantage (standardised when configured) and the value target"""
+        cap = self.policy._traj_key[0] * env.B            # the segment's rows: (horizon, B, |A|) of the last collect()
+        n = C.c_int32()
+        arrs = {'model': np.zeros(cap, np.int32), 'action': np.zeros(cap, np.int32), 'logp': np.zeros(cap, np.float32),
+                'logp_old': np.zeros(cap, np.float32), 'advantage': np.zeros(cap, np.float32), 'value_target': np.zeros(cap, np.float32)}
+        _engine._check(self._L.ramp_policy_train_batch_read(self.policy._h, env.eng._h, C.byref(n), *[a.ctypes.data for a in arrs.values()]))
+        return {k: v[:n.value].copy() for k, v in arrs.items()}
+
+    def loss_and_grad(self, batch: Dict[str, np.ndarray]):
+        """PPO's loss statistics (STATS) and gradient (blob order) on one minibatch of host arrays, with no update: model [n],
+        graph_features [n, in_features_graph], action_mask [n, |A|], action [n], old_logits [n, |A|], advantage [n],
+        value_target [n]."""
+        pol = self.policy
+        model, gf, mask = pol._host_inputs(batch['model'], batch['graph_features'], batch['action_mask'])
+        n, A = len(model), pol.n_actions
+        act = np.ascontiguousarray(batch['action'], dtype=np.int32).reshape(n)
+        old = np.ascontiguousarray(batch['old_logits'], dtype=np.float32).reshape(n, A)
+        adv = np.ascontiguousarray(batch['advantage'], dtype=np.float32).reshape(n)
+        vt = np.ascontiguousarray(batch['value_target'], dtype=np.float32).reshape(n)
+        grad = np.zeros(pol._L.ramp_policy_weight_count(C.byref(pol._cfg)), dtype=np.float32)
+        out = np.zeros(len(STATS), dtype=np.float64)
+        _engine._check(self._L.ramp_ppo_loss_grad(pol._h, C.byref(c_config(self.config)), n, model.ctypes.data, gf.ctypes.data,
+                                                  mask.ctypes.data, act.ctypes.data, old.ctypes.data, adv.ctypes.data, vt.ctypes.data,
+                                                  grad.ctypes.data, out.ctypes.data))
+        return _stats(out), grad
+
+    def adam_state(self):
+        """torch.optim.Adam's state of the flat weight vector: exp_avg, exp_avg_sq (blob order) and the step count"""
+        n = self._L.ramp_policy_weight_count(C.byref(self.policy._cfg))
+        m, v, step = np.zeros(n, np.float32), np.zeros(n, np.float32), C.c_int32()
+        _engine._check(self._L.ramp_policy_learner_state(self.policy._h, m.ctypes.data, v.ctypes.data, C.byref(step)))
+        return m, v, step.value
+
+    def reset(self):
+        """zero Adam's moments and step count"""
+        _engine._check(self._L.ramp_policy_learner_reset(self.policy._h))

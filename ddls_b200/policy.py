@@ -81,6 +81,10 @@ def _bind(L):
     L.ramp_policy_trajectory_record.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32]
     L.ramp_policy_trajectory_read.restype = C.c_int
     L.ramp_policy_trajectory_read.argtypes = [C.c_void_p, C.c_void_p, C.c_int32] + [C.c_void_p] * 8
+    L.ramp_policy_get_weights.restype = C.c_int
+    L.ramp_policy_get_weights.argtypes = [C.c_void_p, C.c_void_p]
+    L.ramp_policy_backward.restype = C.c_int
+    L.ramp_policy_backward.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 6
     L._policy_bound = True
 
 
@@ -136,6 +140,20 @@ def pack_weights(state_dict: Dict, config: Dict, n_actions: int) -> np.ndarray:
             raise ValueError(f'{k}: shape {tuple(v.shape)}, the configuration needs {shapes[k]}')
         parts.append(np.ascontiguousarray(v, dtype=np.float32).ravel())
     return np.concatenate(parts)
+
+
+def unpack_weights(blob, config: Dict, n_actions: int) -> Dict[str, np.ndarray]:
+    """The state_dict of a flat blob, reference key names and shapes (pack_weights' inverse)."""
+    blob = np.asarray(blob, dtype=np.float32)
+    shapes = weight_shapes(config, n_actions)
+    out, at = {}, 0
+    for k in weight_keys(config):
+        n = int(np.prod(shapes[k]))
+        out[k] = blob[at:at + n].reshape(shapes[k]).copy()
+        at += n
+    if at != len(blob):
+        raise ValueError(f'blob has {len(blob)} weights, the configuration {at}')
+    return out
 
 
 def random_state_dict(config: Dict, n_actions: int, seed: int = 0) -> Dict[str, np.ndarray]:
@@ -203,6 +221,28 @@ class DeviceGNNPolicy:
         blob = state_dict if isinstance(state_dict, np.ndarray) else pack_weights(state_dict, self.config, self.n_actions)
         blob = np.ascontiguousarray(blob, dtype=np.float32)
         _engine._check(self._L.ramp_policy_set_weights(self._h, blob.ctypes.data, len(blob)))
+
+    def get_weights(self) -> np.ndarray:
+        """the current weight blob (after a learner step: the updated weights)"""
+        out = np.zeros(self._L.ramp_policy_weight_count(C.byref(self._cfg)), dtype=np.float32)
+        _engine._check(self._L.ramp_policy_get_weights(self._h, out.ctypes.data))
+        return out
+
+    def state_dict(self) -> Dict[str, np.ndarray]:
+        """the current weights under the reference's GNNPolicy key names and shapes (loadable into its checkpoint)"""
+        return unpack_weights(self.get_weights(), self.config, self.n_actions)
+
+    def backward(self, model, graph_features, action_mask, grad_logits, grad_value) -> np.ndarray:
+        """gradient of sum(grad_logits * logits) + sum(grad_value * value) with respect to every weight (blob order) for forward()'s
+        inputs: grad_logits [n, |A|], grad_value [n]"""
+        model, gf, mask = self._host_inputs(model, graph_features, action_mask)
+        n = len(model)
+        gl = _shaped('grad_logits', np.ascontiguousarray(grad_logits, dtype=np.float32), (n, self.n_actions))
+        gv = _shaped('grad_value', np.ascontiguousarray(grad_value, dtype=np.float32), (n,))
+        out = np.zeros(self._L.ramp_policy_weight_count(C.byref(self._cfg)), dtype=np.float32)
+        _engine._check(self._L.ramp_policy_backward(self._h, n, model.ctypes.data, gf.ctypes.data, mask.ctypes.data, gl.ctypes.data,
+                                                    gv.ctypes.data, out.ctypes.data))
+        return out
 
     def embed(self):
         out = np.zeros((self.n_models, self.config['out_features_node']), dtype=np.float32)

@@ -550,6 +550,74 @@ int ramp_policy_trajectory_read(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_
                                 uint8_t* action_mask_out, int32_t* action_out, float* logp_out, float* value_out, double* reward_out,
                                 uint8_t* done_out);
 
+/* ---- the policy's gradient and RLlib's PPO learner step on the device.  fp32 kernels; every weight gradient is summed over the
+ * rows (and a job type's nodes, edges and messages) in a fixed order with f64 accumulators and no atomics, so one call on one
+ * batch gives the same bits every time.  Derivatives as torch defines them: relu (y > 0), leaky_relu (y > 0 ? 1 : 0.01), tanh
+ * (1 - y^2), LayerNorm with a biased variance and eps 1e-5; a zero-in-degree node passes no gradient (its output is the constant 0). */
+/* HOST copy of the current weight blob [ramp_policy_weight_count] (after a learn call: the updated weights) */
+int ramp_policy_get_weights(ramp_policy_t* p, float* out);
+/* gradient of sum(grad_logits . logits) + sum(grad_value . value) with respect to every weight, in blob order, for the read-out on
+ * HOST inputs (as ramp_policy_forward): grad_logits [n][n_actions], grad_value [n] -> grad_weights_out [ramp_policy_weight_count].
+ * The mask is added to the logits with derivative 1 (torch: logits + max(log(mask), finfo.min)); rows whose model is outside
+ * [0, n_models) contribute nothing. */
+int ramp_policy_backward(ramp_policy_t* p, int32_t n, const int32_t* model, const float* graph_features, const uint8_t* action_mask,
+                         const float* grad_logits, const float* grad_value, float* grad_weights_out);
+
+/* PPO's settings (RLlib PPOConfig names; scripts/ramp_job_partitioning_configs/algo/ppo.yaml holds the reference's values) */
+typedef struct {
+    uint64_t seed;                        /* minibatch shuffles: pass p draws its permutation from splitmix64 keyed by (seed, p)   */
+    double gamma, lambda;                 /* GAE                                                                                   */
+    double clip_param, vf_clip_param, vf_loss_coeff, entropy_coeff;
+    double kl_coeff, kl_target;           /* the KL term's coefficient, and the target update_kl adapts it to                      */
+    double grad_clip;                     /* global-norm clip (clip_grad_norm_); <= 0: none                                        */
+    double lr, adam_beta1, adam_beta2, adam_eps;   /* torch.optim.Adam                                                             */
+    int32_t sgd_minibatch_size, num_sgd_iter;
+    int32_t standardize_advantages;       /* 1: (a - mean) / max(1e-4, std) over the train batch (RLlib standardize_fields)       */
+} ramp_ppo_config_t;
+
+/* a minibatch's statistics (stats_out of ramp_ppo_loss_grad; ramp_policy_learn: the mean over the last pass's minibatches) */
+enum { RAMP_PPO_TOTAL_LOSS = 0, RAMP_PPO_POLICY_LOSS, RAMP_PPO_VF_LOSS, RAMP_PPO_ENTROPY, RAMP_PPO_KL,
+       RAMP_PPO_CLIP_FRAC,                /* rows whose clipped surrogate was the smaller term, so the ratio passed no gradient   */
+       RAMP_PPO_GRAD_NORM,                /* global norm of the gradient before clipping                                          */
+       RAMP_PPO_KL_COEFF,                 /* loss_grad: the coefficient used; learn: the coefficient after update_kl              */
+       RAMP_PPO_ROWS,                     /* loss_grad: rows of the minibatch; learn: rows of the train batch                     */
+       RAMP_PPO_STATS_LEN };
+
+/* PPOTorchPolicy.loss (ray/rllib/algorithms/ppo/ppo_torch_policy.py of the ray 3.0.0.dev0 the reference pins) on one minibatch of
+ * HOST inputs, and its gradient, with no update:
+ *   ratio = exp(logp(a) - logp_old(a)),  logp_old from old_logits (the collection weights' logits, masked entries included)
+ *   loss  = mean(-min(adv ratio, adv clamp(ratio, 1 - clip, 1 + clip)) + vf_loss_coeff clamp((V - value_target)^2, 0, vf_clip)
+ *                - entropy_coeff H(pi)) + kl_coeff mean(KL(pi_old || pi))
+ * with torch.distributions.Categorical's entropy and KL: a masked action has probability 0 and adds exactly 0.  grad_out:
+ * [ramp_policy_weight_count] or NULL; stats_out: [RAMP_PPO_STATS_LEN] or NULL. */
+int ramp_ppo_loss_grad(ramp_policy_t* p, const ramp_ppo_config_t* cfg, int32_t n, const int32_t* model, const float* graph_features,
+                       const uint8_t* action_mask, const int32_t* action, const float* old_logits, const float* advantage,
+                       const float* value_target, float* grad_out, double* stats_out);
+/* One PPO learner step on the first n_steps slots of the trajectory of the last ramp_policy_trajectory_begin (RAMP_ERR_BAD_ARG
+ * unless that many slots were recorded since, both phases, in order), on the engine's stream, nothing read back but stats_out:
+ *   1. GAE per episode (RLlib compute_advantages): delta = r + gamma V' (1 - done) - V, adv = delta + gamma lambda (1 - done) adv';
+ *      value_target = adv + V.  A segment that ends before its episode does (truncate_episodes) bootstraps with V of the
+ *      state after its last step: the value recorded in slot n_steps when more slots were recorded, else the value of the
+ *      environment's current state.  The rows of episodes not finished when the decision was taken, t-major, form the train
+ *      batch; its advantages are standardised when cfg asks.
+ *   2. the collection weights' logits of every row, recomputed once (the same kernel and inputs as ramp_policy_act: its bits)
+ *   3. num_sgd_iter passes, each over the train batch shuffled, of minibatch updates: the loss above, its gradient, clip_grad_norm_
+ *      to grad_clip, torch.optim.Adam (moments and step count kept by the policy across calls)
+ *   4. stats_out [RAMP_PPO_STATS_LEN]: the means over the last pass's minibatches, and kl_coeff after RLlib's update_kl (x 1.5 above
+ *      2 kl_target, x 0.5 below kl_target / 2) -- the caller passes it as cfg->kl_coeff next time.
+ * The embeddings become stale (the next forward re-embeds).  num_sgd_iter 0 builds the train batch only. */
+int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_ppo_config_t* cfg, double* stats_out);
+/* HOST copies of the last ramp_policy_learn's train batch (any array may be NULL): n_out rows; per row the job type, the action,
+ * the collected log-probability, the one recomputed from the collection weights' logits (written by the first pass), the
+ * advantage (standardised when asked) and the value target */
+int ramp_policy_train_batch_read(ramp_policy_t* p, ramp_engine_t* eng, int32_t* n_out, int32_t* model_out, int32_t* action_out,
+                                 float* logp_out, float* logp_old_out, float* advantage_out, float* value_target_out);
+/* HOST copies of Adam's state (any may be NULL): exp_avg and exp_avg_sq [ramp_policy_weight_count], and the step count --
+ * torch.optim.Adam's state for the one flat parameter; zeros before the first update */
+int ramp_policy_learner_state(ramp_policy_t* p, float* exp_avg_out, float* exp_avg_sq_out, int32_t* step_out);
+/* zeroes Adam's moments and step count */
+int ramp_policy_learner_reset(ramp_policy_t* p);
+
 #ifdef __cplusplus
 }
 #endif
