@@ -361,17 +361,19 @@ bool build_resident_blob(const ramp_lowered_job_t* j, const ramp_quotient_t& q, 
     for (int32_t c = 0; c < N; ++c) {
         rec[c] = OpRec{q.op_cost[c] + 0.0, q.op_key[c], q.op_worker[c] | (q.op_weight[c] << 16)};
         thr[c] = q.op_threshold[c];
-        // the class's out-entries, flows first, each group in entry order: completing the class appends them to the ready-flow
-        // and ready-non-flow lists in the same order as a walk over the entries would
-        int32_t pos = q.row_ptr[c], n_fl = 0;
-        for (int pass = 0; pass < 2; ++pass)
-            for (int32_t k = q.row_ptr[c]; k < q.row_ptr[c + 1]; ++k) {
-                if ((q.dep_is_flow[k] != 0) != (pass == 0)) continue;
-                const uint32_t lo = dense_key[k] | (uint32_t)(q.dep_group_mask[k] << h.cshift);
-                const uint32_t hi = (q.dep_is_flow[k] ? 1u : 0u) | (q.dep_inc[k] << h.ishift) | ((uint32_t)q.dep_dst[k] << h.dshift);
-                out[pos++] = OutRec{q.dep_run_time[k] + 0.0, lo, hi};
-                n_fl += pass == 0;
-            }
+        // the class's out-entries, flows first, in descending key order (the order the kernel keeps its ready-flow frontier
+        // in: completing the class merges them into it), then the non-flows in entry order
+        std::vector<int32_t> ent;
+        for (int32_t k = q.row_ptr[c]; k < q.row_ptr[c + 1]; ++k) if (q.dep_is_flow[k] != 0) ent.push_back(k);
+        std::stable_sort(ent.begin(), ent.end(), [&](int32_t a, int32_t b) { return dense_key[a] > dense_key[b]; });
+        const int32_t n_fl = (int32_t)ent.size();
+        for (int32_t k = q.row_ptr[c]; k < q.row_ptr[c + 1]; ++k) if (q.dep_is_flow[k] == 0) ent.push_back(k);
+        int32_t pos = q.row_ptr[c];
+        for (const int32_t k : ent) {
+            const uint32_t lo = dense_key[k] | (uint32_t)(q.dep_group_mask[k] << h.cshift);
+            const uint32_t hi = (q.dep_is_flow[k] ? 1u : 0u) | (q.dep_inc[k] << h.ishift) | ((uint32_t)q.dep_dst[k] << h.dshift);
+            out[pos++] = OutRec{q.dep_run_time[k] + 0.0, lo, hi};
+        }
         const int32_t n_nf = q.row_ptr[c + 1] - q.row_ptr[c] - n_fl;
         if (n_fl > 0xFFFF || n_nf > 0x7FFF) return false;
         row[2 * c] = q.row_ptr[c]; row[2 * c + 1] = n_fl | (n_nf << 16);

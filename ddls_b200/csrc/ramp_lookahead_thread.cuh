@@ -338,12 +338,28 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
     for (int i = 0; i < N && i < x.n_cap; ++i) cnt[i * 32] = 0;
     int nO = H.n_src, nF = 0, nNF = 0;
     // JOB:496-506: a completed class's out-entries become ready.  The blob stores them as ready-made frontier entries, flows
-    // first (ramp_engine.cu, build_resident_blob): straight copies, no per-entry flow test or second load
+    // first, in descending key order (ramp_engine.cu, build_resident_blob).  The ready-flow frontier is kept in descending key
+    // order too (entries of equal key adjacent), which is what the small-frontier half's one-pass channel winners need: the
+    // class's flows are merged into it from the back -- a straight copy when the frontier is empty, the usual case -- and
+    // every survivor compaction keeps the order.  Nothing else depends on the order of a frontier.
     auto complete_op = [&](const int op) {
         const int2 row = op_row[op];
         const int e_nf = row.x + (row.y & 0xffff), e_end = e_nf + (row.y >> 16);
-        _Pragma("unroll 1")
-        for (int e = row.x; e < e_nf; ++e) { flows.put(nF, out_rec[e]); ++nF; }
+        if (nF == 0) {
+            _Pragma("unroll 1")
+            for (int e = row.x; e < e_nf; ++e) { flows.put(nF, out_rec[e]); ++nF; }
+        } else {
+            int i = nF - 1, k = nF + (e_nf - row.x) - 1;
+            nF = k + 1;
+            _Pragma("unroll 1")
+            for (int e = e_nf - 1; e >= row.x; --e, --k) {
+                const int4 r = out_rec[e];
+                const uint32_t key = (uint32_t)r.z & kmask;
+                _Pragma("unroll 1")
+                for (int4 f; i >= 0 && ((uint32_t)(f = flows.get(i)).z & kmask) < key; --i, --k) flows.put(k, f);
+                flows.put(k, r);
+            }
+        }
         _Pragma("unroll 1")
         for (int e = e_nf; e < e_end; ++e) { nfs.put(nNF, (uint32_t)out_rec[e].w); ++nNF; }
     };
@@ -406,36 +422,50 @@ __device__ __forceinline__ void thread_lookahead(const LaneCtx& x) {
                 if (ow0) { const u64_t r0 = rem_bits(orr[0]); t_op = (r0 < t_op) ? r0 : t_op; n_active += (int)((uint32_t)orr[0].w >> 16); }
             }
             RAMP_TC(tc.stamp(1);)
-            // ---- C, D, E, I, J, H: dispatched ONCE on the number of ready flow entries; each case is straight-line code ----
+            // ---- C, D, E, I, J, H: dispatched ONCE on the number of ready flow entries; each case is straight-line code
+            // without a branch but the completions: D and H are one pass each over the key-ordered frontier ----
             auto flow_tick = [&](auto nf_tag) {
                 constexpr int NF = decltype(nf_tag)::value;
-                uint32_t gm[NF], key[NF];
 #pragma unroll
                 for (int k = 0; k < NF; ++k) fr[k] = x.f_sm[k * 32 + lane];
-#pragma unroll
-                for (int k = 0; k < NF; ++k) { gm[k] = (uint32_t)fr[k].z >> csh; key[k] = (uint32_t)fr[k].z & kmask; }
+                // D: the entry wins on a channel group of its set unless a ready entry with a larger key lies on that group
+                // too (an empty set -- no channel -- never wins, it only ticks).  In key order the larger keys are the entries
+                // before the entry's run of equal keys, so one pass with the groups they claim gives the pairwise rule.
                 u64_t t_comm = RAMP_INF_BITS;
+                uint32_t seen = 0u, claimed = 0u;       // groups of the entries so far / of those with a larger key
 #pragma unroll
                 for (int k = 0; k < NF; ++k) {
-                    // the entry wins on a channel group of its set unless a ready entry with a larger key lies on that group too
-                    // (an empty set -- no channel -- never wins, it only ticks)
-                    uint32_t open_groups = gm[k];
-#pragma unroll
-                    for (int j = 0; j < NF; ++j) if (j != k && key[j] > key[k]) open_groups &= ~gm[j];
-                    if (open_groups) { const u64_t rem = rem_bits(fr[k]); t_comm = (rem < t_comm) ? rem : t_comm; }
+                    const uint32_t gm = (uint32_t)fr[k].z >> csh;
+                    if (k > 0) claimed = (((uint32_t)fr[k].z & kmask) != ((uint32_t)fr[k - 1].z & kmask)) ? seen : claimed;
+                    const u64_t rem = rem_bits(fr[k]);
+                    t_comm = ((gm & ~claimed) != 0u && rem < t_comm) ? rem : t_comm;
+                    seen |= gm;
                 }
                 take_tick(t_comm, true);
-                int pf = 0;
+                // H: every entry ticks (JOB:561-562); survivors are compacted to the front in order, completed entries go to
+                // the back of the old slots, both by ONE store whose slot is selected
+                int pf = 0, nd = 0;             // survivors; completed entries: the first one's dep word hi in hd0, the
+                uint32_t hd0 = 0u;              // others at slots NF - 2, NF - 3, ...
 #pragma unroll
                 for (int k = 0; k < NF; ++k) {
                     const u64_t rb = rem_bits(fr[k]);
-                    if (rb <= tick_b) { complete_dep((uint32_t)fr[k].w); --to_complete; }        // JOB:561-562
-                    else {
-                        const double r2 = __dsub_rn(__longlong_as_double((long long)rb), tick);
-                        fr[k].x = __double2loint(r2); fr[k].y = __double2hiint(r2); x.f_sm[pf * 32 + lane] = fr[k]; ++pf;
-                    }
+                    const bool done = rb <= tick_b;
+                    const double r2 = __dsub_rn(__longlong_as_double((long long)rb), tick);
+                    int4 f = fr[k];
+                    f.x = __double2loint(r2); f.y = __double2hiint(r2);
+                    hd0 = (done && nd == 0) ? (uint32_t)f.w : hd0;
+                    x.f_sm[(done ? NF - 1 - nd : pf) * 32 + lane] = f;
+                    pf += done ? 0 : 1;
+                    nd += done ? 1 : 0;
                 }
                 nF = pf;
+                // the completed entries' children, in slot order
+                if (nd != 0) {
+                    complete_dep(hd0);
+                    _Pragma("unroll 1")
+                    for (int d = 1; d < nd; ++d) complete_dep((uint32_t)x.f_sm[(NF - 1 - d) * 32 + lane].w);
+                    to_complete -= nd;
+                }
             };
             // by frequency on the quotient of a partitioned job: one ready flow entry, a non-flow tick, none, two, ...
             if (any_nf) {                                           // zero-length tick that completes the ready non-flow deps

@@ -125,7 +125,9 @@ def static_side(lib, tmp):
     body = re.split(r'\n\t\.section\s', dis.split(f'\n{KERNEL}:\n', 1)[1], maxsplit=1)[0]
     ann = re.compile(r'//## File "([^"]+)", line (\d+)(?: inlined at "([^"]+)", line (\d+))?')
     ins = re.compile(r'^\s+/\*[0-9a-f]{4,}\*/\s+\S')
+    bra = re.compile(r'^\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\w+\s+)?(BRA|BSSY)\b')
     n_all = n_inst = n_loop = n_fast = 0
+    n_bra = {'BRA': 0, 'BSSY': 0}
     # nvdisasm prints an instruction's inline chain (innermost frame first, the kernel's own line last) when it changes
     cur, fresh = [], True
     for l in body.splitlines():
@@ -145,9 +147,13 @@ def static_side(lib, tmp):
             inner = cur[-2][0]
             if loop0 <= inner < loop1:
                 n_loop += 1
+                b = bra.match(l)
+                if b:
+                    n_bra[b.group(1)] += 1
             if fast0 <= inner < fast1:
                 n_fast += 1
-    return dict(kernel=n_all, instantiation=n_inst, tick_loop=n_loop, small_frontier_path=n_fast)
+    return dict(kernel=n_all, instantiation=n_inst, tick_loop=n_loop, small_frontier_path=n_fast,
+                tick_loop_bra=n_bra['BRA'], tick_loop_bssy=n_bra['BSSY'])
 
 
 def gpu_line():
@@ -164,6 +170,7 @@ def main():
     ap.add_argument('--n', type=int, default=4096)
     ap.add_argument('--run-times', default='reference', choices=['reference', 'one_to_one'])
     ap.add_argument('--out-lib', default=os.path.join(ROOT, 'build_variants', 'tick_clocks', 'libramp_b200.so'))
+    ap.add_argument('--static-only', action='store_true', help='print the SASS counts of the normal build and stop (no GPU)')
     ap.add_argument('--measure', default=None, help=argparse.SUPPRESS)
     ap.add_argument('--ledger', action='store_true', help=argparse.SUPPRESS)
     args = ap.parse_args()
@@ -172,14 +179,16 @@ def main():
     from ddls_b200 import build
     normal_lib = build.LIB_PATH
     assert os.path.exists(normal_lib), 'build the library first (python -m ddls_b200.build)'
-    variant = build.build(extra_flags=['-DRAMP_TICK_CLOCKS'], out=args.out_lib)
     import tempfile
     with tempfile.TemporaryDirectory() as tmp:
         st = static_side(normal_lib, tmp)
-    print(f'GPU: {gpu_line()}')
     print(f'thread_lookahead<false> in the normal build: {st["instantiation"]} instructions ({st["instantiation"] * 16} B), '
-          f'tick loop {st["tick_loop"]}, small-frontier half {st["small_frontier_path"]}; whole kernel {st["kernel"]} '
-          f'({st["kernel"] * 16} B)')
+          f'tick loop {st["tick_loop"]} ({st["tick_loop_bra"]} BRA, {st["tick_loop_bssy"]} BSSY), small-frontier half '
+          f'{st["small_frontier_path"]}; whole kernel {st["kernel"]} ({st["kernel"] * 16} B)')
+    if args.static_only:
+        return
+    variant = build.build(extra_flags=['-DRAMP_TICK_CLOCKS'], out=args.out_lib)
+    print(f'GPU: {gpu_line()}')
     normal = sub(normal_lib, args, False)
     inst = sub(variant, args, True)
     for r, n in zip(inst, normal):
