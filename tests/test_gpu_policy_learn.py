@@ -12,11 +12,12 @@ import dataclasses
 import numpy as np
 import pytest
 
+from ppo_reference import shuffle_order
+
 pytestmark = pytest.mark.gpu
 
 REL = 1e-4
 FP32_FACTOR = 10
-M64 = (1 << 64) - 1
 
 
 def _kernels():
@@ -182,34 +183,6 @@ def _policy(graphs, seed=4):
     return P.DeviceGNNPolicy(graphs, 17, None, P.random_state_dict(P.DEFAULT_CONFIG, 17, seed=seed))
 
 
-def mix64(x):
-    x = (x + 0x9E3779B97F4A7C15) & M64
-    x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & M64
-    x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & M64
-    return x ^ (x >> 31)
-
-
-def shuffle_order(seed, sgd_pass, n):
-    """shuffle_pos of ramp_policy_learn.cuh for pass `sgd_pass` of a learn call with `seed`: batch row of each position"""
-    key = mix64(seed ^ mix64(sgd_pass + 1))
-    if n <= 1:
-        return np.arange(n)
-    h = ((n - 1).bit_length() + 1) // 2
-    mask = (1 << h) - 1
-    out = []
-    for i in range(n):
-        x = i
-        while True:
-            L, R = x >> h, x & mask
-            for r in range(4):
-                L, R = R, L ^ (mix64(key ^ (r << 40) ^ R) & mask)
-            x = (L << h) | R
-            if x < n:
-                break
-        out.append(x)
-    return np.array(out)
-
-
 def host_batch(pol, traj, tb):
     """the train batch's rows (t-major) as host arrays, with the collection weights' logits"""
     live = traj['live'] & (traj['model'] < pol.n_models)
@@ -248,15 +221,16 @@ def test_first_pass_recomputes_the_collected_log_probabilities_bit_for_bit():
         pol.close(); env.close()
 
 
-@pytest.mark.parametrize('kind', ['full', 'truncated', 'prefix', 'past_the_end'])
+@pytest.mark.parametrize('kind', ['full', 'truncated', 'prefix', 'past_the_end', 'wide'])
 def test_gae_matches_numpy_float64(kind):
     """full episodes; a segment that ends before its episodes do (bootstrapped with the value of the environment's current state);
-    the first half of a recorded segment (bootstrapped with the value recorded at the next step); episodes that end early"""
+    the first half of a recorded segment (bootstrapped with the value recorded at the next step); episodes that end early; full
+    episodes of 1,300 episodes, which the one-CTA kernel compacts and standardises in chunks of 1,024"""
     from ppo_reference import gae64, standardize64
     from ddls_b200.learn import DevicePPOLearner, PPOConfig
     J = 8
-    H = {'full': J, 'truncated': J // 2, 'prefix': J, 'past_the_end': J + 3}[kind]
-    env, graphs = _env(J=J, seed=9)
+    H = {'full': J, 'truncated': J // 2, 'prefix': J, 'past_the_end': J + 3, 'wide': J}[kind]
+    env, graphs = _env(B=1300 if kind == 'wide' else 256, J=J, seed=9)
     pol = _policy(graphs)
     try:
         traj = pol.collect(env, H, sample=True, seed=7)
