@@ -50,6 +50,11 @@ LookaheadKernel lookahead_cta_kernel_for(int nt) {   // one CTA of nt threads pe
     }
 }
 
+// the step kernel with 32 episodes per CTA, or 1 when 32 copies of the running-job table do not fit shared memory
+using StepKernel = void (*)(const StepArgs);
+constexpr size_t STEP_SMEM_MAX = 200 * 1024;
+StepKernel step_kernel_for(int nt) { return nt == 32 ? ramp_step_kernel<32> : ramp_step_kernel<1>; }
+
 struct HostTemplate {
     TemplateDev dev;             // copy of what sits in the device array
     DeviceArray<unsigned char> blob;   // single device allocation holding all arrays
@@ -101,7 +106,7 @@ struct ramp_engine {
     // per-step
     DeviceArray<WorkItem> d_items;
     DeviceArray<Counters> d_counters;
-    DeviceArray<MemoStats> d_stats;
+    DeviceArray<MemoStats> d_stats;      // [0] the cumulative counters the kernels add to, [1] their copy at the last ramp_reset
     DeviceArray<ramp_action_t> d_actions;
     DeviceArray<double> d_step_stats;
     DeviceArray<int32_t> d_n_cluster_steps;
@@ -112,6 +117,13 @@ struct ramp_engine {
     DeviceArray<double> ep_ef, ep_es, ep_rf, tick_util; DeviceArray<int32_t> ep_ei, ep_ri, tick_util_n; DeviceArray<ramp_job_record_t> ep_rec;
     DeviceArray<ramp_arrival_t> d_arrivals;
     DeviceArray<int32_t> d_n_jobs_ep;
+    // ramp_reset copies the caller's arrivals here and uploads them from here, so it returns without waiting for the upload;
+    // ev_stage marks the end of the last upload, which the next reset waits for before it writes the buffer again
+    PinnedArray<ramp_arrival_t> h_arr_stage;
+    Event ev_stage;
+    // ramp_step_kernel: threads per CTA (one per episode) and its dynamic shared memory (the episodes' state on chip)
+    int step_nt = 0;
+    size_t step_smem = 0;
     // lookahead scratch
     DeviceArray<unsigned char> d_scratch;
     uint64_t scratch_stride = 0;
@@ -131,6 +143,7 @@ struct ramp_engine {
     int debug = 0;               // RAMP_DEBUG=1 prints the launch decisions to stderr
     int mode = 0;                // 0 auto, 1 warp-per-lookahead, 2 CTA-per-lookahead (RAMP_LOOKAHEAD_MODE); 1 and 2 make nothing resident
     PinnedArray<int32_t> h_n_work;   // [4]
+    PinnedArray<MemoStats> h_stats;  // [2] read-back of d_stats
     DeviceArray<WorkItem> d_items_big;
     Stream stream2;              // big lookaheads run concurrently with the small ones
     Event ev_fork, ev_join;
@@ -175,7 +188,6 @@ struct ramp_engine {
     double la_ms_total = 0.0;
     int64_t la_launches = 0;
     unsigned long long la_items_base = 0, la_bytes_base = 0, la_qbytes_base = 0;
-    MemoStats memo_base{};       // device counters at the last ramp_reset (memo statistics are reported since the reset)
 };
 
 // A kernel's dynamic shared memory limit (cudaFuncAttributeMaxDynamicSharedMemorySize) belongs to the kernel in the device's
@@ -643,13 +655,15 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     CUDA_TRY(create(e->stream2, cudaStreamNonBlocking));
     CUDA_TRY(create(e->ev_fork, cudaEventDisableTiming));
     CUDA_TRY(create(e->ev_join, cudaEventDisableTiming));
-    CUDA_TRY(alloc_each(1, e->d_counters, e->d_stats));
+    CUDA_TRY(e->d_counters.alloc(1));
+    CUDA_TRY(e->d_stats.alloc(2));
     CUDA_TRY(cudaMemset(e->d_counters.get(), 0, sizeof(Counters)));
-    CUDA_TRY(cudaMemset(e->d_stats.get(), 0, sizeof(MemoStats)));
+    CUDA_TRY(cudaMemset(e->d_stats.get(), 0, 2 * sizeof(MemoStats)));
     CUDA_TRY(e->d_step_stats.alloc((size_t)RAMP_STEP_STATS_LEN * B));
     CUDA_TRY(e->d_ep_export.alloc((size_t)RAMP_EP_LEN * B));
     CUDA_TRY(e->d_es_export.alloc((size_t)RAMP_ES_LEN * B));
     CUDA_TRY(e->h_n_work.alloc(4));
+    CUDA_TRY(e->h_stats.alloc(2));
 
     EpisodeState& ep = e->ep;
     ep.B = B; ep.max_running = cfg.max_running; ep.max_jobs = cfg.max_jobs; ep.n_jobs = 0;
@@ -661,6 +675,8 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     CUDA_TRY(e->ep_ri.alloc((size_t)RI_COUNT * cfg.max_running * B));
     CUDA_TRY(e->ep_rec.alloc((size_t)cfg.max_jobs * B));
     CUDA_TRY(e->d_arrivals.alloc((size_t)cfg.max_jobs * B));
+    CUDA_TRY(e->h_arr_stage.alloc((size_t)cfg.max_jobs * B));
+    CUDA_TRY(create(e->ev_stage, cudaEventDisableTiming));
     ep.ef = e->ep_ef.get(); ep.ei = e->ep_ei.get(); ep.rf = e->ep_rf.get(); ep.ri = e->ep_ri.get(); ep.rec = e->ep_rec.get();
     CUDA_TRY(cudaMemset(ep.ef, 0, sizeof(double) * EF_COUNT * B));
     CUDA_TRY(cudaMemset(ep.ei, 0, sizeof(int32_t) * EI_COUNT * B));
@@ -669,6 +685,16 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     CUDA_TRY(e->d_n_jobs_ep.alloc(B));
     CUDA_TRY(cudaMemset(e->d_n_jobs_ep.get(), 0, sizeof(int32_t) * B));
     ep.n_jobs_ep = e->d_n_jobs_ep.get();
+    // 32 episodes per CTA puts 4,096 episodes on 128 SMs; a table too large for 32 copies in shared memory takes one per CTA
+    {
+        const int rows = step_rows(cfg.max_running, cfg.max_jobs);
+        e->step_nt = step_smem_bytes(32, rows) <= STEP_SMEM_MAX ? 32 : 1;
+        e->step_smem = step_smem_bytes(e->step_nt, rows);
+        if (e->step_smem > STEP_SMEM_MAX)
+            return set_error(RAMP_ERR_CAPACITY, "the running-job table of %d rows needs %zu B of shared memory (max %zu)", rows, e->step_smem,
+                             (size_t)STEP_SMEM_MAX);
+        CUDA_TRY(reserve_dynamic_smem((const void*)step_kernel_for(e->step_nt), e->step_smem));
+    }
 
     for (int k = 0; k < MAX_EVENT_PAIRS; ++k) {
         CUDA_TRY(create(e->ev_a[k], cudaEventDefault));
@@ -840,30 +866,31 @@ int ramp_reset(ramp_engine_t* e, const ramp_arrival_t* arrivals, int32_t n_jobs)
     if (n_jobs < 1 || n_jobs > e->cfg.max_jobs) return set_error(RAMP_ERR_BAD_ARG, "n_jobs %d not in [1, max_jobs=%d]", n_jobs, e->cfg.max_jobs);
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     const int B = e->cfg.n_episodes;
+    cudaStream_t st = e->stream.get();
+    // the caller may overwrite `arrivals` as soon as this returns, so they are copied into the pinned staging buffer (once the
+    // previous reset's upload from it has finished) and uploaded from there in stream order; nothing here waits for the device
+    CUDA_TRY(cudaEventSynchronize(e->ev_stage.get()));
+    const size_t row = sizeof(ramp_arrival_t) * (size_t)n_jobs;
+    memcpy(e->h_arr_stage.get(), arrivals, row * B);
     if (n_jobs == e->cfg.max_jobs) {
-        CUDA_TRY(cudaMemcpyAsync(e->d_arrivals.get(), arrivals, sizeof(ramp_arrival_t) * (size_t)n_jobs * B, cudaMemcpyHostToDevice, e->stream.get()));
+        CUDA_TRY(cudaMemcpyAsync(e->d_arrivals.get(), e->h_arr_stage.get(), row * B, cudaMemcpyHostToDevice, st));
     } else {
-        CUDA_TRY(cudaMemcpy2DAsync(e->d_arrivals.get(), sizeof(ramp_arrival_t) * (size_t)e->cfg.max_jobs, arrivals,
-                                   sizeof(ramp_arrival_t) * (size_t)n_jobs, sizeof(ramp_arrival_t) * (size_t)n_jobs, B,
-                                   cudaMemcpyHostToDevice, e->stream.get()));
+        CUDA_TRY(cudaMemcpy2DAsync(e->d_arrivals.get(), sizeof(ramp_arrival_t) * (size_t)e->cfg.max_jobs, e->h_arr_stage.get(), row, row, B,
+                                   cudaMemcpyHostToDevice, st));
     }
+    CUDA_TRY(cudaEventRecord(e->ev_stage.get(), st));
     e->ep.n_jobs = n_jobs;
-    {
-        std::vector<int32_t> nj(B, n_jobs);
-        CUDA_TRY(cudaMemcpyAsync(e->d_n_jobs_ep.get(), nj.data(), sizeof(int32_t) * B, cudaMemcpyHostToDevice, e->stream.get()));
-        CUDA_TRY(cudaStreamSynchronize(e->stream.get()));     // nj goes out of scope
-    }
     // memo is per env instance per episode: cleared on reset (RCE:269-275)
-    CUDA_TRY(cudaMemsetAsync(e->d_memo_keys.get(), 0, sizeof(unsigned long long) * e->memo_cap, e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(e->d_memo_keys.get(), 0, sizeof(unsigned long long) * e->memo_cap, st));
     // the batch-wide cache of RAMP_MEMO_SHARED (level-2 keys, its result slots and traces) is a pure function of the
     // lowered job and survives the reset; every other mode starts from an empty trace pool
-    if (e->cfg.memo_mode != RAMP_MEMO_SHARED) CUDA_TRY(cudaMemsetAsync(e->pool.top.get(), 0, sizeof(unsigned long long), e->stream.get()));
-    CUDA_TRY(cudaMemcpyAsync(&e->memo_base, e->d_stats.get(), sizeof(MemoStats), cudaMemcpyDeviceToHost, e->stream.get()));   // counters stay cumulative
-    CUDA_TRY(cudaMemsetAsync(e->d_counters.get(), 0, sizeof(Counters), e->stream.get()));
-    ramp_reset_kernel<<<(B + 127) / 128, 128, 0, e->stream.get()>>>(e->ep);
+    if (e->cfg.memo_mode != RAMP_MEMO_SHARED) CUDA_TRY(cudaMemsetAsync(e->pool.top.get(), 0, sizeof(unsigned long long), st));
+    // the counters stay cumulative; memo statistics are reported since this copy of them
+    CUDA_TRY(cudaMemcpyAsync(e->d_stats.get() + 1, e->d_stats.get(), sizeof(MemoStats), cudaMemcpyDeviceToDevice, st));
+    CUDA_TRY(cudaMemsetAsync(e->d_counters.get(), 0, sizeof(Counters), st));
+    ramp_reset_kernel<<<(B + 127) / 128, 128, 0, st>>>(e->ep, e->d_n_jobs_ep.get(), n_jobs);
     e->launches++;
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     return RAMP_OK;
 }
 
@@ -937,7 +964,7 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
     StepArgs s{};
     s.actions = d_actions; s.ep = e->ep; s.res = e->res.view(); s.pool = e->pool.view(); s.counters = e->d_counters.get();
     s.stats_out = d_stats_out; s.n_cluster_steps_out = d_ncs_out; s.fuse_empty_steps = fuse;
-    ramp_step_kernel<<<(B + 63) / 64, 64, 0, st>>>(s);
+    step_kernel_for(e->step_nt)<<<(B + e->step_nt - 1) / e->step_nt, e->step_nt, e->step_smem, st>>>(s);
     e->launches++;
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
@@ -1021,24 +1048,25 @@ int ramp_get_episode_state(ramp_engine_t* e, double* out) {
 
 int ramp_get_memo_stats(ramp_engine_t* e, int64_t* lookups, int64_t* hits, int64_t* lookaheads) {
     if (!e) return set_error(RAMP_ERR_BAD_ARG, "null engine");
+    // the counters and their copy at the last reset, in stream order: one synchronisation
+    CUDA_TRY(cudaMemcpyAsync(e->h_stats.get(), e->d_stats.get(), 2 * sizeof(MemoStats), cudaMemcpyDeviceToHost, e->stream.get()));
     CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
-    MemoStats s{};
-    CUDA_TRY(cudaMemcpy(&s, e->d_stats.get(), sizeof(MemoStats), cudaMemcpyDeviceToHost));
-    if (lookups) *lookups = (int64_t)(s.lookups - e->memo_base.lookups);
-    if (hits) *hits = (int64_t)(s.hits - e->memo_base.hits);
-    if (lookaheads) *lookaheads = (int64_t)(s.lookaheads - e->memo_base.lookaheads);
+    const MemoStats* s = e->h_stats.get();
+    if (lookups) *lookups = (int64_t)(s[0].lookups - s[1].lookups);
+    if (hits) *hits = (int64_t)(s[0].hits - s[1].hits);
+    if (lookaheads) *lookaheads = (int64_t)(s[0].lookaheads - s[1].lookaheads);
     return RAMP_OK;
 }
 
 int ramp_get_memo_stats_ex(ramp_engine_t* e, int64_t out[4]) {
     if (!e || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    CUDA_TRY(cudaMemcpyAsync(e->h_stats.get(), e->d_stats.get(), 2 * sizeof(MemoStats), cudaMemcpyDeviceToHost, e->stream.get()));
     CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
-    MemoStats s{};
-    CUDA_TRY(cudaMemcpy(&s, e->d_stats.get(), sizeof(MemoStats), cudaMemcpyDeviceToHost));
-    out[0] = (int64_t)(s.lookups - e->memo_base.lookups);
-    out[1] = (int64_t)(s.hits - e->memo_base.hits);
-    out[2] = (int64_t)(s.shared_hits - e->memo_base.shared_hits);
-    out[3] = (int64_t)(s.lookaheads - e->memo_base.lookaheads);
+    const MemoStats* s = e->h_stats.get();
+    out[0] = (int64_t)(s[0].lookups - s[1].lookups);
+    out[1] = (int64_t)(s[0].hits - s[1].hits);
+    out[2] = (int64_t)(s[0].shared_hits - s[1].shared_hits);
+    out[3] = (int64_t)(s[0].lookaheads - s[1].lookaheads);
     return RAMP_OK;
 }
 

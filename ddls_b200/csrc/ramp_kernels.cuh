@@ -100,7 +100,9 @@ struct Counters {               // the first four words are zeroed at the start 
 struct MemoStats { unsigned long long lookups, hits, lookaheads, alg_bytes, shared_hits, quotient_bytes; };
 
 // running-job table fields (SoA: [field][row][episode])
-enum { RF_JCT = 0, RF_STARTED, RF_COMM, RF_COMP, RF_UTIL, RF_PART_OP_MEM, RF_PART_DEP, RF_FLOW, RF_ORIG_OP_MEM,
+// RF_COMM_FRAC / RF_COMP_FRAC: the job's comm / jct and comp / jct (RCE:962-982), divided once when it is mounted rather than
+// in every tick of the outer event loop -- the same division of the same operands
+enum { RF_JCT = 0, RF_STARTED, RF_COMM_FRAC, RF_COMP_FRAC, RF_UTIL, RF_PART_OP_MEM, RF_PART_DEP, RF_FLOW, RF_ORIG_OP_MEM,
        RF_ORIG_DEP, RF_COUNT };
 enum { RI_JOB_IDX = 0, RI_N_WORKERS, RI_N_CHANNELS, RI_COUNT };
 
@@ -853,64 +855,125 @@ struct StepArgs {
 
 #define EF(f) ef[(f) * B + b]
 #define EI(f) ei[(f) * B + b]
-#define RF(f, row) rf[((f) * R + (row)) * B + b]
-#define RI(f, row) ri[((f) * R + (row)) * B + b]
 
-__device__ inline void step_register_blocked(const EpisodeState& ep, int b, int job_idx, double* st) {   // RCE:1504-1540
-    const int B = ep.B;
-    int32_t* ei = ep.ei;
+// One episode's scalars and running-job table, wherever they live: field f of the scalars at ef[f * ld], row `row` of the table
+// at rf[(f * rows + row) * ld].  The HBM arrays of EpisodeState are the view {ep.ef + b, ..., ld = B, rows = max_running}; the step
+// kernel runs on a copy in shared memory, {.. + threadIdx.x, ld = CTA threads, rows = step_rows}
+struct EpView {
+    double* ef; int32_t* ei; double* rf; int32_t* ri;
+    int ld, rows;
+};
+#define VF(f) v.ef[(f) * v.ld]
+#define VI(f) v.ei[(f) * v.ld]
+#define VRF(f, row) v.rf[((f) * v.rows + (row)) * v.ld]
+#define VRI(f, row) v.ri[((f) * v.rows + (row)) * v.ld]
+
+__device__ __forceinline__ EpView hbm_view(const EpisodeState& ep, int b) {
+    EpView v;
+    v.ef = ep.ef + b; v.ei = ep.ei + b; v.rf = ep.rf + b; v.ri = ep.ri + b; v.ld = ep.B; v.rows = ep.max_running;
+    return v;
+}
+
+// rows of the running-job table the step kernel keeps on chip: at most max_jobs jobs of an episode ever run
+__host__ __device__ inline int step_rows(int max_running, int max_jobs) { return max_running < max_jobs ? max_running : max_jobs; }
+// shared memory of a step-kernel CTA of nt threads (one per episode)
+__host__ __device__ inline size_t step_smem_bytes(int nt, int rows) {
+    return (size_t)nt * ((size_t)(EF_COUNT + RF_COUNT * rows) * 8 + (size_t)(EI_COUNT + RI_COUNT * rows) * 4);
+}
+
+__device__ __forceinline__ void step_register_blocked(const EpisodeState& ep, const EpView& v, int b, int job_idx, double* st) {   // RCE:1504-1540
     ramp_job_record_t& r = ep.rec[(size_t)b * ep.max_jobs + job_idx];
-    if (EI(EI_QUEUED) == job_idx) EI(EI_QUEUED) = -1;
+    if (VI(EI_QUEUED) == job_idx) VI(EI_QUEUED) = -1;
     if (r.status == RAMP_JS_BLOCKED) return;
     r.status = RAMP_JS_BLOCKED;
-    r.event_seq = EI(EI_EVENT_SEQ)++;
-    EI(EI_NUM_BLOCKED)++;
+    r.event_seq = VI(EI_EVENT_SEQ)++;
+    VI(EI_NUM_BLOCKED)++;
     st[RAMP_SS_NUM_JOBS_BLOCKED] += 1.0;
 }
 
-__device__ inline void step_remove_running(const EpisodeState& ep, int b, int pos) {   // keeps dict (insertion) order
-    const int B = ep.B, R = ep.max_running;
-    double* rf = ep.rf; int32_t* ri = ep.ri; int32_t* ei = ep.ei;
-    const int n = EI(EI_N_RUNNING);
+__device__ __forceinline__ void step_remove_running(const EpView& v, int pos) {   // keeps dict (insertion) order
+    const int n = VI(EI_N_RUNNING);
     for (int k = pos; k + 1 < n; ++k) {
-        for (int f = 0; f < RF_COUNT; ++f) RF(f, k) = RF(f, k + 1);
-        for (int f = 0; f < RI_COUNT; ++f) RI(f, k) = RI(f, k + 1);
+        for (int f = 0; f < RF_COUNT; ++f) VRF(f, k) = VRF(f, k + 1);
+        for (int f = 0; f < RI_COUNT; ++f) VRI(f, k) = VRI(f, k + 1);
     }
-    EI(EI_N_RUNNING) = n - 1;
+    VI(EI_N_RUNNING) = n - 1;
 }
 
-__device__ inline bool step_is_done(const EpisodeState& ep, int b) {   // RCE:1542-1557
-    const int B = ep.B;
-    const double* ef = ep.ef; const int32_t* ei = ep.ei;
-    if (EF(EF_NOW) >= ep.max_sim_time) return true;
-    return (ep.n_jobs_ep[b] - EI(EI_NUM_ARRIVED)) <= 0 && EI(EI_N_RUNNING) == 0 && EI(EI_QUEUED) < 0;
+// n_jobs: ep.n_jobs_ep[b]
+__device__ __forceinline__ bool step_is_done(const EpisodeState& ep, const EpView& v, int n_jobs) {   // RCE:1542-1557
+    if (VF(EF_NOW) >= ep.max_sim_time) return true;
+    return (n_jobs - VI(EI_NUM_ARRIVED)) <= 0 && VI(EI_N_RUNNING) == 0 && VI(EI_QUEUED) < 0;
 }
 
-__device__ inline void step_get_next_job(const EpisodeState& ep, int b) {   // RCE:351-377
-    const int B = ep.B;
-    double* ef = ep.ef; int32_t* ei = ep.ei;
-    const int k = EI(EI_NUM_ARRIVED);
+__device__ __forceinline__ void step_get_next_job(const EpisodeState& ep, const EpView& v, int b) {   // RCE:351-377
+    const int k = VI(EI_NUM_ARRIVED);
     ramp_job_record_t& r = ep.rec[(size_t)b * ep.max_jobs + k];
     r.status = RAMP_JS_QUEUED; r.event_seq = 0;
-    r.time_arrived = EF(EF_NOW); r.time_started = 0.0; r.time_completed = 0.0;
+    r.time_arrived = VF(EF_NOW); r.time_started = 0.0; r.time_completed = 0.0;
     r.jct = r.comm = r.comp = r.util = 0.0;
     const ramp_arrival_t a = ep.arr[(size_t)b * ep.max_jobs + k];
-    EF(EF_LAST_ARRIVAL) = EF(EF_NOW);                                        // RCE:362
-    EF(EF_NEXT_ARRIVAL) = __dadd_rn(EF(EF_NEXT_ARRIVAL), a.interarrival);    // RCE:363
-    EF(EF_LOAD_SUM) = __dadd_rn(EF(EF_LOAD_SUM),
+    VF(EF_LAST_ARRIVAL) = VF(EF_NOW);                                        // RCE:362
+    VF(EF_NEXT_ARRIVAL) = __dadd_rn(VF(EF_NEXT_ARRIVAL), a.interarrival);    // RCE:363
+    VF(EF_LOAD_SUM) = __dadd_rn(VF(EF_LOAD_SUM),
                                 __ddiv_rn(__dadd_rn(a.orig_op_mem, a.orig_dep_size),
-                                          __dsub_rn(EF(EF_NEXT_ARRIVAL), EF(EF_LAST_ARRIVAL))));   // RCE:364
-    EI(EI_LOAD_N)++;
-    EI(EI_NUM_ARRIVED) = k + 1;
+                                          __dsub_rn(VF(EF_NEXT_ARRIVAL), VF(EF_LAST_ARRIVAL))));   // RCE:364
+    VI(EI_LOAD_N)++;
+    VI(EI_NUM_ARRIVED) = k + 1;
 }
 
-__global__ void ramp_step_kernel(const StepArgs s) {
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+// One thread per episode, NT per CTA.  Three parts:
+//   prologue  the episode's scalars and the live rows of its running-job table are copied from HBM into shared memory in one batch
+//             of independent loads;
+//   body      the cluster steps on the on-chip copy: the same f64 operations in the same order as on HBM.  Job records, arrivals,
+//             result slots, traces, es rows and the outputs stay in HBM;
+//   epilogue  the scalars and every table row the body may have written go back to HBM, so every other kernel sees the layout
+//             and the values it always saw.
+template <int NT>
+__global__ void __launch_bounds__(NT) ramp_step_kernel(const StepArgs s) {
+    extern __shared__ __align__(16) unsigned char step_smem[];
+    const int b = blockIdx.x * NT + threadIdx.x;
     const EpisodeState& ep = s.ep;
     const int B = ep.B, R = ep.max_running;
     if (b >= B) return;
-    double* ef = ep.ef; int32_t* ei = ep.ei; double* rf = ep.rf; int32_t* ri = ep.ri;
+    const int rows = step_rows(R, ep.max_jobs);
+    EpView v;
+    v.ld = NT; v.rows = rows;
+    v.ef = reinterpret_cast<double*>(step_smem) + threadIdx.x;                    // [EF_COUNT][NT]
+    v.rf = reinterpret_cast<double*>(step_smem) + EF_COUNT * NT + threadIdx.x;    // [RF_COUNT][rows][NT]
+    v.ei = reinterpret_cast<int32_t*>(reinterpret_cast<double*>(step_smem) + (EF_COUNT + RF_COUNT * rows) * NT) + threadIdx.x;   // [EI_COUNT][NT]
+    v.ri = v.ei + EI_COUNT * NT;                                                   // [RI_COUNT][rows][NT]
+    const EpView h = hbm_view(ep, b);
+
+    // ---- prologue ----
+    {
+        double f64[EF_COUNT];
+        int32_t i32[EI_COUNT];
+#pragma unroll
+        for (int f = 0; f < EF_COUNT; ++f) f64[f] = h.ef[f * h.ld];
+#pragma unroll
+        for (int f = 0; f < EI_COUNT; ++f) i32[f] = h.ei[f * h.ld];
+#pragma unroll
+        for (int f = 0; f < EF_COUNT; ++f) VF(f) = f64[f];
+#pragma unroll
+        for (int f = 0; f < EI_COUNT; ++f) VI(f) = i32[f];
+        const int n0 = i32[EI_N_RUNNING];
+        for (int k = 0; k < n0; ++k) {
+            double rf64[RF_COUNT];
+            int32_t ri32[RI_COUNT];
+#pragma unroll
+            for (int f = 0; f < RF_COUNT; ++f) rf64[f] = h.rf[(f * h.rows + k) * h.ld];
+#pragma unroll
+            for (int f = 0; f < RI_COUNT; ++f) ri32[f] = h.ri[(f * h.rows + k) * h.ld];
+#pragma unroll
+            for (int f = 0; f < RF_COUNT; ++f) VRF(f, k) = rf64[f];
+#pragma unroll
+            for (int f = 0; f < RI_COUNT; ++f) VRI(f, k) = ri32[f];
+        }
+    }
+    const int n_jobs = ep.n_jobs_ep[b];
     const ramp_action_t act = s.actions[b];
+    int hi_row = VI(EI_N_RUNNING);          // rows [0, hi_row) may differ from HBM at the end
 
     double st[RAMP_STEP_STATS_LEN];
     double st0[RAMP_STEP_STATS_LEN];
@@ -918,43 +981,43 @@ __global__ void ramp_step_kernel(const StepArgs s) {
     for (int k = 0; k < RAMP_STEP_STATS_LEN; ++k) { st[k] = 0.0; st0[k] = 0.0; }
     int n_cluster_steps = 0;
 
-    if (!((act.flags & RAMP_ACT_SKIP) || EI(EI_DONE))) {
+    if (!((act.flags & RAMP_ACT_SKIP) || VI(EI_DONE))) {
         for (int cs = 0;; ++cs) {
 #pragma unroll
             for (int k = 0; k < RAMP_STEP_STATS_LEN; ++k) st[k] = 0.0;
-            st[RAMP_SS_STEP_COUNTER] = (double)EI(EI_STEP_COUNTER);            // RCE:309
-            st[RAMP_SS_STEP_START_TIME] = EF(EF_NOW);                          // RCE:310
+            st[RAMP_SS_STEP_COUNTER] = (double)VI(EI_STEP_COUNTER);            // RCE:309
+            st[RAMP_SS_STEP_START_TIME] = VF(EF_NOW);                          // RCE:310
             bool has_action = (cs == 0) && act.template_id >= 0;
             int handled = -1;
             if (has_action) {
-                handled = EI(EI_QUEUED);
-                if (handled < 0 || EI(EI_PLAN_SLOT) < 0) {
-                    if (handled < 0) { EI(EI_STATUS) = RAMP_ST_NO_QUEUED_JOB; atomicCAS(&s.counters->err_episode, 0, b + 1); }
+                handled = VI(EI_QUEUED);
+                if (handled < 0 || VI(EI_PLAN_SLOT) < 0) {
+                    if (handled < 0) { VI(EI_STATUS) = RAMP_ST_NO_QUEUED_JOB; atomicCAS(&s.counters->err_episode, 0, b + 1); }
                     has_action = false;
                 }
             }
             // RCE:914-919: queued jobs not handled by the action are blocked
-            if (!has_action && EI(EI_QUEUED) >= 0) step_register_blocked(ep, b, EI(EI_QUEUED), st);
+            if (!has_action && VI(EI_QUEUED) >= 0) step_register_blocked(ep, v, b, VI(EI_QUEUED), st);
 
             if (has_action) {
-                const int slot = EI(EI_PLAN_SLOT);
-                EI(EI_LAST_SLOT) = slot;
-                st[RAMP_SS_LOOKAHEAD_RAN] = (double)EI(EI_PLAN_RAN);
+                const int slot = VI(EI_PLAN_SLOT);
+                VI(EI_LAST_SLOT) = slot;
+                st[RAMP_SS_LOOKAHEAD_RAN] = (double)VI(EI_PLAN_RAN);
                 ramp_job_record_t& r = ep.rec[(size_t)b * ep.max_jobs + handled];
                 r.status = RAMP_JS_RUNNING;
-                r.time_started = EF(EF_NOW);                                    // RCE:1418
-                EI(EI_QUEUED) = -1;                                             // RCE:1420
+                r.time_started = VF(EF_NOW);                                    // RCE:1418
+                VI(EI_QUEUED) = -1;                                             // RCE:1420
                 const int lst = s.res.status[slot];
                 if (lst != RAMP_ST_OK) {                                        // the reference raises (RCE:462)
-                    EI(EI_STATUS) = lst; atomicCAS(&s.counters->err_episode, 0, b + 1);
-                    step_register_blocked(ep, b, handled, st);
+                    VI(EI_STATUS) = lst; atomicCAS(&s.counters->err_episode, 0, b + 1);
+                    step_register_blocked(ep, v, b, handled, st);
                 } else {
                     const double jct = s.res.jct[slot];
                     if (jct > act.max_acceptable_jct) {                         // RCE:815 (strict)
-                        step_register_blocked(ep, b, handled, st);              // RCE:821-824
-                    } else if (EI(EI_N_RUNNING) >= R) {
-                        EI(EI_STATUS) = RAMP_ST_TABLE_FULL; atomicCAS(&s.counters->err_episode, 0, b + 1);
-                        step_register_blocked(ep, b, handled, st);
+                        step_register_blocked(ep, v, b, handled, st);              // RCE:821-824
+                    } else if (VI(EI_N_RUNNING) >= R) {
+                        VI(EI_STATUS) = RAMP_ST_TABLE_FULL; atomicCAS(&s.counters->err_episode, 0, b + 1);
+                        step_register_blocked(ep, v, b, handled, st);
                     } else {
                         // RCE:830-832: computed by the lookahead kernel for its own mounted-worker count; a memo hit from a job
                         // mounted on a different number of workers recomputes it here (serial sum in tick order)
@@ -971,15 +1034,17 @@ __global__ void ramp_step_kernel(const StepArgs s) {
                                                                      __ddiv_rn(s.pool.tick[off + k], jct)));
                             }
                         }
-                        const int row = EI(EI_N_RUNNING)++;
+                        const int row = VI(EI_N_RUNNING)++;
+                        if (row >= hi_row) hi_row = row + 1;
                         const ramp_arrival_t arr = ep.arr[(size_t)b * ep.max_jobs + handled];
-                        RF(RF_JCT, row) = jct; RF(RF_STARTED, row) = EF(EF_NOW);
-                        RF(RF_COMM, row) = s.res.comm[slot]; RF(RF_COMP, row) = s.res.comp[slot]; RF(RF_UTIL, row) = util;
-                        RF(RF_PART_OP_MEM, row) = act.part_op_mem; RF(RF_PART_DEP, row) = act.part_dep_size;
-                        RF(RF_FLOW, row) = act.flow_size;
-                        RF(RF_ORIG_OP_MEM, row) = arr.orig_op_mem; RF(RF_ORIG_DEP, row) = arr.orig_dep_size;
-                        RI(RI_JOB_IDX, row) = handled; RI(RI_N_WORKERS, row) = act.n_mounted_workers;
-                        RI(RI_N_CHANNELS, row) = act.n_mounted_channels;
+                        VRF(RF_JCT, row) = jct; VRF(RF_STARTED, row) = VF(EF_NOW);
+                        VRF(RF_COMM_FRAC, row) = __ddiv_rn(s.res.comm[slot], jct); VRF(RF_COMP_FRAC, row) = __ddiv_rn(s.res.comp[slot], jct);
+                        VRF(RF_UTIL, row) = util;
+                        VRF(RF_PART_OP_MEM, row) = act.part_op_mem; VRF(RF_PART_DEP, row) = act.part_dep_size;
+                        VRF(RF_FLOW, row) = act.flow_size;
+                        VRF(RF_ORIG_OP_MEM, row) = arr.orig_op_mem; VRF(RF_ORIG_DEP, row) = arr.orig_dep_size;
+                        VRI(RI_JOB_IDX, row) = handled; VRI(RI_N_WORKERS, row) = act.n_mounted_workers;
+                        VRI(RI_N_CHANNELS, row) = act.n_mounted_channels;
                         r.jct = jct; r.comm = s.res.comm[slot]; r.comp = s.res.comp[slot]; r.util = util;
                     }
                 }
@@ -991,34 +1056,34 @@ __global__ void ramp_step_kernel(const StepArgs s) {
             int n_frac = 0, n_iter = 0;
             bool step_done = false;
             while (!step_done) {
-                const double now = EF(EF_NOW);
-                double tick = __dsub_rn(EF(EF_NEXT_ARRIVAL), now);                           // RCE:950
+                const double now = VF(EF_NOW);
+                double tick = __dsub_rn(VF(EF_NEXT_ARRIVAL), now);                           // RCE:950
                 { const double b2 = __dsub_rn(ep.max_sim_time, now); if (b2 < tick) tick = b2; }
-                const int nr = EI(EI_N_RUNNING);
+                const int nr = VI(EI_N_RUNNING);
                 for (int k = 0; k < nr; ++k) {                                               // RCE:951-954
-                    const double remaining = __dsub_rn(RF(RF_JCT, k), __dsub_rn(now, RF(RF_STARTED, k)));
+                    const double remaining = __dsub_rn(VRF(RF_JCT, k), __dsub_rn(now, VRF(RF_STARTED, k)));
                     if (remaining < tick) tick = remaining;
                 }
                 int mounted_workers = 0, mounted_channels = 0;
                 double util_sum = 0.0;
                 for (int k = 0; k < nr; ++k) {                                               // RCE:962-982
-                    const double jct = RF(RF_JCT, k);
+                    const double jct = VRF(RF_JCT, k);
                     const double frac = __ddiv_rn(tick, jct);
-                    const double pom = RF(RF_PART_OP_MEM, k), pds = RF(RF_PART_DEP, k);
-                    const double oom = RF(RF_ORIG_OP_MEM, k), ods = RF(RF_ORIG_DEP, k);
+                    const double pom = VRF(RF_PART_OP_MEM, k), pds = VRF(RF_PART_DEP, k);
+                    const double oom = VRF(RF_ORIG_OP_MEM, k), ods = VRF(RF_ORIG_DEP, k);
                     st[RAMP_SS_COMPUTE_INFO_PROCESSED] = __dadd_rn(st[RAMP_SS_COMPUTE_INFO_PROCESSED], __dmul_rn(pom, frac));
                     st[RAMP_SS_DEP_INFO_PROCESSED] = __dadd_rn(st[RAMP_SS_DEP_INFO_PROCESSED], __dmul_rn(pds, frac));
-                    st[RAMP_SS_FLOW_INFO_PROCESSED] = __dadd_rn(st[RAMP_SS_FLOW_INFO_PROCESSED], __dmul_rn(RF(RF_FLOW, k), frac));
+                    st[RAMP_SS_FLOW_INFO_PROCESSED] = __dadd_rn(st[RAMP_SS_FLOW_INFO_PROCESSED], __dmul_rn(VRF(RF_FLOW, k), frac));
                     st[RAMP_SS_CLUSTER_INFO_PROCESSED] = __dadd_rn(st[RAMP_SS_CLUSTER_INFO_PROCESSED], __dmul_rn(__dadd_rn(pom, pds), frac));
                     st[RAMP_SS_DEMAND_COMPUTE_INFO_PROCESSED] = __dadd_rn(st[RAMP_SS_DEMAND_COMPUTE_INFO_PROCESSED], __dmul_rn(oom, frac));
                     st[RAMP_SS_DEMAND_DEP_INFO_PROCESSED] = __dadd_rn(st[RAMP_SS_DEMAND_DEP_INFO_PROCESSED], __dmul_rn(ods, frac));
                     st[RAMP_SS_DEMAND_TOTAL_INFO_PROCESSED] = __dadd_rn(st[RAMP_SS_DEMAND_TOTAL_INFO_PROCESSED], __dmul_rn(__dadd_rn(oom, ods), frac));
-                    sum_comp_frac = __dadd_rn(sum_comp_frac, __ddiv_rn(RF(RF_COMP, k), jct));
-                    sum_comm_frac = __dadd_rn(sum_comm_frac, __ddiv_rn(RF(RF_COMM, k), jct));
+                    sum_comp_frac = __dadd_rn(sum_comp_frac, VRF(RF_COMP_FRAC, k));
+                    sum_comm_frac = __dadd_rn(sum_comm_frac, VRF(RF_COMM_FRAC, k));
                     ++n_frac;
-                    mounted_workers += RI(RI_N_WORKERS, k);      // workers / channels of distinct jobs are disjoint (ramp_rules.py:1-40)
-                    mounted_channels += RI(RI_N_CHANNELS, k);
-                    util_sum = __dadd_rn(util_sum, RF(RF_UTIL, k));
+                    mounted_workers += VRI(RI_N_WORKERS, k);      // workers / channels of distinct jobs are disjoint (ramp_rules.py:1-40)
+                    mounted_channels += VRI(RI_N_CHANNELS, k);
+                    util_sum = __dadd_rn(util_sum, VRF(RF_UTIL, k));
                 }
                 sum_jobs = __dadd_rn(sum_jobs, (double)nr);                                   // RCE:984
                 sum_workers = __dadd_rn(sum_workers, (double)mounted_workers);               // RCE:986
@@ -1035,43 +1100,43 @@ __global__ void ramp_step_kernel(const StepArgs s) {
                     tu[0] = tick_mounted; tu[1] = tick_cluster;
                 }
                 ++n_iter;
-                EF(EF_NOW) = __dadd_rn(now, tick);                                            // RCE:998
-                const double now2 = EF(EF_NOW);
+                VF(EF_NOW) = __dadd_rn(now, tick);                                            // RCE:998
+                const double now2 = VF(EF_NOW);
 
                 // RCE:1004-1017, 1466-1502
                 int k = 0;
-                while (k < EI(EI_N_RUNNING)) {
-                    const double remaining = __dsub_rn(__dsub_rn(RF(RF_JCT, k), __dsub_rn(now2, RF(RF_STARTED, k))), ep.eps);
+                while (k < VI(EI_N_RUNNING)) {
+                    const double remaining = __dsub_rn(__dsub_rn(VRF(RF_JCT, k), __dsub_rn(now2, VRF(RF_STARTED, k))), ep.eps);
                     if (remaining <= 0.0) {
-                        ramp_job_record_t& r = ep.rec[(size_t)b * ep.max_jobs + RI(RI_JOB_IDX, k)];
+                        ramp_job_record_t& r = ep.rec[(size_t)b * ep.max_jobs + VRI(RI_JOB_IDX, k)];
                         r.status = RAMP_JS_COMPLETED; r.time_completed = now2;
-                        r.event_seq = EI(EI_EVENT_SEQ)++;
-                        EI(EI_NUM_COMPLETED)++;
+                        r.event_seq = VI(EI_EVENT_SEQ)++;
+                        VI(EI_NUM_COMPLETED)++;
                         st[RAMP_SS_NUM_JOBS_COMPLETED] += 1.0;
-                        step_remove_running(ep, b, k);
+                        step_remove_running(v, k);
                         step_done = true;
                     } else {
                         ++k;
                     }
                 }
                 // RCE:1019-1040
-                if ((ep.n_jobs_ep[b] - EI(EI_NUM_ARRIVED)) > 0) {
-                    if (__dadd_rn(now2, ep.eps) >= EF(EF_NEXT_ARRIVAL)) {
-                        const int idx = EI(EI_NUM_ARRIVED);
-                        step_get_next_job(ep, b);
+                if ((n_jobs - VI(EI_NUM_ARRIVED)) > 0) {
+                    if (__dadd_rn(now2, ep.eps) >= VF(EF_NEXT_ARRIVAL)) {
+                        const int idx = VI(EI_NUM_ARRIVED);
+                        step_get_next_job(ep, v, b);
                         st[RAMP_SS_NUM_JOBS_ARRIVED] += 1.0;
-                        if (EI(EI_QUEUED) < 0 && ep.queue_capacity >= 1) EI(EI_QUEUED) = idx;   // RCE:1030-1031
-                        else step_register_blocked(ep, b, idx, st);                             // RCE:1034
+                        if (VI(EI_QUEUED) < 0 && ep.queue_capacity >= 1) VI(EI_QUEUED) = idx;   // RCE:1030-1031
+                        else step_register_blocked(ep, v, b, idx, st);                             // RCE:1034
                         step_done = true;
                     }
                 } else {
-                    EF(EF_NEXT_ARRIVAL) = __longlong_as_double(RAMP_INF_BITS);                  // RCE:1040
+                    VF(EF_NEXT_ARRIVAL) = __longlong_as_double(RAMP_INF_BITS);                  // RCE:1040
                 }
-                if (step_is_done(ep, b)) step_done = true;                                       // RCE:1043
+                if (step_is_done(ep, v, n_jobs)) step_done = true;                                       // RCE:1043
             }
 
             // ---- RCE:1046-1084 ----
-            st[RAMP_SS_STEP_END_TIME] = EF(EF_NOW);
+            st[RAMP_SS_STEP_END_TIME] = VF(EF_NOW);
             st[RAMP_SS_STEP_TIME] = __dsub_rn(st[RAMP_SS_STEP_END_TIME], st[RAMP_SS_STEP_START_TIME]);
             st[RAMP_SS_MEAN_NUM_JOBS_RUNNING] = __ddiv_rn(sum_jobs, (double)n_iter);
             st[RAMP_SS_MEAN_NUM_MOUNTED_WORKERS] = __ddiv_rn(sum_workers, (double)n_iter);
@@ -1094,7 +1159,7 @@ __global__ void ramp_step_kernel(const StepArgs s) {
             st[RAMP_SS_UTIL_CLUSTER_SUM] = util_cluster_sum;
             st[RAMP_SS_NUM_TICKS] = (double)n_iter;
             if (ep.tick_util) ep.tick_util_n[b] = n_iter;
-            st[RAMP_SS_JOB_QUEUE_LENGTH] = EI(EI_QUEUED) >= 0 ? 1.0 : 0.0;                       // RCE:1082
+            st[RAMP_SS_JOB_QUEUE_LENGTH] = VI(EI_QUEUED) >= 0 ? 1.0 : 0.0;                       // RCE:1082
             if (s.ep.es) {
                 // eval_loop.py:50-97: this cluster step into the env-step's row, in cluster-step order; the action step (cs 0) opens
                 // it.  The end-of-episode blocks below come after RCE:1084 logged the step, so they are not in it
@@ -1128,30 +1193,25 @@ __global__ void ramp_step_kernel(const StepArgs s) {
                 RAMP_ES_ADD(ES_TICKS, RAMP_SS_NUM_TICKS);
 #undef RAMP_ES_ADD
             }
-            // RCE:1086-1106: this cluster step's contribution to episode_stats.  The addresses come from the kernel parameter, not
-            // from EF()'s `ef`: the kernel sits at 254 registers, and through `ef` ptxas spilled 8 bytes
-            {
-                double* acc = s.ep.ef + b;
-                const size_t Bs = (size_t)s.ep.B;
+            // RCE:1086-1106: this cluster step's contribution to episode_stats
 #pragma unroll
-                for (int k = 0; k < 7; ++k) acc[(EF_ACC_INFO + k) * Bs] = __dadd_rn(acc[(EF_ACC_INFO + k) * Bs], st[RAMP_SS_COMPUTE_INFO_PROCESSED + k]);
-                acc[EF_ACC_COMP_FRAC * Bs] = __dadd_rn(acc[EF_ACC_COMP_FRAC * Bs], st[RAMP_SS_MEAN_COMPUTE_OVERHEAD_FRAC]);
-                acc[EF_ACC_COMM_FRAC * Bs] = __dadd_rn(acc[EF_ACC_COMM_FRAC * Bs], st[RAMP_SS_MEAN_COMMUNICATION_OVERHEAD_FRAC]);
-                acc[EF_ACC_JOBS_RUNNING * Bs] = __dadd_rn(acc[EF_ACC_JOBS_RUNNING * Bs], st[RAMP_SS_MEAN_NUM_JOBS_RUNNING]);
-                acc[EF_ACC_MOUNTED_WORKERS * Bs] = __dadd_rn(acc[EF_ACC_MOUNTED_WORKERS * Bs], st[RAMP_SS_MEAN_NUM_MOUNTED_WORKERS]);
-                acc[EF_ACC_UTIL_MOUNTED * Bs] = __dadd_rn(acc[EF_ACC_UTIL_MOUNTED * Bs], st[RAMP_SS_UTIL_MOUNTED_SUM]);
-                acc[EF_ACC_UTIL_CLUSTER * Bs] = __dadd_rn(acc[EF_ACC_UTIL_CLUSTER * Bs], st[RAMP_SS_UTIL_CLUSTER_SUM]);
-                acc[EF_ACC_TICKS * Bs] = __dadd_rn(acc[EF_ACC_TICKS * Bs], st[RAMP_SS_NUM_TICKS]);
-                acc[EF_ACC_STEPS * Bs] = __dadd_rn(acc[EF_ACC_STEPS * Bs], 1.0);
-            }
-            EI(EI_STEP_COUNTER)++;                                                                // RCE:1109
-            const bool done = step_is_done(ep, b);
+            for (int k = 0; k < 7; ++k) VF(EF_ACC_INFO + k) = __dadd_rn(VF(EF_ACC_INFO + k), st[RAMP_SS_COMPUTE_INFO_PROCESSED + k]);
+            VF(EF_ACC_COMP_FRAC) = __dadd_rn(VF(EF_ACC_COMP_FRAC), st[RAMP_SS_MEAN_COMPUTE_OVERHEAD_FRAC]);
+            VF(EF_ACC_COMM_FRAC) = __dadd_rn(VF(EF_ACC_COMM_FRAC), st[RAMP_SS_MEAN_COMMUNICATION_OVERHEAD_FRAC]);
+            VF(EF_ACC_JOBS_RUNNING) = __dadd_rn(VF(EF_ACC_JOBS_RUNNING), st[RAMP_SS_MEAN_NUM_JOBS_RUNNING]);
+            VF(EF_ACC_MOUNTED_WORKERS) = __dadd_rn(VF(EF_ACC_MOUNTED_WORKERS), st[RAMP_SS_MEAN_NUM_MOUNTED_WORKERS]);
+            VF(EF_ACC_UTIL_MOUNTED) = __dadd_rn(VF(EF_ACC_UTIL_MOUNTED), st[RAMP_SS_UTIL_MOUNTED_SUM]);
+            VF(EF_ACC_UTIL_CLUSTER) = __dadd_rn(VF(EF_ACC_UTIL_CLUSTER), st[RAMP_SS_UTIL_CLUSTER_SUM]);
+            VF(EF_ACC_TICKS) = __dadd_rn(VF(EF_ACC_TICKS), st[RAMP_SS_NUM_TICKS]);
+            VF(EF_ACC_STEPS) = __dadd_rn(VF(EF_ACC_STEPS), 1.0);
+            VI(EI_STEP_COUNTER)++;                                                                // RCE:1109
+            const bool done = step_is_done(ep, v, n_jobs);
             if (done) {                                                                           // RCE:1111-1121
-                while (EI(EI_N_RUNNING) > 0) {
-                    step_register_blocked(ep, b, RI(RI_JOB_IDX, 0), st);
-                    step_remove_running(ep, b, 0);
+                while (VI(EI_N_RUNNING) > 0) {
+                    step_register_blocked(ep, v, b, VRI(RI_JOB_IDX, 0), st);
+                    step_remove_running(v, 0);
                 }
-                EI(EI_DONE) = 1;
+                VI(EI_DONE) = 1;
             }
             st[RAMP_SS_DONE] = done ? 1.0 : 0.0;
             ++n_cluster_steps;
@@ -1160,7 +1220,7 @@ __global__ void ramp_step_kernel(const StepArgs s) {
                 for (int k = 0; k < RAMP_STEP_STATS_LEN; ++k) st0[k] = st[k];
             }
             // RJPE:394-395: while len(job_queue) == 0 and not is_done(): step(Action())
-            if (!s.fuse_empty_steps || done || EI(EI_QUEUED) >= 0) break;
+            if (!s.fuse_empty_steps || done || VI(EI_QUEUED) >= 0) break;
         }
         if (s.ep.es) {
             // the env-step ends: its row (eval_loop.py:74-83).  np.mean over the cluster steps is their sum (in order) / their number;
@@ -1179,11 +1239,23 @@ __global__ void ramp_step_kernel(const StepArgs s) {
             es[RAMP_ESS_MEAN_MOUNTED_WORKER_UTILISATION_FRAC] = __ddiv_rn(es[RAMP_ESS_MEAN_MOUNTED_WORKER_UTILISATION_FRAC], ticks);
             es[RAMP_ESS_MEAN_CLUSTER_WORKER_UTILISATION_FRAC] = __ddiv_rn(es[RAMP_ESS_MEAN_CLUSTER_WORKER_UTILISATION_FRAC], ticks);
         }
-        if (s.fuse_empty_steps) st0[RAMP_SS_DONE] = EI(EI_DONE) ? 1.0 : 0.0;
+        if (s.fuse_empty_steps) st0[RAMP_SS_DONE] = VI(EI_DONE) ? 1.0 : 0.0;
     } else {
-        st0[RAMP_SS_DONE] = EI(EI_DONE) ? 1.0 : 0.0;
-        st0[RAMP_SS_STEP_COUNTER] = (double)EI(EI_STEP_COUNTER);
-        st0[RAMP_SS_JOB_QUEUE_LENGTH] = EI(EI_QUEUED) >= 0 ? 1.0 : 0.0;
+        st0[RAMP_SS_DONE] = VI(EI_DONE) ? 1.0 : 0.0;
+        st0[RAMP_SS_STEP_COUNTER] = (double)VI(EI_STEP_COUNTER);
+        st0[RAMP_SS_JOB_QUEUE_LENGTH] = VI(EI_QUEUED) >= 0 ? 1.0 : 0.0;
+    }
+
+    // ---- epilogue ----
+#pragma unroll
+    for (int f = 0; f < EF_COUNT; ++f) h.ef[f * h.ld] = VF(f);
+#pragma unroll
+    for (int f = 0; f < EI_COUNT; ++f) h.ei[f * h.ld] = VI(f);
+    for (int k = 0; k < hi_row; ++k) {
+#pragma unroll
+        for (int f = 0; f < RF_COUNT; ++f) h.rf[(f * h.rows + k) * h.ld] = VRF(f, k);
+#pragma unroll
+        for (int f = 0; f < RI_COUNT; ++f) h.ri[(f * h.rows + k) * h.ld] = VRI(f, k);
     }
     if (s.stats_out) {
         double* o = s.stats_out + (size_t)b * RAMP_STEP_STATS_LEN;
@@ -1193,11 +1265,12 @@ __global__ void ramp_step_kernel(const StepArgs s) {
     if (s.n_cluster_steps_out) s.n_cluster_steps_out[b] = n_cluster_steps;
 }
 
-// RCE:202-295 for every episode
-__global__ void ramp_reset_kernel(const EpisodeState ep) {
+// RCE:202-295 for every episode; n_jobs_ep (ep.n_jobs_ep, writable) gets every episode's job count
+__global__ void ramp_reset_kernel(const EpisodeState ep, int32_t* n_jobs_ep, int32_t n_jobs) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     const int B = ep.B;
     if (b >= B) return;
+    n_jobs_ep[b] = n_jobs;
     double* ef = ep.ef; int32_t* ei = ep.ei;
     for (int f = 0; f < EF_COUNT; ++f) EF(f) = 0.0;
     for (int f = 0; f < EI_COUNT; ++f) EI(f) = 0;
@@ -1208,7 +1281,7 @@ __global__ void ramp_reset_kernel(const EpisodeState ep) {
         r.time_arrived = r.time_started = r.time_completed = 0.0; r.jct = r.comm = r.comp = r.util = 0.0;
     }
     EF(EF_NEXT_ARRIVAL) = 0.0;                 // RCE:280
-    step_get_next_job(ep, b);                  // RCE:281
+    step_get_next_job(ep, hbm_view(ep, b), b); // RCE:281
     EI(EI_QUEUED) = 0;
 }
 
@@ -1263,7 +1336,9 @@ __global__ void ramp_episode_stats_kernel(const EpisodeState ep, double* out) {
 
 #undef EF
 #undef EI
-#undef RF
-#undef RI
+#undef VF
+#undef VI
+#undef VRF
+#undef VRI
 
 }  // namespace ramp

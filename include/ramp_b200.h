@@ -185,7 +185,8 @@ int ramp_register_template(ramp_engine_t* eng, const ramp_lowered_job_t* job, in
 int ramp_template_count(ramp_engine_t* eng);
 
 /* ---- batched RampClusterEnvironment.reset / step ------------------------------------------------ */
-/* RCE:202-295 for every episode.  arrivals: HOST [n_episodes][n_jobs]; clears the memo (RCE:269-275). */
+/* RCE:202-295 for every episode.  arrivals: HOST [n_episodes][n_jobs], copied before the call returns (the caller may reuse
+ * the array at once); clears the memo (RCE:269-275).  Asynchronous on the engine stream: it does not wait for the device. */
 int ramp_reset(ramp_engine_t* eng, const ramp_arrival_t* arrivals, int32_t n_jobs);
 
 /* Overwrites arrival rows [first_job, first_job + n) of one episode (HOST rows).  Lets a host-driven caller (the
