@@ -15,6 +15,7 @@
 //                           (gnn_policy.py:283-290), then greedy / categorical action selection written straight into the
 //                           environment's action buffer.  All read-out weights are staged once per CTA in shared memory, laid
 //                           out so that lanes read consecutive words.
+#include <algorithm>
 #include <cfloat>
 #include <cmath>
 #include <cstdint>
@@ -385,6 +386,12 @@ struct ramp_policy {
     int32_t bcap = 0, boot_cap = 0, b_rows = 0;
     DeviceArray<float> b_obs, b_logp, b_logp_old, b_adv, b_vt, b_old, b_value, b_lpx, l_boot;
     DeviceArray<int32_t> b_model, b_action, b_actx, l_boot_act; DeviceArray<uint8_t> b_mask; DeviceArray<double> b_adv64;
+    // IMPALA (ramp_policy_learn_impala / ramp_impala_loss_grad): the fragment rows ([icap], row f L + t) with their read-out at
+    // the current weights and V-trace values, the loss's job types (-1 outside it), the host batch's extra inputs, statistics
+    int32_t icap = 0, i_rows = 0, i_step_cap = 0;
+    DeviceArray<float> i_obs, i_blogp, i_tlogits, i_tvalue, i_tlogp, i_log_rho, i_vs, i_pg;
+    DeviceArray<int32_t> i_model, i_action, i_actx, i_lmodel, i_n_rows; DeviceArray<uint8_t> i_mask, i_done;
+    DeviceArray<double> i_reward, i_step_stats, i_stats;
 };
 
 namespace {
@@ -663,6 +670,72 @@ GradArgs host_batch_args(ramp_policy* p, int32_t n) {
     ga.mb = n; ga.start = 0; ga.n_rows = p->l_n_rows.get() + 1;
     ga.graph_features = p->h_gf.get(); ga.model = p->h_model.get(); ga.mask = p->h_mask.get();
     return ga;
+}
+
+int check_impala_config(const ramp_impala_config_t* cfg) {
+    if (!cfg) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (!(cfg->vtrace_clip_rho_threshold > 0) || !(cfg->vtrace_clip_pg_rho_threshold > 0) || !(cfg->lr >= 0) || !(cfg->adam_eps > 0))
+        return set_error(RAMP_ERR_BAD_ARG, "impala: the clip thresholds and adam_eps must be > 0, lr >= 0");
+    if (cfg->rollout_fragment_length < 0 || cfg->train_batch_size < 1)
+        return set_error(RAMP_ERR_BAD_ARG, "impala: rollout_fragment_length must be >= 0, train_batch_size >= 1");
+    return RAMP_OK;
+}
+
+// IMPALA's per-row arrays for n fragment rows, and statistics for `steps` SGD steps
+int ensure_impala(ramp_policy* p, int32_t n, int32_t steps) {
+    const size_t A = p->P.c.n_actions;
+    if (n > p->icap) {
+        p->icap = 0;
+        CUDA_TRY(alloc_each(n, p->i_blogp, p->i_tvalue, p->i_tlogp, p->i_log_rho, p->i_vs, p->i_pg, p->i_model, p->i_action,
+                            p->i_actx, p->i_lmodel, p->i_done, p->i_reward));
+        CUDA_TRY(p->i_obs.alloc((size_t)n * 11));
+        CUDA_TRY(alloc_each((size_t)n * A, p->i_tlogits, p->i_mask));
+        p->icap = n;
+    }
+    if (!p->i_n_rows.get()) {
+        CUDA_TRY(p->i_n_rows.alloc(1));
+        CUDA_TRY(p->i_stats.alloc(RAMP_IMPALA_STATS_LEN));
+    }
+    if (steps > p->i_step_cap) {
+        p->i_step_cap = 0;
+        CUDA_TRY(p->i_step_stats.alloc((size_t)steps * RAMP_IMPALA_STATS_LEN));
+        p->i_step_cap = steps;
+    }
+    return RAMP_OK;
+}
+
+// one IMPALA batch: the fragment rows [row0, row0 + n_frag L) of the i_* arrays, whose model / action / behaviour log p / reward /
+// done are set, read either from the environment-style rows (obs_dyn, i_obs) or host graph features.  The embeddings of
+// launch_states are current.  Read-out at the current weights -> V-trace -> loss gradient (l_grad, the norm partials) -> the
+// step's statistics into `stats`.  ga: the head-gradient launch (its rows, start, row count and inputs), completed here.
+int impala_batch(ramp_policy* p, cudaStream_t st, const ramp_impala_config_t& cfg, int32_t L, int32_t row0, int32_t n_frag,
+                 const float* obs_dyn, const float* graph_features, const int32_t* model, const uint8_t* mask, const int32_t* action,
+                 const float* blogp, const double* reward, const uint8_t* done, GradArgs ga, double* stats) {
+    const ramp_policy_config_t& c = p->P.c;
+    const size_t A = c.n_actions, r0 = (size_t)row0;
+    int rc;
+    HeadArgs h{};
+    h.n = n_frag * L; h.graph_features = graph_features ? graph_features + r0 * c.in_features_graph : nullptr;
+    h.obs_dyn = obs_dyn ? obs_dyn + r0 * 11 : nullptr; h.graph_static = p->d_gstatic.get();
+    h.model = model + r0; h.mask = mask + r0 * A; h.emb = p->d_emb.get();
+    h.logits = p->i_tlogits.get() + r0 * A; h.value = p->i_tvalue.get() + r0; h.actions = p->i_actx.get() + r0;
+    if ((rc = launch_head(p, h, st)) != RAMP_OK) return rc;
+    VtraceArgs v{};
+    v.L = L; v.n_frag = n_frag; v.row0 = row0; v.A = c.n_actions; v.n_models = c.n_models;
+    v.gamma = cfg.gamma; v.clip_rho = cfg.vtrace_clip_rho_threshold; v.clip_pg_rho = cfg.vtrace_clip_pg_rho_threshold;
+    v.logits = p->i_tlogits.get(); v.value = p->i_tvalue.get();
+    v.model = model; v.action = action; v.blogp = blogp; v.reward = reward; v.done = done;
+    v.tlogp = p->i_tlogp.get(); v.log_rho = p->i_log_rho.get(); v.vs = p->i_vs.get(); v.pg_adv = p->i_pg.get(); v.lmodel = p->i_lmodel.get();
+    ramp_vtrace_kernel<<<(unsigned)((n_frag + 7) / 8), 256, 0, st>>>(v);
+    CUDA_TRY(cudaGetLastError());
+    ga.impala = 1; ga.shuffle = 0; ga.graph_features = graph_features; ga.obs_dyn = obs_dyn; ga.model = p->i_lmodel.get(); ga.mask = mask;
+    ga.action = action; ga.adv = p->i_pg.get(); ga.vt = p->i_vs.get();
+    ga.vf_coeff = (float)cfg.vf_loss_coeff; ga.ent_coeff = (float)cfg.entropy_coeff;
+    if ((rc = launch_grad(p, ga, st)) != RAMP_OK) return rc;
+    ramp_impala_step_stats_kernel<<<1, 1, 0, st>>>(p->l_row_stats.get(), p->l_row_model.get(), ga.mb, row0, p->i_log_rho.get(),
+                                                   cfg.vf_loss_coeff, cfg.entropy_coeff, p->l_norm_part.get(), stats);
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
 }
 
 }  // namespace
@@ -1098,6 +1171,119 @@ int ramp_policy_learner_reset(ramp_policy_t* p) {
     CUDA_TRY(cudaMemset(p->l_adam_m.get(), 0, sizeof(float) * p->n_weights));
     CUDA_TRY(cudaMemset(p->l_adam_v.get(), 0, sizeof(float) * p->n_weights));
     CUDA_TRY(cudaMemset(p->l_step.get(), 0, sizeof(int32_t) * 2));
+    return RAMP_OK;
+}
+
+int ramp_impala_loss_grad(ramp_policy_t* p, const ramp_impala_config_t* cfg, int32_t n_fragments, int32_t fragment_length,
+                          const int32_t* model, const float* graph_features, const uint8_t* action_mask, const int32_t* action,
+                          const float* behaviour_logp, const double* reward, const uint8_t* done, float* grad_out,
+                          double* stats_out, float* vs_out, float* pg_adv_out, float* log_rho_out) {
+    if (!p || !model || !graph_features || !action_mask || !action || !behaviour_logp || !reward || !done)
+        return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = check_impala_config(cfg);
+    if (rc != RAMP_OK) return rc;
+    if (n_fragments < 1 || fragment_length < 1 || (int64_t)n_fragments * fragment_length > INT32_MAX)
+        return set_error(RAMP_ERR_BAD_ARG, "impala: loss of %d fragments of %d rows", n_fragments, fragment_length);
+    const int32_t n = n_fragments * fragment_length;
+    CUDA_TRY(cudaSetDevice(p->device));
+    if ((rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n)) || (rc = ensure_impala(p, n, 1)) ||
+        (rc = upload_host_batch(p, n, model, graph_features, action_mask, nullptr, nullptr, action, nullptr, nullptr, nullptr)))
+        return rc;
+    CUDA_TRY(cudaMemcpy(p->i_blogp.get(), behaviour_logp, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->i_reward.get(), reward, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->i_done.get(), done, (size_t)n, cudaMemcpyHostToDevice));
+    if ((rc = launch_states(p, 0, nullptr, 0, nullptr)) != RAMP_OK) return rc;
+    GradArgs ga = host_batch_args(p, n);
+    if ((rc = impala_batch(p, 0, *cfg, fragment_length, 0, n_fragments, nullptr, p->h_gf.get(), p->h_model.get(), p->h_mask.get(),
+                           p->h_action.get(), p->i_blogp.get(), p->i_reward.get(), p->i_done.get(), ga, p->i_stats.get())) != RAMP_OK)
+        return rc;
+    CUDA_TRY(cudaMemsetAsync(p->i_stats.get() + RAMP_IMPALA_SGD_STEPS, 0, sizeof(double), 0));
+    CUDA_TRY(cudaStreamSynchronize(0));
+    p->i_rows = n;
+    if (grad_out) CUDA_TRY(cudaMemcpy(grad_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    if (stats_out) CUDA_TRY(cudaMemcpy(stats_out, p->i_stats.get(), sizeof(double) * RAMP_IMPALA_STATS_LEN, cudaMemcpyDeviceToHost));
+    if (vs_out) CUDA_TRY(cudaMemcpy(vs_out, p->i_vs.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    if (pg_adv_out) CUDA_TRY(cudaMemcpy(pg_adv_out, p->i_pg.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    if (log_rho_out) CUDA_TRY(cudaMemcpy(log_rho_out, p->i_log_rho.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
+int ramp_policy_learn_impala(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_impala_config_t* cfg, double* stats_out) {
+    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = check_impala_config(cfg);
+    if (rc != RAMP_OK) return rc;
+    ramp_env_buffers_t eb{};
+    if ((rc = ramp_env_buffers(eng, &eb)) != RAMP_OK) return rc;
+    if (n_steps < 1 || n_steps > p->traj_n)
+        return set_error(RAMP_ERR_BAD_ARG, "impala: %d steps asked of a trajectory with %d recorded", n_steps, p->traj_n);
+    if (eb.n_episodes != p->traj_b || eb.n_actions != p->traj_a)
+        return set_error(RAMP_ERR_BAD_ARG, "impala: the trajectory was recorded from another environment");
+    const int32_t L = cfg->rollout_fragment_length ? cfg->rollout_fragment_length : n_steps;
+    if (n_steps % L) return set_error(RAMP_ERR_BAD_ARG, "impala: rollout_fragment_length %d does not divide %d steps", L, n_steps);
+    if (cfg->train_batch_size < L)
+        return set_error(RAMP_ERR_BAD_ARG, "impala: train_batch_size %d is below rollout_fragment_length %d", cfg->train_batch_size, L);
+    const ramp_policy_config_t& c = p->P.c;
+    CUDA_TRY(cudaSetDevice(p->device));
+    cudaStream_t st = ramp_internal_stream(eng);
+    const int32_t B = eb.n_episodes, n_frag = (n_steps / L) * B, R = n_steps * B;
+    const int32_t F = std::min(cfg->train_batch_size / L, n_frag), mb = F * L, n_sgd = (n_frag + F - 1) / F;
+    if ((rc = prepare_learner(p, st)) || (rc = ensure_rows(p, mb)) || (rc = ensure_impala(p, R, n_sgd))) return rc;
+    // 1. the fragment rows, fragment-major
+    ImpalaBatchArgs ba{};
+    ba.T = n_steps; ba.B = B; ba.A = c.n_actions; ba.L = L; ba.n_models = c.n_models;
+    ba.t_obs = p->t_obs.get(); ba.t_model = p->t_model.get(); ba.t_mask = p->t_mask.get(); ba.t_action = p->t_action.get();
+    ba.t_logp = p->t_logp.get(); ba.t_reward = p->t_reward.get(); ba.t_done = p->t_done.get();
+    ba.obs = p->i_obs.get(); ba.model = p->i_model.get(); ba.mask = p->i_mask.get(); ba.action = p->i_action.get();
+    ba.blogp = p->i_blogp.get(); ba.reward = p->i_reward.get(); ba.done = p->i_done.get(); ba.n_rows = p->i_n_rows.get();
+    ramp_impala_batch_kernel<<<(unsigned)((R + 255) / 256), 256, 0, st>>>(ba);
+    CUDA_TRY(cudaGetLastError());
+    // 2. one SGD step per train batch, in order
+    AdamArgs aa{};
+    aa.lr = cfg->lr; aa.beta1 = cfg->adam_beta1; aa.beta2 = cfg->adam_beta2;
+    aa.beta2_f = (float)cfg->adam_beta2; aa.one_m_beta1 = (float)(1.0 - cfg->adam_beta1); aa.one_m_beta2 = (float)(1.0 - cfg->adam_beta2);
+    aa.eps = (float)cfg->adam_eps;
+    aa.max_norm = (float)cfg->grad_clip; aa.n_rows = p->i_n_rows.get(); aa.mb = mb; aa.step = p->l_step.get();
+    aa.m = p->l_adam_m.get(); aa.v = p->l_adam_v.get(); aa.grad = p->l_grad.get(); aa.norm_part = p->l_norm_part.get(); aa.w = p->d_w.get();
+    aa.row_stats = nullptr; aa.stats = p->i_stats.get();             // IMPALA's statistics: ramp_impala_step_stats_kernel
+    for (int k = 0; k < n_sgd; ++k) {
+        const int32_t start = k * mb, nf = std::min(F, n_frag - k * F);
+        // the rounds at the current weights, kept for the backward; from the second step on also the embeddings, which the
+        // previous update made stale (the first uses those the trajectory was collected with)
+        if ((rc = launch_states(p, st, p->i_n_rows.get(), start, k ? p->d_emb.get() : nullptr)) != RAMP_OK) return rc;
+        GradArgs ga{};
+        ga.mb = mb; ga.start = start; ga.n_rows = p->i_n_rows.get();
+        if ((rc = impala_batch(p, st, *cfg, L, start, nf, p->i_obs.get(), nullptr, p->i_model.get(), p->i_mask.get(), p->i_action.get(),
+                               p->i_blogp.get(), p->i_reward.get(), p->i_done.get(), ga,
+                               p->i_step_stats.get() + (size_t)k * RAMP_IMPALA_STATS_LEN)) != RAMP_OK)
+            return rc;
+        aa.start = start;
+        aa.parity = p->adam_parity; p->adam_parity ^= 1;
+        ramp_adam_kernel<<<LRN_GRID, 256, 0, st>>>(aa, p->n_weights);
+        CUDA_TRY(cudaGetLastError());
+    }
+    p->emb_valid = false;
+    p->i_rows = R;
+    // 3. the means over the steps: the call's one read-back
+    ramp_impala_learn_stats_kernel<<<1, 1, 0, st>>>(p->i_step_stats.get(), n_sgd, p->i_stats.get());
+    CUDA_TRY(cudaGetLastError());
+    ramp_internal_count_launches(eng, 2 + 9 * n_sgd);
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, p->i_stats.get(), sizeof(double) * RAMP_IMPALA_STATS_LEN, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return RAMP_OK;
+}
+
+int ramp_impala_vtrace_read(ramp_policy_t* p, int32_t* n_out, float* target_logp_out, float* log_rho_out, float* vs_out,
+                            float* pg_adv_out) {
+    if (!p || !n_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (p->i_rows < 1) return set_error(RAMP_ERR_BAD_ARG, "impala: no V-trace yet (ramp_policy_learn_impala / ramp_impala_loss_grad)");
+    CUDA_TRY(cudaSetDevice(p->device));
+    CUDA_TRY(cudaDeviceSynchronize());
+    const size_t n = (size_t)p->i_rows;
+    *n_out = p->i_rows;
+    if (target_logp_out) CUDA_TRY(cudaMemcpy(target_logp_out, p->i_tlogp.get(), 4 * n, cudaMemcpyDeviceToHost));
+    if (log_rho_out) CUDA_TRY(cudaMemcpy(log_rho_out, p->i_log_rho.get(), 4 * n, cudaMemcpyDeviceToHost));
+    if (vs_out) CUDA_TRY(cudaMemcpy(vs_out, p->i_vs.get(), 4 * n, cudaMemcpyDeviceToHost));
+    if (pg_adv_out) CUDA_TRY(cudaMemcpy(pg_adv_out, p->i_pg.get(), 4 * n, cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
 

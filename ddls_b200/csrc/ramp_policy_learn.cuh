@@ -1,8 +1,10 @@
 // ramp_policy_learn.cuh -- the GNN policy's gradient and RLlib's PPO learner step on the device (include/ramp_b200.h:
-// ramp_policy_backward, ramp_ppo_loss_grad, ramp_policy_learn).  Included by ramp_policy.cu after the forward kernels: the forwards
-// recomputed here repeat theirs operation for operation, so a recomputed logit is the one ramp_policy_act produced, bit for bit.
+// ramp_policy_backward, ramp_ppo_loss_grad, ramp_policy_learn) and RLlib's IMPALA learner step (ramp_impala_loss_grad,
+// ramp_policy_learn_impala).  Included by ramp_policy.cu after the forward kernels: the forwards recomputed here repeat theirs
+// operation for operation, so a recomputed logit is the one ramp_policy_act produced, bit for bit.
 //
-//   ramp_policy_head_grad_kernel    one warp per row: the read-out forward, the upstream gradient (given, or RLlib's PPO loss), and
+//   ramp_policy_head_grad_kernel    one warp per row: the read-out forward, the upstream gradient (given, RLlib's PPO loss or
+//                                   IMPALA's VTraceLoss), and
 //                                   its backward through the logits / value layers, both hidden layers and the graph module; a
 //                                   per-row record of what the weight gradients need
 //   ramp_policy_head_reduce_kernel  one thread per read-out / graph-module weight: its gradient summed over the rows in row order
@@ -14,6 +16,9 @@
 //   ramp_adam_kernel                clip_grad_norm_ + torch.optim.Adam; the minibatch's loss statistics
 //   ramp_ppo_gae_kernel             GAE per episode, t-major compaction of the live rows, advantage standardisation
 //   ramp_ppo_learn_stats_kernel     the last pass's mean statistics and RLlib's KL-coefficient update
+//   ramp_impala_batch_kernel        the trajectory cut into fragments of L rows, fragment-major
+//   ramp_vtrace_kernel              one warp per fragment: target log-probabilities (the head kernel's log-softmax), V-trace in f64
+//   ramp_impala_*_stats_kernel      one SGD step's IMPALA statistics; the call's means over its steps
 //
 // Every weight gradient is a sum in a fixed order with an f64 accumulator and no atomics: one call on one batch gives the same bits.
 #pragma once
@@ -163,6 +168,7 @@ struct GradArgs {
     const float* grad_logits; const float* grad_value;              // given upstream gradient (ramp_policy_backward), or
     const int32_t* action; const float* old_logits; const float* adv; const float* vt;     // PPO's (old_logits != nullptr)
     float clip, vf_clip, vf_coeff, ent_coeff, kl_coeff;
+    int32_t impala;                      // IMPALA's VTraceLoss instead: adv is pg_adv, vt is vs (old_logits unused)
     float* rec; int32_t* row_model; float* row_stats;               // [mb][..] outputs
     float* logp_old;                     // [batch] log-probability of the action under the old logits, or nullptr
 };
@@ -240,7 +246,21 @@ __global__ void __launch_bounds__(256) ramp_policy_head_grad_kernel(const Policy
     const float lp = lane < A ? my_logit - best - logf(denom) : 0.f;      // log-softmax, as act's log-probability
     // ---- upstream gradient: d logits (lane o) and d value ----
     float dl = 0.f, dv = 0.f;
-    if (!g.old_logits) {
+    if (g.impala) {
+        // VTraceLoss (impala_torch_policy.py) on one row, summed, not averaged: -logp(a) pg_adv + vf_coeff 0.5 (V - vs)^2
+        // - ent_coeff H(pi), with vs and pg_adv constants.  A masked action has probability 0 and adds exactly 0.
+        const float pr = ex / denom;
+        const int act = g.action[b];
+        const float lp_a = __shfl_sync(0xffffffffu, lp, act);
+        const float pga = g.adv[b], dvv = val - g.vt[b];
+        const float ent = -warp_sum(pr > 0.f ? pr * lp : 0.f);
+        if (lane < A) dl = -pga * ((lane == act ? 1.f : 0.f) - pr) + g.ent_coeff * pr * (lp + ent);
+        dv = g.vf_coeff * dvv;
+        if (lane == 0) {
+            float* rs = g.row_stats + (size_t)i * RS_N;
+            rs[RS_PI] = -lp_a * pga; rs[RS_VF] = 0.5f * dvv * dvv; rs[RS_ENT] = ent; rs[RS_KL] = 0.f; rs[RS_CLIP] = 0.f;
+        }
+    } else if (!g.old_logits) {
         if (lane < A) dl = g.grad_logits[(size_t)b * A + lane];
         dv = g.grad_value[b];
     } else {
@@ -806,6 +826,120 @@ __global__ void __launch_bounds__(1024) ramp_ppo_gae_kernel(const GaeArgs a) {
         for (int i = threadIdx.x; i < n; i += blockDim.x) a.adv[i] = (float)((a.adv[i] - mean) / sd);
     }
     if (threadIdx.x == 0) *a.n_rows = n;
+}
+
+// ---- IMPALA (ramp_policy_learn_impala, ramp_impala_loss_grad) ----
+
+struct ImpalaBatchArgs {
+    int32_t T, B, A, L, n_models;
+    const float* t_obs; const int32_t* t_model; const uint8_t* t_mask; const int32_t* t_action; const float* t_logp;
+    const double* t_reward; const uint8_t* t_done;
+    float* obs; int32_t* model; uint8_t* mask; int32_t* action; float* blogp; double* reward; uint8_t* done; int32_t* n_rows;
+};
+
+// the first T slots of the trajectory as fragments of L rows, fragment f = (time block f / B, episode f % B), row r = f L + t.
+// A row whose episode had already finished, or had nothing queued (or a job type outside the policy's), gets model -1.
+__global__ void ramp_impala_batch_kernel(const ImpalaBatchArgs a) {
+    const int64_t R = (int64_t)a.T * a.B;
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r == 0) *a.n_rows = (int32_t)R;
+    if (r >= R) return;
+    const int64_t f = r / a.L, t = r - f * a.L, j = f / a.B, b = f - j * a.B;
+    const size_t s = (size_t)(j * a.L + t), i = s * a.B + b;
+    const bool alive = s == 0 || !a.t_done[i - a.B];
+    const int32_t m = a.t_model[i];
+    for (int k = 0; k < 11; ++k) a.obs[r * 11 + k] = a.t_obs[i * 11 + k];
+    for (int k = 0; k < a.A; ++k) a.mask[r * a.A + k] = a.t_mask[i * a.A + k];
+    a.model[r] = alive && m >= 0 && m < a.n_models ? m : -1;
+    a.action[r] = a.t_action[i]; a.blogp[r] = a.t_logp[i]; a.reward[r] = a.t_reward[i]; a.done[r] = a.t_done[i];
+}
+
+struct VtraceArgs {
+    int32_t L, n_frag, row0, A, n_models;
+    double gamma, clip_rho, clip_pg_rho;
+    const float* logits; const float* value;                        // the head kernel's at the current weights
+    const int32_t* model; const int32_t* action; const float* blogp; const double* reward; const uint8_t* done;
+    float* tlogp; float* log_rho; float* vs; float* pg_adv; int32_t* lmodel;
+};
+
+// one warp per fragment: the target log-probability of every row's action -- the head kernel's log-softmax, operation for
+// operation, so at the collection weights it is the collected value bit for bit -- then from_importance_weights (vtrace_torch.py)
+// scanning backwards in f64 with vtrace_drop_last_ts: rows 0 .. L-2 are the loss's, row L-1's value is the bootstrap and vs_{L-1}.
+// A row without a decision has log rho 0, V 0 (the head kernel's), its reward and done, and stays out of the loss (lmodel -1).
+__global__ void __launch_bounds__(256) ramp_vtrace_kernel(const VtraceArgs a) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int f = blockIdx.x * (blockDim.x >> 5) + warp;
+    if (f >= a.n_frag) return;
+    const int64_t r0 = (int64_t)a.row0 + (int64_t)f * a.L;
+    for (int t = 0; t < a.L; ++t) {
+        const int64_t r = r0 + t;
+        const int m = a.model[r];
+        if (m < 0 || m >= a.n_models) {
+            if (lane == 0) { a.tlogp[r] = 0.f; a.log_rho[r] = 0.f; }
+            continue;
+        }
+        const float l = lane < a.A ? a.logits[r * a.A + lane] : -FLT_MAX;
+        const float best = warp_max(l);
+        const float ex = lane < a.A ? expf(l - best) : 0.f;
+        const float denom = warp_sum(ex);
+        const float chosen = __shfl_sync(0xffffffffu, l, a.action[r]);
+        if (lane == 0) {
+            const float lp = chosen - best - logf(denom);
+            a.tlogp[r] = lp;
+            a.log_rho[r] = (float)((double)lp - (double)a.blogp[r]);
+        }
+    }
+    if (lane != 0) return;                                          // lane 0 wrote every row's log-probability above
+    const int64_t rl = r0 + a.L - 1;
+    const double boot = a.value[rl];
+    a.vs[rl] = (float)boot; a.pg_adv[rl] = 0.f; a.lmodel[rl] = -1;
+    double v_next = boot, vs_next = boot, acc = 0.0;                // acc: vs_{t+1} - V_{t+1}
+    for (int t = a.L - 2; t >= 0; --t) {
+        const int64_t r = r0 + t;
+        const int m = a.model[r];
+        const bool valid = m >= 0 && m < a.n_models;
+        const double log_rho = valid ? (double)a.tlogp[r] - (double)a.blogp[r] : 0.0;
+        const double rho = exp(log_rho);
+        const double rho_c = fmin(rho, a.clip_rho), c = fmin(rho, 1.0), rho_pg = fmin(rho, a.clip_pg_rho);
+        const double disc = a.gamma * (1.0 - (a.done[r] ? 1.0 : 0.0));
+        const double V = a.value[r], rw = a.reward[r];
+        acc = rho_c * (rw + disc * v_next - V) + disc * c * acc;
+        const double vs = V + acc;
+        a.vs[r] = (float)vs;
+        a.pg_adv[r] = (float)(rho_pg * (rw + disc * vs_next - V));
+        a.lmodel[r] = valid ? m : -1;
+        v_next = V; vs_next = vs;
+    }
+}
+
+// one SGD step's statistics (RAMP_IMPALA_*): the loss's sums over the loss rows, their mean entropy and rho, the gradient's
+// global norm before clipping.  rows of the step: launch row i is batch row row0 + i.
+__global__ void ramp_impala_step_stats_kernel(const float* row_stats, const int32_t* row_model, int32_t rows, int32_t row0,
+                                              const float* log_rho, double vf_coeff, double ent_coeff, const double* norm_part,
+                                              double* out) {
+    double pi = 0.0, vf = 0.0, ent = 0.0, rho = 0.0;
+    int n = 0;
+    for (int i = 0; i < rows; ++i) {
+        if (row_model[i] < 0) continue;
+        const float* s = row_stats + (size_t)i * RS_N;
+        pi += s[RS_PI]; vf += s[RS_VF]; ent += s[RS_ENT];
+        rho += exp((double)log_rho[row0 + i]);
+        ++n;
+    }
+    out[RAMP_IMPALA_TOTAL_LOSS] = pi + vf_coeff * vf - ent_coeff * ent;
+    out[RAMP_IMPALA_POLICY_LOSS] = pi; out[RAMP_IMPALA_VF_LOSS] = vf;
+    out[RAMP_IMPALA_ENTROPY] = n ? ent / n : 0.0; out[RAMP_IMPALA_MEAN_RHO] = n ? rho / n : 0.0;
+    out[RAMP_IMPALA_GRAD_NORM] = sum_norm_parts(norm_part); out[RAMP_IMPALA_ROWS] = n; out[RAMP_IMPALA_SGD_STEPS] = 1;
+}
+
+// the means over the call's SGD steps, and their number
+__global__ void ramp_impala_learn_stats_kernel(const double* step_stats, int32_t n_steps, double* out) {
+    for (int j = 0; j < RAMP_IMPALA_STATS_LEN; ++j) {
+        double s = 0.0;
+        for (int i = 0; i < n_steps; ++i) s += step_stats[(size_t)i * RAMP_IMPALA_STATS_LEN + j];
+        out[j] = n_steps ? s / n_steps : 0.0;
+    }
+    out[RAMP_IMPALA_SGD_STEPS] = n_steps;
 }
 
 }  // namespace ramp

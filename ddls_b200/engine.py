@@ -168,7 +168,8 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_pinned_alloc', 'ramp_pinned_free', 'ramp_policy_trajectory_begin', 'ramp_policy_trajectory_record', 'ramp_policy_trajectory_read',
                     'ramp_env_read_episode', 'ramp_env_set_agents', 'ramp_env_agent_act', 'ramp_policy_get_weights',
                     'ramp_policy_backward', 'ramp_ppo_loss_grad', 'ramp_policy_learn', 'ramp_policy_train_batch_read',
-                    'ramp_policy_learner_state', 'ramp_policy_learner_reset']
+                    'ramp_policy_learner_state', 'ramp_policy_learner_reset', 'ramp_impala_loss_grad', 'ramp_policy_learn_impala',
+                    'ramp_impala_vtrace_read']
 
 
 def device_bytes():

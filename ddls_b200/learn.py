@@ -9,6 +9,11 @@ The loss, GAE and the KL-coefficient update restate RLlib's PPO (ppo_torch_polic
 PPO.update_kl) as published for the ray the reference pins; RLlib itself is not installed, so they are pinned against a float64
 restatement (tests/test_ppo_model.py, tests/test_gpu_policy_learn.py), not against RLlib.
 
+``DeviceIMPALALearner(policy, config)`` is RLlib's IMPALA learner step on the same trajectory (include/ramp_b200.h:
+ramp_impala_loss_grad, ramp_policy_learn_impala): V-trace (vtrace_torch.py) over fragments of rollout_fragment_length rows and
+VTraceLoss (impala_torch_policy.py), one Adam step per train batch, through the same gradient kernels.  ``IMPALAConfig``'s defaults
+are algo/impala.yaml's; its restatement is tests/impala_reference.py.
+
 There is no CPU fallback: the CUDA library is required."""
 from __future__ import annotations
 
@@ -60,6 +65,41 @@ def c_config(cfg: PPOConfig) -> _CConfig:
     return c
 
 
+IMPALA_STATS = ('total_loss', 'policy_loss', 'vf_loss', 'entropy', 'grad_gnorm', 'mean_rho', 'rows', 'sgd_steps')
+
+
+@dataclasses.dataclass
+class IMPALAConfig:
+    """algo/impala.yaml's values; gamma, lr and train_batch_size from rllib_config.yaml's base, which impala.yaml does not
+    override; torch.optim.Adam's defaults, since RLlib passes it only the lr.  rollout_fragment_length 0: the learn call's
+    horizon (one fragment per episode)."""
+    gamma: float = 0.99
+    vtrace_clip_rho_threshold: float = 1.0
+    vtrace_clip_pg_rho_threshold: float = 1.0
+    vf_loss_coeff: float = 0.5
+    entropy_coeff: float = 0.01
+    grad_clip: float = 40.0           # <= 0: no clipping
+    lr: float = 1e-4
+    adam_beta1: float = 0.9
+    adam_beta2: float = 0.999
+    adam_eps: float = 1e-8
+    rollout_fragment_length: int = 0
+    train_batch_size: int = 200
+
+
+class _CIMPALAConfig(C.Structure):
+    _fields_ = [(n, C.c_double) for n in (
+        'gamma', 'vtrace_clip_rho_threshold', 'vtrace_clip_pg_rho_threshold', 'vf_loss_coeff', 'entropy_coeff', 'grad_clip', 'lr',
+        'adam_beta1', 'adam_beta2', 'adam_eps')] + [('rollout_fragment_length', C.c_int32), ('train_batch_size', C.c_int32)]
+
+
+def c_impala_config(cfg: IMPALAConfig) -> _CIMPALAConfig:
+    c = _CIMPALAConfig()
+    for name, ct in _CIMPALAConfig._fields_:
+        setattr(c, name, int(getattr(cfg, name)) if ct is C.c_int32 else float(getattr(cfg, name)))
+    return c
+
+
 def _bind(L):
     if getattr(L, '_learn_bound', False):
         return
@@ -73,6 +113,12 @@ def _bind(L):
     L.ramp_policy_learner_state.argtypes = [C.c_void_p] * 4
     L.ramp_policy_learner_reset.restype = C.c_int
     L.ramp_policy_learner_reset.argtypes = [C.c_void_p]
+    L.ramp_impala_loss_grad.restype = C.c_int
+    L.ramp_impala_loss_grad.argtypes = [C.c_void_p, C.POINTER(_CIMPALAConfig), C.c_int32, C.c_int32] + [C.c_void_p] * 12
+    L.ramp_policy_learn_impala.restype = C.c_int
+    L.ramp_policy_learn_impala.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CIMPALAConfig), C.c_void_p]
+    L.ramp_impala_vtrace_read.restype = C.c_int
+    L.ramp_impala_vtrace_read.argtypes = [C.c_void_p] * 6
     L._learn_bound = True
 
 
@@ -145,6 +191,74 @@ class DevicePPOLearner:
         m, v, step = np.zeros(n, np.float32), np.zeros(n, np.float32), C.c_int32()
         _engine._check(self._L.ramp_policy_learner_state(self.policy._h, m.ctypes.data, v.ctypes.data, C.byref(step)))
         return m, v, step.value
+
+    def reset(self):
+        """zero Adam's moments and step count"""
+        _engine._check(self._L.ramp_policy_learner_reset(self.policy._h))
+
+
+class DeviceIMPALALearner:
+    """RLlib's IMPALA learner step (V-trace, VTraceLoss, clip_grad_norm_, Adam) on the segment the policy's last collect()
+    recorded, on the device.  Adam's moments and step count are the policy's, shared with DevicePPOLearner."""
+
+    def __init__(self, policy, config: IMPALAConfig = None):
+        """policy: a DeviceGNNPolicy, whose weights the learner updates in place"""
+        self.policy = policy
+        self.config = dataclasses.replace(config) if config is not None else IMPALAConfig()
+        self._L = policy._L
+        _bind(self._L)
+
+    def collect_and_learn(self, env, horizon: int, seed: int = 0):
+        """policy.collect(env, horizon) then learn(); also returns the wall time of each (seconds) and the segment's trajectory."""
+        t0 = time.perf_counter()
+        traj = self.policy.collect(env, horizon, sample=True, seed=seed)
+        t1 = time.perf_counter()
+        stats = self.learn(env, horizon)
+        stats['collect_s'], stats['learn_s'] = t1 - t0, time.perf_counter() - t1
+        return stats, traj
+
+    def learn(self, env, horizon: int) -> Dict[str, float]:
+        """One IMPALA learner step on the first ``horizon`` steps of the segment the policy's last collect(env, ...) recorded: the
+        fragments of rollout_fragment_length rows (0: horizon), one Adam step per train batch of train_batch_size // L fragments,
+        in order.  Returns the means over the call's SGD steps (IMPALA_STATS), and their number as sgd_steps."""
+        out = np.zeros(len(IMPALA_STATS), dtype=np.float64)
+        _engine._check(self._L.ramp_policy_learn_impala(self.policy._h, env.eng._h, int(horizon), C.byref(c_impala_config(self.config)),
+                                                        out.ctypes.data))
+        return {k: float(v) for k, v in zip(IMPALA_STATS, out)}
+
+    def vtrace(self) -> Dict[str, np.ndarray]:
+        """per fragment row (r = f L + t) of the last learn() or loss_and_grad(), as the step that used it computed it: the target
+        log-probability of the action (0 on a row without decision), log rho, vs and pg_advantages"""
+        n = C.c_int32()
+        _engine._check(self._L.ramp_impala_vtrace_read(self.policy._h, C.byref(n), None, None, None, None))
+        arrs = {k: np.zeros(n.value, np.float32) for k in ('target_logp', 'log_rho', 'vs', 'pg_advantages')}
+        _engine._check(self._L.ramp_impala_vtrace_read(self.policy._h, C.byref(n), *[a.ctypes.data for a in arrs.values()]))
+        return arrs
+
+    def loss_and_grad(self, batch: Dict[str, np.ndarray]):
+        """VTraceLoss's statistics (IMPALA_STATS, sgd_steps 0) and gradient (blob order) on host fragments, with no update, and
+        the V-trace values (vs, pg_advantages, log_rho; [n, L]).  batch: arrays with leading shape [n fragments, L rows]: model,
+        graph_features [.., in_features_graph], action_mask [.., |A|], action, behaviour_logp, reward, done."""
+        pol = self.policy
+        n, L = np.shape(batch['model'])[:2]
+        model, gf, mask = pol._host_inputs(np.reshape(batch['model'], -1), np.reshape(batch['graph_features'], (n * L, -1)),
+                                           np.reshape(batch['action_mask'], (n * L, -1)))
+        act = np.ascontiguousarray(batch['action'], dtype=np.int32).reshape(n * L)
+        blogp = np.ascontiguousarray(batch['behaviour_logp'], dtype=np.float32).reshape(n * L)
+        reward = np.ascontiguousarray(batch['reward'], dtype=np.float64).reshape(n * L)
+        done = np.ascontiguousarray(batch['done'], dtype=np.uint8).reshape(n * L)
+        grad = np.zeros(pol._L.ramp_policy_weight_count(C.byref(pol._cfg)), dtype=np.float32)
+        out = np.zeros(len(IMPALA_STATS), dtype=np.float64)
+        vt = {k: np.zeros(n * L, np.float32) for k in ('vs', 'pg_advantages', 'log_rho')}
+        _engine._check(self._L.ramp_impala_loss_grad(pol._h, C.byref(c_impala_config(self.config)), int(n), int(L), model.ctypes.data,
+                                                     gf.ctypes.data, mask.ctypes.data, act.ctypes.data, blogp.ctypes.data,
+                                                     reward.ctypes.data, done.ctypes.data, grad.ctypes.data, out.ctypes.data,
+                                                     *[a.ctypes.data for a in vt.values()]))
+        return {k: float(v) for k, v in zip(IMPALA_STATS, out)}, grad, {k: v.reshape(n, L) for k, v in vt.items()}
+
+    def adam_state(self):
+        """torch.optim.Adam's state of the flat weight vector (the policy's, shared with DevicePPOLearner)"""
+        return DevicePPOLearner.adam_state(self)
 
     def reset(self):
         """zero Adam's moments and step count"""

@@ -619,6 +619,64 @@ int ramp_policy_learner_state(ramp_policy_t* p, float* exp_avg_out, float* exp_a
 /* zeroes Adam's moments and step count */
 int ramp_policy_learner_reset(ramp_policy_t* p);
 
+/* ---- RLlib's IMPALA learner step on the device (ray 3.0.0.dev0, as the reference pins it): ray/rllib/algorithms/impala/
+ * impala_torch_policy.py (VTraceLoss, ImpalaTorchPolicy.loss with _make_time_major and vtrace_drop_last_ts) and
+ * vtrace_torch.py (multi_from_logits, from_importance_weights).  It reuses PPO's gradient kernels and Adam, and Adam's moments
+ * and step count are the same policy-owned state (ramp_policy_learner_state / _reset serve both learners).  Only the reference's
+ * IMPALA is supported: opt_type adam, num_sgd_iter 1, minibatch_buffer_size 1, vtrace_drop_last_ts True. */
+typedef struct {
+    double gamma;                         /* rllib_config.yaml's base (impala.yaml does not set it): 0.99                          */
+    double vtrace_clip_rho_threshold;     /* rho-bar = min(rho, this) in the TD errors (algo/impala.yaml: 1.0)                     */
+    double vtrace_clip_pg_rho_threshold;  /* min(rho, this) weights pg_adv (algo/impala.yaml: 1.0)                                 */
+    double vf_loss_coeff, entropy_coeff;  /* VTraceLoss's coefficients (algo/impala.yaml: 0.5, 0.01)                               */
+    double grad_clip;                     /* global-norm clip (clip_grad_norm_; algo/impala.yaml: 40); <= 0: none                  */
+    double lr, adam_beta1, adam_beta2, adam_eps;   /* torch.optim.Adam; RLlib passes only lr (rllib_config.yaml's base: 1e-4)      */
+    int32_t rollout_fragment_length;      /* L: rows per fragment (0: the call's n_steps)                                          */
+    int32_t train_batch_size;             /* rows per SGD step: floor(train_batch_size / L) whole fragments (rllib_config.yaml: 200) */
+} ramp_impala_config_t;
+
+/* statistics (stats_out of ramp_policy_learn_impala: the means over the call's SGD steps; of ramp_impala_loss_grad: its one batch) */
+enum { RAMP_IMPALA_TOTAL_LOSS = 0,        /* pi_loss + vf_loss_coeff vf_loss - entropy_coeff sum(H): VTraceLoss.total_loss        */
+       RAMP_IMPALA_POLICY_LOSS,           /* -sum(valid logp(a) pg_adv)                                                           */
+       RAMP_IMPALA_VF_LOSS,               /* 0.5 sum(valid (V - vs)^2)                                                            */
+       RAMP_IMPALA_ENTROPY,               /* mean H(pi) over the valid rows (VTraceLoss.mean_entropy; 0 with no valid row)        */
+       RAMP_IMPALA_GRAD_NORM,             /* global norm of the gradient before clipping                                          */
+       RAMP_IMPALA_MEAN_RHO,              /* mean rho = exp(log rho) over the valid rows (0 with no valid row)                    */
+       RAMP_IMPALA_ROWS,                  /* valid rows: decisions in rows 0 .. L-2 of their fragment                             */
+       RAMP_IMPALA_SGD_STEPS,             /* learn: the call's Adam steps; loss_grad: 0                                           */
+       RAMP_IMPALA_STATS_LEN };
+
+/* VTraceLoss on n_fragments fragments of fragment_length (L >= 1) HOST rows each, row r = f L + t, and its gradient, with no
+ * update.  Per row: model (outside [0, n_models): no decision), graph_features, action_mask, action, behaviour_logp (the collected
+ * log-probability), reward, done.  With V and log p(a) from the read-out at the current weights, per fragment:
+ *   log rho = log p(a) - behaviour_logp (0 on a row without decision), rho-bar = min(rho, clip_rho), c = min(rho, 1),
+ *   discount = gamma (1 - done); rows 0 .. L-2 are the loss's, V_{L-1} is the bootstrap and vs_{L-1} = V_{L-1};
+ *   delta_t = rho-bar_t (r_t + discount_t V_{t+1} - V_t), vs_t - V_t = delta_t + discount_t c_t (vs_{t+1} - V_{t+1}),
+ *   pg_adv_t = min(rho_t, clip_pg_rho) (r_t + discount_t vs_{t+1} - V_t)          (f64, stored as fp32)
+ *   total = -sum valid logp(a) pg_adv + vf_loss_coeff 0.5 sum valid (V - vs)^2 - entropy_coeff sum valid H(pi)
+ * valid: a decision in rows 0 .. L-2; vs and pg_adv are constants.  grad_out [ramp_policy_weight_count], stats_out
+ * [RAMP_IMPALA_STATS_LEN], vs_out / pg_adv_out / log_rho_out [n_fragments L]: each may be NULL.  cfg's rollout_fragment_length
+ * and train_batch_size are not used. */
+int ramp_impala_loss_grad(ramp_policy_t* p, const ramp_impala_config_t* cfg, int32_t n_fragments, int32_t fragment_length,
+                          const int32_t* model, const float* graph_features, const uint8_t* action_mask, const int32_t* action,
+                          const float* behaviour_logp, const double* reward, const uint8_t* done, float* grad_out,
+                          double* stats_out, float* vs_out, float* pg_adv_out, float* log_rho_out);
+/* One IMPALA learner step on the first n_steps slots of the trajectory of the last ramp_policy_trajectory_begin (the same checks
+ * as ramp_policy_learn), on the engine's stream, nothing read back but stats_out.  L = rollout_fragment_length (0: n_steps);
+ * RAMP_ERR_BAD_ARG unless L divides n_steps and train_batch_size >= L.  Fragments are each episode's column over L consecutive
+ * slots, ordered time block by time block, then by episode; SGD step k takes fragments [k F, (k + 1) F), F =
+ * floor(train_batch_size / L) (the last step may take fewer), in order, not shuffled.  Per step: the embeddings and the read-out
+ * at the current weights (at the collection weights the target log p(a) is the collected one bit for bit), V-trace and the loss
+ * of ramp_impala_loss_grad over the step's fragments, its gradient, clip_grad_norm_ to grad_clip, torch.optim.Adam.  A row
+ * whose episode had already finished, or had nothing queued, is a row without decision.  stats_out [RAMP_IMPALA_STATS_LEN]:
+ * the means over the call's steps, and their number.  The embeddings become stale (the next forward re-embeds). */
+int ramp_policy_learn_impala(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_impala_config_t* cfg, double* stats_out);
+/* HOST copies of the per-row V-trace values of the last ramp_policy_learn_impala or ramp_impala_loss_grad, fragment-major (row
+ * r = f L + t; each as the step that used it computed it): n_out rows, target log p(a) (0 on a row without decision), log rho, vs,
+ * pg_adv.  Any array may be NULL. */
+int ramp_impala_vtrace_read(ramp_policy_t* p, int32_t* n_out, float* target_logp_out, float* log_rho_out, float* vs_out,
+                            float* pg_adv_out);
+
 #ifdef __cplusplus
 }
 #endif
