@@ -82,6 +82,21 @@ struct TraceArrays {
     TracePool view() const { return TracePool{n_active.get(), tick.get(), top.get(), (uint64_t)n_active.size()}; }
 };
 
+// The buffers of one step's lookaheads when steps overlap (ramp_step_device): the speculative plan and bucket run on the plan
+// stream, the thread kernel on the window's stream, and the commit, the repair launch and the step kernel on the engine stream.
+// ev_consumed marks the end of the step kernel that used the window last; the window's next plan waits for it.
+constexpr int N_WINDOWS = 4;
+struct LookaheadWindow {
+    Stream stream;
+    Event ev_planned, ev_end, ev_consumed;
+    DeviceArray<Counters> counters;
+    DeviceArray<WorkItem> items_res, chunk_items;   // [B], [B][32]
+    DeviceArray<ChunkDesc> chunks;                  // [B]
+    DeviceArray<int32_t> rank, tcount, tbase;       // [B], [max_templates + 1] x 2
+    DeviceArray<SpecRecord> rec;                    // [B]
+    DeviceArray<unsigned char> scratch;             // the thread kernel's slabs, [res_grid][res_scratch_stride]
+};
+
 }  // namespace
 
 struct ramp_engine {
@@ -181,10 +196,21 @@ struct ramp_engine {
     DeviceArray<WorkItem> sa_items;      // [n]: the small, big and resident work lists, one after the other
     DeviceArray<int32_t> sa_rank;        // [n] ramp_bucket_kernel scratch
     DeviceArray<Counters> sa_counters;
+    // overlapped steps (ramp_step_device, DESIGN.md §4)
+    int overlap = 1;                     // RAMP_STEP_OVERLAP=0: every step takes the in-order path
+    LookaheadWindow win[N_WINDOWS];      // allocated by the first overlapped step
+    bool win_ready = false;
+    uint64_t win_seq = 0;
+    Stream plan_stream;
+    Event ev_reset;                      // the last ramp_reset's table clears; the next speculative plan waits for it
+    bool reset_pending = false;
+    DeviceArray<unsigned long long> d_spec_keys, d_repair_keys;   // [memo_cap] each: the result and repair tables
+    int32_t spec_base = 0, repair_base = 0;                         // their result slots: [spec_base, spec_base + 2 memo_cap)
     // instrumentation
     int64_t launches = 0;
     Event ev_a[MAX_EVENT_PAIRS], ev_b[MAX_EVENT_PAIRS];
     int ev_pending = 0;
+    double la_ms_union = 0.0;            // union of the event pairs' intervals (overlapped windows count once)
     double la_ms_total = 0.0;
     int64_t la_launches = 0;
     unsigned long long la_items_base = 0, la_bytes_base = 0, la_qbytes_base = 0;
@@ -210,12 +236,23 @@ cudaError_t ramp::reserve_dynamic_smem(const void* kern, size_t bytes) {
 
 namespace {
 
+// adds the pending event pairs to the lookahead time: their sum, and the union of their intervals (the pairs of overlapped
+// steps' windows run at the same time, so only the union is a share of the steps' time)
 int resolve_events(ramp_engine* e) {
+    std::vector<std::pair<float, float>> iv;
     for (int k = 0; k < e->ev_pending; ++k) {
-        float ms = 0.f;
+        float ms = 0.f, t0 = 0.f;
         CUDA_TRY(cudaEventElapsedTime(&ms, e->ev_a[k].get(), e->ev_b[k].get()));
+        CUDA_TRY(cudaEventElapsedTime(&t0, e->ev_a[0].get(), e->ev_a[k].get()));
         e->la_ms_total += ms;
         e->la_launches++;
+        iv.emplace_back(t0, t0 + ms);
+    }
+    std::sort(iv.begin(), iv.end());
+    for (size_t k = 0; k < iv.size();) {
+        float lo = iv[k].first, hi = iv[k].second;
+        for (++k; k < iv.size() && iv[k].first <= hi; ++k) hi = std::max(hi, iv[k].second);
+        e->la_ms_union += hi - lo;
     }
     e->ev_pending = 0;
     return RAMP_OK;
@@ -463,10 +500,10 @@ ThreadArgs make_thread_args(ramp_engine* e, const ChunkDesc* chunks, const WorkI
 
 // groups the resident work items (list 2 of `c`) by template into chunks of <= 32 for the thread kernel, on the device
 void bucket_resident(ramp_engine* e, const WorkItem* items, Counters* c, WorkItem* chunk_items, ChunkDesc* chunks, int32_t* rank,
-                     cudaStream_t st) {
+                     int32_t* tcount, int32_t* tbase, cudaStream_t st) {
     BucketArgs ba{};
     ba.items = items; ba.n_items = &c->n_work_res; ba.n_templates = (int32_t)e->templates.size();
-    ba.tcount = e->d_tcount.get(); ba.tbase = e->d_tbase.get(); ba.chunk_items = chunk_items; ba.chunks = chunks;
+    ba.tcount = tcount; ba.tbase = tbase; ba.chunk_items = chunk_items; ba.chunks = chunks;
     ba.n_chunks = &c->n_chunks; ba.cursor = &c->chunk_cursor; ba.rank = rank;
     ramp_bucket_kernel<<<1, 1024, 0, st>>>(ba);
     e->launches++;
@@ -561,6 +598,102 @@ template <class T> int env_upload(ramp_engine* e, T** dst, const void* src, size
     return RAMP_OK;
 }
 
+// the action rows the engine writes itself, in stream order (ramp_step_host, the device environment): their steps take the
+// in-order path
+bool engine_owned(const ramp_engine* e, const void* p) {
+    const uintptr_t q = (uintptr_t)p;
+    auto in = [q](const void* base, size_t bytes) { return q >= (uintptr_t)base && q < (uintptr_t)base + bytes; };
+    if (in(e->d_actions.get(), sizeof(ramp_action_t) * e->d_actions.size())) return true;
+    for (const auto& a : e->env_allocs) if (in(a.get(), a.size())) return true;
+    return false;
+}
+
+// the windows' buffers, and slabs for the thread kernel's current grid and stride
+int ensure_windows(ramp_engine* e) {
+    const int B = e->cfg.n_episodes;
+    const size_t nt = (size_t)e->cfg.max_templates + 1;
+    if (!e->win_ready) {
+        CUDA_TRY(create(e->plan_stream, cudaStreamNonBlocking));
+        CUDA_TRY(create(e->ev_reset, cudaEventDisableTiming));
+        for (LookaheadWindow& w : e->win) {
+            CUDA_TRY(create(w.stream, cudaStreamNonBlocking));
+            CUDA_TRY(create(w.ev_planned, cudaEventDisableTiming));
+            CUDA_TRY(create(w.ev_end, cudaEventDisableTiming));
+            CUDA_TRY(create(w.ev_consumed, cudaEventDisableTiming));
+            CUDA_TRY(w.counters.alloc(1));
+            CUDA_TRY(cudaMemset(w.counters.get(), 0, sizeof(Counters)));
+            CUDA_TRY(alloc_each(B, w.items_res, w.chunks, w.rank, w.rec));
+            CUDA_TRY(w.chunk_items.alloc((size_t)B * 32));
+            CUDA_TRY(alloc_each(nt, w.tcount, w.tbase));
+            CUDA_TRY(cudaMemset(w.tcount.get(), 0, sizeof(int32_t) * nt));
+        }
+        e->win_ready = true;
+    }
+    const uint64_t bytes = e->res_scratch_stride * (uint64_t)e->res_grid;
+    for (LookaheadWindow& w : e->win) {
+        if (w.scratch.size() == bytes) continue;
+        // every window's thread kernel ends before the step kernel of its step, so the engine stream's end covers them all
+        CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
+        CUDA_TRY(w.scratch.alloc(bytes));
+    }
+    return RAMP_OK;
+}
+
+void launch_step_kernel(ramp_engine* e, const ramp_action_t* d_actions, int32_t fuse, double* d_stats_out, int32_t* d_ncs_out) {
+    const int B = e->cfg.n_episodes;
+    StepArgs s{};
+    s.actions = d_actions; s.ep = e->ep; s.res = e->res.view(); s.pool = e->pool.view(); s.counters = e->d_counters.get();
+    s.stats_out = d_stats_out; s.n_cluster_steps_out = d_ncs_out; s.fuse_empty_steps = fuse;
+    step_kernel_for(e->step_nt)<<<(B + e->step_nt - 1) / e->step_nt, e->step_nt, e->step_smem, e->stream.get()>>>(s);
+    e->launches++;
+}
+
+// One step whose lookaheads may run while the steps before it are still running (DESIGN.md §4):
+//   plan stream     speculative plan (actions read ahead of the step), bucket
+//   window stream   thread kernel
+//   engine stream   commit (the exact plan, in stream order), repair bucket + thread kernel (lookaheads the speculative plan
+//                   missed because the actions changed after it read them; normally none), step kernel
+int step_overlapped(ramp_engine* e, const ramp_action_t* d_actions, int32_t fuse, double* d_stats_out, int32_t* d_ncs_out) {
+    int rc = ensure_windows(e);
+    if (rc != RAMP_OK) return rc;
+    const int B = e->cfg.n_episodes, grid_b = (B + 127) / 128;
+    const int32_t n_templates = (int32_t)e->templates.size();
+    LookaheadWindow& w = e->win[e->win_seq++ % N_WINDOWS];
+    cudaStream_t ps = e->plan_stream.get(), ws = w.stream.get(), st = e->stream.get();
+    if (e->ev_pending >= MAX_EVENT_PAIRS) { CUDA_TRY(cudaStreamSynchronize(st)); rc = resolve_events(e); if (rc) return rc; }
+    CUDA_TRY(cudaStreamWaitEvent(ps, w.ev_consumed.get(), 0));
+    if (e->reset_pending) { CUDA_TRY(cudaStreamWaitEvent(ps, e->ev_reset.get(), 0)); e->reset_pending = false; }
+    SpecPlanArgs sp{};
+    sp.actions = d_actions; sp.templates = e->d_templates.get(); sp.n_templates = n_templates; sp.B = B;
+    sp.keys = e->d_spec_keys.get(); sp.mask = e->memo_cap - 1; sp.slot_base = e->spec_base;
+    sp.items_res = w.items_res.get(); sp.counters = w.counters.get(); sp.rec = w.rec.get();
+    ramp_spec_plan_kernel<<<grid_b, 128, 0, ps>>>(sp);
+    CUDA_TRY(cudaEventRecord(e->ev_a[e->ev_pending].get(), ps));
+    bucket_resident(e, w.items_res.get(), w.counters.get(), w.chunk_items.get(), w.chunks.get(), w.rank.get(), w.tcount.get(), w.tbase.get(), ps);
+    CUDA_TRY(cudaEventRecord(w.ev_planned.get(), ps));
+    CUDA_TRY(cudaStreamWaitEvent(ws, w.ev_planned.get(), 0));
+    ThreadArgs ta = make_thread_args(e, w.chunks.get(), w.chunk_items.get(), w.counters.get(), e->res.view(), e->pool.view(), e->d_stats.get());
+    ta.scratch = w.scratch.get();
+    ramp_lookahead_thread_kernel<<<e->res_grid, RAMP_THREAD_CTA, e->res_smem, ws>>>(ta);
+    CUDA_TRY(cudaEventRecord(e->ev_b[e->ev_pending].get(), ws));
+    e->ev_pending++;
+    CUDA_TRY(cudaEventRecord(w.ev_end.get(), ws));
+    CUDA_TRY(cudaStreamWaitEvent(st, w.ev_end.get(), 0));
+    CommitArgs c{};
+    c.actions = d_actions; c.templates = e->d_templates.get(); c.n_templates = n_templates; c.ep = e->ep;
+    c.memo.keys = e->d_memo_keys.get(); c.memo.mask = e->memo_cap - 1; c.memo.mode = e->cfg.memo_mode; c.memo.vals = e->d_memo_vals.get();
+    c.rec = w.rec.get(); c.repair_keys = e->d_repair_keys.get(); c.repair_mask = e->memo_cap - 1; c.repair_base = e->repair_base;
+    c.items_res = w.items_res.get(); c.win_counters = w.counters.get(); c.counters = e->d_counters.get(); c.stats = e->d_stats.get();
+    ramp_commit_kernel<<<grid_b, 128, 0, st>>>(c);
+    bucket_resident(e, w.items_res.get(), w.counters.get(), w.chunk_items.get(), w.chunks.get(), w.rank.get(), w.tcount.get(), w.tbase.get(), st);
+    ramp_lookahead_thread_kernel<<<e->res_grid, RAMP_THREAD_CTA, e->res_smem, st>>>(ta);   // the repair launch: usually no chunk
+    launch_step_kernel(e, d_actions, fuse, d_stats_out, d_ncs_out);
+    CUDA_TRY(cudaEventRecord(w.ev_consumed.get(), st));
+    e->launches += 4;
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
+}
+
 }  // namespace
 
 // hooks for the other translation units of the library (ramp_policy.cu); not part of the C ABI
@@ -619,6 +752,7 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
         if (!strcmp(v, "thread_unfolded")) e->use_quotient = 0;
     }
     if (const char* v = getenv("RAMP_DEBUG")) e->debug = atoi(v);
+    if (const char* v = getenv("RAMP_STEP_OVERLAP")) e->overlap = atoi(v) != 0;   // 0: the in-order path only (tests compare the two)
     if (const char* v = getenv("RAMP_DENSE_FACTOR")) e->dense_factor = atof(v);
     cudaDeviceProp prop{};
     CUDA_TRY(cudaGetDeviceProperties(&prop, cfg.device));
@@ -635,7 +769,13 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     while (e->memo_cap2 < (uint32_t)cfg.max_templates * 2u) e->memo_cap2 <<= 1;
     CUDA_TRY(e->d_memo_keys2.alloc(e->memo_cap2));
     CUDA_TRY(cudaMemset(e->d_memo_keys2.get(), 0, sizeof(unsigned long long) * e->memo_cap2));
-    e->n_slots = (int32_t)e->memo_cap + B + (int32_t)e->memo_cap2;
+    // slots: the memo's positions, B for RAMP_MEMO_OFF, the level-2 cache, then the result and repair tables of overlapped steps
+    e->spec_base = (int32_t)e->memo_cap + B + (int32_t)e->memo_cap2;
+    e->repair_base = e->spec_base + (int32_t)e->memo_cap;
+    e->n_slots = e->repair_base + (int32_t)e->memo_cap;
+    CUDA_TRY(alloc_each(e->memo_cap, e->d_spec_keys, e->d_repair_keys));
+    CUDA_TRY(cudaMemset(e->d_spec_keys.get(), 0, sizeof(unsigned long long) * e->memo_cap));
+    CUDA_TRY(cudaMemset(e->d_repair_keys.get(), 0, sizeof(unsigned long long) * e->memo_cap));
     CUDA_TRY(e->res.alloc(e->n_slots));
     CUDA_TRY(cudaMemset(e->res.status.get(), 0, sizeof(int32_t) * e->n_slots));
 
@@ -708,6 +848,10 @@ int ramp_engine_destroy(ramp_engine_t* e) {
     if (!e) return RAMP_OK;
     cudaSetDevice(e->cfg.device);
     cudaStreamSynchronize(e->stream.get());
+    if (e->win_ready) {
+        cudaStreamSynchronize(e->plan_stream.get());
+        for (LookaheadWindow& w : e->win) cudaStreamSynchronize(w.stream.get());
+    }
     delete e;
     return RAMP_OK;
 }
@@ -882,6 +1026,12 @@ int ramp_reset(ramp_engine_t* e, const ramp_arrival_t* arrivals, int32_t n_jobs)
     e->ep.n_jobs = n_jobs;
     // memo is per env instance per episode: cleared on reset (RCE:269-275)
     CUDA_TRY(cudaMemsetAsync(e->d_memo_keys.get(), 0, sizeof(unsigned long long) * e->memo_cap, st));
+    if (e->win_ready) {
+        // every window of an enqueued step ends before that step's step kernel, so these clears come after all of them; the
+        // next speculative plan waits for them
+        CUDA_TRY(cudaMemsetAsync(e->d_spec_keys.get(), 0, sizeof(unsigned long long) * e->memo_cap, st));
+        CUDA_TRY(cudaMemsetAsync(e->d_repair_keys.get(), 0, sizeof(unsigned long long) * e->memo_cap, st));
+    }
     // the batch-wide cache of RAMP_MEMO_SHARED (level-2 keys, its result slots and traces) is a pure function of the
     // lowered job and survives the reset; every other mode starts from an empty trace pool
     if (e->cfg.memo_mode != RAMP_MEMO_SHARED) CUDA_TRY(cudaMemsetAsync(e->pool.top.get(), 0, sizeof(unsigned long long), st));
@@ -890,6 +1040,7 @@ int ramp_reset(ramp_engine_t* e, const ramp_arrival_t* arrivals, int32_t n_jobs)
     CUDA_TRY(cudaMemsetAsync(e->d_counters.get(), 0, sizeof(Counters), st));
     ramp_reset_kernel<<<(B + 127) / 128, 128, 0, st>>>(e->ep, e->d_n_jobs_ep.get(), n_jobs);
     e->launches++;
+    if (e->win_ready) { CUDA_TRY(cudaEventRecord(e->ev_reset.get(), st)); e->reset_pending = true; }
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
 }
@@ -930,6 +1081,10 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     if (e->n_nonresident > 0) { int rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
     if (e->n_resident > 0) { int rc = ensure_thread_scratch(e); if (rc != RAMP_OK) return rc; }
+    // the overlapped path covers per-episode memo keys on resident templates; steps with engine-written actions, a template
+    // on the warp / CTA kernels (their launch shape needs the work counts on the host) or another memo mode run in order
+    if (e->overlap && e->cfg.memo_mode == RAMP_MEMO_REFERENCE && e->n_nonresident == 0 && e->n_resident > 0 && !engine_owned(e, d_actions))
+        return step_overlapped(e, d_actions, fuse, d_stats_out, d_ncs_out);
     const int B = e->cfg.n_episodes;
     cudaStream_t st = e->stream.get();
     CUDA_TRY(cudaMemsetAsync(e->d_counters.get(), 0, 4 * sizeof(int32_t), st));   // both work lists' counts and cursors
@@ -946,7 +1101,8 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
         CUDA_TRY(cudaEventRecord(e->ev_a[e->ev_pending].get(), st));
         // memo misses on resident templates: one THREAD per lookahead, grouped on the device.  Their count stays there: idle
         // CTAs find the chunk cursor exhausted and exit.
-        if (e->n_resident > 0) bucket_resident(e, e->d_items_res.get(), e->d_counters.get(), e->d_chunk_items.get(), e->d_chunks.get(), e->d_rank.get(), st);
+        if (e->n_resident > 0) bucket_resident(e, e->d_items_res.get(), e->d_counters.get(), e->d_chunk_items.get(), e->d_chunks.get(), e->d_rank.get(),
+                                        e->d_tcount.get(), e->d_tbase.get(), st);
         int n_small = 0, n_big = 0;
         if (e->n_nonresident > 0) {
             // the number of memo misses of each size class decides the kernel shapes: a 16-byte read-back (~10 us) against
@@ -961,11 +1117,7 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
         CUDA_TRY(cudaEventRecord(e->ev_b[e->ev_pending].get(), st));
         e->ev_pending++;
     }
-    StepArgs s{};
-    s.actions = d_actions; s.ep = e->ep; s.res = e->res.view(); s.pool = e->pool.view(); s.counters = e->d_counters.get();
-    s.stats_out = d_stats_out; s.n_cluster_steps_out = d_ncs_out; s.fuse_empty_steps = fuse;
-    step_kernel_for(e->step_nt)<<<(B + e->step_nt - 1) / e->step_nt, e->step_nt, e->step_smem, st>>>(s);
-    e->launches++;
+    launch_step_kernel(e, d_actions, fuse, d_stats_out, d_ncs_out);
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
 }
@@ -1148,7 +1300,8 @@ int ramp_run_lookaheads(ramp_engine_t* e, const int32_t* template_ids, int32_t n
     Counters c{}; c.n_work = n_small; c.n_work_big = n_big; c.n_work_res = n_res;
     CUDA_TRY(cudaMemcpyAsync(e->sa_items.get(), items.data(), sizeof(WorkItem) * n, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(e->sa_counters.get(), &c, sizeof(Counters), cudaMemcpyHostToDevice, st));
-    if (n_res > 0) bucket_resident(e, d_res, e->sa_counters.get(), e->sa_chunk_items.get(), e->sa_chunks.get(), e->sa_rank.get(), st);
+    if (n_res > 0) bucket_resident(e, d_res, e->sa_counters.get(), e->sa_chunk_items.get(), e->sa_chunks.get(), e->sa_rank.get(),
+                                    e->d_tcount.get(), e->d_tbase.get(), st);
     // traces of standalone runs go to a private pool sized n x trace_cap when requested
     TraceArrays priv;
     const bool want_trace = trace_n && trace_tick && trace_cap > 0;
@@ -1213,10 +1366,28 @@ int ramp_get_lookahead_kernel_time(ramp_engine_t* e, double* total_ms, int64_t* 
     if (launches) *launches = e->la_launches;
     if (work_items) *work_items = (int64_t)(s.lookaheads - e->la_items_base);
     if (alg_bytes) *alg_bytes = (int64_t)(s.alg_bytes - e->la_bytes_base);
-    if (reset) { e->la_ms_total = 0.0; e->la_launches = 0; e->la_items_base = s.lookaheads; e->la_bytes_base = s.alg_bytes; e->la_qbytes_base = s.quotient_bytes; }
+    if (reset) { e->la_ms_total = 0.0; e->la_ms_union = 0.0; e->la_launches = 0; e->la_items_base = s.lookaheads; e->la_bytes_base = s.alg_bytes; e->la_qbytes_base = s.quotient_bytes; }
     return RAMP_OK;
 }
 
+
+int ramp_get_lookahead_kernel_union(ramp_engine_t* e, double* union_ms) {
+    if (!e || !union_ms) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
+    int rc = resolve_events(e);
+    if (rc) return rc;
+    *union_ms = e->la_ms_union;
+    return RAMP_OK;
+}
+
+int ramp_get_memo_speculative_unused(ramp_engine_t* e, int64_t* unused) {
+    if (!e || !unused) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    CUDA_TRY(cudaMemcpyAsync(e->h_stats.get(), e->d_stats.get(), 2 * sizeof(MemoStats), cudaMemcpyDeviceToHost, e->stream.get()));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
+    const MemoStats* s = e->h_stats.get();
+    *unused = (int64_t)((s[0].lookaheads - s[1].lookaheads) - (s[0].ran - s[1].ran));
+    return RAMP_OK;
+}
 
 int ramp_get_quotient_bytes(ramp_engine_t* e, int64_t* quotient_bytes) {
     if (!e || !quotient_bytes) return set_error(RAMP_ERR_BAD_ARG, "null argument");

@@ -97,7 +97,9 @@ struct Counters {               // the first four words are zeroed at the start 
     int32_t _pad;
 };
 
-struct MemoStats { unsigned long long lookups, hits, lookaheads, alg_bytes, shared_hits, quotient_bytes; };
+// ran: plan decisions that ran a lookahead (EI_PLAN_RAN = 1).  lookaheads counts every lookahead executed, including the
+// speculative ones of overlapped steps whose episode turned out not to be live: lookaheads - ran of them went unused
+struct MemoStats { unsigned long long lookups, hits, lookaheads, alg_bytes, shared_hits, quotient_bytes, ran; };
 
 // running-job table fields (SoA: [field][row][episode])
 // RF_COMM_FRAC / RF_COMP_FRAC: the job's comm / jct and comp / jct (RCE:962-982), divided once when it is mounted rather than
@@ -821,6 +823,11 @@ __global__ void ramp_plan_kernel(const PlanArgs p) {
             if (old == key) { slot = (int)pos; break; }                   // hit RCE:495-498
             pos = (pos + 1u) & cap_mask;
         }
+        // RAMP_MEMO_REFERENCE keys are per episode, so only this thread touches `pos`: vals[] holds the slot of the key's result,
+        // which an overlapped step's commit kernel (ramp_commit_kernel) may have put outside the memo's own positions
+        if (p.memo.mode == RAMP_MEMO_REFERENCE && slot >= 0) {
+            if (ran) p.memo.vals[pos] = slot; else slot = p.memo.vals[pos];
+        }
         atomicAdd(&p.stats->lookups, 1ull);
         if (slot >= 0 && !ran) atomicAdd(&p.stats->hits, 1ull);
     }
@@ -832,11 +839,146 @@ __global__ void ramp_plan_kernel(const PlanArgs p) {
     ei[EI_PLAN_SLOT * B + b] = slot;
     ei[EI_PLAN_RAN * B + b] = ran ? 1 : 0;
     if (ran) {
+        atomicAdd(&p.stats->ran, 1ull);
         WorkItem it; it.template_id = act.template_id; it.slot = slot; it.episode = b; it.n_mounted_workers = act.n_mounted_workers;
         if (T.size_class == 2) p.items_res[atomicAdd(&p.counters->n_work_res, 1)] = it;
         else if (T.size_class) p.items_big[atomicAdd(&p.counters->n_work_big, 1)] = it;
         else p.items[atomicAdd(&p.counters->n_work, 1)] = it;
     }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Overlapped steps (RAMP_MEMO_REFERENCE, resident templates; DESIGN.md §4).  A lookahead's result is a function of its template
+// alone, so the lookaheads of step s + 1 can run before step s has finished: the speculative plan of step s + 1 treats every
+// episode with a valid, non-skip action as live and runs each (episode, template) once per reset, into a result table of its
+// own.  The commit kernel then applies ramp_plan_kernel's rule exactly, in stream order, on the memo table and takes each slot
+// from the result table.  An episode whose action changed after the speculative plan read it is planned again by the commit,
+// into a repair table whose lookaheads run on the engine stream before the step kernel.
+
+struct SpecRecord { int32_t flags, template_id, n_mounted_workers, slot; };   // what the speculative plan read, and its slot (-1: none)
+
+// the result-table key: one lookahead per (episode, canonical template) between two resets
+__device__ __forceinline__ unsigned long long spec_key(int b, const TemplateDev& T) {
+    return ((unsigned long long)(b + 1) << 32) | (unsigned long long)(uint32_t)(T.canon_id + 1);
+}
+
+// lookup-or-insert of `key`: its position (-1: table full), *inserted when this call put it there
+__device__ __forceinline__ int claim_key(unsigned long long* keys, uint32_t mask, unsigned long long key, bool* inserted) {
+    uint32_t pos = (uint32_t)splitmix64(key) & mask;
+    *inserted = false;
+    for (uint32_t probe = 0; probe <= mask; ++probe) {
+        const unsigned long long old = atomicCAS(&keys[pos], 0ull, key);
+        if (old == 0ull) { *inserted = true; return (int)pos; }
+        if (old == key) return (int)pos;
+        pos = (pos + 1u) & mask;
+    }
+    return -1;
+}
+
+struct SpecPlanArgs {
+    const ramp_action_t* actions;   // [B] read before the steps ahead of this one have run: a caller may still be writing it
+    const TemplateDev* templates;
+    int32_t n_templates, B;
+    unsigned long long* keys;       // result table
+    uint32_t mask;
+    int32_t slot_base;              // result slot of position 0
+    WorkItem* items_res;            // [B] the window's work list
+    Counters* counters;             // the window's
+    SpecRecord* rec;                // [B]
+};
+
+__global__ void ramp_spec_plan_kernel(const SpecPlanArgs p) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= p.B) return;
+    // each field once, through volatile loads: a torn row only fails the commit's comparison
+    const volatile ramp_action_t* va = p.actions + b;
+    SpecRecord r;
+    r.flags = va->flags; r.template_id = va->template_id; r.n_mounted_workers = va->n_mounted_workers; r.slot = -1;
+    if (!(r.flags & RAMP_ACT_SKIP) && r.template_id >= 0 && r.template_id < p.n_templates) {
+        const TemplateDev& T = p.templates[r.template_id];
+        bool inserted = false;
+        const int pos = T.size_class == 2 ? claim_key(p.keys, p.mask, spec_key(b, T), &inserted) : -1;
+        if (pos >= 0) {
+            r.slot = p.slot_base + pos;
+            if (inserted) {
+                WorkItem it; it.template_id = r.template_id; it.slot = r.slot; it.episode = b; it.n_mounted_workers = r.n_mounted_workers;
+                p.items_res[atomicAdd(&p.counters->n_work_res, 1)] = it;
+            }
+        }
+    }
+    p.rec[b] = r;
+}
+
+struct CommitArgs {
+    const ramp_action_t* actions;   // [B] in stream order
+    const TemplateDev* templates;
+    int32_t n_templates;
+    EpisodeState ep;
+    MemoTable memo;                 // RAMP_MEMO_REFERENCE: keys and vals
+    const SpecRecord* rec;          // [B] the window's speculative plan
+    unsigned long long* repair_keys;
+    uint32_t repair_mask;
+    int32_t repair_base;            // result slot of repair position 0
+    WorkItem* items_res;            // [B] repair work list (the window's, its lookaheads have finished)
+    Counters* win_counters;
+    Counters* counters;             // the engine's: err_episode
+    MemoStats* stats;
+};
+
+// ramp_plan_kernel's rule for RAMP_MEMO_REFERENCE, statement for statement, except where the slot comes from
+__global__ void ramp_commit_kernel(const CommitArgs p) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    const int B = p.ep.B;
+    if (b >= B) return;
+    int32_t* ei = p.ep.ei;
+    ei[EI_PLAN_SLOT * B + b] = -1;
+    ei[EI_PLAN_RAN * B + b] = 0;
+    const ramp_action_t act = p.actions[b];
+    if ((act.flags & RAMP_ACT_SKIP) || ei[EI_DONE * B + b]) return;
+    if (act.template_id < 0) return;
+    if (act.template_id >= p.n_templates) {
+        atomicCAS(&p.counters->err_episode, 0, b + 1);
+        ei[EI_STATUS * B + b] = RAMP_ST_BAD_TEMPLATE;
+        return;
+    }
+    if (ei[EI_QUEUED * B + b] < 0) return;
+    const TemplateDev& T = p.templates[act.template_id];
+    const uint32_t cap_mask = p.memo.mask;
+    const unsigned long long key = ((unsigned long long)(b + 1) << 32) | ((unsigned long long)(T.model_id & 0xFFFF) << 16)
+                                   | (unsigned long long)(T.degree & 0xFFFF);
+    bool ran = false;
+    const int pos = claim_key(p.memo.keys, cap_mask, key, &ran);
+    atomicAdd(&p.stats->lookups, 1ull);
+    if (pos >= 0 && !ran) atomicAdd(&p.stats->hits, 1ull);
+    int slot = -1;
+    if (pos >= 0) {
+        if (!ran) slot = p.memo.vals[pos];
+        else {
+            const SpecRecord r = p.rec[b];
+            if (r.slot >= 0 && r.flags == act.flags && r.template_id == act.template_id && r.n_mounted_workers == act.n_mounted_workers) {
+                slot = r.slot;
+            } else {
+                bool inserted = false;
+                const int q = claim_key(p.repair_keys, p.repair_mask, spec_key(b, T), &inserted);
+                if (q >= 0) {
+                    slot = p.repair_base + q;
+                    if (inserted) {
+                        WorkItem it; it.template_id = act.template_id; it.slot = slot; it.episode = b; it.n_mounted_workers = act.n_mounted_workers;
+                        p.items_res[atomicAdd(&p.win_counters->n_work_res, 1)] = it;
+                    }
+                }
+            }
+            if (slot >= 0) p.memo.vals[pos] = slot;
+        }
+    }
+    if (slot < 0) {
+        atomicCAS(&p.counters->err_episode, 0, b + 1);
+        ei[EI_STATUS * B + b] = RAMP_ST_TABLE_FULL;
+        return;
+    }
+    ei[EI_PLAN_SLOT * B + b] = slot;
+    ei[EI_PLAN_RAN * B + b] = ran ? 1 : 0;
+    if (ran) atomicAdd(&p.stats->ran, 1ull);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -747,8 +747,14 @@ __global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(
             if (c < *a.n_chunks) {
                 const ChunkDesc ch = a.chunks[c];
                 cd = make_int4(c, ch.template_id, ch.count, 0);
-                hv = __ldcg(reinterpret_cast<const int4*>(&a.hints[ch.template_id]));
-                hj = __ldcg(&a.hint_jct[ch.template_id]);
+                // n_ticks is the record's flag: acquired first, the rest of the record is read only when it is set
+                const TemplateHints* hp = &a.hints[ch.template_id];
+                int n_ticks = 0;
+                asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(n_ticks) : "l"(&hp->n_ticks) : "memory");
+                if (n_ticks > 0) {
+                    hv = make_int4(n_ticks, __ldcg(&hp->max_o), __ldcg(&hp->max_f), __ldcg(&hp->max_nf));
+                    hj = __ldcg(&a.hint_jct[ch.template_id]);
+                }
             }
             s_chunk = cd; s_hint = hv; s_hint_jct = hj;
         }
@@ -830,9 +836,14 @@ __global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(
         const SimFinal R = s_fin[lane];           // written before the DONE count ledger_run acquired
         int status = (R.status == RAMP_ST_OK) ? status0 : R.status;
         if (direct && status == RAMP_ST_OK && R.tick_no != hint.n_ticks) status = RAMP_ST_TRACE_OVERFLOW;   // cannot happen
-        if (!fast && status == RAMP_ST_OK) {                      // every lane of the chunk writes the same values
-            *reinterpret_cast<int4*>(&a.hints[tmpl]) = make_int4(R.tick_no, R.max_o, R.max_f, R.max_nf);
+        if (!fast && status == RAMP_ST_OK) {
+            // every lookahead of the template writes the same values, from this CTA or from one of another lookahead window
+            // running at the same time; n_ticks (> 0) is stored last with release semantics, so a reader that acquires it sees
+            // the whole record
+            TemplateHints* hp = &a.hints[tmpl];
+            hp->max_o = R.max_o; hp->max_f = R.max_f; hp->max_nf = R.max_nf;
             a.hint_jct[tmpl] = __dmul_rn(S.t, (double)num_training_steps);
+            asm volatile("st.release.gpu.global.b32 [%0], %1;" :: "l"(&hp->n_ticks), "r"(R.tick_no) : "memory");
         }
 
         // ---- results (RCE:450-452) ----

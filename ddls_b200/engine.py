@@ -133,6 +133,8 @@ def load_library():
     L.ramp_get_episode_stats.argtypes = [C.c_void_p, C.c_void_p]
     L.ramp_get_memo_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.ramp_get_memo_stats_ex.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
+    L.ramp_get_memo_speculative_unused.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
+    L.ramp_get_lookahead_kernel_union.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
     L.ramp_get_last_lookahead.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
     L.ramp_run_lookaheads.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_int32, C.POINTER(C.c_float)]
@@ -146,7 +148,8 @@ def load_library():
                  'ramp_reset', 'ramp_set_arrivals', 'ramp_step_host', 'ramp_step_device', 'ramp_sync', 'ramp_check_status',
                  'ramp_get_job_records', 'ramp_get_episode_state', 'ramp_episode_state_device', 'ramp_export_episode_state_to',
                  'ramp_get_episode_stats', 'ramp_get_memo_stats', 'ramp_get_memo_stats_ex', 'ramp_get_last_lookahead', 'ramp_run_lookaheads',
-                 'ramp_debug_template_info', 'ramp_debug_device_bytes', 'ramp_get_lookahead_kernel_time'):
+                 'ramp_debug_template_info', 'ramp_debug_device_bytes', 'ramp_get_lookahead_kernel_time',
+                 'ramp_get_memo_speculative_unused', 'ramp_get_lookahead_kernel_union'):
         getattr(L, name).restype = C.c_int
     _lib = L
     return L
@@ -156,7 +159,7 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_register_template', 'ramp_template_count', 'ramp_reset', 'ramp_set_arrivals', 'ramp_step_host',
                     'ramp_step_device', 'ramp_sync', 'ramp_check_status', 'ramp_get_job_records',
                     'ramp_get_episode_state', 'ramp_episode_state_device', 'ramp_export_episode_state_to', 'ramp_get_episode_stats',
-                    'ramp_get_memo_stats', 'ramp_get_memo_stats_ex',
+                    'ramp_get_memo_stats', 'ramp_get_memo_stats_ex', 'ramp_get_memo_speculative_unused', 'ramp_get_lookahead_kernel_union',
                     'ramp_get_last_lookahead', 'ramp_run_lookaheads', 'ramp_debug_template_info', 'ramp_launch_count', 'ramp_debug_device_bytes',
                     'ramp_get_lookahead_kernel_time', 'ramp_expand_template', 'ramp_free_expanded_job', 'ramp_free_expanded_aux', 'ramp_first_fit_place',
                     'ramp_quotient_template', 'ramp_free_quotient', 'ramp_get_quotient_bytes', 'ramp_set_job_count',
@@ -351,6 +354,13 @@ class RampEngine:
         _check(self._L.ramp_get_memo_stats_ex(self._h, out))
         return dict(lookups=out[0], hits=out[1], shared_hits=out[2], lookaheads=out[3])
 
+    def speculative_unused(self):
+        """Lookaheads executed since the last reset that no plan used: overlapped steps run the lookaheads of episodes that turn
+        out not to be live when their step runs."""
+        unused = C.c_int64()
+        _check(self._L.ramp_get_memo_speculative_unused(self._h, C.byref(unused)))
+        return unused.value
+
     def last_lookahead(self, episode):
         res = np.zeros(1, dtype=LOOKAHEAD_RESULT_DTYPE)
         tn = np.zeros(self.trace_cap, dtype=np.int32)
@@ -398,9 +408,12 @@ class RampEngine:
         self._L.ramp_get_quotient_bytes.restype = C.c_int
         self._L.ramp_get_quotient_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
         _check(self._L.ramp_get_quotient_bytes(self._h, C.byref(qb)))
+        union = C.c_double()
+        _check(self._L.ramp_get_lookahead_kernel_union(self._h, C.byref(union)))
         _check(self._L.ramp_get_lookahead_kernel_time(self._h, C.byref(ms), C.byref(nl), C.byref(ni), C.byref(nb),
                                                       1 if reset else 0))
-        return dict(total_ms=ms.value, launches=nl.value, work_items=ni.value, algorithmic_bytes=nb.value,
+        # total_ms adds up every step's lookahead interval; union_ms counts the overlapping windows of overlapped steps once
+        return dict(total_ms=ms.value, union_ms=union.value, launches=nl.value, work_items=ni.value, algorithmic_bytes=nb.value,
                     quotient_bytes=qb.value)
 
 

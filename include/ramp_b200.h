@@ -209,7 +209,12 @@ int ramp_set_limits(ramp_engine_t* eng, double max_simulation_run_time, int32_t 
 int ramp_step_host(ramp_engine_t* eng, const ramp_action_t* actions, int32_t fuse_empty_steps,
                    double* stats_out, int32_t* n_cluster_steps_out);
 /* Same with DEVICE pointers (inputs already resident in HBM, outputs left there); asynchronous on the
- * engine stream -- call ramp_sync() before reading. */
+ * engine stream -- call ramp_sync() before reading.
+ * Action readiness: the actions may be written in stream order on the engine stream after the previous call returns.  With
+ * RAMP_MEMO_REFERENCE and every template resident, the lookaheads of a call are planned from the actions as soon as the call
+ * is made, while earlier steps still run, and the plan is checked against the actions in stream order: an episode whose
+ * action changed since is planned again and its lookaheads run before the step (DESIGN.md section 4).  Actions written
+ * ahead of the call are never planned again; engine-owned action buffers always take the in-order path. */
 int ramp_step_device(ramp_engine_t* eng, const ramp_action_t* d_actions, int32_t fuse_empty_steps,
                      double* d_stats_out, int32_t* d_n_cluster_steps_out);
 int ramp_sync(ramp_engine_t* eng);
@@ -255,6 +260,9 @@ int ramp_get_episode_stats(ramp_engine_t* eng, double* out /* HOST [n_episodes][
 int ramp_get_memo_stats(ramp_engine_t* eng, int64_t* lookups, int64_t* hits, int64_t* lookaheads);
 /* {lookups, per-episode hits, batch-wide (shared) hits, lookaheads executed} since the last reset */
 int ramp_get_memo_stats_ex(ramp_engine_t* eng, int64_t out[4]);
+/* lookaheads executed since the last reset whose plan did not use them: overlapped steps plan every episode with a valid,
+ * non-skip action, and the ones that are not live when their step runs leave their lookahead unused */
+int ramp_get_memo_speculative_unused(ramp_engine_t* eng, int64_t* unused);
 /* the lookahead (memoised or fresh) used by episode `episode`'s most recent mount: result + trace
  * (tick_counter_to_active_workers_tick_size RCE:467); trace buffers are HOST, capacity trace_cap. */
 int ramp_get_last_lookahead(ramp_engine_t* eng, int32_t episode, ramp_lookahead_result_t* res,
@@ -287,6 +295,9 @@ int ramp_get_lookahead_kernel_time(ramp_engine_t* eng, double* total_ms, int64_t
 /* the same 20 N + 19 E + 12 T + 24 accounting on the sizes of the symmetry quotients the thread-per-lookahead kernel really
  * simulated (since the last reset of the counters above; read it BEFORE resetting them) */
 int ramp_get_quotient_bytes(ramp_engine_t* eng, int64_t* quotient_bytes);
+/* total_ms above adds every step's lookahead interval; the lookaheads of overlapped steps run at the same time, so this is
+ * the union of the same intervals (ms, reset with them) */
+int ramp_get_lookahead_kernel_union(ramp_engine_t* eng, double* union_ms);
 
 /* ---- native template expansion (SURVEY.md 8f-1): what OpPartition / update_dep_run_times / the SRPT schedulers /
  * FirstFitDepPlacer compute for ONE job placed on a block of servers (sub-op k of every split op on server k), without
