@@ -701,6 +701,13 @@ int ramp_internal_set_error(int code, const char* msg) { g_last_error = msg; ret
 cudaStream_t ramp_internal_stream(ramp_engine_t* e) { return e->stream.get(); }
 int ramp_internal_device(ramp_engine_t* e) { return e->cfg.device; }
 void ramp_internal_count_launches(ramp_engine_t* e, int n) { e->launches += n; }
+// the device environment's per-episode return and env-step count (ramp_es_*); RAMP_ERR_BAD_ARG without an environment
+int ramp_internal_env_returns(ramp_engine_t* e, const double** ret, const int32_t** n_decided) {
+    if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
+    *ret = e->env.ret;
+    *n_decided = e->env.n_decided;
+    return RAMP_OK;
+}
 
 extern "C" {
 

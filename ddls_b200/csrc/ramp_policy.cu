@@ -1288,3 +1288,5 @@ int ramp_impala_vtrace_read(ramp_policy_t* p, int32_t* n_out, float* target_logp
 }
 
 }  // extern "C"
+
+#include "ramp_es.cuh"

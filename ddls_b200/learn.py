@@ -14,6 +14,11 @@ ramp_impala_loss_grad, ramp_policy_learn_impala): V-trace (vtrace_torch.py) over
 VTraceLoss (impala_torch_policy.py), one Adam step per train batch, through the same gradient kernels.  ``IMPALAConfig``'s defaults
 are algo/impala.yaml's; its restatement is tests/impala_reference.py.
 
+``DeviceESLearner(policy, config)`` is RLlib's evolution strategies (include/ramp_b200.h: ramp_es_*): the environment's episodes
+are a population of antithetic weight perturbations, one weight set per episode in one batch, then centered ranks, the
+noise-weighted sum and optimizers.Adam on the device.  ``ESConfig``'s defaults are algo/es.yaml's; its restatement is
+tests/es_reference.py.
+
 There is no CPU fallback: the CUDA library is required."""
 from __future__ import annotations
 
@@ -263,3 +268,209 @@ class DeviceIMPALALearner:
     def reset(self):
         """zero Adam's moments and step count"""
         _engine._check(self._L.ramp_policy_learner_reset(self.policy._h))
+
+
+ES_STATS = ('episode_reward_mean', 'episode_len_mean', 'timesteps_this_iter', 'episodes_this_iter', 'weights_norm', 'grad_norm',
+            'update_ratio', 'eval_return_mean', 'rounds')
+
+
+@dataclasses.dataclass
+class ESConfig:
+    """algo/es.yaml's algo_config over the epoch loop's base (train_batch_size 200: es.yaml comments its own out); optimizers.Adam's
+    betas and epsilon.  action_noise_std is accepted and has no effect on a Discrete action space, as in RLlib.
+    observation_filter: 'NoFilter' only -- RLlib's MeanStdFilter (es.yaml) standardises the flattened observation, padded edge
+    indices and action mask included, which the GNN reads back as they are."""
+    noise_stdev: float = 0.02
+    stepsize: float = 0.01
+    l2_coeff: float = 0.005
+    eval_prob: float = 0.03
+    episodes_per_batch: int = 1000
+    train_batch_size: int = 200
+    report_length: int = 10
+    noise_size: int = 250_000_000
+    adam_beta1: float = 0.99
+    adam_beta2: float = 0.999
+    adam_eps: float = 1e-8
+    action_noise_std: float = 0.01
+    observation_filter: str = 'NoFilter'
+    n_eval: int = None                # eval episodes per round; None: max(1, round(B eval_prob / (2 - eval_prob))), made even with B
+    seed: int = 0
+
+
+class _CESConfig(C.Structure):
+    _fields_ = [('seed', C.c_uint64)] + [(n, C.c_double) for n in (
+        'noise_stdev', 'stepsize', 'l2_coeff', 'adam_beta1', 'adam_beta2', 'adam_eps')] + [
+        (n, C.c_int32) for n in ('episodes_per_batch', 'train_batch_size', 'n_eval', 'report_length')]
+
+
+def shared_noise_table(size: int) -> np.ndarray:
+    """RLlib's shared noise table (es.py create_shared_noise), bit for bit.  At the default size it takes seconds and 1 GB as
+    float32 (2 GB more while numpy draws it in float64)."""
+    return np.random.RandomState(123).randn(int(size)).astype(np.float32)
+
+
+def _bind_es(L):
+    if getattr(L, '_es_bound', False):
+        return
+    for name, args in (('ramp_es_create', [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+                       ('ramp_es_round_begin', [C.c_void_p, C.c_void_p, C.POINTER(_CESConfig), C.c_int32]),
+                       ('ramp_es_act', [C.c_void_p, C.c_void_p, C.c_int32]),
+                       ('ramp_es_round_end', [C.c_void_p, C.c_void_p, C.c_void_p]),
+                       ('ramp_es_step', [C.c_void_p, C.POINTER(_CESConfig), C.c_void_p]),
+                       ('ramp_es_update', [C.c_void_p, C.POINTER(_CESConfig), C.c_int32] + [C.c_void_p] * 5),
+                       ('ramp_es_read', [C.c_void_p] * 12),
+                       ('ramp_es_act_read', [C.c_void_p] * 5),
+                       ('ramp_es_state', [C.c_void_p] * 4),
+                       ('ramp_es_reset', [C.c_void_p])):
+        getattr(L, name).restype = C.c_int
+        getattr(L, name).argtypes = args
+    L.ramp_es_destroy.restype = None
+    L.ramp_es_destroy.argtypes = [C.c_void_p]
+    L._es_bound = True
+
+
+class DeviceESLearner:
+    """RLlib's ES training step (es.py training_step) with a DeviceRampJobPartitioningEnvironment's B episodes as the population:
+    per round, N = (B - E) / 2 antithetic pairs (episode 2i at theta + sigma eps_i, 2i + 1 at theta - sigma eps_i) and E eval
+    episodes at theta, one weight set per episode in one batch; rounds repeat until episodes_per_batch noisy episodes and
+    train_batch_size noisy env-steps were collected; then centered ranks, the noise-weighted sum and optimizers.Adam on the
+    device.  The Adam state is this learner's own: the policy's (DevicePPOLearner / DeviceIMPALALearner) is left alone."""
+
+    def __init__(self, policy, config: ESConfig = None, noise: np.ndarray = None):
+        """policy: a DeviceGNNPolicy, whose weights the learner updates in place.  noise: the shared noise table (float32); None
+        draws shared_noise_table(config.noise_size)."""
+        self.policy = policy
+        self.config = dataclasses.replace(config) if config is not None else ESConfig()
+        if self.config.observation_filter != 'NoFilter':
+            raise ValueError(f"observation_filter {self.config.observation_filter!r}: only 'NoFilter' is supported (MeanStdFilter would "
+                             'standardise the padded edge indices and the action mask the GNN reads back from the observation)')
+        self._L = policy._L
+        _bind_es(self._L)
+        noise = shared_noise_table(self.config.noise_size) if noise is None else np.ascontiguousarray(noise, dtype=np.float32).ravel()
+        self.noise_size = len(noise)
+        self._h = C.c_void_p()
+        _engine._check(self._L.ramp_es_create(policy._h, noise.ctypes.data, self.noise_size, C.byref(self._h)))
+        self._B = 0
+
+    def close(self):
+        if getattr(self, '_h', None):
+            self._L.ramp_es_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def n_eval(self, B: int) -> int:
+        """eval episodes per round of a B-episode environment: config.n_eval, else RLlib's expected share of eval episodes
+        B eval_prob / (2 - eval_prob), at least 1, plus one when B - E would be odd"""
+        if self.config.n_eval is not None:
+            return int(self.config.n_eval)
+        p = self.config.eval_prob
+        E = max(1, int(round(B * p / (2.0 - p))))
+        return E + ((B - E) & 1)
+
+    def _c(self, B: int) -> _CESConfig:
+        c = self.config
+        return _CESConfig(int(c.seed) & (2 ** 64 - 1), float(c.noise_stdev), float(c.stepsize), float(c.l2_coeff), float(c.adam_beta1),
+                          float(c.adam_beta2), float(c.adam_eps), int(c.episodes_per_batch), int(c.train_batch_size), self.n_eval(B),
+                          int(c.report_length))
+
+    def begin_round(self, env, rnd: int):
+        """after env.reset(): round rnd's noise indices, weight sets and embeddings (round 0 starts a new step)"""
+        B = self._B = env.B
+        if B - self.n_eval(B) < 2:
+            raise ValueError(f'{B} episodes less {self.n_eval(B)} eval episodes leave no antithetic pair')
+        _engine._check(self._L.ramp_es_round_begin(self._h, env.eng._h, C.byref(self._c(B)), int(rnd)))
+
+    def act(self, env, t: int):
+        """env-step t of the round: every episode's sampled action from its own weight set into the environment's action buffer"""
+        _engine._check(self._L.ramp_es_act(self._h, env.eng._h, int(t)))
+
+    def end_round(self, env) -> bool:
+        """the round's returns and env-steps into the step record; True while another round is needed"""
+        more = C.c_int32()
+        _engine._check(self._L.ramp_es_round_end(self._h, env.eng._h, C.byref(more)))
+        return bool(more.value)
+
+    def step(self) -> Dict[str, float]:
+        """the update on the step record of the rounds since the last begin_round(env, 0) (ranks, g, Adam); ES_STATS"""
+        out = np.zeros(len(ES_STATS), dtype=np.float64)
+        _engine._check(self._L.ramp_es_step(self._h, C.byref(self._c(self._B)), out.ctypes.data))
+        return {k: float(v) for k, v in zip(ES_STATS, out)}
+
+    def learn(self, env, timing: bool = False) -> Dict[str, float]:
+        """One ES training step (ES_STATS).  Each round resets env and runs env.J env-steps, so every episode ends in it; the
+        round synchronises once, at its end.  timing=True also synchronises after the embeddings and adds the wall time (seconds)
+        of the embeddings (embed_s), of the rollouts (rollout_s) and of the update (update_s)."""
+        B = env.B
+        times = dict(embed_s=0.0, rollout_s=0.0)
+        rnd, more = 0, True
+        while more:
+            env.reset()
+            t0 = time.perf_counter()
+            self.begin_round(env, rnd)
+            if timing:
+                env.eng.sync()
+            t1 = time.perf_counter()
+            for t in range(env.J):
+                self.act(env, t)
+                env.step_device()
+            more = self.end_round(env)
+            _, _, done = env.read()                        # raises what a step would have raised
+            if not done.all():
+                raise Exception(f'{int((~done).sum())} of {B} episodes are not done after {env.J} env-steps')
+            t2 = time.perf_counter()
+            times['embed_s'] += t1 - t0
+            times['rollout_s'] += t2 - t1
+            rnd += 1
+        t3 = time.perf_counter()
+        stats = self.step()
+        if timing:
+            stats.update(times, update_s=time.perf_counter() - t3)
+        return stats
+
+    def update(self, noise_index, returns):
+        """the update on host inputs: noise_index [n], returns [n, 2] (R+, R-) -> (ES_STATS, ranks [n, 2], g [n_weights]); theta
+        and the Adam state change as in learn()"""
+        idx = np.ascontiguousarray(noise_index, dtype=np.int32).ravel()
+        ret = np.ascontiguousarray(returns, dtype=np.float32).reshape(len(idx), 2)
+        ranks = np.zeros((len(idx), 2), np.float32)
+        g = np.zeros(self._L.ramp_policy_weight_count(C.byref(self.policy._cfg)), np.float32)
+        out = np.zeros(len(ES_STATS), dtype=np.float64)
+        _engine._check(self._L.ramp_es_update(self._h, C.byref(self._c(2 * len(idx) + 1)), len(idx), idx.ctypes.data, ret.ctypes.data,
+                                              ranks.ctypes.data, g.ctypes.data, out.ctypes.data))
+        return {k: float(v) for k, v in zip(ES_STATS, out)}, ranks, g
+
+    def last_step(self) -> Dict[str, np.ndarray]:
+        """the last step's record: noise_index [n], returns and lengths [n, 2], the act seeds in order (round-major, env-step t of
+        a round at r J + t), ranks [n, 2], g, eval_returns and eval_lengths"""
+        n, ne, ns = C.c_int32(), C.c_int32(), C.c_int32()
+        _engine._check(self._L.ramp_es_read(self._h, C.byref(n), C.byref(ne), C.byref(ns), *([None] * 9)))
+        n, ne, ns = n.value, ne.value, ns.value
+        out = dict(noise_index=np.zeros(n, np.int32), returns=np.zeros((n, 2), np.float32), lengths=np.zeros((n, 2), np.int32),
+                   seeds=np.zeros(ns, np.uint64), ranks=np.zeros((n, 2), np.float32),
+                   g=np.zeros(self._L.ramp_policy_weight_count(C.byref(self.policy._cfg)), np.float32),
+                   eval_returns=np.zeros(ne, np.float32), eval_lengths=np.zeros(ne, np.int32))
+        _engine._check(self._L.ramp_es_read(self._h, None, None, None, *[a.ctypes.data for a in out.values()]))
+        return out
+
+    def act_read(self, env):
+        """the last act's logits [B, |A|], log-probabilities [B] and actions [B]"""
+        B, A = env.B, self.policy.n_actions
+        logits, logp, actions = np.zeros((B, A), np.float32), np.zeros(B, np.float32), np.zeros(B, np.int32)
+        _engine._check(self._L.ramp_es_act_read(self._h, env.eng._h, logits.ctypes.data, logp.ctypes.data, actions.ctypes.data))
+        return logits, logp, actions
+
+    def adam_state(self):
+        """optimizers.Adam's m, v (blob order) and t"""
+        n = self._L.ramp_policy_weight_count(C.byref(self.policy._cfg))
+        m, v, t = np.zeros(n, np.float32), np.zeros(n, np.float32), C.c_int32()
+        _engine._check(self._L.ramp_es_state(self._h, m.ctypes.data, v.ctypes.data, C.byref(t)))
+        return m, v, t.value
+
+    def reset(self):
+        """zero the ES Adam state"""
+        _engine._check(self._L.ramp_es_reset(self._h))

@@ -688,6 +688,77 @@ int ramp_policy_learn_impala(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_ste
 int ramp_impala_vtrace_read(ramp_policy_t* p, int32_t* n_out, float* target_logp_out, float* log_rho_out, float* vs_out,
                             float* pg_adv_out);
 
+/* ---- RLlib's evolution strategies (ES) training step on the device (ray/rllib/algorithms/es: es.py training_step,
+ * utils.py compute_centered_ranks / batched_weighted_sum, optimizers.py Adam).  The B episodes of a device environment are one
+ * population: episode 2i runs theta + sigma eps_i, episode 2i + 1 runs theta - sigma eps_i (i < N = (B - n_eval) / 2), the last
+ * n_eval episodes run theta; eps_i = noise[k_i : k_i + n] of a HOST table given at creation.  The ES Adam state belongs to the
+ * ES object: the policy's torch-Adam state (ramp_policy_learner_state) is never touched.  No float atomics: one seed gives the
+ * same weights bit for bit. */
+typedef struct ramp_es ramp_es_t;
+
+typedef struct {
+    uint64_t seed;                        /* noise indices and the sampled actions' draws are keyed by (seed, iteration, round, .)  */
+    double noise_stdev;                   /* sigma (algo/es.yaml: 0.02)                                                            */
+    double stepsize, l2_coeff;            /* Adam's step size, the L2 term of -g + l2_coeff theta (es.yaml: 0.01, 0.005)          */
+    double adam_beta1, adam_beta2, adam_eps;       /* optimizers.Adam: 0.99, 0.999, 1e-8                                           */
+    int32_t episodes_per_batch;           /* rounds run until at least this many noisy episodes ... (es.yaml: 1000)                 */
+    int32_t train_batch_size;             /* ... and at least this many noisy env-steps were collected (200)                        */
+    int32_t n_eval;                       /* unperturbed evaluation episodes per round: the last n_eval of the environment's       */
+    int32_t report_length;                /* episode_reward_mean: the mean over the last report_length steps' eval means (10)      */
+} ramp_es_config_t;
+
+/* statistics of a training step (es.py's result and info) */
+enum { RAMP_ES_EPISODE_REWARD_MEAN = 0,   /* mean of the last report_length steps' mean eval return (NaN before any eval episode) */
+       RAMP_ES_EPISODE_LEN_MEAN,          /* mean env-steps of this step's eval episodes (NaN without one)                        */
+       RAMP_ES_TIMESTEPS_THIS_ITER,       /* env-steps of the noisy episodes (ramp_es_update: 0)                                  */
+       RAMP_ES_EPISODES_THIS_ITER,        /* noisy episodes: 2 x pairs                                                            */
+       RAMP_ES_WEIGHTS_NORM,              /* sum theta^2 after the update                                                         */
+       RAMP_ES_GRAD_NORM,                 /* sum g^2                                                                              */
+       RAMP_ES_UPDATE_RATIO,              /* ||step|| / ||theta before the update||                                               */
+       RAMP_ES_EVAL_RETURN_MEAN,          /* mean return of this step's eval episodes (NaN without one)                           */
+       RAMP_ES_ROUNDS,                    /* rounds of the environment this step ran (ramp_es_update: 0)                          */
+       RAMP_ES_STATS_LEN };
+
+/* An ES learner for the policy: uploads noise[noise_size] (a HOST float32 table, RLlib's shared noise table); RAMP_ERR_BAD_ARG
+ * when noise_size < ramp_policy_weight_count. */
+int ramp_es_create(ramp_policy_t* p, const float* noise, int64_t noise_size, ramp_es_t** out);
+void ramp_es_destroy(ramp_es_t* es);
+/* One round of a training step starts: the caller has just reset the environment (its episode streams are drawn on the host).
+ * Round r of iteration it draws pair i's noise index uniformly on [0, noise_size - n] from splitmix64 keyed by (seed, it, r,
+ * 2i), forms every set's weights fl(theta +- fl(sigma eps)) and embeds every (set, job type) in one launch, on the engine's
+ * stream.  Round 0 starts a new step record.  RAMP_ERR_BAD_ARG unless B - n_eval is even and >= 2, or when the policy does
+ * not fit the environment (as ramp_policy_act). */
+int ramp_es_round_begin(ramp_es_t* es, ramp_engine_t* eng, const ramp_es_config_t* cfg, int32_t round);
+/* Env-step t of the round: every episode's sampled action from its own set's weights into the environment's action buffer, one
+ * warp per episode -- ramp_policy_decide's arithmetic and draw (row b, sample 1) with the seed splitmix64 keyed by (seed,
+ * iteration, round, 2t + 1), which is recorded.  No synchronisation. */
+int ramp_es_act(ramp_es_t* es, ramp_engine_t* eng, int32_t t);
+/* The round's end: every episode's return (float of the environment's f64 sum) and env-step count into the step record, one
+ * synchronisation.  *more_out = 1 while the record holds fewer than episodes_per_batch noisy episodes or train_batch_size noisy
+ * env-steps. */
+int ramp_es_round_end(ramp_es_t* es, ramp_engine_t* eng, int32_t* more_out);
+/* The update on the step record: ramp_es_update on its pairs, plus the eval statistics; the policy's weights change in place
+ * and its embeddings become stale.  stats_out [RAMP_ES_STATS_LEN] or NULL. */
+int ramp_es_step(ramp_es_t* es, const ramp_es_config_t* cfg, double* stats_out);
+/* The update on HOST inputs: returns [n_pairs][2] (R+, R-) of pairs with noise indices noise_index [n_pairs] ->
+ *   ranks = compute_centered_ranks over the 2 n_pairs returns in pair order, ties in index order (a stable argsort)
+ *   g = sum_i (rank+_i - rank-_i) eps_i / (2 n_pairs)          (f64 sums in pair order, stored as float32)
+ *   optimizers.Adam on -g + l2_coeff theta, every operation float32, theta written in place.
+ * ranks_out [n_pairs][2], grad_out [ramp_policy_weight_count], stats_out [RAMP_ES_STATS_LEN]: each may be NULL. */
+int ramp_es_update(ramp_es_t* es, const ramp_es_config_t* cfg, int32_t n_pairs, const int32_t* noise_index, const float* returns,
+                   float* ranks_out, float* grad_out, double* stats_out);
+/* HOST copies of the last step's record (any array may be NULL; the counts first): its pairs' noise indices [n_pairs], returns
+ * and env-steps [n_pairs][2], the act seeds in order [n_seeds], the ranks [n_pairs][2], g [ramp_policy_weight_count], the eval
+ * episodes' returns and env-steps [n_eval] */
+int ramp_es_read(ramp_es_t* es, int32_t* n_pairs_out, int32_t* n_eval_out, int32_t* n_seeds_out, int32_t* noise_index_out,
+                 float* returns_out, int32_t* lengths_out, uint64_t* seeds_out, float* ranks_out, float* grad_out,
+                 float* eval_returns_out, int32_t* eval_lengths_out);
+/* HOST copies of the last ramp_es_act's logits [B][n_actions], log-probabilities [B] and actions [B] (any may be NULL) */
+int ramp_es_act_read(ramp_es_t* es, ramp_engine_t* eng, float* logits_out, float* logp_out, int32_t* actions_out);
+/* HOST copies of the ES Adam state (any may be NULL): m, v [ramp_policy_weight_count] and t; ramp_es_reset zeroes them */
+int ramp_es_state(ramp_es_t* es, float* m_out, float* v_out, int32_t* t_out);
+int ramp_es_reset(ramp_es_t* es);
+
 #ifdef __cplusplus
 }
 #endif
