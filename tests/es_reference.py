@@ -118,6 +118,69 @@ class Adam:
         return (theta + step).astype(np.float32), ratio
 
 
+def reward_mean(eval_means, report_length):
+    """es_finish's episode_reward_mean: the mean of the last report_length steps' eval return means (steps without eval episodes
+    add none), NaN before the first"""
+    last = list(eval_means)[-report_length:]
+    return float(np.mean(last)) if last else float('nan')
+
+
+# ---- the launch rules of the population and update kernels (ramp_es.cuh), so that a test can say which of their loops it runs
+
+ES_GRID, ES_THREADS, ES_PAIR_CHUNK = 264, 256, 1024     # ramp_es_update_kernel: CTAs, threads, pairs staged per chunk
+EMBED_CTAS_PER_SM = 2          # ramp_es_embed_kernel: 256 threads at 80 registers fit 3 CTAs per SM; es_scratch caps it at 2
+HEAD_WARPS, HEAD_CTAS_PER_SM = 8, 4                     # ramp_es_act: 8-warp CTAs, at most 4 per SM
+
+
+def population_loops(B, n_eval, n_models, sm_count):
+    """the trip counts of one round's population kernels on a device of sm_count SMs: pairs, sets, (set, job type) items, the
+    embed grid and its largest items per CTA, head warps and their largest episodes per warp"""
+    n_pairs = (B - n_eval) // 2
+    n_sets = 2 * n_pairs + 1
+    items = n_sets * n_models
+    grid = min(EMBED_CTAS_PER_SM * sm_count, items)
+    warps = HEAD_WARPS * max(1, min(-(-B // HEAD_WARPS), HEAD_CTAS_PER_SM * sm_count))
+    return dict(n_pairs=n_pairs, n_sets=n_sets, items=items, embed_grid=grid, items_per_cta=-(-items // grid), head_warps=warps,
+                episodes_per_warp=-(-B // warps))
+
+
+def update_loops(n_pairs, n):
+    """ramp_es_update_kernel's trip counts: pair chunks, and the weight passes of CTA 0 and of the last CTA"""
+    stride = ES_GRID * ES_THREADS
+    passes = [len(range(c * ES_THREADS, n, stride)) for c in (0, ES_GRID - 1)]
+    return dict(pair_chunks=-(-n_pairs // ES_PAIR_CHUNK), max_weight_passes=passes[0], min_weight_passes=passes[1])
+
+
+def set_of_episode(b, n_pairs):
+    """episode b < 2 n_pairs runs set b; the eval episodes run theta, set 2 n_pairs"""
+    return b if b < 2 * n_pairs else 2 * n_pairs
+
+
+def episodes_of_set(s, B, n_pairs):
+    return [s] if s < 2 * n_pairs else list(range(2 * n_pairs, B))
+
+
+def coverage_sets(B, n_eval, n_models, sm_count, n_random=12, seed=0):
+    """{path: weight sets} covering every loop of the population kernels that the round runs: the first and last pair, the eval
+    set, the last (set, job type) item, items on the 2nd, 3rd and last pass of CTA 0, of a middle CTA and of the last CTA (item k
+    runs on CTA k mod grid), episodes on the 2nd and 3rd pass of the first and last head warp (episode b on warp b mod warps),
+    and n_random sets drawn with seed.  The last episode stands for the last warp's last pass.  Paths a round does not reach are
+    left out."""
+    k = population_loops(B, n_eval, n_models, sm_count)
+    N, G, W, items = k['n_pairs'], k['embed_grid'], k['head_warps'], k['items']
+    out = {'first and last pair': [0, 1, 2 * N - 2, 2 * N - 1], 'eval set': [2 * N] if n_eval else [],
+           'last item': [(items - 1) // n_models]}
+    for c in (0, G // 2, G - 1):
+        last = (items - 1 - c) // G
+        out[f'CTA {c}, passes 2, 3, last'] = sorted({(p * G + c) // n_models for p in (1, 2, last) if 1 <= p <= last})
+    for p in (1, 2):
+        if p * W < B:
+            out[f'warp pass {p + 1}'] = sorted({set_of_episode(b, N) for b in (p * W, min(p * W + W - 1, B - 1))})
+    rng = np.random.default_rng(seed)
+    out['random'] = sorted(int(s) for s in rng.choice(2 * N, min(n_random, 2 * N), replace=False))
+    return {path: sets for path, sets in out.items() if sets}
+
+
 def global_grad(theta, g, l2_coeff):
     """es.py: -g + l2_coeff * theta, float32"""
     return (-g + np.float32(l2_coeff) * theta).astype(np.float32)

@@ -1,8 +1,9 @@
 """CPU: the numpy restatement of RLlib's ES update in tests/es_reference.py, which the device ES learner is checked against."""
 import numpy as np
 
-from es_reference import (Adam, compute_centered_ranks, compute_ranks, es_gradient, es_gradient64, global_grad, mix64, noise_indices,
-                          perturbed, training_step)
+from es_reference import (Adam, compute_centered_ranks, compute_ranks, coverage_sets, episodes_of_set, es_gradient, es_gradient64,
+                          global_grad, mix64, noise_indices, perturbed, population_loops, reward_mean, set_of_episode, training_step,
+                          update_loops)
 
 
 def test_ranks_equal_rllibs_default_argsort_without_ties():
@@ -88,3 +89,41 @@ def test_splitmix64_and_noise_indices():
     assert idx.min() >= 0 and idx.max() <= 60 and len(np.unique(idx)) == 61
     np.testing.assert_array_equal(idx, noise_indices(3, 1, 2, 1000, 100, 40))
     assert (idx != noise_indices(3, 1, 3, 1000, 100, 40)).any()
+
+
+def test_reward_mean_is_es_finishs_window():
+    assert np.isnan(reward_mean([], 10))
+    assert reward_mean([1.0, 3.0], 10) == 2.0
+    assert reward_mean(np.arange(12.0), 10) == np.arange(2.0, 12.0).mean()
+
+
+def test_population_loops_on_a_132_sm_part():
+    """the trip counts the GPU tests assert, for the H100's 132 SMs: gnn.yaml at 8,704 episodes, three job types"""
+    k = population_loops(8704, 2, 3, 132)
+    assert (k['n_pairs'], k['n_sets'], k['items'], k['embed_grid']) == (4351, 8703, 26109, 264)
+    assert k['items_per_cta'] == 99 and k['head_warps'] == 4224 and k['episodes_per_warp'] == 3
+    k = population_loops(16, 2, 2, 132)                       # the twin-environment test: one item per CTA, one episode per warp
+    assert k['embed_grid'] == k['items'] == 30 and k['items_per_cta'] == 1 and k['episodes_per_warp'] == 1
+    assert update_loops(1024, 10)['pair_chunks'] == 1 and update_loops(1025, 10)['pair_chunks'] == 2
+    u = update_loops(1100, 305_187)
+    assert (u['pair_chunks'], u['max_weight_passes'], u['min_weight_passes']) == (2, 5, 4)
+    assert update_loops(1, 21_920)['max_weight_passes'] == 1
+
+
+def test_coverage_sets_reach_every_loop():
+    B, E, M, sm = 8704, 2, 3, 132
+    k = population_loops(B, E, M, sm)
+    N, G, W = k['n_pairs'], k['embed_grid'], k['head_warps']
+    cov = coverage_sets(B, E, M, sm)
+    sets = sorted({s for v in cov.values() for s in v})
+    assert 20 <= len(sets) <= 40 and all(0 <= s <= 2 * N for s in sets)
+    items = {it for s in sets for it in range(s * M, (s + 1) * M)}
+    for c in (0, G - 1):
+        passes = {it // G for it in items if it % G == c}
+        assert {1, 2, (k['items'] - 1 - c) // G} <= passes, c
+    assert k['items'] - 1 in items
+    eps = {b for s in sets for b in episodes_of_set(s, B, N)}
+    assert {b // W for b in eps} == {0, 1, 2} and B - 1 in eps and {0, 1, 2 * N - 2, 2 * N - 1} <= eps
+    assert [set_of_episode(b, N) for b in (2 * N - 1, 2 * N, B - 1)] == [2 * N - 1, 2 * N, 2 * N]
+    assert episodes_of_set(2 * N, B, N) == [B - 2, B - 1]
+    assert 'eval set' not in coverage_sets(16, 0, 2, sm)          # n_eval = 0: every episode runs its own set
