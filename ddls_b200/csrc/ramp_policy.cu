@@ -382,7 +382,7 @@ struct ramp_policy {
     // host-input batches of ramp_policy_backward / ramp_ppo_loss_grad
     int32_t hcap = 0;
     DeviceArray<int32_t> h_model, h_action; DeviceArray<float> h_gf, h_gl, h_gv, h_old, h_adv, h_vt; DeviceArray<uint8_t> h_mask;
-    // ramp_policy_learn's train batch ([horizon * B] rows, live rows first, t-major) and bootstrap values ([B])
+    // ramp_policy_learn's / ramp_policy_learn_pg's train batch ([horizon * B] rows, live rows first, t-major) and bootstrap values ([B])
     int32_t bcap = 0, boot_cap = 0, b_rows = 0;
     DeviceArray<float> b_obs, b_logp, b_logp_old, b_adv, b_vt, b_old, b_value, b_lpx, l_boot;
     DeviceArray<int32_t> b_model, b_action, b_actx, l_boot_act; DeviceArray<uint8_t> b_mask; DeviceArray<double> b_adv64;
@@ -665,6 +665,17 @@ int upload_host_batch(ramp_policy* p, int32_t n, const int32_t* model, const flo
     return RAMP_OK;
 }
 
+// the train batch of ramp_policy_learn / ramp_policy_learn_pg for `rows` trajectory slots
+int ensure_batch(ramp_policy* p, int32_t rows) {
+    if (rows <= p->bcap) return RAMP_OK;
+    p->bcap = 0;
+    CUDA_TRY(alloc_each(rows, p->b_logp, p->b_logp_old, p->b_adv, p->b_vt, p->b_value, p->b_lpx, p->b_model, p->b_action, p->b_actx, p->b_adv64));
+    CUDA_TRY(p->b_obs.alloc((size_t)rows * 11));
+    CUDA_TRY(alloc_each((size_t)rows * p->P.c.n_actions, p->b_mask, p->b_old));
+    p->bcap = rows;
+    return RAMP_OK;
+}
+
 GradArgs host_batch_args(ramp_policy* p, int32_t n) {
     GradArgs ga{};
     ga.mb = n; ga.start = 0; ga.n_rows = p->l_n_rows.get() + 1;
@@ -678,6 +689,12 @@ int check_impala_config(const ramp_impala_config_t* cfg) {
         return set_error(RAMP_ERR_BAD_ARG, "impala: the clip thresholds and adam_eps must be > 0, lr >= 0");
     if (cfg->rollout_fragment_length < 0 || cfg->train_batch_size < 1)
         return set_error(RAMP_ERR_BAD_ARG, "impala: rollout_fragment_length must be >= 0, train_batch_size >= 1");
+    return RAMP_OK;
+}
+
+int check_pg_config(const ramp_pg_config_t* cfg) {
+    if (!cfg) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (!(cfg->gamma >= 0) || !(cfg->lr >= 0) || !(cfg->adam_eps > 0)) return set_error(RAMP_ERR_BAD_ARG, "pg: gamma and lr must be >= 0, adam_eps > 0");
     return RAMP_OK;
 }
 
@@ -1045,14 +1062,7 @@ int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, con
     CUDA_TRY(cudaSetDevice(p->device));
     cudaStream_t st = ramp_internal_stream(eng);
     const int32_t B = eb.n_episodes, rows = n_steps * B, mb = cfg->sgd_minibatch_size, n_mb = (rows + mb - 1) / mb;
-    if ((rc = prepare_learner(p, st)) || (rc = ensure_rows(p, mb))) return rc;
-    if (rows > p->bcap) {
-        p->bcap = 0;
-        CUDA_TRY(alloc_each(rows, p->b_logp, p->b_logp_old, p->b_adv, p->b_vt, p->b_value, p->b_lpx, p->b_model, p->b_action, p->b_actx, p->b_adv64));
-        CUDA_TRY(p->b_obs.alloc((size_t)rows * 11));
-        CUDA_TRY(alloc_each((size_t)rows * c.n_actions, p->b_mask, p->b_old));
-        p->bcap = rows;
-    }
+    if ((rc = prepare_learner(p, st)) || (rc = ensure_rows(p, mb)) || (rc = ensure_batch(p, rows))) return rc;
     if (B > p->boot_cap) {
         p->boot_cap = 0;
         CUDA_TRY(alloc_each(B, p->l_boot, p->l_boot_act));
@@ -1132,7 +1142,7 @@ int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, con
 int ramp_policy_train_batch_read(ramp_policy_t* p, ramp_engine_t* eng, int32_t* n_out, int32_t* model_out, int32_t* action_out,
                                  float* logp_out, float* logp_old_out, float* advantage_out, float* value_target_out) {
     if (!p || !eng || !n_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    if (p->b_rows < 1) return set_error(RAMP_ERR_BAD_ARG, "ppo: no train batch (ramp_policy_learn)");
+    if (p->b_rows < 1) return set_error(RAMP_ERR_BAD_ARG, "ppo: no train batch (ramp_policy_learn / ramp_policy_learn_pg)");
     cudaStream_t st = ramp_internal_stream(eng);
     CUDA_TRY(cudaMemcpyAsync(n_out, p->l_n_rows.get(), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -1284,6 +1294,84 @@ int ramp_impala_vtrace_read(ramp_policy_t* p, int32_t* n_out, float* target_logp
     if (log_rho_out) CUDA_TRY(cudaMemcpy(log_rho_out, p->i_log_rho.get(), 4 * n, cudaMemcpyDeviceToHost));
     if (vs_out) CUDA_TRY(cudaMemcpy(vs_out, p->i_vs.get(), 4 * n, cudaMemcpyDeviceToHost));
     if (pg_adv_out) CUDA_TRY(cudaMemcpy(pg_adv_out, p->i_pg.get(), 4 * n, cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
+// pg_torch_policy.py pg_torch_loss: -mean(logp(a) advantages) over the train batch, on host rows
+int ramp_pg_loss_grad(ramp_policy_t* p, const ramp_pg_config_t* cfg, int32_t n, const int32_t* model, const float* graph_features,
+                      const uint8_t* action_mask, const int32_t* action, const float* advantage, float* grad_out, double* stats_out) {
+    if (!p || !model || !graph_features || !action_mask || !action || !advantage) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = check_pg_config(cfg);
+    if (rc != RAMP_OK) return rc;
+    if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "pg: loss of %d rows", n);
+    CUDA_TRY(cudaSetDevice(p->device));
+    if ((rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n)) ||
+        (rc = upload_host_batch(p, n, model, graph_features, action_mask, nullptr, nullptr, action, nullptr, advantage, nullptr)))
+        return rc;
+    GradArgs ga = host_batch_args(p, n);
+    ga.pg = 1; ga.action = p->h_action.get(); ga.adv = p->h_adv.get();
+    if ((rc = launch_states(p, 0, nullptr, 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, 0)) != RAMP_OK) return rc;
+    ramp_pg_stats_kernel<<<1, 1>>>(p->l_row_stats.get(), p->l_row_model.get(), p->h_adv.get(), n, ga.n_rows, p->l_norm_part.get(), p->l_stats.get());
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(0));
+    if (grad_out) CUDA_TRY(cudaMemcpy(grad_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    if (stats_out) CUDA_TRY(cudaMemcpy(stats_out, p->l_stats.get(), sizeof(double) * RAMP_PG_STATS_LEN, cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
+// PG's training step (algorithms/pg: one learn_on_batch per train batch): post_process_advantages (compute_advantages with
+// use_gae False, use_critic False, last_r 0), pg_torch_loss, torch.optim.Adam
+int ramp_policy_learn_pg(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_pg_config_t* cfg, double* stats_out) {
+    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = check_pg_config(cfg);
+    if (rc != RAMP_OK) return rc;
+    ramp_env_buffers_t eb{};
+    if ((rc = ramp_env_buffers(eng, &eb)) != RAMP_OK) return rc;
+    if (n_steps < 1 || n_steps > p->traj_n)
+        return set_error(RAMP_ERR_BAD_ARG, "pg: %d steps asked of a trajectory with %d recorded", n_steps, p->traj_n);
+    if (eb.n_episodes != p->traj_b || eb.n_actions != p->traj_a)
+        return set_error(RAMP_ERR_BAD_ARG, "pg: the trajectory was recorded from another environment");
+    const ramp_policy_config_t& c = p->P.c;
+    CUDA_TRY(cudaSetDevice(p->device));
+    cudaStream_t st = ramp_internal_stream(eng);
+    const int32_t B = eb.n_episodes, rows = n_steps * B;
+    if ((rc = prepare_learner(p, st)) || (rc = ensure_rows(p, rows)) || (rc = ensure_batch(p, rows))) return rc;
+    // 1. the discounted returns (ramp_ppo_gae_kernel without values: lambda 1, V = 0, a 0 bootstrap), the live rows t-major
+    GaeArgs ge{};
+    ge.T = n_steps; ge.B = B; ge.A = c.n_actions; ge.n_models = c.n_models; ge.standardize = 0;
+    ge.gamma = cfg->gamma; ge.lambda = 1.0;
+    ge.t_obs = p->t_obs.get(); ge.t_model = p->t_model.get(); ge.t_mask = p->t_mask.get(); ge.t_action = p->t_action.get();
+    ge.t_logp = p->t_logp.get(); ge.t_value = nullptr; ge.t_reward = p->t_reward.get(); ge.t_done = p->t_done.get();
+    ge.boot = nullptr; ge.adv64 = p->b_adv64.get();
+    ge.obs = p->b_obs.get(); ge.model = p->b_model.get(); ge.mask = p->b_mask.get(); ge.action = p->b_action.get(); ge.logp = p->b_logp.get();
+    ge.adv = p->b_adv.get(); ge.vt = p->b_vt.get(); ge.n_rows = p->l_n_rows.get();
+    ramp_ppo_gae_kernel<<<1, 1024, 0, st>>>(ge);
+    CUDA_TRY(cudaGetLastError());
+    // 2. the loss's gradient over the whole batch at the collection weights (the embeddings the trajectory was collected with);
+    //    the log p(a) the gradient kernel recomputes goes to b_logp_old
+    GradArgs ga{};
+    ga.mb = rows; ga.start = 0; ga.n_rows = p->l_n_rows.get(); ga.shuffle = 0; ga.obs_dyn = p->b_obs.get(); ga.model = p->b_model.get();
+    ga.mask = p->b_mask.get(); ga.action = p->b_action.get(); ga.adv = p->b_adv.get(); ga.pg = 1; ga.logp_old = p->b_logp_old.get();
+    if ((rc = launch_states(p, st, p->l_n_rows.get(), 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, st)) != RAMP_OK) return rc;
+    // 3. one Adam step; with no row in the batch, none (the step count stays)
+    AdamArgs aa{};
+    aa.lr = cfg->lr; aa.beta1 = cfg->adam_beta1; aa.beta2 = cfg->adam_beta2;
+    aa.beta2_f = (float)cfg->adam_beta2; aa.one_m_beta1 = (float)(1.0 - cfg->adam_beta1); aa.one_m_beta2 = (float)(1.0 - cfg->adam_beta2);
+    aa.eps = (float)cfg->adam_eps;
+    aa.max_norm = (float)cfg->grad_clip; aa.n_rows = p->l_n_rows.get(); aa.mb = rows; aa.start = 0; aa.step = p->l_step.get();
+    aa.m = p->l_adam_m.get(); aa.v = p->l_adam_v.get(); aa.grad = p->l_grad.get(); aa.norm_part = p->l_norm_part.get(); aa.w = p->d_w.get();
+    aa.row_stats = nullptr; aa.stats = p->l_stats.get();            // PG's statistics: ramp_pg_stats_kernel, after it
+    aa.parity = p->adam_parity; p->adam_parity ^= 1;
+    ramp_adam_kernel<<<LRN_GRID, 256, 0, st>>>(aa, p->n_weights);
+    // 4. the statistics: the call's one read-back
+    ramp_pg_stats_kernel<<<1, 1, 0, st>>>(p->l_row_stats.get(), p->l_row_model.get(), p->b_adv.get(), rows, p->l_n_rows.get(),
+                                          p->l_norm_part.get(), p->l_stats.get());
+    CUDA_TRY(cudaGetLastError());
+    p->emb_valid = false;
+    p->b_rows = rows;
+    ramp_internal_count_launches(eng, 8);
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, p->l_stats.get(), sizeof(double) * RAMP_PG_STATS_LEN, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     return RAMP_OK;
 }
 

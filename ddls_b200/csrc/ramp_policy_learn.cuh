@@ -1,10 +1,10 @@
 // ramp_policy_learn.cuh -- the GNN policy's gradient and RLlib's PPO learner step on the device (include/ramp_b200.h:
-// ramp_policy_backward, ramp_ppo_loss_grad, ramp_policy_learn) and RLlib's IMPALA learner step (ramp_impala_loss_grad,
-// ramp_policy_learn_impala).  Included by ramp_policy.cu after the forward kernels: the forwards recomputed here repeat theirs
+// ramp_policy_backward, ramp_ppo_loss_grad, ramp_policy_learn), RLlib's IMPALA learner step (ramp_impala_loss_grad,
+// ramp_policy_learn_impala) and RLlib's PG learner step (ramp_pg_loss_grad, ramp_policy_learn_pg).  Included by ramp_policy.cu after the forward kernels: the forwards recomputed here repeat theirs
 // operation for operation, so a recomputed logit is the one ramp_policy_act produced, bit for bit.
 //
-//   ramp_policy_head_grad_kernel    one warp per row: the read-out forward, the upstream gradient (given, RLlib's PPO loss or
-//                                   IMPALA's VTraceLoss), and
+//   ramp_policy_head_grad_kernel    one warp per row: the read-out forward, the upstream gradient (given, RLlib's PPO loss,
+//                                   IMPALA's VTraceLoss or PG's loss), and
 //                                   its backward through the logits / value layers, both hidden layers and the graph module; a
 //                                   per-row record of what the weight gradients need
 //   ramp_policy_head_reduce_kernel  one thread per read-out / graph-module weight: its gradient summed over the rows in row order
@@ -14,11 +14,13 @@
 //                                   out-edge CSR; the job type's weight gradients summed over its items in order
 //   ramp_grad_finish_kernel         the job types' gradients summed in model order; per-CTA partial squared norms
 //   ramp_adam_kernel                clip_grad_norm_ + torch.optim.Adam; the minibatch's loss statistics
-//   ramp_ppo_gae_kernel             GAE per episode, t-major compaction of the live rows, advantage standardisation
+//   ramp_ppo_gae_kernel             GAE per episode, t-major compaction of the live rows, advantage standardisation; without
+//                                   values (PG) the discounted returns
 //   ramp_ppo_learn_stats_kernel     the last pass's mean statistics and RLlib's KL-coefficient update
 //   ramp_impala_batch_kernel        the trajectory cut into fragments of L rows, fragment-major
 //   ramp_vtrace_kernel              one warp per fragment: target log-probabilities (the head kernel's log-softmax), V-trace in f64
 //   ramp_impala_*_stats_kernel      one SGD step's IMPALA statistics; the call's means over its steps
+//   ramp_pg_stats_kernel            PG's statistics
 //
 // Every weight gradient is a sum in a fixed order with an f64 accumulator and no atomics: one call on one batch gives the same bits.
 #pragma once
@@ -169,6 +171,7 @@ struct GradArgs {
     const int32_t* action; const float* old_logits; const float* adv; const float* vt;     // PPO's (old_logits != nullptr)
     float clip, vf_clip, vf_coeff, ent_coeff, kl_coeff;
     int32_t impala;                      // IMPALA's VTraceLoss instead: adv is pg_adv, vt is vs (old_logits unused)
+    int32_t pg;                          // PG's loss instead: adv is the discounted return (old_logits, vt unused)
     float* rec; int32_t* row_model; float* row_stats;               // [mb][..] outputs
     float* logp_old;                     // [batch] log-probability of the action under the old logits, or nullptr
 };
@@ -259,6 +262,21 @@ __global__ void __launch_bounds__(256) ramp_policy_head_grad_kernel(const Policy
         if (lane == 0) {
             float* rs = g.row_stats + (size_t)i * RS_N;
             rs[RS_PI] = -lp_a * pga; rs[RS_VF] = 0.5f * dvv * dvv; rs[RS_ENT] = ent; rs[RS_KL] = 0.f; rs[RS_CLIP] = 0.f;
+        }
+    } else if (g.pg) {
+        // PGTorchPolicy's loss (pg_torch_policy.py): -mean(logp(a) adv) over the batch's rows, no value term.  A masked action
+        // has probability 0 and gets exactly 0.  The row's statistics are log p(a) and H(pi), for reporting only.
+        const float inv_n = 1.0f / (float)min(g.mb, n - g.start);
+        const float pr = ex / denom;
+        const int act = g.action[b];
+        const float lp_a = __shfl_sync(0xffffffffu, lp, act);
+        const float gs = g.adv[b] * inv_n;
+        const float ent = -warp_sum(pr > 0.f ? pr * lp : 0.f);
+        if (lane < A) dl = -gs * ((lane == act ? 1.f : 0.f) - pr);
+        if (lane == 0) {
+            float* rs = g.row_stats + (size_t)i * RS_N;
+            rs[RS_PI] = lp_a; rs[RS_VF] = 0.f; rs[RS_ENT] = ent; rs[RS_KL] = 0.f; rs[RS_CLIP] = 0.f;
+            if (g.logp_old) g.logp_old[b] = lp_a;
         }
     } else if (!g.old_logits) {
         if (lane < A) dl = g.grad_logits[(size_t)b * A + lane];
@@ -757,14 +775,16 @@ struct GaeArgs {
     int32_t T, B, A, n_models, standardize;
     double gamma, lambda;
     const float* t_obs; const int32_t* t_model; const uint8_t* t_mask; const int32_t* t_action; const float* t_logp;
-    const float* t_value; const double* t_reward; const uint8_t* t_done;
-    const float* boot;                   // [B] value of the state after the last step
+    const float* t_value; const double* t_reward; const uint8_t* t_done;   // t_value nullptr: no critic (PG), V = 0
+    const float* boot;                   // [B] value of the state after the last step (unused without t_value)
     double* adv64;                       // [T][B] scratch
     float* obs; int32_t* model; uint8_t* mask; int32_t* action; float* logp; float* adv; float* vt; int32_t* n_rows;   // the batch
 };
 
 // one CTA: GAE (RLlib compute_advantages, use_gae) per episode, one thread per episode scanning backwards; then the rows of
-// episodes that were not finished when the decision was taken and had a queued job, t-major; then (a - mean) / max(1e-4, std)
+// episodes that were not finished when the decision was taken and had a queued job, t-major; then (a - mean) / max(1e-4, std).
+// Without values (t_value nullptr, lambda 1) the scan is r_t + gamma (1 - done_t) next with a 0 bootstrap: RLlib's
+// compute_advantages(use_gae=False, use_critic=False, last_r=0), discount_cumsum's recursion in f64; value_target = advantage.
 __global__ void __launch_bounds__(1024) ramp_ppo_gae_kernel(const GaeArgs a) {
     __shared__ double s_red[32];
     __shared__ int s_scan[32];
@@ -776,7 +796,8 @@ __global__ void __launch_bounds__(1024) ramp_ppo_gae_kernel(const GaeArgs a) {
             const size_t i = (size_t)t * B + b;
             if (!alive(t, b)) { a.adv64[i] = 0.0; continue; }
             const double nonterm = a.t_done[i] ? 0.0 : 1.0;
-            const double V = a.t_value[i], Vn = t == T - 1 ? (double)a.boot[b] : (double)a.t_value[i + B];
+            const double V = a.t_value ? (double)a.t_value[i] : 0.0;
+            const double Vn = !a.t_value ? 0.0 : t == T - 1 ? (double)a.boot[b] : (double)a.t_value[i + B];
             const double delta = a.t_reward[i] + a.gamma * Vn * nonterm - V;
             next = delta + a.gamma * a.lambda * nonterm * next;
             a.adv64[i] = next;
@@ -808,7 +829,7 @@ __global__ void __launch_bounds__(1024) ramp_ppo_gae_kernel(const GaeArgs a) {
                 for (int k = 0; k < a.A; ++k) a.mask[(size_t)pos * a.A + k] = a.t_mask[i * a.A + k];
                 a.model[pos] = a.t_model[i]; a.action[pos] = a.t_action[i]; a.logp[pos] = a.t_logp[i];
                 a.adv[pos] = (float)a.adv64[i];
-                a.vt[pos] = (float)(a.adv64[i] + (double)a.t_value[i]);
+                a.vt[pos] = (float)(a.adv64[i] + (a.t_value ? (double)a.t_value[i] : 0.0));
             }
             base += s_scan[nw - 1];
             __syncthreads();
@@ -940,6 +961,28 @@ __global__ void ramp_impala_learn_stats_kernel(const double* step_stats, int32_t
         out[j] = n_steps ? s / n_steps : 0.0;
     }
     out[RAMP_IMPALA_SGD_STEPS] = n_steps;
+}
+
+// ---- PG (ramp_policy_learn_pg, ramp_pg_loss_grad) ----
+
+// PG's statistics (RAMP_PG_*) over the launch's first min(mb, *n_rows) rows (row i is batch row i: PG does not shuffle):
+// policy_loss = -sum(logp(a) adv) / rows, the rows the head-gradient kernel divides by; the mean entropy over the rows with a
+// decision
+__global__ void ramp_pg_stats_kernel(const float* row_stats, const int32_t* row_model, const float* adv, int32_t mb, const int32_t* n_rows,
+                                     const double* norm_part, double* out) {
+    const int rows = max(0, min(mb, *n_rows));
+    double pi = 0.0, ent = 0.0;
+    int k = 0;
+    for (int i = 0; i < rows; ++i) {
+        if (row_model[i] < 0) continue;
+        const float* s = row_stats + (size_t)i * RS_N;
+        pi += (double)s[RS_PI] * (double)adv[i]; ent += s[RS_ENT];
+        ++k;
+    }
+    out[RAMP_PG_POLICY_LOSS] = rows ? -pi / rows : 0.0;
+    out[RAMP_PG_ENTROPY] = k ? ent / k : 0.0;
+    out[RAMP_PG_GRAD_NORM] = sum_norm_parts(norm_part);
+    out[RAMP_PG_ROWS] = rows;
 }
 
 }  // namespace ramp

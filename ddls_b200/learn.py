@@ -14,6 +14,11 @@ ramp_impala_loss_grad, ramp_policy_learn_impala): V-trace (vtrace_torch.py) over
 VTraceLoss (impala_torch_policy.py), one Adam step per train batch, through the same gradient kernels.  ``IMPALAConfig``'s defaults
 are algo/impala.yaml's; its restatement is tests/impala_reference.py.
 
+``DevicePGLearner(policy, config)`` is RLlib's PG learner step (include/ramp_b200.h: ramp_pg_loss_grad, ramp_policy_learn_pg):
+discounted returns with no bootstrap (postprocessing.compute_advantages, use_critic False) and -mean(logp(a) return)
+(pg_torch_policy.py), one Adam step per segment, through the same gradient kernels.  ``PGConfig``'s defaults are algo/pg.yaml's
+over rllib_config.yaml's base; its restatement is tests/pg_reference.py.
+
 ``DeviceESLearner(policy, config)`` is RLlib's evolution strategies (include/ramp_b200.h: ramp_es_*): the environment's episodes
 are a population of antithetic weight perturbations, one weight set per episode in one batch, then centered ranks, the
 noise-weighted sum and optimizers.Adam on the device.  ``ESConfig``'s defaults are algo/es.yaml's; its restatement is
@@ -260,6 +265,100 @@ class DeviceIMPALALearner:
                                                      reward.ctypes.data, done.ctypes.data, grad.ctypes.data, out.ctypes.data,
                                                      *[a.ctypes.data for a in vt.values()]))
         return {k: float(v) for k, v in zip(IMPALA_STATS, out)}, grad, {k: v.reshape(n, L) for k, v in vt.items()}
+
+    def adam_state(self):
+        """torch.optim.Adam's state of the flat weight vector (the policy's, shared with DevicePPOLearner)"""
+        return DevicePPOLearner.adam_state(self)
+
+    def reset(self):
+        """zero Adam's moments and step count"""
+        _engine._check(self._L.ramp_policy_learner_reset(self.policy._h))
+
+
+PG_STATS = ('policy_loss', 'entropy', 'grad_gnorm', 'rows')
+
+
+@dataclasses.dataclass
+class PGConfig:
+    """rllib_config.yaml's gamma and lr (algo/pg.yaml sets neither); torch.optim.Adam's defaults, since RLlib passes it only the lr;
+    PG sets no grad_clip (<= 0: no clipping)."""
+    gamma: float = 0.99
+    lr: float = 1e-4
+    grad_clip: float = 0.0
+    adam_beta1: float = 0.9
+    adam_beta2: float = 0.999
+    adam_eps: float = 1e-8
+
+
+class _CPGConfig(C.Structure):
+    _fields_ = [(n, C.c_double) for n in ('gamma', 'grad_clip', 'lr', 'adam_beta1', 'adam_beta2', 'adam_eps')]
+
+
+def c_pg_config(cfg: PGConfig) -> _CPGConfig:
+    return _CPGConfig(*(float(getattr(cfg, n)) for n, _ in _CPGConfig._fields_))
+
+
+def _bind_pg(L):
+    if getattr(L, '_pg_bound', False):
+        return
+    _bind(L)
+    L.ramp_pg_loss_grad.restype = C.c_int
+    L.ramp_pg_loss_grad.argtypes = [C.c_void_p, C.POINTER(_CPGConfig), C.c_int32] + [C.c_void_p] * 7
+    L.ramp_policy_learn_pg.restype = C.c_int
+    L.ramp_policy_learn_pg.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CPGConfig), C.c_void_p]
+    L._pg_bound = True
+
+
+class DevicePGLearner:
+    """RLlib's PG learner step (discounted returns, pg_torch_loss, Adam) on the segment the policy's last collect() recorded, on
+    the device.  Adam's moments and step count are the policy's, shared with DevicePPOLearner and DeviceIMPALALearner."""
+
+    def __init__(self, policy, config: PGConfig = None):
+        """policy: a DeviceGNNPolicy, whose weights the learner updates in place"""
+        self.policy = policy
+        self.config = dataclasses.replace(config) if config is not None else PGConfig()
+        self._L = policy._L
+        _bind_pg(self._L)
+
+    def collect_and_learn(self, env, horizon: int, seed: int = 0):
+        """policy.collect(env, horizon) then learn(); also returns the wall time of each (seconds) and the segment's trajectory."""
+        t0 = time.perf_counter()
+        traj = self.policy.collect(env, horizon, sample=True, seed=seed)
+        t1 = time.perf_counter()
+        stats = self.learn(env, horizon)
+        stats['collect_s'], stats['learn_s'] = t1 - t0, time.perf_counter() - t1
+        return stats, traj
+
+    def learn(self, env, horizon: int) -> Dict[str, float]:
+        """One PG learner step on the first ``horizon`` steps of the segment the policy's last collect(env, ...) recorded: one train
+        batch of every decision of the segment, one Adam step.  Each episode's advantage is its discounted return; a segment that
+        ends before its episode does is not bootstrapped (PG's last_r is 0).  There is no train_batch_size: under RLlib's
+        batch_mode complete_episodes a train batch is whole episodes, so the caller sizes env.B and the horizon so that the
+        segment holds the env-steps it wants per update (pg's train_batch_size is 200) and its episodes end inside it.  Returns
+        PG_STATS; a segment with no decision makes no update and leaves Adam's step count as it was."""
+        out = np.zeros(len(PG_STATS), dtype=np.float64)
+        _engine._check(self._L.ramp_policy_learn_pg(self.policy._h, env.eng._h, int(horizon), C.byref(c_pg_config(self.config)),
+                                                    out.ctypes.data))
+        return {k: float(v) for k, v in zip(PG_STATS, out)}
+
+    def train_batch(self, env) -> Dict[str, np.ndarray]:
+        """the last learn()'s train batch: per live row, t-major, the job type, action, collected log-probability, the one the
+        gradient kernel recomputed at the collection weights (logp_old) and the discounted return (advantage, value_target)"""
+        return DevicePPOLearner.train_batch(self, env)
+
+    def loss_and_grad(self, batch: Dict[str, np.ndarray]):
+        """pg_torch_loss's statistics (PG_STATS) and gradient (blob order) on host rows, with no update: model [n],
+        graph_features [n, in_features_graph], action_mask [n, |A|], action [n], advantage [n]."""
+        pol = self.policy
+        model, gf, mask = pol._host_inputs(batch['model'], batch['graph_features'], batch['action_mask'])
+        n = len(model)
+        act = np.ascontiguousarray(batch['action'], dtype=np.int32).reshape(n)
+        adv = np.ascontiguousarray(batch['advantage'], dtype=np.float32).reshape(n)
+        grad = np.zeros(pol._L.ramp_policy_weight_count(C.byref(pol._cfg)), dtype=np.float32)
+        out = np.zeros(len(PG_STATS), dtype=np.float64)
+        _engine._check(self._L.ramp_pg_loss_grad(pol._h, C.byref(c_pg_config(self.config)), n, model.ctypes.data, gf.ctypes.data,
+                                                 mask.ctypes.data, act.ctypes.data, adv.ctypes.data, grad.ctypes.data, out.ctypes.data))
+        return {k: float(v) for k, v in zip(PG_STATS, out)}, grad
 
     def adam_state(self):
         """torch.optim.Adam's state of the flat weight vector (the policy's, shared with DevicePPOLearner)"""

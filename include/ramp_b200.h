@@ -621,7 +621,8 @@ int ramp_ppo_loss_grad(ramp_policy_t* p, const ramp_ppo_config_t* cfg, int32_t n
 int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_ppo_config_t* cfg, double* stats_out);
 /* HOST copies of the last ramp_policy_learn's train batch (any array may be NULL): n_out rows; per row the job type, the action,
  * the collected log-probability, the one recomputed from the collection weights' logits (written by the first pass), the
- * advantage (standardised when asked) and the value target */
+ * advantage (standardised when asked) and the value target.  After a ramp_policy_learn_pg, PG's batch: advantage and value
+ * target are the discounted return. */
 int ramp_policy_train_batch_read(ramp_policy_t* p, ramp_engine_t* eng, int32_t* n_out, int32_t* model_out, int32_t* action_out,
                                  float* logp_out, float* logp_old_out, float* advantage_out, float* value_target_out);
 /* HOST copies of Adam's state (any may be NULL): exp_avg and exp_avg_sq [ramp_policy_weight_count], and the step count --
@@ -687,6 +688,42 @@ int ramp_policy_learn_impala(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_ste
  * pg_adv.  Any array may be NULL. */
 int ramp_impala_vtrace_read(ramp_policy_t* p, int32_t* n_out, float* target_logp_out, float* log_rho_out, float* vs_out,
                             float* pg_adv_out);
+
+/* ---- RLlib's PG (REINFORCE) learner step on the device (ray 3.0.0.dev0, as the reference pins it): ray/rllib/algorithms/pg/
+ * pg_torch_policy.py (pg_torch_loss; postprocess_trajectory -> utils.post_process_advantages) and
+ * ray/rllib/evaluation/postprocessing.py (compute_advantages with use_gae False, use_critic False, last_r 0; discount_cumsum).
+ * It reuses PPO's gradient kernels and Adam, and Adam's moments and step count are the same policy-owned state
+ * (ramp_policy_learner_state / _reset serve every gradient learner). */
+typedef struct {
+    double gamma;                         /* discount_cumsum's gamma (rllib_config.yaml: 0.99)                                     */
+    double grad_clip;                     /* global-norm clip (clip_grad_norm_); <= 0: none (PG sets none, the default)            */
+    double lr, adam_beta1, adam_beta2, adam_eps;   /* torch.optim.Adam; RLlib passes only lr (rllib_config.yaml: 1e-4)             */
+} ramp_pg_config_t;
+
+/* statistics (stats_out of ramp_policy_learn_pg and ramp_pg_loss_grad) */
+enum { RAMP_PG_POLICY_LOSS = 0,           /* -sum(logp(a) advantage) / rows: pg_torch_loss's policy_loss                           */
+       RAMP_PG_ENTROPY,                   /* mean H(pi) over the rows with a decision (reporting only: not in the loss)            */
+       RAMP_PG_GRAD_NORM,                 /* global norm of the gradient before clipping                                          */
+       RAMP_PG_ROWS,                      /* rows the loss is averaged over                                                       */
+       RAMP_PG_STATS_LEN };
+
+/* pg_torch_loss on n HOST rows, and its gradient, with no update: loss = -mean(logp(a) advantage) over the n rows, log p(a) the
+ * log-softmax of the masked logits at the current weights; no value, entropy or KL term.  A row whose model is outside
+ * [0, n_models) adds nothing but counts in the mean.  grad_out [ramp_policy_weight_count] and stats_out [RAMP_PG_STATS_LEN] may
+ * be NULL; cfg's gamma is not used. */
+int ramp_pg_loss_grad(ramp_policy_t* p, const ramp_pg_config_t* cfg, int32_t n, const int32_t* model, const float* graph_features,
+                      const uint8_t* action_mask, const int32_t* action, const float* advantage, float* grad_out, double* stats_out);
+/* One PG learner step on the first n_steps slots of the trajectory of the last ramp_policy_trajectory_begin (the same checks as
+ * ramp_policy_learn), on the engine's stream, nothing read back but stats_out:
+ *   1. per episode, the discounted return adv_t = r_t + gamma (1 - done_t) adv_{t+1} (f64, stored as fp32), with adv = 0 after
+ *      the segment's last slot even when the episode goes on: PG does not bootstrap.  The rows of episodes not finished when the
+ *      decision was taken and with a queued job, t-major, form the train batch (ramp_ppo_gae_kernel's batch); no standardisation.
+ *   2. one Adam step over the whole batch: the loss of ramp_pg_loss_grad at the current (collection) weights, its gradient,
+ *      clip_grad_norm_ to grad_clip when > 0, torch.optim.Adam.  A batch with no row is no update: the step count stays.
+ *   3. stats_out [RAMP_PG_STATS_LEN].
+ * The embeddings become stale (the next forward re-embeds).  ramp_policy_train_batch_read then returns this batch: logp_old is the
+ * log p(a) the gradient kernel recomputed at the collection weights, advantage and value_target are both the discounted return. */
+int ramp_policy_learn_pg(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_pg_config_t* cfg, double* stats_out);
 
 /* ---- RLlib's evolution strategies (ES) training step on the device (ray/rllib/algorithms/es: es.py training_step,
  * utils.py compute_centered_ranks / batched_weighted_sum, optimizers.py Adam).  The B episodes of a device environment are one
