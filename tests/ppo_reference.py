@@ -2,7 +2,8 @@
 
   policy64       GNNPolicy's forward (tests/gnn_reference.py), vectorised (MeanPool's mailbox mean through index_add), as a function of
                  a state_dict of float64 tensors, so torch.autograd gives every weight's gradient on graphs of 20,000 nodes; pinned to
-                 the module restatement GNNPolicy run in float64 in tests/test_ppo_model.py
+                 the module restatement GNNPolicy run in float64 in tests/test_ppo_model.py; optionally with named ReLU branches
+                 forced and every activation site's inputs recorded (tests/tie_reference.py)
   ppo_loss64     PPOTorchPolicy.loss (ray/rllib/algorithms/ppo/ppo_torch_policy.py) with torch.distributions.Categorical
   gae64          RLlib compute_advantages (use_gae) per episode of a recorded segment, and the train batch's rows, t-major
   standardize64  RLlib's standardize_fields: (a - mean) / max(1e-4, std)
@@ -29,12 +30,26 @@ def _ln(x, w, b):
     return (x - mean) / torch.sqrt(var + 1e-5) * w + b
 
 
-def _act(x, kind):
+def _act(x, kind, forced=None):
+    """the activation; forced: {(item, unit): on} -- those units of the [items, units] pre-activation x take the positive branch
+    (on) or the other one whatever x's sign, so that their output moves by |x| and their derivative is the forced branch's"""
+    if forced:
+        if kind == 'tanh':
+            raise ValueError('tanh has no branches to force')
+        on = x.detach() > 0
+        for (i, u), b in forced.items():
+            on[i, u] = bool(b)
+        return x * torch.where(on, 1.0, 0.0 if kind == 'relu' else 0.01).to(x.dtype)
     if kind == 'relu':
         return torch.relu(x)
     if kind == 'leaky_relu':
         return F.leaky_relu(x, 0.01)
     return torch.tanh(x)
+
+
+def _sites(forced, module, model, rnd):
+    """forced branches {(module, model, round, item, unit): on} of one module instance -> {(item, unit): on}"""
+    return {(s[3], s[4]): b for s, b in (forced or {}).items() if s[:3] == (module, model, rnd)}
 
 
 def params64(sd, requires_grad=True, dtype=torch.float64):
@@ -47,7 +62,11 @@ def _dtype(p):
     return next(iter(p.values())).dtype
 
 
-def embed64(p, c, nf, ef, src, dst):
+def embed64(p, c, nf, ef, src, dst, model=0, forced=None, record=None):
+    """GNNPolicy.embed of one job type (`model`).  Its activation sites are named (module, model, round, item, unit), module
+    'node' (item: node), 'edge' (edge), 'own' (the reduce module on a node's own state; item: node) or 'msg' (on an edge's
+    message; item: edge).  forced: {site: on}, branches taken whatever the pre-activation's sign (_act); record(module, model,
+    round, pre-activation, Linear input, weight, bias), when given, sees every activation site's inputs."""
     z = torch.as_tensor(np.asarray(nf), dtype=_dtype(p))
     ef = torch.as_tensor(np.asarray(ef), dtype=_dtype(p)).reshape(len(src), c['in_features_edge'])
     src, dst = torch.as_tensor(np.asarray(src, dtype=np.int64)), torch.as_tensor(np.asarray(dst, dtype=np.int64))
@@ -56,18 +75,24 @@ def embed64(p, c, nf, ef, src, dst):
     for r in range(c['num_rounds']):
         pre = f'gnn_module.layers.{r}.'
 
-        def mod(name, x):
+        def mod(name, site, x):
             x = _ln(x, p[pre + name + '.0.weight'], p[pre + name + '.0.bias'])
-            return _act(x @ p[pre + name + '.1.weight'].T + p[pre + name + '.1.bias'], a)
-        hn, he = mod('node_module', z), mod('edge_module', ef)
-        local = mod('reduce_module', torch.cat([hn, torch.zeros_like(hn)], 1))
-        msgs = mod('reduce_module', torch.cat([hn[src], he], 1))
+            W, b = p[pre + name + '.1.weight'], p[pre + name + '.1.bias']
+            y = x @ W.T + b
+            if record is not None:
+                record(site, model, r, y.detach(), x.detach(), W.detach(), b.detach())
+            return _act(y, a, _sites(forced, site, model, r))
+        hn, he = mod('node_module', 'node', z), mod('edge_module', 'edge', ef)
+        local = mod('reduce_module', 'own', torch.cat([hn, torch.zeros_like(hn)], 1))
+        msgs = mod('reduce_module', 'msg', torch.cat([hn[src], he], 1))
         total = local.index_add(0, dst, msgs)
         z = torch.where(deg > 0, total / (deg + 1.0), torch.zeros_like(total))
     return z.mean(0)
 
 
-def head64(p, c, emb_rows, graph_features, action_mask):
+def head64(p, c, emb_rows, graph_features, action_mask, forced=None, record=None):
+    """the read-out of the rows.  Its activation sites are ('hidden' | 'value', -1, -1, row, unit): the policy's and the value
+    branch's hidden units; forced and record as in embed64"""
     mask = torch.as_tensor(np.asarray(action_mask), dtype=_dtype(p))
     x = torch.cat([torch.as_tensor(np.asarray(graph_features), dtype=_dtype(p)), mask], 1)
     g = _ln(x, p['graph_module.0.weight'], p['graph_module.0.bias']) @ p['graph_module.1.weight'].T + p['graph_module.1.bias']
@@ -76,20 +101,28 @@ def head64(p, c, emb_rows, graph_features, action_mask):
     def fc(name, v):
         return v @ p[f'logit_module.{name}._model.0.weight'].T + p[f'logit_module.{name}._model.0.bias']
     fa = c['fcnet_activation']
-    logits = fc('_logits', _act(fc('_hidden_layers.0', final), fa))
-    value = fc('_value_branch', _act(fc('_value_branch_separate.0', final), fa))[:, 0]
+
+    def hidden(name, site):
+        y = fc(name, final)
+        if record is not None:
+            W, b = (p[f'logit_module.{name}._model.0.{k}'].detach() for k in ('weight', 'bias'))
+            record(site, -1, -1, y.detach(), final.detach(), W, b)
+        return _act(y, fa, _sites(forced, site, -1, -1))
+    logits = fc('_logits', hidden('_hidden_layers.0', 'hidden'))
+    value = fc('_value_branch', hidden('_value_branch_separate.0', 'value'))[:, 0]
     if c['apply_action_mask']:
         logits = logits + torch.clamp(torch.log(mask), min=F32_MIN)
     return logits, value
 
 
-def policy64(p, c, graphs, model, graph_features, action_mask):
-    """logits, value of the rows (every model must be in range); graphs: objects with nf, ef, src, dst"""
+def policy64(p, c, graphs, model, graph_features, action_mask, forced=None, record=None):
+    """logits, value of the rows (every model must be in range); graphs: objects with nf, ef, src, dst.  forced: {site: on},
+    branches taken whatever the pre-activation's sign; record: sees every activation site's inputs (embed64, head64)"""
     model = np.asarray(model)
     used = sorted(set(model.tolist()))
-    emb = {m: embed64(p, c, graphs[m].nf, graphs[m].ef, graphs[m].src, graphs[m].dst) for m in used}
+    emb = {m: embed64(p, c, graphs[m].nf, graphs[m].ef, graphs[m].src, graphs[m].dst, m, forced, record) for m in used}
     rows = torch.stack([emb[m] for m in model.tolist()])
-    return head64(p, c, rows, graph_features, action_mask)
+    return head64(p, c, rows, graph_features, action_mask, forced, record)
 
 
 def _as(x, dt):
