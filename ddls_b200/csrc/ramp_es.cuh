@@ -162,8 +162,9 @@ __global__ void __launch_bounds__(256) ramp_es_head_kernel(const PolicyDev P, co
     __shared__ float s_warp[8][2 * POL_MAX_DIM];
     const ramp_policy_config_t& c = P.c;
     const int gin = c.in_features_graph + c.n_actions, og = c.out_features_graph, on = c.out_features_node, fin = on + og;
-    const int H = c.fcnet_hidden, A = c.n_actions, hpl = H / 32;
+    const int H = c.fcnet_hidden, A = c.n_actions;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpc = blockDim.x >> 5;
+    const int hpl = (H - lane + 31) / 32;                               // this lane's hidden units lane + 32 i < H
     float* xb = s_warp[warp];
     float* fb = xb + POL_MAX_DIM;
     for (int b = blockIdx.x * wpc + warp; b < a.n; b += gridDim.x * wpc) {
@@ -198,8 +199,8 @@ __global__ void __launch_bounds__(256) ramp_es_head_kernel(const PolicyDev P, co
         float h[POL_MAX_HPL];
 #pragma unroll
         for (int i = 0; i < POL_MAX_HPL; ++i) {
+            const int j = lane + 32 * i;
             if (i < hpl) {
-                const int j = lane + 32 * i;
                 float p = w[P.hb + j];
                 const float* row = w + P.hW + (size_t)j * fin;           // blob is [H][fin]
                 for (int k = 0; k < fin; ++k) p += row[k] * fb[k];

@@ -11,7 +11,8 @@
 //                           this runs once per weight set, not per decision.
 //   ramp_policy_head_kernel persistent CTAs, one warp per episode: graph module LN -> Linear over [graph features | action mask]
 //                           (gnn_policy.py:96-109, 271), concat with the model's node-mean embedding, the RLlib fully-connected
-//                           read-out (one hidden layer, logits; separate value branch), + max(log(mask), FLT_MIN) on the logits
+//                           read-out (one hidden layer, logits; a separate value branch, or under vf_share_layers the value
+//                           layer on the policy's hidden layer), + max(log(mask), FLT_MIN) on the logits
 //                           (gnn_policy.py:283-290), then greedy / categorical action selection written straight into the
 //                           environment's action buffer.  All read-out weights are staged once per CTA in shared memory, laid
 //                           out so that lanes read consecutive words.
@@ -183,10 +184,11 @@ struct HeadArgs {
 };
 
 __host__ __device__ inline size_t head_smem_floats(const ramp_policy_config_t& c, int warps) {
-    const int gin = c.in_features_graph + c.n_actions, fin = c.out_features_node + c.out_features_graph, H = c.fcnet_hidden, A = c.n_actions;
+    const int gin = c.in_features_graph + c.n_actions, fin = c.out_features_node + c.out_features_graph, A = c.n_actions;
+    const size_t layers = c.vf_share_layers ? 1 : 2, Hp = 32 * (size_t)((c.fcnet_hidden + 31) / 32);
     return (size_t)2 * gin + (size_t)c.out_features_graph * gin + c.out_features_graph      // graph module
-           + (size_t)2 * fin * H + 2 * (size_t)H                                           // hidden layers (policy, value), transposed
-           + (size_t)A * H + A + H + 1                                                      // logits, value
+           + layers * (fin * Hp + Hp)                                                      // hidden layers (policy, value), transposed
+           + (size_t)A * Hp + A + Hp + 1                                                    // logits, value
            + (size_t)warps * 2 * POL_MAX_DIM;                                               // per-warp staging
 }
 
@@ -197,17 +199,21 @@ __device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
     return x ^ (x >> 31);
 }
 
-__global__ void __launch_bounds__(256) ramp_policy_head_kernel(const PolicyDev P, const HeadArgs a) {
+// at most 80 registers (three CTAs per SM), what the kernel used before its read-out was padded to Hp: left alone, ptxas takes 113
+__global__ void __launch_bounds__(256, 3) ramp_policy_head_kernel(const PolicyDev P, const HeadArgs a) {
     extern __shared__ float sm[];
     const ramp_policy_config_t& c = P.c;
     const int gin = c.in_features_graph + c.n_actions, og = c.out_features_graph, on = c.out_features_node, fin = on + og;
-    const int H = c.fcnet_hidden, A = c.n_actions, hpl = H / 32;
+    // the hidden units padded to Hp, a multiple of 32, with zero weights and biases: a padding unit is 0 and adds exactly 0 to the
+    // split-K sums below (Hp = H when 32 | H)
+    const int H = c.fcnet_hidden, Hp = 32 * ((H + 31) / 32), A = c.n_actions, hpl = Hp / 32;
+    const bool share = c.vf_share_layers;                             // no value hidden layer: the value reads h
     float* s_gln_w = sm;                 float* s_gln_b = s_gln_w + gin;
     float* s_gW = s_gln_b + gin;         float* s_gb = s_gW + (size_t)og * gin;
-    float* s_hWt = s_gb + og;            float* s_hb = s_hWt + (size_t)fin * H;      // [fin][H]: lanes read consecutive hidden units
-    float* s_vhWt = s_hb + H;            float* s_vhb = s_vhWt + (size_t)fin * H;
-    float* s_lW = s_vhb + H;             float* s_lb = s_lW + (size_t)A * H;         // [A][H]
-    float* s_vW = s_lb + A;              float* s_vb = s_vW + H;
+    float* s_hWt = s_gb + og;            float* s_hb = s_hWt + (size_t)fin * Hp;     // [fin][Hp]: lanes read consecutive hidden units
+    float* s_vhWt = s_hb + Hp;           float* s_vhb = s_vhWt + (share ? 0 : (size_t)fin * Hp);
+    float* s_lW = s_vhb + (share ? 0 : Hp); float* s_lb = s_lW + (size_t)A * Hp;     // [A][Hp]
+    float* s_vW = s_lb + A;              float* s_vb = s_vW + Hp;
     float* s_warp = s_vb + 1;
     const float* w = P.w;
     for (int i = threadIdx.x; i < gin; i += blockDim.x) { s_gln_w[i] = w[P.gln_w + i]; s_gln_b[i] = w[P.gln_b + i]; }
@@ -215,13 +221,23 @@ __global__ void __launch_bounds__(256) ramp_policy_head_kernel(const PolicyDev P
     for (int i = threadIdx.x; i < og; i += blockDim.x) s_gb[i] = w[P.gb + i];
     for (int i = threadIdx.x; i < fin * H; i += blockDim.x) {
         const int j = i / fin, k = i - j * fin;                       // blob is [H][fin]
-        s_hWt[(size_t)k * H + j] = w[P.hW + i];
-        s_vhWt[(size_t)k * H + j] = w[P.vhW + i];
+        s_hWt[(size_t)k * Hp + j] = w[P.hW + i];
+        if (!share) s_vhWt[(size_t)k * Hp + j] = w[P.vhW + i];
     }
-    for (int i = threadIdx.x; i < H; i += blockDim.x) { s_hb[i] = w[P.hb + i]; s_vhb[i] = w[P.vhb + i]; s_vW[i] = w[P.vW + i]; }
-    for (int i = threadIdx.x; i < A * H; i += blockDim.x) s_lW[i] = w[P.lW + i];
+    for (int i = threadIdx.x; i < H; i += blockDim.x) { s_hb[i] = w[P.hb + i]; if (!share) s_vhb[i] = w[P.vhb + i]; s_vW[i] = w[P.vW + i]; }
+    for (int i = threadIdx.x; i < A * H; i += blockDim.x) { const int o = i / H; s_lW[(size_t)o * Hp + (i - o * H)] = w[P.lW + i]; }
     for (int i = threadIdx.x; i < A; i += blockDim.x) s_lb[i] = w[P.lb + i];
     if (threadIdx.x == 0) s_vb[0] = w[P.vb];
+    if (Hp != H) {
+        const int pad = Hp - H;
+        for (int i = threadIdx.x; i < fin * pad; i += blockDim.x) {
+            const int k = i / pad, j = H + (i - k * pad);
+            s_hWt[(size_t)k * Hp + j] = 0.f;
+            if (!share) s_vhWt[(size_t)k * Hp + j] = 0.f;
+        }
+        for (int i = threadIdx.x; i < pad; i += blockDim.x) { s_hb[H + i] = 0.f; if (!share) s_vhb[H + i] = 0.f; s_vW[H + i] = 0.f; }
+        for (int i = threadIdx.x; i < A * pad; i += blockDim.x) { const int o = i / pad; s_lW[(size_t)o * Hp + H + (i - o * pad)] = 0.f; }
+    }
     __syncthreads();
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpc = blockDim.x >> 5;
@@ -257,20 +273,32 @@ __global__ void __launch_bounds__(256) ramp_policy_head_kernel(const PolicyDev P
         __syncwarp();
         // ---- read-out: hidden layer of the policy and of the value branch, each lane owns units lane + 32 i ----
         float h[POL_MAX_HPL], hv[POL_MAX_HPL];
+        if (share) {
 #pragma unroll
-        for (int i = 0; i < POL_MAX_HPL; ++i) {
-            if (i < hpl) {
-                const int j = lane + 32 * i;
-                float p = s_hb[j], q = s_vhb[j];
-                for (int k = 0; k < fin; ++k) { const float f = fb[k]; p += s_hWt[(size_t)k * H + j] * f; q += s_vhWt[(size_t)k * H + j] * f; }
-                h[i] = act_fn(p, c.fcnet_activation); hv[i] = act_fn(q, c.fcnet_activation);
+            for (int i = 0; i < POL_MAX_HPL; ++i) {
+                if (i < hpl) {
+                    const int j = lane + 32 * i;
+                    float p = s_hb[j];
+                    for (int k = 0; k < fin; ++k) p += s_hWt[(size_t)k * Hp + j] * fb[k];
+                    h[i] = hv[i] = act_fn(p, c.fcnet_activation);
+                }
+            }
+        } else {
+#pragma unroll
+            for (int i = 0; i < POL_MAX_HPL; ++i) {
+                if (i < hpl) {
+                    const int j = lane + 32 * i;
+                    float p = s_hb[j], q = s_vhb[j];
+                    for (int k = 0; k < fin; ++k) { const float f = fb[k]; p += s_hWt[(size_t)k * Hp + j] * f; q += s_vhWt[(size_t)k * Hp + j] * f; }
+                    h[i] = act_fn(p, c.fcnet_activation); hv[i] = act_fn(q, c.fcnet_activation);
+                }
             }
         }
         float my_logit = -FLT_MAX;
         for (int o = 0; o < A; ++o) {
             float p = 0.f;
 #pragma unroll
-            for (int i = 0; i < POL_MAX_HPL; ++i) if (i < hpl) p += h[i] * s_lW[(size_t)o * H + lane + 32 * i];
+            for (int i = 0; i < POL_MAX_HPL; ++i) if (i < hpl) p += h[i] * s_lW[(size_t)o * Hp + lane + 32 * i];
             p = warp_sum(p) + s_lb[o];
             if (c.apply_action_mask && !a.mask[(size_t)b * A + o]) p += -FLT_MAX;   // + max(log 0, finfo.min) (gnn_policy.py:285-290)
             if (lane == o) my_logit = p;
@@ -372,7 +400,7 @@ struct ramp_policy {
     // learner (ramp_policy_backward / ramp_ppo_loss_grad / ramp_policy_learn): gradient, Adam's moments and step count, per job type
     // gradients, norm partials; per-row scratch for `lcap` rows, the head segments for `seg_n` rows
     bool learner_ready = false, gmodels_ready = false;
-    int32_t adam_parity = 0, lcap = 0, seg_n = 0;
+    int32_t adam_parity = 0, lcap = 0, seg_n = 0, seg_count = 0;
     int64_t seg_total = 0;
     DeviceArray<float> l_grad, l_adam_m, l_adam_v, l_gpart, l_rec, l_row_stats;
     DeviceArray<int32_t> l_n_rows, l_step, l_row_model;
@@ -413,7 +441,8 @@ int64_t layout(const ramp_policy_config_t& c, PolicyDev* P) {
     const int gin = c.in_features_graph + c.n_actions, fin = c.out_features_node + c.out_features_graph, H = c.fcnet_hidden;
     const int64_t gln_w = take(gin), gln_b = take(gin), gW = take((int64_t)c.out_features_graph * gin), gb = take(c.out_features_graph);
     const int64_t hW = take((int64_t)H * fin), hb = take(H), lW = take((int64_t)c.n_actions * H), lb = take(c.n_actions);
-    const int64_t vhW = take((int64_t)H * fin), vhb = take(H), vW = take(H), vb = take(1);
+    const int64_t vhW = c.vf_share_layers ? -1 : take((int64_t)H * fin), vhb = c.vf_share_layers ? -1 : take(H);   // no value hidden layer
+    const int64_t vW = take(H), vb = take(1);
     if (P) { P->gln_w = gln_w; P->gln_b = gln_b; P->gW = gW; P->gb = gb; P->hW = hW; P->hb = hb; P->lW = lW; P->lb = lb;
              P->vhW = vhW; P->vhb = vhb; P->vW = vW; P->vb = vb; }
     return o;
@@ -428,8 +457,11 @@ int check_config(const ramp_policy_config_t& c) {
     if (!in(c.out_features_graph, 1, 32) || !in(c.n_actions, 1, 32) || c.in_features_graph + c.n_actions > POL_MAX_DIM)
         return set_error(RAMP_ERR_BAD_ARG, "policy: out_features_graph and n_actions must be <= 32");
     if (c.num_rounds < 2 || c.num_rounds > POL_MAX_ROUNDS) return set_error(RAMP_ERR_BAD_ARG, "policy: num_rounds must be in [2, %d] (gnn.py:40-41)", POL_MAX_ROUNDS);
-    if (c.fcnet_hidden < 32 || c.fcnet_hidden % 32 || c.fcnet_hidden > 32 * POL_MAX_HPL)
-        return set_error(RAMP_ERR_BAD_ARG, "policy: fcnet_hidden must be a multiple of 32 in [32, %d]", 32 * POL_MAX_HPL);
+    // a multiple of 32, or action_space.n: the width the algorithm configs set (algo/{ppo,impala,pg,es}.yaml), at most 32
+    const bool h32 = c.fcnet_hidden >= 32 && c.fcnet_hidden % 32 == 0 && c.fcnet_hidden <= 32 * POL_MAX_HPL;
+    if (!h32 && c.fcnet_hidden != c.n_actions)
+        return set_error(RAMP_ERR_BAD_ARG, "policy: fcnet_hidden must be a multiple of 32 in [32, %d] or n_actions (%d)", 32 * POL_MAX_HPL, c.n_actions);
+    if (!in(c.vf_share_layers, 0, 1)) return set_error(RAMP_ERR_BAD_ARG, "policy: vf_share_layers must be 0 or 1");
     if (!in(c.aggregator_activation, 0, 1) || !(c.fcnet_activation == 0 || c.fcnet_activation == 2))
         return set_error(RAMP_ERR_BAD_ARG, "policy: unsupported activation");
     if (c.n_models < 1) return set_error(RAMP_ERR_BAD_ARG, "policy: n_models must be >= 1");
@@ -579,9 +611,9 @@ int ensure_rows(ramp_policy* p, int32_t n) {
     }
     if (n != p->seg_n) {
         Seg s[HEAD_SEGS];
-        head_segs(p->P, p->l_rec.get(), n, s);
+        p->seg_count = head_segs(p->P, p->l_rec.get(), n, s);
         p->seg_total = 0;
-        for (const Seg& x : s) p->seg_total += seg_size(x);
+        for (int k = 0; k < p->seg_count; ++k) p->seg_total += seg_size(s[k]);
         CUDA_TRY(cudaMemcpy(p->l_segs.get(), s, sizeof(s), cudaMemcpyHostToDevice));
         p->seg_n = n;
     }
@@ -613,7 +645,7 @@ int launch_grad(ramp_policy* p, GradArgs ga, cudaStream_t st) {
     ramp_policy_head_grad_kernel<<<(ga.mb + LRN_WARPS - 1) / LRN_WARPS, LRN_WARPS * 32, 0, st>>>(p->P, ga);
     int64_t grid = (p->seg_total + 255) / 256;
     if (grid > 4 * p->sm_count) grid = 4 * p->sm_count;
-    ramp_policy_head_reduce_kernel<<<(unsigned)grid, 256, 0, st>>>(p->P, p->l_segs.get(), HEAD_SEGS, p->seg_total, p->l_grad.get());
+    ramp_policy_head_reduce_kernel<<<(unsigned)grid, 256, 0, st>>>(p->P, p->l_segs.get(), p->seg_count, p->seg_total, p->l_grad.get());
     EmbGradArgs eg{};
     eg.rec = p->l_rec.get(); eg.row_model = p->l_row_model.get(); eg.rows = ga.mb; eg.gpart = p->l_gpart.get(); eg.n_gnn = gnn_weight_count(p);
     ramp_gnn_embed_grad_kernel<EMB_BACKWARD><<<p->P.c.n_models, 256, 0, st>>>(p->P, p->d_models.get(), p->d_gmodels.get(), eg);

@@ -44,8 +44,9 @@ __host__ __device__ inline HeadRec head_rec(const ramp_policy_config_t& c) {
     r.dpg = o; o += og;                  // d graph-module Linear output
     r.fb = o; o += fin;                  // read-out input
     r.de = o; o += on;                   // d emb[model]
-    r.h = o; o += H; r.hv = o; o += H;   // hidden activations (policy, value)
-    r.dh = o; o += H; r.dhv = o; o += H; // d hidden pre-activations
+    const bool sep = !c.vf_share_layers; // under vf_share_layers the value reads h: no hv / dhv (-1)
+    r.h = o; o += H; r.hv = sep ? o : -1; o += sep ? H : 0;      // hidden activations (policy, value)
+    r.dh = o; o += H; r.dhv = sep ? o : -1; o += sep ? H : 0;    // d hidden pre-activations
     r.dl = o; o += A; r.dv = o; o += 1;  // d logits, d value
     r.stride = o;
     return r;
@@ -181,10 +182,12 @@ __global__ void __launch_bounds__(256) ramp_policy_head_grad_kernel(const Policy
     __shared__ float s_dh[LRN_WARPS][32 * POL_MAX_HPL], s_dhv[LRN_WARPS][32 * POL_MAX_HPL];
     const ramp_policy_config_t& c = P.c;
     const int gin = c.in_features_graph + c.n_actions, og = c.out_features_graph, on = c.out_features_node, fin = on + og;
-    const int H = c.fcnet_hidden, A = c.n_actions, hpl = H / 32, fa = c.fcnet_activation;
+    const int H = c.fcnet_hidden, A = c.n_actions, fa = c.fcnet_activation;
+    const bool share = c.vf_share_layers;
     const HeadRec R = head_rec(c);
     const float* w = P.w;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int hpl = (H - lane + 31) / 32;                          // this lane's hidden units lane + 32 u < H
     const int i = blockIdx.x * LRN_WARPS + warp;
     if (i >= g.mb) return;
     float* rec = g.rec + (size_t)i * R.stride;
@@ -222,12 +225,19 @@ __global__ void __launch_bounds__(256) ramp_policy_head_grad_kernel(const Policy
     float h[POL_MAX_HPL], hv[POL_MAX_HPL];
 #pragma unroll
     for (int u = 0; u < POL_MAX_HPL; ++u) {
+        const int j = lane + 32 * u;
         if (u < hpl) {
-            const int j = lane + 32 * u;
-            float p = w[P.hb + j], q = w[P.vhb + j];
-            const float* hr = w + P.hW + (size_t)j * fin; const float* vr = w + P.vhW + (size_t)j * fin;
-            for (int k = 0; k < fin; ++k) { const float f = fb[k]; p += hr[k] * f; q += vr[k] * f; }
-            h[u] = act_fn(p, fa); hv[u] = act_fn(q, fa);
+            float p = w[P.hb + j];
+            const float* hr = w + P.hW + (size_t)j * fin;
+            if (share) {
+                for (int k = 0; k < fin; ++k) p += hr[k] * fb[k];
+                h[u] = hv[u] = act_fn(p, fa);
+            } else {
+                float q = w[P.vhb + j];
+                const float* vr = w + P.vhW + (size_t)j * fin;
+                for (int k = 0; k < fin; ++k) { const float f = fb[k]; p += hr[k] * f; q += vr[k] * f; }
+                h[u] = act_fn(p, fa); hv[u] = act_fn(q, fa);
+            }
         }
     }
     float my_logit = -FLT_MAX;
@@ -317,20 +327,27 @@ __global__ void __launch_bounds__(256) ramp_policy_head_grad_kernel(const Policy
     float* dhs = s_dh[warp]; float* dvs = s_dhv[warp];
 #pragma unroll
     for (int u = 0; u < POL_MAX_HPL; ++u) {
+        const int j = lane + 32 * u;
         if (u < hpl) {
-            const int j = lane + 32 * u;
             float d = 0.f;
             for (int o = 0; o < A; ++o) d += db[o] * w[P.lW + (size_t)o * H + j];
-            const float dp = d * act_grad(h[u], fa), dq = dv * w[P.vW + j] * act_grad(hv[u], fa);
-            dhs[j] = dp; dvs[j] = dq;
-            rec[R.h + j] = h[u]; rec[R.hv + j] = hv[u]; rec[R.dh + j] = dp; rec[R.dhv + j] = dq;
+            if (share) {                 // h feeds the logits and the value: dh = (sum_o dl_o lW[o][j] + dv vW[j]) act'(h)
+                const float dp = (d + dv * w[P.vW + j]) * act_grad(h[u], fa);
+                dhs[j] = dp;
+                rec[R.h + j] = h[u]; rec[R.dh + j] = dp;
+            } else {
+                const float dp = d * act_grad(h[u], fa), dq = dv * w[P.vW + j] * act_grad(hv[u], fa);
+                dhs[j] = dp; dvs[j] = dq;
+                rec[R.h + j] = h[u]; rec[R.hv + j] = hv[u]; rec[R.dh + j] = dp; rec[R.dhv + j] = dq;
+            }
         }
     }
     __syncwarp();
     // ---- hidden layers -> read-out input [emb | graph module] ----
     for (int k = lane; k < fin; k += 32) {
         float d = 0.f;
-        for (int j = 0; j < H; ++j) d += w[P.hW + (size_t)j * fin + k] * dhs[j] + w[P.vhW + (size_t)j * fin + k] * dvs[j];
+        if (share) for (int j = 0; j < H; ++j) d += w[P.hW + (size_t)j * fin + k] * dhs[j];
+        else for (int j = 0; j < H; ++j) d += w[P.hW + (size_t)j * fin + k] * dhs[j] + w[P.vhW + (size_t)j * fin + k] * dvs[j];
         db[k] = d;
     }
     __syncwarp();
@@ -344,7 +361,7 @@ __global__ void __launch_bounds__(256) ramp_policy_head_grad_kernel(const Policy
     }
 }
 
-// the read-out's and graph module's segments in blob order (host: the learner's setup)
+// the read-out's and graph module's segments in blob order (host: the learner's setup); their count (at most HEAD_SEGS)
 inline int head_segs(const PolicyDev& P, const float* rec, int mb, Seg* s) {
     const ramp_policy_config_t& c = P.c;
     const HeadRec R = head_rec(c);
@@ -362,9 +379,11 @@ inline int head_segs(const PolicyDev& P, const float* rec, int mb, Seg* s) {
     s[k++] = seg(SEG_SUM, H, 0, R.dh, 0, P.hb);
     s[k++] = seg(SEG_OUTER, A, H, R.dl, R.h, P.lW);
     s[k++] = seg(SEG_SUM, A, 0, R.dl, 0, P.lb);
-    s[k++] = seg(SEG_OUTER, H, fin, R.dhv, R.fb, P.vhW);
-    s[k++] = seg(SEG_SUM, H, 0, R.dhv, 0, P.vhb);
-    s[k++] = seg(SEG_OUTER, 1, H, R.dv, R.hv, P.vW);
+    if (!c.vf_share_layers) {
+        s[k++] = seg(SEG_OUTER, H, fin, R.dhv, R.fb, P.vhW);
+        s[k++] = seg(SEG_SUM, H, 0, R.dhv, 0, P.vhb);
+    }
+    s[k++] = seg(SEG_OUTER, 1, H, R.dv, c.vf_share_layers ? R.h : R.hv, P.vW);
     s[k++] = seg(SEG_SUM, 1, 0, R.dv, 0, P.vb);
     return k;
 }

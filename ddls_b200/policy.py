@@ -25,11 +25,28 @@ DEFAULT_CONFIG = dict(in_features_node=5, in_features_edge=2, in_features_graph=
                       out_features_node=16, out_features_graph=8, num_rounds=2, aggregator_activation='relu', fcnet_hiddens=(256,),
                       fcnet_activation='relu', apply_action_mask=True)
 
+ALGOS = ('ppo', 'impala', 'pg', 'es')
+
+
+def algo_model_config(algo: str, n_actions: int) -> Dict:
+    """gnn.yaml with the model overrides of scripts/ramp_job_partitioning_configs/algo/{algo}.yaml: fcnet_hiddens [n_actions]
+    ("must == action_space.n"); ppo.yaml sets vf_share_layers False, impala / pg / es.yaml leave RLlib's MODEL_DEFAULTS value, True
+    (the value layer reads the policy's hidden layer).  DQN / Ape-X keep gnn.yaml's [256] and are not device learners."""
+    if algo not in ALGOS:
+        raise ValueError(f'no device learner for algorithm {algo!r} (one of {ALGOS})')
+    return dict(DEFAULT_CONFIG, fcnet_hiddens=(int(n_actions),), vf_share_layers=algo != 'ppo')
+
+
+def _shared(config: Dict) -> bool:
+    """RLlib's vf_share_layers: absent means gnn.yaml's model, a separate value branch"""
+    return bool(config.get('vf_share_layers', False))
+
 
 class _Config(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ('in_features_node', 'in_features_edge', 'in_features_graph', 'n_actions', 'out_features_msg',
                                           'out_features_hidden', 'out_features_node', 'out_features_graph', 'num_rounds', 'fcnet_hidden',
-                                          'aggregator_activation', 'fcnet_activation', 'apply_action_mask', 'n_models')]
+                                          'aggregator_activation', 'fcnet_activation', 'apply_action_mask', 'n_models',
+                                          'vf_share_layers')]
 
 
 def c_config(config: Dict, n_actions: int, n_models: int) -> _Config:
@@ -38,7 +55,7 @@ def c_config(config: Dict, n_actions: int, n_models: int) -> _Config:
     return _Config(c['in_features_node'], c['in_features_edge'], c['in_features_graph'], int(n_actions), c['out_features_msg'],
                    c['out_features_hidden'], c['out_features_node'], c['out_features_graph'], c['num_rounds'],
                    tuple(c['fcnet_hiddens'])[0], ACTIVATIONS[c['aggregator_activation']], ACTIVATIONS[c['fcnet_activation']],
-                   1 if c['apply_action_mask'] else 0, int(n_models))
+                   1 if c['apply_action_mask'] else 0, int(n_models), 1 if _shared(c) else 0)
 
 
 def _shaped(name, a, shape):
@@ -88,17 +105,23 @@ def _bind(L):
     L._policy_bound = True
 
 
+def _readout(config: Dict) -> Sequence[str]:
+    names = ['logit_module._hidden_layers.0', 'logit_module._logits', 'logit_module._value_branch_separate.0', 'logit_module._value_branch']
+    return [n for n in names if not (_shared(config) and '_separate' in n)]
+
+
 def weight_keys(config: Dict) -> Sequence[str]:
     """state_dict keys of the reference's GNNPolicy in blob order (weights then biases per module): gnn_module.layers.{r}.
     {node,edge,reduce}_module.{0: LayerNorm, 1: Linear}; graph_module.{0,1}; the RLlib FullyConnectedNetwork read-out
-    (logit_module._hidden_layers.0, ._logits, ._value_branch_separate.0, ._value_branch; each a SlimFC whose Linear is ._model.0)."""
+    (logit_module._hidden_layers.0, ._logits, ._value_branch_separate.0, ._value_branch; each a SlimFC whose Linear is ._model.0).
+    Under vf_share_layers there is no ._value_branch_separate: ._value_branch reads ._hidden_layers.0's output."""
     keys = []
     for r in range(config['num_rounds']):
         for mod in ('node_module', 'edge_module', 'reduce_module'):
             for layer in (0, 1):
                 keys += [f'gnn_module.layers.{r}.{mod}.{layer}.weight', f'gnn_module.layers.{r}.{mod}.{layer}.bias']
     keys += ['graph_module.0.weight', 'graph_module.0.bias', 'graph_module.1.weight', 'graph_module.1.bias']
-    for name in ('logit_module._hidden_layers.0', 'logit_module._logits', 'logit_module._value_branch_separate.0', 'logit_module._value_branch'):
+    for name in _readout(config):
         keys += [f'{name}._model.0.weight', f'{name}._model.0.bias']
     return keys
 
@@ -120,20 +143,28 @@ def weight_shapes(config: Dict, n_actions: int) -> Dict[str, tuple]:
     gin, fin = c['in_features_graph'] + n_actions, c['out_features_node'] + c['out_features_graph']
     shapes.update({'graph_module.0.weight': (gin,), 'graph_module.0.bias': (gin,), 'graph_module.1.weight': (c['out_features_graph'], gin),
                    'graph_module.1.bias': (c['out_features_graph'],)})
-    for name, (o, i) in (('logit_module._hidden_layers.0', (H, fin)), ('logit_module._logits', (n_actions, H)),
-                         ('logit_module._value_branch_separate.0', (H, fin)), ('logit_module._value_branch', (1, H))):
+    dims = {'logit_module._hidden_layers.0': (H, fin), 'logit_module._logits': (n_actions, H),
+            'logit_module._value_branch_separate.0': (H, fin), 'logit_module._value_branch': (1, H)}
+    for name in _readout(config):
+        o, i = dims[name]
         shapes[f'{name}._model.0.weight'] = (o, i)
         shapes[f'{name}._model.0.bias'] = (o,)
     return shapes
 
 
 def pack_weights(state_dict: Dict, config: Dict, n_actions: int) -> np.ndarray:
-    """Flat fp32 blob from a GNNPolicy state_dict (torch tensors or arrays); shapes are checked against the configuration."""
+    """Flat fp32 blob from a GNNPolicy state_dict (torch tensors or arrays); shapes are checked against the configuration, and a
+    value branch the configuration's vf_share_layers does not have is refused."""
     shapes = weight_shapes(config, n_actions)
+    for k in state_dict:
+        if k.startswith('logit_module._value_branch_separate.') and _shared(config):
+            raise KeyError(f'state_dict has {k!r}: a separate value branch, but the configuration shares the value layers '
+                           '(vf_share_layers)')
     parts = []
     for k in weight_keys(config):
         if k not in state_dict:
-            raise KeyError(f'state_dict has no {k!r}')
+            hint = ' (a checkpoint with vf_share_layers?)' if '_value_branch_separate' in k else ''
+            raise KeyError(f'state_dict has no {k!r}{hint}')
         v = state_dict[k]
         v = v.detach().cpu().numpy() if hasattr(v, 'detach') else np.asarray(v)
         if tuple(v.shape) != shapes[k]:

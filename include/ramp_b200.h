@@ -496,7 +496,8 @@ int ramp_env_read(ramp_engine_t* eng, double* reward, uint8_t* done, int32_t* qu
 /* ---- the GNN policy forward on the device (SURVEY.md 8f-3): GNNPolicy.forward (ml_models/policies/gnn_policy.py:137-296) =
  * num_rounds MeanPool message-passing rounds over the queued job's graph (ml_models/models/mean_pool.py:107-150, gnn.py:84-92),
  * the mean of the node embeddings, a graph module over [graph features | action mask] (gnn_policy.py:96-109), and an RLlib
- * FullyConnectedNetwork read-out (fcnet_hiddens, separate value branch) with the log-mask added to the logits
+ * FullyConnectedNetwork read-out (fcnet_hiddens; a separate value branch, or the value layer on the policy's hidden layer under
+ * vf_share_layers) with the log-mask added to the logits
  * (gnn_policy.py:283-290).  What the policy sees of a job's ops and deps is fixed per job TYPE (node / edge features:
  * observation.py:503-567), so the message passing is run once per model and weight set (ramp_policy_embed: one CTA per model);
  * per decision only the graph module + read-out run (one warp per episode, weights staged in shared memory), reading the
@@ -508,16 +509,21 @@ typedef struct {
     int32_t n_actions;                                               /* action_space.n = max_partitions_per_op + 1    */
     int32_t out_features_msg, out_features_hidden, out_features_node, out_features_graph;   /* 32, 64, 16, 8          */
     int32_t num_rounds;                                              /* >= 2 (gnn.py:40-41)                           */
-    int32_t fcnet_hidden;                                            /* one hidden layer of the read-out (256)        */
+    int32_t fcnet_hidden;                                            /* one hidden layer of the read-out (256): a     */
+                                                                     /* multiple of 32 in [32, 512], or n_actions     */
     int32_t aggregator_activation;                                   /* 0 relu, 1 leaky_relu(0.01)                    */
     int32_t fcnet_activation;                                        /* 0 relu, 2 tanh                                */
     int32_t apply_action_mask;
     int32_t n_models;
+    int32_t vf_share_layers;                                         /* 0: separate value branch; 1: RLlib's          */
+                                                                     /* vf_share_layers, the value layer [1][H] reads */
+                                                                     /* the policy's hidden layer                     */
 } ramp_policy_config_t;
 typedef struct ramp_policy ramp_policy_t;
 /* number of fp32 words of the weight blob for `cfg`, in torch state_dict order of GNNPolicy: per round [node LN w,b | node
  * Linear W,b | edge LN w,b | edge Linear W,b | reduce LN w,b | reduce Linear W,b]; graph LN w,b | graph Linear W,b; read-out hidden
- * W,b | logits W,b | value hidden W,b | value W,b.  Every W is [out][in] row-major as torch.nn.Linear keeps it. */
+ * W,b | logits W,b | value hidden W,b (not under vf_share_layers) | value W,b.  Every W is [out][in] row-major as torch.nn.Linear
+ * keeps it. */
 int64_t ramp_policy_weight_count(const ramp_policy_config_t* cfg);
 int ramp_policy_create(int device, const ramp_policy_config_t* cfg, ramp_policy_t** out);
 void ramp_policy_destroy(ramp_policy_t* p);

@@ -23,16 +23,20 @@ def main():
     ap.add_argument('--noise-size', type=int, default=250_000_000)
     ap.add_argument('--seed', type=int, default=0)
     ap.add_argument('--out', default=None)
+    ap.add_argument('--model', choices=('gnn', 'algo'), default='gnn',
+                    help="gnn: gnn.yaml's read-out ([256], separate value branch); algo: algo/es.yaml's (policy.algo_model_config)")
     args = ap.parse_args()
     from ddls_b200 import workload
     from ddls_b200.batched import DeviceRampJobPartitioningEnvironment
     from ddls_b200.learn import DeviceESLearner, ESConfig, shared_noise_table
-    from ddls_b200.policy import DeviceGNNPolicy
+    from ddls_b200.policy import DeviceGNNPolicy, algo_model_config
 
     graphs = [workload.make_graph('resnet')]
     env = DeviceRampJobPartitioningEnvironment((4, 4, 4), graphs, n_episodes=args.episodes, jobs_per_episode=args.jobs, seed=args.seed,
                                                prewarm=True)
-    pol = DeviceGNNPolicy(graphs, env.max_partitions_per_op + 1, seed=args.seed)
+    n_actions = env.max_partitions_per_op + 1
+    model = algo_model_config('es', n_actions) if args.model == 'algo' else None
+    pol = DeviceGNNPolicy(graphs, n_actions, config=model, seed=args.seed)
     t0 = time.perf_counter()
     noise = shared_noise_table(args.noise_size)
     noise_s = time.perf_counter() - t0

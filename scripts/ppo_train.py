@@ -23,15 +23,19 @@ def main():
     ap.add_argument('--num-sgd-iter', type=int, default=None, help="override ppo.yaml's 50 passes")
     ap.add_argument('--seed', type=int, default=0)
     ap.add_argument('--out', default=None)
+    ap.add_argument('--model', choices=('gnn', 'algo'), default='gnn',
+                    help="gnn: gnn.yaml's read-out ([256], separate value branch); algo: algo/ppo.yaml's (policy.algo_model_config)")
     args = ap.parse_args()
     from ddls_b200 import workload
     from ddls_b200.batched import DeviceRampJobPartitioningEnvironment
     from ddls_b200.learn import DevicePPOLearner, PPOConfig
-    from ddls_b200.policy import DeviceGNNPolicy
+    from ddls_b200.policy import DeviceGNNPolicy, algo_model_config
 
     graphs = [workload.make_graph('resnet')]
     env = DeviceRampJobPartitioningEnvironment((4, 4, 4), graphs, n_episodes=args.episodes, jobs_per_episode=args.jobs, seed=args.seed)
-    pol = DeviceGNNPolicy(graphs, env.max_partitions_per_op + 1, seed=args.seed)
+    n_actions = env.max_partitions_per_op + 1
+    model = algo_model_config('ppo', n_actions) if args.model == 'algo' else None
+    pol = DeviceGNNPolicy(graphs, n_actions, config=model, seed=args.seed)
     cfg = PPOConfig(seed=args.seed)
     if args.num_sgd_iter is not None:
         cfg.num_sgd_iter = args.num_sgd_iter
