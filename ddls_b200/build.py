@@ -8,7 +8,7 @@ LIB_PATH = os.path.join(HERE, 'libramp_b200.so')
 SOURCES = [os.path.join(HERE, 'csrc', 'ramp_engine.cu'), os.path.join(HERE, 'csrc', 'ramp_expand.cpp'),
            os.path.join(HERE, 'csrc', 'ramp_quotient.cpp'), os.path.join(HERE, 'csrc', 'ramp_policy.cu')]
 DEPS = SOURCES + [os.path.join(HERE, 'csrc', 'ramp_kernels.cuh'), os.path.join(HERE, 'csrc', 'ramp_lookahead_cta.cuh'),
-                  os.path.join(HERE, 'csrc', 'ramp_lookahead_thread.cuh'), os.path.join(HERE, 'csrc', 'ramp_env.cuh'),
+                  os.path.join(HERE, 'csrc', 'ramp_lookahead_thread.cuh'), os.path.join(HERE, 'csrc', 'ramp_env.cuh'), os.path.join(HERE, 'csrc', 'ramp_env_io.cuh'),
                   os.path.join(HERE, 'csrc', 'ramp_owned.cuh'), os.path.join(HERE, 'csrc', 'ramp_policy_learn.cuh'),
                   os.path.join(HERE, 'csrc', 'ramp_es.cuh'),
                   os.path.join(os.path.dirname(HERE), 'include', 'ramp_b200.h')]

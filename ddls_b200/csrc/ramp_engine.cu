@@ -16,6 +16,7 @@
 
 #include "ramp_kernels.cuh"
 #include "ramp_env.cuh"
+#include "ramp_env_io.cuh"
 #include "ramp_owned.cuh"
 
 using namespace ramp;
@@ -183,11 +184,19 @@ struct ramp_engine {
     EnvDev env{};
     std::vector<DeviceArray<unsigned char>> env_allocs;
     PinnedArray<int32_t> env_h_need;     // [0] = count, [1] = error flag; [2], [3]: the same, read by ramp_env_read; [4] engine error episode
+                                         // [6..7] ramp_env_ingest's range word
     PinnedArray<unsigned char> env_h_mirror;   // host arrays of ramp_env_host_mirror
     bool env_unchecked_decide = false;   // a ramp_env_decide without need_host_out has not been looked at yet
     bool env_agents_set = false;         // ramp_env_set_agents ran
     DeviceArray<double> steplog_stats, steplog_rewards;   // ramp_env_steplog_begin: [horizon][RAMP_ENV_STEP_STATS_LEN][B], [horizon][B]
     DeviceArray<int32_t> steplog_actions;                 // [horizon][B]
+    // i/o in caller-owned device memory (ramp_env_ingest / ramp_env_export), allocated by the first call that needs them
+    DeviceArray<float> env_graph_static;                  // [n_models][6] ramp_env_set_graph_static
+    DeviceArray<unsigned long long> env_range_err;        // [1] ramp_env_ingest_kernel's sticky word
+    DeviceArray<long long> env_range_val;                 // [B] the out-of-set action recorded with it
+    Event env_ev_to_caller, env_ev_to_engine;             // the caller's stream waits for the engine's / the engine's for the caller's
+    uint32_t env_ingest_seq = 0;                          // ingest calls since the word was last cleared
+    bool env_range_armed = false;                         // a ramp_env_ingest ran since the word was last looked at
     // standalone lookahead buffers
     DeviceArray<WorkItem> sa_chunk_items;
     DeviceArray<ChunkDesc> sa_chunks;
@@ -596,6 +605,50 @@ template <class T> int env_upload(ramp_engine* e, T** dst, const void* src, size
     if (src && n) CUDA_TRY(cudaMemcpy(e->env_allocs.back().get(), src, sizeof(T) * n, cudaMemcpyHostToDevice));
     else CUDA_TRY(cudaMemset(e->env_allocs.back().get(), 0, sizeof(T) * std::max<size_t>(n, 1)));
     return RAMP_OK;
+}
+
+// makes `to` wait for the work queued on `from` so far
+int env_fence(cudaEvent_t ev, cudaStream_t from, cudaStream_t to) {
+    CUDA_TRY(cudaEventRecord(ev, from));
+    CUDA_TRY(cudaStreamWaitEvent(to, ev, 0));
+    return RAMP_OK;
+}
+
+// the range word and the events of ramp_env_ingest / ramp_env_export, made by the first of them; the word is cleared on the
+// engine stream, which both calls fence their kernels behind
+int env_io_ready(ramp_engine* e) {
+    if (e->env_ev_to_engine) return RAMP_OK;
+    CUDA_TRY(e->env_range_err.alloc(1));
+    CUDA_TRY(e->env_range_val.alloc((size_t)e->env.B));
+    CUDA_TRY(cudaMemsetAsync(e->env_range_err.get(), 0xFF, sizeof(unsigned long long), e->stream.get()));
+    CUDA_TRY(create(e->env_ev_to_caller, cudaEventDisableTiming));
+    CUDA_TRY(create(e->env_ev_to_engine, cudaEventDisableTiming));
+    return RAMP_OK;
+}
+
+// queues the copy of the range word to env_h_need[6..7]; the caller synchronises the engine stream before env_range_raise
+int env_range_fetch(ramp_engine* e) {
+    CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 6, e->env_range_err.get(), sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                             e->stream.get()));
+    return RAMP_OK;
+}
+
+// RJPE:314-316 for the first out-of-set action ramp_env_ingest recorded, if any.  Raising clears the word and the step's invalid-
+// action word, as the step that raised is not taken any further.
+int env_range_raise(ramp_engine* e) {
+    e->env_range_armed = false;
+    const unsigned long long w = *reinterpret_cast<const unsigned long long*>(e->env_h_need.get() + 6);
+    if (w == ENV_NO_RANGE_ERR) return RAMP_OK;
+    const int b = (int)(uint32_t)w;
+    long long a = 0;
+    CUDA_TRY(cudaMemcpy(&a, e->env_range_val.get() + b, sizeof(long long), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemsetAsync(e->env_range_err.get(), 0xFF, sizeof(unsigned long long), e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(e->env.err, 0, sizeof(int32_t), e->stream.get()));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
+    e->env_ingest_seq = 0;
+    std::string set;
+    for (int k = 0; k <= e->env.max_degree; ++k) set += (k ? ", " : "") + std::to_string(k);
+    return set_error(RAMP_ERR_BAD_ARG, "episode %d: Action %lld not in action set [%s]. (RJPE:314-316)", b, a, set.c_str());
 }
 
 // the action rows the engine writes itself, in stream order (ramp_step_host, the device environment): their steps take the
@@ -1487,6 +1540,11 @@ int ramp_env_reset(ramp_engine_t* e, const int32_t* model_of, const double* frac
     CUDA_TRY(cudaMemsetAsync(v.job_tmpl, 0xFF, sizeof(int32_t) * n, e->stream.get()));          // -1
     CUDA_TRY(cudaMemsetAsync(v.ret, 0, sizeof(double) * (size_t)v.B, e->stream.get()));
     CUDA_TRY(cudaMemsetAsync(v.err, 0, sizeof(int32_t), e->stream.get()));
+    if (e->env_range_err.get()) {
+        CUDA_TRY(cudaMemsetAsync(e->env_range_err.get(), 0xFF, sizeof(unsigned long long), e->stream.get()));
+        e->env_ingest_seq = 0;
+        e->env_range_armed = false;
+    }
     int rc = ramp_reset(e, arrivals, v.J);
     if (rc != RAMP_OK) return rc;
     ramp_env_update_kernel<<<(v.B + 127) / 128, 128, 0, e->stream.get()>>>(v, e->ep, nullptr, 1);
@@ -1536,7 +1594,10 @@ int ramp_env_decide(ramp_engine_t* e, const int32_t* actions, int32_t* n_need_ho
     if (n_need_host_out) {
         CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get(), v.n_need_host, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 1, v.err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        const bool range = e->env_range_armed;
+        if (range) { int rc = env_range_fetch(e); if (rc != RAMP_OK) return rc; }
         CUDA_TRY(cudaStreamSynchronize(st));
+        if (range) { int rc = env_range_raise(e); if (rc != RAMP_OK) return rc; }
         if (e->env_h_need.get()[1] != 0) {
             CUDA_TRY(cudaMemset(v.err, 0, sizeof(int32_t)));
             return set_error(RAMP_ERR_BAD_ARG, "episode %d: the action is invalid given its action mask (RJPE:314-319)", e->env_h_need.get()[1] - 1);
@@ -1602,9 +1663,13 @@ int ramp_env_read(ramp_engine_t* e, double* reward, uint8_t* done, int32_t* queu
         // in `err`; episodes the tables could not decide were left unplaced, which only the LAST decide's count can show
         CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 2, v.n_need_host, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 3, v.err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        int rc = ramp_sync(e);
+        const bool range = e->env_range_armed;
+        int rc = range ? env_range_fetch(e) : RAMP_OK;
+        if (rc != RAMP_OK) return rc;
+        rc = ramp_sync(e);
         if (rc != RAMP_OK) return rc;
         e->env_unchecked_decide = false;
+        if (range && (rc = env_range_raise(e)) != RAMP_OK) return rc;      // RJPE:314-316 before 317-319
         if (e->env_h_need.get()[3] != 0) {
             CUDA_TRY(cudaMemset(v.err, 0, sizeof(int32_t)));
             return set_error(RAMP_ERR_BAD_ARG, "episode %d: the action is invalid given its action mask (RJPE:314-319)", e->env_h_need.get()[3] - 1);
@@ -1614,10 +1679,72 @@ int ramp_env_read(ramp_engine_t* e, double* reward, uint8_t* done, int32_t* queu
         return e->env_h_need.get()[4] != 0 ? ramp_check_status(e, nullptr, nullptr) : RAMP_OK;
     }
     {
-        int rc = ramp_sync(e);
+        const bool range = e->env_range_armed;
+        int rc = range ? env_range_fetch(e) : RAMP_OK;
         if (rc != RAMP_OK) return rc;
+        rc = ramp_sync(e);
+        if (rc != RAMP_OK) return rc;
+        if (range && (rc = env_range_raise(e)) != RAMP_OK) return rc;
     }
     return e->env_h_need.get()[4] != 0 ? ramp_check_status(e, nullptr, nullptr) : RAMP_OK;
+}
+
+int ramp_env_set_graph_static(ramp_engine_t* e, const float* graph_static) {
+    if (!e || !e->has_env || !graph_static) return set_error(RAMP_ERR_BAD_ARG, "no environment or no statistics");
+    const size_t n = (size_t)e->env.n_models * ENV_GF_STATIC;
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    CUDA_TRY(cudaStreamSynchronize(e->stream.get()));      // no export queued behind the engine stream still reads the old table
+    if (!e->env_graph_static.get()) CUDA_TRY(e->env_graph_static.alloc(n));
+    CUDA_TRY(cudaMemcpy(e->env_graph_static.get(), graph_static, sizeof(float) * n, cudaMemcpyHostToDevice));
+    return RAMP_OK;
+}
+
+// RJPE:300-322 (the action, range-checked as RJPE:314-316 does) from caller-owned device memory, on the caller's stream
+int ramp_env_ingest(ramp_engine_t* e, const void* actions, int32_t dtype, void* stream) {
+    if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
+    if (!actions) return set_error(RAMP_ERR_BAD_ARG, "null actions");
+    if (dtype != RAMP_ACTIONS_INT32 && dtype != RAMP_ACTIONS_INT64)
+        return set_error(RAMP_ERR_BAD_ARG, "actions dtype %d is neither RAMP_ACTIONS_INT32 nor RAMP_ACTIONS_INT64", dtype);
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    int rc = env_io_ready(e);
+    if (rc != RAMP_OK) return rc;
+    EnvDev& v = e->env;
+    cudaStream_t cs = (cudaStream_t)stream, st = e->stream.get();
+    // the last ramp_env_advance wrote `done` and read `actions` (its env-step record), both on the engine stream
+    if ((rc = env_fence(e->env_ev_to_caller.get(), st, cs)) != RAMP_OK) return rc;
+    EnvIngestArgs a{};
+    a.actions = actions; a.is64 = dtype == RAMP_ACTIONS_INT64; a.B = v.B; a.max_degree = v.max_degree; a.seq = e->env_ingest_seq++;
+    a.done = v.done; a.out = v.actions; a.range_err = e->env_range_err.get(); a.range_val = e->env_range_val.get();
+    ramp_env_ingest_kernel<<<(v.B + 127) / 128, 128, 0, cs>>>(a);
+    e->launches++;
+    CUDA_TRY(cudaGetLastError());
+    e->env_range_armed = true;
+    return env_fence(e->env_ev_to_engine.get(), cs, st);       // ramp_env_decide reads what the kernel wrote
+}
+
+// RampJobPartitioningObservation (ramp_job_partitioning_observation.py:275, observation.py:80-131, 358-498), reward and done of the
+// last ramp_env_advance into caller-owned device memory, on the caller's stream
+int ramp_env_export(ramp_engine_t* e, void* stream, const ramp_env_export_t* out) {
+    if (!e || !e->has_env || !out) return set_error(RAMP_ERR_BAD_ARG, "no environment or no outputs");
+    if (out->graph_features && !e->env_graph_static.get())
+        return set_error(RAMP_ERR_BAD_ARG, "graph_features needs the per-graph statistics: call ramp_env_set_graph_static first");
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    int rc = env_io_ready(e);
+    if (rc != RAMP_OK) return rc;
+    const EnvDev& v = e->env;
+    cudaStream_t cs = (cudaStream_t)stream, st = e->stream.get();
+    if ((rc = env_fence(e->env_ev_to_caller.get(), st, cs)) != RAMP_OK) return rc;     // ramp_env_update_kernel's outputs
+    EnvExportArgs a{};
+    a.B = v.B; a.A = v.max_degree + 1; a.n_models = v.n_models;
+    a.queued_model = v.queued_model; a.obs_dyn = v.obs_dyn; a.mask = v.action_mask; a.reward = v.reward; a.done = v.done;
+    a.graph_static = e->env_graph_static.get();
+    a.model = reinterpret_cast<long long*>(out->model); a.graph_features = out->graph_features; a.action_mask = out->action_mask;
+    a.reward_out = out->reward; a.done_out = out->done;
+    const long long n = (long long)v.B * (ENV_GF_BASE + a.A);
+    ramp_env_export_kernel<<<(unsigned)((n + 255) / 256), 256, 0, cs>>>(a);
+    e->launches++;
+    CUDA_TRY(cudaGetLastError());
+    return env_fence(e->env_ev_to_engine.get(), cs, st);       // the next step's kernels overwrite what the kernel reads
 }
 
 

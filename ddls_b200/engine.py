@@ -174,7 +174,8 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_policy_learner_state', 'ramp_policy_learner_reset', 'ramp_impala_loss_grad', 'ramp_policy_learn_impala',
                     'ramp_impala_vtrace_read', 'ramp_es_create', 'ramp_es_destroy', 'ramp_es_round_begin', 'ramp_es_act',
                     'ramp_es_round_end', 'ramp_es_step', 'ramp_es_update', 'ramp_es_read', 'ramp_es_act_read', 'ramp_es_state',
-                    'ramp_es_reset', 'ramp_pg_loss_grad', 'ramp_policy_learn_pg']
+                    'ramp_es_reset', 'ramp_pg_loss_grad', 'ramp_policy_learn_pg',
+                    'ramp_env_set_graph_static', 'ramp_env_ingest', 'ramp_env_export']
 
 
 def device_bytes():

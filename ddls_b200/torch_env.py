@@ -1,0 +1,147 @@
+"""The device environment with PyTorch CUDA tensors in and out, ordered on the caller's stream.
+
+``TorchRampJobPartitioningEnvironment`` wraps a ``DeviceRampJobPartitioningEnvironment``: ``step(actions)`` takes an int32 or int64
+CUDA tensor [B] and returns the reference's observation (``model`` [B] int64, ``graph_features`` [B, 17 + |A|] float32 in
+RampJobPartitioningObservation's layout, ``action_mask`` [B, |A|] bool), ``reward`` [B] float64 and ``done`` [B] bool as CUDA tensors.
+Every kernel that touches a tensor runs on ``torch.cuda.current_stream()`` (include/ramp_b200.h: ramp_env_ingest / ramp_env_export),
+so a torch policy feeds the environment and reads it back at device speed, and the caching allocator never needs ``record_stream``.
+What the policy observes of a job type whatever the cluster holds -- node and edge features, edge endpoints, the six per-graph
+statistics -- is ``static``, uploaded once per job type.  This is the only module of the package that imports torch."""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+
+from . import engine as _engine
+from .batched import DeviceRampJobPartitioningEnvironment
+from .observation import static_observation
+
+ACTIONS_INT32, ACTIONS_INT64 = 0, 1           # include/ramp_b200.h RAMP_ACTIONS_*
+N_GRAPH_FEATURES = 17                          # graph_features columns before the action mask
+OUTPUTS = ('model', 'graph_features', 'action_mask', 'reward', 'done')
+
+
+class _Export(C.Structure):
+    _fields_ = [('model', C.c_void_p), ('graph_features', C.c_void_p), ('action_mask', C.c_void_p), ('reward', C.c_void_p),
+                ('done', C.c_void_p)]
+
+
+def _bind(L):
+    for name in ('ramp_env_set_graph_static', 'ramp_env_ingest', 'ramp_env_export'):
+        getattr(L, name).restype = C.c_int
+    L.ramp_env_set_graph_static.argtypes = [C.c_void_p, C.c_void_p]
+    L.ramp_env_ingest.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+    L.ramp_env_export.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_Export)]
+
+
+def static_tensors(graphs, device='cpu'):
+    """Per job type: ``node_features`` [N, 5], ``edge_features`` [E, 2] float32, ``edges_src`` / ``edges_dst`` [E] int64 and
+    ``graph_static`` [6] float32 -- ``observation.static_observation`` as tensors on `device`, what GNNPolicy embeds."""
+    out = []
+    for g in graphs:
+        st = static_observation(g)
+        out.append({'node_features': torch.from_numpy(st['node_features']).to(device),
+                    'edge_features': torch.from_numpy(st['edge_features']).to(device),
+                    'edges_src': torch.from_numpy(st['edges_src'].astype(np.int64)).to(device),
+                    'edges_dst': torch.from_numpy(st['edges_dst'].astype(np.int64)).to(device),
+                    'graph_static': torch.from_numpy(st['graph_static']).to(device)})
+    return out
+
+
+class TorchRampJobPartitioningEnvironment:
+    def __init__(self, *args, prewarm: bool = False, **kw):
+        """The arguments of ``DeviceRampJobPartitioningEnvironment`` (``device`` picks cuda:<device>).  A failed construction
+        frees what it allocated."""
+        env = DeviceRampJobPartitioningEnvironment.__new__(DeviceRampJobPartitioningEnvironment)
+        try:
+            env.__init__(*args, prewarm=prewarm, **kw)
+            self.env = env
+            self.device = torch.device('cuda', int(kw.get('device', 0)))
+            self.B, self.n_actions = env.B, env.max_partitions_per_op + 1
+            self._L, self._h = env.eng._L, env.eng._h
+            _bind(self._L)
+            self.static = static_tensors([m.graph for m in env.models], self.device)
+            table = np.ascontiguousarray(np.stack([st['graph_static'].cpu().numpy() for st in self.static]), dtype=np.float32)
+            _engine._check(self._L.ramp_env_set_graph_static(self._h, table.ctypes.data))
+        except BaseException:
+            eng = getattr(env, 'eng', None)
+            if eng is not None:
+                eng.close()
+            raise
+
+    # ---- pass-throughs ------------------------------------------------------------------------------------------------
+    def episode_stats(self):
+        return self.env.episode_stats()
+
+    def decisions(self):
+        return self.env.decisions()
+
+    def record_steps(self, horizon: int):
+        self.env.record_steps(horizon)
+
+    def recorded_steps(self):
+        return self.env.recorded_steps()
+
+    def close(self):
+        env = getattr(self, 'env', None)
+        if env is not None:
+            env.close()
+            self.env = None
+
+    # ---- the environment -----------------------------------------------------------------------------------------------
+    def check(self):
+        """Synchronises and raises what the steps since the last check deferred: an action outside the action set, an action
+        the mask forbids (apply_action_mask=True), a simulation error."""
+        _engine._check(self._L.ramp_env_read(self._h, None, None, None, None, None))
+
+    def reset(self):
+        """RampJobPartitioningEnvironment.reset for every episode; the first observation: {model, graph_features, action_mask}."""
+        self.env.reset()
+        obs = self._export(None)
+        return {k: obs[k] for k in ('model', 'graph_features', 'action_mask')}
+
+    def step(self, actions: torch.Tensor, out=None):
+        """One RampJobPartitioningEnvironment.step per episode.  actions: int32 / int64 [B] on this environment's device.  Returns
+        (obs, reward, done, info): fresh tensors, or the tensors of ``out`` (a dict keyed by 'model', 'graph_features',
+        'action_mask', 'reward', 'done'; any subset) written in place.  Does not synchronise when the device tables decide every
+        placement (``prewarm=True``, no model splits its ops unevenly); errors then surface at ``check()`` or the next synchronising
+        call.  Otherwise the host's placer decides the rest, as ``step_device()`` does."""
+        if not isinstance(actions, torch.Tensor):
+            raise TypeError(f'actions must be a torch.Tensor, not {type(actions).__name__}')
+        if actions.dtype not in (torch.int32, torch.int64):
+            raise TypeError(f'actions must be int32 or int64, not {actions.dtype}')
+        if actions.device != self.device:
+            raise ValueError(f'actions are on {actions.device}, the environment on {self.device}')
+        if tuple(actions.shape) != (self.B,):
+            raise ValueError(f'actions have shape {tuple(actions.shape)}, expected ({self.B},)')
+        actions = actions.contiguous()
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        dtype = ACTIONS_INT64 if actions.dtype == torch.int64 else ACTIONS_INT32
+        _engine._check(self._L.ramp_env_ingest(self._h, actions.data_ptr(), dtype, stream))
+        self.env.step_device()                         # decides and steps on the actions the ingest kernel wrote
+        res = self._export(out)
+        obs = {k: res[k] for k in ('model', 'graph_features', 'action_mask')}
+        return obs, res['reward'], res['done'], {}
+
+    def _export(self, out):
+        B, A = self.B, self.n_actions
+        spec = {'model': ((B,), torch.int64), 'graph_features': ((B, N_GRAPH_FEATURES + A), torch.float32),
+                'action_mask': ((B, A), torch.bool), 'reward': ((B,), torch.float64), 'done': ((B,), torch.bool)}
+        out = dict(out or {})
+        unknown = set(out) - set(OUTPUTS)
+        if unknown:
+            raise ValueError(f'unknown outputs {sorted(unknown)}; expected a subset of {list(OUTPUTS)}')
+        res = {}
+        for k, (shape, dtype) in spec.items():
+            t = out.get(k)
+            if t is None:
+                t = torch.empty(shape, dtype=dtype, device=self.device)
+            elif t.dtype != dtype or tuple(t.shape) != shape or t.device != self.device or not t.is_contiguous():
+                raise ValueError(f"out['{k}'] must be a contiguous {dtype} tensor of shape {shape} on {self.device}, "
+                                 f'not {t.dtype} {tuple(t.shape)} on {t.device}')
+            res[k] = t
+        ex = _Export(*[res[k].data_ptr() for k in OUTPUTS])
+        _engine._check(self._L.ramp_env_export(self._h, torch.cuda.current_stream(self.device).cuda_stream, C.byref(ex)))
+        return res

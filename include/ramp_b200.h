@@ -489,8 +489,34 @@ enum { RAMP_AGENT_RANDOM = 0, RAMP_AGENT_SIPML, RAMP_AGENT_ACCEPTABLE_JCT, RAMP_
        RAMP_AGENT_NO_PARALLELISM, RAMP_AGENT_COUNT };
 int ramp_env_set_agents(ramp_engine_t* eng, const int32_t* kind, const int32_t* param);
 int ramp_env_agent_act(ramp_engine_t* eng, uint64_t seed);
-/* also raises what ramp_check_status would (RAMP_ERR_SIM) -- one synchronisation per step for a host-side policy */
+/* also raises what ramp_check_status would (RAMP_ERR_SIM) -- one synchronisation per step for a host-side policy.  After a
+ * ramp_env_ingest it also raises the first action outside the action set (see below). */
 int ramp_env_read(ramp_engine_t* eng, double* reward, uint8_t* done, int32_t* queued_model, float* obs_dynamic, uint8_t* action_mask);
+
+/* ---- the environment's i/o in caller-owned DEVICE memory (e.g. PyTorch CUDA tensors), ordered on the caller's stream.
+ * ramp_env_ingest runs one thread per episode on `stream`: it reads actions [n_episodes] (dtype RAMP_ACTIONS_INT32 / _INT64) and
+ * writes ramp_env_buffers_t.actions, for ramp_env_decide(eng, NULL, ...) to use.  An action of a live episode outside the action set
+ * [0, max_degree] is written as 0 and the first one is kept in a sticky word: the next ramp_env_read, or ramp_env_decide with
+ * need_host_out, raises it as RJPE:314-316 does ("Action a not in action set [...]"), whatever apply_action_mask says.
+ * ramp_env_export writes, on `stream`, RampJobPartitioningObservation's row for every episode (ramp_job_partitioning_observation.py:
+ * 275) and the step's reward and done; any pointer of `out` may be NULL.  Values of finished episodes are what ramp_env_read gives.
+ * Both calls fence the engine stream with events: the caller's stream first waits for the engine's queued work (the last
+ * ramp_env_advance), and the engine stream then waits for the kernel, so neither stream reads a buffer the other still writes and
+ * the caller's allocator may reuse its memory in its own stream order.  ramp_env_set_graph_static uploads the six per-graph
+ * statistics of every model (HOST [n_models][6] float32, observation.py:425-469), which graph_features needs. */
+#define RAMP_ACTIONS_INT32 0
+#define RAMP_ACTIONS_INT64 1
+typedef struct {
+    int64_t* model;               /* [B] model of the queued job (-1 none)                                           */
+    float*   graph_features;      /* [B][17 + n_actions]: obs_dynamic[0:9], graph_static[model][0:6], obs_dynamic[9:11],
+                                     then the action mask as 0.0 / 1.0                                                */
+    uint8_t* action_mask;         /* [B][n_actions] 0 / 1                                                            */
+    double*  reward;              /* [B]                                                                             */
+    uint8_t* done;                /* [B] 0 / 1                                                                       */
+} ramp_env_export_t;
+int ramp_env_set_graph_static(ramp_engine_t* eng, const float* graph_static);
+int ramp_env_ingest(ramp_engine_t* eng, const void* actions, int32_t dtype, void* stream);
+int ramp_env_export(ramp_engine_t* eng, void* stream, const ramp_env_export_t* out);
 
 
 /* ---- the GNN policy forward on the device (SURVEY.md 8f-3): GNNPolicy.forward (ml_models/policies/gnn_policy.py:137-296) =
