@@ -21,6 +21,7 @@
 #include <cmath>
 #include <cstdint>
 #include <cstring>
+#include <map>
 #include <vector>
 
 #include "ramp_owned.cuh"
@@ -358,6 +359,38 @@ __global__ void ramp_trajectory_record_kernel(const TrajArgs a) {
     }
 }
 
+// ramp_policy_forward_device / ramp_policy_backward_device: caller-owned device rows gathered into the staging buffers the host
+// paths upload into, so that every kernel after this one runs on its usual inputs
+struct PolicyIngestArgs {
+    int32_t n, is64, n_models, in_graph, A;
+    int64_t gf_stride;                    // floats from one graph_features row to the next (>= in_graph)
+    const void* model; const float* graph_features; const uint8_t* mask; const float* grad_logits; const float* grad_value;
+    int32_t* model_out; float* gf_out; uint8_t* mask_out;
+    float* gl_out; float* gv_out;         // nullptr: a forward
+    int32_t* n_rows_out;                  // the row count for the gradient kernels, or nullptr
+};
+
+// one thread per (row, column): column k < in_graph gathers a graph feature, k < A a mask byte (and a logit's upstream
+// gradient); column 0 the model, as int32 -- any value outside [0, n_models) becomes -1, so an int64 is never wrapped into range
+__global__ void ramp_policy_ingest_kernel(const PolicyIngestArgs a) {
+    const int W = a.in_graph > a.A ? a.in_graph : a.A;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)a.n * W) return;
+    const int b = (int)(i / W), k = (int)(i - (long long)b * W);
+    if (k < a.in_graph) a.gf_out[(size_t)b * a.in_graph + k] = a.graph_features[(size_t)b * a.gf_stride + k];
+    if (k < a.A) {
+        const size_t o = (size_t)b * a.A + k;
+        a.mask_out[o] = a.mask[o] ? 1 : 0;
+        if (a.gl_out) a.gl_out[o] = a.grad_logits[o];
+    }
+    if (k == 0) {
+        const long long x = a.is64 ? static_cast<const long long*>(a.model)[b] : (long long)static_cast<const int32_t*>(a.model)[b];
+        a.model_out[b] = x >= 0 && x < a.n_models ? (int32_t)x : -1;
+        if (a.gv_out) a.gv_out[b] = a.grad_value[b];
+        if (b == 0 && a.n_rows_out) *a.n_rows_out = a.n;
+    }
+}
+
 }  // namespace ramp
 
 #include "ramp_policy_learn.cuh"
@@ -398,14 +431,20 @@ struct ramp_policy {
     DeviceArray<float> t_obs, t_logp, t_value; DeviceArray<int32_t> t_model, t_action;
     DeviceArray<uint8_t> t_mask, t_done; DeviceArray<double> t_reward;
     // learner (ramp_policy_backward / ramp_ppo_loss_grad / ramp_policy_learn): gradient, Adam's moments and step count, per job type
-    // gradients, norm partials; per-row scratch for `lcap` rows, the head segments for `seg_n` rows
-    bool learner_ready = false, gmodels_ready = false;
-    int32_t adam_parity = 0, lcap = 0, seg_n = 0, seg_count = 0;
-    int64_t seg_total = 0;
+    // gradients, norm partials; per-row scratch for `lcap` rows; the head segments of every row count seen since l_rec was last
+    // allocated (a segment points into l_rec), `segs` those of the current one
+    // states_current: the MeanPool states kept in d_gmodels are those of a whole-batch forward at the current weights
+    bool learner_ready = false, gmodels_ready = false, states_current = false;
+    int32_t adam_parity = 0, lcap = 0;
+    struct SegTable { DeviceArray<Seg> d; int32_t count = 0; int64_t total = 0; };
+    std::map<int32_t, SegTable> seg_tables;
+    const SegTable* segs = nullptr;
     DeviceArray<float> l_grad, l_adam_m, l_adam_v, l_gpart, l_rec, l_row_stats;
     DeviceArray<int32_t> l_n_rows, l_step, l_row_model;
     DeviceArray<double> l_norm_part, l_stats, l_mb_stats;
-    DeviceArray<Seg> l_segs;
+    // the end of the last call that touched the scratch above, the staging or the embeddings (made by the first device-path call;
+    // until then every call keeps its own synchronisation and nothing is recorded)
+    Event ev_done;
     DeviceArray<GradModelDev> d_gmodels;
     // host-input batches of ramp_policy_backward / ramp_ppo_loss_grad
     int32_t hcap = 0;
@@ -477,17 +516,39 @@ int ensure_outputs(ramp_policy* p, int32_t n) {
     return RAMP_OK;
 }
 
+// the job-type table d_models is uploaded by ramp_policy_set_model, once per change
 int launch_embed(ramp_policy* p, cudaStream_t st) {
     for (size_t m = 0; m < p->models.size(); ++m)
         if (!p->models[m].set) return set_error(RAMP_ERR_BAD_ARG, "policy: model %zu was never registered (ramp_policy_set_model)", m);
     if (!p->weights_set) return set_error(RAMP_ERR_BAD_ARG, "policy: no weights (ramp_policy_set_weights)");
-    std::vector<ModelDev> h(p->models.size());
-    for (size_t m = 0; m < h.size(); ++m) h[m] = p->models[m].d;
-    CUDA_TRY(cudaMemcpyAsync(p->d_models.get(), h.data(), sizeof(ModelDev) * h.size(), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaStreamSynchronize(st));                                  // `h` is pageable
-    ramp_gnn_embed_kernel<<<(unsigned)h.size(), 256, 0, st>>>(p->P, p->d_models.get(), p->d_emb.get());
+    ramp_gnn_embed_kernel<<<(unsigned)p->models.size(), 256, 0, st>>>(p->P, p->d_models.get(), p->d_emb.get());
     CUDA_TRY(cudaGetLastError());
     p->emb_valid = true;
+    p->states_current = false;
+    return RAMP_OK;
+}
+
+// the policy's scratch is reused by every call: a call's stream first waits for the end of the previous call, on whatever stream
+// it ran, and the call then marks its own end.  Both are no-ops until a device-path call made the event.
+int fence_in(ramp_policy* p, cudaStream_t st) {
+    if (p->ev_done) CUDA_TRY(cudaStreamWaitEvent(st, p->ev_done.get(), 0));
+    return RAMP_OK;
+}
+
+int fence_out(ramp_policy* p, cudaStream_t st) {
+    if (p->ev_done) CUDA_TRY(cudaEventRecord(p->ev_done.get(), st));
+    return RAMP_OK;
+}
+
+// the f_* staging of the read-out on n rows (ramp_policy_forward / _decide / _forward_device)
+int stage_forward(ramp_policy* p, int32_t n) {
+    if (n <= p->fcap) return RAMP_OK;
+    const ramp_policy_config_t& c = p->P.c;
+    p->fcap = 0;                          // until every buffer has the new size
+    CUDA_TRY(alloc_each(n, p->f_model, p->f_actions, p->f_value, p->f_logp));
+    CUDA_TRY(p->f_gf.alloc((size_t)n * c.in_features_graph));
+    CUDA_TRY(alloc_each((size_t)n * c.n_actions, p->f_mask, p->f_logits));
+    p->fcap = n;
     return RAMP_OK;
 }
 
@@ -501,6 +562,18 @@ int launch_head(ramp_policy* p, const HeadArgs& a, cudaStream_t st) {
     return RAMP_OK;
 }
 
+// the read-out of the n rows staged in f_* on `st`, embedding first when the embeddings are stale; logits / value / logp may be
+// nullptr
+int launch_forward(ramp_policy* p, cudaStream_t st, int32_t n, int32_t sample, uint64_t seed, float* logits, float* value, float* logp) {
+    int rc;
+    if (!p->emb_valid && (rc = launch_embed(p, st)) != RAMP_OK) return rc;
+    HeadArgs a{};
+    a.n = n; a.graph_features = p->f_gf.get(); a.model = p->f_model.get(); a.mask = p->f_mask.get(); a.emb = p->d_emb.get(); a.graph_static = p->d_gstatic.get();
+    a.logits = logits; a.value = value; a.logp = logp; a.actions = p->f_actions.get();
+    a.sample = sample; a.seed = seed;
+    return launch_head(p, a, st);
+}
+
 // the read-out on host inputs (ramp_policy_forward / ramp_policy_decide), in buffers of its own: what the last act left for
 // ramp_policy_read and the trajectory stays as it was
 int head_on_host(ramp_policy* p, int32_t n, const int32_t* model, const float* graph_features, const uint8_t* action_mask, int32_t sample,
@@ -510,22 +583,11 @@ int head_on_host(ramp_policy* p, int32_t n, const int32_t* model, const float* g
     const ramp_policy_config_t& c = p->P.c;
     CUDA_TRY(cudaSetDevice(p->device));
     int rc;
-    if (!p->emb_valid && (rc = launch_embed(p, 0)) != RAMP_OK) return rc;
-    if (n > p->fcap) {
-        p->fcap = 0;                      // until every buffer has the new size
-        CUDA_TRY(alloc_each(n, p->f_model, p->f_actions, p->f_value, p->f_logp));
-        CUDA_TRY(p->f_gf.alloc((size_t)n * c.in_features_graph));
-        CUDA_TRY(alloc_each((size_t)n * c.n_actions, p->f_mask, p->f_logits));
-        p->fcap = n;
-    }
+    if ((rc = fence_in(p, 0)) != RAMP_OK || (rc = stage_forward(p, n)) != RAMP_OK) return rc;
     CUDA_TRY(cudaMemcpy(p->f_model.get(), model, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(p->f_gf.get(), graph_features, sizeof(float) * (size_t)n * c.in_features_graph, cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(p->f_mask.get(), action_mask, (size_t)n * c.n_actions, cudaMemcpyHostToDevice));
-    HeadArgs a{};
-    a.n = n; a.graph_features = p->f_gf.get(); a.model = p->f_model.get(); a.mask = p->f_mask.get(); a.emb = p->d_emb.get(); a.graph_static = p->d_gstatic.get();
-    a.logits = p->f_logits.get(); a.value = p->f_value.get(); a.logp = p->f_logp.get(); a.actions = p->f_actions.get();
-    a.sample = sample; a.seed = seed;
-    if ((rc = launch_head(p, a, 0)) != RAMP_OK) return rc;
+    if ((rc = launch_forward(p, 0, n, sample, seed, p->f_logits.get(), p->f_value.get(), p->f_logp.get())) != RAMP_OK) return rc;
     CUDA_TRY(cudaStreamSynchronize(0));
     if (logits_out) CUDA_TRY(cudaMemcpy(logits_out, p->f_logits.get(), sizeof(float) * (size_t)n * c.n_actions, cudaMemcpyDeviceToHost));
     if (value_out) CUDA_TRY(cudaMemcpy(value_out, p->f_value.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
@@ -554,7 +616,6 @@ int ensure_learner(ramp_policy* p) {
     CUDA_TRY(p->l_step.alloc(2));
     CUDA_TRY(p->l_norm_part.alloc(LRN_GRID));
     CUDA_TRY(p->l_stats.alloc(RAMP_PPO_STATS_LEN));
-    CUDA_TRY(p->l_segs.alloc(HEAD_SEGS));
     CUDA_TRY(p->d_gmodels.alloc(p->P.c.n_models));
     CUDA_TRY(cudaMemset(p->l_adam_m.get(), 0, sizeof(float) * nw));
     CUDA_TRY(cudaMemset(p->l_adam_v.get(), 0, sizeof(float) * nw));
@@ -565,7 +626,7 @@ int ensure_learner(ramp_policy* p) {
 }
 
 // every job type's forward states and records for the embedding backward, sized by its graph
-int ensure_gmodels(ramp_policy* p) {
+int ensure_gmodels(ramp_policy* p, cudaStream_t st) {
     if (p->gmodels_ready) return RAMP_OK;
     const ramp_policy_config_t& c = p->P.c;
     const GnnDims D = gnn_dims(c);
@@ -594,35 +655,42 @@ int ensure_gmodels(ramp_policy* p) {
         }
         h[m] = hm.g;
     }
-    CUDA_TRY(cudaMemcpy(p->d_gmodels.get(), h.data(), sizeof(GradModelDev) * h.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpyAsync(p->d_gmodels.get(), h.data(), sizeof(GradModelDev) * h.size(), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));                                  // `h` is pageable
     p->gmodels_ready = true;
     return RAMP_OK;
 }
 
-// per-row scratch for minibatches of n rows, and the head segments summing exactly n rows
-int ensure_rows(ramp_policy* p, int32_t n) {
+// per-row scratch for minibatches of n rows, and the head segments summing exactly n rows: uploaded on `st` the first time n is
+// seen, so a PPO loop whose last minibatch is short does not synchronise every time the row count alternates
+int ensure_rows(ramp_policy* p, int32_t n, cudaStream_t st) {
     if (n > p->lcap) {
         p->lcap = 0;
-        p->seg_n = 0;
+        p->segs = nullptr;
+        p->seg_tables.clear();
         CUDA_TRY(p->l_rec.alloc((size_t)n * head_rec(p->P.c).stride));
         CUDA_TRY(p->l_row_stats.alloc((size_t)n * RS_N));
         CUDA_TRY(p->l_row_model.alloc(n));
         p->lcap = n;
     }
-    if (n != p->seg_n) {
+    auto it = p->seg_tables.find(n);
+    if (it == p->seg_tables.end()) {
         Seg s[HEAD_SEGS];
-        p->seg_count = head_segs(p->P, p->l_rec.get(), n, s);
-        p->seg_total = 0;
-        for (int k = 0; k < p->seg_count; ++k) p->seg_total += seg_size(s[k]);
-        CUDA_TRY(cudaMemcpy(p->l_segs.get(), s, sizeof(s), cudaMemcpyHostToDevice));
-        p->seg_n = n;
+        ramp_policy::SegTable t;
+        t.count = head_segs(p->P, p->l_rec.get(), n, s);
+        for (int k = 0; k < t.count; ++k) t.total += seg_size(s[k]);
+        CUDA_TRY(t.d.alloc(HEAD_SEGS));
+        CUDA_TRY(cudaMemcpyAsync(t.d.get(), s, sizeof(s), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaStreamSynchronize(st));                              // `s` is pageable
+        it = p->seg_tables.emplace(n, std::move(t)).first;
     }
+    p->segs = &it->second;
     return RAMP_OK;
 }
 
 int prepare_learner(ramp_policy* p, cudaStream_t st) {
     int rc;
-    if ((rc = ensure_learner(p)) != RAMP_OK || (rc = ensure_gmodels(p)) != RAMP_OK) return rc;
+    if ((rc = ensure_learner(p)) != RAMP_OK || (rc = ensure_gmodels(p, st)) != RAMP_OK) return rc;
     if (!p->emb_valid && (rc = launch_embed(p, st)) != RAMP_OK) return rc;
     return RAMP_OK;
 }
@@ -634,6 +702,7 @@ int launch_states(ramp_policy* p, cudaStream_t st, const int32_t* n_rows, int32_
     eg.n_rows = n_rows; eg.start = start; eg.emb = emb;
     ramp_gnn_embed_grad_kernel<EMB_FORWARD><<<p->P.c.n_models, 256, 0, st>>>(p->P, p->d_models.get(), p->d_gmodels.get(), eg);
     CUDA_TRY(cudaGetLastError());
+    p->states_current = n_rows == nullptr;                         // a learn call's minibatch past the batch's end keeps none
     return RAMP_OK;
 }
 
@@ -643,9 +712,9 @@ int launch_grad(ramp_policy* p, GradArgs ga, cudaStream_t st) {
     ga.rec = p->l_rec.get(); ga.row_model = p->l_row_model.get(); ga.row_stats = p->l_row_stats.get();
     ga.emb = p->d_emb.get(); ga.graph_static = p->d_gstatic.get();
     ramp_policy_head_grad_kernel<<<(ga.mb + LRN_WARPS - 1) / LRN_WARPS, LRN_WARPS * 32, 0, st>>>(p->P, ga);
-    int64_t grid = (p->seg_total + 255) / 256;
+    int64_t grid = (p->segs->total + 255) / 256;
     if (grid > 4 * p->sm_count) grid = 4 * p->sm_count;
-    ramp_policy_head_reduce_kernel<<<(unsigned)grid, 256, 0, st>>>(p->P, p->l_segs.get(), p->seg_count, p->seg_total, p->l_grad.get());
+    ramp_policy_head_reduce_kernel<<<(unsigned)grid, 256, 0, st>>>(p->P, p->segs->d.get(), p->segs->count, p->segs->total, p->l_grad.get());
     EmbGradArgs eg{};
     eg.rec = p->l_rec.get(); eg.row_model = p->l_row_model.get(); eg.rows = ga.mb; eg.gpart = p->l_gpart.get(); eg.n_gnn = gnn_weight_count(p);
     ramp_gnn_embed_grad_kernel<EMB_BACKWARD><<<p->P.c.n_models, 256, 0, st>>>(p->P, p->d_models.get(), p->d_gmodels.get(), eg);
@@ -668,23 +737,29 @@ void ppo_terms(GradArgs& ga, const ramp_ppo_config_t& cfg) {
     ga.ent_coeff = (float)cfg.entropy_coeff; ga.kl_coeff = (float)cfg.kl_coeff;
 }
 
+// the h_* staging of a batch of n rows (ramp_policy_backward / the loss calls / ramp_policy_backward_device)
+int stage_host_batch(ramp_policy* p, int32_t n) {
+    if (n <= p->hcap) return RAMP_OK;
+    const ramp_policy_config_t& c = p->P.c;
+    p->hcap = 0;
+    CUDA_TRY(alloc_each(n, p->h_model, p->h_action, p->h_gv, p->h_adv, p->h_vt));
+    CUDA_TRY(p->h_gf.alloc((size_t)n * c.in_features_graph));
+    CUDA_TRY(alloc_each((size_t)n * (size_t)c.n_actions, p->h_gl, p->h_old, p->h_mask));
+    p->hcap = n;
+    return RAMP_OK;
+}
+
 // the host inputs of ramp_policy_backward / ramp_ppo_loss_grad on the device (any pointer may be NULL: not copied)
 int upload_host_batch(ramp_policy* p, int32_t n, const int32_t* model, const float* gf, const uint8_t* mask, const float* gl,
                       const float* gv, const int32_t* action, const float* old_logits, const float* adv, const float* vt) {
     const ramp_policy_config_t& c = p->P.c;
     const size_t A = c.n_actions;
-    if (n > p->hcap) {
-        p->hcap = 0;
-        CUDA_TRY(alloc_each(n, p->h_model, p->h_action, p->h_gv, p->h_adv, p->h_vt));
-        CUDA_TRY(p->h_gf.alloc((size_t)n * c.in_features_graph));
-        CUDA_TRY(alloc_each((size_t)n * A, p->h_gl, p->h_old, p->h_mask));
-        p->hcap = n;
-    }
+    int rc = stage_host_batch(p, n);
+    if (rc != RAMP_OK) return rc;
     auto put = [&](void* dst, const void* src, size_t bytes) -> int {
         if (src) CUDA_TRY(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
         return RAMP_OK;
     };
-    int rc;
     if ((rc = put(p->h_model.get(), model, 4 * (size_t)n)) || (rc = put(p->h_gf.get(), gf, 4 * (size_t)n * c.in_features_graph)) ||
         (rc = put(p->h_mask.get(), mask, (size_t)n * A)) || (rc = put(p->h_gl.get(), gl, 4 * (size_t)n * A)) ||
         (rc = put(p->h_gv.get(), gv, 4 * (size_t)n)) || (rc = put(p->h_action.get(), action, 4 * (size_t)n)) ||
@@ -713,6 +788,51 @@ GradArgs host_batch_args(ramp_policy* p, int32_t n) {
     ga.mb = n; ga.start = 0; ga.n_rows = p->l_n_rows.get() + 1;
     ga.graph_features = p->h_gf.get(); ga.model = p->h_model.get(); ga.mask = p->h_mask.get();
     return ga;
+}
+
+// the gradient of the n rows staged in h_* (with their upstream gradients h_gl, h_gv) into l_grad, on `st`; the MeanPool states
+// are run again unless `reuse_states` and the kept ones are those of the current weights
+int launch_backward(ramp_policy* p, cudaStream_t st, int32_t n, bool reuse_states) {
+    GradArgs ga = host_batch_args(p, n);
+    ga.grad_logits = p->h_gl.get(); ga.grad_value = p->h_gv.get();
+    int rc;
+    if (!(reuse_states && p->emb_valid && p->states_current) && (rc = launch_states(p, st, nullptr, 0, nullptr)) != RAMP_OK) return rc;
+    return launch_grad(p, ga, st);
+}
+
+// the caller's device rows into the staging on `st` (ramp_policy_forward_device / _backward_device): model, graph features,
+// mask into f_* (gl == nullptr) or h_* with the upstream gradients and the row count
+int launch_ingest(ramp_policy* p, cudaStream_t st, int32_t n, const void* model, int32_t model_dtype, const float* graph_features,
+                  int64_t gf_stride, const uint8_t* mask, const float* gl, const float* gv) {
+    const ramp_policy_config_t& c = p->P.c;
+    PolicyIngestArgs a{};
+    a.n = n; a.is64 = model_dtype == RAMP_MODEL_INT64; a.n_models = c.n_models; a.in_graph = c.in_features_graph; a.A = c.n_actions;
+    a.gf_stride = gf_stride; a.model = model; a.graph_features = graph_features; a.mask = mask; a.grad_logits = gl; a.grad_value = gv;
+    if (gl) {
+        a.model_out = p->h_model.get(); a.gf_out = p->h_gf.get(); a.mask_out = p->h_mask.get();
+        a.gl_out = p->h_gl.get(); a.gv_out = p->h_gv.get(); a.n_rows_out = p->l_n_rows.get() + 1;
+    } else {
+        a.model_out = p->f_model.get(); a.gf_out = p->f_gf.get(); a.mask_out = p->f_mask.get();
+    }
+    const long long threads = (long long)n * std::max(c.in_features_graph, c.n_actions);
+    ramp_policy_ingest_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
+}
+
+// the checks every device-path call makes; creates the fencing event on the first one
+int device_call_ready(ramp_policy* p, int32_t n, const void* model, int32_t model_dtype, const float* graph_features, int64_t gf_stride,
+                      const uint8_t* mask) {
+    if (!model || !graph_features || !mask) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (model_dtype != RAMP_MODEL_INT32 && model_dtype != RAMP_MODEL_INT64)
+        return set_error(RAMP_ERR_BAD_ARG, "policy: model dtype %d is neither RAMP_MODEL_INT32 nor RAMP_MODEL_INT64", model_dtype);
+    if (gf_stride < p->P.c.in_features_graph)
+        return set_error(RAMP_ERR_BAD_ARG, "policy: graph_features row stride %lld is below in_features_graph (%d)", (long long)gf_stride,
+                         p->P.c.in_features_graph);
+    if (n < 0) return set_error(RAMP_ERR_BAD_ARG, "policy: %d rows", n);
+    CUDA_TRY(cudaSetDevice(p->device));
+    if (!p->ev_done) CUDA_TRY(create(p->ev_done, cudaEventDisableTiming));
+    return RAMP_OK;
 }
 
 int check_impala_config(const ramp_impala_config_t* cfg) {
@@ -892,6 +1012,8 @@ int ramp_policy_set_model(ramp_policy_t* p, int32_t model, int32_t n_nodes, int3
     CUDA_TRY(cudaMemcpy(p->d_gstatic.get() + (size_t)model * 6, graph_static, sizeof(float) * 6, cudaMemcpyHostToDevice));
     hm.g = g;
     hm.d = d;
+    CUDA_TRY(cudaMemcpy(p->d_models.get() + model, &d, sizeof(ModelDev), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaDeviceSynchronize());                                    // a kernel on any stream may read the table next
     hm.set = true;
     p->emb_valid = false;
     return RAMP_OK;
@@ -900,8 +1022,8 @@ int ramp_policy_set_model(ramp_policy_t* p, int32_t model, int32_t n_nodes, int3
 int ramp_policy_embed(ramp_policy_t* p, float* embeddings_out) {
     if (!p) return set_error(RAMP_ERR_BAD_ARG, "null policy");
     CUDA_TRY(cudaSetDevice(p->device));
-    int rc = launch_embed(p, 0);
-    if (rc != RAMP_OK) return rc;
+    int rc;
+    if ((rc = fence_in(p, 0)) != RAMP_OK || (rc = launch_embed(p, 0)) != RAMP_OK) return rc;
     CUDA_TRY(cudaStreamSynchronize(0));
     if (embeddings_out)
         CUDA_TRY(cudaMemcpy(embeddings_out, p->d_emb.get(), sizeof(float) * (size_t)p->P.c.n_models * p->P.c.out_features_node, cudaMemcpyDeviceToHost));
@@ -931,13 +1053,14 @@ int ramp_policy_act(ramp_policy_t* p, ramp_engine_t* eng, int32_t sample, uint64
     CUDA_TRY(cudaSetDevice(p->device));
     cudaStream_t st = ramp_internal_stream(eng);
     int launches = 1;
+    if ((rc = fence_in(p, st)) != RAMP_OK) return rc;
     if (!p->emb_valid) { if ((rc = launch_embed(p, st)) != RAMP_OK) return rc; ++launches; }
     if ((rc = ensure_outputs(p, eb.n_episodes)) != RAMP_OK) return rc;
     HeadArgs a{};
     a.n = eb.n_episodes; a.obs_dyn = eb.obs_dynamic; a.graph_static = p->d_gstatic.get(); a.model = eb.queued_model; a.done = eb.done;
     a.mask = eb.action_mask; a.emb = p->d_emb.get(); a.logits = p->d_logits.get(); a.value = p->d_value.get(); a.logp = p->d_logp.get(); a.actions = eb.actions;
     a.sample = sample; a.seed = seed ^ (0x9E3779B97F4A7C15ull * (++p->act_calls));
-    if ((rc = launch_head(p, a, st)) != RAMP_OK) return rc;
+    if ((rc = launch_head(p, a, st)) != RAMP_OK || (rc = fence_out(p, st)) != RAMP_OK) return rc;
     p->act_n = eb.n_episodes;
     ramp_internal_count_launches(eng, launches);
     return RAMP_OK;
@@ -1045,15 +1168,64 @@ int ramp_policy_backward(ramp_policy_t* p, int32_t n, const int32_t* model, cons
     if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "policy: backward of %d rows", n);
     CUDA_TRY(cudaSetDevice(p->device));
     int rc;
-    if ((rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n)) ||
+    if ((rc = fence_in(p, 0)) || (rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n, 0)) ||
         (rc = upload_host_batch(p, n, model, graph_features, action_mask, grad_logits, grad_value, nullptr, nullptr, nullptr, nullptr)))
         return rc;
-    GradArgs ga = host_batch_args(p, n);
-    ga.grad_logits = p->h_gl.get(); ga.grad_value = p->h_gv.get();
-    if ((rc = launch_states(p, 0, nullptr, 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, 0)) != RAMP_OK) return rc;
+    if ((rc = launch_backward(p, 0, n, false)) != RAMP_OK) return rc;
     CUDA_TRY(cudaStreamSynchronize(0));
     CUDA_TRY(cudaMemcpy(grad_weights_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
     return RAMP_OK;
+}
+
+int ramp_policy_set_weights_device(ramp_policy_t* p, const float* weights, int64_t n, void* stream) {
+    if (!p || !weights) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (n != p->n_weights) return set_error(RAMP_ERR_BAD_ARG, "policy: %lld weights given, the configuration has %lld", (long long)n, (long long)p->n_weights);
+    CUDA_TRY(cudaSetDevice(p->device));
+    if (!p->ev_done) CUDA_TRY(create(p->ev_done, cudaEventDisableTiming));
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc;
+    if ((rc = fence_in(p, st)) != RAMP_OK) return rc;                    // a queued call may still read the old set
+    CUDA_TRY(cudaMemcpyAsync(p->d_w.get(), weights, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
+    p->weights_set = true;
+    p->emb_valid = false;
+    return fence_out(p, st);
+}
+
+int ramp_policy_forward_device(ramp_policy_t* p, void* stream, int32_t n, const void* model, int32_t model_dtype,
+                               const float* graph_features, int64_t graph_features_stride, const uint8_t* action_mask,
+                               float* logits_out, float* value_out) {
+    if (!p || !logits_out || !value_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = device_call_ready(p, n, model, model_dtype, graph_features, graph_features_stride, action_mask);
+    if (rc != RAMP_OK || n == 0) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = stage_forward(p, n)) != RAMP_OK || (rc = fence_in(p, st)) != RAMP_OK ||
+        (rc = launch_ingest(p, st, n, model, model_dtype, graph_features, graph_features_stride, action_mask, nullptr, nullptr)) != RAMP_OK)
+        return rc;
+    // once a backward has set up the learner, stale embeddings are remade by the gradient kernel's forward instance: the same
+    // bits, and its kept states spare the next backward a second pass over the MeanPool rounds (the fused learners do the same)
+    if (!p->emb_valid && p->learner_ready && p->gmodels_ready) {
+        if ((rc = launch_states(p, st, nullptr, 0, p->d_emb.get())) != RAMP_OK) return rc;
+        p->emb_valid = true;
+    }
+    if ((rc = launch_forward(p, st, n, 0, 0, logits_out, value_out, nullptr)) != RAMP_OK) return rc;
+    return fence_out(p, st);
+}
+
+int ramp_policy_backward_device(ramp_policy_t* p, void* stream, int32_t n, const void* model, int32_t model_dtype,
+                                const float* graph_features, int64_t graph_features_stride, const uint8_t* action_mask,
+                                const float* grad_logits, const float* grad_value, float* grad_weights_out) {
+    if (!p || !grad_logits || !grad_value || !grad_weights_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = device_call_ready(p, n, model, model_dtype, graph_features, graph_features_stride, action_mask);
+    if (rc != RAMP_OK) return rc;
+    if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "policy: backward of %d rows", n);
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = fence_in(p, st)) != RAMP_OK || (rc = prepare_learner(p, st)) != RAMP_OK || (rc = ensure_rows(p, n, st)) != RAMP_OK ||
+        (rc = stage_host_batch(p, n)) != RAMP_OK ||
+        (rc = launch_ingest(p, st, n, model, model_dtype, graph_features, graph_features_stride, action_mask, grad_logits, grad_value)) != RAMP_OK ||
+        (rc = launch_backward(p, st, n, true)) != RAMP_OK)
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(grad_weights_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToDevice, st));
+    return fence_out(p, st);
 }
 
 int ramp_ppo_loss_grad(ramp_policy_t* p, const ramp_ppo_config_t* cfg, int32_t n, const int32_t* model, const float* graph_features,
@@ -1065,7 +1237,7 @@ int ramp_ppo_loss_grad(ramp_policy_t* p, const ramp_ppo_config_t* cfg, int32_t n
     if (rc != RAMP_OK) return rc;
     if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "ppo: loss of %d rows", n);
     CUDA_TRY(cudaSetDevice(p->device));
-    if ((rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n)) ||
+    if ((rc = fence_in(p, 0)) || (rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n, 0)) ||
         (rc = upload_host_batch(p, n, model, graph_features, action_mask, nullptr, nullptr, action, old_logits, advantage, value_target)))
         return rc;
     GradArgs ga = host_batch_args(p, n);
@@ -1094,7 +1266,7 @@ int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, con
     CUDA_TRY(cudaSetDevice(p->device));
     cudaStream_t st = ramp_internal_stream(eng);
     const int32_t B = eb.n_episodes, rows = n_steps * B, mb = cfg->sgd_minibatch_size, n_mb = (rows + mb - 1) / mb;
-    if ((rc = prepare_learner(p, st)) || (rc = ensure_rows(p, mb)) || (rc = ensure_batch(p, rows))) return rc;
+    if ((rc = fence_in(p, st)) || (rc = prepare_learner(p, st)) || (rc = ensure_rows(p, mb, st)) || (rc = ensure_batch(p, rows))) return rc;
     if (B > p->boot_cap) {
         p->boot_cap = 0;
         CUDA_TRY(alloc_each(B, p->l_boot, p->l_boot_act));
@@ -1228,7 +1400,7 @@ int ramp_impala_loss_grad(ramp_policy_t* p, const ramp_impala_config_t* cfg, int
         return set_error(RAMP_ERR_BAD_ARG, "impala: loss of %d fragments of %d rows", n_fragments, fragment_length);
     const int32_t n = n_fragments * fragment_length;
     CUDA_TRY(cudaSetDevice(p->device));
-    if ((rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n)) || (rc = ensure_impala(p, n, 1)) ||
+    if ((rc = fence_in(p, 0)) || (rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n, 0)) || (rc = ensure_impala(p, n, 1)) ||
         (rc = upload_host_batch(p, n, model, graph_features, action_mask, nullptr, nullptr, action, nullptr, nullptr, nullptr)))
         return rc;
     CUDA_TRY(cudaMemcpy(p->i_blogp.get(), behaviour_logp, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
@@ -1269,7 +1441,7 @@ int ramp_policy_learn_impala(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_ste
     cudaStream_t st = ramp_internal_stream(eng);
     const int32_t B = eb.n_episodes, n_frag = (n_steps / L) * B, R = n_steps * B;
     const int32_t F = std::min(cfg->train_batch_size / L, n_frag), mb = F * L, n_sgd = (n_frag + F - 1) / F;
-    if ((rc = prepare_learner(p, st)) || (rc = ensure_rows(p, mb)) || (rc = ensure_impala(p, R, n_sgd))) return rc;
+    if ((rc = fence_in(p, st)) || (rc = prepare_learner(p, st)) || (rc = ensure_rows(p, mb, st)) || (rc = ensure_impala(p, R, n_sgd))) return rc;
     // 1. the fragment rows, fragment-major
     ImpalaBatchArgs ba{};
     ba.T = n_steps; ba.B = B; ba.A = c.n_actions; ba.L = L; ba.n_models = c.n_models;
@@ -1337,7 +1509,7 @@ int ramp_pg_loss_grad(ramp_policy_t* p, const ramp_pg_config_t* cfg, int32_t n, 
     if (rc != RAMP_OK) return rc;
     if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "pg: loss of %d rows", n);
     CUDA_TRY(cudaSetDevice(p->device));
-    if ((rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n)) ||
+    if ((rc = fence_in(p, 0)) || (rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n, 0)) ||
         (rc = upload_host_batch(p, n, model, graph_features, action_mask, nullptr, nullptr, action, nullptr, advantage, nullptr)))
         return rc;
     GradArgs ga = host_batch_args(p, n);
@@ -1367,7 +1539,7 @@ int ramp_policy_learn_pg(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, 
     CUDA_TRY(cudaSetDevice(p->device));
     cudaStream_t st = ramp_internal_stream(eng);
     const int32_t B = eb.n_episodes, rows = n_steps * B;
-    if ((rc = prepare_learner(p, st)) || (rc = ensure_rows(p, rows)) || (rc = ensure_batch(p, rows))) return rc;
+    if ((rc = fence_in(p, st)) || (rc = prepare_learner(p, st)) || (rc = ensure_rows(p, rows, st)) || (rc = ensure_batch(p, rows))) return rc;
     // 1. the discounted returns (ramp_ppo_gae_kernel without values: lambda 1, V = 0, a 0 bootstrap), the live rows t-major
     GaeArgs ge{};
     ge.T = n_steps; ge.B = B; ge.A = c.n_actions; ge.n_models = c.n_models; ge.standardize = 0;

@@ -175,7 +175,8 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_impala_vtrace_read', 'ramp_es_create', 'ramp_es_destroy', 'ramp_es_round_begin', 'ramp_es_act',
                     'ramp_es_round_end', 'ramp_es_step', 'ramp_es_update', 'ramp_es_read', 'ramp_es_act_read', 'ramp_es_state',
                     'ramp_es_reset', 'ramp_pg_loss_grad', 'ramp_policy_learn_pg',
-                    'ramp_env_set_graph_static', 'ramp_env_ingest', 'ramp_env_export']
+                    'ramp_env_set_graph_static', 'ramp_env_ingest', 'ramp_env_export',
+                    'ramp_policy_set_weights_device', 'ramp_policy_forward_device', 'ramp_policy_backward_device']
 
 
 def device_bytes():

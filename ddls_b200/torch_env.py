@@ -6,7 +6,8 @@ RampJobPartitioningObservation's layout, ``action_mask`` [B, |A|] bool), ``rewar
 Every kernel that touches a tensor runs on ``torch.cuda.current_stream()`` (include/ramp_b200.h: ramp_env_ingest / ramp_env_export),
 so a torch policy feeds the environment and reads it back at device speed, and the caching allocator never needs ``record_stream``.
 What the policy observes of a job type whatever the cluster holds -- node and edge features, edge endpoints, the six per-graph
-statistics -- is ``static``, uploaded once per job type.  This is the only module of the package that imports torch."""
+statistics -- is ``static``, uploaded once per job type.  With ``torch_policy`` it is one of the two modules of the package that
+import torch."""
 from __future__ import annotations
 
 import ctypes as C

@@ -607,6 +607,35 @@ int ramp_policy_get_weights(ramp_policy_t* p, float* out);
 int ramp_policy_backward(ramp_policy_t* p, int32_t n, const int32_t* model, const float* graph_features, const uint8_t* action_mask,
                          const float* grad_logits, const float* grad_value, float* grad_weights_out);
 
+/* ---- the policy's forward and backward on caller-owned DEVICE memory (e.g. PyTorch CUDA tensors), ordered on the caller's stream,
+ * for a training loop written outside the library.  None of the three synchronises the host once every buffer has grown to its
+ * size and each row count has been seen once: growing a buffer synchronises once, and the first backward of a new row count n
+ * allocates and uploads that count's head-gradient segment table (a small table per distinct n, kept until the per-row scratch
+ * grows past its largest n) and synchronises the stream once.  A loop whose batch sizes vary pays this once per size.  The policy's staging,
+ * per-row records, gradient and embeddings are reused by every call: each call's stream first waits for an event recorded at the
+ * end of the policy's previous call, on whatever stream that ran, host-input calls included, and records it again when done, so
+ * calls alternating between streams are ordered without a device synchronisation.
+ * ramp_policy_set_weights_device: a device-to-device copy of weights [ramp_policy_weight_count] into the policy's blob, enqueued on
+ * `stream`; the embeddings become stale.
+ * ramp_policy_forward_device: ramp_policy_forward's read-out of n rows (the job types embedded first on `stream` when stale):
+ * model [n] (model_dtype RAMP_MODEL_INT32 / _INT64; any value outside [0, n_models) -- a finished episode's -1, an int64 that
+ * int32 would wrap -- makes its row dead: logits and value 0), graph_features rows graph_features_stride floats apart of which the
+ * first in_features_graph are read (the environment's [n][17 + n_actions] rows in place), action_mask [n][n_actions] bytes (0 / non-0)
+ * -> logits_out [n][n_actions], value_out [n], the bits ramp_policy_forward gives for the same inputs.
+ * ramp_policy_backward_device: ramp_policy_backward's gradient for the same inputs and grad_logits [n][n_actions], grad_value [n]
+ * -> grad_weights_out [ramp_policy_weight_count]: ramp_policy_backward's bits.  A dead row passes no gradient.  Once a backward has
+ * run, a forward that finds the embeddings stale remakes them with the gradient kernel's forward instance (the same bits) and
+ * keeps its MeanPool states, and the next backward at the same weights reuses them instead of running the rounds again. */
+#define RAMP_MODEL_INT32 0
+#define RAMP_MODEL_INT64 1
+int ramp_policy_set_weights_device(ramp_policy_t* p, const float* weights, int64_t n, void* stream);
+int ramp_policy_forward_device(ramp_policy_t* p, void* stream, int32_t n, const void* model, int32_t model_dtype,
+                               const float* graph_features, int64_t graph_features_stride, const uint8_t* action_mask,
+                               float* logits_out, float* value_out);
+int ramp_policy_backward_device(ramp_policy_t* p, void* stream, int32_t n, const void* model, int32_t model_dtype,
+                                const float* graph_features, int64_t graph_features_stride, const uint8_t* action_mask,
+                                const float* grad_logits, const float* grad_value, float* grad_weights_out);
+
 /* PPO's settings (RLlib PPOConfig names; scripts/ramp_job_partitioning_configs/algo/ppo.yaml holds the reference's values) */
 typedef struct {
     uint64_t seed;                        /* minibatch shuffles: pass p draws its permutation from splitmix64 keyed by (seed, p)   */
