@@ -85,8 +85,11 @@ struct TraceArrays {
 
 // The buffers of one step's lookaheads when steps overlap (ramp_step_device): the speculative plan and bucket run on the plan
 // stream, the thread kernel on the window's stream, and the commit, the repair launch and the step kernel on the engine stream.
-// ev_consumed marks the end of the step kernel that used the window last; the window's next plan waits for it.
-constexpr int N_WINDOWS = 4;
+// ev_consumed marks the end of the repair launch that used the window last, the last reader of its lists; the window's next
+// plan waits for it.  A window holds only its lists (about 0.56 KB per episode); the thread kernel's HBM slabs are one pool
+// shared by every launch.  N_WINDOWS (DESIGN.md §4): enough windows that planning a step never waits for a window while the
+// SMs have free thread-kernel slots.
+constexpr int N_WINDOWS = 16;
 struct LookaheadWindow {
     Stream stream;
     Event ev_planned, ev_end, ev_consumed;
@@ -95,7 +98,6 @@ struct LookaheadWindow {
     DeviceArray<ChunkDesc> chunks;                  // [B]
     DeviceArray<int32_t> rank, tcount, tbase;       // [B], [max_templates + 1] x 2
     DeviceArray<SpecRecord> rec;                    // [B]
-    DeviceArray<unsigned char> scratch;             // the thread kernel's slabs, [res_grid][res_scratch_stride]
 };
 
 }  // namespace
@@ -168,8 +170,10 @@ struct ramp_engine {
     int n_resident = 0, n_nonresident = 0;
     int32_t res_tmpl_cap = 0, res_n_cap = 0, res_spill_ops = 0, res_spill_deps = 0;
     int res_grid = 0;
+    int res_per_sm = 0;                    // thread-kernel CTAs one SM holds at once
     size_t res_smem = 0;
-    DeviceArray<unsigned char> d_res_scratch;
+    DeviceArray<unsigned char> d_res_scratch;   // the slab pool: [sm_count][res_per_sm][res_scratch_stride], shared by every launch
+    DeviceArray<uint32_t> d_res_slab_mask;      // [sm_count]: the slabs held by running CTAs (ramp_lookahead_thread.cuh)
     uint64_t res_scratch_stride = 0;
     DeviceArray<WorkItem> d_items_res;
     DeviceArray<WorkItem> d_chunk_items;   // [B][32]
@@ -472,25 +476,41 @@ int identity_quotient(const ramp_lowered_job_t* j, ramp_quotient_t* q) {
 
 // shared memory / grid / HBM slabs of the thread-per-lookahead kernel for the resident templates registered so far
 int ensure_thread_scratch(ramp_engine* e) {
-    const size_t smem = thread_smem_bytes(e->res_tmpl_cap, e->res_n_cap);
-    if (smem > 220 * 1024) return set_error(RAMP_ERR_CAPACITY, "resident templates need %zu B of shared memory (max 220 KiB)", smem);
+    const size_t need = thread_smem_bytes(e->res_tmpl_cap, e->res_n_cap);
+    if (need > 220 * 1024) return set_error(RAMP_ERR_CAPACITY, "resident templates need %zu B of shared memory (max 220 KiB)", need);
+    // At most 2 CTAs per SM, whichever launches they belong to: a CTA asks for at least the shared memory that keeps a third
+    // one off the SM.  Two CTAs are four warps, one per scheduler of the SM; with a third, two sim warps share a scheduler,
+    // and on config 3 the overlapped step got slower (DESIGN.md §4).
+    int sm_smem = 0, blk_reserved = 0;
+    CUDA_TRY(cudaDeviceGetAttribute(&sm_smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, e->cfg.device));
+    CUDA_TRY(cudaDeviceGetAttribute(&blk_reserved, cudaDevAttrReservedSharedMemoryPerBlock, e->cfg.device));
+    cudaFuncAttributes fa{};
+    CUDA_TRY(cudaFuncGetAttributes(&fa, ramp_lookahead_thread_kernel));
+    const size_t three = (size_t)sm_smem / 3 - fa.sharedSizeBytes - (size_t)blk_reserved;   // the most at which 3 CTAs fit
+    const size_t smem = std::max(need, align_up((uint64_t)three + 1, 128));
     if (smem != e->res_smem || e->res_grid == 0) {
         CUDA_TRY(reserve_dynamic_smem((const void*)ramp_lookahead_thread_kernel, smem));
         CUDA_TRY(cudaFuncSetAttribute(ramp_lookahead_thread_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
         int occ = 0;
         CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ramp_lookahead_thread_kernel, RAMP_THREAD_CTA, smem));
-        if (occ < 1) occ = 1;
-        // one chunk = up to 32 lookaheads; enough resident CTAs for every episode to miss at once, at most 2 per SM
+        occ = std::max(occ, 1);
+        // one chunk = up to 32 lookaheads; enough resident CTAs for every episode to miss at once
         const int want = (e->cfg.n_episodes + 31) / 32 + 8;
-        e->res_grid = std::max(1, std::min(std::min(e->sm_count * occ, e->sm_count * 2), want));
+        e->res_grid = std::max(1, std::min(e->sm_count * occ, want));
+        e->res_per_sm = occ;
         e->res_smem = smem;
-        if (e->debug) fprintf(stderr, "[ramp] thread kernel: %zu B dynamic shared memory, %d CTAs of %d threads per SM fit, grid %d\n",
-                              smem, occ, RAMP_THREAD_CTA, e->res_grid);
+        if (e->debug) fprintf(stderr, "[ramp] thread kernel: %zu B dynamic shared memory (%zu B needed), %d CTAs of %d threads per SM fit, grid %d\n",
+                              smem, need, occ, RAMP_THREAD_CTA, e->res_grid);
     }
+    // one slab per CTA that can be resident, whichever launch it belongs to: every thread kernel in flight is ordered before
+    // the engine stream's end (a window's kernel before its step's commit)
     const uint64_t stride = thread_scratch_bytes(e->res_spill_ops, e->res_spill_deps, e->cfg.trace_cap);
-    if (stride != e->res_scratch_stride || stride * (uint64_t)e->res_grid != e->d_res_scratch.size()) {
+    const uint64_t n_slabs = (uint64_t)e->sm_count * (uint64_t)e->res_per_sm;
+    if (stride != e->res_scratch_stride || stride * n_slabs != e->d_res_scratch.size()) {
         CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
-        CUDA_TRY(e->d_res_scratch.alloc(stride * (uint64_t)e->res_grid));
+        CUDA_TRY(e->d_res_scratch.alloc(stride * n_slabs));
+        if (e->d_res_slab_mask.size() != (size_t)e->sm_count) CUDA_TRY(e->d_res_slab_mask.alloc((size_t)e->sm_count));
+        CUDA_TRY(cudaMemset(e->d_res_slab_mask.get(), 0, sizeof(uint32_t) * (size_t)e->sm_count));
         e->res_scratch_stride = stride;
     }
     return RAMP_OK;
@@ -501,6 +521,7 @@ ThreadArgs make_thread_args(ramp_engine* e, const ChunkDesc* chunks, const WorkI
     ThreadArgs a{};
     a.templates = e->d_templates.get(); a.chunks = chunks; a.n_chunks = &c->n_chunks; a.cursor = &c->chunk_cursor; a.items = chunk_items;
     a.scratch = e->d_res_scratch.get(); a.scratch_stride = e->res_scratch_stride;
+    a.slab_mask = e->d_res_slab_mask.get(); a.slab_groups = e->sm_count; a.slabs_per_sm = e->res_per_sm;
     a.res = res; a.pool = pool; a.trace_cap = e->cfg.trace_cap;
     a.tmpl_cap = e->res_tmpl_cap; a.n_cap = e->res_n_cap; a.spill_ops = e->res_spill_ops; a.spill_deps = e->res_spill_deps;
     a.stats = stats; a.hints = e->d_hints.get(); a.hint_jct = e->d_hint_jct.get();
@@ -661,7 +682,7 @@ bool engine_owned(const ramp_engine* e, const void* p) {
     return false;
 }
 
-// the windows' buffers, and slabs for the thread kernel's current grid and stride
+// the windows' buffers
 int ensure_windows(ramp_engine* e) {
     const int B = e->cfg.n_episodes;
     const size_t nt = (size_t)e->cfg.max_templates + 1;
@@ -681,13 +702,6 @@ int ensure_windows(ramp_engine* e) {
             CUDA_TRY(cudaMemset(w.tcount.get(), 0, sizeof(int32_t) * nt));
         }
         e->win_ready = true;
-    }
-    const uint64_t bytes = e->res_scratch_stride * (uint64_t)e->res_grid;
-    for (LookaheadWindow& w : e->win) {
-        if (w.scratch.size() == bytes) continue;
-        // every window's thread kernel ends before the step kernel of its step, so the engine stream's end covers them all
-        CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
-        CUDA_TRY(w.scratch.alloc(bytes));
     }
     return RAMP_OK;
 }
@@ -726,7 +740,6 @@ int step_overlapped(ramp_engine* e, const ramp_action_t* d_actions, int32_t fuse
     CUDA_TRY(cudaEventRecord(w.ev_planned.get(), ps));
     CUDA_TRY(cudaStreamWaitEvent(ws, w.ev_planned.get(), 0));
     ThreadArgs ta = make_thread_args(e, w.chunks.get(), w.chunk_items.get(), w.counters.get(), e->res.view(), e->pool.view(), e->d_stats.get());
-    ta.scratch = w.scratch.get();
     ramp_lookahead_thread_kernel<<<e->res_grid, RAMP_THREAD_CTA, e->res_smem, ws>>>(ta);
     CUDA_TRY(cudaEventRecord(e->ev_b[e->ev_pending].get(), ws));
     e->ev_pending++;
@@ -740,8 +753,8 @@ int step_overlapped(ramp_engine* e, const ramp_action_t* d_actions, int32_t fuse
     ramp_commit_kernel<<<grid_b, 128, 0, st>>>(c);
     bucket_resident(e, w.items_res.get(), w.counters.get(), w.chunk_items.get(), w.chunks.get(), w.rank.get(), w.tcount.get(), w.tbase.get(), st);
     ramp_lookahead_thread_kernel<<<e->res_grid, RAMP_THREAD_CTA, e->res_smem, st>>>(ta);   // the repair launch: usually no chunk
-    launch_step_kernel(e, d_actions, fuse, d_stats_out, d_ncs_out);
     CUDA_TRY(cudaEventRecord(w.ev_consumed.get(), st));
+    launch_step_kernel(e, d_actions, fuse, d_stats_out, d_ncs_out);
     e->launches += 4;
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;

@@ -89,8 +89,10 @@ struct ThreadArgs {
     const int32_t* n_chunks;        // device-side count
     int32_t* cursor;                // device-side chunk cursor (persistent CTAs pull chunks)
     const WorkItem* items;          // [chunk][32]
-    unsigned char* scratch;         // [gridDim.x][scratch_stride]: per-CTA spill + temp trace
+    unsigned char* scratch;         // [slab_groups * slabs_per_sm][scratch_stride]: spill + temp trace, one slab per resident CTA
     uint64_t scratch_stride;
+    uint32_t* slab_mask;            // [slab_groups]: bit k set = slab k of the group is held by a running CTA
+    int32_t slab_groups, slabs_per_sm;
     ResultSlots res;
     TracePool pool;
     int32_t trace_cap;
@@ -694,6 +696,43 @@ __device__ __forceinline__ LedgerSums ledger_run(const LedgerCtx& y) {
     return S;
 }
 
+// ---------------------------------------------------------------------------------------------------
+// HBM slabs.  Only a chunk that runs without its template's hints, or whose trace did not get its pool allocation, touches
+// one, so slabs are not tied to a launch: the pool has one per CTA that can be resident at once (slabs_per_sm on each SM),
+// shared by every launch in flight, and a CTA holds one from the chunk that needs it to the end of that chunk.  The CTA's
+// %smid picks the group it claims from; a group whose slabs are all held (two SMs whose ids fall in one group) is waited on.
+struct SlabView { int4* f_gl; int4* o_gl; double* tmp_tick; uint32_t* nf_gl; int32_t* oi_gl; int32_t* tmp_n; };
+__device__ __forceinline__ SlabView slab_view(const ThreadArgs& a, int k) {
+    SlabView v;
+    unsigned char* slab = a.scratch + (uint64_t)k * a.scratch_stride;
+    v.f_gl = reinterpret_cast<int4*>(slab);                                              // [spill_deps][32]
+    v.o_gl = v.f_gl + (size_t)a.spill_deps * 32;                                         // [spill_ops][32]
+    v.tmp_tick = reinterpret_cast<double*>(v.o_gl + (size_t)a.spill_ops * 32);           // [trace_cap][32]
+    v.nf_gl = reinterpret_cast<uint32_t*>(v.tmp_tick + (size_t)a.trace_cap * 32);        // [spill_deps][32]
+    v.oi_gl = reinterpret_cast<int32_t*>(v.nf_gl + (size_t)a.spill_deps * 32);           // [spill_ops][32]
+    v.tmp_n = v.oi_gl + (size_t)a.spill_ops * 32;                                        // [trace_cap][32]
+    return v;
+}
+__device__ int claim_slab(const ThreadArgs& a) {
+    uint32_t sm;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    const int g = (int)(sm % (uint32_t)a.slab_groups);
+    const uint32_t all = (a.slabs_per_sm >= 32) ? 0xffffffffu : ((1u << a.slabs_per_sm) - 1u);
+    for (;;) {
+        const uint32_t free = ~__ldcg(&a.slab_mask[g]) & all;
+        if (free == 0u) { __nanosleep(256); continue; }
+        const uint32_t bit = 1u << (__ffs((int)free) - 1);
+        if ((atomicOr(&a.slab_mask[g], bit) & bit) == 0u) {
+            __threadfence();          // acquire: the last holder's accesses to the slab came before its release
+            return g * a.slabs_per_sm + __ffs((int)bit) - 1;
+        }
+    }
+}
+__device__ __forceinline__ void release_slab(const ThreadArgs& a, int k) {
+    __threadfence();                  // release: this CTA's accesses to the slab (the barrier before ordered both warps') come first
+    atomicAnd(&a.slab_mask[k / a.slabs_per_sm], ~(1u << (k % a.slabs_per_sm)));
+}
+
 __global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(const ThreadArgs a) {
     extern __shared__ __align__(128) unsigned char smem_thr[];
     __shared__ __align__(8) unsigned long long mbar;
@@ -703,6 +742,7 @@ __global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(
     __shared__ int4 s_chunk;                         // {chunk, template (-1: none left), count, -}
     __shared__ int4 s_hint;                          // TemplateHints of the chunk's template
     __shared__ double s_hint_jct;
+    __shared__ int32_t s_slab;                       // the chunk's slab (-1: none)
     const int lane = threadIdx.x & 31;
     const bool is_sim = threadIdx.x < 32;           // warp 0: tick loops; warp 1: ledger lanes
     unsigned char* st = smem_thr + a.tmpl_cap;                      // per-lane state, by decreasing alignment
@@ -716,15 +756,9 @@ __global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(
     x.wk_sm = reinterpret_cast<uint32_t*>(x.oi_sm + RAMP_T_OCAP * 32);                   // [WCAP][32]
     x.ck_sm = x.wk_sm + RAMP_T_WCAP * 32;                                                // [CCAP][32]
     x.cnt_sm = reinterpret_cast<uint16_t*>(x.ck_sm + RAMP_T_CCAP * 32);                  // [n_cap][32]
-    unsigned char* slab = a.scratch + (uint64_t)blockIdx.x * a.scratch_stride;
-    x.f_gl = reinterpret_cast<int4*>(slab);                                              // [spill_deps][32]
-    x.o_gl = x.f_gl + (size_t)a.spill_deps * 32;                                         // [spill_ops][32]
-    double* tmp_tick = reinterpret_cast<double*>(x.o_gl + (size_t)a.spill_ops * 32);     // [trace_cap][32]
-    x.nf_gl = reinterpret_cast<uint32_t*>(tmp_tick + (size_t)a.trace_cap * 32);          // [spill_deps][32]
-    x.oi_gl = reinterpret_cast<int32_t*>(x.nf_gl + (size_t)a.spill_deps * 32);           // [spill_ops][32]
-    int32_t* tmp_n = x.oi_gl + (size_t)a.spill_ops * 32;                                 // [trace_cap][32]
     x.ring = ring; x.head = &s_head[lane]; x.tail = &s_tail[lane]; x.fin = &s_fin[lane];
     x.lane = lane; x.n_cap = a.n_cap;
+    int held = -1;                                                  // ledger lane 0: the slab this CTA holds
 
     if (threadIdx.x == 0) {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&mbar)));
@@ -759,6 +793,7 @@ __global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(
             s_chunk = cd; s_hint = hv; s_hint_jct = hj;
         }
         __syncthreads();
+        if (threadIdx.x == 32 && held >= 0) { release_slab(a, held); held = -1; }
         const int4 cd = s_chunk;
         if (cd.y < 0) break;
         const int c = cd.x, tmpl = cd.y, count = cd.z;
@@ -806,9 +841,19 @@ __global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(
                     const unsigned long long o = atomicAdd(a.pool.top, (unsigned long long)hint.n_ticks);
                     if (o + (unsigned long long)hint.n_ticks <= a.pool.len) off = (long long)o; else status0 = RAMP_ST_TRACE_OVERFLOW;
                 }
+            }
+            // a slab when a sim lane may spill (no hints) or a ledger lane keeps its trace aside (no pool allocation yet)
+            int slab = -1;
+            if (__any_sync(0xffffffffu, active && off < 0) && lane == 0) slab = claim_slab(a);
+            slab = __shfl_sync(0xffffffffu, slab, 0);
+            if (lane == 0) { held = slab; s_slab = slab; }
+            if (active) {
                 y.ring = ring; y.head = &s_head[lane]; y.tail = &s_tail[lane]; y.lane = lane;
                 if (off >= 0) { y.tr_n = a.pool.n_active + off; y.tr_tick = a.pool.tick + off; y.tr_stride = 1; y.tr_cap = hint.n_ticks; }
-                else { y.tr_n = tmp_n + lane; y.tr_tick = tmp_tick + lane; y.tr_stride = 32; y.tr_cap = a.trace_cap; }
+                else {
+                    const SlabView v = slab_view(a, slab);
+                    y.tr_n = v.tmp_n + lane; y.tr_tick = v.tmp_tick + lane; y.tr_stride = 32; y.tr_cap = a.trace_cap;
+                }
                 s_tr_cap[lane] = y.tr_cap;
                 // utilisation inside the tick loop when an earlier lookahead of the template left its completion time
                 nmw = item.n_mounted_workers > 0 ? item.n_mounted_workers : H.orig_workers;
@@ -820,11 +865,15 @@ __global__ void __launch_bounds__(RAMP_THREAD_CTA) ramp_lookahead_thread_kernel(
                 }
             }
         }
-        __syncthreads();              // ring counters reset and s_tr_cap set; every thread has read s_chunk / s_hint
+        __syncthreads();              // ring counters reset, s_tr_cap and the slab set; every thread has read s_chunk / s_hint
 
         if (is_sim) {
             if (active) {
                 x.tr_cap = s_tr_cap[lane];
+                if (!fast) {
+                    const SlabView v = slab_view(a, s_slab);
+                    x.f_gl = v.f_gl; x.o_gl = v.o_gl; x.nf_gl = v.nf_gl; x.oi_gl = v.oi_gl;
+                }
                 // one instantiation per line: scripts/tick_cycles.py finds each one's SASS by the line it is inlined at
                 if (fast) thread_lookahead<false>(x);
                 else thread_lookahead<true>(x);

@@ -1,6 +1,6 @@
 """Latency / throughput of the thread-per-lookahead kernel on the bench job's quotient (run on the GPU box).
 
-    python scripts/microbench_thread.py [run_times]
+    python scripts/microbench_thread.py [run_times [n ...]]
 """
 import json
 import sys
@@ -16,7 +16,7 @@ g = synth.resnet_like_graph()
 eng = engine.RampEngine(n_episodes=4096, n_cluster_workers=64, max_jobs=1, trace_cap=4096)
 tids = [eng.register_template(build_template(g, d, RampShape(4, 4, 4), run_times=mode)) for d in (2, 4, 8, 16)]
 eng.run_lookaheads(np.array(tids, dtype=np.int32))
-for n in (1, 32, 128, 512, 1024, 2048, 4096, 8192, 16384):
+for n in [int(v) for v in sys.argv[2:]] or (1, 32, 128, 512, 1024, 2048, 4096, 8192, 16384):
     ids = np.array([tids[k % 4] for k in range(n)], dtype=np.int32)
     best = 1e9
     for _ in range(3):
