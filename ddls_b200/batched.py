@@ -92,6 +92,86 @@ def jobs_params(models: Sequence[_Model], frac: Tuple[float, float], num_trainin
 
 _default_jobs_params = jobs_params              # the environment's constructor argument of the same name shadows it
 
+PLACE_SMEM_PER_WARP = 12288                     # include/ramp_b200.h RAMP_ENV_PLACE_SMEM_PER_WARP
+
+
+def candidate_blocks(shape: Tuple[int, int, int], max_degree: int):
+    """The blocks RampFirstFitOpPlacer tries for an op of d sub-ops, d = 1 and every even d <= max_degree, in its (block shape,
+    origin) order (utils.py:333-383, 394-443, 491-530), each as its servers' indices ((c * R + r) * S + s) in get_block order.
+    Blocks check_block always rejects (a server outside the cluster) are left out.  Returns (cand_ptr, blocks): the blocks of
+    degree d are blocks[cand_ptr[d]:cand_ptr[d + 1]]."""
+    from .placer import _block_shapes, _factor_pairs, _get_block
+    index = {(c, r, s): (c * shape[1] + r) * shape[2] + s for c in range(shape[0]) for r in range(shape[1]) for s in range(shape[2])}
+    cand_ptr, blocks = [0, 0], []
+    for d in range(1, max_degree + 1):
+        if d == 1 or d % 2 == 0:
+            for bs in _block_shapes(_factor_pairs(d), shape) + [(d, d, -1), (d, 1, 1)]:
+                I, J_, K = (shape[0] - bs[0]) + 1, (shape[1] - bs[1]) + 1, (shape[2] - bs[2]) + 1
+                if I <= 0 or J_ <= 0 or K <= 0:
+                    continue
+                for i in range(I):
+                    for j in range(J_):
+                        for k in range(K):
+                            block = _get_block(bs[0], bs[1], bs[2], shape, (i, j, k))
+                            if any(sv not in index for sv in block) or len(set(block)) != d:
+                                continue                                                             # check_block fails on it
+                            blocks.append([index[sv] for sv in block])
+        cand_ptr.append(len(blocks))
+    return cand_ptr, blocks
+
+
+def canonical_mask(coords, shape: Tuple[int, int, int], n_words: int):
+    """The servers `coords` with each coordinate axis relabelled 0, 1, ... over the values it takes (the order-preserving
+    relabelling of the template key of ``_place_many``), as a bit set over the servers of `shape`: what ramp_env_place_kernel
+    looks the lowered job up by.  Two server sets have the same mask exactly when they have the same template key."""
+    ranks = [{v: i for i, v in enumerate(sorted({c[ax] for c in coords}))} for ax in range(3)]
+    words = [0] * n_words
+    for c in coords:
+        j = (ranks[0][c[0]] * shape[1] + ranks[1][c[1]]) * shape[2] + ranks[2][c[2]]
+        words[j >> 6] |= 1 << (j & 63)
+    return tuple(words)
+
+
+def placer_tables(models: Sequence['_Model'], max_degree: int):
+    """What ramp_env_place_kernel needs of every model (include/ramp_b200.h ramp_env_placer_tables_t): per model its ops in
+    topo_sort order (utils.py:100-115, as ramp_first_fit_place orders them), the parents of each op in the graph's edge order, the
+    bytes of each op, and the sub-ops of each op at every degree.  Op indices are within the model, from 0."""
+    op_ptr, topo, par_ptr, parents, need = [0], [], [0], [], []
+    for model in models:
+        g, n = model.graph, model.n
+        par = [[] for _ in range(n + 1)]
+        children = [[] for _ in range(n + 1)]
+        for (u, v) in g.edges:
+            par[v].append(u)
+            children[u].append(v)
+        left = [list(p) for p in par]
+        seq = [v for v in range(1, n + 1) if not left[v]]
+        for v in seq:                                         # seq grows while it is walked: the queue of topo_sort
+            for c in children[v]:
+                left[c].remove(v)
+                if not left[c]:
+                    seq.append(c)
+        if len(seq) != n:
+            raise ValueError(f'model {g.name}: the graph has a cycle')
+        topo += [v - 1 for v in seq]
+        for v in range(1, n + 1):
+            parents += [u - 1 for u in par[v]]
+            par_ptr.append(len(parents))
+        need += model.mem
+        op_ptr.append(op_ptr[-1] + n)
+    splits = np.ones((max_degree + 1, op_ptr[-1]), dtype=np.int32)
+    for d in range(1, max_degree + 1):
+        splits[d] = np.concatenate([np.asarray(m.splits(d), dtype=np.int32) for m in models])
+    return dict(op_ptr=np.asarray(op_ptr, dtype=np.int32), topo=np.asarray(topo, dtype=np.int32),
+                par_ptr=np.asarray(par_ptr, dtype=np.int32), parents=np.asarray(parents, dtype=np.int32).reshape(-1),
+                need=np.asarray(need, dtype=np.float64), splits=splits)
+
+
+def place_smem_per_warp(n_workers: int, max_ops: int) -> int:
+    """Shared memory ramp_env_place_kernel keeps per warp: free memory of every server (and 8 doubles of slack for the template
+    key), one candidate index per op of the largest model."""
+    return (8 * (n_workers + 8) + 4 * max_ops + 7) // 8 * 8
+
 
 class BatchedRampJobPartitioningEnvironment:
     def __init__(self, shape: Tuple[int, int, int], graphs: Sequence[ForwardGraph], n_episodes: int, jobs_per_episode: int = 8,
@@ -461,38 +541,31 @@ class DeviceRampJobPartitioningEnvironment(BatchedRampJobPartitioningEnvironment
     is ``ramp_env_decide`` -> ``ramp_env_advance`` and, through ``step``, one read-back of the outputs.  ``device_buffers()`` gives
     the raw device pointers for a policy that lives on the GPU (then nothing crosses PCIe).  The host is asked only for what the
     tables cannot decide: jobs whose ops take different numbers of sub-ops, and the first use of a block geometry (it lowers the
-    job natively, registers it and fills the table)."""
+    job natively, registers it and fills the table).
 
-    def __init__(self, *args, prewarm: bool = False, **kw):
+    place_on_device=True places the jobs whose ops split unevenly on the device too (ramp_env_place_kernel: the same first-fit
+    placer, one warp per episode) and finds their lowered job by the canonical mask of the servers used; the host then only
+    lowers each new (model, degree, canonical mask) once, and a warmed environment never calls the host's placer.  It needs
+    ``place_smem_per_warp(servers, ops of the largest model)`` <= PLACE_SMEM_PER_WARP bytes; past that the environment warns and
+    keeps the host path (``self.place_on_device`` is then False)."""
+
+    def __init__(self, *args, prewarm: bool = False, place_on_device: bool = False, **kw):
         import ctypes as C
         super().__init__(*args, **kw)
-        from .placer import _block_shapes, _factor_pairs, _get_block
         D, nw, shape = self.max_partitions_per_op, self.n_words, (self.shape.c, self.shape.r, self.shape.s)
         self._geom_index: Dict[tuple, int] = {}
         self._geom_example: Dict[tuple, list] = {}          # (degree, geometry index) -> one block with that geometry
-        cand_ptr, cand_mask, cand_geom = [0, 0], [], []
-        for d in range(1, D + 1):
-            if d == 1 or d % 2 == 0:
-                shapes = _block_shapes(_factor_pairs(d), shape) + [(d, d, -1), (d, 1, 1)]          # utils.py:333-383, 491-530
-                for bs in shapes:                                                                   # utils.py:394-443
-                    I, J_, K = (shape[0] - bs[0]) + 1, (shape[1] - bs[1]) + 1, (shape[2] - bs[2]) + 1
-                    if I <= 0 or J_ <= 0 or K <= 0:
-                        continue
-                    for i in range(I):
-                        for j in range(J_):
-                            for k in range(K):
-                                block = _get_block(bs[0], bs[1], bs[2], shape, (i, j, k))
-                                if any(sv not in self._server_index for sv in block) or len(set(block)) != d:
-                                    continue                                                         # check_block fails on it
-                                words = [0] * nw
-                                for sv in block:
-                                    ix = self._server_index[sv]
-                                    words[ix >> 6] |= (1 << (ix & 63))
-                                cand_mask.append(words)
-                                gi = self._geometry(sorted(block))
-                                cand_geom.append(gi)
-                                self._geom_example.setdefault((d, gi), sorted(block))
-            cand_ptr.append(len(cand_mask))
+        cand_ptr, self._cand_blocks = candidate_blocks(shape, D)
+        cand_mask, cand_geom = [], []
+        for blk in self._cand_blocks:
+            words = [0] * nw
+            for ix in blk:
+                words[ix >> 6] |= (1 << (ix & 63))
+            cand_mask.append(words)
+            coords = [self._servers[ix] for ix in sorted(blk)]
+            gi = self._geometry(coords)
+            cand_geom.append(gi)
+            self._geom_example.setdefault((len(blk), gi), coords)
         self._n_geoms = max(len(self._geom_index), 1)
         M = len(self.models)
         uniform = np.zeros((M, D + 1), dtype=np.uint8)
@@ -553,8 +626,42 @@ class DeviceRampJobPartitioningEnvironment(BatchedRampJobPartitioningEnvironment
         self._need = np.zeros(B, dtype=np.int32)
         self._prewarmed = False
         self._decides_all = None
+        self.place_on_device = bool(place_on_device)
+        self._geom_mask_set = set()                         # (model, degree, canonical mask) entries given to the device table
+        if self.place_on_device:
+            self._set_placer_tables(cand_ptr)
         if prewarm:
             self.prewarm()
+
+    def _set_placer_tables(self, cand_ptr):
+        import ctypes as C
+        import warnings
+        need = place_smem_per_warp(self.W, max(m.n for m in self.models))
+        if need > PLACE_SMEM_PER_WARP:
+            warnings.warn(f'place_on_device: {self.W} servers and {max(m.n for m in self.models)} ops need {need} bytes of shared '
+                          f'memory per warp, more than {PLACE_SMEM_PER_WARP}; jobs whose ops split unevenly stay with the host placer')
+            self.place_on_device = False
+            return
+        t = placer_tables(self.models, self.max_partitions_per_op)
+        t['cand_offset'] = np.ascontiguousarray(np.cumsum([0] + [len(b) for b in self._cand_blocks]), dtype=np.int32)
+        t['cand_servers'] = np.ascontiguousarray([ix for b in self._cand_blocks for ix in b], dtype=np.int32).reshape(-1)
+        assert int(t['cand_offset'].shape[0]) == cand_ptr[-1] + 1
+
+        class _Tables(C.Structure):
+            _fields_ = [('n_ops_total', C.c_int32), ('memory_capacity', C.c_double)] + [
+                (k, C.c_void_p) for k in ('op_ptr', 'topo', 'par_ptr', 'parents', 'need', 'splits', 'cand_offset', 'cand_servers')]
+        self._placer_keep = {k: np.ascontiguousarray(v) for k, v in t.items()}
+        tab = _Tables(int(t['op_ptr'][-1]), A100_MEMORY, *[self._placer_keep[k].ctypes.data for k in
+                      ('op_ptr', 'topo', 'par_ptr', 'parents', 'need', 'splits', 'cand_offset', 'cand_servers')])
+        L = self.eng._L
+        L.ramp_env_set_placer_tables.restype = C.c_int
+        L.ramp_env_set_placer_tables.argtypes = [C.c_void_p, C.c_void_p]
+        L.ramp_env_set_geometry_template.restype = C.c_int
+        L.ramp_env_set_geometry_template.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
+        _engine._check(L.ramp_env_set_placer_tables(self.eng._h, C.byref(tab)))
+
+    def _canonical_mask(self, coords):
+        return canonical_mask(coords, (self.shape.c, self.shape.r, self.shape.s), self.n_words)
 
     def prewarm(self):
         """Lowers and registers the job of every (model, degree, block geometry) the device can choose, so that no step waits
@@ -781,6 +888,13 @@ class DeviceRampJobPartitioningEnvironment(BatchedRampJobPartitioningEnvironment
                 if gkey < self._n_geoms and (m, d, gkey) not in self._table_set:
                     _engine._check(L.ramp_env_set_template(h, m, d, gkey, tid, mt.ctypes.data))
                     self._table_set.add((m, d, gkey))
+            elif tid >= 0 and self.place_on_device:
+                coords = [self._servers[i] for i in range(self.W) if (words[i >> 6] >> (i & 63)) & 1]
+                cm = self._canonical_mask(coords)
+                if (m, d, cm) not in self._geom_mask_set:
+                    cw = np.array(cm, dtype=np.uint64)
+                    _engine._check(L.ramp_env_set_geometry_template(h, m, d, cw.ctypes.data, tid, mt.ctypes.data))
+                    self._geom_mask_set.add((m, d, cm))
             for b in bs:
                 _engine._check(L.ramp_env_patch(h, b, tid, mask.ctypes.data, mt.ctypes.data))
 

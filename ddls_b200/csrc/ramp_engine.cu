@@ -192,6 +192,15 @@ struct ramp_engine {
     PinnedArray<unsigned char> env_h_mirror;   // host arrays of ramp_env_host_mirror
     bool env_unchecked_decide = false;   // a ramp_env_decide without need_host_out has not been looked at yet
     bool env_agents_set = false;         // ramp_env_set_agents ran
+    // device placement of uneven jobs (ramp_env_set_placer_tables); the geometry table's host copy decides every insertion
+    bool has_placer = false;
+    int32_t env_shape[3] = {0, 0, 0};
+    PlaceDev place{};
+    std::vector<unsigned long long> place_keys;         // [cap][n_words + 1], as the device table
+    std::vector<int32_t> place_tids;                    // [cap]
+    uint32_t place_count = 0;
+    DeviceArray<unsigned long long> place_table_keys;
+    DeviceArray<int32_t> place_table_tid;
     DeviceArray<double> steplog_stats, steplog_rewards;   // ramp_env_steplog_begin: [horizon][RAMP_ENV_STEP_STATS_LEN][B], [horizon][B]
     DeviceArray<int32_t> steplog_actions;                 // [horizon][B]
     // i/o in caller-owned device memory (ramp_env_ingest / ramp_env_export), allocated by the first call that needs them
@@ -1484,6 +1493,7 @@ int ramp_env_create(ramp_engine_t* e, const ramp_env_config_t* c) {
         return set_error(RAMP_ERR_BAD_ARG, "bad environment shape");
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     EnvDev& v = e->env;
+    for (int k = 0; k < 3; ++k) e->env_shape[k] = c->shape[k];
     v.B = B; v.J = J; v.n_words = nw; v.n_models = M; v.max_degree = D; v.n_geoms = G; v.n_workers = n_workers;
     v.apply_mask = c->apply_action_mask; v.fail_reward = c->fail_reward; v.success_reward = c->success_reward;
     v.num_training_steps = (double)c->num_training_steps;
@@ -1536,6 +1546,117 @@ int ramp_env_set_template(ramp_engine_t* e, int32_t model, int32_t degree, int32
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     CUDA_TRY(cudaMemcpy(v.tmpl_of + ((size_t)model * (v.max_degree + 1) + degree) * v.n_geoms + geom, &template_id, sizeof(int32_t), cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(v.tmpl_mount + (size_t)template_id * 6, mount, sizeof(double) * 6, cudaMemcpyHostToDevice));
+    return RAMP_OK;
+}
+
+int ramp_env_set_placer_tables(ramp_engine_t* e, const ramp_env_placer_tables_t* t) {
+    if (!e || !e->has_env || !t || !t->op_ptr || !t->topo || !t->par_ptr || !t->parents || !t->need || !t->splits || !t->cand_offset ||
+        !t->cand_servers)
+        return set_error(RAMP_ERR_BAD_ARG, "no environment or a null table");
+    if (e->has_placer) return set_error(RAMP_ERR_BAD_ARG, "the environment already has its placer tables");
+    const EnvDev& v = e->env;
+    const int M = v.n_models, D = v.max_degree, N = t->n_ops_total, W = v.n_workers;
+    int max_ops = 0;
+    for (int m = 0; m < M; ++m) max_ops = std::max(max_ops, t->op_ptr[m + 1] - t->op_ptr[m]);
+    if (t->op_ptr[0] != 0 || t->op_ptr[M] != N || N < 1) return set_error(RAMP_ERR_BAD_ARG, "op_ptr does not cover n_ops_total");
+    PlaceDev p{};
+    p.n_ops_total = N; p.capacity = t->memory_capacity;
+    p.smem_mem_words = W + 8;
+    p.smem_bytes_per_warp = (8 * p.smem_mem_words + 4 * max_ops + 7) / 8 * 8;
+    if (p.smem_bytes_per_warp > RAMP_ENV_PLACE_SMEM_PER_WARP)
+        return set_error(RAMP_ERR_BAD_ARG, "device placement needs %d bytes of shared memory per warp (%d servers, %d ops); the limit is %d",
+                         p.smem_bytes_per_warp, W, max_ops, RAMP_ENV_PLACE_SMEM_PER_WARP);
+    p.shape_r = e->env_shape[1]; p.shape_s = e->env_shape[2];
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    std::vector<int32_t> cand_ptr((size_t)D + 2);
+    CUDA_TRY(cudaMemcpy(cand_ptr.data(), v.cand_ptr, sizeof(int32_t) * (D + 2), cudaMemcpyDeviceToHost));
+    const int n_cand = cand_ptr[D + 1];
+    int rc;
+    if ((rc = env_upload(e, &p.op_ptr, t->op_ptr, (size_t)M + 1))) return rc;
+    if ((rc = env_upload(e, &p.topo, t->topo, (size_t)N))) return rc;
+    if ((rc = env_upload(e, &p.par_ptr, t->par_ptr, (size_t)N + 1))) return rc;
+    if ((rc = env_upload(e, &p.parents, t->parents, (size_t)t->par_ptr[N]))) return rc;
+    if ((rc = env_upload(e, &p.need, t->need, (size_t)N))) return rc;
+    if ((rc = env_upload(e, &p.splits, t->splits, (size_t)(D + 1) * N))) return rc;
+    if ((rc = env_upload(e, &p.cand_offset, t->cand_offset, (size_t)n_cand + 1))) return rc;
+    if ((rc = env_upload(e, &p.cand_servers, t->cand_servers, (size_t)t->cand_offset[n_cand]))) return rc;
+    if ((rc = env_upload<int32_t>(e, &p.host_list, nullptr, (size_t)v.B))) return rc;
+    if ((rc = env_upload<int32_t>(e, &p.n_host, nullptr, 1))) return rc;
+    const uint32_t cap = 64;
+    e->place_keys.assign((size_t)cap * (v.n_words + 1), 0ull);
+    e->place_tids.assign(cap, -1);
+    e->place_count = 0;
+    CUDA_TRY(e->place_table_keys.alloc(e->place_keys.size()));
+    CUDA_TRY(e->place_table_tid.alloc(cap));
+    CUDA_TRY(cudaMemcpy(e->place_table_keys.get(), e->place_keys.data(), sizeof(unsigned long long) * e->place_keys.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(e->place_table_tid.get(), e->place_tids.data(), sizeof(int32_t) * cap, cudaMemcpyHostToDevice));
+    p.table_keys = e->place_table_keys.get(); p.table_tid = e->place_table_tid.get(); p.table_mask = cap - 1;
+    e->place = p;
+    e->has_placer = true;
+    return RAMP_OK;
+}
+
+// the slot of `key` ([n_words + 1]) in the host copy of the geometry table: its entry, or the empty slot that ends its probe
+static uint32_t place_slot(const ramp_engine* e, const unsigned long long* key, uint32_t mask) {
+    const int nw = e->env.n_words;
+    unsigned long long h = 0ull;
+    for (int w = 0; w <= nw; ++w) h = env_geom_hash_step(h, key[w]);
+    for (uint32_t slot = (uint32_t)h & mask;; slot = (slot + 1) & mask) {
+        const unsigned long long* k = e->place_keys.data() + (size_t)slot * (nw + 1);
+        if (k[0] == 0ull || std::equal(k, k + nw + 1, key)) return slot;
+    }
+}
+
+int ramp_env_set_geometry_template(ramp_engine_t* e, int32_t model, int32_t degree, const uint64_t* canonical_mask, int32_t template_id,
+                                   const double mount[6]) {
+    if (!e || !e->has_placer || !canonical_mask || !mount) return set_error(RAMP_ERR_BAD_ARG, "no placer tables or a null argument");
+    const EnvDev& v = e->env;
+    if (model < 0 || model >= v.n_models || degree < 1 || degree > v.max_degree || template_id < 0 || template_id >= (int32_t)e->templates.size())
+        return set_error(RAMP_ERR_BAD_ARG, "bad geometry table entry (model %d degree %d template %d)", model, degree, template_id);
+    const int nw = v.n_words;
+    std::vector<unsigned long long> key((size_t)nw + 1);
+    key[0] = ((unsigned long long)(model + 1) << 32) | (unsigned long long)degree;
+    for (int w = 0; w < nw; ++w) key[1 + w] = canonical_mask[w];
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    cudaStream_t st = e->stream.get();
+    uint32_t cap = (uint32_t)e->place_tids.size();
+    uint32_t slot = place_slot(e, key.data(), cap - 1);
+    const bool fresh = e->place_keys[(size_t)slot * (nw + 1)] == 0ull;
+    if (fresh && 2 * (e->place_count + 1) > cap) {
+        // at most half full: rehash the host copy into twice the slots and upload it whole
+        std::vector<unsigned long long> old_keys;
+        std::vector<int32_t> old_tids;
+        old_keys.swap(e->place_keys); old_tids.swap(e->place_tids);
+        cap *= 2;
+        e->place_keys.assign((size_t)cap * (nw + 1), 0ull);
+        e->place_tids.assign(cap, -1);
+        for (size_t o = 0; o < old_tids.size(); ++o) {
+            const unsigned long long* k = old_keys.data() + o * (nw + 1);
+            if (k[0] == 0ull) continue;
+            const uint32_t to = place_slot(e, k, cap - 1);
+            std::copy(k, k + nw + 1, e->place_keys.begin() + (size_t)to * (nw + 1));
+            e->place_tids[to] = old_tids[o];
+        }
+        DeviceArray<unsigned long long> keys;
+        DeviceArray<int32_t> tids;
+        CUDA_TRY(keys.alloc(e->place_keys.size()));
+        CUDA_TRY(tids.alloc(cap));
+        CUDA_TRY(cudaMemcpyAsync(keys.get(), e->place_keys.data(), sizeof(unsigned long long) * e->place_keys.size(), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(tids.get(), e->place_tids.data(), sizeof(int32_t) * cap, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        e->place_table_keys = std::move(keys);            // frees the old table: no kernel queued on the stream reads it any more
+        e->place_table_tid = std::move(tids);
+        e->place.table_keys = e->place_table_keys.get(); e->place.table_tid = e->place_table_tid.get(); e->place.table_mask = cap - 1;
+        slot = place_slot(e, key.data(), cap - 1);
+    }
+    if (fresh) e->place_count++;
+    std::copy(key.begin(), key.end(), e->place_keys.begin() + (size_t)slot * (nw + 1));
+    e->place_tids[slot] = template_id;
+    // on the engine stream, behind every kernel queued so far (pageable sources: the copies are staged before the calls return)
+    CUDA_TRY(cudaMemcpyAsync(v.tmpl_mount + (size_t)template_id * 6, mount, sizeof(double) * 6, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(e->place_table_tid.get() + slot, &e->place_tids[slot], sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(e->place_table_keys.get() + (size_t)slot * (nw + 1), key.data(), sizeof(unsigned long long) * (nw + 1),
+                             cudaMemcpyHostToDevice, st));
     return RAMP_OK;
 }
 
@@ -1604,8 +1725,19 @@ int ramp_env_decide(ramp_engine_t* e, const int32_t* actions, int32_t* n_need_ho
     ramp_env_decide_kernel<<<(v.B + 127) / 128, 128, 0, st>>>(v, e->ep, e->d_actions.get());
     e->launches++;
     CUDA_TRY(cudaGetLastError());
+    if (e->has_placer) {
+        // the decide kernel's list length stays on the device: the grid covers every episode and each warp reads the length
+        const PlaceDev& p = e->place;
+        CUDA_TRY(cudaMemsetAsync(p.n_host, 0, sizeof(int32_t), st));
+        const int grid = std::max(1, std::min((v.B + ENV_PLACE_WARPS - 1) / ENV_PLACE_WARPS, e->sm_count * 4));
+        ramp_env_place_kernel<<<grid, ENV_PLACE_WARPS * 32, (size_t)ENV_PLACE_WARPS * p.smem_bytes_per_warp, st>>>(v, p, e->d_actions.get());
+        e->launches++;
+        CUDA_TRY(cudaGetLastError());
+    }
+    const int32_t* host_count = e->has_placer ? e->place.n_host : v.n_need_host;
+    const int32_t* host_list = e->has_placer ? e->place.host_list : v.need_host;
     if (n_need_host_out) {
-        CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get(), v.n_need_host, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get(), host_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 1, v.err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         const bool range = e->env_range_armed;
         if (range) { int rc = env_range_fetch(e); if (rc != RAMP_OK) return rc; }
@@ -1617,7 +1749,7 @@ int ramp_env_decide(ramp_engine_t* e, const int32_t* actions, int32_t* n_need_ho
         }
         *n_need_host_out = e->env_h_need.get()[0];
         if (need_host_out && e->env_h_need.get()[0] > 0)
-            CUDA_TRY(cudaMemcpy(need_host_out, v.need_host, sizeof(int32_t) * e->env_h_need.get()[0], cudaMemcpyDeviceToHost));
+            CUDA_TRY(cudaMemcpy(need_host_out, host_list, sizeof(int32_t) * e->env_h_need.get()[0], cudaMemcpyDeviceToHost));
     } else {
         e->env_unchecked_decide = true;      // looked at by the next ramp_env_read
     }
@@ -1674,7 +1806,8 @@ int ramp_env_read(ramp_engine_t* e, double* reward, uint8_t* done, int32_t* queu
     if (e->env_unchecked_decide) {
         // decisions taken without the host looking (a device-resident policy): an invalid action under apply_action_mask is sticky
         // in `err`; episodes the tables could not decide were left unplaced, which only the LAST decide's count can show
-        CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 2, v.n_need_host, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 2, e->has_placer ? e->place.n_host : v.n_need_host, sizeof(int32_t),
+                                 cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 3, v.err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         const bool range = e->env_range_armed;
         int rc = range ? env_range_fetch(e) : RAMP_OK;

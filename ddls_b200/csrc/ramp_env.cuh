@@ -4,6 +4,8 @@
 //   ramp_env_decide_kernel  RJPE:300-343 + RampFirstFitOpPlacer (agents/placers/utils.py:394-443, 532-582) for jobs whose ops all
 //                           take `degree` sub-ops: the first candidate block (host-enumerated in the reference's shape / origin
 //                           order) with no busy server; template by (model, degree, geometry); action row for the engine
+//   ramp_env_place_kernel   (opt-in) the same placer for jobs whose ops take different numbers of sub-ops, one warp per episode
+//                           the decide kernel listed for the host; template by (model, degree, canonical mask of the servers)
 //   ramp_env_update_kernel  after the cluster step: reward (rewards/job_acceptance.py), servers of the accepted job, occupancy =
 //                           OR over the running jobs, and the next queued job's dynamic graph features + action mask
 //                           (observations/ramp_job_partitioning_observation.py:80-131, 358-498); the template id of the
@@ -197,6 +199,166 @@ __global__ void ramp_env_update_kernel(const EnvDev v, const EpisodeState ep, co
     }
     o[9] = env_feature((double)(v.n_workers - free_workers) / (double)v.n_workers, v.machine_epsilon);
     o[10] = env_feature((double)n_running / (double)v.n_workers, v.machine_epsilon);
+}
+
+// ---- device placement of jobs whose ops split unevenly (ramp_env_set_placer_tables) -----------------------------------------
+struct PlaceDev {
+    int32_t n_ops_total, smem_mem_words, smem_bytes_per_warp, shape_r, shape_s;
+    double capacity;
+    const int32_t* op_ptr; const int32_t* topo; const int32_t* par_ptr; const int32_t* parents; const double* need;
+    const int32_t* splits; const int32_t* cand_offset; const int32_t* cand_servers;
+    // (model, degree, canonical mask) -> template: open addressing, linear probing; key word 0 is (model + 1) << 32 | degree
+    // (0 = empty slot), words 1..n_words the mask
+    const unsigned long long* table_keys;   // [table_cap][n_words + 1]
+    const int32_t* table_tid;               // [table_cap]
+    uint32_t table_mask;                    // table_cap - 1 (a power of two)
+    int32_t* host_list; int32_t* n_host;    // [B] episodes the host decides after this kernel, their number
+};
+
+constexpr int ENV_PLACE_WARPS = 4;          // warps per CTA: 4 x RAMP_ENV_PLACE_SMEM_PER_WARP is the default 48 KB
+
+__host__ __device__ __forceinline__ unsigned long long env_geom_hash_step(unsigned long long h, unsigned long long w) {
+    h ^= w + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2);
+    h ^= h >> 31; h *= 0xBF58476D1CE4E5B9ull; h ^= h >> 29;
+    return h;
+}
+
+// RampFirstFitOpPlacer (ramp_first_fit_place, csrc/ramp_expand.cpp) for the episodes ramp_env_decide_kernel listed in need_host,
+// one warp per episode, on a cluster whose free servers hold memory_capacity bytes.  An op's placement is a candidate block
+// index (a parent's servers are always one of the blocks), so per episode the warp keeps one int per op and one double of free
+// memory per server in shared memory.  The memory arithmetic is the C++'s, in its order, with no contraction.  The union of the
+// chosen blocks, relabelled axis by axis (the host's template key), is looked up in the geometry table: a hit writes the action
+// row, tid and placed as ramp_env_decide_kernel does; a miss, and a uniform job (its block geometry had no template), is listed
+// for the host.  A job that cannot be placed keeps the empty row the decide kernel wrote: it is blocked.
+__global__ void __launch_bounds__(ENV_PLACE_WARPS * 32) ramp_env_place_kernel(const EnvDev v, const PlaceDev p, ramp_action_t* rows) {
+    extern __shared__ double env_place_smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const int W = v.n_workers, nw = v.n_words, R = p.shape_r, S = p.shape_s, C = W / (R * S);
+    double* mem = env_place_smem + (size_t)wib * (p.smem_bytes_per_warp / 8);
+    int32_t* where = (int32_t*)(mem + p.smem_mem_words);
+    const int n_list = *v.n_need_host;
+    for (int i = blockIdx.x * ENV_PLACE_WARPS + wib; i < n_list; i += gridDim.x * ENV_PLACE_WARPS) {
+        const int b = v.need_host[i];
+        const int q = v.decided_job[b], a = v.actions[b];
+        const int m = v.model_of[(size_t)b * v.J + q];
+        if (v.uniform[m * (v.max_degree + 1) + a]) {                               // a block geometry without its template
+            if (lane == 0) p.host_list[atomicAdd(p.n_host, 1)] = b;
+            continue;
+        }
+        for (int s = lane; s < W; s += 32) mem[s] = p.capacity;
+        __syncwarp();
+        const unsigned long long* busy = v.busy + (size_t)b * nw;
+        const int base = p.op_ptr[m], n = p.op_ptr[m + 1] - base;
+        const int32_t* sp = p.splits + (size_t)a * p.n_ops_total + base;
+        bool ok = true;
+        for (int t = 0; t < n; ++t) {
+            const int op = p.topo[base + t];
+            const int split = sp[op];
+            const double need = p.need[base + op];
+            int c = -1;
+            // parent_collective_placement (utils.py:258-314): the first parent, in edge order, on `split` servers that together
+            // hold `need` bytes
+            for (int k = p.par_ptr[base + op]; k < p.par_ptr[base + op + 1] && c < 0; ++k) {
+                const int pa = p.parents[k];
+                if (sp[pa] != split) continue;
+                const int32_t* sv = p.cand_servers + p.cand_offset[where[pa]];
+                double avail = 0.0;
+                for (int j = 0; j < split; ++j) avail = __dadd_rn(avail, mem[sv[j]]);
+                if (avail >= need) c = where[pa];
+            }
+            const double op_size = __ddiv_rn(need, (double)split);
+            if (c < 0) {
+                // regular_collective_placement (utils.py:333-383): the first block of `split` servers, in ff_block order, with
+                // no busy server and op_size bytes free on each; none when split exceeds the cluster (an empty range)
+                const int c0 = v.cand_ptr[split], c1 = v.cand_ptr[split + 1];
+                for (int c32 = c0; c32 < c1 && c < 0; c32 += 32) {
+                    const int cc = c32 + lane;
+                    bool fit = cc < c1;
+                    if (fit) {
+                        const unsigned long long* cm = v.cand_mask + (size_t)cc * nw;
+                        for (int w = 0; w < nw; ++w) fit = fit && ((busy[w] & cm[w]) == 0ull);
+                        const int32_t* sv = p.cand_servers + p.cand_offset[cc];
+                        for (int j = 0; j < split && fit; ++j) fit = mem[sv[j]] >= op_size;
+                    }
+                    const unsigned bal = __ballot_sync(0xffffffffu, fit);
+                    if (bal) c = c32 + __ffs(bal) - 1;
+                }
+                if (c < 0) { ok = false; break; }
+            }
+            __syncwarp();
+            const int32_t* sv = p.cand_servers + p.cand_offset[c];
+            for (int j = lane; j < split; j += 32) mem[sv[j]] = __dsub_rn(mem[sv[j]], op_size);
+            if (lane == 0) where[op] = c;
+            __syncwarp();
+        }
+        if (!ok) continue;                                                          // blocked (RCE:914-919)
+        // the servers the job uses, and the template key: each coordinate axis relabelled 0, 1, ... over the values it takes;
+        // the free-memory array is scratch from here on (8 * (W + 8) bytes hold the axis ranks and the canonical mask)
+        unsigned long long used = 0ull;                                             // word `lane` of the union
+        if (lane < nw)
+            for (int t = 0; t < n; ++t) used |= v.cand_mask[(size_t)where[t] * nw + lane];
+        uint16_t* rank = (uint16_t*)mem;                                            // [C + R + S]
+        unsigned long long* canon = (unsigned long long*)mem + (C + R + S + 3) / 4; // [nw]
+        __syncwarp();
+        for (int x = lane; x < C + R + S; x += 32) rank[x] = 0;
+        for (int w = lane; w < nw; w += 32) canon[w] = 0ull;
+        __syncwarp();
+        for (int s0 = 0; s0 < W; s0 += 32) {                                       // whole-warp rounds: every lane shuffles
+            const int s = s0 + lane;
+            const unsigned long long u = __shfl_sync(0xffffffffu, used, (s >> 6) & 31);
+            if (s < W && ((u >> (s & 63)) & 1ull)) { rank[s / (R * S)] = 1; rank[C + (s / S) % R] = 1; rank[C + R + s % S] = 1; }
+        }
+        __syncwarp();
+        if (lane == 0) {                                                            // flags -> exclusive prefix per axis
+            int r = 0;
+            for (int x = 0; x < C + R + S; ++x) {
+                if (x == C || x == C + R) r = 0;
+                const int f = rank[x];
+                rank[x] = (uint16_t)r;
+                r += f;
+            }
+        }
+        __syncwarp();
+        for (int s0 = 0; s0 < W; s0 += 32) {
+            const int s = s0 + lane;
+            const unsigned long long u = __shfl_sync(0xffffffffu, used, (s >> 6) & 31);
+            if (s < W && ((u >> (s & 63)) & 1ull)) {
+                const int j = ((int)rank[s / (R * S)] * R + (int)rank[C + (s / S) % R]) * S + (int)rank[C + R + s % S];
+                atomicOr(canon + (j >> 6), 1ull << (j & 63));
+            }
+        }
+        __syncwarp();
+        int t_id = -1;
+        if (lane == 0) {
+            const unsigned long long key0 = ((unsigned long long)(m + 1) << 32) | (unsigned long long)a;
+            unsigned long long h = env_geom_hash_step(0ull, key0);
+            for (int w = 0; w < nw; ++w) h = env_geom_hash_step(h, canon[w]);
+            for (uint32_t slot = (uint32_t)h & p.table_mask;; slot = (slot + 1) & p.table_mask) {
+                const unsigned long long* k = p.table_keys + (size_t)slot * (nw + 1);
+                if (k[0] == 0ull) break;
+                bool eq = k[0] == key0;
+                for (int w = 0; w < nw && eq; ++w) eq = k[1 + w] == canon[w];
+                if (eq) { t_id = p.table_tid[slot]; break; }
+            }
+        }
+        t_id = __shfl_sync(0xffffffffu, t_id, 0);
+        if (t_id < 0) {
+            if (lane == 0) p.host_list[atomicAdd(p.n_host, 1)] = b;
+            continue;
+        }
+        if (lane < nw) v.placed[(size_t)b * nw + lane] = used;
+        if (lane == 0) {
+            const double* mt = v.tmpl_mount + (size_t)t_id * 6;
+            const double ov = v.macc[(size_t)b * v.J + q];
+            ramp_action_t row;
+            row.max_acceptable_jct = isnan(ov) ? __dmul_rn(v.frac[(size_t)b * v.J + q], mt[0]) : ov;
+            row.part_op_mem = mt[1]; row.part_dep_size = mt[2]; row.flow_size = mt[3];
+            row.n_mounted_workers = (int32_t)mt[4]; row.n_mounted_channels = (int32_t)mt[5];
+            row.template_id = t_id; row.flags = 0;
+            v.tid[b] = t_id;
+            rows[b] = row;
+        }
+    }
 }
 
 // The reference's heuristic agents (ddls/environments/ramp_job_partitioning/agents/*.py), restated line for line on the action

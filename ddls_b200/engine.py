@@ -164,7 +164,7 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_get_lookahead_kernel_time', 'ramp_expand_template', 'ramp_free_expanded_job', 'ramp_free_expanded_aux', 'ramp_first_fit_place',
                     'ramp_quotient_template', 'ramp_free_quotient', 'ramp_get_quotient_bytes', 'ramp_set_job_count',
                     'ramp_set_limits', 'ramp_first_fit_place_many', 'ramp_env_create', 'ramp_env_set_template',
-                    'ramp_env_reset', 'ramp_env_buffers', 'ramp_env_host_mirror', 'ramp_env_decide', 'ramp_env_patch', 'ramp_env_advance', 'ramp_env_read', 'ramp_get_last_step_stats', 'ramp_env_read_state',
+                    'ramp_env_reset', 'ramp_env_buffers', 'ramp_env_host_mirror', 'ramp_env_decide', 'ramp_env_patch', 'ramp_env_set_placer_tables', 'ramp_env_set_geometry_template', 'ramp_env_advance', 'ramp_env_read', 'ramp_get_last_step_stats', 'ramp_env_read_state',
                     'ramp_enable_env_step_stats', 'ramp_get_env_step_stats', 'ramp_env_steplog_begin', 'ramp_env_steplog_read',
                     'ramp_enable_tick_lists', 'ramp_get_tick_lists', 'ramp_policy_weight_count', 'ramp_policy_create', 'ramp_policy_destroy', 'ramp_policy_set_weights', 'ramp_policy_set_model',
                     'ramp_policy_embed', 'ramp_policy_forward', 'ramp_policy_decide', 'ramp_policy_act', 'ramp_policy_read',

@@ -52,12 +52,12 @@ def static_tensors(graphs, device='cpu'):
 
 
 class TorchRampJobPartitioningEnvironment:
-    def __init__(self, *args, prewarm: bool = False, **kw):
-        """The arguments of ``DeviceRampJobPartitioningEnvironment`` (``device`` picks cuda:<device>).  A failed construction
-        frees what it allocated."""
+    def __init__(self, *args, prewarm: bool = False, place_on_device: bool = False, **kw):
+        """The arguments of ``DeviceRampJobPartitioningEnvironment`` (``device`` picks cuda:<device>; ``place_on_device`` places
+        jobs whose ops split unevenly on the device).  A failed construction frees what it allocated."""
         env = DeviceRampJobPartitioningEnvironment.__new__(DeviceRampJobPartitioningEnvironment)
         try:
-            env.__init__(*args, prewarm=prewarm, **kw)
+            env.__init__(*args, prewarm=prewarm, place_on_device=place_on_device, **kw)
             self.env = env
             self.device = torch.device('cuda', int(kw.get('device', 0)))
             self.B, self.n_actions = env.B, env.max_partitions_per_op + 1

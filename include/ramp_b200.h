@@ -444,6 +444,33 @@ int ramp_env_buffers(ramp_engine_t* eng, ramp_env_buffers_t* out);
 int ramp_env_decide(ramp_engine_t* eng, const int32_t* actions, int32_t* n_need_host_out, int32_t* need_host_out);
 int ramp_env_patch(ramp_engine_t* eng, int32_t episode, int32_t template_id, const uint64_t* server_mask, const double mount[6]);
 int ramp_env_advance(ramp_engine_t* eng);
+
+/* Device placement of jobs whose ops split unevenly.  Once ramp_env_set_placer_tables ran, ramp_env_decide places every episode
+ * the tables above list for the host on the device instead (ramp_env_place_kernel, one warp per episode): the reference's
+ * first-fit op placer, op by op in topological order (parent collective placement first, then the first free candidate block
+ * with the memory), then the lowered job by (model, degree, canonical mask of the servers used) from a table filled by
+ * ramp_env_set_geometry_template.  need_host_out then lists only the episodes whose canonical mask is not in that table yet, and
+ * uniform jobs whose block geometry has no template.  The canonical mask relabels each coordinate axis of the used servers to
+ * 0, 1, ... in order and sets bit (c * R + r) * S + s of each relabelled server.  Per warp the kernel keeps the free memory of
+ * every server and one candidate index per op in shared memory: 8 * (servers + 8) + 4 * (ops of the largest model) bytes, which
+ * must not exceed RAMP_ENV_PLACE_SMEM_PER_WARP. */
+#define RAMP_ENV_PLACE_SMEM_PER_WARP 12288
+typedef struct {
+    int32_t n_ops_total;          /* ops of every model together                                                   */
+    double  memory_capacity;      /* free bytes of every server when the job is placed                             */
+    const int32_t* op_ptr;        /* [n_models + 1] the ops of model m are op_ptr[m] .. op_ptr[m + 1] - 1          */
+    const int32_t* topo;          /* [n_ops_total] per model: op indices (within the model, from 0) in topo_sort order */
+    const int32_t* par_ptr;       /* [n_ops_total + 1] parents of op g are parents[par_ptr[g] .. par_ptr[g + 1])   */
+    const int32_t* parents;       /* op indices within the model, in the graph's edge order                        */
+    const double*  need;          /* [n_ops_total] activation + parameter bytes of each op                         */
+    const int32_t* splits;        /* [max_degree + 1][n_ops_total] sub-ops of each op at each degree (>= 1)        */
+    const int32_t* cand_offset;   /* [n_cand + 1] servers of candidate c are cand_servers[cand_offset[c] ..)       */
+    const int32_t* cand_servers;  /* the servers of each candidate block in the placer's block order               */
+} ramp_env_placer_tables_t;
+int ramp_env_set_placer_tables(ramp_engine_t* eng, const ramp_env_placer_tables_t* tables);
+/* (model, degree, canonical_mask [n_words]) -> template_id; mount as ramp_env_set_template.  Replaces an existing entry. */
+int ramp_env_set_geometry_template(ramp_engine_t* eng, int32_t model, int32_t degree, const uint64_t* canonical_mask,
+                                   int32_t template_id, const double mount[6]);
 /* HOST copies of the outputs (any may be NULL) */
 /* The reference leaves step_stats['mean_mounted_worker_utilisation_frac'] / ['mean_cluster_worker_utilisation_frac'] as LISTS with
  * one entry per outer-loop iteration of the step (RCE:989-994); RAMP_SS_UTIL_*_SUM / RAMP_SS_NUM_TICKS carry their sum and length.
