@@ -26,20 +26,8 @@ namespace {
 constexpr int MAX_EVENT_PAIRS = 64;
 constexpr int RAMP_SMEM_CARVEOUT = 100;   // percent of the unified L1/shared array given to shared memory
 
-// Templates whose quotient blob does not fit shared memory run on the warp kernel (one lookahead per warp) or the CTA kernel
-// (one lookahead per CTA).  The warp kernel runs in 4-warp CTAs, or in 1-warp CTAs beside a CTA kernel: they fill the
-// registers and shared memory the CTA kernel leaves on every SM at a finer grain.
+// Templates whose quotient blob does not fit shared memory run on the CTA kernel (one lookahead per CTA).
 using LookaheadKernel = void (*)(const LookaheadArgs);
-constexpr int WARP_NT = 128, SPLIT_WARP_NT = 32;    // threads per CTA of the warp kernel alone / beside a CTA kernel
-LookaheadKernel warp_kernel() { return ramp_lookahead_kernel<WARP_NT / 32>; }
-LookaheadKernel split_warp_kernel() { return ramp_lookahead_kernel<SPLIT_WARP_NT / 32>; }
-
-// the dense shape of the warp kernel: smaller shared-memory frontiers, 16 instead of 12 lookahead warps per SM
-constexpr int DENSE_F_CAP = 256, DENSE_OPS_CAP = 32, DENSE_NT = 128;
-LookaheadKernel lookahead_dense_kernel() { return ramp_lookahead_kernel<DENSE_NT / 32, DENSE_F_CAP, DENSE_OPS_CAP>; }
-
-constexpr int64_t BIG_THRESHOLD = 60000;          // N + E from which one CTA per lookahead beats one warp (size class 1)
-constexpr double SPLIT_ALPHA = 1.3;               // 64-thread-CTA split while 2 n_big + n_small <= SPLIT_ALPHA x register slots
 constexpr int32_t RESIDENT_MAX_BYTES = 96 * 1024; // largest quotient blob that goes resident on the thread kernel
 
 LookaheadKernel lookahead_cta_kernel_for(int nt) {   // one CTA of nt threads per lookahead
@@ -145,26 +133,17 @@ struct ramp_engine {
     // lookahead scratch
     DeviceArray<unsigned char> d_scratch;
     uint64_t scratch_stride = 0;
-    int grid = 0;                // resident CTAs of the warp kernel's 4-warp shape
-    size_t smem_bytes = 0;
-    // CTA-per-lookahead variant (lower latency; used when a launch has fewer work items than warp slots)
-    int cta_nt = 0;              // 0 = pick 128 or 64 threads per launch; RAMP_LOOKAHEAD_CTA_THREADS forces one
-    int dense_grid = 0;          // resident CTAs of the dense warp-kernel shape
-    size_t dense_smem_bytes = 0;
-    double dense_factor = 2.0;   // the dense shape runs a step's lookaheads when there are more than dense_factor x warp slots
+    // CTA-per-lookahead kernel (templates that are not resident)
+    int cta_nt = 0;              // 0 = pick 256, 128 or 64 threads per launch; RAMP_LOOKAHEAD_CTA_THREADS forces one
     int cta_grid = 0;            // resident CTAs of the 128-thread variant
     int cta64_grid = 0;          // resident CTAs of the 64-thread variant
     int cta256_grid = 0;         // resident CTAs of the 256-thread variant
     int cta_grid_for(int nt) const { return nt == 256 ? cta256_grid : nt == 128 ? cta_grid : cta64_grid; }
     size_t cta_smem_bytes = 0;
-    size_t smem2_bytes = 0;      // dynamic shared memory of the 1-warp CTAs used beside a CTA kernel
     int debug = 0;               // RAMP_DEBUG=1 prints the launch decisions to stderr
-    int mode = 0;                // 0 auto, 1 warp-per-lookahead, 2 CTA-per-lookahead (RAMP_LOOKAHEAD_MODE); 1 and 2 make nothing resident
-    PinnedArray<int32_t> h_n_work;   // [4]
+    bool cta_only = false;       // RAMP_LOOKAHEAD_MODE=cta: nothing resident, every lookahead on the CTA kernel
+    PinnedArray<int32_t> h_n_work;   // [1] read-back of Counters::n_work
     PinnedArray<MemoStats> h_stats;  // [2] read-back of d_stats
-    DeviceArray<WorkItem> d_items_big;
-    Stream stream2;              // big lookaheads run concurrently with the small ones
-    Event ev_fork, ev_join;
     // resident (quotient) templates: thread-per-lookahead kernel
     int use_quotient = 1;        // 0 (RAMP_LOOKAHEAD_MODE=thread_unfolded): resident blobs are built from the unfolded job (identity quotient)
     int n_resident = 0, n_nonresident = 0;
@@ -215,7 +194,7 @@ struct ramp_engine {
     DeviceArray<ChunkDesc> sa_chunks;
     ResultArrays sa_res;
     int32_t sa_cap = 0;
-    DeviceArray<WorkItem> sa_items;      // [n]: the small, big and resident work lists, one after the other
+    DeviceArray<WorkItem> sa_items;      // [n]: the non-resident and resident work lists, one after the other
     DeviceArray<int32_t> sa_rank;        // [n] ramp_bucket_kernel scratch
     DeviceArray<Counters> sa_counters;
     // overlapped steps (ramp_step_device, DESIGN.md §4)
@@ -280,39 +259,10 @@ int resolve_events(ramp_engine* e) {
     return RAMP_OK;
 }
 
-// (re)allocates the per-CTA scratch slabs for the largest registered template and picks the grid
+// (re)allocates the per-CTA scratch slabs for the largest registered template and picks the CTA kernel's grids
 int ensure_scratch(ramp_engine* e) {
     const uint64_t trace_bytes = align_up((uint64_t)e->cfg.trace_cap * 12, 16);
     const uint64_t stride = align_up(std::max<uint64_t>(e->max_scratch, 16), 256) + align_up(trace_bytes, 256);
-    const size_t smem = lookahead_smem_per_warp(e->max_w, e->max_c, e->par_cap) * (size_t)(WARP_NT / 32);
-    if (smem > 200 * 1024)
-        return set_error(RAMP_ERR_CAPACITY, "a template needs %zu B of shared memory for its worker/channel key arrays (max 200 KiB)", smem);
-    if (smem != e->smem_bytes || e->grid == 0) {
-        LookaheadKernel kern = warp_kernel();
-        CUDA_TRY(reserve_dynamic_smem((const void*)kern, smem));
-        // all lookahead kernels ask for the same L1/shared split: kernels with different carve-outs cannot share an SM,
-        // which would serialise the CTA kernel and the warp kernel when they are launched side by side
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
-        int occ = 0;
-        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, WARP_NT, smem));
-        if (occ < 1) occ = 1;
-        e->grid = e->sm_count * occ;     // persistent CTAs: a whole number of waves (SMs x resident CTAs per SM)
-        e->smem_bytes = smem;
-        // the block scheduler spreads the 1-warp CTAs used beside a CTA kernel and the CTA kernel's over all SMs
-        const size_t smem2 = lookahead_smem_per_warp(e->max_w, e->max_c, e->par_cap) * (size_t)(SPLIT_WARP_NT / 32);
-        LookaheadKernel kern2 = split_warp_kernel();
-        CUDA_TRY(reserve_dynamic_smem((const void*)kern2, smem2));
-        CUDA_TRY(cudaFuncSetAttribute(kern2, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
-        e->smem2_bytes = smem2;
-        const size_t smem_d = lookahead_smem_per_warp(e->max_w, e->max_c, e->par_cap, DENSE_F_CAP, DENSE_OPS_CAP) * (size_t)(DENSE_NT / 32);
-        LookaheadKernel kern_d = lookahead_dense_kernel();
-        CUDA_TRY(reserve_dynamic_smem((const void*)kern_d, smem_d));
-        CUDA_TRY(cudaFuncSetAttribute(kern_d, cudaFuncAttributePreferredSharedMemoryCarveout, RAMP_SMEM_CARVEOUT));
-        int occ_d = 0;
-        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_d, kern_d, DENSE_NT, smem_d));
-        e->dense_grid = e->sm_count * std::max(occ_d, 1);
-        e->dense_smem_bytes = smem_d;
-    }
     const size_t cta_smem = lookahead_cta_smem(e->max_w, e->max_c, e->par_cap);
     if (cta_smem > 200 * 1024)
         return set_error(RAMP_ERR_CAPACITY, "a template needs %zu B of shared memory (max 200 KiB)", cta_smem);
@@ -324,12 +274,13 @@ int ensure_scratch(ramp_engine* e) {
             int occ = 0;
             CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, nt, cta_smem));
             if (occ < 1) occ = 1;
+            // persistent CTAs: a whole number of waves (SMs x resident CTAs per SM)
             (nt == 256 ? e->cta256_grid : nt == 128 ? e->cta_grid : e->cta64_grid) = e->sm_count * occ;
         }
         e->cta_smem_bytes = cta_smem;
     }
-    // one slab per lookahead in flight; the warp kernel and one of the CTA kernels may run side by side
-    const int n_slabs = std::max(e->grid * (WARP_NT / 32) + std::max(e->cta_grid, e->cta64_grid), e->dense_grid * (DENSE_NT / 32));
+    // one slab per CTA of the largest grid: one CTA kernel runs at a time, on the engine stream
+    const int n_slabs = std::max({e->cta256_grid, e->cta_grid, e->cta64_grid});
     if (stride != e->scratch_stride || stride * (uint64_t)n_slabs != e->d_scratch.size()) {
         CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
         CUDA_TRY(e->d_scratch.alloc(stride * (uint64_t)n_slabs));
@@ -344,8 +295,6 @@ LookaheadArgs make_lookahead_args(ramp_engine* e, const WorkItem* items, Counter
     a.templates = e->d_templates.get();
     a.items = items;
     a.n_work = &counters->n_work;
-    a.items_b = nullptr;
-    a.n_work_b = nullptr;
     a.cursor = &counters->work_cursor;
     a.scratch = e->d_scratch.get();
     a.scratch_stride = e->scratch_stride;
@@ -550,80 +499,29 @@ void bucket_resident(ramp_engine* e, const WorkItem* items, Counters* c, WorkIte
 
 // Launches the lookaheads of a step or of a standalone run (ramp_run_lookaheads), so both pick kernels by the same rule.
 // The resident ones, already bucketed into chunks, run on the thread kernel over thread_grid CTAs (0: there are none).  The
-// others come as two work lists whose sizes the host knows: small (list 0 of `c`) and big (list 1).
+// n others (list 0 of `c`, a count the host knows) run on the CTA kernel after them.
 int launch_lookaheads(ramp_engine* e, const ChunkDesc* chunks, const WorkItem* chunk_items, int thread_grid,
-                      const WorkItem* items, int n_small, const WorkItem* items_big, int n_big, Counters* c,
-                      const ResultSlots& res, const TracePool& pool, MemoStats* stats, cudaStream_t st) {
+                      const WorkItem* items, int n, Counters* c, const ResultSlots& res, const TracePool& pool,
+                      MemoStats* stats, cudaStream_t st) {
     if (thread_grid > 0) {
         ThreadArgs ta = make_thread_args(e, chunks, chunk_items, c, res, pool, stats);
         ramp_lookahead_thread_kernel<<<thread_grid, RAMP_THREAD_CTA, e->res_smem, st>>>(ta);
         e->launches++;
     }
-    if (n_small + n_big == 0) return RAMP_OK;
-    LookaheadArgs a = make_lookahead_args(e, items, c, res, pool, stats);
-    LookaheadArgs ab = a;
-    ab.items = items_big; ab.n_work = &c->n_work_big; ab.cursor = &c->work_cursor_big;
-    const int wpb = WARP_NT / 32;
-    const int warp_slots = e->grid * wpb;
-    // The big lookaheads set the latency, the small ones the load.  While everything fits the SMs' warp slots at once
-    // (registers cap every mix at cta_grid x 4 warps) each big lookahead gets a 256-thread CTA if 8 warps per big one still
-    // fit (2.4 ms instead of 2.9 ms for the bench job), else a 128-thread CTA; while the big ones still fit as 64-thread CTAs
-    // and the small ones need at most a short second wave they get those; beyond that everything goes through the warp
-    // kernel, the big list first (longest-processing-time-first keeps the tail short).  The CTA kernel runs on a second
-    // stream beside the warp kernel for the small list.
+    if (n == 0) return RAMP_OK;
+    // Each lookahead sets the latency.  While they all fit the SMs at once (registers cap the CTA kernel at cta_grid x 4
+    // warps) each gets a 256-thread CTA if 8 warps per lookahead still fit (2.4 ms instead of 2.9 ms for the bench job), else a
+    // 128-thread CTA; beyond that 64-thread CTAs, persistent over as many waves as it takes.  RAMP_LOOKAHEAD_CTA_THREADS
+    // overrides the thread count.
     const int reg_slots = e->cta_grid * 4;
-    int split_nt = 0;
-    if (e->mode != 1 && n_big > 0) {
-        if (n_big <= e->cta256_grid && 8 * n_big + n_small <= reg_slots) split_nt = 256;
-        else if (n_big <= e->cta_grid && 4 * n_big + n_small <= reg_slots) split_nt = 128;
-        else if (n_big <= e->cta64_grid && 2 * n_big + n_small <= (int)(SPLIT_ALPHA * reg_slots)) split_nt = 64;
-    }
-    const bool split = split_nt != 0;
-    if (e->debug) fprintf(stderr, "[ramp] lookaheads: small=%d big=%d warp_slots=%d reg_slots=%d -> %s %d\n", n_small, n_big,
-                          warp_slots, reg_slots, split ? "split (CTA || warp), CTA threads" : "single warp kernel, big first", split_nt);
-    if (split) {
-        // the second stream starts after all that is queued on `st`: a standalone run's uploads and bucket kernel, the
-        // thread kernel
-        CUDA_TRY(cudaEventRecord(e->ev_fork.get(), st));
-        CUDA_TRY(cudaStreamWaitEvent(e->stream2.get(), e->ev_fork.get(), 0));
-        const int grid = std::min(n_big, e->cta_grid_for(split_nt));
-        lookahead_cta_kernel_for(split_nt)<<<grid, split_nt, e->cta_smem_bytes, e->stream2.get()>>>(ab);
-        CUDA_TRY(cudaEventRecord(e->ev_join.get(), e->stream2.get()));
-        e->launches++;
-        if (n_small > 0) {
-            LookaheadArgs as = a;
-            as.scratch = a.scratch + (uint64_t)std::max(e->cta_grid, e->cta64_grid) * a.scratch_stride;   // slabs past the CTA kernel's
-            const int wpb2 = SPLIT_WARP_NT / 32;
-            const int g2 = std::max(1, std::min(e->grid * wpb / wpb2, (n_small + wpb2 - 1) / wpb2));   // never more warps than slabs
-            split_warp_kernel()<<<g2, SPLIT_WARP_NT, e->smem2_bytes, st>>>(as);
-            e->launches++;
-        }
-        CUDA_TRY(cudaStreamWaitEvent(st, e->ev_join.get(), 0));
-    } else if (e->mode == 2) {
-        // each list on a CTA kernel of its own: RAMP_LOOKAHEAD_CTA_THREADS threads per CTA, else 128 while the list fits
-        // one wave of them and 64 beyond
-        auto cta_list = [&](const LookaheadArgs& l, int n) {
-            const int nt = e->cta_nt ? e->cta_nt : (n <= e->cta_grid ? 128 : 64);
-            lookahead_cta_kernel_for(nt)<<<std::min(e->cta_grid_for(nt), n), nt, e->cta_smem_bytes, st>>>(l);
-            e->launches++;
-        };
-        if (n_big > 0) cta_list(ab, n_big);
-        if (n_small > 0) cta_list(a, n_small);
-    } else {
-        LookaheadArgs all = ab;                      // list A = big, list B = small, one cursor
-        all.items_b = items; all.n_work_b = &c->n_work;
-        const int n_all = n_small + n_big;
-        if (e->mode == 0 && e->dense_grid * (DENSE_NT / 32) > warp_slots && n_all > (int)(e->dense_factor * warp_slots)) {
-            // far more lookaheads than slots: throughput matters, not the latency of one -> 16 warps per SM
-            const int wd = DENSE_NT / 32;
-            const int g = std::max(1, std::min(e->dense_grid, (n_all + wd - 1) / wd));
-            lookahead_dense_kernel()<<<g, DENSE_NT, e->dense_smem_bytes, st>>>(all);
-        } else {
-            const int g = std::max(1, std::min(e->grid, (n_all + wpb - 1) / wpb));
-            warp_kernel()<<<g, WARP_NT, e->smem_bytes, st>>>(all);
-        }
-        e->launches++;
-    }
+    int nt = 64;
+    if (n <= e->cta256_grid && 8 * n <= reg_slots) nt = 256;
+    else if (n <= e->cta_grid && 4 * n <= reg_slots) nt = 128;
+    if (e->cta_nt) nt = e->cta_nt;
+    const int grid = std::min(n, e->cta_grid_for(nt));
+    if (e->debug) fprintf(stderr, "[ramp] lookaheads: non-resident=%d reg_slots=%d -> CTA threads %d, grid %d\n", n, reg_slots, nt, grid);
+    lookahead_cta_kernel_for(nt)<<<grid, nt, e->cta_smem_bytes, st>>>(make_lookahead_args(e, items, c, res, pool, stats));
+    e->launches++;
     return RAMP_OK;
 }
 
@@ -828,14 +726,15 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
         e->cta_nt = nt;
     }
     if (const char* v = getenv("RAMP_LOOKAHEAD_MODE")) {
-        // warp / cta: every template goes to that kernel (no resident quotient blobs); thread_unfolded: the thread kernel on
-        // the unfolded job (identity quotient); anything else: automatic (resident whenever the quotient blob fits)
-        e->mode = !strcmp(v, "warp") ? 1 : !strcmp(v, "cta") ? 2 : 0;
-        if (!strcmp(v, "thread_unfolded")) e->use_quotient = 0;
+        // auto (or thread): resident whenever the quotient blob fits; cta: every template on the CTA kernel (no resident
+        // quotient blobs); thread_unfolded: the thread kernel on the unfolded job (identity quotient)
+        if (!strcmp(v, "cta")) e->cta_only = true;
+        else if (!strcmp(v, "thread_unfolded")) e->use_quotient = 0;
+        else if (strcmp(v, "auto") != 0 && strcmp(v, "thread") != 0)
+            return set_error(RAMP_ERR_BAD_ARG, "RAMP_LOOKAHEAD_MODE must be auto, thread, thread_unfolded or cta, not '%s'", v);
     }
     if (const char* v = getenv("RAMP_DEBUG")) e->debug = atoi(v);
     if (const char* v = getenv("RAMP_STEP_OVERLAP")) e->overlap = atoi(v) != 0;   // 0: the in-order path only (tests compare the two)
-    if (const char* v = getenv("RAMP_DENSE_FACTOR")) e->dense_factor = atof(v);
     cudaDeviceProp prop{};
     CUDA_TRY(cudaGetDeviceProperties(&prop, cfg.device));
     e->sm_count = prop.multiProcessorCount;
@@ -866,7 +765,7 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     CUDA_TRY(e->pool.alloc(std::max<uint64_t>(4ull << 20, (uint64_t)B * 8ull * 2048ull)));      // B=1: 48 MiB; B=4096: 805 MiB
     CUDA_TRY(cudaMemset(e->pool.top.get(), 0, sizeof(unsigned long long)));
 
-    CUDA_TRY(alloc_each(B, e->d_items, e->d_items_big, e->d_items_res, e->d_chunks, e->d_rank, e->d_actions, e->d_n_cluster_steps));
+    CUDA_TRY(alloc_each(B, e->d_items, e->d_items_res, e->d_chunks, e->d_rank, e->d_actions, e->d_n_cluster_steps));
     CUDA_TRY(e->d_chunk_items.alloc((size_t)B * 32));
     CUDA_TRY(alloc_each((size_t)cfg.max_templates + 1, e->d_tcount, e->d_tbase));
     CUDA_TRY(cudaMemset(e->d_tcount.get(), 0, sizeof(int32_t) * ((size_t)cfg.max_templates + 1)));
@@ -874,9 +773,6 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     CUDA_TRY(cudaMemset(e->d_hints.get(), 0, sizeof(TemplateHints) * (size_t)cfg.max_templates));
     CUDA_TRY(e->d_hint_jct.alloc(cfg.max_templates));
     CUDA_TRY(cudaMemset(e->d_hint_jct.get(), 0, sizeof(double) * (size_t)cfg.max_templates));
-    CUDA_TRY(create(e->stream2, cudaStreamNonBlocking));
-    CUDA_TRY(create(e->ev_fork, cudaEventDisableTiming));
-    CUDA_TRY(create(e->ev_join, cudaEventDisableTiming));
     CUDA_TRY(e->d_counters.alloc(1));
     CUDA_TRY(e->d_stats.alloc(2));
     CUDA_TRY(cudaMemset(e->d_counters.get(), 0, sizeof(Counters)));
@@ -884,7 +780,7 @@ int ramp_engine_create(const ramp_config_t* cfg_in, ramp_engine_t** out) {
     CUDA_TRY(e->d_step_stats.alloc((size_t)RAMP_STEP_STATS_LEN * B));
     CUDA_TRY(e->d_ep_export.alloc((size_t)RAMP_EP_LEN * B));
     CUDA_TRY(e->d_es_export.alloc((size_t)RAMP_ES_LEN * B));
-    CUDA_TRY(e->h_n_work.alloc(4));
+    CUDA_TRY(e->h_n_work.alloc(1));
     CUDA_TRY(e->h_stats.alloc(2));
 
     EpisodeState& ep = e->ep;
@@ -1041,7 +937,7 @@ int ramp_register_template(ramp_engine_t* e, const ramp_lowered_job_t* j, int32_
     d.n_ops = N; d.n_deps = E; d.n_workers = W; d.n_channels = C;
     d.num_training_steps = j->num_training_steps; d.model_id = j->model_id; d.degree = j->degree;
     d.n_src = (int32_t)src.size(); d.canon_id = canon;
-    d.size_class = ((int64_t)N + (int64_t)E >= BIG_THRESHOLD) ? 1 : 0;
+    d.size_class = 0;
     d.par_in_smem = par_in_smem ? 1 : 0;
     d._pad0 = 0;
     d.op_rec = (const int4*)(base + segs[0].off); d.op_n_parents = (const uint16_t*)(base + segs[1].off);
@@ -1052,7 +948,7 @@ int ramp_register_template(ramp_engine_t* e, const ramp_lowered_job_t* j, int32_
     d.algorithmic_bytes_static = 20ull * (uint64_t)N + 19ull * (uint64_t)E + 24ull;
     // ---- symmetry quotient -> resident blob for the thread-per-lookahead kernel ----
     d.res_blob = nullptr; d.res_bytes = 0; d.res_n_ops = 0; d.res_n_deps = 0; d._pad2 = 0;
-    if (e->mode == 0) {
+    if (!e->cta_only) {
         ramp_quotient_t q{};
         const int qrc = e->use_quotient ? ramp_quotient_template(j, &q) : identity_quotient(j, &q);
         if (qrc != RAMP_OK) return set_error(qrc, "ramp_quotient_template failed (%d)", qrc);
@@ -1076,7 +972,7 @@ int ramp_register_template(ramp_engine_t* e, const ramp_lowered_job_t* j, int32_
     const int32_t id = (int32_t)e->templates.size();
     CUDA_TRY(cudaMemcpy(e->d_templates.get() + id, &d, sizeof(TemplateDev), cudaMemcpyHostToDevice));
     if (d.size_class == 2) e->n_resident++; else e->n_nonresident++;
-    if (d.size_class != 2) {       // the warp / CTA kernels' slabs and shared-memory tables are sized by the jobs that use them
+    if (d.size_class != 2) {       // the CTA kernel's slabs and shared-memory tables are sized by the jobs that use them
         e->max_scratch = std::max(e->max_scratch, d.scratch_bytes);
         e->max_w = std::max(e->max_w, W);
         e->max_c = std::max(e->max_c, std::max(C, 1));
@@ -1164,18 +1060,18 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
     if (e->n_nonresident > 0) { int rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
     if (e->n_resident > 0) { int rc = ensure_thread_scratch(e); if (rc != RAMP_OK) return rc; }
     // the overlapped path covers per-episode memo keys on resident templates; steps with engine-written actions, a template
-    // on the warp / CTA kernels (their launch shape needs the work counts on the host) or another memo mode run in order
+    // on the CTA kernel (its launch shape needs the work count on the host) or another memo mode run in order
     if (e->overlap && e->cfg.memo_mode == RAMP_MEMO_REFERENCE && e->n_nonresident == 0 && e->n_resident > 0 && !engine_owned(e, d_actions))
         return step_overlapped(e, d_actions, fuse, d_stats_out, d_ncs_out);
     const int B = e->cfg.n_episodes;
     cudaStream_t st = e->stream.get();
-    CUDA_TRY(cudaMemsetAsync(e->d_counters.get(), 0, 4 * sizeof(int32_t), st));   // both work lists' counts and cursors
+    CUDA_TRY(cudaMemsetAsync(e->d_counters.get(), 0, 2 * sizeof(int32_t), st));   // n_work and work_cursor
     PlanArgs p{};
     p.actions = d_actions; p.templates = e->d_templates.get(); p.n_templates = (int32_t)e->templates.size();
     p.ep = e->ep; p.memo.keys = e->d_memo_keys.get(); p.memo.mask = e->memo_cap - 1; p.memo.mode = e->cfg.memo_mode;
     p.memo.vals = e->d_memo_vals.get(); p.memo.keys2 = e->d_memo_keys2.get(); p.memo.mask2 = e->memo_cap2 - 1;
     p.memo.slot2_base = (int32_t)e->memo_cap + e->cfg.n_episodes;
-    p.items = e->d_items.get(); p.items_big = e->d_items_big.get(); p.items_res = e->d_items_res.get(); p.counters = e->d_counters.get(); p.stats = e->d_stats.get();
+    p.items = e->d_items.get(); p.items_res = e->d_items_res.get(); p.counters = e->d_counters.get(); p.stats = e->d_stats.get();
     ramp_plan_kernel<<<(B + 127) / 128, 128, 0, st>>>(p);
     e->launches++;
     if (!e->templates.empty()) {
@@ -1185,16 +1081,16 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
         // CTAs find the chunk cursor exhausted and exit.
         if (e->n_resident > 0) bucket_resident(e, e->d_items_res.get(), e->d_counters.get(), e->d_chunk_items.get(), e->d_chunks.get(), e->d_rank.get(),
                                         e->d_tcount.get(), e->d_tbase.get(), st);
-        int n_small = 0, n_big = 0;
+        int n_nonres = 0;
         if (e->n_nonresident > 0) {
-            // the number of memo misses of each size class decides the kernel shapes: a 16-byte read-back (~10 us) against
-            // multi-ms kernels
-            CUDA_TRY(cudaMemcpyAsync(e->h_n_work.get(), &e->d_counters.get()->n_work, sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
+            // the number of memo misses on non-resident templates decides the CTA kernel's shape: a 4-byte read-back (~10 us)
+            // against multi-ms kernels
+            CUDA_TRY(cudaMemcpyAsync(e->h_n_work.get(), &e->d_counters.get()->n_work, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));
-            n_small = e->h_n_work.get()[0]; n_big = e->h_n_work.get()[2];
+            n_nonres = e->h_n_work.get()[0];
         }
-        int rc = launch_lookaheads(e, e->d_chunks.get(), e->d_chunk_items.get(), e->n_resident > 0 ? e->res_grid : 0, e->d_items.get(), n_small,
-                                   e->d_items_big.get(), n_big, e->d_counters.get(), e->res.view(), e->pool.view(), e->d_stats.get(), st);
+        int rc = launch_lookaheads(e, e->d_chunks.get(), e->d_chunk_items.get(), e->n_resident > 0 ? e->res_grid : 0, e->d_items.get(), n_nonres,
+                                   e->d_counters.get(), e->res.view(), e->pool.view(), e->d_stats.get(), st);
         if (rc != RAMP_OK) return rc;
         CUDA_TRY(cudaEventRecord(e->ev_b[e->ev_pending].get(), st));
         e->ev_pending++;
@@ -1350,19 +1246,20 @@ int ramp_run_lookaheads(ramp_engine_t* e, const int32_t* template_ids, int32_t n
     for (int32_t k = 0; k < n; ++k)
         if (template_ids[k] < 0 || template_ids[k] >= (int32_t)e->templates.size())
             return set_error(RAMP_ERR_BAD_ARG, "template id %d at %d is not registered", template_ids[k], k);
-    // the step's three work lists, by size class: small and big (warp / CTA kernels), resident (thread kernel), each in item order
-    std::vector<WorkItem> lists[3];
+    // the step's two work lists: non-resident (CTA kernel) and resident (thread kernel), each in item order
+    std::vector<WorkItem> lists[2];
     std::vector<int32_t> per_template(e->templates.size(), 0);
     for (int32_t k = 0; k < n; ++k) {
-        const int32_t t = template_ids[k], size_class = e->templates[t].dev.size_class;
-        lists[size_class].push_back(WorkItem{t, k, -1, 0});
-        if (size_class == 2) per_template[t]++;
+        const int32_t t = template_ids[k];
+        const bool resident = e->templates[t].dev.size_class == 2;
+        lists[resident].push_back(WorkItem{t, k, -1, 0});
+        if (resident) per_template[t]++;
     }
-    const int n_small = (int)lists[0].size(), n_big = (int)lists[1].size(), n_res = (int)lists[2].size();
+    const int n_nonres = (int)lists[0].size(), n_res = (int)lists[1].size();
     int n_chunks = 0;                   // what ramp_bucket_kernel will make of the resident list
     for (int32_t m : per_template) n_chunks += (m + 31) / 32;
     int rc = RAMP_OK;
-    if (n_small + n_big > 0) { rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
+    if (n_nonres > 0) { rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
     if (n_res > 0) { rc = ensure_thread_scratch(e); if (rc != RAMP_OK) return rc; }
     cudaStream_t st = e->stream.get();
     if (n > e->sa_cap) {
@@ -1376,10 +1273,9 @@ int ramp_run_lookaheads(ramp_engine_t* e, const int32_t* template_ids, int32_t n
     std::vector<WorkItem> items;
     items.reserve(n);
     for (const auto& l : lists) items.insert(items.end(), l.begin(), l.end());
-    WorkItem* const d_small = e->sa_items.get();
-    WorkItem* const d_big = d_small + n_small;
-    WorkItem* const d_res = d_big + n_big;
-    Counters c{}; c.n_work = n_small; c.n_work_big = n_big; c.n_work_res = n_res;
+    WorkItem* const d_nonres = e->sa_items.get();
+    WorkItem* const d_res = d_nonres + n_nonres;
+    Counters c{}; c.n_work = n_nonres; c.n_work_res = n_res;
     CUDA_TRY(cudaMemcpyAsync(e->sa_items.get(), items.data(), sizeof(WorkItem) * n, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(e->sa_counters.get(), &c, sizeof(Counters), cudaMemcpyHostToDevice, st));
     if (n_res > 0) bucket_resident(e, d_res, e->sa_counters.get(), e->sa_chunk_items.get(), e->sa_chunks.get(), e->sa_rank.get(),
@@ -1397,8 +1293,8 @@ int ramp_run_lookaheads(ramp_engine_t* e, const int32_t* template_ids, int32_t n
     cudaEvent_t ea = e->ev_a[MAX_EVENT_PAIRS - 1].get(), eb = e->ev_b[MAX_EVENT_PAIRS - 1].get();
     if (e->ev_pending >= MAX_EVENT_PAIRS - 1) { CUDA_TRY(cudaStreamSynchronize(st)); rc = resolve_events(e); if (rc) return rc; }
     CUDA_TRY(cudaEventRecord(ea, st));
-    rc = launch_lookaheads(e, e->sa_chunks.get(), e->sa_chunk_items.get(), n_res > 0 ? std::min(e->res_grid, n_chunks) : 0, d_small, n_small,
-                           d_big, n_big, e->sa_counters.get(), e->sa_res.view(), pool, nullptr, st);
+    rc = launch_lookaheads(e, e->sa_chunks.get(), e->sa_chunk_items.get(), n_res > 0 ? std::min(e->res_grid, n_chunks) : 0, d_nonres, n_nonres,
+                           e->sa_counters.get(), e->sa_res.view(), pool, nullptr, st);
     if (rc != RAMP_OK) return rc;
     CUDA_TRY(cudaEventRecord(eb, st));
     CUDA_TRY(cudaGetLastError());

@@ -3,7 +3,7 @@
 // Reference semantics (cwfparsonson/ddls @ 9e0b5ba; RCE = ddls/environments/ramp_cluster/
 // ramp_cluster_environment.py, JOB = ddls/demands/jobs/job.py):
 //   ramp_plan_kernel       memo lookup/insert of _perform_lookahead_job_completion_time   RCE:469-518, 269-275
-//   ramp_lookahead_kernel  _run_lookahead tick loop                                        RCE:379-467
+//   ramp_lookahead_cta_kernel / ramp_lookahead_thread_kernel  _run_lookahead tick loop    RCE:379-467
 //   ramp_step_kernel       step(): block/mount/register lookahead/outer event loop/stats    RCE:894-1167
 //
 // All simulation arithmetic is IEEE f64 without FMA contraction (compile with -fmad=false), in the
@@ -34,7 +34,7 @@ struct TemplateDev {
     int32_t n_ops, n_deps, n_workers, n_channels;
     int32_t num_training_steps, model_id, degree, n_src;
     int32_t canon_id;           // id of the first registered byte-identical template (exact memo key)
-    int32_t size_class;         // 0: small (one warp per lookahead is fastest), 1: big (one CTA per lookahead is fastest),
+    int32_t size_class;         // 0: not resident (one CTA per lookahead, ramp_lookahead_cta_kernel),
                                 // 2: resident (quotient blob in shared memory, one THREAD per lookahead)
     int32_t par_in_smem;        // parent counters fit the shared-memory byte counters (max in-degree <= 255, N <= par_cap)
     int32_t _pad0;
@@ -52,7 +52,7 @@ struct TemplateDev {
     uint64_t scratch_bytes;       // HBM-side dynamic state one running lookahead of this template may need
     uint64_t algorithmic_bytes_static; // 20 N + 19 E + 24 (SURVEY.md 8d), + 12 T added per run
     // symmetry quotient (ramp_quotient.cpp) packed for the thread-per-lookahead kernel (ramp_lookahead_thread.cuh): one blob
-    // that is bulk-copied into shared memory; null when the job is not resident-eligible (size_class 0 / 1 then)
+    // that is bulk-copied into shared memory; null when the job is not resident-eligible (size_class 0 then)
     const unsigned char* res_blob;
     int32_t res_bytes;            // multiple of 16
     int32_t res_n_ops, res_n_deps, _pad2;
@@ -84,11 +84,9 @@ struct TracePool {
     uint64_t len;
 };
 
-struct Counters {               // the first four words are zeroed at the start of every step
-    int32_t n_work;             // work list 0: small lookaheads (or all of them for standalone runs)
+struct Counters {               // the first two words (n_work, work_cursor) are zeroed at the start of every step
+    int32_t n_work;             // work list 0: lookaheads on non-resident templates (the CTA kernel)
     int32_t work_cursor;
-    int32_t n_work_big;         // work list 1: big lookaheads
-    int32_t work_cursor_big;
     int32_t err_episode;        // first episode that recorded an error (+1), 0 if none
     int32_t err_status;
     int32_t n_work_res;         // work list 2: lookaheads on resident (quotient) templates; zeroed at the start of every step
@@ -155,11 +153,9 @@ struct MemoTable {
 
 struct LookaheadArgs {
     const TemplateDev* templates;
-    const WorkItem* items;      // work list A, consumed first (the big lookaheads: longest-processing-time-first)
-    const int32_t* n_work;      // device-side count of list A
-    const WorkItem* items_b;    // work list B, consumed after A (may be null)
-    const int32_t* n_work_b;    // device-side count of list B (may be null)
-    int32_t* cursor;            // device-side work cursor over A then B (persistent warps / CTAs pull items)
+    const WorkItem* items;      // the work list
+    const int32_t* n_work;      // its device-side count
+    int32_t* cursor;            // device-side work cursor over it (persistent CTAs pull items)
     unsigned char* scratch;     // [gridDim.x][scratch_stride]
     uint64_t scratch_stride;
     ResultSlots res;
@@ -172,8 +168,8 @@ struct LookaheadArgs {
 
 __host__ __device__ inline uint64_t align_up(uint64_t x, uint64_t a) { return (x + a - 1) / a * a; }
 
-// HBM-side dynamic state of one running lookahead, carved out of the owning warp's scratch slab.  The hot state
-// (op frontier, the first RAMP_F_CAP entries of the dep frontier, per-worker / per-channel winners) lives in
+// HBM-side dynamic state of one running lookahead, carved out of the owning CTA's scratch slab.  The hot state
+// (op frontier, the first RAMP_CTA_F_CAP entries of the dep frontier, per-worker / per-channel winners) lives in
 // shared memory; HBM holds the parent counters, the overflow of the two frontiers and the tick trace.
 struct ScratchView {
     uint32_t* par_done;              // [N] len(parent_deps_completed) JOB:530
@@ -181,7 +177,7 @@ struct ScratchView {
     int2*     ops_b_ovf[2];          // [N]
     unsigned long long* f_km_ovf;    // [E] overflow of the shared-memory dep frontier: packed dep words
     double*   f_rem_ovf;             // [E]                                              remaining times
-    unsigned long long* f_km_ovf2;   // [E] second buffer (CTA-per-lookahead kernel compacts by ping-pong)
+    unsigned long long* f_km_ovf2;   // [E] second buffer (the CTA kernel compacts by ping-pong)
     double*   f_rem_ovf2;            // [E]
     unsigned long long* nf_ovf;      // [E] overflow of the shared-memory list of ready non-flow deps
     int32_t*  rq_ovf;                // [N] overflow of the CTA kernel's queue of ops readied in the current tick
@@ -265,11 +261,8 @@ __device__ __forceinline__ double util_sum(const double* term, int n_rec) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// _run_lookahead (RCE:379-467): ONE WARP per lookahead; WPB independent warps per CTA; persistent warps pull
-// work items from a device-side cursor.  No block barriers: per-tick frontiers are tens to hundreds of
-// items, so a warp keeps its lanes busy and all cross-lane traffic is shuffles / ballots / shared atomics.
-// A lone warp is bound by dependent memory round trips, so the ready frontiers are staged in shared memory
-// (HBM only on overflow) and the remaining global phases issue a whole batch of loads before consuming any.
+// Building blocks of _run_lookahead (RCE:379-467) on one CTA per lookahead (ramp_lookahead_cta.cuh).  The ready frontiers
+// are staged in shared memory (HBM only on overflow) and the global phases issue a whole batch of loads before consuming any.
 //
 // Per tick (letters as in SURVEY.md 3.3):
 //   A  per-worker arg-max over ready ops           -> atomicMax of rank keys into smem wkey[]      (RCE:562-590, 44-67)
@@ -284,53 +277,26 @@ __device__ __forceinline__ double util_sum(const double* term, int n_rec) {
 //   E  tick = min(t_op, t_comm)                                                                     (RCE:426)
 //   H  every flow of the pre-tick snapshot: rem -= min(tick, rem); == 0 -> completed: atomicAdd on the child's parent
 //      counter, == n_parents -> the child is readied (its op index is queued; the 24-byte records of all ops readied in
-//      the tick are fetched in ONE batch, the loads overlapping G).  Survivors are slid down in place. (RCE:733-775)
+//      the tick are fetched in ONE batch)                                                               (RCE:733-775)
 //   G  op winners: same; completed -> the CSR rows of all ops completed in this tick are appended to the flow frontier /
 //      the non-flow list as one flattened, coalesced copy (first ticked next tick == the RCE:429 snapshot). (RCE:691-716)
-//   I,J lane 0 accumulates t / comm / comp and the trace in tick order                              (RCE:442-445, 777-791)
+//   I,J one thread accumulates t / comm / comp and the trace in tick order                           (RCE:442-445, 777-791)
 #ifndef RAMP_U
 #define RAMP_U 2            // batch depth: independent loads in flight per lane per phase
 #endif
 #ifndef RAMP_OPS_CAP
 #define RAMP_OPS_CAP 48     // op-frontier records kept in shared memory per buffer (overflow goes to HBM)
 #endif
-#ifndef RAMP_F_CAP
-#define RAMP_F_CAP 384      // flow-frontier entries kept in shared memory (overflow goes to HBM); sized so that 12 lookahead warps fit an SM
-#endif
-
 #ifndef RAMP_NF_CAP
 #define RAMP_NF_CAP 64      // ready non-flow deps kept in shared memory (they live for exactly one tick)
 #endif
 
 struct OpsView { int4* a_sm; int2* b_sm; int4* a_ovf; int2* b_ovf; };
-template <int OC = RAMP_OPS_CAP>
 __device__ __forceinline__ void ops_get(const OpsView& v, int k, int4& ra, int2& rb) {
-    if (k < OC) { ra = v.a_sm[k]; rb = v.b_sm[k]; } else { ra = v.a_ovf[k - OC]; rb = v.b_ovf[k - OC]; }
+    if (k < RAMP_OPS_CAP) { ra = v.a_sm[k]; rb = v.b_sm[k]; } else { ra = v.a_ovf[k - RAMP_OPS_CAP]; rb = v.b_ovf[k - RAMP_OPS_CAP]; }
 }
-template <int OC = RAMP_OPS_CAP>
 __device__ __forceinline__ void ops_put(const OpsView& v, int k, const int4 ra, const int2 rb) {
-    if (k < OC) { v.a_sm[k] = ra; v.b_sm[k] = rb; } else { v.a_ovf[k - OC] = ra; v.b_ovf[k - OC] = rb; }
-}
-// dep frontier entry = the packed dep word (TemplateDev::dep_kd) + the remaining time: 16 B
-// a readied op is first recorded as its op index only (in the row slot); its 24-byte record is fetched later, all
-// records of a tick in one batch, so that the tick waits for ONE L2 round trip instead of one per 32-dep group
-template <int OC = RAMP_OPS_CAP>
-__device__ __forceinline__ void ops_put_child(const OpsView& v, int k, int child) {
-    if (k < OC) v.b_sm[k] = make_int2(child, 0); else v.b_ovf[k - OC] = make_int2(child, 0);
-}
-template <int OC = RAMP_OPS_CAP>
-__device__ __forceinline__ int ops_get_child(const OpsView& v, int k) {
-    return (k < OC) ? v.b_sm[k].x : v.b_ovf[k - OC].x;
-}
-
-struct FrontView { unsigned long long* kd_sm; double* rem_sm; unsigned long long* kd_ovf; double* rem_ovf; };
-template <int FC = RAMP_F_CAP>
-__device__ __forceinline__ void f_get(const FrontView& v, int k, unsigned long long& kd, double& rem) {
-    if (k < FC) { kd = v.kd_sm[k]; rem = v.rem_sm[k]; } else { kd = v.kd_ovf[k - FC]; rem = v.rem_ovf[k - FC]; }
-}
-template <int FC = RAMP_F_CAP>
-__device__ __forceinline__ void f_put(const FrontView& v, int k, unsigned long long kd, double rem) {
-    if (k < FC) { v.kd_sm[k] = kd; v.rem_sm[k] = rem; } else { v.kd_ovf[k - FC] = kd; v.rem_ovf[k - FC] = rem; }
+    if (k < RAMP_OPS_CAP) { v.a_sm[k] = ra; v.b_sm[k] = rb; } else { v.a_ovf[k - RAMP_OPS_CAP] = ra; v.b_ovf[k - RAMP_OPS_CAP] = rb; }
 }
 
 // parent counter of op `child` += 1, returns the new value (JOB:530).  Small jobs keep one BYTE per op in shared memory
@@ -342,401 +308,6 @@ __device__ __forceinline__ uint32_t par_inc(bool in_smem, uint32_t* par_sm, uint
         return ((old >> sh) & 0xFFu) + 1u;
     }
     return atomicAdd(&par_gl[child], 1u) + 1u;
-}
-
-// bytes of shared memory one lookahead warp needs
-__host__ __device__ inline size_t lookahead_smem_per_warp(int w_cap, int c_cap, int par_cap, int f_cap = RAMP_F_CAP, int ops_cap = RAMP_OPS_CAP) {
-    size_t b = 0;
-    b += (size_t)2 * ops_cap * 16;               // op records a (ping-pong)
-    b += (size_t)f_cap * 8 * 2;                  // kd, rem
-    b += (size_t)RAMP_NF_CAP * 8;                // ready non-flow deps
-    b += (size_t)2 * ops_cap * 8;                // op records b
-    b += (size_t)(w_cap + 2 * c_cap) * 4;        // wkey, ckey (this tick / next tick)
-    b += (size_t)par_cap;                        // parent counters (bytes)
-    return (b + 15) & ~(size_t)15;
-}
-
-// FC / OC: flow-frontier entries / op-frontier records kept in shared memory per warp.  The engine instantiates a roomy
-// shape (384 / 48: 12 warps per SM) and a dense one (256 / 32: 16 warps per SM) for steps with far more lookaheads than slots
-template <int WPB, int FC = RAMP_F_CAP, int OC = RAMP_OPS_CAP>
-__global__ void __launch_bounds__(WPB * 32) ramp_lookahead_kernel(const LookaheadArgs a) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    const unsigned FULL = 0xffffffffu;
-    const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    const unsigned lt_mask = (1u << lane) - 1u;
-    unsigned char* my_smem = smem_raw + (size_t)warp * lookahead_smem_per_warp(a.w_cap, a.c_cap, a.par_cap, FC, OC);
-    // layout by decreasing alignment: int4 | 8-byte arrays | 4-byte arrays
-    int4* ops_a_sm0 = reinterpret_cast<int4*>(my_smem);                                  // [2][OC]
-    FrontView fr;
-    fr.kd_sm = reinterpret_cast<unsigned long long*>(ops_a_sm0 + 2 * OC);      // [FC]
-    fr.rem_sm = reinterpret_cast<double*>(fr.kd_sm + FC);                        // [FC]
-    unsigned long long* nf_sm = reinterpret_cast<unsigned long long*>(fr.rem_sm + FC);   // [RAMP_NF_CAP]
-    int2* ops_b_sm0 = reinterpret_cast<int2*>(nf_sm + RAMP_NF_CAP);                      // [2][OC]
-    uint32_t* wkey = reinterpret_cast<uint32_t*>(ops_b_sm0 + 2 * OC);          // [w_cap] best key among the ready ops on the worker
-    uint32_t* ckey0 = wkey + a.w_cap;                                                    // [2][c_cap] best key among the ready flows on the channel
-    uint32_t* par_sm = ckey0 + 2 * a.c_cap;                                              // [par_cap / 4] byte parent counters
-
-    unsigned char* slab = a.scratch + (uint64_t)(blockIdx.x * WPB + warp) * a.scratch_stride;
-    const uint64_t trace_region = a.scratch_stride - align_up((uint64_t)a.trace_cap * 12, 16);
-    const double INF = __longlong_as_double(RAMP_INF_BITS);
-
-    for (;;) {
-        int wi = 0;
-        if (lane == 0) wi = atomicAdd(a.cursor, 1);
-        wi = __shfl_sync(FULL, wi, 0);
-        const int n_a = *a.n_work;
-        const int n_b = a.n_work_b ? *a.n_work_b : 0;
-        if (wi >= n_a + n_b) break;
-        const WorkItem item = (wi < n_a) ? a.items[wi] : a.items_b[wi - n_a];
-        const TemplateDev& T = a.templates[item.template_id];
-        const int N = T.n_ops, E = T.n_deps, W = T.n_workers, C = T.n_channels;
-        const ScratchView sv = carve(slab, N, E, trace_region, a.trace_cap);
-        fr.kd_ovf = sv.f_km_ovf; fr.rem_ovf = sv.f_rem_ovf;
-        unsigned long long* nf_ovf = sv.nf_ovf;
-
-        const int4* __restrict__ t_op_rec = T.op_rec;
-        const int2* __restrict__ t_op_row = T.op_row;
-        const uint16_t* __restrict__ t_n_parents = T.op_n_parents;
-        const unsigned long long* __restrict__ t_dep_kd = T.dep_kd;
-        const double* __restrict__ t_dep_rt = T.dep_rt;
-        uint32_t* par_done = sv.par_done;
-        const bool psm = T.par_in_smem != 0;
-        const uint32_t kmask = T.kd_kmask, cmask = T.kd_cmask;
-        const int csh = T.kd_cshift, fsh = T.kd_fshift, dsh = T.kd_dshift;
-
-        // ---- init (JOB:432-484) ----
-        if (psm) { for (int i = lane; i < (N + 3) / 4; i += 32) par_sm[i] = 0u; }
-        else { for (int i = lane; i < N; i += 32) par_done[i] = 0u; }
-        for (int i = lane; i < W; i += 32) wkey[i] = 0u;
-        for (int i = lane; i < 2 * a.c_cap; i += 32) ckey0[i] = 0u;
-        uint32_t* ck_cur = ckey0;             // winners among the deps of this tick's snapshot
-        uint32_t* ck_nxt = ckey0 + a.c_cap;   // being built for the next tick (all zero at the start of a tick)
-        OpsView ops, ops_n;
-        ops.a_sm = ops_a_sm0; ops.b_sm = ops_b_sm0; ops.a_ovf = sv.ops_a_ovf[0]; ops.b_ovf = sv.ops_b_ovf[0];
-        ops_n.a_sm = ops_a_sm0 + OC; ops_n.b_sm = ops_b_sm0 + OC; ops_n.a_ovf = sv.ops_a_ovf[1]; ops_n.b_ovf = sv.ops_b_ovf[1];
-        for (int k = lane; k < T.n_src; k += 32) {
-            const int op = __ldg(&T.src_ops[k]);
-            ops_put<OC>(ops, k, __ldg(&t_op_rec[op]), __ldg(&t_op_row[op]));          // RCE:1334
-        }
-        __syncwarp();
-
-        // warp-uniform state
-        int nO = T.n_src;          // ready ops
-        int nF = 0;                // ready flows (the frontier holds no dead entries)
-        int nNF = 0;               // ready non-flow deps: zero run time (RCE:542-560), so each lives for exactly one tick
-        int ops_completed = 0, deps_completed = 0;
-        int tick_no = 0;
-        int status = RAMP_ST_OK;
-        double t = 0.0, comm = 0.0, comp = 0.0;   // lane 0: Stopwatch UT:485-496, JOB:170-171
-
-        for (;;) {
-            const bool big_ops = nO > 32 * 32;          // more op iterations per lane than win_mask has bits
-
-            // ---- A ----
-            for (int k = lane; k < nO; k += 32) {
-                int4 ra; int2 rb;
-                ops_get<OC>(ops, k, ra, rb);
-                atomicMax(&wkey[ra.w], (uint32_t)ra.z);
-            }
-            __syncwarp();
-
-            // ---- B ----
-            uint32_t win_mask = 0u;
-            double mo = INF;
-            int na = 0;
-            {
-                int j = 0;
-                for (int k = lane; k < nO; k += 32, ++j) {
-                    int4 ra; int2 rb;
-                    ops_get<OC>(ops, k, ra, rb);
-                    if (wkey[ra.w] == (uint32_t)ra.z) {
-                        if (j < 32) win_mask |= 1u << j;
-                        ++na;
-                        const double rem = __hiloint2double(ra.y, ra.x);
-                        mo = (rem < mo) ? rem : mo;
-                    }
-                }
-            }
-            const double t_op = warp_min_f64(mo);
-            const int n_active = warp_sum_i32(na);
-
-            // ---- C, D: ck_cur[c] holds the arg-max key over the ready flows on channel c (built while the previous tick
-            //      compacted its survivors and appended its arrivals), so the winners are the entries that match it ----
-            const bool any_nf = nNF > 0;
-            double t_comm = 0.0;
-            if (!any_nf) {
-                double md = INF;
-                for (int k = lane; k < nF; k += 32) {
-                    unsigned long long kd; double rem;
-                    f_get<FC>(fr, k, kd, rem);
-                    const uint32_t c = (uint32_t)(kd >> csh) & cmask;
-                    if (c != cmask && ck_cur[c] == ((uint32_t)kd & kmask)) md = (rem < md) ? rem : md;
-                }
-                t_comm = warp_min_f64(md);
-            }
-            __syncwarp();
-            // a tick that freezes the flows (any_nf) leaves the winners table as it is: its arrivals vote into ck_cur
-            if (!any_nf) { for (int c = lane; c < C; c += 32) ck_cur[c] = 0u; }   // else: this table is the next tick's "next"
-            uint32_t* ck_vote = any_nf ? ck_cur : ck_nxt;
-            // ---- E ----
-            const double tick = (t_comm < t_op) ? t_comm : t_op;
-
-            // ---- I, J ----
-            if (lane == 0) {
-                const bool ticked_ops = n_active > 0;
-                const bool ticked_flows = (!any_nf) && (nF > 0);                 // RCE:434-439
-                if (ticked_ops && ticked_flows) { comm = __dadd_rn(comm, tick); comp = __dadd_rn(comp, tick); }
-                else if (ticked_flows) comm = __dadd_rn(comm, tick);
-                else if (ticked_ops) comp = __dadd_rn(comp, tick);
-                t = __dadd_rn(t, tick);
-                if (tick_no < a.trace_cap) { sv.tr_n[tick_no] = n_active; sv.tr_tick[tick_no] = tick; }
-                else status = RAMP_ST_TRACE_OVERFLOW;
-            }
-            ++tick_no;
-
-            // ---- H: the deps of the pre-tick snapshot.  A tick with ready non-flow deps is a zero-length tick that completes
-            //      exactly those (RCE:412-422, 718-731) and leaves the flows untouched; any other tick ticks every flow
-            //      [0, nF): survivors slide down to [0, p) and vote for the next tick's channel winners.  32 per iteration ----
-            int nO_next = 0;
-            int p = 0;
-            if (any_nf) {
-                for (int kb = 0; kb < nNF; kb += 32) {
-                    const int k = kb + lane;
-                    const bool valid = k < nNF;
-                    uint32_t cnt = 0u, np = 1u;
-                    int child = 0;
-                    if (valid) {                                                                // JOB:525-536
-                        const unsigned long long kd = (k < RAMP_NF_CAP) ? nf_sm[k] : nf_ovf[k - RAMP_NF_CAP];
-                        child = (int)(kd >> dsh);
-                        cnt = par_inc(psm, par_sm, par_done, child);                            // JOB:530
-                        np = psm ? (uint32_t)(kd >> (fsh + 1)) & 0xFFu : (uint32_t)__ldg(&t_n_parents[child]);
-                    }
-                    const bool readied = valid && (cnt == np);                                   // JOB:531 (fires once)
-                    const unsigned m = __ballot_sync(FULL, readied);
-                    if (readied) ops_put_child<OC>(ops_n, nO_next + __popc(m & lt_mask), child);
-                    nO_next += __popc(m);
-                }
-                deps_completed += nNF;
-                p = nF;
-                __syncwarp();
-            } else {
-                int ddone = 0;
-                // one group of 32 flows.  FULLG: all 32 lanes hold an entry (every group but the last); INSM: the group lies in
-                // the shared-memory part of the frontier (then so does everything it writes: p <= kb)
-                auto h_group = [&](auto full_tag, auto insm_tag, const int kb) {
-                    constexpr bool FULLG = decltype(full_tag)::value;
-                    constexpr bool INSM = decltype(insm_tag)::value;
-                    const int k = kb + lane;
-                    const int n_here = FULLG ? 32 : ((nF - kb < 32) ? (nF - kb) : 32);
-                    const bool valid = FULLG ? true : (lane < n_here);
-                    unsigned long long kd = 0ull;
-                    double rem = 1.0;
-                    if (INSM) { if (valid) { kd = fr.kd_sm[k]; rem = fr.rem_sm[k]; } }
-                    else { if (valid) f_get<FC>(fr, k, kd, rem); }
-                    const double r2 = tick_down(rem, tick);                                         // JOB:561
-                    const bool done = valid && (r2 == 0.0);                                         // JOB:562
-                    const bool keep = valid && !done;
-                    const uint32_t c = (uint32_t)(kd >> csh) & cmask;
-                    if (keep && c != cmask) atomicMax(&ck_nxt[c], (uint32_t)kd & kmask);            // RCE:665-689 for the next tick
-                    const unsigned dmask = __ballot_sync(FULL, done);
-                    if (dmask == 0u) {
-                        if (p == kb) {                                 // nothing before it died either: update in place
-                            if (valid) { if (INSM) fr.rem_sm[k] = r2; else if (k < FC) fr.rem_sm[k] = r2; else fr.rem_ovf[k - FC] = r2; }
-                        } else {
-                            __syncwarp();                              // all lanes have read before anything is written over
-                            if (valid) { if (INSM) { fr.kd_sm[p + lane] = kd; fr.rem_sm[p + lane] = r2; } else f_put<FC>(fr, p + lane, kd, r2); }
-                        }
-                        p += n_here;                                   // warp-uniform: every valid entry of the group survives
-                    } else {
-                        // JOB:525-536 for the completing lanes
-                        uint32_t cnt = 0u, np = 1u;
-                        int child = 0;
-                        if (done) {
-                            child = (int)(kd >> dsh);
-                            cnt = par_inc(psm, par_sm, par_done, child);                            // JOB:530
-                            np = psm ? (uint32_t)(kd >> (fsh + 1)) & 0xFFu : (uint32_t)__ldg(&t_n_parents[child]);
-                        }
-                        ddone += __popc(dmask);
-                        const unsigned vm = FULLG ? FULL : ((1u << n_here) - 1u);
-                        const unsigned mk = vm & ~dmask;
-                        __syncwarp();
-                        if (keep) {
-                            const int q = p + __popc(mk & lt_mask);
-                            if (INSM) { fr.kd_sm[q] = kd; fr.rem_sm[q] = r2; } else f_put<FC>(fr, q, kd, r2);
-                        }
-                        p += __popc(mk);
-                        const bool readied = done && (cnt == np);                                    // JOB:531 (fires once)
-                        const unsigned m = __ballot_sync(FULL, readied);
-                        if (readied) ops_put_child<OC>(ops_n, nO_next + __popc(m & lt_mask), child);
-                        nO_next += __popc(m);
-                    }
-                };
-                const int n_full = nF & ~31;                           // entries covered by full groups
-                const int n_full_sm = (n_full < FC) ? n_full : FC;   // FC is a multiple of 32
-                int kb = 0;
-                for (; kb < n_full_sm; kb += 32) h_group(std::true_type{}, std::true_type{}, kb);
-                for (; kb < nF; kb += 32) h_group(std::false_type{}, std::false_type{}, kb);
-                deps_completed += ddone;
-            }
-            // the records of the ops readied above: the first 32 are loaded here and stored after G (the loads fly while G
-            // runs), any more are fetched in place
-            const int n_ready = nO_next;
-            __syncwarp();
-            int4 rdy_a = make_int4(0, 0, 0, 0);
-            int2 rdy_b = make_int2(0, 0);
-            if (lane < n_ready) {
-                const int child = ops_get_child<OC>(ops_n, lane);
-                rdy_a = __ldg(&t_op_rec[child]);
-                rdy_b = __ldg(&t_op_row[child]);
-            }
-            for (int k = 32 + lane; k < n_ready; k += 32) {
-                const int child = ops_get_child<OC>(ops_n, k);
-                ops_put<OC>(ops_n, k, __ldg(&t_op_rec[child]), __ldg(&t_op_row[child]));
-            }
-
-            // ---- G: tick the op winners; rows of the completed ops are appended at [p, tail) ----
-            int tail = p;
-            int nNF_next = 0;                   // this tick's non-flow arrivals (the previous ones were all consumed above)
-            {
-                int j = 0;
-                for (int kb = 0; kb < nO; kb += 32, ++j) {
-                    const int k = kb + lane;
-                    const bool valid = k < nO;
-                    int4 ra = make_int4(0, 0, 0, 0);
-                    int2 rb = make_int2(0, 0);
-                    bool done = false;
-                    if (valid) {
-                        ops_get<OC>(ops, k, ra, rb);
-                        bool win;
-                        if (big_ops) win = wkey[ra.w] == (uint32_t)ra.z;
-                        else { win = ((win_mask >> j) & 1u) != 0u; wkey[ra.w] = 0u; }   // release the winner slot
-                        if (win) {
-                            const double rem = tick_down(__hiloint2double(ra.y, ra.x), tick);   // JOB:555
-                            if (rem == 0.0) done = true;                                        // JOB:556
-                            else { ra.x = __double2loint(rem); ra.y = __double2hiint(rem); }
-                        }
-                    }
-                    const bool keep = valid && !done;
-                    const unsigned km_ = __ballot_sync(FULL, keep);
-                    if (keep) ops_put<OC>(ops_n, nO_next + __popc(km_ & lt_mask), ra, rb);
-                    nO_next += __popc(km_);
-                    const unsigned dm = __ballot_sync(FULL, done);
-                    if (dm) {
-                        // JOB:496-506: the out-edges of every op completed here become ready: the rows are copied as ONE
-                        // flattened range so that all template loads of a batch are in flight together.
-                        ops_completed += __popc(dm);
-                        const int deg = done ? rb.y : 0;
-                        int inc = deg;
-#pragma unroll
-                        for (int o = 1; o < 32; o <<= 1) {
-                            const int v = __shfl_up_sync(FULL, inc, o);
-                            if (lane >= o) inc += v;
-                        }
-                        const int total = __shfl_sync(FULL, inc, 31);
-                        const int exc = inc - deg;
-                        for (int jb = 0; jb < total; jb += 32 * RAMP_U) {
-                            unsigned long long kd[RAMP_U];
-                            double rt[RAMP_U];
-#pragma unroll
-                            for (int u = 0; u < RAMP_U; ++u) {
-                                kd[u] = 0ull; rt[u] = 0.0;
-                                if (jb + u * 32 >= total) continue;          // warp-uniform: nothing left for this slice
-                                const int jf = jb + u * 32 + lane;
-                                const int jc = jf < total ? jf : total - 1;
-                                int lo = 0;                 // owner = first lane whose inclusive prefix exceeds jc
-#pragma unroll
-                                for (int step = 16; step > 0; step >>= 1) {
-                                    const int v = __shfl_sync(FULL, inc, lo + step - 1);
-                                    if (v <= jc) lo += step;
-                                }
-                                const int o_start = __shfl_sync(FULL, rb.x, lo);
-                                const int o_exc = __shfl_sync(FULL, exc, lo);
-                                const int e = o_start + (jc - o_exc);
-                                if (jf < total) {
-                                    kd[u] = __ldg(&t_dep_kd[e]);
-                                    rt[u] = __ldg(&t_dep_rt[e]);                                // RCE:542-560
-                                }
-                            }
-#pragma unroll
-                            for (int u = 0; u < RAMP_U; ++u) {
-                                if (jb + u * 32 >= total) continue;      // warp-uniform
-                                const int jf = jb + u * 32 + lane;
-                                const bool valid = jf < total;
-                                const bool flow = valid && (((kd[u] >> fsh) & 1ull) != 0ull);
-                                const unsigned fm = __ballot_sync(FULL, flow);
-                                const unsigned nm = __ballot_sync(FULL, valid && !flow);
-                                if (flow) {
-                                    f_put<FC>(fr, tail + __popc(fm & lt_mask), kd[u], rt[u]);
-                                    const uint32_t c = (uint32_t)(kd[u] >> csh) & cmask;
-                                    if (c != cmask) atomicMax(&ck_vote[c], (uint32_t)kd[u] & kmask);
-                                } else if (valid) {
-                                    const int q = nNF_next + __popc(nm & lt_mask);
-                                    if (q < RAMP_NF_CAP) nf_sm[q] = kd[u]; else nf_ovf[q - RAMP_NF_CAP] = kd[u];
-                                }
-                                tail += __popc(fm);
-                                nNF_next += __popc(nm);
-                            }
-                        }
-                    }
-                }
-            }
-            if (lane < n_ready) ops_put<OC>(ops_n, lane, rdy_a, rdy_b);
-            if (big_ops) { __syncwarp(); for (int i = lane; i < W; i += 32) wkey[i] = 0u; }
-            nNF = nNF_next;
-            __syncwarp();
-
-            // ---- K, L ----
-            const bool finished = (ops_completed == N) && (deps_completed == E);     // JOB:549-551
-            if (!finished && isinf(tick)) status = RAMP_ST_INFINITE_TICK;             // RCE:462
-            if (finished || isinf(tick)) break;
-            nF = tail;
-            nO = nO_next;
-            { const OpsView tmp = ops; ops = ops_n; ops_n = tmp; }
-            if (!any_nf) { uint32_t* tmp = ck_cur; ck_cur = ck_nxt; ck_nxt = tmp; }
-        }
-
-        // ---- results (RCE:450-452): copy the trace to an exactly-sized pool allocation ----
-        const int n_rec = tick_no < a.trace_cap ? tick_no : a.trace_cap;
-        long long off = -1;
-        __syncwarp();
-        const double steps = (double)T.num_training_steps;
-        const double jct = __dmul_rn(__shfl_sync(FULL, t, 0), steps);
-        const int nmw = item.n_mounted_workers > 0 ? item.n_mounted_workers : W;
-        // utilisation terms go to the (now free) head of the dep-frontier overflow area
-        double* term = sv.f_rem_ovf2;
-        const bool can_util = (status == RAMP_ST_OK) && (tick_no <= a.trace_cap) && (n_rec <= E);
-        if (can_util) util_terms(sv.tr_n, sv.tr_tick, term, n_rec, (double)nmw, jct, lane, 32);
-        __syncwarp();
-        if (lane == 0) {
-            a.res.jct[item.slot] = jct;
-            a.res.comm[item.slot] = __dmul_rn(comm, steps);
-            a.res.comp[item.slot] = __dmul_rn(comp, steps);
-            a.res.n_ticks[item.slot] = tick_no;
-            a.res.util[item.slot] = can_util ? util_sum(term, n_rec) : 0.0;
-            a.res.util_nmw[item.slot] = can_util ? nmw : -1;
-            if (a.pool.top != nullptr) {
-                const unsigned long long o = atomicAdd(a.pool.top, (unsigned long long)n_rec);
-                if (o + (unsigned long long)n_rec <= a.pool.len) off = (long long)o;
-                else if (status == RAMP_ST_OK) status = RAMP_ST_TRACE_OVERFLOW;
-            }
-            a.res.trace_off[item.slot] = off;
-            a.res.status[item.slot] = status;
-            if (a.stats) {
-                atomicAdd(&a.stats->lookaheads, 1ull);
-                atomicAdd(&a.stats->alg_bytes, (unsigned long long)(T.algorithmic_bytes_static + 12ull * (unsigned long long)tick_no));
-            }
-        }
-        off = __shfl_sync(FULL, off, 0);
-        __syncwarp();
-        if (off >= 0) {
-            for (int k = lane; k < n_rec; k += 32) {
-                a.pool.n_active[off + k] = sv.tr_n[k];
-                a.pool.tick[off + k] = sv.tr_tick[k];
-            }
-        }
-        __syncwarp();
-    }
 }
 
 }  // namespace ramp
@@ -753,8 +324,7 @@ struct PlanArgs {
     int32_t n_templates;
     EpisodeState ep;
     MemoTable memo;
-    WorkItem* items;                // [B] small lookaheads
-    WorkItem* items_big;            // [B] big lookaheads
+    WorkItem* items;                // [B] lookaheads on non-resident templates
     WorkItem* items_res;            // [B] lookaheads on resident templates
     Counters* counters;
     MemoStats* stats;
@@ -842,7 +412,6 @@ __global__ void ramp_plan_kernel(const PlanArgs p) {
         atomicAdd(&p.stats->ran, 1ull);
         WorkItem it; it.template_id = act.template_id; it.slot = slot; it.episode = b; it.n_mounted_workers = act.n_mounted_workers;
         if (T.size_class == 2) p.items_res[atomicAdd(&p.counters->n_work_res, 1)] = it;
-        else if (T.size_class) p.items_big[atomicAdd(&p.counters->n_work_big, 1)] = it;
         else p.items[atomicAdd(&p.counters->n_work, 1)] = it;
     }
 }

@@ -1,9 +1,8 @@
 // ramp_lookahead_cta.cuh -- _run_lookahead (RCE:379-467) with ONE CTA (NW warps) per lookahead.
 //
-// Same algorithm, records and shared-memory staging as the warp-per-lookahead kernel in ramp_kernels.cuh; the per-tick
-// passes are spread over the CTA's warps so a single lookahead finishes sooner.  The engine picks this kernel when a
-// step has fewer un-memoised lookaheads than the GPU has warp slots (latency matters) and the warp-per-lookahead
-// kernel when there are many (instruction efficiency matters).
+// Runs every lookahead whose template is not resident (its quotient blob does not fit shared memory, or
+// RAMP_LOOKAHEAD_MODE=cta); the per-tick passes are spread over the CTA's warps so a single lookahead finishes sooner.
+// The engine picks 256, 128 or 64 threads per CTA by how many such lookaheads a launch has (launch_lookaheads).
 //
 // The dep frontier is one list updated IN PLACE (completed entries are marked dead, ticks that freeze the flows write
 // nothing) and compacted into the other buffer only when more than half of it is dead; newly ready deps are appended
@@ -99,10 +98,8 @@ __global__ void __launch_bounds__(NW * 32, RAMP_CTA_MIN_WARPS / NW) ramp_lookahe
         if (tid == 0) s_work = atomicAdd(a.cursor, 1);
         __syncthreads();
         const int wi = s_work;
-        const int n_a = *a.n_work;
-        const int n_b = a.n_work_b ? *a.n_work_b : 0;
-        if (wi >= n_a + n_b) break;
-        const WorkItem item = (wi < n_a) ? a.items[wi] : a.items_b[wi - n_a];
+        if (wi >= *a.n_work) break;
+        const WorkItem item = a.items[wi];
         const TemplateDev& T = a.templates[item.template_id];
         const int N = T.n_ops, E = T.n_deps, W = T.n_workers, C = T.n_channels;
         const ScratchView sv = carve(slab, N, E, trace_region, a.trace_cap);

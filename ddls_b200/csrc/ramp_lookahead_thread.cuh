@@ -15,7 +15,7 @@
 //     class, the ready-op / ready-flow / ready-non-flow frontiers (first OCAP / FCAP / NFCAP entries; the rest spills to an
 //     HBM slab laid out the same way), and small per-worker-group / per-channel-group winner tables.
 //
-// Per tick (letters as in SURVEY.md 3.3; same arithmetic, same order as ramp_lookahead_kernel):
+// Per tick (letters as in SURVEY.md 3.3; same arithmetic, same order as ramp_lookahead_cta_kernel):
 //   A,B  winners among the ready op classes per worker group (largest rank key), t_op = min remaining, active workers =
 //        sum of the winners' class sizes                                                        (RCE:562-606, 44-67, 709-715)
 //   C    a ready non-flow dep makes this a zero-length tick that completes exactly the non-flows  (RCE:412-422, 520-540, 718-731)

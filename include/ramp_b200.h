@@ -9,7 +9,7 @@
  *     RampClusterEnvironment.step      RCE:894-1179 -> ramp_step_host / ramp_step_device
  *       _place_ops/_schedule_ops/_place_deps/_schedule_deps RCE:1305-1415 -> ramp_register_template (+ per-step mount rows)
  *       _perform_lookahead_job_completion_time + memo dicts RCE:469-518, RCE:269-275 -> memo hash table inside the step
- *       _run_lookahead                  RCE:379-467  -> ramp_lookahead_thread_kernel, or ramp_lookahead_kernel /
+ *       _run_lookahead                  RCE:379-467  -> ramp_lookahead_thread_kernel, or
  *                                                       ramp_lookahead_cta_kernel for jobs too large for it
  *                                                       (also callable alone: ramp_run_lookaheads)
  *       _register_completed_lookahead   RCE:793-888  -> ramp_step_kernel
@@ -278,7 +278,7 @@ int ramp_run_lookaheads(ramp_engine_t* eng, const int32_t* template_ids, int32_t
                         ramp_lookahead_result_t* results, int32_t* trace_n_active, double* trace_tick,
                         int32_t trace_cap, float* kernel_ms_out);
 /* How a registered template runs, for tests and diagnostics: out[0] size class (2 = resident: the thread-per-lookahead
- * kernel on its quotient, 0 / 1 = the warp / CTA kernels), out[1..2] the resident quotient's classes and dep entries
+ * kernel on its quotient, 0 = the CTA kernel), out[1..2] the resident quotient's classes and dep entries
  * (0 when not resident), out[3..6] what the first completed lookahead of the template recorded for the later ones
  * (ticks, largest ready-op / ready-flow / ready-non-flow frontiers; all 0 before), *hint_jct (may be NULL) its job
  * completion time.  Waits for the engine stream. */

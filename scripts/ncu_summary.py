@@ -42,7 +42,7 @@ for r in rows[2:]:
         'l2_hit_pct': f(r, 'lts__t_sector_hit_rate.pct'),
         'inst': f(r, 'smsp__inst_executed.sum'),
     })
-# group launches of the same step: bench launches per step either one warp kernel or (CTA kernel, warp kernel)
+# group launches of the same step: a bench step launches the thread kernel, the CTA kernel or both, the thread kernel first
 total_bytes = sum((l['dram_read_MB'] + l['dram_write_MB']) * 1e6 for l in launches)
 n_steps = sum(1 for l in launches if 'cta' not in l['kernel']) or len(launches)
 out = {'_what': what, 'dram_bytes_per_launch': total_bytes / max(n_steps, 1), 'n_launches': len(launches), 'n_steps': n_steps,

@@ -111,7 +111,7 @@ CASES = [
     ('cfg3-resnet50-64w', 4096, 0, 'one_to_one', 0, None, False),
     ('cfg3-resnet50-64w', 4096, 0, 'reference', 0, None, True),
 ] + [(c, 4096, 0, 'reference', m, None, False) for c in ('cfg3-resnet50-64w', 'cfg4-bert-256w') for m in (1, 2, 3)] \
-  + [(c, 4096, 0, 'reference', 0, lm, False) for c in ('cfg3-resnet50-64w', 'cfg4-bert-256w') for lm in ('warp', 'cta', 'thread_unfolded')]
+  + [(c, 4096, 0, 'reference', 0, lm, False) for c in ('cfg3-resnet50-64w', 'cfg4-bert-256w') for lm in ('cta', 'thread_unfolded')]
 
 
 def _case_id(c):

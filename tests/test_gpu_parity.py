@@ -28,12 +28,12 @@ def eng_mod():
 
 
 # every lookahead kernel: one THREAD per lookahead on the symmetry quotient (the default whenever the quotient fits shared
-# memory), the same kernel on the unfolded job, one warp per lookahead, one CTA per lookahead
-MODES = ['thread', 'thread_unfolded', 'warp', 'cta']
+# memory), the same kernel on the unfolded job, one CTA per lookahead
+MODES = ['thread', 'thread_unfolded', 'cta']
 THREAD_MODES = ['thread', 'thread_unfolded']
 # every mode on a template's first launch, and the thread kernel's second route too: a later launch of a template reads the
 # TemplateHints the first one recorded, keeps every list in shared memory, writes its trace in place and sums the utilisation
-# inside the tick loop (the warp / CTA kernels keep no hints)
+# inside the tick loop (the CTA kernel keeps no hints)
 MODE_LAUNCHES = [pytest.param(m, 'first', id=m) for m in MODES] + [pytest.param(m, 'hinted', id=f'{m}-hinted') for m in THREAD_MODES]
 
 
@@ -165,24 +165,24 @@ def test_episode_replay_vs_reference_golden(fname, memo_mode, eng_mod):
     eng.close()
 
 
-@pytest.mark.parametrize('shape', ['roomy', 'dense'])
+@pytest.mark.parametrize('shape', ['roomy', 'cta'])
 @pytest.mark.parametrize('fname', FILES)
 def test_episode_replay_vs_oracle_bit_exact(fname, shape, eng_mod, oracle_lib):
-    """Same replay, CUDA vs CPU oracle: every step_stats entry and job record identical (bit-exact f64).  'dense' forces the
-    warp kernel's 16-warps-per-SM shape (smaller shared-memory frontiers) that steps with far more lookaheads than slots use."""
+    """Same replay, CUDA vs CPU oracle: every step_stats entry and job record identical (bit-exact f64).  'cta' makes no
+    template resident, so every step's lookaheads take the non-resident route: the work-count read-back and the CTA kernel."""
     import os
     from ddls_b200.engine import action_row
     g = Golden(fname)
     arr = g.arrivals()
     env = oracle_lib.OracleEnv(g.n_cluster_workers, max_jobs=len(arr), memo_models=max(g.n_models, 1))
     env.reset(arr, max_simulation_run_time=g.max_sim_time)
-    if shape == 'dense':
-        os.environ['RAMP_DENSE_FACTOR'] = '0'
+    if shape == 'cta':
+        os.environ['RAMP_LOOKAHEAD_MODE'] = 'cta'
     try:
         eng = eng_mod.RampEngine(n_episodes=2, n_cluster_workers=g.n_cluster_workers, max_jobs=len(arr),
                                  max_simulation_run_time=g.max_sim_time, trace_cap=1 << 16)
     finally:
-        os.environ.pop('RAMP_DENSE_FACTOR', None)
+        os.environ.pop('RAMP_LOOKAHEAD_MODE', None)
     tids = [eng.register_template(t) for t in g.templates]
     eng.reset(np.stack([arr, arr]))
     for s in range(g.n_steps):
@@ -315,11 +315,12 @@ def test_infinite_tick_raises_like_reference(eng_mod):
     eng.close()
 
 
-@pytest.mark.parametrize('mode,cta_threads', [('warp', '0'), ('cta', '64'), ('cta', '128'), ('cta', '256'), ('auto', '0'),
+@pytest.mark.parametrize('mode,cta_threads', [('cta', '0'), ('cta', '64'), ('cta', '128'), ('cta', '256'), ('auto', '0'),
                                                ('thread_unfolded', '0')])
 def test_many_mixed_items_per_launch(mode, cta_threads, eng_mod, oracle_lib):
-    """Hundreds of lookaheads of four very different sizes in one launch, persistent CTAs/warps processing several items
-    each: every result equals the oracle's (this configuration once exposed a shared-memory race in the CTA kernel)."""
+    """Hundreds of lookaheads of four very different sizes in one launch, persistent CTAs processing several items each:
+    every result equals the oracle's (this configuration once exposed a shared-memory race in the CTA kernel).  ('cta', '0')
+    leaves the thread count to the launch rule: 6,000 items are more than one wave, so they run on persistent 64-thread CTAs."""
     import os
     from ddls_b200 import synth
     from ddls_b200.template_builder import build_template, RampShape
@@ -345,6 +346,19 @@ def test_many_mixed_items_per_launch(mode, cta_threads, eng_mod, oracle_lib):
             assert (res['jct'][sel] == want[d]['jct']).all() and (res['comm'][sel] == want[d]['comm']).all()
             assert (res['comp'][sel] == want[d]['comp']).all() and (res['n_ticks'][sel] == want[d]['n_ticks']).all()
     eng.close()
+
+
+@pytest.mark.parametrize('mode', ['warp', 'dense'])
+def test_unknown_lookahead_mode_fails_engine_creation(mode, eng_mod):
+    """RAMP_LOOKAHEAD_MODE names a route (auto or thread, thread_unfolded, cta); any other value, such as warp, fails
+    engine creation instead of quietly running the automatic route."""
+    import os
+    os.environ['RAMP_LOOKAHEAD_MODE'] = mode
+    try:
+        with pytest.raises(Exception, match='RAMP_LOOKAHEAD_MODE'):
+            eng_mod.RampEngine(n_episodes=1, n_cluster_workers=8, max_jobs=1)
+    finally:
+        os.environ.pop('RAMP_LOOKAHEAD_MODE', None)
 
 
 def test_shared_memo_survives_reset_and_matches_reference_mode(eng_mod):
@@ -410,7 +424,7 @@ def _fan_template(M, W, seed):
 
 @pytest.mark.parametrize('mode,cta_threads,launch',
                          [pytest.param(m, c, 'first', id=f'{m}-{c}') for m, c in
-                          [('warp', '0'), ('cta', '64'), ('cta', '128'), ('cta', '256'), ('thread', '0'), ('thread_unfolded', '0')]]
+                          [('cta', '64'), ('cta', '128'), ('cta', '256'), ('thread', '0'), ('thread_unfolded', '0')]]
                          + [pytest.param(m, '0', 'hinted', id=f'{m}-0-hinted') for m in THREAD_MODES])
 @pytest.mark.parametrize('M,W', [(200, 4), (3000, 6)])
 def test_wide_fan_overflows_every_shared_memory_list(M, W, mode, cta_threads, launch, eng_mod, oracle_lib):
@@ -430,7 +444,7 @@ def test_wide_fan_overflows_every_shared_memory_list(M, W, mode, cta_threads, la
     if launch == 'hinted':
         eng.run_lookaheads(np.full(5, tid, dtype=np.int32))
         h = eng.template_info(tid)
-        assert (h['size_class'] == 2) == (M == 200)             # M = 3000: the quotient blob exceeds 96 KB (warp kernel)
+        assert (h['size_class'] == 2) == (M == 200)             # M = 3000: the quotient blob exceeds 96 KB (CTA kernel)
         if M == 200:
             assert h['n_ticks'] == want['n_ticks'] and h['max_f'] > 16
     res, _, tn, tt = eng.run_lookaheads(np.full(5, tid, dtype=np.int32), want_trace=True)

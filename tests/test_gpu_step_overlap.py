@@ -159,10 +159,10 @@ def test_other_memo_modes_unchanged(memo_mode):
 
 
 def test_nonresident_templates_fall_back():
-    """With a template on the warp / CTA kernels registered, steps run in order and still match."""
+    """With a template on the CTA kernel registered, steps run in order and still match."""
     config, B = 'cfg2-resnet50-32w', 128
     wl, actions = _workload(config, B, seed=4)
-    os.environ['RAMP_LOOKAHEAD_MODE'] = 'warp'
+    os.environ['RAMP_LOOKAHEAD_MODE'] = 'cta'
     try:
         from ddls_b200 import engine, workload
         cfg = workload.CONFIGS[config]

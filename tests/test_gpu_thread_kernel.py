@@ -24,7 +24,7 @@ from ddls_b200.quotient import quotient as native_quotient
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FILES = golden_files()
 THREAD_MODES = ['thread', 'thread_unfolded']
-MODES = THREAD_MODES + ['warp', 'cta']
+MODES = THREAD_MODES + ['cta']
 OCAP, FASTF, FCAP, NFCAP, WCAP, CCAP = 8, 6, 16, 8, 8, 32    # RAMP_T_* of the normal build
 RES_MAX_BYTES = 96 * 1024                                 # ramp_engine.cu res_max_bytes
 MODEL_MAX_WORK = 20_000_000                               # (classes + entries) x ticks the Python model is run for
@@ -170,10 +170,10 @@ def test_32_channel_groups_are_never_resident(n_groups):
     assert not resident_rule(job, q)
 
 
-# which golden templates the 'thread' / 'thread_unfolded' modes really run on the thread kernel (the rest go to the warp /
-# CTA kernels): {file: (resident in thread mode, resident in thread_unfolded mode)}, template indices
+# which golden templates the 'thread' / 'thread_unfolded' modes really run on the thread kernel (the rest go to the CTA
+# kernel): {file: (resident in thread mode, resident in thread_unfolded mode)}, template indices
 #   Not resident: quotient blobs over 96 KB (e.g. resnet64_deg4_full: 6,673 entries x 16 B), or key bits + channel groups
-#   over 32 (e.g. chain8 templates 0-2 and 14: 49 channel groups).  Their 'thread' parity runs test the warp / CTA kernels.
+#   over 32 (e.g. chain8 templates 0-2 and 14: 49 channel groups).  Their 'thread' parity runs test the CTA kernel.
 RESIDENT = {
     'bert256_shard.npz': ([], []),
     'chain8.npz': ([3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 15], [3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 15]),
