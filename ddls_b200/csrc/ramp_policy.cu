@@ -688,11 +688,13 @@ int ensure_rows(ramp_policy* p, int32_t n, cudaStream_t st) {
     return RAMP_OK;
 }
 
-int prepare_learner(ramp_policy* p, cudaStream_t st) {
+// the start of every gradient call on `st`, after the previous call: the learner, every job type's states, current embeddings
+// and per-row scratch for minibatches of `rows` rows
+int prepare_learner(ramp_policy* p, cudaStream_t st, int32_t rows) {
     int rc;
-    if ((rc = ensure_learner(p)) != RAMP_OK || (rc = ensure_gmodels(p, st)) != RAMP_OK) return rc;
+    if ((rc = fence_in(p, st)) != RAMP_OK || (rc = ensure_learner(p)) != RAMP_OK || (rc = ensure_gmodels(p, st)) != RAMP_OK) return rc;
     if (!p->emb_valid && (rc = launch_embed(p, st)) != RAMP_OK) return rc;
-    return RAMP_OK;
+    return ensure_rows(p, rows, st);
 }
 
 // the MeanPool rounds of every job type, kept for the backward (and the embeddings when `emb` is given); nothing for a minibatch
@@ -724,7 +726,7 @@ int launch_grad(ramp_policy* p, GradArgs ga, cudaStream_t st) {
     return RAMP_OK;
 }
 
-int check_ppo_config(const ramp_ppo_config_t* cfg) {
+int check_learner_config(const ramp_ppo_config_t* cfg) {
     if (!cfg) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     if (cfg->sgd_minibatch_size < 1 || cfg->num_sgd_iter < 0) return set_error(RAMP_ERR_BAD_ARG, "ppo: sgd_minibatch_size must be >= 1, num_sgd_iter >= 0");
     if (!(cfg->clip_param > 0) || !(cfg->vf_clip_param > 0) || !(cfg->lr >= 0) || !(cfg->adam_eps > 0))
@@ -835,7 +837,7 @@ int device_call_ready(ramp_policy* p, int32_t n, const void* model, int32_t mode
     return RAMP_OK;
 }
 
-int check_impala_config(const ramp_impala_config_t* cfg) {
+int check_learner_config(const ramp_impala_config_t* cfg) {
     if (!cfg) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     if (!(cfg->vtrace_clip_rho_threshold > 0) || !(cfg->vtrace_clip_pg_rho_threshold > 0) || !(cfg->lr >= 0) || !(cfg->adam_eps > 0))
         return set_error(RAMP_ERR_BAD_ARG, "impala: the clip thresholds and adam_eps must be > 0, lr >= 0");
@@ -844,9 +846,71 @@ int check_impala_config(const ramp_impala_config_t* cfg) {
     return RAMP_OK;
 }
 
-int check_pg_config(const ramp_pg_config_t* cfg) {
+int check_learner_config(const ramp_pg_config_t* cfg) {
     if (!cfg) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     if (!(cfg->gamma >= 0) || !(cfg->lr >= 0) || !(cfg->adam_eps > 0)) return set_error(RAMP_ERR_BAD_ARG, "pg: gamma and lr must be >= 0, adam_eps > 0");
+    return RAMP_OK;
+}
+
+// the opening of every learn call: the algorithm's own configuration check, then a trajectory of at least n_steps recorded from
+// eng's environment; the messages start with `tag`.  Leaves the policy's device current and the engine stream in *st.
+template <class Cfg>
+int learn_begin(ramp_policy* p, ramp_engine_t* eng, const Cfg* cfg, int32_t n_steps, const char* tag, ramp_env_buffers_t* eb,
+                cudaStream_t* st) {
+    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = check_learner_config(cfg);
+    if (rc != RAMP_OK || (rc = ramp_env_buffers(eng, eb)) != RAMP_OK) return rc;
+    if (n_steps < 1 || n_steps > p->traj_n)
+        return set_error(RAMP_ERR_BAD_ARG, "%s: %d steps asked of a trajectory with %d recorded", tag, n_steps, p->traj_n);
+    if (eb->n_episodes != p->traj_b || eb->n_actions != p->traj_a)
+        return set_error(RAMP_ERR_BAD_ARG, "%s: the trajectory was recorded from another environment", tag);
+    CUDA_TRY(cudaSetDevice(p->device));
+    *st = ramp_internal_stream(eng);
+    return RAMP_OK;
+}
+
+// GAE (ramp_ppo_gae_kernel) over the trajectory's first T steps into the train batch b_*, on `st`.  boot: the value of the state
+// after the last step; nullptr: no critic (PG's discounted returns: V = 0, a 0 bootstrap)
+int launch_gae(ramp_policy* p, cudaStream_t st, int32_t T, int32_t B, double gamma, double lambda, int32_t standardize, const float* boot) {
+    GaeArgs ge{};
+    ge.T = T; ge.B = B; ge.A = p->P.c.n_actions; ge.n_models = p->P.c.n_models; ge.standardize = standardize;
+    ge.gamma = gamma; ge.lambda = lambda;
+    ge.t_obs = p->t_obs.get(); ge.t_model = p->t_model.get(); ge.t_mask = p->t_mask.get(); ge.t_action = p->t_action.get();
+    ge.t_logp = p->t_logp.get(); ge.t_value = boot ? p->t_value.get() : nullptr; ge.t_reward = p->t_reward.get(); ge.t_done = p->t_done.get();
+    ge.boot = boot; ge.adv64 = p->b_adv64.get();
+    ge.obs = p->b_obs.get(); ge.model = p->b_model.get(); ge.mask = p->b_mask.get(); ge.action = p->b_action.get(); ge.logp = p->b_logp.get();
+    ge.adv = p->b_adv.get(); ge.vt = p->b_vt.get(); ge.n_rows = p->l_n_rows.get();
+    ramp_ppo_gae_kernel<<<1, 1024, 0, st>>>(ge);
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
+}
+
+// clip_grad_norm_ and torch.optim.Adam at cfg's settings on the policy's gradient, moments and step count, for minibatches of mb
+// rows of a batch of *n_rows rows; the caller sets the minibatch's start and where its statistics go
+template <class Cfg>
+AdamArgs adam_args(ramp_policy* p, const Cfg& cfg, const int32_t* n_rows, int32_t mb) {
+    AdamArgs aa{};
+    aa.lr = cfg.lr; aa.beta1 = cfg.adam_beta1; aa.beta2 = cfg.adam_beta2;
+    aa.beta2_f = (float)cfg.adam_beta2; aa.one_m_beta1 = (float)(1.0 - cfg.adam_beta1); aa.one_m_beta2 = (float)(1.0 - cfg.adam_beta2);
+    aa.eps = (float)cfg.adam_eps;
+    aa.max_norm = (float)cfg.grad_clip; aa.n_rows = n_rows; aa.mb = mb; aa.step = p->l_step.get();
+    aa.m = p->l_adam_m.get(); aa.v = p->l_adam_v.get(); aa.grad = p->l_grad.get(); aa.norm_part = p->l_norm_part.get(); aa.w = p->d_w.get();
+    return aa;
+}
+
+// one Adam step on `st`: it reads the step count the previous step wrote
+int launch_adam(ramp_policy* p, AdamArgs aa, cudaStream_t st) {
+    aa.parity = p->adam_parity; p->adam_parity ^= 1;
+    ramp_adam_kernel<<<LRN_GRID, 256, 0, st>>>(aa, p->n_weights);
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
+}
+
+// the end of the gradient calls on host rows (stream 0): the gradient and n_stats statistics from `stats` (either out may be nullptr)
+int host_batch_end(ramp_policy* p, float* grad_out, double* stats_out, const double* stats, int n_stats) {
+    CUDA_TRY(cudaStreamSynchronize(0));
+    if (grad_out) CUDA_TRY(cudaMemcpy(grad_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    if (stats_out) CUDA_TRY(cudaMemcpy(stats_out, stats, sizeof(double) * n_stats, cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
 
@@ -1168,13 +1232,11 @@ int ramp_policy_backward(ramp_policy_t* p, int32_t n, const int32_t* model, cons
     if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "policy: backward of %d rows", n);
     CUDA_TRY(cudaSetDevice(p->device));
     int rc;
-    if ((rc = fence_in(p, 0)) || (rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n, 0)) ||
-        (rc = upload_host_batch(p, n, model, graph_features, action_mask, grad_logits, grad_value, nullptr, nullptr, nullptr, nullptr)))
+    if ((rc = prepare_learner(p, 0, n)) ||
+        (rc = upload_host_batch(p, n, model, graph_features, action_mask, grad_logits, grad_value, nullptr, nullptr, nullptr, nullptr)) ||
+        (rc = launch_backward(p, 0, n, false)))
         return rc;
-    if ((rc = launch_backward(p, 0, n, false)) != RAMP_OK) return rc;
-    CUDA_TRY(cudaStreamSynchronize(0));
-    CUDA_TRY(cudaMemcpy(grad_weights_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
-    return RAMP_OK;
+    return host_batch_end(p, grad_weights_out, nullptr, nullptr, 0);
 }
 
 int ramp_policy_set_weights_device(ramp_policy_t* p, const float* weights, int64_t n, void* stream) {
@@ -1219,8 +1281,7 @@ int ramp_policy_backward_device(ramp_policy_t* p, void* stream, int32_t n, const
     if (rc != RAMP_OK) return rc;
     if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "policy: backward of %d rows", n);
     cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = fence_in(p, st)) != RAMP_OK || (rc = prepare_learner(p, st)) != RAMP_OK || (rc = ensure_rows(p, n, st)) != RAMP_OK ||
-        (rc = stage_host_batch(p, n)) != RAMP_OK ||
+    if ((rc = prepare_learner(p, st, n)) != RAMP_OK || (rc = stage_host_batch(p, n)) != RAMP_OK ||
         (rc = launch_ingest(p, st, n, model, model_dtype, graph_features, graph_features_stride, action_mask, grad_logits, grad_value)) != RAMP_OK ||
         (rc = launch_backward(p, st, n, true)) != RAMP_OK)
         return rc;
@@ -1233,11 +1294,11 @@ int ramp_ppo_loss_grad(ramp_policy_t* p, const ramp_ppo_config_t* cfg, int32_t n
                        const float* value_target, float* grad_out, double* stats_out) {
     if (!p || !model || !graph_features || !action_mask || !action || !old_logits || !advantage || !value_target)
         return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    int rc = check_ppo_config(cfg);
+    int rc = check_learner_config(cfg);
     if (rc != RAMP_OK) return rc;
     if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "ppo: loss of %d rows", n);
     CUDA_TRY(cudaSetDevice(p->device));
-    if ((rc = fence_in(p, 0)) || (rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n, 0)) ||
+    if ((rc = prepare_learner(p, 0, n)) ||
         (rc = upload_host_batch(p, n, model, graph_features, action_mask, nullptr, nullptr, action, old_logits, advantage, value_target)))
         return rc;
     GradArgs ga = host_batch_args(p, n);
@@ -1246,27 +1307,16 @@ int ramp_ppo_loss_grad(ramp_policy_t* p, const ramp_ppo_config_t* cfg, int32_t n
     if ((rc = launch_states(p, 0, nullptr, 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, 0)) != RAMP_OK) return rc;
     ramp_ppo_minibatch_stats_kernel<<<1, 1>>>(p->l_row_stats.get(), n, ga.vf_coeff, ga.ent_coeff, ga.kl_coeff, p->l_norm_part.get(), p->l_stats.get());
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(0));
-    if (grad_out) CUDA_TRY(cudaMemcpy(grad_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
-    if (stats_out) CUDA_TRY(cudaMemcpy(stats_out, p->l_stats.get(), sizeof(double) * RAMP_PPO_STATS_LEN, cudaMemcpyDeviceToHost));
-    return RAMP_OK;
+    return host_batch_end(p, grad_out, stats_out, p->l_stats.get(), RAMP_PPO_STATS_LEN);
 }
 
 int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_ppo_config_t* cfg, double* stats_out) {
-    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    int rc = check_ppo_config(cfg);
-    if (rc != RAMP_OK) return rc;
     ramp_env_buffers_t eb{};
-    if ((rc = ramp_env_buffers(eng, &eb)) != RAMP_OK) return rc;
-    if (n_steps < 1 || n_steps > p->traj_n)
-        return set_error(RAMP_ERR_BAD_ARG, "ppo: %d steps asked of a trajectory with %d recorded", n_steps, p->traj_n);
-    if (eb.n_episodes != p->traj_b || eb.n_actions != p->traj_a)
-        return set_error(RAMP_ERR_BAD_ARG, "ppo: the trajectory was recorded from another environment");
-    const ramp_policy_config_t& c = p->P.c;
-    CUDA_TRY(cudaSetDevice(p->device));
-    cudaStream_t st = ramp_internal_stream(eng);
+    cudaStream_t st;
+    int rc = learn_begin(p, eng, cfg, n_steps, "ppo", &eb, &st);
+    if (rc != RAMP_OK) return rc;
     const int32_t B = eb.n_episodes, rows = n_steps * B, mb = cfg->sgd_minibatch_size, n_mb = (rows + mb - 1) / mb;
-    if ((rc = fence_in(p, st)) || (rc = prepare_learner(p, st)) || (rc = ensure_rows(p, mb, st)) || (rc = ensure_batch(p, rows))) return rc;
+    if ((rc = prepare_learner(p, st, mb)) || (rc = ensure_batch(p, rows))) return rc;
     if (B > p->boot_cap) {
         p->boot_cap = 0;
         CUDA_TRY(alloc_each(B, p->l_boot, p->l_boot_act));
@@ -1287,16 +1337,7 @@ int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, con
         ++launches;
     }
     // 2. GAE, the live rows t-major, standardised advantages
-    GaeArgs ge{};
-    ge.T = n_steps; ge.B = B; ge.A = c.n_actions; ge.n_models = c.n_models; ge.standardize = cfg->standardize_advantages;
-    ge.gamma = cfg->gamma; ge.lambda = cfg->lambda;
-    ge.t_obs = p->t_obs.get(); ge.t_model = p->t_model.get(); ge.t_mask = p->t_mask.get(); ge.t_action = p->t_action.get();
-    ge.t_logp = p->t_logp.get(); ge.t_value = p->t_value.get(); ge.t_reward = p->t_reward.get(); ge.t_done = p->t_done.get();
-    ge.boot = boot; ge.adv64 = p->b_adv64.get();
-    ge.obs = p->b_obs.get(); ge.model = p->b_model.get(); ge.mask = p->b_mask.get(); ge.action = p->b_action.get(); ge.logp = p->b_logp.get();
-    ge.adv = p->b_adv.get(); ge.vt = p->b_vt.get(); ge.n_rows = p->l_n_rows.get();
-    ramp_ppo_gae_kernel<<<1, 1024, 0, st>>>(ge);
-    CUDA_TRY(cudaGetLastError());
+    if ((rc = launch_gae(p, st, n_steps, B, cfg->gamma, cfg->lambda, cfg->standardize_advantages, boot)) != RAMP_OK) return rc;
     // 3. the collection weights' logits of every row: the head kernel again, so they are act's bits
     HeadArgs ho{};
     ho.n = rows; ho.obs_dyn = p->b_obs.get(); ho.graph_static = p->d_gstatic.get(); ho.model = p->b_model.get(); ho.mask = p->b_mask.get();
@@ -1307,12 +1348,7 @@ int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, con
     ga.mb = mb; ga.n_rows = p->l_n_rows.get(); ga.shuffle = 1; ga.obs_dyn = p->b_obs.get(); ga.model = p->b_model.get();
     ga.mask = p->b_mask.get(); ga.action = p->b_action.get(); ga.old_logits = p->b_old.get(); ga.adv = p->b_adv.get(); ga.vt = p->b_vt.get();
     ppo_terms(ga, *cfg);
-    AdamArgs aa{};
-    aa.lr = cfg->lr; aa.beta1 = cfg->adam_beta1; aa.beta2 = cfg->adam_beta2;
-    aa.beta2_f = (float)cfg->adam_beta2; aa.one_m_beta1 = (float)(1.0 - cfg->adam_beta1); aa.one_m_beta2 = (float)(1.0 - cfg->adam_beta2);
-    aa.eps = (float)cfg->adam_eps;
-    aa.max_norm = (float)cfg->grad_clip; aa.n_rows = p->l_n_rows.get(); aa.mb = mb; aa.step = p->l_step.get();
-    aa.m = p->l_adam_m.get(); aa.v = p->l_adam_v.get(); aa.grad = p->l_grad.get(); aa.norm_part = p->l_norm_part.get(); aa.w = p->d_w.get();
+    AdamArgs aa = adam_args(p, *cfg, p->l_n_rows.get(), mb);
     aa.row_stats = p->l_row_stats.get(); aa.vf_coeff = ga.vf_coeff; aa.ent_coeff = ga.ent_coeff; aa.kl_coeff = ga.kl_coeff;
     for (int pass = 0; pass < cfg->num_sgd_iter; ++pass) {
         ga.key = mix64(cfg->seed ^ mix64((uint64_t)pass + 1));
@@ -1324,10 +1360,8 @@ int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, con
             if ((rc = launch_states(p, st, p->l_n_rows.get(), ga.start, pass || k ? p->d_emb.get() : nullptr)) != RAMP_OK ||
                 (rc = launch_grad(p, ga, st)) != RAMP_OK)
                 return rc;
-            aa.parity = p->adam_parity; p->adam_parity ^= 1;
             aa.stats = p->l_mb_stats.get() + (size_t)k * RAMP_PPO_STATS_LEN;
-            ramp_adam_kernel<<<LRN_GRID, 256, 0, st>>>(aa, p->n_weights);
-            CUDA_TRY(cudaGetLastError());
+            if ((rc = launch_adam(p, aa, st)) != RAMP_OK) return rc;
             launches += 6;
         }
     }
@@ -1394,13 +1428,13 @@ int ramp_impala_loss_grad(ramp_policy_t* p, const ramp_impala_config_t* cfg, int
                           double* stats_out, float* vs_out, float* pg_adv_out, float* log_rho_out) {
     if (!p || !model || !graph_features || !action_mask || !action || !behaviour_logp || !reward || !done)
         return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    int rc = check_impala_config(cfg);
+    int rc = check_learner_config(cfg);
     if (rc != RAMP_OK) return rc;
     if (n_fragments < 1 || fragment_length < 1 || (int64_t)n_fragments * fragment_length > INT32_MAX)
         return set_error(RAMP_ERR_BAD_ARG, "impala: loss of %d fragments of %d rows", n_fragments, fragment_length);
     const int32_t n = n_fragments * fragment_length;
     CUDA_TRY(cudaSetDevice(p->device));
-    if ((rc = fence_in(p, 0)) || (rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n, 0)) || (rc = ensure_impala(p, n, 1)) ||
+    if ((rc = prepare_learner(p, 0, n)) || (rc = ensure_impala(p, n, 1)) ||
         (rc = upload_host_batch(p, n, model, graph_features, action_mask, nullptr, nullptr, action, nullptr, nullptr, nullptr)))
         return rc;
     CUDA_TRY(cudaMemcpy(p->i_blogp.get(), behaviour_logp, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
@@ -1412,10 +1446,8 @@ int ramp_impala_loss_grad(ramp_policy_t* p, const ramp_impala_config_t* cfg, int
                            p->h_action.get(), p->i_blogp.get(), p->i_reward.get(), p->i_done.get(), ga, p->i_stats.get())) != RAMP_OK)
         return rc;
     CUDA_TRY(cudaMemsetAsync(p->i_stats.get() + RAMP_IMPALA_SGD_STEPS, 0, sizeof(double), 0));
-    CUDA_TRY(cudaStreamSynchronize(0));
+    if ((rc = host_batch_end(p, grad_out, stats_out, p->i_stats.get(), RAMP_IMPALA_STATS_LEN)) != RAMP_OK) return rc;
     p->i_rows = n;
-    if (grad_out) CUDA_TRY(cudaMemcpy(grad_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
-    if (stats_out) CUDA_TRY(cudaMemcpy(stats_out, p->i_stats.get(), sizeof(double) * RAMP_IMPALA_STATS_LEN, cudaMemcpyDeviceToHost));
     if (vs_out) CUDA_TRY(cudaMemcpy(vs_out, p->i_vs.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
     if (pg_adv_out) CUDA_TRY(cudaMemcpy(pg_adv_out, p->i_pg.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
     if (log_rho_out) CUDA_TRY(cudaMemcpy(log_rho_out, p->i_log_rho.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
@@ -1423,25 +1455,18 @@ int ramp_impala_loss_grad(ramp_policy_t* p, const ramp_impala_config_t* cfg, int
 }
 
 int ramp_policy_learn_impala(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_impala_config_t* cfg, double* stats_out) {
-    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    int rc = check_impala_config(cfg);
-    if (rc != RAMP_OK) return rc;
     ramp_env_buffers_t eb{};
-    if ((rc = ramp_env_buffers(eng, &eb)) != RAMP_OK) return rc;
-    if (n_steps < 1 || n_steps > p->traj_n)
-        return set_error(RAMP_ERR_BAD_ARG, "impala: %d steps asked of a trajectory with %d recorded", n_steps, p->traj_n);
-    if (eb.n_episodes != p->traj_b || eb.n_actions != p->traj_a)
-        return set_error(RAMP_ERR_BAD_ARG, "impala: the trajectory was recorded from another environment");
+    cudaStream_t st;
+    int rc = learn_begin(p, eng, cfg, n_steps, "impala", &eb, &st);
+    if (rc != RAMP_OK) return rc;
     const int32_t L = cfg->rollout_fragment_length ? cfg->rollout_fragment_length : n_steps;
     if (n_steps % L) return set_error(RAMP_ERR_BAD_ARG, "impala: rollout_fragment_length %d does not divide %d steps", L, n_steps);
     if (cfg->train_batch_size < L)
         return set_error(RAMP_ERR_BAD_ARG, "impala: train_batch_size %d is below rollout_fragment_length %d", cfg->train_batch_size, L);
     const ramp_policy_config_t& c = p->P.c;
-    CUDA_TRY(cudaSetDevice(p->device));
-    cudaStream_t st = ramp_internal_stream(eng);
     const int32_t B = eb.n_episodes, n_frag = (n_steps / L) * B, R = n_steps * B;
     const int32_t F = std::min(cfg->train_batch_size / L, n_frag), mb = F * L, n_sgd = (n_frag + F - 1) / F;
-    if ((rc = fence_in(p, st)) || (rc = prepare_learner(p, st)) || (rc = ensure_rows(p, mb, st)) || (rc = ensure_impala(p, R, n_sgd))) return rc;
+    if ((rc = prepare_learner(p, st, mb)) || (rc = ensure_impala(p, R, n_sgd))) return rc;
     // 1. the fragment rows, fragment-major
     ImpalaBatchArgs ba{};
     ba.T = n_steps; ba.B = B; ba.A = c.n_actions; ba.L = L; ba.n_models = c.n_models;
@@ -1452,13 +1477,8 @@ int ramp_policy_learn_impala(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_ste
     ramp_impala_batch_kernel<<<(unsigned)((R + 255) / 256), 256, 0, st>>>(ba);
     CUDA_TRY(cudaGetLastError());
     // 2. one SGD step per train batch, in order
-    AdamArgs aa{};
-    aa.lr = cfg->lr; aa.beta1 = cfg->adam_beta1; aa.beta2 = cfg->adam_beta2;
-    aa.beta2_f = (float)cfg->adam_beta2; aa.one_m_beta1 = (float)(1.0 - cfg->adam_beta1); aa.one_m_beta2 = (float)(1.0 - cfg->adam_beta2);
-    aa.eps = (float)cfg->adam_eps;
-    aa.max_norm = (float)cfg->grad_clip; aa.n_rows = p->i_n_rows.get(); aa.mb = mb; aa.step = p->l_step.get();
-    aa.m = p->l_adam_m.get(); aa.v = p->l_adam_v.get(); aa.grad = p->l_grad.get(); aa.norm_part = p->l_norm_part.get(); aa.w = p->d_w.get();
-    aa.row_stats = nullptr; aa.stats = p->i_stats.get();             // IMPALA's statistics: ramp_impala_step_stats_kernel
+    AdamArgs aa = adam_args(p, *cfg, p->i_n_rows.get(), mb);
+    aa.stats = p->i_stats.get();                                      // IMPALA's statistics: ramp_impala_step_stats_kernel
     for (int k = 0; k < n_sgd; ++k) {
         const int32_t start = k * mb, nf = std::min(F, n_frag - k * F);
         // the rounds at the current weights, kept for the backward; from the second step on also the embeddings, which the
@@ -1471,9 +1491,7 @@ int ramp_policy_learn_impala(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_ste
                                p->i_step_stats.get() + (size_t)k * RAMP_IMPALA_STATS_LEN)) != RAMP_OK)
             return rc;
         aa.start = start;
-        aa.parity = p->adam_parity; p->adam_parity ^= 1;
-        ramp_adam_kernel<<<LRN_GRID, 256, 0, st>>>(aa, p->n_weights);
-        CUDA_TRY(cudaGetLastError());
+        if ((rc = launch_adam(p, aa, st)) != RAMP_OK) return rc;
     }
     p->emb_valid = false;
     p->i_rows = R;
@@ -1505,11 +1523,11 @@ int ramp_impala_vtrace_read(ramp_policy_t* p, int32_t* n_out, float* target_logp
 int ramp_pg_loss_grad(ramp_policy_t* p, const ramp_pg_config_t* cfg, int32_t n, const int32_t* model, const float* graph_features,
                       const uint8_t* action_mask, const int32_t* action, const float* advantage, float* grad_out, double* stats_out) {
     if (!p || !model || !graph_features || !action_mask || !action || !advantage) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    int rc = check_pg_config(cfg);
+    int rc = check_learner_config(cfg);
     if (rc != RAMP_OK) return rc;
     if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "pg: loss of %d rows", n);
     CUDA_TRY(cudaSetDevice(p->device));
-    if ((rc = fence_in(p, 0)) || (rc = prepare_learner(p, 0)) || (rc = ensure_rows(p, n, 0)) ||
+    if ((rc = prepare_learner(p, 0, n)) ||
         (rc = upload_host_batch(p, n, model, graph_features, action_mask, nullptr, nullptr, action, nullptr, advantage, nullptr)))
         return rc;
     GradArgs ga = host_batch_args(p, n);
@@ -1517,40 +1535,20 @@ int ramp_pg_loss_grad(ramp_policy_t* p, const ramp_pg_config_t* cfg, int32_t n, 
     if ((rc = launch_states(p, 0, nullptr, 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, 0)) != RAMP_OK) return rc;
     ramp_pg_stats_kernel<<<1, 1>>>(p->l_row_stats.get(), p->l_row_model.get(), p->h_adv.get(), n, ga.n_rows, p->l_norm_part.get(), p->l_stats.get());
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(0));
-    if (grad_out) CUDA_TRY(cudaMemcpy(grad_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
-    if (stats_out) CUDA_TRY(cudaMemcpy(stats_out, p->l_stats.get(), sizeof(double) * RAMP_PG_STATS_LEN, cudaMemcpyDeviceToHost));
-    return RAMP_OK;
+    return host_batch_end(p, grad_out, stats_out, p->l_stats.get(), RAMP_PG_STATS_LEN);
 }
 
 // PG's training step (algorithms/pg: one learn_on_batch per train batch): post_process_advantages (compute_advantages with
 // use_gae False, use_critic False, last_r 0), pg_torch_loss, torch.optim.Adam
 int ramp_policy_learn_pg(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_pg_config_t* cfg, double* stats_out) {
-    if (!p || !eng) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    int rc = check_pg_config(cfg);
-    if (rc != RAMP_OK) return rc;
     ramp_env_buffers_t eb{};
-    if ((rc = ramp_env_buffers(eng, &eb)) != RAMP_OK) return rc;
-    if (n_steps < 1 || n_steps > p->traj_n)
-        return set_error(RAMP_ERR_BAD_ARG, "pg: %d steps asked of a trajectory with %d recorded", n_steps, p->traj_n);
-    if (eb.n_episodes != p->traj_b || eb.n_actions != p->traj_a)
-        return set_error(RAMP_ERR_BAD_ARG, "pg: the trajectory was recorded from another environment");
-    const ramp_policy_config_t& c = p->P.c;
-    CUDA_TRY(cudaSetDevice(p->device));
-    cudaStream_t st = ramp_internal_stream(eng);
+    cudaStream_t st;
+    int rc = learn_begin(p, eng, cfg, n_steps, "pg", &eb, &st);
+    if (rc != RAMP_OK) return rc;
     const int32_t B = eb.n_episodes, rows = n_steps * B;
-    if ((rc = fence_in(p, st)) || (rc = prepare_learner(p, st)) || (rc = ensure_rows(p, rows, st)) || (rc = ensure_batch(p, rows))) return rc;
+    if ((rc = prepare_learner(p, st, rows)) || (rc = ensure_batch(p, rows))) return rc;
     // 1. the discounted returns (ramp_ppo_gae_kernel without values: lambda 1, V = 0, a 0 bootstrap), the live rows t-major
-    GaeArgs ge{};
-    ge.T = n_steps; ge.B = B; ge.A = c.n_actions; ge.n_models = c.n_models; ge.standardize = 0;
-    ge.gamma = cfg->gamma; ge.lambda = 1.0;
-    ge.t_obs = p->t_obs.get(); ge.t_model = p->t_model.get(); ge.t_mask = p->t_mask.get(); ge.t_action = p->t_action.get();
-    ge.t_logp = p->t_logp.get(); ge.t_value = nullptr; ge.t_reward = p->t_reward.get(); ge.t_done = p->t_done.get();
-    ge.boot = nullptr; ge.adv64 = p->b_adv64.get();
-    ge.obs = p->b_obs.get(); ge.model = p->b_model.get(); ge.mask = p->b_mask.get(); ge.action = p->b_action.get(); ge.logp = p->b_logp.get();
-    ge.adv = p->b_adv.get(); ge.vt = p->b_vt.get(); ge.n_rows = p->l_n_rows.get();
-    ramp_ppo_gae_kernel<<<1, 1024, 0, st>>>(ge);
-    CUDA_TRY(cudaGetLastError());
+    if ((rc = launch_gae(p, st, n_steps, B, cfg->gamma, 1.0, 0, nullptr)) != RAMP_OK) return rc;
     // 2. the loss's gradient over the whole batch at the collection weights (the embeddings the trajectory was collected with);
     //    the log p(a) the gradient kernel recomputes goes to b_logp_old
     GradArgs ga{};
@@ -1558,15 +1556,9 @@ int ramp_policy_learn_pg(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, 
     ga.mask = p->b_mask.get(); ga.action = p->b_action.get(); ga.adv = p->b_adv.get(); ga.pg = 1; ga.logp_old = p->b_logp_old.get();
     if ((rc = launch_states(p, st, p->l_n_rows.get(), 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, st)) != RAMP_OK) return rc;
     // 3. one Adam step; with no row in the batch, none (the step count stays)
-    AdamArgs aa{};
-    aa.lr = cfg->lr; aa.beta1 = cfg->adam_beta1; aa.beta2 = cfg->adam_beta2;
-    aa.beta2_f = (float)cfg->adam_beta2; aa.one_m_beta1 = (float)(1.0 - cfg->adam_beta1); aa.one_m_beta2 = (float)(1.0 - cfg->adam_beta2);
-    aa.eps = (float)cfg->adam_eps;
-    aa.max_norm = (float)cfg->grad_clip; aa.n_rows = p->l_n_rows.get(); aa.mb = rows; aa.start = 0; aa.step = p->l_step.get();
-    aa.m = p->l_adam_m.get(); aa.v = p->l_adam_v.get(); aa.grad = p->l_grad.get(); aa.norm_part = p->l_norm_part.get(); aa.w = p->d_w.get();
-    aa.row_stats = nullptr; aa.stats = p->l_stats.get();            // PG's statistics: ramp_pg_stats_kernel, after it
-    aa.parity = p->adam_parity; p->adam_parity ^= 1;
-    ramp_adam_kernel<<<LRN_GRID, 256, 0, st>>>(aa, p->n_weights);
+    AdamArgs aa = adam_args(p, *cfg, p->l_n_rows.get(), rows);
+    aa.stats = p->l_stats.get();                                      // PG's statistics: ramp_pg_stats_kernel, after it
+    if ((rc = launch_adam(p, aa, st)) != RAMP_OK) return rc;
     // 4. the statistics: the call's one read-back
     ramp_pg_stats_kernel<<<1, 1, 0, st>>>(p->l_row_stats.get(), p->l_row_model.get(), p->b_adv.get(), rows, p->l_n_rows.get(),
                                           p->l_norm_part.get(), p->l_stats.get());

@@ -67,11 +67,13 @@ class _CConfig(C.Structure):
                                                     ('standardize_advantages', C.c_int32)]
 
 
-def c_config(cfg: PPOConfig) -> _CConfig:
-    c = _CConfig()
-    for f in _CConfig._fields_:
-        v = getattr(cfg, f[0])
-        setattr(c, f[0], int(v) & (2 ** 64 - 1) if f[0] == 'seed' else (int(v) if f[1] is C.c_int32 else float(v)))
+def _c_struct(struct, cfg, **override):
+    """the config dataclass cfg as the C structure `struct`, field by field of its _fields_ (a keyword overrides cfg's attribute):
+    a uint64 masked to 64 bits, an int32 as int, a double as float"""
+    c = struct()
+    for name, ct in struct._fields_:
+        v = override[name] if name in override else getattr(cfg, name)
+        setattr(c, name, int(v) & (2 ** 64 - 1) if ct is C.c_uint64 else int(v) if ct is C.c_int32 else float(v))
     return c
 
 
@@ -103,49 +105,54 @@ class _CIMPALAConfig(C.Structure):
         'adam_beta1', 'adam_beta2', 'adam_eps')] + [('rollout_fragment_length', C.c_int32), ('train_batch_size', C.c_int32)]
 
 
-def c_impala_config(cfg: IMPALAConfig) -> _CIMPALAConfig:
-    c = _CIMPALAConfig()
-    for name, ct in _CIMPALAConfig._fields_:
-        setattr(c, name, int(getattr(cfg, name)) if ct is C.c_int32 else float(getattr(cfg, name)))
-    return c
-
-
 def _bind(L):
+    """every learner call's signature, once per library"""
     if getattr(L, '_learn_bound', False):
         return
-    L.ramp_ppo_loss_grad.restype = C.c_int
-    L.ramp_ppo_loss_grad.argtypes = [C.c_void_p, C.POINTER(_CConfig), C.c_int32] + [C.c_void_p] * 9
-    L.ramp_policy_learn.restype = C.c_int
-    L.ramp_policy_learn.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CConfig), C.c_void_p]
-    L.ramp_policy_train_batch_read.restype = C.c_int
-    L.ramp_policy_train_batch_read.argtypes = [C.c_void_p, C.c_void_p] + [C.c_void_p] * 7
-    L.ramp_policy_learner_state.restype = C.c_int
-    L.ramp_policy_learner_state.argtypes = [C.c_void_p] * 4
-    L.ramp_policy_learner_reset.restype = C.c_int
-    L.ramp_policy_learner_reset.argtypes = [C.c_void_p]
-    L.ramp_impala_loss_grad.restype = C.c_int
-    L.ramp_impala_loss_grad.argtypes = [C.c_void_p, C.POINTER(_CIMPALAConfig), C.c_int32, C.c_int32] + [C.c_void_p] * 12
-    L.ramp_policy_learn_impala.restype = C.c_int
-    L.ramp_policy_learn_impala.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CIMPALAConfig), C.c_void_p]
-    L.ramp_impala_vtrace_read.restype = C.c_int
-    L.ramp_impala_vtrace_read.argtypes = [C.c_void_p] * 6
+    for name, args in (('ramp_ppo_loss_grad', [C.c_void_p, C.POINTER(_CConfig), C.c_int32] + [C.c_void_p] * 9),
+                       ('ramp_policy_learn', [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CConfig), C.c_void_p]),
+                       ('ramp_policy_train_batch_read', [C.c_void_p, C.c_void_p] + [C.c_void_p] * 7),
+                       ('ramp_policy_learner_state', [C.c_void_p] * 4),
+                       ('ramp_policy_learner_reset', [C.c_void_p]),
+                       ('ramp_impala_loss_grad', [C.c_void_p, C.POINTER(_CIMPALAConfig), C.c_int32, C.c_int32] + [C.c_void_p] * 12),
+                       ('ramp_policy_learn_impala', [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CIMPALAConfig), C.c_void_p]),
+                       ('ramp_impala_vtrace_read', [C.c_void_p] * 6),
+                       ('ramp_pg_loss_grad', [C.c_void_p, C.POINTER(_CPGConfig), C.c_int32] + [C.c_void_p] * 7),
+                       ('ramp_policy_learn_pg', [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CPGConfig), C.c_void_p]),
+                       ('ramp_es_create', [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+                       ('ramp_es_round_begin', [C.c_void_p, C.c_void_p, C.POINTER(_CESConfig), C.c_int32]),
+                       ('ramp_es_act', [C.c_void_p, C.c_void_p, C.c_int32]),
+                       ('ramp_es_round_end', [C.c_void_p, C.c_void_p, C.c_void_p]),
+                       ('ramp_es_step', [C.c_void_p, C.POINTER(_CESConfig), C.c_void_p]),
+                       ('ramp_es_update', [C.c_void_p, C.POINTER(_CESConfig), C.c_int32] + [C.c_void_p] * 5),
+                       ('ramp_es_read', [C.c_void_p] * 12),
+                       ('ramp_es_act_read', [C.c_void_p] * 5),
+                       ('ramp_es_state', [C.c_void_p] * 4),
+                       ('ramp_es_reset', [C.c_void_p])):
+        getattr(L, name).restype = C.c_int
+        getattr(L, name).argtypes = args
+    L.ramp_es_destroy.restype = None
+    L.ramp_es_destroy.argtypes = [C.c_void_p]
     L._learn_bound = True
 
 
-def _stats(raw) -> Dict[str, float]:
-    return {k: float(v) for k, v in zip(STATS, raw)}
+def _stats(keys, out) -> Dict[str, float]:
+    return {k: float(v) for k, v in zip(keys, out)}
 
 
-class DevicePPOLearner:
-    def __init__(self, policy, config: PPOConfig = None):
+class _GradientLearner:
+    """What the PPO, IMPALA and PG learners share: the policy whose weights they update in place, and Adam's moments and step
+    count, which are the policy's -- one set, whichever of the three learners made the step."""
+    _Config = None                    # the learner's config dataclass
+
+    def __init__(self, policy, config=None):
         """policy: a DeviceGNNPolicy, whose weights the learner updates in place (Adam's state lives with the policy)."""
         self.policy = policy
-        self.config = dataclasses.replace(config) if config is not None else PPOConfig()
+        self.config = dataclasses.replace(config) if config is not None else self._Config()
         self._L = policy._L
         _bind(self._L)
-        self._calls = 0
 
-    def collect_and_learn(self, env, horizon: int, seed: int = 0) -> Dict[str, float]:
+    def collect_and_learn(self, env, horizon: int, seed: int = 0):
         """policy.collect(env, horizon) then learn(); also returns the wall time of each (seconds) and the segment's trajectory."""
         t0 = time.perf_counter()
         traj = self.policy.collect(env, horizon, sample=True, seed=seed)
@@ -154,6 +161,35 @@ class DevicePPOLearner:
         stats['collect_s'], stats['learn_s'] = t1 - t0, time.perf_counter() - t1
         return stats, traj
 
+    def adam_state(self):
+        """torch.optim.Adam's state of the flat weight vector: exp_avg, exp_avg_sq (blob order) and the step count"""
+        n = self._L.ramp_policy_weight_count(C.byref(self.policy._cfg))
+        m, v, step = np.zeros(n, np.float32), np.zeros(n, np.float32), C.c_int32()
+        _engine._check(self._L.ramp_policy_learner_state(self.policy._h, m.ctypes.data, v.ctypes.data, C.byref(step)))
+        return m, v, step.value
+
+    def reset(self):
+        """zero Adam's moments and step count"""
+        _engine._check(self._L.ramp_policy_learner_reset(self.policy._h))
+
+
+def _train_batch(self, env) -> Dict[str, np.ndarray]:
+    """the last learn()'s train batch: per live row, t-major, the job type, action, collected log-probability, the one the gradient
+    kernel recomputed from the collection weights (logp_old), the advantage and the value target (PPO: standardised when configured,
+    and GAE's target; PG: both the discounted return)"""
+    cap = self.policy._traj_key[0] * env.B            # the segment's rows: (horizon, B, |A|) of the last collect()
+    n = C.c_int32()
+    arrs = {'model': np.zeros(cap, np.int32), 'action': np.zeros(cap, np.int32), 'logp': np.zeros(cap, np.float32),
+            'logp_old': np.zeros(cap, np.float32), 'advantage': np.zeros(cap, np.float32), 'value_target': np.zeros(cap, np.float32)}
+    _engine._check(self._L.ramp_policy_train_batch_read(self.policy._h, env.eng._h, C.byref(n), *[a.ctypes.data for a in arrs.values()]))
+    return {k: v[:n.value].copy() for k, v in arrs.items()}
+
+
+class DevicePPOLearner(_GradientLearner):
+    _Config = PPOConfig
+    _calls = 0
+    train_batch = _train_batch
+
     def learn(self, env, horizon: int) -> Dict[str, float]:
         """One PPO learner step on the first ``horizon`` steps of the segment the policy's last collect(env, ...) recorded (a shorter
         horizon bootstraps its advantages with the value recorded at the next step): the statistics averaged over the
@@ -161,21 +197,12 @@ class DevicePPOLearner:
         Call k of this learner shuffles with the seed config.seed + k."""
         cfg = dataclasses.replace(self.config, seed=self.config.seed + self._calls)
         out = np.zeros(len(STATS), dtype=np.float64)
-        _engine._check(self._L.ramp_policy_learn(self.policy._h, env.eng._h, int(horizon), C.byref(c_config(cfg)), out.ctypes.data))
+        _engine._check(self._L.ramp_policy_learn(self.policy._h, env.eng._h, int(horizon), C.byref(_c_struct(_CConfig, cfg)),
+                                                 out.ctypes.data))
         self._calls += 1
-        stats = _stats(out)
+        stats = _stats(STATS, out)
         self.config.kl_coeff = stats['kl_coeff']
         return stats
-
-    def train_batch(self, env) -> Dict[str, np.ndarray]:
-        """the last learn()'s train batch: per live row, t-major, the job type, action, collected log-probability, the one
-        recomputed from the collection weights, the advantage (standardised when configured) and the value target"""
-        cap = self.policy._traj_key[0] * env.B            # the segment's rows: (horizon, B, |A|) of the last collect()
-        n = C.c_int32()
-        arrs = {'model': np.zeros(cap, np.int32), 'action': np.zeros(cap, np.int32), 'logp': np.zeros(cap, np.float32),
-                'logp_old': np.zeros(cap, np.float32), 'advantage': np.zeros(cap, np.float32), 'value_target': np.zeros(cap, np.float32)}
-        _engine._check(self._L.ramp_policy_train_batch_read(self.policy._h, env.eng._h, C.byref(n), *[a.ctypes.data for a in arrs.values()]))
-        return {k: v[:n.value].copy() for k, v in arrs.items()}
 
     def loss_and_grad(self, batch: Dict[str, np.ndarray]):
         """PPO's loss statistics (STATS) and gradient (blob order) on one minibatch of host arrays, with no update: model [n],
@@ -190,51 +217,25 @@ class DevicePPOLearner:
         vt = np.ascontiguousarray(batch['value_target'], dtype=np.float32).reshape(n)
         grad = np.zeros(pol._L.ramp_policy_weight_count(C.byref(pol._cfg)), dtype=np.float32)
         out = np.zeros(len(STATS), dtype=np.float64)
-        _engine._check(self._L.ramp_ppo_loss_grad(pol._h, C.byref(c_config(self.config)), n, model.ctypes.data, gf.ctypes.data,
-                                                  mask.ctypes.data, act.ctypes.data, old.ctypes.data, adv.ctypes.data, vt.ctypes.data,
-                                                  grad.ctypes.data, out.ctypes.data))
-        return _stats(out), grad
-
-    def adam_state(self):
-        """torch.optim.Adam's state of the flat weight vector: exp_avg, exp_avg_sq (blob order) and the step count"""
-        n = self._L.ramp_policy_weight_count(C.byref(self.policy._cfg))
-        m, v, step = np.zeros(n, np.float32), np.zeros(n, np.float32), C.c_int32()
-        _engine._check(self._L.ramp_policy_learner_state(self.policy._h, m.ctypes.data, v.ctypes.data, C.byref(step)))
-        return m, v, step.value
-
-    def reset(self):
-        """zero Adam's moments and step count"""
-        _engine._check(self._L.ramp_policy_learner_reset(self.policy._h))
+        _engine._check(self._L.ramp_ppo_loss_grad(pol._h, C.byref(_c_struct(_CConfig, self.config)), n, model.ctypes.data,
+                                                  gf.ctypes.data, mask.ctypes.data, act.ctypes.data, old.ctypes.data, adv.ctypes.data,
+                                                  vt.ctypes.data, grad.ctypes.data, out.ctypes.data))
+        return _stats(STATS, out), grad
 
 
-class DeviceIMPALALearner:
+class DeviceIMPALALearner(_GradientLearner):
     """RLlib's IMPALA learner step (V-trace, VTraceLoss, clip_grad_norm_, Adam) on the segment the policy's last collect()
     recorded, on the device.  Adam's moments and step count are the policy's, shared with DevicePPOLearner."""
-
-    def __init__(self, policy, config: IMPALAConfig = None):
-        """policy: a DeviceGNNPolicy, whose weights the learner updates in place"""
-        self.policy = policy
-        self.config = dataclasses.replace(config) if config is not None else IMPALAConfig()
-        self._L = policy._L
-        _bind(self._L)
-
-    def collect_and_learn(self, env, horizon: int, seed: int = 0):
-        """policy.collect(env, horizon) then learn(); also returns the wall time of each (seconds) and the segment's trajectory."""
-        t0 = time.perf_counter()
-        traj = self.policy.collect(env, horizon, sample=True, seed=seed)
-        t1 = time.perf_counter()
-        stats = self.learn(env, horizon)
-        stats['collect_s'], stats['learn_s'] = t1 - t0, time.perf_counter() - t1
-        return stats, traj
+    _Config = IMPALAConfig
 
     def learn(self, env, horizon: int) -> Dict[str, float]:
         """One IMPALA learner step on the first ``horizon`` steps of the segment the policy's last collect(env, ...) recorded: the
         fragments of rollout_fragment_length rows (0: horizon), one Adam step per train batch of train_batch_size // L fragments,
         in order.  Returns the means over the call's SGD steps (IMPALA_STATS), and their number as sgd_steps."""
         out = np.zeros(len(IMPALA_STATS), dtype=np.float64)
-        _engine._check(self._L.ramp_policy_learn_impala(self.policy._h, env.eng._h, int(horizon), C.byref(c_impala_config(self.config)),
-                                                        out.ctypes.data))
-        return {k: float(v) for k, v in zip(IMPALA_STATS, out)}
+        _engine._check(self._L.ramp_policy_learn_impala(self.policy._h, env.eng._h, int(horizon),
+                                                        C.byref(_c_struct(_CIMPALAConfig, self.config)), out.ctypes.data))
+        return _stats(IMPALA_STATS, out)
 
     def vtrace(self) -> Dict[str, np.ndarray]:
         """per fragment row (r = f L + t) of the last learn() or loss_and_grad(), as the step that used it computed it: the target
@@ -260,19 +261,11 @@ class DeviceIMPALALearner:
         grad = np.zeros(pol._L.ramp_policy_weight_count(C.byref(pol._cfg)), dtype=np.float32)
         out = np.zeros(len(IMPALA_STATS), dtype=np.float64)
         vt = {k: np.zeros(n * L, np.float32) for k in ('vs', 'pg_advantages', 'log_rho')}
-        _engine._check(self._L.ramp_impala_loss_grad(pol._h, C.byref(c_impala_config(self.config)), int(n), int(L), model.ctypes.data,
-                                                     gf.ctypes.data, mask.ctypes.data, act.ctypes.data, blogp.ctypes.data,
-                                                     reward.ctypes.data, done.ctypes.data, grad.ctypes.data, out.ctypes.data,
-                                                     *[a.ctypes.data for a in vt.values()]))
-        return {k: float(v) for k, v in zip(IMPALA_STATS, out)}, grad, {k: v.reshape(n, L) for k, v in vt.items()}
-
-    def adam_state(self):
-        """torch.optim.Adam's state of the flat weight vector (the policy's, shared with DevicePPOLearner)"""
-        return DevicePPOLearner.adam_state(self)
-
-    def reset(self):
-        """zero Adam's moments and step count"""
-        _engine._check(self._L.ramp_policy_learner_reset(self.policy._h))
+        _engine._check(self._L.ramp_impala_loss_grad(pol._h, C.byref(_c_struct(_CIMPALAConfig, self.config)), int(n), int(L),
+                                                     model.ctypes.data, gf.ctypes.data, mask.ctypes.data, act.ctypes.data,
+                                                     blogp.ctypes.data, reward.ctypes.data, done.ctypes.data, grad.ctypes.data,
+                                                     out.ctypes.data, *[a.ctypes.data for a in vt.values()]))
+        return _stats(IMPALA_STATS, out), grad, {k: v.reshape(n, L) for k, v in vt.items()}
 
 
 PG_STATS = ('policy_loss', 'entropy', 'grad_gnorm', 'rows')
@@ -294,40 +287,11 @@ class _CPGConfig(C.Structure):
     _fields_ = [(n, C.c_double) for n in ('gamma', 'grad_clip', 'lr', 'adam_beta1', 'adam_beta2', 'adam_eps')]
 
 
-def c_pg_config(cfg: PGConfig) -> _CPGConfig:
-    return _CPGConfig(*(float(getattr(cfg, n)) for n, _ in _CPGConfig._fields_))
-
-
-def _bind_pg(L):
-    if getattr(L, '_pg_bound', False):
-        return
-    _bind(L)
-    L.ramp_pg_loss_grad.restype = C.c_int
-    L.ramp_pg_loss_grad.argtypes = [C.c_void_p, C.POINTER(_CPGConfig), C.c_int32] + [C.c_void_p] * 7
-    L.ramp_policy_learn_pg.restype = C.c_int
-    L.ramp_policy_learn_pg.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CPGConfig), C.c_void_p]
-    L._pg_bound = True
-
-
-class DevicePGLearner:
+class DevicePGLearner(_GradientLearner):
     """RLlib's PG learner step (discounted returns, pg_torch_loss, Adam) on the segment the policy's last collect() recorded, on
     the device.  Adam's moments and step count are the policy's, shared with DevicePPOLearner and DeviceIMPALALearner."""
-
-    def __init__(self, policy, config: PGConfig = None):
-        """policy: a DeviceGNNPolicy, whose weights the learner updates in place"""
-        self.policy = policy
-        self.config = dataclasses.replace(config) if config is not None else PGConfig()
-        self._L = policy._L
-        _bind_pg(self._L)
-
-    def collect_and_learn(self, env, horizon: int, seed: int = 0):
-        """policy.collect(env, horizon) then learn(); also returns the wall time of each (seconds) and the segment's trajectory."""
-        t0 = time.perf_counter()
-        traj = self.policy.collect(env, horizon, sample=True, seed=seed)
-        t1 = time.perf_counter()
-        stats = self.learn(env, horizon)
-        stats['collect_s'], stats['learn_s'] = t1 - t0, time.perf_counter() - t1
-        return stats, traj
+    _Config = PGConfig
+    train_batch = _train_batch
 
     def learn(self, env, horizon: int) -> Dict[str, float]:
         """One PG learner step on the first ``horizon`` steps of the segment the policy's last collect(env, ...) recorded: one train
@@ -337,14 +301,9 @@ class DevicePGLearner:
         segment holds the env-steps it wants per update (pg's train_batch_size is 200) and its episodes end inside it.  Returns
         PG_STATS; a segment with no decision makes no update and leaves Adam's step count as it was."""
         out = np.zeros(len(PG_STATS), dtype=np.float64)
-        _engine._check(self._L.ramp_policy_learn_pg(self.policy._h, env.eng._h, int(horizon), C.byref(c_pg_config(self.config)),
+        _engine._check(self._L.ramp_policy_learn_pg(self.policy._h, env.eng._h, int(horizon), C.byref(_c_struct(_CPGConfig, self.config)),
                                                     out.ctypes.data))
-        return {k: float(v) for k, v in zip(PG_STATS, out)}
-
-    def train_batch(self, env) -> Dict[str, np.ndarray]:
-        """the last learn()'s train batch: per live row, t-major, the job type, action, collected log-probability, the one the
-        gradient kernel recomputed at the collection weights (logp_old) and the discounted return (advantage, value_target)"""
-        return DevicePPOLearner.train_batch(self, env)
+        return _stats(PG_STATS, out)
 
     def loss_and_grad(self, batch: Dict[str, np.ndarray]):
         """pg_torch_loss's statistics (PG_STATS) and gradient (blob order) on host rows, with no update: model [n],
@@ -356,17 +315,10 @@ class DevicePGLearner:
         adv = np.ascontiguousarray(batch['advantage'], dtype=np.float32).reshape(n)
         grad = np.zeros(pol._L.ramp_policy_weight_count(C.byref(pol._cfg)), dtype=np.float32)
         out = np.zeros(len(PG_STATS), dtype=np.float64)
-        _engine._check(self._L.ramp_pg_loss_grad(pol._h, C.byref(c_pg_config(self.config)), n, model.ctypes.data, gf.ctypes.data,
-                                                 mask.ctypes.data, act.ctypes.data, adv.ctypes.data, grad.ctypes.data, out.ctypes.data))
-        return {k: float(v) for k, v in zip(PG_STATS, out)}, grad
-
-    def adam_state(self):
-        """torch.optim.Adam's state of the flat weight vector (the policy's, shared with DevicePPOLearner)"""
-        return DevicePPOLearner.adam_state(self)
-
-    def reset(self):
-        """zero Adam's moments and step count"""
-        _engine._check(self._L.ramp_policy_learner_reset(self.policy._h))
+        _engine._check(self._L.ramp_pg_loss_grad(pol._h, C.byref(_c_struct(_CPGConfig, self.config)), n, model.ctypes.data,
+                                                 gf.ctypes.data, mask.ctypes.data, act.ctypes.data, adv.ctypes.data, grad.ctypes.data,
+                                                 out.ctypes.data))
+        return _stats(PG_STATS, out), grad
 
 
 ES_STATS = ('episode_reward_mean', 'episode_len_mean', 'timesteps_this_iter', 'episodes_this_iter', 'weights_norm', 'grad_norm',
@@ -408,26 +360,6 @@ def shared_noise_table(size: int) -> np.ndarray:
     return np.random.RandomState(123).randn(int(size)).astype(np.float32)
 
 
-def _bind_es(L):
-    if getattr(L, '_es_bound', False):
-        return
-    for name, args in (('ramp_es_create', [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
-                       ('ramp_es_round_begin', [C.c_void_p, C.c_void_p, C.POINTER(_CESConfig), C.c_int32]),
-                       ('ramp_es_act', [C.c_void_p, C.c_void_p, C.c_int32]),
-                       ('ramp_es_round_end', [C.c_void_p, C.c_void_p, C.c_void_p]),
-                       ('ramp_es_step', [C.c_void_p, C.POINTER(_CESConfig), C.c_void_p]),
-                       ('ramp_es_update', [C.c_void_p, C.POINTER(_CESConfig), C.c_int32] + [C.c_void_p] * 5),
-                       ('ramp_es_read', [C.c_void_p] * 12),
-                       ('ramp_es_act_read', [C.c_void_p] * 5),
-                       ('ramp_es_state', [C.c_void_p] * 4),
-                       ('ramp_es_reset', [C.c_void_p])):
-        getattr(L, name).restype = C.c_int
-        getattr(L, name).argtypes = args
-    L.ramp_es_destroy.restype = None
-    L.ramp_es_destroy.argtypes = [C.c_void_p]
-    L._es_bound = True
-
-
 class DeviceESLearner:
     """RLlib's ES training step (es.py training_step) with a DeviceRampJobPartitioningEnvironment's B episodes as the population:
     per round, N = (B - E) / 2 antithetic pairs (episode 2i at theta + sigma eps_i, 2i + 1 at theta - sigma eps_i) and E eval
@@ -444,7 +376,7 @@ class DeviceESLearner:
             raise ValueError(f"observation_filter {self.config.observation_filter!r}: only 'NoFilter' is supported (MeanStdFilter would "
                              'standardise the padded edge indices and the action mask the GNN reads back from the observation)')
         self._L = policy._L
-        _bind_es(self._L)
+        _bind(self._L)
         noise = shared_noise_table(self.config.noise_size) if noise is None else np.ascontiguousarray(noise, dtype=np.float32).ravel()
         self.noise_size = len(noise)
         self._h = C.c_void_p()
@@ -472,10 +404,7 @@ class DeviceESLearner:
         return E + ((B - E) & 1)
 
     def _c(self, B: int) -> _CESConfig:
-        c = self.config
-        return _CESConfig(int(c.seed) & (2 ** 64 - 1), float(c.noise_stdev), float(c.stepsize), float(c.l2_coeff), float(c.adam_beta1),
-                          float(c.adam_beta2), float(c.adam_eps), int(c.episodes_per_batch), int(c.train_batch_size), self.n_eval(B),
-                          int(c.report_length))
+        return _c_struct(_CESConfig, self.config, n_eval=self.n_eval(B))
 
     def begin_round(self, env, rnd: int):
         """after env.reset(): round rnd's noise indices, weight sets and embeddings (round 0 starts a new step)"""
@@ -498,7 +427,7 @@ class DeviceESLearner:
         """the update on the step record of the rounds since the last begin_round(env, 0) (ranks, g, Adam); ES_STATS"""
         out = np.zeros(len(ES_STATS), dtype=np.float64)
         _engine._check(self._L.ramp_es_step(self._h, C.byref(self._c(self._B)), out.ctypes.data))
-        return {k: float(v) for k, v in zip(ES_STATS, out)}
+        return _stats(ES_STATS, out)
 
     def learn(self, env, timing: bool = False) -> Dict[str, float]:
         """One ES training step (ES_STATS).  Each round resets env and runs env.J env-steps, so every episode ends in it; the
@@ -541,7 +470,7 @@ class DeviceESLearner:
         out = np.zeros(len(ES_STATS), dtype=np.float64)
         _engine._check(self._L.ramp_es_update(self._h, C.byref(self._c(2 * len(idx) + 1)), len(idx), idx.ctypes.data, ret.ctypes.data,
                                               ranks.ctypes.data, g.ctypes.data, out.ctypes.data))
-        return {k: float(v) for k, v in zip(ES_STATS, out)}, ranks, g
+        return _stats(ES_STATS, out), ranks, g
 
     def last_step(self) -> Dict[str, np.ndarray]:
         """the last step's record: noise_index [n], returns and lengths [n, 2], the act seeds in order (round-major, env-step t of
