@@ -10,7 +10,7 @@ SOURCES = [os.path.join(HERE, 'csrc', 'ramp_engine.cu'), os.path.join(HERE, 'csr
 DEPS = SOURCES + [os.path.join(HERE, 'csrc', 'ramp_kernels.cuh'), os.path.join(HERE, 'csrc', 'ramp_lookahead_cta.cuh'),
                   os.path.join(HERE, 'csrc', 'ramp_lookahead_thread.cuh'), os.path.join(HERE, 'csrc', 'ramp_env.cuh'), os.path.join(HERE, 'csrc', 'ramp_env_io.cuh'),
                   os.path.join(HERE, 'csrc', 'ramp_owned.cuh'), os.path.join(HERE, 'csrc', 'ramp_policy_learn.cuh'),
-                  os.path.join(HERE, 'csrc', 'ramp_es.cuh'),
+                  os.path.join(HERE, 'csrc', 'ramp_es.cuh'), os.path.join(HERE, 'csrc', 'ramp_population.cuh'),
                   os.path.join(os.path.dirname(HERE), 'include', 'ramp_b200.h')]
 
 NVCC_FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo',

@@ -200,8 +200,9 @@ __device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
     return x ^ (x >> 31);
 }
 
-// at most 80 registers (three CTAs per SM), what the kernel used before its read-out was padded to Hp: left alone, ptxas takes 113
-__global__ void __launch_bounds__(256, 3) ramp_policy_head_kernel(const PolicyDev P, const HeadArgs a) {
+// ramp_policy_head_kernel's statements with the weight blob `w` (P's layout), CTA `cta` of n_ctas: shared with the population's
+// head kernel, which runs one weight set per blockIdx.y
+__device__ __forceinline__ void head_body(const PolicyDev& P, const float* w, const HeadArgs& a, int cta, int n_ctas) {
     extern __shared__ float sm[];
     const ramp_policy_config_t& c = P.c;
     const int gin = c.in_features_graph + c.n_actions, og = c.out_features_graph, on = c.out_features_node, fin = on + og;
@@ -216,7 +217,6 @@ __global__ void __launch_bounds__(256, 3) ramp_policy_head_kernel(const PolicyDe
     float* s_lW = s_vhb + (share ? 0 : Hp); float* s_lb = s_lW + (size_t)A * Hp;     // [A][Hp]
     float* s_vW = s_lb + A;              float* s_vb = s_vW + Hp;
     float* s_warp = s_vb + 1;
-    const float* w = P.w;
     for (int i = threadIdx.x; i < gin; i += blockDim.x) { s_gln_w[i] = w[P.gln_w + i]; s_gln_b[i] = w[P.gln_b + i]; }
     for (int i = threadIdx.x; i < og * gin; i += blockDim.x) s_gW[i] = w[P.gW + i];
     for (int i = threadIdx.x; i < og; i += blockDim.x) s_gb[i] = w[P.gb + i];
@@ -244,7 +244,7 @@ __global__ void __launch_bounds__(256, 3) ramp_policy_head_kernel(const PolicyDe
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpc = blockDim.x >> 5;
     float* xb = s_warp + (size_t)warp * 2 * POL_MAX_DIM;                // graph-module input, then the read-out input
     float* fb = xb + POL_MAX_DIM;
-    for (int b = blockIdx.x * wpc + warp; b < a.n; b += gridDim.x * wpc) {
+    for (int b = cta * wpc + warp; b < a.n; b += n_ctas * wpc) {
         const int m = a.model[b];
         const bool live = m >= 0 && m < c.n_models && !(a.done && a.done[b]);
         if (!live) {                                                    // nothing queued: the action is ignored by the environment
@@ -337,6 +337,11 @@ __global__ void __launch_bounds__(256, 3) ramp_policy_head_kernel(const PolicyDe
         }
         __syncwarp();
     }
+}
+
+// at most 80 registers (three CTAs per SM), what the kernel used before its read-out was padded to Hp: left alone, ptxas takes 113
+__global__ void __launch_bounds__(256, 3) ramp_policy_head_kernel(const PolicyDev P, const HeadArgs a) {
+    head_body(P, P.w, a, blockIdx.x, gridDim.x);
 }
 
 // one launch per phase instead of a handful of small device-to-device copies
@@ -625,32 +630,36 @@ int ensure_learner(ramp_policy* p) {
     return RAMP_OK;
 }
 
+// one job type's forward states and records for the embedding backward (N nodes, E edges), appended to `allocs`
+int alloc_grad_scratch(const ramp_policy_config_t& c, size_t N, size_t E, std::vector<DeviceArray<unsigned char>>& allocs, GradModelDev& g) {
+    const GnnDims D = gnn_dims(c);
+    const size_t half = c.out_features_msg / 2, R = c.num_rounds;
+    auto take = [&](size_t floats, float** dst) -> int {
+        allocs.emplace_back();
+        CUDA_TRY(allocs.back().alloc(sizeof(float) * floats));
+        *dst = (float*)allocs.back().get();
+        return RAMP_OK;
+    };
+    int rc;
+    if ((rc = take(R * N * D.zs, &g.z)) || (rc = take(R * N * half, &g.hn)) || (rc = take(R * E * half, &g.he)) ||
+        (rc = take(N * D.zs, &g.dz)) || (rc = take(N * D.zs, &g.dz2)) || (rc = take(N * half, &g.dhn)) ||
+        (rc = take(N * D.nrs, &g.nrec)) || (rc = take(E * D.ers, &g.erec)) || (rc = take((N + E) * D.mrs, &g.mrec)) ||
+        (rc = take((N + E) * c.out_features_msg, &g.mdx)))
+        return rc;
+    return RAMP_OK;
+}
+
 // every job type's forward states and records for the embedding backward, sized by its graph
 int ensure_gmodels(ramp_policy* p, cudaStream_t st) {
     if (p->gmodels_ready) return RAMP_OK;
-    const ramp_policy_config_t& c = p->P.c;
-    const GnnDims D = gnn_dims(c);
-    const size_t half = c.out_features_msg / 2, R = c.num_rounds;
     std::vector<GradModelDev> h(p->models.size());
     for (size_t m = 0; m < h.size(); ++m) {
         HostModel& hm = p->models[m];
         if (!hm.set) return set_error(RAMP_ERR_BAD_ARG, "policy: model %zu was never registered (ramp_policy_set_model)", m);
         if (!hm.grad_ready) {
             hm.lallocs.clear();
-            const size_t N = hm.d.n_nodes, E = hm.d.n_edges;
-            auto take = [&](size_t floats, float** dst) -> int {
-                hm.lallocs.emplace_back();
-                CUDA_TRY(hm.lallocs.back().alloc(sizeof(float) * floats));
-                *dst = (float*)hm.lallocs.back().get();
-                return RAMP_OK;
-            };
-            GradModelDev& g = hm.g;
-            int rc;
-            if ((rc = take(R * N * D.zs, &g.z)) || (rc = take(R * N * half, &g.hn)) || (rc = take(R * E * half, &g.he)) ||
-                (rc = take(N * D.zs, &g.dz)) || (rc = take(N * D.zs, &g.dz2)) || (rc = take(N * half, &g.dhn)) ||
-                (rc = take(N * D.nrs, &g.nrec)) || (rc = take(E * D.ers, &g.erec)) || (rc = take((N + E) * D.mrs, &g.mrec)) ||
-                (rc = take((N + E) * c.out_features_msg, &g.mdx)))
-                return rc;
+            const int rc = alloc_grad_scratch(p->P.c, hm.d.n_nodes, hm.d.n_edges, hm.lallocs, hm.g);
+            if (rc != RAMP_OK) return rc;
             hm.grad_ready = true;
         }
         h[m] = hm.g;
@@ -1574,3 +1583,4 @@ int ramp_policy_learn_pg(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, 
 }  // extern "C"
 
 #include "ramp_es.cuh"
+#include "ramp_population.cuh"

@@ -177,7 +177,9 @@ struct GradArgs {
     float* logp_old;                     // [batch] log-probability of the action under the old logits, or nullptr
 };
 
-__global__ void __launch_bounds__(256) ramp_policy_head_grad_kernel(const PolicyDev P, const GradArgs g) {
+// ramp_policy_head_grad_kernel's statements for launch row i with the weight blob `w` (P's layout): shared with the population's
+// head-gradient kernel
+__device__ __forceinline__ void head_grad_body(const PolicyDev& P, const float* w, const GradArgs& g, const int i) {
     __shared__ float s_x[LRN_WARPS][POL_MAX_DIM], s_f[LRN_WARPS][POL_MAX_DIM], s_d[LRN_WARPS][POL_MAX_DIM];
     __shared__ float s_dh[LRN_WARPS][32 * POL_MAX_HPL], s_dhv[LRN_WARPS][32 * POL_MAX_HPL];
     const ramp_policy_config_t& c = P.c;
@@ -185,10 +187,8 @@ __global__ void __launch_bounds__(256) ramp_policy_head_grad_kernel(const Policy
     const int H = c.fcnet_hidden, A = c.n_actions, fa = c.fcnet_activation;
     const bool share = c.vf_share_layers;
     const HeadRec R = head_rec(c);
-    const float* w = P.w;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int hpl = (H - lane + 31) / 32;                          // this lane's hidden units lane + 32 u < H
-    const int i = blockIdx.x * LRN_WARPS + warp;
     if (i >= g.mb) return;
     float* rec = g.rec + (size_t)i * R.stride;
     const int n = *g.n_rows, pos = g.start + i;
@@ -361,6 +361,10 @@ __global__ void __launch_bounds__(256) ramp_policy_head_grad_kernel(const Policy
     }
 }
 
+__global__ void __launch_bounds__(256) ramp_policy_head_grad_kernel(const PolicyDev P, const GradArgs g) {
+    head_grad_body(P, P.w, g, blockIdx.x * LRN_WARPS + (threadIdx.x >> 5));
+}
+
 // the read-out's and graph module's segments in blob order (host: the learner's setup); their count (at most HEAD_SEGS)
 inline int head_segs(const PolicyDev& P, const float* rec, int mb, Seg* s) {
     const ramp_policy_config_t& c = P.c;
@@ -432,11 +436,13 @@ struct EmbGradArgs {
     float* gpart; int64_t n_gnn;                                    // backward: [n_models][n_gnn] per job type gradients of the rounds' weights
 };
 
+// ramp_gnn_embed_grad_kernel's statements for job type m with the weight blob `w` (P's layout), by the whole CTA: shared with the
+// population's instances, which run one (weight set, job type) item after another
 template <int MODE>
-__global__ void __launch_bounds__(256, 1) ramp_gnn_embed_grad_kernel(const PolicyDev P, const ModelDev* models, const GradModelDev* gms, const EmbGradArgs g) {
+__device__ __forceinline__ void embed_grad_body(const PolicyDev& P, const float* w, const ModelDev* models, const GradModelDev* gms,
+                                                const EmbGradArgs& g, const int m) {
     __shared__ float s_a[8][POL_MAX_DIM], s_b[8][POL_MAX_DIM], s_demb[POL_MAX_DIM];
     const ramp_policy_config_t& c = P.c;
-    const int m = blockIdx.x;
     const ModelDev M = models[m];
     const GradModelDev G = gms[m];
     const GnnDims D = gnn_dims(c);
@@ -445,7 +451,6 @@ __global__ void __launch_bounds__(256, 1) ramp_gnn_embed_grad_kernel(const Polic
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
     const int on = c.out_features_node, msg = c.out_features_msg, half = msg / 2, ine = c.in_features_edge, ak = c.aggregator_activation;
     const int N = M.n_nodes, E = M.n_edges;
-    const float* w = P.w;
     if (MODE == EMB_BACKWARD) {
         // ---- d emb[m]: the rows of this job type, in row order ----
         int any = 0;
@@ -672,6 +677,11 @@ __global__ void __launch_bounds__(256, 1) ramp_gnn_embed_grad_kernel(const Polic
     }
 }
 
+template <int MODE>
+__global__ void __launch_bounds__(256, 1) ramp_gnn_embed_grad_kernel(const PolicyDev P, const ModelDev* models, const GradModelDev* gms, const EmbGradArgs g) {
+    embed_grad_body<MODE>(P, P.w, models, gms, g, blockIdx.x);
+}
+
 // block-wide sum in a fixed order (every thread gets it)
 __device__ __forceinline__ double block_sum(double v, double* s_red) {
 #pragma unroll
@@ -686,7 +696,7 @@ __device__ __forceinline__ double block_sum(double v, double* s_red) {
     return t;
 }
 
-__global__ void __launch_bounds__(256) ramp_grad_finish_kernel(const float* gpart, int32_t n_models, int64_t n_gnn, int64_t n_w, float* grad, double* norm_part) {
+__device__ __forceinline__ void grad_finish_body(const float* gpart, int32_t n_models, int64_t n_gnn, int64_t n_w, float* grad, double* norm_part) {
     __shared__ double s_red[32];
     double q = 0.0;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_w; e += (int64_t)gridDim.x * blockDim.x) {
@@ -703,6 +713,10 @@ __global__ void __launch_bounds__(256) ramp_grad_finish_kernel(const float* gpar
     }
     q = block_sum(q, s_red);
     if (threadIdx.x == 0) norm_part[blockIdx.x] = q;
+}
+
+__global__ void __launch_bounds__(256) ramp_grad_finish_kernel(const float* gpart, int32_t n_models, int64_t n_gnn, int64_t n_w, float* grad, double* norm_part) {
+    grad_finish_body(gpart, n_models, n_gnn, n_w, grad, norm_part);
 }
 
 // the minibatch's statistics (RAMP_PPO_*): means over its rows, and the gradient's global norm before clipping
@@ -734,7 +748,7 @@ struct AdamArgs {
     const float* row_stats; float vf_coeff, ent_coeff, kl_coeff; double* stats;   // RAMP_PPO_STATS_LEN for this minibatch
 };
 
-__global__ void __launch_bounds__(256) ramp_adam_kernel(const AdamArgs a, int64_t n_w) {
+__device__ __forceinline__ void adam_body(const AdamArgs& a, int64_t n_w) {
     __shared__ double s_norm;
     const int rows = max(0, min(a.mb, *a.n_rows - a.start));
     const int t0 = a.step[a.parity];
@@ -764,6 +778,8 @@ __global__ void __launch_bounds__(256) ramp_adam_kernel(const AdamArgs a, int64_
     }
 }
 
+__global__ void __launch_bounds__(256) ramp_adam_kernel(const AdamArgs a, int64_t n_w) { adam_body(a, n_w); }
+
 // ramp_ppo_loss_grad's statistics (no update)
 __global__ void ramp_ppo_minibatch_stats_kernel(const float* row_stats, int32_t rows, float vf_coeff, float ent_coeff, float kl_coeff,
                                                 const double* norm_part, double* out) {
@@ -771,7 +787,7 @@ __global__ void ramp_ppo_minibatch_stats_kernel(const float* row_stats, int32_t 
 }
 
 // the mean of the last pass's minibatch statistics, and RLlib's PPO update_kl from its mean KL
-__global__ void ramp_ppo_learn_stats_kernel(const double* mb_stats, int32_t n_mb, float kl_coeff, float kl_target, const int32_t* n_rows, double* out) {
+__device__ __forceinline__ void learn_stats_body(const double* mb_stats, int32_t n_mb, float kl_coeff, float kl_target, const int32_t* n_rows, double* out) {
     double s[RAMP_PPO_STATS_LEN] = {};
     int k = 0;
     for (int i = 0; i < n_mb; ++i) {
@@ -790,6 +806,10 @@ __global__ void ramp_ppo_learn_stats_kernel(const double* mb_stats, int32_t n_mb
     out[RAMP_PPO_ROWS] = *n_rows;
 }
 
+__global__ void ramp_ppo_learn_stats_kernel(const double* mb_stats, int32_t n_mb, float kl_coeff, float kl_target, const int32_t* n_rows, double* out) {
+    learn_stats_body(mb_stats, n_mb, kl_coeff, kl_target, n_rows, out);
+}
+
 struct GaeArgs {
     int32_t T, B, A, n_models, standardize;
     double gamma, lambda;
@@ -804,19 +824,21 @@ struct GaeArgs {
 // episodes that were not finished when the decision was taken and had a queued job, t-major; then (a - mean) / max(1e-4, std).
 // Without values (t_value nullptr, lambda 1) the scan is r_t + gamma (1 - done_t) next with a 0 bootstrap: RLlib's
 // compute_advantages(use_gae=False, use_critic=False, last_r=0), discount_cumsum's recursion in f64; value_target = advantage.
-__global__ void __launch_bounds__(1024) ramp_ppo_gae_kernel(const GaeArgs a) {
+// ramp_ppo_gae_kernel's statements over a.B episodes whose trajectory rows are ld apart (the population's groups are column slices
+// of one [T][K b] trajectory); the batch a.B T rows long
+__device__ __forceinline__ void gae_body(const GaeArgs& a, const int ld) {
     __shared__ double s_red[32];
     __shared__ int s_scan[32];
     const int T = a.T, B = a.B;
-    auto alive = [&](int t, int b) { return t == 0 || !a.t_done[(size_t)(t - 1) * B + b]; };
+    auto alive = [&](int t, int b) { return t == 0 || !a.t_done[(size_t)(t - 1) * ld + b]; };
     for (int b = threadIdx.x; b < B; b += blockDim.x) {
         double next = 0.0;
         for (int t = T - 1; t >= 0; --t) {
-            const size_t i = (size_t)t * B + b;
+            const size_t i = (size_t)t * ld + b;
             if (!alive(t, b)) { a.adv64[i] = 0.0; continue; }
             const double nonterm = a.t_done[i] ? 0.0 : 1.0;
             const double V = a.t_value ? (double)a.t_value[i] : 0.0;
-            const double Vn = !a.t_value ? 0.0 : t == T - 1 ? (double)a.boot[b] : (double)a.t_value[i + B];
+            const double Vn = !a.t_value ? 0.0 : t == T - 1 ? (double)a.boot[b] : (double)a.t_value[i + ld];
             const double delta = a.t_reward[i] + a.gamma * Vn * nonterm - V;
             next = delta + a.gamma * a.lambda * nonterm * next;
             a.adv64[i] = next;
@@ -828,7 +850,7 @@ __global__ void __launch_bounds__(1024) ramp_ppo_gae_kernel(const GaeArgs a) {
     for (int t = 0; t < T; ++t) {
         for (int b0 = 0; b0 < B; b0 += blockDim.x) {
             const int b = b0 + threadIdx.x;
-            const size_t i = (size_t)t * B + b;
+            const size_t i = (size_t)t * ld + b;
             const int flag = b < B && alive(t, b) && a.t_model[i] >= 0 && a.t_model[i] < a.n_models;
             int x = flag;
 #pragma unroll
@@ -867,6 +889,8 @@ __global__ void __launch_bounds__(1024) ramp_ppo_gae_kernel(const GaeArgs a) {
     }
     if (threadIdx.x == 0) *a.n_rows = n;
 }
+
+__global__ void __launch_bounds__(1024) ramp_ppo_gae_kernel(const GaeArgs a) { gae_body(a, a.B); }
 
 // ---- IMPALA (ramp_policy_learn_impala, ramp_impala_loss_grad) ----
 

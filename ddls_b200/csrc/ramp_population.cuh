@@ -1,0 +1,526 @@
+// ramp_population.cuh -- K independent PPO trainings of the GNN policy in one environment batch (include/ramp_b200.h:
+// ramp_population_*).  Included by ramp_policy.cu after the learner.
+//
+// The environment's B = K b episodes are K contiguous groups of b; group k acts with weight set k and learns only from its own
+// episodes with its own ramp_ppo_config_t.  Every kernel here runs the statements of the single policy's kernel (the shared
+// *_body functions of ramp_policy.cu / ramp_policy_learn.cuh) on one set's slice, with the set taken from the launch:
+//
+//   ramp_pop_embed_grad_kernel   persistent CTAs over (set, job type) items, grid-strided past the resident CTAs: the MeanPool
+//                                rounds (forward: states kept, embeddings [K][n_models][out_node]) or their backward
+//   ramp_pop_head_kernel         blockIdx.y = set: the read-out of the set's episodes / rows, its weights staged per CTA
+//   ramp_pop_gae_kernel          one 1,024-thread CTA per group: GAE over the group's columns of the [T][B] trajectory, its live
+//                                rows t-major into the group's slice of the train batch, standardised with the group's mean / std
+//   ramp_pop_head_grad_kernel    one warp per (set, minibatch row): the rows of every group's minibatch in one launch
+//   ramp_pop_head_reduce_kernel  one thread per (set, read-out weight): the sum over the set's rows in row order
+//   ramp_pop_finish_kernel / ramp_pop_adam_kernel   blockIdx.y = set: the job types' sum, the norm partials, clip and Adam
+//   ramp_pop_learn_stats_kernel  one thread per set: the last pass's means and update_kl
+//
+// So group k computes what one policy with set k's weights computes on a b-episode environment with the same episode streams, bit
+// for bit: no float atomics, and every reduction in the single kernel's order.
+#pragma once
+
+namespace ramp {
+
+struct PopHead {
+    int32_t per;                          // episodes / rows of one set
+    int64_t n_weights;
+    const unsigned long long* seeds;      // [K] the sets' act seeds (sample), mixed with `mix` as ramp_policy_act mixes its call count
+    unsigned long long mix;
+};
+
+__global__ void __launch_bounds__(256, 3) ramp_pop_head_kernel(const PolicyDev P, const HeadArgs base, const PopHead ph) {
+    const int s = blockIdx.y;
+    const size_t o = (size_t)s * ph.per, A = P.c.n_actions;
+    HeadArgs a = base;
+    a.n = ph.per;
+    a.model += o; a.mask += o * A; a.actions += o;
+    if (a.obs_dyn) a.obs_dyn += o * 11;
+    if (a.graph_features) a.graph_features += o * P.c.in_features_graph;
+    if (a.done) a.done += o;
+    if (a.logits) a.logits += o * A;
+    if (a.value) a.value += o;
+    if (a.logp) a.logp += o;
+    a.emb += (size_t)s * P.c.n_models * P.c.out_features_node;
+    if (a.sample) a.seed = ph.seeds[s] ^ ph.mix;
+    head_body(P, P.w + (size_t)s * ph.n_weights, a, blockIdx.x, gridDim.x);
+}
+
+struct PopEmbed {
+    int32_t K;
+    int64_t n_weights;
+    int32_t rec_stride;                   // backward: floats per head record
+};
+
+// item = set n_models + job type; the forward's n_rows / emb and the backward's records and partials are the set's slices
+template <int MODE>
+__global__ void __launch_bounds__(256, 1) ramp_pop_embed_grad_kernel(const PolicyDev P, const ModelDev* models, const GradModelDev* gms,
+                                                                     const EmbGradArgs g, const PopEmbed pe) {
+    const int nm = P.c.n_models;
+    for (int item = blockIdx.x; item < pe.K * nm; item += gridDim.x) {
+        const int s = item / nm, m = item - s * nm;
+        EmbGradArgs e = g;
+        if (MODE == EMB_FORWARD) {
+            if (e.n_rows) e.n_rows += s;
+            if (e.emb) e.emb += (size_t)s * nm * P.c.out_features_node;
+        } else {
+            e.rec += (size_t)s * e.rows * pe.rec_stride;
+            e.row_model += (size_t)s * e.rows;
+            e.gpart += (size_t)s * nm * e.n_gnn;
+        }
+        embed_grad_body<MODE>(P, P.w + (size_t)s * pe.n_weights, models, gms + (size_t)s * nm, e, m);
+        __syncthreads();                  // the next item reuses the shared staging
+    }
+}
+
+__global__ void __launch_bounds__(1024) ramp_pop_gae_kernel(const GaeArgs* sets, int32_t ld) {
+    const GaeArgs a = sets[blockIdx.x];
+    gae_body(a, ld);
+}
+
+// sets[k]: group k's GradArgs for a minibatch starting at 0 (records, row model and statistics already at k mb); keys: the pass's [K]
+__global__ void __launch_bounds__(256) ramp_pop_head_grad_kernel(const PolicyDev P, const GradArgs* sets, int32_t K, int32_t mb, int32_t start,
+                                                                 const unsigned long long* keys, int32_t first_pass, int64_t n_weights) {
+    const int gi = blockIdx.x * LRN_WARPS + (threadIdx.x >> 5);
+    if (gi >= K * mb) return;
+    const int s = gi / mb;
+    GradArgs g = sets[s];
+    g.start = start; g.key = keys[s];
+    if (!first_pass) g.logp_old = nullptr;
+    head_grad_body(P, P.w + (size_t)s * n_weights, g, gi - s * mb);
+}
+
+// ramp_policy_head_reduce_kernel per set: segs hold set 0's records; set k's are k rec_shift floats further, its gradient and
+// weights k n_weights further
+__global__ void __launch_bounds__(256) ramp_pop_head_reduce_kernel(const PolicyDev P, const Seg* segs, int32_t n_segs, int64_t total, int32_t K,
+                                                                   int64_t rec_shift, int64_t n_weights, float* grad) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < K * total; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t s = e / total;
+        int si = 0;
+        int64_t off = e - s * total;
+        while (si + 1 < n_segs && off >= seg_size(segs[si])) { off -= seg_size(segs[si]); ++si; }
+        Seg sg = segs[si];
+        sg.rec += s * rec_shift;
+        grad[s * n_weights + sg.w + off] = seg_element(sg, off, P.w + s * n_weights);
+    }
+}
+
+__global__ void __launch_bounds__(256) ramp_pop_finish_kernel(const float* gpart, int32_t n_models, int64_t n_gnn, int64_t n_w, float* grad, double* norm_part) {
+    const size_t s = blockIdx.y;
+    grad_finish_body(gpart + s * n_models * n_gnn, n_models, n_gnn, n_w, grad + s * n_w, norm_part + s * LRN_GRID);
+}
+
+// sets[k]: group k's AdamArgs for minibatch 0 of a pass; minibatch j starts at `start` and writes its statistics j rows further
+__global__ void __launch_bounds__(256) ramp_pop_adam_kernel(const AdamArgs* sets, int32_t start, int32_t j, int32_t parity, int64_t n_w) {
+    AdamArgs a = sets[blockIdx.y];
+    a.start = start; a.parity = parity; a.stats += (size_t)j * RAMP_PPO_STATS_LEN;
+    adam_body(a, n_w);
+}
+
+// kl: [K][2] the sets' kl_coeff and kl_target
+__global__ void ramp_pop_learn_stats_kernel(const double* mb_stats, int32_t n_mb, int32_t n_mb_used, const float* kl, const int32_t* n_rows,
+                                            double* out, int32_t K) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= K) return;
+    learn_stats_body(mb_stats + (size_t)s * n_mb * RAMP_PPO_STATS_LEN, n_mb_used, kl[2 * s], kl[2 * s + 1], n_rows + s,
+                     out + (size_t)s * RAMP_PPO_STATS_LEN);
+}
+
+}  // namespace ramp
+
+struct ramp_population {
+    ramp_policy* p = nullptr;             // the template: configuration, job types, act outputs and trajectory (not owned)
+    int32_t K = 0;
+    int64_t nw = 0;
+    int32_t embed_ctas = 0;               // CTAs of the embedding launches: at most the resident ones
+    DeviceArray<float> d_w, d_emb;        // [K][n_weights], [K][n_models][out_node]
+    bool emb_valid = false;
+    unsigned long long act_calls = 0;
+    DeviceArray<unsigned long long> d_seeds, d_keys;
+    std::vector<DeviceArray<unsigned char>> gallocs;     // every (set, job type)'s MeanPool states and backward scratch
+    DeviceArray<GradModelDev> d_gms;      // [K][n_models]
+    bool gms_ready = false;
+    // the learner: per set what ramp_policy keeps for one, stacked set-major
+    bool learner_ready = false;
+    int32_t parity = 0, lcap = 0, bcap = 0, boot_cap = 0;
+    DeviceArray<float> l_grad, l_m, l_v, l_gpart, l_rec, l_row_stats, l_boot, d_kl;
+    DeviceArray<int32_t> l_step, l_n_rows, l_row_model, l_boot_act;
+    DeviceArray<double> l_norm_part, l_stats, l_mb_stats;
+    std::map<int32_t, ramp_policy::SegTable> seg_tables;
+    DeviceArray<float> b_obs, b_logp, b_logp_old, b_adv, b_vt, b_old, b_value, b_lpx;
+    DeviceArray<int32_t> b_model, b_action, b_actx; DeviceArray<uint8_t> b_mask; DeviceArray<double> b_adv64;
+    DeviceArray<GaeArgs> d_gae; DeviceArray<GradArgs> d_grad; DeviceArray<AdamArgs> d_adam;
+};
+
+namespace {
+
+int pop_check_set(const ramp_population* q, int32_t set) {
+    if (!q) return set_error(RAMP_ERR_BAD_ARG, "null population");
+    if (set < 0 || set >= q->K) return set_error(RAMP_ERR_BAD_ARG, "population: set %d outside [0, %d)", set, q->K);
+    return RAMP_OK;
+}
+
+// every (set, job type)'s forward states and backward scratch; the job types' out-edge CSR is the template's
+int pop_ensure_gms(ramp_population* q) {
+    if (q->gms_ready) return RAMP_OK;
+    ramp_policy* p = q->p;
+    const int nm = p->P.c.n_models;
+    std::vector<GradModelDev> h((size_t)q->K * nm);
+    q->gallocs.clear();
+    for (int m = 0; m < nm; ++m) {
+        const HostModel& hm = p->models[m];
+        if (!hm.set) return set_error(RAMP_ERR_BAD_ARG, "policy: model %d was never registered (ramp_policy_set_model)", m);
+        for (int s = 0; s < q->K; ++s) {
+            GradModelDev& g = h[(size_t)s * nm + m];
+            g = hm.g;
+            const int rc = alloc_grad_scratch(p->P.c, hm.d.n_nodes, hm.d.n_edges, q->gallocs, g);
+            if (rc != RAMP_OK) return rc;
+        }
+    }
+    CUDA_TRY(q->d_gms.alloc(h.size()));
+    CUDA_TRY(cudaMemcpy(q->d_gms.get(), h.data(), sizeof(GradModelDev) * h.size(), cudaMemcpyHostToDevice));
+    q->gms_ready = true;
+    return RAMP_OK;
+}
+
+int pop_launch_embed(ramp_population* q, cudaStream_t st, EmbGradArgs eg, bool forward) {
+    ramp_policy* p = q->p;
+    PopEmbed pe{};
+    pe.K = q->K; pe.n_weights = q->nw; pe.rec_stride = head_rec(p->P.c).stride;
+    PolicyDev P = p->P;
+    P.w = q->d_w.get();
+    if (forward) ramp_pop_embed_grad_kernel<EMB_FORWARD><<<q->embed_ctas, 256, 0, st>>>(P, p->d_models.get(), q->d_gms.get(), eg, pe);
+    else ramp_pop_embed_grad_kernel<EMB_BACKWARD><<<q->embed_ctas, 256, 0, st>>>(P, p->d_models.get(), q->d_gms.get(), eg, pe);
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
+}
+
+// the embeddings of every set at its current weights (the single policy's act re-embeds the same way when they are stale)
+int pop_embed(ramp_population* q, cudaStream_t st) {
+    int rc;
+    if ((rc = pop_ensure_gms(q)) != RAMP_OK) return rc;
+    EmbGradArgs eg{};
+    eg.emb = q->d_emb.get();
+    if ((rc = pop_launch_embed(q, st, eg, true)) != RAMP_OK) return rc;
+    q->emb_valid = true;
+    return RAMP_OK;
+}
+
+int pop_launch_head(ramp_population* q, const HeadArgs& a, int32_t per, const unsigned long long* seeds, unsigned long long mix, cudaStream_t st) {
+    ramp_policy* p = q->p;
+    const int wpc = 8;
+    int gx = (per + wpc - 1) / wpc;
+    const int cap = std::max(1, (2 * p->sm_count + q->K - 1) / q->K);      // about the single launch's 2 CTAs per SM in all
+    gx = std::max(1, std::min(gx, cap));
+    PolicyDev P = p->P;
+    P.w = q->d_w.get();
+    PopHead ph{};
+    ph.per = per; ph.n_weights = q->nw; ph.seeds = seeds; ph.mix = mix;
+    ramp_pop_head_kernel<<<dim3(gx, q->K), wpc * 32, p->head_smem, st>>>(P, a, ph);
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
+}
+
+int pop_ensure_learner(ramp_population* q) {
+    if (q->learner_ready) return RAMP_OK;
+    ramp_policy* p = q->p;
+    const size_t n = (size_t)q->K * q->nw, K = q->K;
+    CUDA_TRY(alloc_each(n, q->l_grad, q->l_m, q->l_v));
+    CUDA_TRY(q->l_gpart.alloc(K * p->P.c.n_models * gnn_weight_count(p)));
+    CUDA_TRY(q->l_step.alloc(2 * K));
+    CUDA_TRY(q->l_n_rows.alloc(K));
+    CUDA_TRY(q->l_norm_part.alloc(K * LRN_GRID));
+    CUDA_TRY(q->l_stats.alloc(K * RAMP_PPO_STATS_LEN));
+    CUDA_TRY(q->d_kl.alloc(2 * K));
+    CUDA_TRY(q->d_gae.alloc(K));
+    CUDA_TRY(q->d_grad.alloc(K));
+    CUDA_TRY(q->d_adam.alloc(K));
+    CUDA_TRY(cudaMemset(q->l_m.get(), 0, sizeof(float) * n));
+    CUDA_TRY(cudaMemset(q->l_v.get(), 0, sizeof(float) * n));
+    CUDA_TRY(cudaMemset(q->l_step.get(), 0, sizeof(int32_t) * 2 * K));
+    q->parity = 0;
+    q->learner_ready = true;
+    return RAMP_OK;
+}
+
+// per-row scratch for K minibatches of mb rows, and the head segments of set 0's mb records
+int pop_ensure_rows(ramp_population* q, int32_t mb, cudaStream_t st, const ramp_policy::SegTable** segs) {
+    const ramp_policy_config_t& c = q->p->P.c;
+    const size_t n = (size_t)q->K * mb;
+    if (mb > q->lcap) {
+        q->lcap = 0;
+        q->seg_tables.clear();
+        CUDA_TRY(q->l_rec.alloc(n * head_rec(c).stride));
+        CUDA_TRY(q->l_row_stats.alloc(n * RS_N));
+        CUDA_TRY(q->l_row_model.alloc(n));
+        q->lcap = mb;
+    }
+    auto it = q->seg_tables.find(mb);
+    if (it == q->seg_tables.end()) {
+        Seg s[HEAD_SEGS];
+        ramp_policy::SegTable t;
+        t.count = head_segs(q->p->P, q->l_rec.get(), mb, s);
+        for (int k = 0; k < t.count; ++k) t.total += seg_size(s[k]);
+        CUDA_TRY(t.d.alloc(HEAD_SEGS));
+        CUDA_TRY(cudaMemcpyAsync(t.d.get(), s, sizeof(s), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaStreamSynchronize(st));                              // `s` is pageable
+        it = q->seg_tables.emplace(mb, std::move(t)).first;
+    }
+    *segs = &it->second;
+    return RAMP_OK;
+}
+
+// the train batch for K groups of `rows` trajectory slots each
+int pop_ensure_batch(ramp_population* q, int32_t rows) {
+    if (rows <= q->bcap) return RAMP_OK;
+    const size_t n = (size_t)q->K * rows;
+    q->bcap = 0;
+    CUDA_TRY(alloc_each(n, q->b_logp, q->b_logp_old, q->b_adv, q->b_vt, q->b_value, q->b_lpx, q->b_model, q->b_action, q->b_actx, q->b_adv64));
+    CUDA_TRY(q->b_obs.alloc(n * 11));
+    CUDA_TRY(alloc_each(n * q->p->P.c.n_actions, q->b_mask, q->b_old));
+    q->bcap = rows;
+    return RAMP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int ramp_population_create(ramp_policy_t* p, int32_t n_sets, ramp_population_t** out) {
+    if (!p || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (n_sets < 1) return set_error(RAMP_ERR_BAD_ARG, "population: %d weight sets", n_sets);
+    if (!p->weights_set) return set_error(RAMP_ERR_BAD_ARG, "policy: no weights (ramp_policy_set_weights)");
+    CUDA_TRY(cudaSetDevice(p->device));
+    std::unique_ptr<ramp_population> q(new ramp_population());
+    q->p = p; q->K = n_sets; q->nw = p->n_weights;
+    const ramp_policy_config_t& c = p->P.c;
+    int per_sm = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ramp_pop_embed_grad_kernel<EMB_BACKWARD>, 256, 0));
+    q->embed_ctas = std::max(1, std::min(n_sets * c.n_models, std::max(1, per_sm) * p->sm_count));
+    CUDA_TRY(reserve_dynamic_smem((const void*)ramp_pop_head_kernel, p->head_smem));
+    CUDA_TRY(q->d_w.alloc((size_t)n_sets * q->nw));
+    CUDA_TRY(q->d_emb.alloc((size_t)n_sets * c.n_models * c.out_features_node));
+    CUDA_TRY(q->d_seeds.alloc(n_sets));
+    CUDA_TRY(cudaDeviceSynchronize());                                    // a running call may still update the template's weights
+    for (int s = 0; s < n_sets; ++s)
+        CUDA_TRY(cudaMemcpy(q->d_w.get() + (size_t)s * q->nw, p->d_w.get(), sizeof(float) * q->nw, cudaMemcpyDeviceToDevice));
+    *out = q.release();
+    return RAMP_OK;
+}
+
+void ramp_population_destroy(ramp_population_t* q) {
+    if (!q) return;
+    cudaSetDevice(q->p->device);
+    delete q;
+}
+
+int ramp_population_set_weights(ramp_population_t* q, int32_t set, const float* weights, int64_t n) {
+    int rc = pop_check_set(q, set);
+    if (rc != RAMP_OK) return rc;
+    if (!weights) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (n != q->nw) return set_error(RAMP_ERR_BAD_ARG, "population: %lld weights given for set %d, the configuration has %lld", (long long)n, set, (long long)q->nw);
+    CUDA_TRY(cudaSetDevice(q->p->device));
+    CUDA_TRY(cudaDeviceSynchronize());                                    // a running rollout may still read the old set
+    CUDA_TRY(cudaMemcpy(q->d_w.get() + (size_t)set * q->nw, weights, sizeof(float) * n, cudaMemcpyHostToDevice));
+    q->emb_valid = false;
+    return RAMP_OK;
+}
+
+int ramp_population_get_weights(ramp_population_t* q, int32_t set, float* out) {
+    int rc = pop_check_set(q, set);
+    if (rc != RAMP_OK) return rc;
+    if (!out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    CUDA_TRY(cudaSetDevice(q->p->device));
+    CUDA_TRY(cudaDeviceSynchronize());                                    // a learn call may still be updating them
+    CUDA_TRY(cudaMemcpy(out, q->d_w.get() + (size_t)set * q->nw, sizeof(float) * q->nw, cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
+int ramp_population_act(ramp_population_t* q, ramp_engine_t* eng, int32_t sample, const uint64_t* seeds) {
+    if (!q || !eng || (sample && !seeds)) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    ramp_policy* p = q->p;
+    ramp_env_buffers_t eb{};
+    int rc = ramp_env_buffers(eng, &eb);
+    if (rc != RAMP_OK) return rc;
+    const ramp_policy_config_t& c = p->P.c;
+    if (ramp_internal_device(eng) != p->device) return set_error(RAMP_ERR_BAD_ARG, "policy and engine live on different devices");
+    if (eb.n_actions != c.n_actions) return set_error(RAMP_ERR_BAD_ARG, "policy has %d actions, the environment %d", c.n_actions, eb.n_actions);
+    if (c.in_features_graph != 17) return set_error(RAMP_ERR_BAD_ARG, "the environment emits 17 graph features, the policy expects %d", c.in_features_graph);
+    if (eb.n_models > c.n_models) return set_error(RAMP_ERR_BAD_ARG, "the environment has %d job types, the policy %d", eb.n_models, c.n_models);
+    if (eb.n_episodes % q->K)
+        return set_error(RAMP_ERR_BAD_ARG, "population: %d episodes do not split into %d groups of equal size", eb.n_episodes, q->K);
+    CUDA_TRY(cudaSetDevice(p->device));
+    cudaStream_t st = ramp_internal_stream(eng);
+    int launches = 1;
+    if ((rc = fence_in(p, st)) != RAMP_OK) return rc;
+    if (!q->emb_valid) { if ((rc = pop_embed(q, st)) != RAMP_OK) return rc; ++launches; }
+    if ((rc = ensure_outputs(p, eb.n_episodes)) != RAMP_OK) return rc;
+    if (sample) CUDA_TRY(cudaMemcpyAsync(q->d_seeds.get(), seeds, sizeof(uint64_t) * q->K, cudaMemcpyHostToDevice, st));
+    HeadArgs a{};
+    a.obs_dyn = eb.obs_dynamic; a.graph_static = p->d_gstatic.get(); a.model = eb.queued_model; a.done = eb.done;
+    a.mask = eb.action_mask; a.emb = q->d_emb.get(); a.logits = p->d_logits.get(); a.value = p->d_value.get(); a.logp = p->d_logp.get(); a.actions = eb.actions;
+    a.sample = sample;
+    if ((rc = pop_launch_head(q, a, eb.n_episodes / q->K, q->d_seeds.get(), 0x9E3779B97F4A7C15ull * (++q->act_calls), st)) != RAMP_OK ||
+        (rc = fence_out(p, st)) != RAMP_OK)
+        return rc;
+    p->act_n = eb.n_episodes;                                             // ramp_policy_read and the trajectory take act's outputs
+    ramp_internal_count_launches(eng, launches);
+    return RAMP_OK;
+}
+
+int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_steps, const ramp_ppo_config_t* cfgs, double* stats_out) {
+    if (!q || !cfgs) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    ramp_policy* p = q->p;
+    const int32_t K = q->K;
+    for (int s = 0; s < K; ++s) {
+        int rc = check_learner_config(&cfgs[s]);
+        if (rc != RAMP_OK) return rc;
+        if (cfgs[s].sgd_minibatch_size != cfgs[0].sgd_minibatch_size)
+            return set_error(RAMP_ERR_BAD_ARG, "population: sgd_minibatch_size of set %d (%d) differs from set 0's (%d)", s,
+                             cfgs[s].sgd_minibatch_size, cfgs[0].sgd_minibatch_size);
+        if (cfgs[s].num_sgd_iter != cfgs[0].num_sgd_iter)
+            return set_error(RAMP_ERR_BAD_ARG, "population: num_sgd_iter of set %d (%d) differs from set 0's (%d)", s,
+                             cfgs[s].num_sgd_iter, cfgs[0].num_sgd_iter);
+    }
+    ramp_env_buffers_t eb{};
+    cudaStream_t st;
+    int rc = learn_begin(p, eng, cfgs, n_steps, "population", &eb, &st);
+    if (rc != RAMP_OK) return rc;
+    if (eb.n_episodes % K) return set_error(RAMP_ERR_BAD_ARG, "population: %d episodes do not split into %d groups of equal size", eb.n_episodes, K);
+    const ramp_policy_config_t& c = p->P.c;
+    const int32_t B = eb.n_episodes, b = B / K, rows = n_steps * b, mb = cfgs[0].sgd_minibatch_size, n_mb = (rows + mb - 1) / mb;
+    const int32_t n_pass = cfgs[0].num_sgd_iter, A = c.n_actions, on = c.out_features_node, nm = c.n_models;
+    const size_t R = rows;
+    const ramp_policy::SegTable* segs = nullptr;
+    if ((rc = fence_in(p, st)) || (rc = pop_ensure_learner(q)) || (rc = pop_ensure_gms(q)) || (rc = pop_ensure_rows(q, mb, st, &segs)) ||
+        (rc = pop_ensure_batch(q, rows)))
+        return rc;
+    if (!q->emb_valid && (rc = pop_embed(q, st)) != RAMP_OK) return rc;
+    if (B > q->boot_cap) {
+        q->boot_cap = 0;
+        CUDA_TRY(alloc_each(B, q->l_boot, q->l_boot_act));
+        q->boot_cap = B;
+    }
+    if ((size_t)K * n_mb * RAMP_PPO_STATS_LEN > q->l_mb_stats.size()) CUDA_TRY(q->l_mb_stats.alloc((size_t)K * n_mb * RAMP_PPO_STATS_LEN));
+    if ((size_t)K * std::max(n_pass, 1) > q->d_keys.size()) CUDA_TRY(q->d_keys.alloc((size_t)K * std::max(n_pass, 1)));
+    // every group's arguments: set s's slices of the trajectory's columns, the train batch, the scratch and the learner state
+    const HeadRec HR = head_rec(c);
+    std::vector<GaeArgs> gae(K);
+    std::vector<GradArgs> grad(K);
+    std::vector<AdamArgs> adam(K);
+    std::vector<float> kl(2 * K);
+    std::vector<unsigned long long> keys((size_t)K * std::max(n_pass, 1));
+    const float* boot = p->t_value.get() + (size_t)n_steps * B;
+    if (n_steps == p->traj_n) boot = q->l_boot.get();
+    for (int s = 0; s < K; ++s) {
+        const ramp_ppo_config_t& cfg = cfgs[s];
+        const size_t col = (size_t)s * b, r0 = (size_t)s * R, q0 = (size_t)s * mb;
+        GaeArgs& ge = gae[s];
+        ge.T = n_steps; ge.B = b; ge.A = A; ge.n_models = nm; ge.standardize = cfg.standardize_advantages;
+        ge.gamma = cfg.gamma; ge.lambda = cfg.lambda;
+        ge.t_obs = p->t_obs.get() + col * 11; ge.t_model = p->t_model.get() + col; ge.t_mask = p->t_mask.get() + col * A;
+        ge.t_action = p->t_action.get() + col; ge.t_logp = p->t_logp.get() + col; ge.t_value = p->t_value.get() + col;
+        ge.t_reward = p->t_reward.get() + col; ge.t_done = p->t_done.get() + col;
+        ge.boot = boot + col; ge.adv64 = q->b_adv64.get() + col;
+        ge.obs = q->b_obs.get() + r0 * 11; ge.model = q->b_model.get() + r0; ge.mask = q->b_mask.get() + r0 * A; ge.action = q->b_action.get() + r0;
+        ge.logp = q->b_logp.get() + r0; ge.adv = q->b_adv.get() + r0; ge.vt = q->b_vt.get() + r0; ge.n_rows = q->l_n_rows.get() + s;
+        GradArgs& ga = grad[s];
+        ga.mb = mb; ga.n_rows = q->l_n_rows.get() + s; ga.shuffle = 1; ga.obs_dyn = q->b_obs.get() + r0 * 11; ga.model = q->b_model.get() + r0;
+        ga.mask = q->b_mask.get() + r0 * A; ga.action = q->b_action.get() + r0; ga.old_logits = q->b_old.get() + r0 * A;
+        ga.adv = q->b_adv.get() + r0; ga.vt = q->b_vt.get() + r0; ga.graph_static = p->d_gstatic.get(); ga.emb = q->d_emb.get() + (size_t)s * nm * on;
+        ga.rec = q->l_rec.get() + q0 * HR.stride; ga.row_model = q->l_row_model.get() + q0; ga.row_stats = q->l_row_stats.get() + q0 * RS_N;
+        ga.logp_old = q->b_logp_old.get() + r0;
+        ppo_terms(ga, cfg);
+        AdamArgs& aa = adam[s];
+        aa = adam_args(p, cfg, q->l_n_rows.get() + s, mb);
+        aa.step = q->l_step.get() + 2 * s; aa.m = q->l_m.get() + (size_t)s * q->nw; aa.v = q->l_v.get() + (size_t)s * q->nw;
+        aa.grad = q->l_grad.get() + (size_t)s * q->nw; aa.norm_part = q->l_norm_part.get() + (size_t)s * LRN_GRID; aa.w = q->d_w.get() + (size_t)s * q->nw;
+        aa.row_stats = ga.row_stats; aa.vf_coeff = ga.vf_coeff; aa.ent_coeff = ga.ent_coeff; aa.kl_coeff = ga.kl_coeff;
+        aa.stats = q->l_mb_stats.get() + (size_t)s * n_mb * RAMP_PPO_STATS_LEN;
+        kl[2 * s] = (float)cfg.kl_coeff; kl[2 * s + 1] = (float)cfg.kl_target;
+        for (int pass = 0; pass < n_pass; ++pass) keys[(size_t)pass * K + s] = mix64(cfg.seed ^ mix64((uint64_t)pass + 1));
+    }
+    CUDA_TRY(cudaMemcpyAsync(q->d_gae.get(), gae.data(), sizeof(GaeArgs) * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(q->d_grad.get(), grad.data(), sizeof(GradArgs) * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(q->d_adam.get(), adam.data(), sizeof(AdamArgs) * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(q->d_kl.get(), kl.data(), sizeof(float) * 2 * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(q->d_keys.get(), keys.data(), sizeof(unsigned long long) * keys.size(), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));                                  // the vectors are pageable
+    PolicyDev P = p->P;
+    P.w = q->d_w.get();
+    int launches = 2;                                                     // GAE, old logits
+    // 1. the value of the state after the last step, as ramp_policy_learn takes it
+    if (n_steps == p->traj_n) {
+        HeadArgs hb{};
+        hb.obs_dyn = eb.obs_dynamic; hb.graph_static = p->d_gstatic.get(); hb.model = eb.queued_model; hb.done = eb.done;
+        hb.mask = eb.action_mask; hb.emb = q->d_emb.get(); hb.value = q->l_boot.get(); hb.actions = q->l_boot_act.get();
+        if ((rc = pop_launch_head(q, hb, b, nullptr, 0, st)) != RAMP_OK) return rc;
+        ++launches;
+    }
+    // 2. GAE, one CTA per group
+    ramp_pop_gae_kernel<<<K, 1024, 0, st>>>(q->d_gae.get(), B);
+    CUDA_TRY(cudaGetLastError());
+    // 3. the collection weights' logits of every row
+    HeadArgs ho{};
+    ho.obs_dyn = q->b_obs.get(); ho.graph_static = p->d_gstatic.get(); ho.model = q->b_model.get(); ho.mask = q->b_mask.get();
+    ho.emb = q->d_emb.get(); ho.logits = q->b_old.get(); ho.value = q->b_value.get(); ho.logp = q->b_lpx.get(); ho.actions = q->b_actx.get();
+    if ((rc = pop_launch_head(q, ho, rows, nullptr, 0, st)) != RAMP_OK) return rc;
+    // 4. minibatch j of every group in the same launches
+    int64_t rgrid = (K * segs->total + 255) / 256;
+    if (rgrid > 4 * p->sm_count) rgrid = 4 * p->sm_count;
+    for (int pass = 0; pass < n_pass; ++pass) {
+        for (int j = 0; j < n_mb; ++j) {
+            const int32_t start = j * mb;
+            EmbGradArgs ef{};
+            ef.n_rows = q->l_n_rows.get(); ef.start = start; ef.emb = pass || j ? q->d_emb.get() : nullptr;
+            if ((rc = pop_launch_embed(q, st, ef, true)) != RAMP_OK) return rc;
+            ramp_pop_head_grad_kernel<<<(K * mb + LRN_WARPS - 1) / LRN_WARPS, LRN_WARPS * 32, 0, st>>>(
+                P, q->d_grad.get(), K, mb, start, q->d_keys.get() + (size_t)pass * K, pass == 0, q->nw);
+            ramp_pop_head_reduce_kernel<<<(unsigned)rgrid, 256, 0, st>>>(P, segs->d.get(), segs->count, segs->total, K,
+                                                                         (int64_t)mb * HR.stride, q->nw, q->l_grad.get());
+            EmbGradArgs eb2{};
+            eb2.rec = q->l_rec.get(); eb2.row_model = q->l_row_model.get(); eb2.rows = mb; eb2.gpart = q->l_gpart.get(); eb2.n_gnn = gnn_weight_count(p);
+            if ((rc = pop_launch_embed(q, st, eb2, false)) != RAMP_OK) return rc;
+            ramp_pop_finish_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->l_gpart.get(), nm, gnn_weight_count(p), q->nw, q->l_grad.get(),
+                                                                      q->l_norm_part.get());
+            ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_adam.get(), start, j, q->parity, q->nw);
+            q->parity ^= 1;
+            CUDA_TRY(cudaGetLastError());
+            launches += 6;
+        }
+    }
+    if (n_pass > 0) q->emb_valid = false;
+    // 5. every set's last-pass statistics and adapted KL coefficient: the call's one read-back
+    ramp_pop_learn_stats_kernel<<<(K + 127) / 128, 128, 0, st>>>(q->l_mb_stats.get(), n_mb, n_pass > 0 ? n_mb : 0, q->d_kl.get(),
+                                                                q->l_n_rows.get(), q->l_stats.get(), K);
+    CUDA_TRY(cudaGetLastError());
+    ramp_internal_count_launches(eng, launches + 1);
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, q->l_stats.get(), sizeof(double) * K * RAMP_PPO_STATS_LEN, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return fence_out(p, st);
+}
+
+int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_avg_out, float* exp_avg_sq_out, int32_t* step_out) {
+    int rc = pop_check_set(q, set);
+    if (rc != RAMP_OK) return rc;
+    CUDA_TRY(cudaSetDevice(q->p->device));
+    const size_t n = q->nw;
+    if (!q->learner_ready) {
+        if (exp_avg_out) memset(exp_avg_out, 0, sizeof(float) * n);
+        if (exp_avg_sq_out) memset(exp_avg_sq_out, 0, sizeof(float) * n);
+        if (step_out) *step_out = 0;
+        return RAMP_OK;
+    }
+    CUDA_TRY(cudaDeviceSynchronize());                                    // a learn call may still be updating them
+    if (exp_avg_out) CUDA_TRY(cudaMemcpy(exp_avg_out, q->l_m.get() + (size_t)set * n, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    if (exp_avg_sq_out) CUDA_TRY(cudaMemcpy(exp_avg_sq_out, q->l_v.get() + (size_t)set * n, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    if (step_out) CUDA_TRY(cudaMemcpy(step_out, q->l_step.get() + 2 * set + q->parity, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
+int ramp_population_embed_ctas(ramp_population_t* q, int32_t* ctas_out) {
+    if (!q || !ctas_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    *ctas_out = q->embed_ctas;
+    return RAMP_OK;
+}
+
+}  // extern "C"

@@ -176,7 +176,9 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_es_round_end', 'ramp_es_step', 'ramp_es_update', 'ramp_es_read', 'ramp_es_act_read', 'ramp_es_state',
                     'ramp_es_reset', 'ramp_pg_loss_grad', 'ramp_policy_learn_pg',
                     'ramp_env_set_graph_static', 'ramp_env_ingest', 'ramp_env_export',
-                    'ramp_policy_set_weights_device', 'ramp_policy_forward_device', 'ramp_policy_backward_device']
+                    'ramp_policy_set_weights_device', 'ramp_policy_forward_device', 'ramp_policy_backward_device',
+                    'ramp_population_create', 'ramp_population_destroy', 'ramp_population_set_weights', 'ramp_population_get_weights',
+                    'ramp_population_act', 'ramp_population_learn', 'ramp_population_learner_state', 'ramp_population_embed_ctas']
 
 
 def device_bytes():

@@ -128,7 +128,9 @@ def _bind(L):
                        ('ramp_es_read', [C.c_void_p] * 12),
                        ('ramp_es_act_read', [C.c_void_p] * 5),
                        ('ramp_es_state', [C.c_void_p] * 4),
-                       ('ramp_es_reset', [C.c_void_p])):
+                       ('ramp_es_reset', [C.c_void_p]),
+                       ('ramp_population_learn', [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CConfig), C.c_void_p]),
+                       ('ramp_population_learner_state', [C.c_void_p, C.c_int32] + [C.c_void_p] * 3)):
         getattr(L, name).restype = C.c_int
         getattr(L, name).argtypes = args
     L.ramp_es_destroy.restype = None
@@ -221,6 +223,47 @@ class DevicePPOLearner(_GradientLearner):
                                                   gf.ctypes.data, mask.ctypes.data, act.ctypes.data, old.ctypes.data, adv.ctypes.data,
                                                   vt.ctypes.data, grad.ctypes.data, out.ctypes.data))
         return _stats(STATS, out), grad
+
+
+class DevicePopulationPPOLearner:
+    """DevicePPOLearner for every set of a DeviceGNNPolicyPopulation at once: group k of the environment learns only from its own
+    episodes with configs[k], and ends each call with the weights, Adam state, statistics and kl_coeff a DevicePPOLearner with
+    configs[k] would reach on a group-sized environment with the same episode streams, bit for bit.  Every minibatch step runs
+    all K sets in the same launches.  sgd_minibatch_size and num_sgd_iter set that launch loop, so the K configs must agree on them."""
+
+    def __init__(self, population, configs):
+        configs = [dataclasses.replace(c) for c in configs]
+        if len(configs) != population.K:
+            raise ValueError(f'{len(configs)} configs for a population of {population.K} sets')
+        for name in ('sgd_minibatch_size', 'num_sgd_iter'):
+            values = [getattr(c, name) for c in configs]
+            if len(set(values)) > 1:
+                raise ValueError(f'{name} must be the same for every set (it sets the launch loop): {values}')
+        self.population, self.configs = population, configs
+        self._calls = 0
+        self._L = population._L
+        _bind(self._L)
+
+    def learn(self, env, horizon: int):
+        """One PPO learner step per set on the first ``horizon`` steps of the population's last collect(env, ...): a list of K stats
+        dicts (STATS).  Set k's call c shuffles with configs[k].seed + c, and its kl_coeff is adapted as DevicePPOLearner's."""
+        pop = self.population
+        pop.group_size(env)
+        cfgs = (_CConfig * pop.K)(*[_c_struct(_CConfig, c, seed=c.seed + self._calls) for c in self.configs])
+        out = np.zeros((pop.K, len(STATS)), dtype=np.float64)
+        _engine._check(self._L.ramp_population_learn(pop._h, env.eng._h, int(horizon), cfgs, out.ctypes.data))
+        self._calls += 1
+        stats = [_stats(STATS, row) for row in out]
+        for c, s in zip(self.configs, stats):
+            c.kl_coeff = s['kl_coeff']
+        return stats
+
+    def adam_state(self, k: int):
+        """set k's torch.optim.Adam state: exp_avg, exp_avg_sq (blob order) and the step count"""
+        n = self._L.ramp_policy_weight_count(C.byref(self.population.template._cfg))
+        m, v, step = np.zeros(n, np.float32), np.zeros(n, np.float32), C.c_int32()
+        _engine._check(self._L.ramp_population_learner_state(self.population._h, int(k), m.ctypes.data, v.ctypes.data, C.byref(step)))
+        return m, v, step.value
 
 
 class DeviceIMPALALearner(_GradientLearner):

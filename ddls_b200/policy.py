@@ -355,12 +355,16 @@ class DeviceGNNPolicy:
         ``logp``, ``value``) and what came back (``reward``, ``done`` after the step); ``live`` marks the decisions of episodes that
         were not finished yet.  The arrays are views of page-locked buffers owned by the policy: valid until the next ``collect()`` /
         ``close()`` -- copy what must outlive that."""
+        return self._collect(env, horizon, lambda t: self.act(env, sample=sample, seed=seed + t), reset)
+
+    def _collect(self, env, horizon: int, act, reset: bool):
+        """collect() with act(t) deciding env-step t (this policy's act, or a population's that writes this policy's act outputs)"""
         L, h = self._L, self._h
         if reset:
             env.reset()
         _engine._check(L.ramp_policy_trajectory_begin(h, env.eng._h, int(horizon)))
         for t in range(horizon):
-            self.act(env, sample=sample, seed=seed + t)
+            act(t)
             _engine._check(L.ramp_policy_trajectory_record(h, env.eng._h, t, 0))
             env.step_device()
             _engine._check(L.ramp_policy_trajectory_record(h, env.eng._h, t, 1))
@@ -373,3 +377,143 @@ class DeviceGNNPolicy:
         out['done'] = buf['done'].astype(bool)
         out['live'] = np.concatenate([np.ones((1, B), dtype=bool), ~out['done'][:-1]], axis=0) & (out['model'] >= 0)
         return out
+
+
+GOLDEN = 0x9E3779B97F4A7C15            # ramp_policy_act mixes seed ^ GOLDEN * (its call count)
+ROW_MIX = 0xD1342543DE82EF95           # ... then the episode index: splitmix64(seed ^ ROW_MIX * b)
+_M64 = 2 ** 64 - 1
+
+
+def splitmix64(x: int) -> int:
+    x = (x + GOLDEN) & _M64
+    x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & _M64
+    return x ^ (x >> 31)
+
+
+def act_draw_key(seed: int, calls: int, b: int) -> int:
+    """the 64-bit draw of episode b in a policy's act call number `calls` (from 1) made with `seed` (ramp_policy_head_kernel)"""
+    return splitmix64((seed ^ (GOLDEN * calls)) & _M64 ^ ((b * ROW_MIX) & _M64))
+
+
+def population_draw(seeds: Sequence[int], calls: int, b: int, group_size: int):
+    """(group k, local index i, draw) of episode b of a population's act call number `calls`: group k's seed, the population's call
+    count and i = b - k group_size -- the draw of episode i of a single policy whose act got seeds[k] on a group_size-episode twin"""
+    k = b // group_size
+    i = b - k * group_size
+    return k, i, act_draw_key(int(seeds[k]) & _M64, calls, i)
+
+
+def _bind_population(L):
+    if getattr(L, '_population_bound', False):
+        return
+    for name, args in (('ramp_population_create', [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]),
+                       ('ramp_population_set_weights', [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]),
+                       ('ramp_population_get_weights', [C.c_void_p, C.c_int32, C.c_void_p]),
+                       ('ramp_population_act', [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+                       ('ramp_population_embed_ctas', [C.c_void_p, C.c_void_p])):
+        getattr(L, name).restype = C.c_int
+        getattr(L, name).argtypes = args
+    L.ramp_population_destroy.restype = None
+    L.ramp_population_destroy.argtypes = [C.c_void_p]
+    L._population_bound = True
+
+
+class DeviceGNNPolicyPopulation:
+    """K weight sets of one configuration acting on one DeviceRampJobPartitioningEnvironment: its B = K b episodes are K contiguous
+    groups of b, group k decided by set k.  Group k's decisions are, bit for bit, those a DeviceGNNPolicy holding set k's weights
+    makes on a b-episode environment with the same episode streams (include/ramp_b200.h: ramp_population_*).
+    DevicePopulationPPOLearner trains the K sets, each with its own PPOConfig."""
+
+    def __init__(self, graphs, n_actions: int, config: Optional[Dict] = None, state_dicts: Sequence = (), device: int = 0):
+        """graphs, n_actions, config: as DeviceGNNPolicy's; state_dicts: one GNNPolicy state_dict (or blob) per set, K = their number."""
+        state_dicts = list(state_dicts)
+        if not state_dicts:
+            raise ValueError('a population needs at least one state_dict')
+        cfg = dict(DEFAULT_CONFIG)
+        cfg.update(config or {})
+        blobs = []
+        for k, sd in enumerate(state_dicts):          # every set's shapes are checked before anything is allocated
+            try:
+                blob = sd if isinstance(sd, np.ndarray) else pack_weights(sd, cfg, int(n_actions))
+            except (KeyError, ValueError) as e:
+                raise ValueError(f'state_dicts[{k}]: {e}') from None
+            blob = np.ascontiguousarray(blob, dtype=np.float32)
+            n = sum(int(np.prod(v)) for v in weight_shapes(cfg, int(n_actions)).values())
+            if blob.shape != (n,):
+                raise ValueError(f'state_dicts[{k}]: a blob of shape {blob.shape}, the configuration has {n} weights')
+            blobs.append(blob)
+        self.K, self.graphs, self.device = len(blobs), list(graphs), device
+        self.template = DeviceGNNPolicy(graphs, n_actions, cfg, state_dict=blobs[0], device=device)
+        self.config, self.n_actions, self.n_models = self.template.config, self.template.n_actions, self.template.n_models
+        self._L = self.template._L
+        _bind_population(self._L)
+        self._h = C.c_void_p()
+        _engine._check(self._L.ramp_population_create(self.template._h, self.K, C.byref(self._h)))
+        for k, blob in enumerate(blobs[1:], 1):
+            self.set_weights(k, blob)
+
+    def close(self):
+        if getattr(self, '_h', None):
+            self._L.ramp_population_destroy(self._h)
+            self._h = None
+        if getattr(self, 'template', None) is not None:
+            self.template.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_weights(self, k: int, state_dict):
+        blob = state_dict if isinstance(state_dict, np.ndarray) else pack_weights(state_dict, self.config, self.n_actions)
+        blob = np.ascontiguousarray(blob, dtype=np.float32)
+        _engine._check(self._L.ramp_population_set_weights(self._h, int(k), blob.ctypes.data, len(blob)))
+
+    def get_weights(self, k: int) -> np.ndarray:
+        out = np.zeros(self._L.ramp_policy_weight_count(C.byref(self.template._cfg)), dtype=np.float32)
+        _engine._check(self._L.ramp_population_get_weights(self._h, int(k), out.ctypes.data))
+        return out
+
+    def gnn_state_dict(self, k: int) -> Dict[str, np.ndarray]:
+        """set k's weights under the reference's GNNPolicy key names and shapes"""
+        return unpack_weights(self.get_weights(k), self.config, self.n_actions)
+
+    def policy(self, k: int) -> DeviceGNNPolicy:
+        """a standalone DeviceGNNPolicy holding set k's current weights (e.g. for agents.evaluate)"""
+        return DeviceGNNPolicy(self.graphs, self.n_actions, self.config, state_dict=self.get_weights(k), device=self.device)
+
+    def group_size(self, env) -> int:
+        """b, the episodes of one group; ValueError unless K divides the environment's B"""
+        if env.B % self.K:
+            raise ValueError(f'{env.B} episodes do not split into {self.K} groups of equal size')
+        return env.B // self.K
+
+    def _seeds(self, seed) -> np.ndarray:
+        seeds = [seed] * self.K if np.isscalar(seed) else list(seed)
+        if len(seeds) != self.K:
+            raise ValueError(f'{len(seeds)} seeds for {self.K} sets')
+        return np.array([int(s) & _M64 for s in seeds], dtype=np.uint64)
+
+    def act(self, env, sample: bool = False, seed=0):
+        """one decision per episode, group k by set k; seed: group k's act seed, one for all or a sequence of K"""
+        self.group_size(env)
+        seeds = self._seeds(seed)
+        _engine._check(self._L.ramp_population_act(self._h, env.eng._h, 1 if sample else 0, seeds.ctypes.data))
+
+    def collect(self, env, horizon: int, sample: bool = True, seed=0, reset: bool = True):
+        """DeviceGNNPolicy.collect for every group at once: env-step t acts with seeds seed_k + t; arrays [horizon, B, ...], group k
+        in columns k b .. (k + 1) b - 1"""
+        self.group_size(env)
+        seeds = self._seeds(seed)
+        return self.template._collect(env, horizon, lambda t: self.act(env, sample=sample, seed=[int(s) + t for s in seeds]), reset)
+
+    def read(self, env):
+        return self.template.read(env)
+
+    def embed_ctas(self) -> int:
+        """CTAs of the MeanPool launches; each runs the (set, job type) items c, c + ctas, ..."""
+        n = C.c_int32()
+        _engine._check(self._L.ramp_population_embed_ctas(self._h, C.byref(n)))
+        return n.value

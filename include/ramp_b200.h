@@ -884,6 +884,32 @@ int ramp_es_act_read(ramp_es_t* es, ramp_engine_t* eng, float* logits_out, float
 int ramp_es_state(ramp_es_t* es, float* m_out, float* v_out, int32_t* t_out);
 int ramp_es_reset(ramp_es_t* es);
 
+/* ---- A population of K independent PPO trainings in one environment batch.  The environment's B = K b episodes are K contiguous
+ * groups of b; group k acts with weight set k and learns only from its own episodes with its own ramp_ppo_config_t.  Group k
+ * computes, bit for bit, what one policy holding set k's weights (ramp_policy_act, ramp_policy_learn with config k) computes on a
+ * b-episode environment with the same episode streams.  The kernels run every group in the same launches: the MeanPool rounds
+ * and their backward on one CTA per (set, job type) item, grid-strided past the resident CTAs; no float atomics. */
+typedef struct ramp_population ramp_population_t;
+/* K = n_sets weight sets with p's configuration and job types, each a copy of p's current weights, and K Adam states at zero.  p
+ * stays the population's template: its job types must not change, and it must outlive the population.  The population's act
+ * writes p's act outputs, so ramp_policy_read and ramp_policy_trajectory_* on p record the population's decisions. */
+int ramp_population_create(ramp_policy_t* p, int32_t n_sets, ramp_population_t** out);
+void ramp_population_destroy(ramp_population_t* q);
+/* set k's weights from / to a HOST blob of ramp_policy_weight_count floats */
+int ramp_population_set_weights(ramp_population_t* q, int32_t set, const float* weights, int64_t n);
+int ramp_population_get_weights(ramp_population_t* q, int32_t set, float* out);
+/* ramp_policy_act for every group: episode k b + i draws as episode i of a policy whose ramp_policy_act got seeds[k] (HOST,
+ * [n_sets]; may be NULL when sample is 0) with the population's call count.  RAMP_ERR_BAD_ARG unless n_sets divides B. */
+int ramp_population_act(ramp_population_t* q, ramp_engine_t* eng, int32_t sample, const uint64_t* seeds);
+/* ramp_policy_learn for every group on its columns of the template's trajectory, with cfgs[k] (HOST, [n_sets]); every config must
+ * have the same sgd_minibatch_size and num_sgd_iter.  stats_out: [n_sets][RAMP_PPO_STATS_LEN] or NULL. */
+int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_steps, const ramp_ppo_config_t* cfgs, double* stats_out);
+/* HOST copies of set k's Adam state, as ramp_policy_learner_state */
+int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_avg_out, float* exp_avg_sq_out, int32_t* step_out);
+/* the CTAs of the population's MeanPool launches: n_sets n_models items, at most the resident CTAs, each CTA runs items
+ * c, c + ctas, ... */
+int ramp_population_embed_ctas(ramp_population_t* q, int32_t* ctas_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,0 +1,116 @@
+"""K PPO trainings in one batch on a config-3-like environment (64 workers, ResNet-50): learn-call and minibatch-step time of
+DevicePopulationPPOLearner against K sequential DevicePPOLearner calls, and every set's mean return per iteration.
+
+    python scripts/population_train.py --out profiles/h100_population_ppo_train.jsonl
+
+Timing rows ('kind': 'timing'): for each K, one collect on a K b-episode environment (b episodes per group) with ppo.yaml's
+settings except num_sgd_iter, then learn calls timed with a device synchronise around each, alternating with the single
+learner's call on a b-episode environment; the single call is timed once per repeat and multiplied by K (the K sequential calls
+would do the same work K times).  minibatch_step_ms is the call's time over its minibatch steps (num_sgd_iter x minibatches).
+Each measurement repeats `--repeats` times.  Return rows ('kind': 'returns'): a grid over lr x entropy_coeff, --iters iterations
+of collect + learn, each set's mean episode return (the group's summed rewards over its episodes).  The first row names the card,
+its power limit and max SM clock, read in the same process."""
+import argparse
+import dataclasses
+import json
+import os
+import subprocess
+import sys
+import time
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def card():
+    try:
+        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
+                           text=True).stdout.strip().splitlines()[0].split(', ')
+        return {'gpu': q[0], 'power_limit': q[1], 'max_sm_clock': q[2]}
+    except Exception as e:                                       # noqa: BLE001 -- recorded, not hidden
+        return {'gpu': f'unknown ({e})'}
+
+
+def env_of(graphs, B, J, seed):
+    from ddls_b200.batched import DeviceRampJobPartitioningEnvironment
+    return DeviceRampJobPartitioningEnvironment((4, 4, 4), graphs, n_episodes=B, jobs_per_episode=J, seed=seed)
+
+
+def timed(fn, sync):
+    sync()
+    t0 = time.perf_counter()
+    out = fn()
+    sync()
+    return time.perf_counter() - t0, out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--ks', default='1,8,32,128')
+    ap.add_argument('--b', type=int, default=128, help='episodes per group')
+    ap.add_argument('--horizon', type=int, default=4)
+    ap.add_argument('--jobs', type=int, default=4)
+    ap.add_argument('--num-sgd-iter', type=int, default=1, help='ppo.yaml has 50; the timed calls run this many passes')
+    ap.add_argument('--repeats', type=int, default=3)
+    ap.add_argument('--grid-k', type=int, default=8)
+    ap.add_argument('--iters', type=int, default=5)
+    ap.add_argument('--out', default='profiles/h100_population_ppo_train.jsonl')
+    a = ap.parse_args()
+    import torch
+    from ddls_b200 import policy as P, workload
+    from ddls_b200.learn import DevicePopulationPPOLearner, DevicePPOLearner, PPOConfig
+    if not torch.cuda.is_available():
+        raise SystemExit('population_train.py measures on the GPU; no CUDA device is visible')
+    sync = torch.cuda.synchronize
+    graphs = [workload.make_graph('resnet')]
+    A = 17
+    cfg0 = P.algo_model_config('ppo', A)
+    base = PPOConfig(num_sgd_iter=a.num_sgd_iter)
+    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+    out = open(a.out, 'w')
+
+    def emit(row):                                               # written as measured: a cut-short run keeps what it measured
+        print(json.dumps(row), flush=True)
+        out.write(json.dumps(row) + '\n')
+        out.flush()
+
+    emit(dict(kind='card', **card(), b=a.b, horizon=a.horizon, jobs=a.jobs, num_sgd_iter=a.num_sgd_iter,
+              sgd_minibatch_size=base.sgd_minibatch_size))
+    # the single learner on a b-episode environment
+    senv = env_of(graphs, a.b, a.jobs, seed=1)
+    spol = P.DeviceGNNPolicy(graphs, A, cfg0, P.random_state_dict(cfg0, A, seed=0))
+    slrn = DevicePPOLearner(spol, base)
+    spol.collect(senv, a.horizon, seed=0)
+    slrn.learn(senv, a.horizon)                                  # warm-up
+    for K in [int(k) for k in a.ks.split(',')]:
+        env = env_of(graphs, K * a.b, a.jobs, seed=1)
+        pop = P.DeviceGNNPolicyPopulation(graphs, A, cfg0, [P.random_state_dict(cfg0, A, seed=k) for k in range(K)])
+        lrn = DevicePopulationPPOLearner(pop, [dataclasses.replace(base, seed=k) for k in range(K)])
+        pop.collect(env, a.horizon, seed=list(range(K)))
+        lrn.learn(env, a.horizon)                                # warm-up: every buffer and launch shape
+        for r in range(a.repeats):
+            tp, stats = timed(lambda: lrn.learn(env, a.horizon), sync)
+            ts, _ = timed(lambda: slrn.learn(senv, a.horizon), sync)
+            n_mb = -(-(a.horizon * a.b) // base.sgd_minibatch_size) * a.num_sgd_iter
+            emit(dict(kind='timing', K=K, repeat=r, population_learn_s=tp, population_minibatch_step_ms=1e3 * tp / n_mb,
+                      single_learn_s=ts, single_x_K_learn_s=ts * K, single_minibatch_step_ms=1e3 * ts / n_mb,
+                      embed_ctas=pop.embed_ctas(), train_rows=[int(s['rows']) for s in stats][:4]))
+        pop.close()
+        del env
+    # returns: a grid over lr x entropy_coeff
+    lrs, ents = [1e-4, 3e-4, 1e-3, 3e-3], [0.0, 0.01]
+    grid = [(lr, e) for lr in lrs for e in ents][:a.grid_k]
+    K = len(grid)
+    env = env_of(graphs, K * a.b, a.jobs, seed=2)
+    pop = P.DeviceGNNPolicyPopulation(graphs, A, cfg0, [P.random_state_dict(cfg0, A, seed=0)] * K)
+    lrn = DevicePopulationPPOLearner(pop, [dataclasses.replace(base, lr=lr, entropy_coeff=e, seed=k) for k, (lr, e) in enumerate(grid)])
+    for it in range(a.iters):
+        traj = pop.collect(env, a.jobs, seed=[100 * it + k for k in range(K)])
+        ret = (traj['reward'] * traj['live']).sum(axis=0).reshape(K, a.b).mean(axis=1)
+        lrn.learn(env, a.jobs)
+        emit(dict(kind='returns', iteration=it, sets=[dict(lr=lr, entropy_coeff=e, mean_return=float(x)) for (lr, e), x in zip(grid, ret)]))
+    pop.close()
+    out.close()
+
+
+if __name__ == '__main__':
+    main()
