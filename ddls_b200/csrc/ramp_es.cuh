@@ -1,13 +1,13 @@
 // ramp_es.cuh -- RLlib's evolution strategies training step on the device (include/ramp_b200.h: ramp_es_*; ray/rllib/algorithms/es:
 // es.py training_step, utils.py, optimizers.py).  Included at the end of ramp_policy.cu: the population runs the policy's forward
-// with a weight set per episode, in the same arithmetic order as ramp_gnn_embed_kernel and ramp_policy_head_kernel.
+// bodies (gnn_embed_body, head_row) with a weight set per episode.
 //
 //   ramp_es_perturb_kernel   the population's weight sets: set 2i = fl(theta + fl(sigma eps_i)), set 2i+1 = fl(theta - fl(sigma
 //                            eps_i)), set 2N = theta
-//   ramp_es_embed_kernel     es_embed_one for every (set, job type): persistent CTAs, each with its own scratch, so the scratch
+//   ramp_es_embed_kernel     gnn_embed_body for every (set, job type): persistent CTAs, each with its own scratch, so the scratch
 //                            scales with the grid, not with the population
-//   ramp_es_head_kernel      ramp_policy_head_kernel's read-out and categorical draw, one warp per episode, reading its set's
-//                            read-out weights from global memory (no value branch: ES does not use it)
+//   ramp_es_head_kernel      head_row with sample = 1, one warp per episode, reading its set's read-out weights from global memory
+//                            (no value: ES does not use it)
 //   ramp_es_collect_kernel   each episode's return (float of the f64 sum) and env-step count
 //   ramp_es_rank_kernel      compute_centered_ranks, one thread per value; ties go to index order (a stable argsort)
 //   ramp_es_update_kernel    g = sum_i (rank+_i - rank-_i) eps_i / 2N per weight (f64 in pair order), optimizers.Adam on
@@ -35,94 +35,6 @@ __global__ void ramp_es_perturb_kernel(const float* theta, const float* noise, c
     }
 }
 
-// ramp_gnn_embed_kernel's statements for one job type with the weight blob `w`, by the whole CTA, into emb_out[out_node]; M's z0 / z1 /
-// hn / he are the scratch.  A copy rather than a function the two kernels share, so that ramp_gnn_embed_kernel's code stays as it was
-__device__ __forceinline__ void es_embed_one(const PolicyDev& P, const float* w, const ModelDev& M, float* emb_out) {
-    __shared__ float sbuf[8][POL_MAX_DIM];
-    if (M.n_nodes <= 0) return;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
-    float* buf = sbuf[warp];
-    const int half = P.c.out_features_msg / 2, msg = P.c.out_features_msg, akind = P.c.aggregator_activation;
-    const float* zin = M.nf;
-    int zin_stride = P.c.in_features_node;
-    float* zout = M.z0;
-    for (int r = 0; r < P.c.num_rounds; ++r) {
-        const RoundW R = P.rounds[r];
-        // ---- node module on every node, edge module on every edge (mean_pool.py:120-127) ----
-        for (int v = warp; v < M.n_nodes; v += n_warps) {
-            for (int k = lane; k < R.in; k += 32) buf[k] = zin[(size_t)v * zin_stride + k];
-            __syncwarp();
-            warp_layer_norm(buf, R.in, w + R.nln_w, w + R.nln_b, lane);
-            for (int o = lane; o < half; o += 32) {
-                float a = w[R.nb + o];
-                const float* row = w + R.nW + (size_t)o * R.in;
-                for (int k = 0; k < R.in; ++k) a += row[k] * buf[k];
-                M.hn[(size_t)v * half + o] = act_fn(a, akind);
-            }
-            __syncwarp();
-        }
-        const int ine = P.c.in_features_edge;
-        for (int e = warp; e < M.n_edges; e += n_warps) {
-            for (int k = lane; k < ine; k += 32) buf[k] = M.ef[(size_t)e * ine + k];
-            __syncwarp();
-            warp_layer_norm(buf, ine, w + R.eln_w, w + R.eln_b, lane);
-            for (int o = lane; o < half; o += 32) {
-                float a = w[R.eb + o];
-                const float* row = w + R.eW + (size_t)o * ine;
-                for (int k = 0; k < ine; ++k) a += row[k] * buf[k];
-                M.he[(size_t)e * half + o] = act_fn(a, akind);
-            }
-            __syncwarp();
-        }
-        __syncthreads();
-        // ---- per destination node: mean of reduce_module over [own state, messages] (mean_pool.py:129-150) ----
-        for (int v = warp; v < M.n_nodes; v += n_warps) {
-            const int e0 = M.in_ptr[v], e1 = M.in_ptr[v + 1];
-            float acc[POL_MAX_DIM / 32];
-#pragma unroll
-            for (int i = 0; i < POL_MAX_DIM / 32; ++i) acc[i] = 0.f;
-            if (e1 > e0) {                                          // DGL leaves zero-in-degree nodes at zero
-                for (int mi = -1; mi < e1 - e0; ++mi) {
-                    const int src = mi < 0 ? v : M.in_src[e0 + mi];
-                    for (int k = lane; k < half; k += 32) {
-                        buf[k] = M.hn[(size_t)src * half + k];
-                        buf[half + k] = mi < 0 ? 0.f : M.he[(size_t)M.in_edge[e0 + mi] * half + k];
-                    }
-                    __syncwarp();
-                    warp_layer_norm(buf, msg, w + R.rln_w, w + R.rln_b, lane);
-#pragma unroll
-                    for (int i = 0; i < POL_MAX_DIM / 32; ++i) {
-                        const int o = lane + 32 * i;
-                        if (o < R.out) {
-                            float a = w[R.rb + o];
-                            const float* row = w + R.rW + (size_t)o * msg;
-                            for (int k = 0; k < msg; ++k) a += row[k] * buf[k];
-                            acc[i] += act_fn(a, akind);
-                        }
-                    }
-                    __syncwarp();
-                }
-            }
-            const float inv = 1.0f / (float)(e1 - e0 + 1);
-#pragma unroll
-            for (int i = 0; i < POL_MAX_DIM / 32; ++i) {
-                const int o = lane + 32 * i;
-                if (o < R.out) zout[(size_t)v * POL_MAX_DIM + o] = acc[i] * inv;
-            }
-        }
-        __syncthreads();
-        zin = zout; zin_stride = POL_MAX_DIM;
-        zout = (zout == M.z0) ? M.z1 : M.z0;
-    }
-    // ---- mean over the job's nodes (gnn_policy.py:262-268) ----
-    const int od = P.c.out_features_node;
-    for (int o = threadIdx.x; o < od; o += blockDim.x) {
-        float s = 0.f;
-        for (int v = 0; v < M.n_nodes; ++v) s += zin[(size_t)v * POL_MAX_DIM + o];
-        emb_out[o] = s / (float)M.n_nodes;
-    }
-}
-
 struct EsEmbedArgs {
     int32_t n_sets, n_models;
     int64_t n_weights;
@@ -143,99 +55,25 @@ __global__ void __launch_bounds__(256) ramp_es_embed_kernel(const PolicyDev P, c
         const int s = item / a.n_models, m = item - s * a.n_models;
         ModelDev M = models[m];
         M.z0 = z0; M.z1 = z1; M.hn = hn; M.he = he;
-        es_embed_one(P, a.sets + (size_t)s * a.n_weights, M, a.emb + (size_t)item * P.c.out_features_node);
+        gnn_embed_body(P, a.sets + (size_t)s * a.n_weights, M, a.emb + (size_t)item * P.c.out_features_node);
         __syncthreads();                  // the next item reuses the scratch
     }
 }
 
 struct EsHeadArgs {
-    int32_t n, n_pairs;                   // episodes; episode b < 2 n_pairs runs set b, the others set 2 n_pairs
+    int32_t n_pairs;                      // episode b < 2 n_pairs runs set b, the others set 2 n_pairs
     int64_t n_weights;
-    const float* sets; const float* emb;  // [sets][n_weights], [sets][n_models][out_node]
-    const float* obs_dyn; const float* graph_static; const int32_t* model; const uint8_t* done; const uint8_t* mask;
-    float* logits; float* logp; int32_t* actions;
-    unsigned long long seed;
+    const float* sets;                    // [sets][n_weights]; HeadArgs::emb is [sets][n_models][out_node]
 };
 
-// ramp_policy_head_kernel with sample = 1, statement for statement, the weights read from the episode's set
-__global__ void __launch_bounds__(256) ramp_es_head_kernel(const PolicyDev P, const EsHeadArgs a) {
+// head_row on each episode with its set's weights read from global memory; the act has no value
+__global__ void __launch_bounds__(256) ramp_es_head_kernel(const PolicyDev P, const HeadArgs a, const EsHeadArgs e) {
     __shared__ float s_warp[8][2 * POL_MAX_DIM];
-    const ramp_policy_config_t& c = P.c;
-    const int gin = c.in_features_graph + c.n_actions, og = c.out_features_graph, on = c.out_features_node, fin = on + og;
-    const int H = c.fcnet_hidden, A = c.n_actions;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpc = blockDim.x >> 5;
-    const int hpl = (H - lane + 31) / 32;                               // this lane's hidden units lane + 32 i < H
-    float* xb = s_warp[warp];
-    float* fb = xb + POL_MAX_DIM;
     for (int b = blockIdx.x * wpc + warp; b < a.n; b += gridDim.x * wpc) {
-        const int m = a.model[b];
-        const bool live = m >= 0 && m < c.n_models && !a.done[b];
-        if (!live) {
-            if (lane < A) a.logits[(size_t)b * A + lane] = 0.f;
-            if (lane == 0) { a.actions[b] = 0; a.logp[b] = 0.f; }
-            continue;
-        }
-        const int s = b < 2 * a.n_pairs ? b : 2 * a.n_pairs;
-        const float* w = a.sets + (size_t)s * a.n_weights;
-        for (int k = lane; k < gin; k += 32) {
-            float x;
-            if (k >= c.in_features_graph) x = a.mask[(size_t)b * A + (k - c.in_features_graph)] ? 1.f : 0.f;
-            else if (k < 9) x = a.obs_dyn[(size_t)b * 11 + k];
-            else if (k < 15) x = a.graph_static[(size_t)m * 6 + (k - 9)];
-            else x = a.obs_dyn[(size_t)b * 11 + (k - 6)];
-            xb[k] = x;
-        }
-        __syncwarp();
-        warp_layer_norm(xb, gin, w + P.gln_w, w + P.gln_b, lane);
-        const float* emb = a.emb + ((size_t)s * c.n_models + m) * on;
-        for (int k = lane; k < on; k += 32) fb[k] = emb[k];
-        if (lane < og) {
-            float g = w[P.gb + lane];
-            const float* row = w + P.gW + (size_t)lane * gin;
-            for (int k = 0; k < gin; ++k) g += row[k] * xb[k];
-            fb[on + lane] = g;
-        }
-        __syncwarp();
-        float h[POL_MAX_HPL];
-#pragma unroll
-        for (int i = 0; i < POL_MAX_HPL; ++i) {
-            const int j = lane + 32 * i;
-            if (i < hpl) {
-                float p = w[P.hb + j];
-                const float* row = w + P.hW + (size_t)j * fin;           // blob is [H][fin]
-                for (int k = 0; k < fin; ++k) p += row[k] * fb[k];
-                h[i] = act_fn(p, c.fcnet_activation);
-            }
-        }
-        float my_logit = -FLT_MAX;
-        for (int o = 0; o < A; ++o) {
-            float p = 0.f;
-#pragma unroll
-            for (int i = 0; i < POL_MAX_HPL; ++i) if (i < hpl) p += h[i] * w[P.lW + (size_t)o * H + lane + 32 * i];
-            p = warp_sum(p) + w[P.lb + o];
-            if (c.apply_action_mask && !a.mask[(size_t)b * A + o]) p += -FLT_MAX;
-            if (lane == o) my_logit = p;
-        }
-        float best = my_logit; int arg = lane < A ? lane : 0x7fffffff;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oa = __shfl_xor_sync(0xffffffffu, arg, o);
-            if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
-        }
-        const float ex = lane < A ? expf(my_logit - best) : 0.f;
-        const float denom = warp_sum(ex);
-        float cum = ex;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const float t = __shfl_up_sync(0xffffffffu, cum, o); if (lane >= o) cum += t; }
-        const unsigned long long r = splitmix64(a.seed ^ ((unsigned long long)b * 0xD1342543DE82EF95ull));
-        const float u = (float)(r >> 40) * (1.0f / 16777216.0f) * denom;
-        const unsigned ok = __ballot_sync(0xffffffffu, lane < A && ex > 0.f && cum > u);
-        const int action = ok ? __ffs(ok) - 1 : arg;
-        const float chosen = __shfl_sync(0xffffffffu, my_logit, action);
-        if (lane < A) a.logits[(size_t)b * A + lane] = my_logit;
-        if (lane == 0) { a.actions[b] = action; a.logp[b] = chosen - best - logf(denom); }
-        __syncwarp();
+        const int s = b < 2 * e.n_pairs ? b : 2 * e.n_pairs;
+        head_row(P.c, ReadoutBlob(P, e.sets + (size_t)s * e.n_weights), a, a.emb + (size_t)s * P.c.n_models * P.c.out_features_node, b,
+                 s_warp[warp], lane);
     }
 }
 
@@ -557,15 +395,16 @@ int ramp_es_act(ramp_es_t* es, ramp_engine_t* eng, int32_t t) {
     if (eb.n_episodes != es->B) return set_error(RAMP_ERR_BAD_ARG, "es: the round was begun on another environment");
     ramp_policy* p = es->p;
     CUDA_TRY(cudaSetDevice(p->device));
-    EsHeadArgs a{};
-    a.n = es->B; a.n_pairs = es->n_pairs; a.n_weights = es->n; a.sets = es->sets.get(); a.emb = es->emb.get();
-    a.obs_dyn = eb.obs_dynamic; a.graph_static = p->d_gstatic.get(); a.model = eb.queued_model; a.done = eb.done; a.mask = eb.action_mask;
-    a.logits = es->logits.get(); a.logp = es->logp.get(); a.actions = eb.actions;
-    a.seed = es_key(es->cfg.seed, es->iteration, es->round, 2 * (uint64_t)(uint32_t)t + 1);
+    HeadArgs a{};
+    a.n = es->B; a.obs_dyn = eb.obs_dynamic; a.graph_static = p->d_gstatic.get(); a.model = eb.queued_model; a.done = eb.done;
+    a.mask = eb.action_mask; a.emb = es->emb.get(); a.logits = es->logits.get(); a.logp = es->logp.get(); a.actions = eb.actions;
+    a.sample = 1; a.seed = es_key(es->cfg.seed, es->iteration, es->round, 2 * (uint64_t)(uint32_t)t + 1);
     es->h_seeds.push_back(a.seed);
+    EsHeadArgs e{};
+    e.n_pairs = es->n_pairs; e.n_weights = es->n; e.sets = es->sets.get();
     const int wpc = 8;
     int grid = std::min((a.n + wpc - 1) / wpc, p->sm_count * 4);
-    ramp_es_head_kernel<<<std::max(grid, 1), wpc * 32, 0, ramp_internal_stream(eng)>>>(p->P, a);
+    ramp_es_head_kernel<<<std::max(grid, 1), wpc * 32, 0, ramp_internal_stream(eng)>>>(p->P, a, e);
     CUDA_TRY(cudaGetLastError());
     ramp_internal_count_launches(eng, 1);
     return RAMP_OK;

@@ -16,6 +16,11 @@
 //                           (gnn_policy.py:283-290), then greedy / categorical action selection written straight into the
 //                           environment's action buffer.  All read-out weights are staged once per CTA in shared memory, laid
 //                           out so that lanes read consecutive words.
+//
+// Each forward's statements exist once: meanpool_round / node_mean / gnn_embed_body for the embedding, head_row for one
+// episode's read-out.  The kernels here, ES's (ramp_es.cuh), the learner's forward (ramp_policy_learn.cuh) and the population's
+// (ramp_population.cuh) all run them, each with its own weight blob and launch shape, so a weight set gives the same bits in every
+// one of them.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -81,92 +86,107 @@ __device__ __forceinline__ void warp_layer_norm(float* buf, int n, const float* 
     __syncwarp();
 }
 
-__global__ void __launch_bounds__(256) ramp_gnn_embed_kernel(const PolicyDev P, const ModelDev* models, float* emb) {
-    __shared__ float sbuf[8][POL_MAX_DIM];
-    const ModelDev M = models[blockIdx.x];
-    if (M.n_nodes <= 0) return;
+// One MeanPool round (mean_pool.py:120-150) with the weight blob `w` on M's graph, by the whole CTA: the round's input zin (rows
+// zin_stride apart) -> its output zout (rows zout_stride apart); hn / he get the node and edge modules' outputs.  buf: this warp's
+// POL_MAX_DIM floats of shared staging.  Every forward of the rounds runs these statements, so they give the same bits.
+__device__ __forceinline__ void meanpool_round(const PolicyDev& P, const float* w, const RoundW& R, const ModelDev& M, const float* zin,
+                                               int zin_stride, float* zout, int zout_stride, float* hn, float* he, float* buf) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
-    float* buf = sbuf[warp];
     const int half = P.c.out_features_msg / 2, msg = P.c.out_features_msg, akind = P.c.aggregator_activation;
+    // ---- node module on every node, edge module on every edge (mean_pool.py:120-127) ----
+    for (int v = warp; v < M.n_nodes; v += n_warps) {
+        for (int k = lane; k < R.in; k += 32) buf[k] = zin[(size_t)v * zin_stride + k];
+        __syncwarp();
+        warp_layer_norm(buf, R.in, w + R.nln_w, w + R.nln_b, lane);
+        for (int o = lane; o < half; o += 32) {
+            float a = w[R.nb + o];
+            const float* row = w + R.nW + (size_t)o * R.in;
+            for (int k = 0; k < R.in; ++k) a += row[k] * buf[k];
+            hn[(size_t)v * half + o] = act_fn(a, akind);
+        }
+        __syncwarp();
+    }
+    const int ine = P.c.in_features_edge;
+    for (int e = warp; e < M.n_edges; e += n_warps) {
+        for (int k = lane; k < ine; k += 32) buf[k] = M.ef[(size_t)e * ine + k];
+        __syncwarp();
+        warp_layer_norm(buf, ine, w + R.eln_w, w + R.eln_b, lane);
+        for (int o = lane; o < half; o += 32) {
+            float a = w[R.eb + o];
+            const float* row = w + R.eW + (size_t)o * ine;
+            for (int k = 0; k < ine; ++k) a += row[k] * buf[k];
+            he[(size_t)e * half + o] = act_fn(a, akind);
+        }
+        __syncwarp();
+    }
+    __syncthreads();
+    // ---- per destination node: mean of reduce_module over [own state, messages] (mean_pool.py:129-150) ----
+    for (int v = warp; v < M.n_nodes; v += n_warps) {
+        const int e0 = M.in_ptr[v], e1 = M.in_ptr[v + 1];
+        float acc[POL_MAX_DIM / 32];
+#pragma unroll
+        for (int i = 0; i < POL_MAX_DIM / 32; ++i) acc[i] = 0.f;
+        if (e1 > e0) {                                              // DGL leaves zero-in-degree nodes at zero
+            for (int mi = -1; mi < e1 - e0; ++mi) {
+                const int src = mi < 0 ? v : M.in_src[e0 + mi];
+                for (int k = lane; k < half; k += 32) {
+                    buf[k] = hn[(size_t)src * half + k];
+                    buf[half + k] = mi < 0 ? 0.f : he[(size_t)M.in_edge[e0 + mi] * half + k];
+                }
+                __syncwarp();
+                warp_layer_norm(buf, msg, w + R.rln_w, w + R.rln_b, lane);
+#pragma unroll
+                for (int i = 0; i < POL_MAX_DIM / 32; ++i) {
+                    const int o = lane + 32 * i;
+                    if (o < R.out) {
+                        float a = w[R.rb + o];
+                        const float* row = w + R.rW + (size_t)o * msg;
+                        for (int k = 0; k < msg; ++k) a += row[k] * buf[k];
+                        acc[i] += act_fn(a, akind);
+                    }
+                }
+                __syncwarp();
+            }
+        }
+        const float inv = 1.0f / (float)(e1 - e0 + 1);
+#pragma unroll
+        for (int i = 0; i < POL_MAX_DIM / 32; ++i) {
+            const int o = lane + 32 * i;
+            if (o < R.out) zout[(size_t)v * zout_stride + o] = acc[i] * inv;
+        }
+    }
+    __syncthreads();
+}
+
+// the mean over the job's n_nodes node states (rows `stride` apart) into emb_out[od] (gnn_policy.py:262-268), by the whole CTA
+__device__ __forceinline__ void node_mean(const float* z, int stride, int n_nodes, int od, float* emb_out) {
+    for (int o = threadIdx.x; o < od; o += blockDim.x) {
+        float s = 0.f;
+        for (int v = 0; v < n_nodes; ++v) s += z[(size_t)v * stride + o];
+        emb_out[o] = s / (float)n_nodes;
+    }
+}
+
+// the embedding of one job type with the weight blob `w` into emb_out[out_node], by the whole CTA; M's z0 / z1 (ping-pong round
+// states) and hn / he are the scratch
+__device__ __forceinline__ void gnn_embed_body(const PolicyDev& P, const float* w, const ModelDev& M, float* emb_out) {
+    __shared__ float sbuf[8][POL_MAX_DIM];
+    if (M.n_nodes <= 0) return;
+    float* buf = sbuf[threadIdx.x >> 5];
     const float* zin = M.nf;
     int zin_stride = P.c.in_features_node;
     float* zout = M.z0;
     for (int r = 0; r < P.c.num_rounds; ++r) {
         const RoundW R = P.rounds[r];
-        const float* w = P.w;
-        // ---- node module on every node, edge module on every edge (mean_pool.py:120-127) ----
-        for (int v = warp; v < M.n_nodes; v += n_warps) {
-            for (int k = lane; k < R.in; k += 32) buf[k] = zin[(size_t)v * zin_stride + k];
-            __syncwarp();
-            warp_layer_norm(buf, R.in, w + R.nln_w, w + R.nln_b, lane);
-            for (int o = lane; o < half; o += 32) {
-                float a = w[R.nb + o];
-                const float* row = w + R.nW + (size_t)o * R.in;
-                for (int k = 0; k < R.in; ++k) a += row[k] * buf[k];
-                M.hn[(size_t)v * half + o] = act_fn(a, akind);
-            }
-            __syncwarp();
-        }
-        const int ine = P.c.in_features_edge;
-        for (int e = warp; e < M.n_edges; e += n_warps) {
-            for (int k = lane; k < ine; k += 32) buf[k] = M.ef[(size_t)e * ine + k];
-            __syncwarp();
-            warp_layer_norm(buf, ine, w + R.eln_w, w + R.eln_b, lane);
-            for (int o = lane; o < half; o += 32) {
-                float a = w[R.eb + o];
-                const float* row = w + R.eW + (size_t)o * ine;
-                for (int k = 0; k < ine; ++k) a += row[k] * buf[k];
-                M.he[(size_t)e * half + o] = act_fn(a, akind);
-            }
-            __syncwarp();
-        }
-        __syncthreads();
-        // ---- per destination node: mean of reduce_module over [own state, messages] (mean_pool.py:129-150) ----
-        for (int v = warp; v < M.n_nodes; v += n_warps) {
-            const int e0 = M.in_ptr[v], e1 = M.in_ptr[v + 1];
-            float acc[POL_MAX_DIM / 32];
-#pragma unroll
-            for (int i = 0; i < POL_MAX_DIM / 32; ++i) acc[i] = 0.f;
-            if (e1 > e0) {                                          // DGL leaves zero-in-degree nodes at zero
-                for (int mi = -1; mi < e1 - e0; ++mi) {
-                    const int src = mi < 0 ? v : M.in_src[e0 + mi];
-                    for (int k = lane; k < half; k += 32) {
-                        buf[k] = M.hn[(size_t)src * half + k];
-                        buf[half + k] = mi < 0 ? 0.f : M.he[(size_t)M.in_edge[e0 + mi] * half + k];
-                    }
-                    __syncwarp();
-                    warp_layer_norm(buf, msg, w + R.rln_w, w + R.rln_b, lane);
-#pragma unroll
-                    for (int i = 0; i < POL_MAX_DIM / 32; ++i) {
-                        const int o = lane + 32 * i;
-                        if (o < R.out) {
-                            float a = w[R.rb + o];
-                            const float* row = w + R.rW + (size_t)o * msg;
-                            for (int k = 0; k < msg; ++k) a += row[k] * buf[k];
-                            acc[i] += act_fn(a, akind);
-                        }
-                    }
-                    __syncwarp();
-                }
-            }
-            const float inv = 1.0f / (float)(e1 - e0 + 1);
-#pragma unroll
-            for (int i = 0; i < POL_MAX_DIM / 32; ++i) {
-                const int o = lane + 32 * i;
-                if (o < R.out) zout[(size_t)v * POL_MAX_DIM + o] = acc[i] * inv;
-            }
-        }
-        __syncthreads();
+        meanpool_round(P, w, R, M, zin, zin_stride, zout, POL_MAX_DIM, M.hn, M.he, buf);
         zin = zout; zin_stride = POL_MAX_DIM;
         zout = (zout == M.z0) ? M.z1 : M.z0;
     }
-    // ---- mean over the job's nodes (gnn_policy.py:262-268) ----
-    const int od = P.c.out_features_node;
-    for (int o = threadIdx.x; o < od; o += blockDim.x) {
-        float s = 0.f;
-        for (int v = 0; v < M.n_nodes; ++v) s += zin[(size_t)v * POL_MAX_DIM + o];
-        emb[(size_t)blockIdx.x * od + o] = s / (float)M.n_nodes;
-    }
+    node_mean(zin, POL_MAX_DIM, M.n_nodes, P.c.out_features_node, emb_out);
+}
+
+__global__ void __launch_bounds__(256) ramp_gnn_embed_kernel(const PolicyDev P, const ModelDev* models, float* emb) {
+    gnn_embed_body(P, P.w, models[blockIdx.x], emb + (size_t)blockIdx.x * P.c.out_features_node);
 }
 
 struct HeadArgs {
@@ -200,19 +220,147 @@ __device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
     return x ^ (x >> 31);
 }
 
-// ramp_policy_head_kernel's statements with the weight blob `w` (P's layout), CTA `cta` of n_ctas: shared with the population's
-// head kernel, which runs one weight set per blockIdx.y
+// The read-out's weights in one of two layouts, read by head_row.  ReadoutStaged: head_body's per-CTA copy in shared memory, the
+// hidden and logit weights transposed to [fin][Hp] / [A][Hp] so that lanes read consecutive hidden units, padded with zero
+// weights and biases to Hp, a multiple of 32 (Hp = H when 32 | H).  ReadoutBlob: the blob's own [H][fin] / [A][H] rows in global
+// memory.  A lane owns the hidden units lane + 32 i, i < units(lane): Hp / 32 of them in the staged copy, padding included -- a
+// padding unit is 0 and adds exactly 0 to a split-K sum that starts from +0, so both layouts give the same bits.
+struct ReadoutWeights { const float *gln_w, *gln_b, *gW, *gb, *hW, *hb, *vhW, *vhb, *lW, *lb, *vW, *vb; };
+
+struct ReadoutStaged : ReadoutWeights {
+    int Hp;
+    __device__ int units(int) const { return Hp / 32; }
+    __device__ float hw(const float* W, int k, int j) const { return W[(size_t)k * Hp + j]; }     // hidden unit j, input k
+    __device__ float lw(int o, int j) const { return lW[(size_t)o * Hp + j]; }                  // logit o, hidden unit j
+};
+
+struct ReadoutBlob : ReadoutWeights {
+    int H, fin;
+    __device__ ReadoutBlob(const PolicyDev& P, const float* w)
+        : ReadoutWeights{w + P.gln_w, w + P.gln_b, w + P.gW, w + P.gb, w + P.hW, w + P.hb, w + P.vhW, w + P.vhb, w + P.lW, w + P.lb, w + P.vW, w + P.vb},
+          H(P.c.fcnet_hidden), fin(P.c.out_features_node + P.c.out_features_graph) {}
+    __device__ int units(int lane) const { return (H - lane + 31) / 32; }
+    __device__ float hw(const float* W, int k, int j) const { return W[(size_t)j * fin + k]; }
+    __device__ float lw(int o, int j) const { return lW[(size_t)o * H + j]; }
+};
+
+// The read-out of episode / row b with the weights W, by one warp (gnn_policy.py:96-109, 262-290): [graph features | action
+// mask] -> LN -> Linear, concat with the job type's embedding emb[m], the hidden layer(s), the logits + max(log(mask), FLT_MIN),
+// the value (only when a.value is given), then the first maximal logit or a categorical draw.  xb: this warp's 2 POL_MAX_DIM
+// floats of shared staging.
+template <class W_>
+__device__ __forceinline__ void head_row(const ramp_policy_config_t& c, const W_& W, const HeadArgs& a, const float* emb, int b, float* xb,
+                                         int lane) {
+    const int gin = c.in_features_graph + c.n_actions, og = c.out_features_graph, on = c.out_features_node, fin = on + og;
+    const int A = c.n_actions, hpl = W.units(lane);
+    const int m = a.model[b];
+    const bool live = m >= 0 && m < c.n_models && !(a.done && a.done[b]);
+    if (!live) {                                                        // nothing queued: the action is ignored by the environment
+        if (lane < A && a.logits) a.logits[(size_t)b * A + lane] = 0.f;
+        if (lane == 0) { a.actions[b] = 0; if (a.value) a.value[b] = 0.f; if (a.logp) a.logp[b] = 0.f; }
+        return;
+    }
+    float* fb = xb + POL_MAX_DIM;
+    // ---- [graph features | action mask] (observation.py:298-300) -> LN -> Linear (gnn_policy.py:96-109) ----
+    for (int k = lane; k < gin; k += 32) {
+        float x;
+        if (k >= c.in_features_graph) x = a.mask[(size_t)b * A + (k - c.in_features_graph)] ? 1.f : 0.f;
+        else if (a.graph_features) x = a.graph_features[(size_t)b * c.in_features_graph + k];
+        else if (k < 9) x = a.obs_dyn[(size_t)b * 11 + k];
+        else if (k < 15) x = a.graph_static[(size_t)m * 6 + (k - 9)];
+        else x = a.obs_dyn[(size_t)b * 11 + (k - 6)];
+        xb[k] = x;
+    }
+    __syncwarp();
+    warp_layer_norm(xb, gin, W.gln_w, W.gln_b, lane);
+    for (int k = lane; k < on; k += 32) fb[k] = emb[(size_t)m * on + k];
+    if (lane < og) {
+        float g = W.gb[lane];
+        const float* row = W.gW + (size_t)lane * gin;
+        for (int k = 0; k < gin; ++k) g += row[k] * xb[k];
+        fb[on + lane] = g;
+    }
+    __syncwarp();
+    // ---- read-out: hidden layer of the policy and of the value branch, each lane owns units lane + 32 i ----
+    float h[POL_MAX_HPL], hv[POL_MAX_HPL];
+    if (c.vf_share_layers || !a.value) {                                // no value hidden layer (the value reads h), or no value
+#pragma unroll
+        for (int i = 0; i < POL_MAX_HPL; ++i) {
+            if (i < hpl) {
+                const int j = lane + 32 * i;
+                float p = W.hb[j];
+                for (int k = 0; k < fin; ++k) p += W.hw(W.hW, k, j) * fb[k];
+                h[i] = hv[i] = act_fn(p, c.fcnet_activation);
+            }
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < POL_MAX_HPL; ++i) {
+            if (i < hpl) {
+                const int j = lane + 32 * i;
+                float p = W.hb[j], q = W.vhb[j];
+                for (int k = 0; k < fin; ++k) { const float f = fb[k]; p += W.hw(W.hW, k, j) * f; q += W.hw(W.vhW, k, j) * f; }
+                h[i] = act_fn(p, c.fcnet_activation); hv[i] = act_fn(q, c.fcnet_activation);
+            }
+        }
+    }
+    float my_logit = -FLT_MAX;
+    for (int o = 0; o < A; ++o) {
+        float p = 0.f;
+#pragma unroll
+        for (int i = 0; i < POL_MAX_HPL; ++i) if (i < hpl) p += h[i] * W.lw(o, lane + 32 * i);
+        p = warp_sum(p) + W.lb[o];
+        if (c.apply_action_mask && !a.mask[(size_t)b * A + o]) p += -FLT_MAX;   // + max(log 0, finfo.min) (gnn_policy.py:285-290)
+        if (lane == o) my_logit = p;
+    }
+    float val = 0.f;
+    if (a.value) {
+#pragma unroll
+        for (int i = 0; i < POL_MAX_HPL; ++i) if (i < hpl) val += hv[i] * W.vW[lane + 32 * i];
+        val = warp_sum(val) + W.vb[0];
+    }
+    // ---- action: first maximal logit, or a categorical draw over softmax(logits) ----
+    float best = my_logit; int arg = lane < A ? lane : 0x7fffffff;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oa = __shfl_xor_sync(0xffffffffu, arg, o);
+        if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
+    }
+    const float ex = lane < A ? expf(my_logit - best) : 0.f;
+    const float denom = warp_sum(ex);
+    int action = arg;
+    if (a.sample) {
+        float cum = ex;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const float t = __shfl_up_sync(0xffffffffu, cum, o); if (lane >= o) cum += t; }
+        const unsigned long long r = splitmix64(a.seed ^ ((unsigned long long)b * 0xD1342543DE82EF95ull));
+        const float u = (float)(r >> 40) * (1.0f / 16777216.0f) * denom;
+        const unsigned ok = __ballot_sync(0xffffffffu, lane < A && ex > 0.f && cum > u);
+        action = ok ? __ffs(ok) - 1 : arg;
+    }
+    const float chosen = __shfl_sync(0xffffffffu, my_logit, action);
+    if (lane < A && a.logits) a.logits[(size_t)b * A + lane] = my_logit;
+    if (lane == 0) {
+        a.actions[b] = action;
+        if (a.value) a.value[b] = val;
+        if (a.logp) a.logp[b] = chosen - best - logf(denom);
+    }
+    __syncwarp();
+}
+
+// ramp_policy_head_kernel's statements with the weight blob `w` (P's layout), CTA `cta` of n_ctas: the read-out weights staged in
+// shared memory, then head_row on the CTA's episodes.  Shared with the population's head kernel, which runs one weight set per
+// blockIdx.y
 __device__ __forceinline__ void head_body(const PolicyDev& P, const float* w, const HeadArgs& a, int cta, int n_ctas) {
     extern __shared__ float sm[];
     const ramp_policy_config_t& c = P.c;
     const int gin = c.in_features_graph + c.n_actions, og = c.out_features_graph, on = c.out_features_node, fin = on + og;
-    // the hidden units padded to Hp, a multiple of 32, with zero weights and biases: a padding unit is 0 and adds exactly 0 to the
-    // split-K sums below (Hp = H when 32 | H)
-    const int H = c.fcnet_hidden, Hp = 32 * ((H + 31) / 32), A = c.n_actions, hpl = Hp / 32;
-    const bool share = c.vf_share_layers;                             // no value hidden layer: the value reads h
+    const int H = c.fcnet_hidden, Hp = 32 * ((H + 31) / 32), A = c.n_actions;
+    const bool share = c.vf_share_layers;                             // no value hidden layer
     float* s_gln_w = sm;                 float* s_gln_b = s_gln_w + gin;
     float* s_gW = s_gln_b + gin;         float* s_gb = s_gW + (size_t)og * gin;
-    float* s_hWt = s_gb + og;            float* s_hb = s_hWt + (size_t)fin * Hp;     // [fin][Hp]: lanes read consecutive hidden units
+    float* s_hWt = s_gb + og;            float* s_hb = s_hWt + (size_t)fin * Hp;     // [fin][Hp]
     float* s_vhWt = s_hb + Hp;           float* s_vhb = s_vhWt + (share ? 0 : (size_t)fin * Hp);
     float* s_lW = s_vhb + (share ? 0 : Hp); float* s_lb = s_lW + (size_t)A * Hp;     // [A][Hp]
     float* s_vW = s_lb + A;              float* s_vb = s_vW + Hp;
@@ -241,102 +389,10 @@ __device__ __forceinline__ void head_body(const PolicyDev& P, const float* w, co
     }
     __syncthreads();
 
+    const ReadoutStaged W{{s_gln_w, s_gln_b, s_gW, s_gb, s_hWt, s_hb, s_vhWt, s_vhb, s_lW, s_lb, s_vW, s_vb}, Hp};
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpc = blockDim.x >> 5;
     float* xb = s_warp + (size_t)warp * 2 * POL_MAX_DIM;                // graph-module input, then the read-out input
-    float* fb = xb + POL_MAX_DIM;
-    for (int b = cta * wpc + warp; b < a.n; b += n_ctas * wpc) {
-        const int m = a.model[b];
-        const bool live = m >= 0 && m < c.n_models && !(a.done && a.done[b]);
-        if (!live) {                                                    // nothing queued: the action is ignored by the environment
-            if (lane < A && a.logits) a.logits[(size_t)b * A + lane] = 0.f;
-            if (lane == 0) { a.actions[b] = 0; if (a.value) a.value[b] = 0.f; if (a.logp) a.logp[b] = 0.f; }
-            continue;
-        }
-        // ---- [graph features | action mask] (observation.py:298-300) -> LN -> Linear (gnn_policy.py:96-109) ----
-        for (int k = lane; k < gin; k += 32) {
-            float x;
-            if (k >= c.in_features_graph) x = a.mask[(size_t)b * A + (k - c.in_features_graph)] ? 1.f : 0.f;
-            else if (a.graph_features) x = a.graph_features[(size_t)b * c.in_features_graph + k];
-            else if (k < 9) x = a.obs_dyn[(size_t)b * 11 + k];
-            else if (k < 15) x = a.graph_static[(size_t)m * 6 + (k - 9)];
-            else x = a.obs_dyn[(size_t)b * 11 + (k - 6)];
-            xb[k] = x;
-        }
-        __syncwarp();
-        warp_layer_norm(xb, gin, s_gln_w, s_gln_b, lane);
-        for (int k = lane; k < on; k += 32) fb[k] = a.emb[(size_t)m * on + k];
-        if (lane < og) {
-            float g = s_gb[lane];
-            const float* row = s_gW + (size_t)lane * gin;
-            for (int k = 0; k < gin; ++k) g += row[k] * xb[k];
-            fb[on + lane] = g;
-        }
-        __syncwarp();
-        // ---- read-out: hidden layer of the policy and of the value branch, each lane owns units lane + 32 i ----
-        float h[POL_MAX_HPL], hv[POL_MAX_HPL];
-        if (share) {
-#pragma unroll
-            for (int i = 0; i < POL_MAX_HPL; ++i) {
-                if (i < hpl) {
-                    const int j = lane + 32 * i;
-                    float p = s_hb[j];
-                    for (int k = 0; k < fin; ++k) p += s_hWt[(size_t)k * Hp + j] * fb[k];
-                    h[i] = hv[i] = act_fn(p, c.fcnet_activation);
-                }
-            }
-        } else {
-#pragma unroll
-            for (int i = 0; i < POL_MAX_HPL; ++i) {
-                if (i < hpl) {
-                    const int j = lane + 32 * i;
-                    float p = s_hb[j], q = s_vhb[j];
-                    for (int k = 0; k < fin; ++k) { const float f = fb[k]; p += s_hWt[(size_t)k * Hp + j] * f; q += s_vhWt[(size_t)k * Hp + j] * f; }
-                    h[i] = act_fn(p, c.fcnet_activation); hv[i] = act_fn(q, c.fcnet_activation);
-                }
-            }
-        }
-        float my_logit = -FLT_MAX;
-        for (int o = 0; o < A; ++o) {
-            float p = 0.f;
-#pragma unroll
-            for (int i = 0; i < POL_MAX_HPL; ++i) if (i < hpl) p += h[i] * s_lW[(size_t)o * Hp + lane + 32 * i];
-            p = warp_sum(p) + s_lb[o];
-            if (c.apply_action_mask && !a.mask[(size_t)b * A + o]) p += -FLT_MAX;   // + max(log 0, finfo.min) (gnn_policy.py:285-290)
-            if (lane == o) my_logit = p;
-        }
-        float val = 0.f;
-#pragma unroll
-        for (int i = 0; i < POL_MAX_HPL; ++i) if (i < hpl) val += hv[i] * s_vW[lane + 32 * i];
-        val = warp_sum(val) + s_vb[0];
-        // ---- action: first maximal logit, or a categorical draw over softmax(logits) ----
-        float best = my_logit; int arg = lane < A ? lane : 0x7fffffff;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oa = __shfl_xor_sync(0xffffffffu, arg, o);
-            if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
-        }
-        const float ex = lane < A ? expf(my_logit - best) : 0.f;
-        const float denom = warp_sum(ex);
-        int action = arg;
-        if (a.sample) {
-            float cum = ex;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { const float t = __shfl_up_sync(0xffffffffu, cum, o); if (lane >= o) cum += t; }
-            const unsigned long long r = splitmix64(a.seed ^ ((unsigned long long)b * 0xD1342543DE82EF95ull));
-            const float u = (float)(r >> 40) * (1.0f / 16777216.0f) * denom;
-            const unsigned ok = __ballot_sync(0xffffffffu, lane < A && ex > 0.f && cum > u);
-            action = ok ? __ffs(ok) - 1 : arg;
-        }
-        const float chosen = __shfl_sync(0xffffffffu, my_logit, action);
-        if (lane < A && a.logits) a.logits[(size_t)b * A + lane] = my_logit;
-        if (lane == 0) {
-            a.actions[b] = action;
-            if (a.value) a.value[b] = val;
-            if (a.logp) a.logp[b] = chosen - best - logf(denom);
-        }
-        __syncwarp();
-    }
+    for (int b = cta * wpc + warp; b < a.n; b += n_ctas * wpc) head_row(c, W, a, a.emb, b, xb, lane);
 }
 
 // at most 80 registers (three CTAs per SM), what the kernel used before its read-out was padded to Hp: left alone, ptxas takes 113
@@ -411,6 +467,35 @@ struct HostModel {
     bool grad_ready = false;
 };
 
+struct SegTable { DeviceArray<Seg> d; int32_t count = 0; int64_t total = 0; };
+
+// The learner's device buffers for K weight sets, stacked set-major: the single policy holds them with K = 1, a population
+// (ramp_population.cuh) with its K.  Each capacity stays 0 until every buffer it covers has the new size.
+struct LearnerBuffers {
+    int32_t K = 1;
+    // gradient, Adam's moments and step counts (two per set, read and written by alternate steps: `parity`), per job type
+    // gradients, norm partials, statistics, each minibatch's statistics, the train batch's row count per set
+    bool ready = false;
+    int32_t parity = 0;
+    DeviceArray<float> grad, adam_m, adam_v, gpart;
+    DeviceArray<int32_t> step, n_rows;
+    DeviceArray<double> norm_part, stats, mb_stats;
+    // every (set, job type)'s MeanPool states and backward scratch, [K][n_models]
+    bool gmodels_ready = false;
+    DeviceArray<GradModelDev> gmodels;
+    // per-row scratch for K minibatches of `lcap` rows; the head segments of set 0's records for every row count seen since `rec`
+    // was last allocated (a segment points into rec), `segs` those of the current one
+    int32_t lcap = 0;
+    DeviceArray<float> rec, row_stats;
+    DeviceArray<int32_t> row_model;
+    std::map<int32_t, SegTable> seg_tables;
+    const SegTable* segs = nullptr;
+    // the train batch (K groups of [horizon * b] rows, live rows first, t-major) and the bootstrap values ([B])
+    int32_t bcap = 0, boot_cap = 0;
+    DeviceArray<float> b_obs, b_logp, b_logp_old, b_adv, b_vt, b_old, b_value, b_lpx, boot;
+    DeviceArray<int32_t> b_model, b_action, b_actx, boot_act; DeviceArray<uint8_t> b_mask; DeviceArray<double> b_adv64;
+};
+
 struct ramp_policy {
     int device = 0;
     PolicyDev P{};
@@ -435,29 +520,17 @@ struct ramp_policy {
     int32_t traj_n = 0;                   // slots recorded in order, both phases, since ramp_policy_trajectory_begin
     DeviceArray<float> t_obs, t_logp, t_value; DeviceArray<int32_t> t_model, t_action;
     DeviceArray<uint8_t> t_mask, t_done; DeviceArray<double> t_reward;
-    // learner (ramp_policy_backward / ramp_ppo_loss_grad / ramp_policy_learn): gradient, Adam's moments and step count, per job type
-    // gradients, norm partials; per-row scratch for `lcap` rows; the head segments of every row count seen since l_rec was last
-    // allocated (a segment points into l_rec), `segs` those of the current one
-    // states_current: the MeanPool states kept in d_gmodels are those of a whole-batch forward at the current weights
-    bool learner_ready = false, gmodels_ready = false, states_current = false;
-    int32_t adam_parity = 0, lcap = 0;
-    struct SegTable { DeviceArray<Seg> d; int32_t count = 0; int64_t total = 0; };
-    std::map<int32_t, SegTable> seg_tables;
-    const SegTable* segs = nullptr;
-    DeviceArray<float> l_grad, l_adam_m, l_adam_v, l_gpart, l_rec, l_row_stats;
-    DeviceArray<int32_t> l_n_rows, l_step, l_row_model;
-    DeviceArray<double> l_norm_part, l_stats, l_mb_stats;
+    // learner (ramp_policy_backward / ramp_ppo_loss_grad / ramp_policy_learn / _learn_pg / _learn_impala)
+    // states_current: the MeanPool states kept in L.gmodels are those of a whole-batch forward at the current weights
+    LearnerBuffers L;
+    bool states_current = false;
     // the end of the last call that touched the scratch above, the staging or the embeddings (made by the first device-path call;
     // until then every call keeps its own synchronisation and nothing is recorded)
     Event ev_done;
-    DeviceArray<GradModelDev> d_gmodels;
-    // host-input batches of ramp_policy_backward / ramp_ppo_loss_grad
+    // host-input batches of ramp_policy_backward / ramp_ppo_loss_grad, and their row count on the device
     int32_t hcap = 0;
-    DeviceArray<int32_t> h_model, h_action; DeviceArray<float> h_gf, h_gl, h_gv, h_old, h_adv, h_vt; DeviceArray<uint8_t> h_mask;
-    // ramp_policy_learn's / ramp_policy_learn_pg's train batch ([horizon * B] rows, live rows first, t-major) and bootstrap values ([B])
-    int32_t bcap = 0, boot_cap = 0, b_rows = 0;
-    DeviceArray<float> b_obs, b_logp, b_logp_old, b_adv, b_vt, b_old, b_value, b_lpx, l_boot;
-    DeviceArray<int32_t> b_model, b_action, b_actx, l_boot_act; DeviceArray<uint8_t> b_mask; DeviceArray<double> b_adv64;
+    DeviceArray<int32_t> h_model, h_action, h_n_rows; DeviceArray<float> h_gf, h_gl, h_gv, h_old, h_adv, h_vt; DeviceArray<uint8_t> h_mask;
+    int32_t b_rows = 0;                   // the rows of the last train batch (ramp_policy_train_batch_read)
     // IMPALA (ramp_policy_learn_impala / ramp_impala_loss_grad): the fragment rows ([icap], row f L + t) with their read-out at
     // the current weights and V-trace values, the loss's job types (-1 outside it), the host batch's extra inputs, statistics
     int32_t icap = 0, i_rows = 0, i_step_cap = 0;
@@ -612,21 +685,21 @@ uint64_t mix64(uint64_t x) {              // splitmix64, as the kernels' splitmi
 
 int64_t gnn_weight_count(const ramp_policy* p) { return p->P.gln_w; }     // the rounds come first in the blob
 
-int ensure_learner(ramp_policy* p) {
-    if (p->learner_ready) return RAMP_OK;
-    const size_t nw = (size_t)p->n_weights;
-    CUDA_TRY(alloc_each(nw, p->l_grad, p->l_adam_m, p->l_adam_v));
-    CUDA_TRY(p->l_gpart.alloc((size_t)p->P.c.n_models * gnn_weight_count(p)));
-    CUDA_TRY(p->l_n_rows.alloc(2));                                  // [0] learn's train batch, [1] a host batch
-    CUDA_TRY(p->l_step.alloc(2));
-    CUDA_TRY(p->l_norm_part.alloc(LRN_GRID));
-    CUDA_TRY(p->l_stats.alloc(RAMP_PPO_STATS_LEN));
-    CUDA_TRY(p->d_gmodels.alloc(p->P.c.n_models));
-    CUDA_TRY(cudaMemset(p->l_adam_m.get(), 0, sizeof(float) * nw));
-    CUDA_TRY(cudaMemset(p->l_adam_v.get(), 0, sizeof(float) * nw));
-    CUDA_TRY(cudaMemset(p->l_step.get(), 0, sizeof(int32_t) * 2));
-    p->adam_parity = 0;
-    p->learner_ready = true;
+// L's gradient, Adam state (zeroed), job-type partials, norm partials and statistics for the K sets of p's configuration
+int ensure_learner(LearnerBuffers& L, const ramp_policy* p) {
+    if (L.ready) return RAMP_OK;
+    const size_t K = L.K, n = K * (size_t)p->n_weights;
+    CUDA_TRY(alloc_each(n, L.grad, L.adam_m, L.adam_v));
+    CUDA_TRY(L.gpart.alloc(K * p->P.c.n_models * gnn_weight_count(p)));
+    CUDA_TRY(L.n_rows.alloc(K));
+    CUDA_TRY(L.step.alloc(2 * K));
+    CUDA_TRY(L.norm_part.alloc(K * LRN_GRID));
+    CUDA_TRY(L.stats.alloc(K * RAMP_PPO_STATS_LEN));
+    CUDA_TRY(cudaMemset(L.adam_m.get(), 0, sizeof(float) * n));
+    CUDA_TRY(cudaMemset(L.adam_v.get(), 0, sizeof(float) * n));
+    CUDA_TRY(cudaMemset(L.step.get(), 0, sizeof(int32_t) * 2 * K));
+    L.parity = 0;
+    L.ready = true;
     return RAMP_OK;
 }
 
@@ -649,9 +722,18 @@ int alloc_grad_scratch(const ramp_policy_config_t& c, size_t N, size_t E, std::v
     return RAMP_OK;
 }
 
-// every job type's forward states and records for the embedding backward, sized by its graph
+// the [K][n_models] table of forward states and backward scratch `h` into L.gmodels, on `st`
+int upload_gmodels(LearnerBuffers& L, const std::vector<GradModelDev>& h, cudaStream_t st) {
+    if (L.gmodels.size() < h.size()) CUDA_TRY(L.gmodels.alloc(h.size()));
+    CUDA_TRY(cudaMemcpyAsync(L.gmodels.get(), h.data(), sizeof(GradModelDev) * h.size(), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));                                  // `h` is pageable
+    L.gmodels_ready = true;
+    return RAMP_OK;
+}
+
+// every job type's forward states and records for the embedding backward, sized by its graph and kept with it
 int ensure_gmodels(ramp_policy* p, cudaStream_t st) {
-    if (p->gmodels_ready) return RAMP_OK;
+    if (p->L.gmodels_ready) return RAMP_OK;
     std::vector<GradModelDev> h(p->models.size());
     for (size_t m = 0; m < h.size(); ++m) {
         HostModel& hm = p->models[m];
@@ -664,36 +746,58 @@ int ensure_gmodels(ramp_policy* p, cudaStream_t st) {
         }
         h[m] = hm.g;
     }
-    CUDA_TRY(cudaMemcpyAsync(p->d_gmodels.get(), h.data(), sizeof(GradModelDev) * h.size(), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaStreamSynchronize(st));                                  // `h` is pageable
-    p->gmodels_ready = true;
-    return RAMP_OK;
+    return upload_gmodels(p->L, h, st);
 }
 
-// per-row scratch for minibatches of n rows, and the head segments summing exactly n rows: uploaded on `st` the first time n is
-// seen, so a PPO loop whose last minibatch is short does not synchronise every time the row count alternates
-int ensure_rows(ramp_policy* p, int32_t n, cudaStream_t st) {
-    if (n > p->lcap) {
-        p->lcap = 0;
-        p->segs = nullptr;
-        p->seg_tables.clear();
-        CUDA_TRY(p->l_rec.alloc((size_t)n * head_rec(p->P.c).stride));
-        CUDA_TRY(p->l_row_stats.alloc((size_t)n * RS_N));
-        CUDA_TRY(p->l_row_model.alloc(n));
-        p->lcap = n;
+// per-row scratch for K minibatches of n rows, and the head segments summing exactly n of set 0's rows: uploaded on `st` the first
+// time n is seen, so a PPO loop whose last minibatch is short does not synchronise every time the row count alternates
+int ensure_rows(LearnerBuffers& L, const PolicyDev& P, int32_t n, cudaStream_t st) {
+    if (n > L.lcap) {
+        const size_t rows = (size_t)L.K * n;
+        L.lcap = 0;
+        L.segs = nullptr;
+        L.seg_tables.clear();
+        CUDA_TRY(L.rec.alloc(rows * head_rec(P.c).stride));
+        CUDA_TRY(L.row_stats.alloc(rows * RS_N));
+        CUDA_TRY(L.row_model.alloc(rows));
+        L.lcap = n;
     }
-    auto it = p->seg_tables.find(n);
-    if (it == p->seg_tables.end()) {
+    auto it = L.seg_tables.find(n);
+    if (it == L.seg_tables.end()) {
         Seg s[HEAD_SEGS];
-        ramp_policy::SegTable t;
-        t.count = head_segs(p->P, p->l_rec.get(), n, s);
+        SegTable t;
+        t.count = head_segs(P, L.rec.get(), n, s);
         for (int k = 0; k < t.count; ++k) t.total += seg_size(s[k]);
         CUDA_TRY(t.d.alloc(HEAD_SEGS));
         CUDA_TRY(cudaMemcpyAsync(t.d.get(), s, sizeof(s), cudaMemcpyHostToDevice, st));
         CUDA_TRY(cudaStreamSynchronize(st));                              // `s` is pageable
-        it = p->seg_tables.emplace(n, std::move(t)).first;
+        it = L.seg_tables.emplace(n, std::move(t)).first;
     }
-    p->segs = &it->second;
+    L.segs = &it->second;
+    return RAMP_OK;
+}
+
+// the train batch for K groups of `rows` trajectory slots each
+int ensure_batch(LearnerBuffers& L, const ramp_policy_config_t& c, int32_t rows) {
+    if (rows <= L.bcap) return RAMP_OK;
+    const size_t n = (size_t)L.K * rows;
+    L.bcap = 0;
+    CUDA_TRY(alloc_each(n, L.b_logp, L.b_logp_old, L.b_adv, L.b_vt, L.b_value, L.b_lpx, L.b_model, L.b_action, L.b_actx, L.b_adv64));
+    CUDA_TRY(L.b_obs.alloc(n * 11));
+    CUDA_TRY(alloc_each(n * c.n_actions, L.b_mask, L.b_old));
+    L.bcap = rows;
+    return RAMP_OK;
+}
+
+// a PPO learn call's bootstrap values for B episodes and statistics for K sets of n_mb minibatches
+int ensure_ppo(LearnerBuffers& L, int32_t B, int32_t n_mb) {
+    if (B > L.boot_cap) {
+        L.boot_cap = 0;
+        CUDA_TRY(alloc_each(B, L.boot, L.boot_act));
+        L.boot_cap = B;
+    }
+    const size_t n = (size_t)L.K * n_mb * RAMP_PPO_STATS_LEN;
+    if (n > L.mb_stats.size()) CUDA_TRY(L.mb_stats.alloc(n));
     return RAMP_OK;
 }
 
@@ -701,9 +805,9 @@ int ensure_rows(ramp_policy* p, int32_t n, cudaStream_t st) {
 // and per-row scratch for minibatches of `rows` rows
 int prepare_learner(ramp_policy* p, cudaStream_t st, int32_t rows) {
     int rc;
-    if ((rc = fence_in(p, st)) != RAMP_OK || (rc = ensure_learner(p)) != RAMP_OK || (rc = ensure_gmodels(p, st)) != RAMP_OK) return rc;
+    if ((rc = fence_in(p, st)) != RAMP_OK || (rc = ensure_learner(p->L, p)) != RAMP_OK || (rc = ensure_gmodels(p, st)) != RAMP_OK) return rc;
     if (!p->emb_valid && (rc = launch_embed(p, st)) != RAMP_OK) return rc;
-    return ensure_rows(p, rows, st);
+    return ensure_rows(p->L, p->P, rows, st);
 }
 
 // the MeanPool rounds of every job type, kept for the backward (and the embeddings when `emb` is given); nothing for a minibatch
@@ -711,7 +815,7 @@ int prepare_learner(ramp_policy* p, cudaStream_t st, int32_t rows) {
 int launch_states(ramp_policy* p, cudaStream_t st, const int32_t* n_rows, int32_t start, float* emb) {
     EmbGradArgs eg{};
     eg.n_rows = n_rows; eg.start = start; eg.emb = emb;
-    ramp_gnn_embed_grad_kernel<EMB_FORWARD><<<p->P.c.n_models, 256, 0, st>>>(p->P, p->d_models.get(), p->d_gmodels.get(), eg);
+    ramp_gnn_embed_grad_kernel<EMB_FORWARD><<<p->P.c.n_models, 256, 0, st>>>(p->P, p->d_models.get(), p->L.gmodels.get(), eg);
     CUDA_TRY(cudaGetLastError());
     p->states_current = n_rows == nullptr;                         // a learn call's minibatch past the batch's end keeps none
     return RAMP_OK;
@@ -720,17 +824,17 @@ int launch_states(ramp_policy* p, cudaStream_t st, const int32_t* n_rows, int32_
 // head gradient -> head reduction -> embedding gradient (from launch_states' states) -> per-job-type sum and norm partials:
 // the gradient in l_grad
 int launch_grad(ramp_policy* p, GradArgs ga, cudaStream_t st) {
-    ga.rec = p->l_rec.get(); ga.row_model = p->l_row_model.get(); ga.row_stats = p->l_row_stats.get();
+    ga.rec = p->L.rec.get(); ga.row_model = p->L.row_model.get(); ga.row_stats = p->L.row_stats.get();
     ga.emb = p->d_emb.get(); ga.graph_static = p->d_gstatic.get();
     ramp_policy_head_grad_kernel<<<(ga.mb + LRN_WARPS - 1) / LRN_WARPS, LRN_WARPS * 32, 0, st>>>(p->P, ga);
-    int64_t grid = (p->segs->total + 255) / 256;
+    int64_t grid = (p->L.segs->total + 255) / 256;
     if (grid > 4 * p->sm_count) grid = 4 * p->sm_count;
-    ramp_policy_head_reduce_kernel<<<(unsigned)grid, 256, 0, st>>>(p->P, p->segs->d.get(), p->segs->count, p->segs->total, p->l_grad.get());
+    ramp_policy_head_reduce_kernel<<<(unsigned)grid, 256, 0, st>>>(p->P, p->L.segs->d.get(), p->L.segs->count, p->L.segs->total, p->L.grad.get());
     EmbGradArgs eg{};
-    eg.rec = p->l_rec.get(); eg.row_model = p->l_row_model.get(); eg.rows = ga.mb; eg.gpart = p->l_gpart.get(); eg.n_gnn = gnn_weight_count(p);
-    ramp_gnn_embed_grad_kernel<EMB_BACKWARD><<<p->P.c.n_models, 256, 0, st>>>(p->P, p->d_models.get(), p->d_gmodels.get(), eg);
-    ramp_grad_finish_kernel<<<LRN_GRID, 256, 0, st>>>(p->l_gpart.get(), p->P.c.n_models, gnn_weight_count(p), p->n_weights,
-                                                       p->l_grad.get(), p->l_norm_part.get());
+    eg.rec = p->L.rec.get(); eg.row_model = p->L.row_model.get(); eg.rows = ga.mb; eg.gpart = p->L.gpart.get(); eg.n_gnn = gnn_weight_count(p);
+    ramp_gnn_embed_grad_kernel<EMB_BACKWARD><<<p->P.c.n_models, 256, 0, st>>>(p->P, p->d_models.get(), p->L.gmodels.get(), eg);
+    ramp_grad_finish_kernel<<<LRN_GRID, 256, 0, st>>>(p->L.gpart.get(), p->P.c.n_models, gnn_weight_count(p), p->n_weights,
+                                                       p->L.grad.get(), p->L.norm_part.get());
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
 }
@@ -754,6 +858,7 @@ int stage_host_batch(ramp_policy* p, int32_t n) {
     const ramp_policy_config_t& c = p->P.c;
     p->hcap = 0;
     CUDA_TRY(alloc_each(n, p->h_model, p->h_action, p->h_gv, p->h_adv, p->h_vt));
+    if (!p->h_n_rows.get()) CUDA_TRY(p->h_n_rows.alloc(1));
     CUDA_TRY(p->h_gf.alloc((size_t)n * c.in_features_graph));
     CUDA_TRY(alloc_each((size_t)n * (size_t)c.n_actions, p->h_gl, p->h_old, p->h_mask));
     p->hcap = n;
@@ -775,7 +880,7 @@ int upload_host_batch(ramp_policy* p, int32_t n, const int32_t* model, const flo
         (rc = put(p->h_mask.get(), mask, (size_t)n * A)) || (rc = put(p->h_gl.get(), gl, 4 * (size_t)n * A)) ||
         (rc = put(p->h_gv.get(), gv, 4 * (size_t)n)) || (rc = put(p->h_action.get(), action, 4 * (size_t)n)) ||
         (rc = put(p->h_old.get(), old_logits, 4 * (size_t)n * A)) || (rc = put(p->h_adv.get(), adv, 4 * (size_t)n)) ||
-        (rc = put(p->h_vt.get(), vt, 4 * (size_t)n)) || (rc = put(p->l_n_rows.get() + 1, &n, 4)))
+        (rc = put(p->h_vt.get(), vt, 4 * (size_t)n)) || (rc = put(p->h_n_rows.get(), &n, 4)))
         return rc;
     for (int32_t b = 0; b < n; ++b)
         if (action && model[b] >= 0 && model[b] < c.n_models && (action[b] < 0 || action[b] >= c.n_actions))
@@ -783,20 +888,9 @@ int upload_host_batch(ramp_policy* p, int32_t n, const int32_t* model, const flo
     return RAMP_OK;
 }
 
-// the train batch of ramp_policy_learn / ramp_policy_learn_pg for `rows` trajectory slots
-int ensure_batch(ramp_policy* p, int32_t rows) {
-    if (rows <= p->bcap) return RAMP_OK;
-    p->bcap = 0;
-    CUDA_TRY(alloc_each(rows, p->b_logp, p->b_logp_old, p->b_adv, p->b_vt, p->b_value, p->b_lpx, p->b_model, p->b_action, p->b_actx, p->b_adv64));
-    CUDA_TRY(p->b_obs.alloc((size_t)rows * 11));
-    CUDA_TRY(alloc_each((size_t)rows * p->P.c.n_actions, p->b_mask, p->b_old));
-    p->bcap = rows;
-    return RAMP_OK;
-}
-
 GradArgs host_batch_args(ramp_policy* p, int32_t n) {
     GradArgs ga{};
-    ga.mb = n; ga.start = 0; ga.n_rows = p->l_n_rows.get() + 1;
+    ga.mb = n; ga.start = 0; ga.n_rows = p->h_n_rows.get();
     ga.graph_features = p->h_gf.get(); ga.model = p->h_model.get(); ga.mask = p->h_mask.get();
     return ga;
 }
@@ -821,7 +915,7 @@ int launch_ingest(ramp_policy* p, cudaStream_t st, int32_t n, const void* model,
     a.gf_stride = gf_stride; a.model = model; a.graph_features = graph_features; a.mask = mask; a.grad_logits = gl; a.grad_value = gv;
     if (gl) {
         a.model_out = p->h_model.get(); a.gf_out = p->h_gf.get(); a.mask_out = p->h_mask.get();
-        a.gl_out = p->h_gl.get(); a.gv_out = p->h_gv.get(); a.n_rows_out = p->l_n_rows.get() + 1;
+        a.gl_out = p->h_gl.get(); a.gv_out = p->h_gv.get(); a.n_rows_out = p->h_n_rows.get();
     } else {
         a.model_out = p->f_model.get(); a.gf_out = p->f_gf.get(); a.mask_out = p->f_mask.get();
     }
@@ -886,9 +980,9 @@ int launch_gae(ramp_policy* p, cudaStream_t st, int32_t T, int32_t B, double gam
     ge.gamma = gamma; ge.lambda = lambda;
     ge.t_obs = p->t_obs.get(); ge.t_model = p->t_model.get(); ge.t_mask = p->t_mask.get(); ge.t_action = p->t_action.get();
     ge.t_logp = p->t_logp.get(); ge.t_value = boot ? p->t_value.get() : nullptr; ge.t_reward = p->t_reward.get(); ge.t_done = p->t_done.get();
-    ge.boot = boot; ge.adv64 = p->b_adv64.get();
-    ge.obs = p->b_obs.get(); ge.model = p->b_model.get(); ge.mask = p->b_mask.get(); ge.action = p->b_action.get(); ge.logp = p->b_logp.get();
-    ge.adv = p->b_adv.get(); ge.vt = p->b_vt.get(); ge.n_rows = p->l_n_rows.get();
+    ge.boot = boot; ge.adv64 = p->L.b_adv64.get();
+    ge.obs = p->L.b_obs.get(); ge.model = p->L.b_model.get(); ge.mask = p->L.b_mask.get(); ge.action = p->L.b_action.get(); ge.logp = p->L.b_logp.get();
+    ge.adv = p->L.b_adv.get(); ge.vt = p->L.b_vt.get(); ge.n_rows = p->L.n_rows.get();
     ramp_ppo_gae_kernel<<<1, 1024, 0, st>>>(ge);
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
@@ -902,14 +996,14 @@ AdamArgs adam_args(ramp_policy* p, const Cfg& cfg, const int32_t* n_rows, int32_
     aa.lr = cfg.lr; aa.beta1 = cfg.adam_beta1; aa.beta2 = cfg.adam_beta2;
     aa.beta2_f = (float)cfg.adam_beta2; aa.one_m_beta1 = (float)(1.0 - cfg.adam_beta1); aa.one_m_beta2 = (float)(1.0 - cfg.adam_beta2);
     aa.eps = (float)cfg.adam_eps;
-    aa.max_norm = (float)cfg.grad_clip; aa.n_rows = n_rows; aa.mb = mb; aa.step = p->l_step.get();
-    aa.m = p->l_adam_m.get(); aa.v = p->l_adam_v.get(); aa.grad = p->l_grad.get(); aa.norm_part = p->l_norm_part.get(); aa.w = p->d_w.get();
+    aa.max_norm = (float)cfg.grad_clip; aa.n_rows = n_rows; aa.mb = mb; aa.step = p->L.step.get();
+    aa.m = p->L.adam_m.get(); aa.v = p->L.adam_v.get(); aa.grad = p->L.grad.get(); aa.norm_part = p->L.norm_part.get(); aa.w = p->d_w.get();
     return aa;
 }
 
 // one Adam step on `st`: it reads the step count the previous step wrote
 int launch_adam(ramp_policy* p, AdamArgs aa, cudaStream_t st) {
-    aa.parity = p->adam_parity; p->adam_parity ^= 1;
+    aa.parity = p->L.parity; p->L.parity ^= 1;
     ramp_adam_kernel<<<LRN_GRID, 256, 0, st>>>(aa, p->n_weights);
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
@@ -918,7 +1012,7 @@ int launch_adam(ramp_policy* p, AdamArgs aa, cudaStream_t st) {
 // the end of the gradient calls on host rows (stream 0): the gradient and n_stats statistics from `stats` (either out may be nullptr)
 int host_batch_end(ramp_policy* p, float* grad_out, double* stats_out, const double* stats, int n_stats) {
     CUDA_TRY(cudaStreamSynchronize(0));
-    if (grad_out) CUDA_TRY(cudaMemcpy(grad_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    if (grad_out) CUDA_TRY(cudaMemcpy(grad_out, p->L.grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
     if (stats_out) CUDA_TRY(cudaMemcpy(stats_out, stats, sizeof(double) * n_stats, cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
@@ -974,8 +1068,8 @@ int impala_batch(ramp_policy* p, cudaStream_t st, const ramp_impala_config_t& cf
     ga.action = action; ga.adv = p->i_pg.get(); ga.vt = p->i_vs.get();
     ga.vf_coeff = (float)cfg.vf_loss_coeff; ga.ent_coeff = (float)cfg.entropy_coeff;
     if ((rc = launch_grad(p, ga, st)) != RAMP_OK) return rc;
-    ramp_impala_step_stats_kernel<<<1, 1, 0, st>>>(p->l_row_stats.get(), p->l_row_model.get(), ga.mb, row0, p->i_log_rho.get(),
-                                                   cfg.vf_loss_coeff, cfg.entropy_coeff, p->l_norm_part.get(), stats);
+    ramp_impala_step_stats_kernel<<<1, 1, 0, st>>>(p->L.row_stats.get(), p->L.row_model.get(), ga.mb, row0, p->i_log_rho.get(),
+                                                   cfg.vf_loss_coeff, cfg.entropy_coeff, p->L.norm_part.get(), stats);
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
 }
@@ -1045,7 +1139,7 @@ int ramp_policy_set_model(ramp_policy_t* p, int32_t model, int32_t n_nodes, int3
     HostModel& hm = p->models[model];
     hm.allocs.clear();
     hm.lallocs.clear();
-    hm.set = hm.grad_ready = p->gmodels_ready = false;
+    hm.set = hm.grad_ready = p->L.gmodels_ready = false;
     // incoming-edge lists by destination, in edge order (the order DGL delivers a node's mailbox is not observable through a mean)
     std::vector<int32_t> ptr(n_nodes + 1, 0), ine(n_edges), ins(n_edges);
     for (int e = 0; e < n_edges; ++e) ptr[edges_dst[e] + 1]++;
@@ -1274,7 +1368,7 @@ int ramp_policy_forward_device(ramp_policy_t* p, void* stream, int32_t n, const 
         return rc;
     // once a backward has set up the learner, stale embeddings are remade by the gradient kernel's forward instance: the same
     // bits, and its kept states spare the next backward a second pass over the MeanPool rounds (the fused learners do the same)
-    if (!p->emb_valid && p->learner_ready && p->gmodels_ready) {
+    if (!p->emb_valid && p->L.ready && p->L.gmodels_ready) {
         if ((rc = launch_states(p, st, nullptr, 0, p->d_emb.get())) != RAMP_OK) return rc;
         p->emb_valid = true;
     }
@@ -1294,7 +1388,7 @@ int ramp_policy_backward_device(ramp_policy_t* p, void* stream, int32_t n, const
         (rc = launch_ingest(p, st, n, model, model_dtype, graph_features, graph_features_stride, action_mask, grad_logits, grad_value)) != RAMP_OK ||
         (rc = launch_backward(p, st, n, true)) != RAMP_OK)
         return rc;
-    CUDA_TRY(cudaMemcpyAsync(grad_weights_out, p->l_grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(grad_weights_out, p->L.grad.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToDevice, st));
     return fence_out(p, st);
 }
 
@@ -1314,9 +1408,9 @@ int ramp_ppo_loss_grad(ramp_policy_t* p, const ramp_ppo_config_t* cfg, int32_t n
     ga.action = p->h_action.get(); ga.old_logits = p->h_old.get(); ga.adv = p->h_adv.get(); ga.vt = p->h_vt.get();
     ppo_terms(ga, *cfg);
     if ((rc = launch_states(p, 0, nullptr, 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, 0)) != RAMP_OK) return rc;
-    ramp_ppo_minibatch_stats_kernel<<<1, 1>>>(p->l_row_stats.get(), n, ga.vf_coeff, ga.ent_coeff, ga.kl_coeff, p->l_norm_part.get(), p->l_stats.get());
+    ramp_ppo_minibatch_stats_kernel<<<1, 1>>>(p->L.row_stats.get(), n, ga.vf_coeff, ga.ent_coeff, ga.kl_coeff, p->L.norm_part.get(), p->L.stats.get());
     CUDA_TRY(cudaGetLastError());
-    return host_batch_end(p, grad_out, stats_out, p->l_stats.get(), RAMP_PPO_STATS_LEN);
+    return host_batch_end(p, grad_out, stats_out, p->L.stats.get(), RAMP_PPO_STATS_LEN);
 }
 
 int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, const ramp_ppo_config_t* cfg, double* stats_out) {
@@ -1325,13 +1419,7 @@ int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, con
     int rc = learn_begin(p, eng, cfg, n_steps, "ppo", &eb, &st);
     if (rc != RAMP_OK) return rc;
     const int32_t B = eb.n_episodes, rows = n_steps * B, mb = cfg->sgd_minibatch_size, n_mb = (rows + mb - 1) / mb;
-    if ((rc = prepare_learner(p, st, mb)) || (rc = ensure_batch(p, rows))) return rc;
-    if (B > p->boot_cap) {
-        p->boot_cap = 0;
-        CUDA_TRY(alloc_each(B, p->l_boot, p->l_boot_act));
-        p->boot_cap = B;
-    }
-    if ((size_t)n_mb * RAMP_PPO_STATS_LEN > p->l_mb_stats.size()) CUDA_TRY(p->l_mb_stats.alloc((size_t)n_mb * RAMP_PPO_STATS_LEN));
+    if ((rc = prepare_learner(p, st, mb)) || (rc = ensure_batch(p->L, p->P.c, rows)) || (rc = ensure_ppo(p->L, B, n_mb))) return rc;
     int launches = 2;                                                   // GAE, old logits
     // 1. the value of the state after the last step (RLlib's truncate_episodes bootstrap): when the trajectory goes on, the value
     //    act recorded in slot n_steps; after its last recorded slot, the environment's current state, by the head kernel on its
@@ -1340,36 +1428,36 @@ int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, con
     if (n_steps == p->traj_n) {
         HeadArgs hb{};
         hb.n = B; hb.obs_dyn = eb.obs_dynamic; hb.graph_static = p->d_gstatic.get(); hb.model = eb.queued_model; hb.done = eb.done;
-        hb.mask = eb.action_mask; hb.emb = p->d_emb.get(); hb.value = p->l_boot.get(); hb.actions = p->l_boot_act.get();
+        hb.mask = eb.action_mask; hb.emb = p->d_emb.get(); hb.value = p->L.boot.get(); hb.actions = p->L.boot_act.get();
         if ((rc = launch_head(p, hb, st)) != RAMP_OK) return rc;
-        boot = p->l_boot.get();
+        boot = p->L.boot.get();
         ++launches;
     }
     // 2. GAE, the live rows t-major, standardised advantages
     if ((rc = launch_gae(p, st, n_steps, B, cfg->gamma, cfg->lambda, cfg->standardize_advantages, boot)) != RAMP_OK) return rc;
     // 3. the collection weights' logits of every row: the head kernel again, so they are act's bits
     HeadArgs ho{};
-    ho.n = rows; ho.obs_dyn = p->b_obs.get(); ho.graph_static = p->d_gstatic.get(); ho.model = p->b_model.get(); ho.mask = p->b_mask.get();
-    ho.emb = p->d_emb.get(); ho.logits = p->b_old.get(); ho.value = p->b_value.get(); ho.logp = p->b_lpx.get(); ho.actions = p->b_actx.get();
+    ho.n = rows; ho.obs_dyn = p->L.b_obs.get(); ho.graph_static = p->d_gstatic.get(); ho.model = p->L.b_model.get(); ho.mask = p->L.b_mask.get();
+    ho.emb = p->d_emb.get(); ho.logits = p->L.b_old.get(); ho.value = p->L.b_value.get(); ho.logp = p->L.b_lpx.get(); ho.actions = p->L.b_actx.get();
     if ((rc = launch_head(p, ho, st)) != RAMP_OK) return rc;
     // 4. num_sgd_iter shuffled passes of minibatch updates; a minibatch past the batch's end (its size is on the device) is a no-op
     GradArgs ga{};
-    ga.mb = mb; ga.n_rows = p->l_n_rows.get(); ga.shuffle = 1; ga.obs_dyn = p->b_obs.get(); ga.model = p->b_model.get();
-    ga.mask = p->b_mask.get(); ga.action = p->b_action.get(); ga.old_logits = p->b_old.get(); ga.adv = p->b_adv.get(); ga.vt = p->b_vt.get();
+    ga.mb = mb; ga.n_rows = p->L.n_rows.get(); ga.shuffle = 1; ga.obs_dyn = p->L.b_obs.get(); ga.model = p->L.b_model.get();
+    ga.mask = p->L.b_mask.get(); ga.action = p->L.b_action.get(); ga.old_logits = p->L.b_old.get(); ga.adv = p->L.b_adv.get(); ga.vt = p->L.b_vt.get();
     ppo_terms(ga, *cfg);
-    AdamArgs aa = adam_args(p, *cfg, p->l_n_rows.get(), mb);
-    aa.row_stats = p->l_row_stats.get(); aa.vf_coeff = ga.vf_coeff; aa.ent_coeff = ga.ent_coeff; aa.kl_coeff = ga.kl_coeff;
+    AdamArgs aa = adam_args(p, *cfg, p->L.n_rows.get(), mb);
+    aa.row_stats = p->L.row_stats.get(); aa.vf_coeff = ga.vf_coeff; aa.ent_coeff = ga.ent_coeff; aa.kl_coeff = ga.kl_coeff;
     for (int pass = 0; pass < cfg->num_sgd_iter; ++pass) {
         ga.key = mix64(cfg->seed ^ mix64((uint64_t)pass + 1));
-        ga.logp_old = pass == 0 ? p->b_logp_old.get() : nullptr;
+        ga.logp_old = pass == 0 ? p->L.b_logp_old.get() : nullptr;
         for (int k = 0; k < n_mb; ++k) {
             // the rounds at the current weights, kept for the backward; from the second minibatch on also the embeddings, which
             // the previous update made stale (the first uses those the old logits were computed with)
             ga.start = aa.start = k * mb;
-            if ((rc = launch_states(p, st, p->l_n_rows.get(), ga.start, pass || k ? p->d_emb.get() : nullptr)) != RAMP_OK ||
+            if ((rc = launch_states(p, st, p->L.n_rows.get(), ga.start, pass || k ? p->d_emb.get() : nullptr)) != RAMP_OK ||
                 (rc = launch_grad(p, ga, st)) != RAMP_OK)
                 return rc;
-            aa.stats = p->l_mb_stats.get() + (size_t)k * RAMP_PPO_STATS_LEN;
+            aa.stats = p->L.mb_stats.get() + (size_t)k * RAMP_PPO_STATS_LEN;
             if ((rc = launch_adam(p, aa, st)) != RAMP_OK) return rc;
             launches += 6;
         }
@@ -1377,11 +1465,11 @@ int ramp_policy_learn(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, con
     if (cfg->num_sgd_iter > 0) p->emb_valid = false;
     p->b_rows = rows;
     // 5. the last pass's statistics and the adapted KL coefficient: the call's one read-back
-    ramp_ppo_learn_stats_kernel<<<1, 1, 0, st>>>(p->l_mb_stats.get(), cfg->num_sgd_iter > 0 ? n_mb : 0, (float)cfg->kl_coeff,
-                                                 (float)cfg->kl_target, p->l_n_rows.get(), p->l_stats.get());
+    ramp_ppo_learn_stats_kernel<<<1, 1, 0, st>>>(p->L.mb_stats.get(), cfg->num_sgd_iter > 0 ? n_mb : 0, (float)cfg->kl_coeff,
+                                                 (float)cfg->kl_target, p->L.n_rows.get(), p->L.stats.get());
     CUDA_TRY(cudaGetLastError());
     ramp_internal_count_launches(eng, launches + 1);
-    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, p->l_stats.get(), sizeof(double) * RAMP_PPO_STATS_LEN, cudaMemcpyDeviceToHost, st));
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, p->L.stats.get(), sizeof(double) * RAMP_PPO_STATS_LEN, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     return RAMP_OK;
 }
@@ -1391,15 +1479,15 @@ int ramp_policy_train_batch_read(ramp_policy_t* p, ramp_engine_t* eng, int32_t* 
     if (!p || !eng || !n_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     if (p->b_rows < 1) return set_error(RAMP_ERR_BAD_ARG, "ppo: no train batch (ramp_policy_learn / ramp_policy_learn_pg)");
     cudaStream_t st = ramp_internal_stream(eng);
-    CUDA_TRY(cudaMemcpyAsync(n_out, p->l_n_rows.get(), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(n_out, p->L.n_rows.get(), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     const size_t n = (size_t)*n_out;
-    if (model_out) CUDA_TRY(cudaMemcpyAsync(model_out, p->b_model.get(), 4 * n, cudaMemcpyDeviceToHost, st));
-    if (action_out) CUDA_TRY(cudaMemcpyAsync(action_out, p->b_action.get(), 4 * n, cudaMemcpyDeviceToHost, st));
-    if (logp_out) CUDA_TRY(cudaMemcpyAsync(logp_out, p->b_logp.get(), 4 * n, cudaMemcpyDeviceToHost, st));
-    if (logp_old_out) CUDA_TRY(cudaMemcpyAsync(logp_old_out, p->b_logp_old.get(), 4 * n, cudaMemcpyDeviceToHost, st));
-    if (advantage_out) CUDA_TRY(cudaMemcpyAsync(advantage_out, p->b_adv.get(), 4 * n, cudaMemcpyDeviceToHost, st));
-    if (value_target_out) CUDA_TRY(cudaMemcpyAsync(value_target_out, p->b_vt.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (model_out) CUDA_TRY(cudaMemcpyAsync(model_out, p->L.b_model.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (action_out) CUDA_TRY(cudaMemcpyAsync(action_out, p->L.b_action.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (logp_out) CUDA_TRY(cudaMemcpyAsync(logp_out, p->L.b_logp.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (logp_old_out) CUDA_TRY(cudaMemcpyAsync(logp_old_out, p->L.b_logp_old.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (advantage_out) CUDA_TRY(cudaMemcpyAsync(advantage_out, p->L.b_adv.get(), 4 * n, cudaMemcpyDeviceToHost, st));
+    if (value_target_out) CUDA_TRY(cudaMemcpyAsync(value_target_out, p->L.b_vt.get(), 4 * n, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     return RAMP_OK;
 }
@@ -1407,27 +1495,27 @@ int ramp_policy_train_batch_read(ramp_policy_t* p, ramp_engine_t* eng, int32_t* 
 int ramp_policy_learner_state(ramp_policy_t* p, float* exp_avg_out, float* exp_avg_sq_out, int32_t* step_out) {
     if (!p) return set_error(RAMP_ERR_BAD_ARG, "null policy");
     CUDA_TRY(cudaSetDevice(p->device));
-    if (!p->learner_ready) {
+    if (!p->L.ready) {
         if (exp_avg_out) memset(exp_avg_out, 0, sizeof(float) * p->n_weights);
         if (exp_avg_sq_out) memset(exp_avg_sq_out, 0, sizeof(float) * p->n_weights);
         if (step_out) *step_out = 0;
         return RAMP_OK;
     }
     CUDA_TRY(cudaDeviceSynchronize());                                    // a learn call may still be updating them
-    if (exp_avg_out) CUDA_TRY(cudaMemcpy(exp_avg_out, p->l_adam_m.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
-    if (exp_avg_sq_out) CUDA_TRY(cudaMemcpy(exp_avg_sq_out, p->l_adam_v.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
-    if (step_out) CUDA_TRY(cudaMemcpy(step_out, p->l_step.get() + p->adam_parity, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    if (exp_avg_out) CUDA_TRY(cudaMemcpy(exp_avg_out, p->L.adam_m.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    if (exp_avg_sq_out) CUDA_TRY(cudaMemcpy(exp_avg_sq_out, p->L.adam_v.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToHost));
+    if (step_out) CUDA_TRY(cudaMemcpy(step_out, p->L.step.get() + p->L.parity, sizeof(int32_t), cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
 
 int ramp_policy_learner_reset(ramp_policy_t* p) {
     if (!p) return set_error(RAMP_ERR_BAD_ARG, "null policy");
     CUDA_TRY(cudaSetDevice(p->device));
-    if (!p->learner_ready) return RAMP_OK;
+    if (!p->L.ready) return RAMP_OK;
     CUDA_TRY(cudaDeviceSynchronize());
-    CUDA_TRY(cudaMemset(p->l_adam_m.get(), 0, sizeof(float) * p->n_weights));
-    CUDA_TRY(cudaMemset(p->l_adam_v.get(), 0, sizeof(float) * p->n_weights));
-    CUDA_TRY(cudaMemset(p->l_step.get(), 0, sizeof(int32_t) * 2));
+    CUDA_TRY(cudaMemset(p->L.adam_m.get(), 0, sizeof(float) * p->n_weights));
+    CUDA_TRY(cudaMemset(p->L.adam_v.get(), 0, sizeof(float) * p->n_weights));
+    CUDA_TRY(cudaMemset(p->L.step.get(), 0, sizeof(int32_t) * 2));
     return RAMP_OK;
 }
 
@@ -1542,9 +1630,9 @@ int ramp_pg_loss_grad(ramp_policy_t* p, const ramp_pg_config_t* cfg, int32_t n, 
     GradArgs ga = host_batch_args(p, n);
     ga.pg = 1; ga.action = p->h_action.get(); ga.adv = p->h_adv.get();
     if ((rc = launch_states(p, 0, nullptr, 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, 0)) != RAMP_OK) return rc;
-    ramp_pg_stats_kernel<<<1, 1>>>(p->l_row_stats.get(), p->l_row_model.get(), p->h_adv.get(), n, ga.n_rows, p->l_norm_part.get(), p->l_stats.get());
+    ramp_pg_stats_kernel<<<1, 1>>>(p->L.row_stats.get(), p->L.row_model.get(), p->h_adv.get(), n, ga.n_rows, p->L.norm_part.get(), p->L.stats.get());
     CUDA_TRY(cudaGetLastError());
-    return host_batch_end(p, grad_out, stats_out, p->l_stats.get(), RAMP_PG_STATS_LEN);
+    return host_batch_end(p, grad_out, stats_out, p->L.stats.get(), RAMP_PG_STATS_LEN);
 }
 
 // PG's training step (algorithms/pg: one learn_on_batch per train batch): post_process_advantages (compute_advantages with
@@ -1555,27 +1643,27 @@ int ramp_policy_learn_pg(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, 
     int rc = learn_begin(p, eng, cfg, n_steps, "pg", &eb, &st);
     if (rc != RAMP_OK) return rc;
     const int32_t B = eb.n_episodes, rows = n_steps * B;
-    if ((rc = prepare_learner(p, st, rows)) || (rc = ensure_batch(p, rows))) return rc;
+    if ((rc = prepare_learner(p, st, rows)) || (rc = ensure_batch(p->L, p->P.c, rows))) return rc;
     // 1. the discounted returns (ramp_ppo_gae_kernel without values: lambda 1, V = 0, a 0 bootstrap), the live rows t-major
     if ((rc = launch_gae(p, st, n_steps, B, cfg->gamma, 1.0, 0, nullptr)) != RAMP_OK) return rc;
     // 2. the loss's gradient over the whole batch at the collection weights (the embeddings the trajectory was collected with);
     //    the log p(a) the gradient kernel recomputes goes to b_logp_old
     GradArgs ga{};
-    ga.mb = rows; ga.start = 0; ga.n_rows = p->l_n_rows.get(); ga.shuffle = 0; ga.obs_dyn = p->b_obs.get(); ga.model = p->b_model.get();
-    ga.mask = p->b_mask.get(); ga.action = p->b_action.get(); ga.adv = p->b_adv.get(); ga.pg = 1; ga.logp_old = p->b_logp_old.get();
-    if ((rc = launch_states(p, st, p->l_n_rows.get(), 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, st)) != RAMP_OK) return rc;
+    ga.mb = rows; ga.start = 0; ga.n_rows = p->L.n_rows.get(); ga.shuffle = 0; ga.obs_dyn = p->L.b_obs.get(); ga.model = p->L.b_model.get();
+    ga.mask = p->L.b_mask.get(); ga.action = p->L.b_action.get(); ga.adv = p->L.b_adv.get(); ga.pg = 1; ga.logp_old = p->L.b_logp_old.get();
+    if ((rc = launch_states(p, st, p->L.n_rows.get(), 0, nullptr)) != RAMP_OK || (rc = launch_grad(p, ga, st)) != RAMP_OK) return rc;
     // 3. one Adam step; with no row in the batch, none (the step count stays)
-    AdamArgs aa = adam_args(p, *cfg, p->l_n_rows.get(), rows);
-    aa.stats = p->l_stats.get();                                      // PG's statistics: ramp_pg_stats_kernel, after it
+    AdamArgs aa = adam_args(p, *cfg, p->L.n_rows.get(), rows);
+    aa.stats = p->L.stats.get();                                      // PG's statistics: ramp_pg_stats_kernel, after it
     if ((rc = launch_adam(p, aa, st)) != RAMP_OK) return rc;
     // 4. the statistics: the call's one read-back
-    ramp_pg_stats_kernel<<<1, 1, 0, st>>>(p->l_row_stats.get(), p->l_row_model.get(), p->b_adv.get(), rows, p->l_n_rows.get(),
-                                          p->l_norm_part.get(), p->l_stats.get());
+    ramp_pg_stats_kernel<<<1, 1, 0, st>>>(p->L.row_stats.get(), p->L.row_model.get(), p->L.b_adv.get(), rows, p->L.n_rows.get(),
+                                          p->L.norm_part.get(), p->L.stats.get());
     CUDA_TRY(cudaGetLastError());
     p->emb_valid = false;
     p->b_rows = rows;
     ramp_internal_count_launches(eng, 8);
-    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, p->l_stats.get(), sizeof(double) * RAMP_PG_STATS_LEN, cudaMemcpyDeviceToHost, st));
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, p->L.stats.get(), sizeof(double) * RAMP_PG_STATS_LEN, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     return RAMP_OK;
 }

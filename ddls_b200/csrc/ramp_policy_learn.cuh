@@ -425,9 +425,9 @@ __host__ __device__ inline GnnDims gnn_dims(const ramp_policy_config_t& c) {
     return d;
 }
 
-// ramp_gnn_embed_grad_kernel runs in two launches around the head gradient: EMB_FORWARD runs the MeanPool rounds and keeps every
-// round's states (and writes the embeddings when `emb` is given: ramp_gnn_embed_kernel's arithmetic, the same bits), EMB_BACKWARD
-// runs backward from them.  A forward for a minibatch past the batch's end does nothing: no update ran, the kept states are current.
+// ramp_gnn_embed_grad_kernel runs in two launches around the head gradient: EMB_FORWARD runs the MeanPool rounds (meanpool_round,
+// as every forward does) and keeps every round's states (and writes the embeddings when `emb` is given: node_mean, the same bits
+// as ramp_gnn_embed_kernel's), EMB_BACKWARD runs backward from them.  A forward for a minibatch past the batch's end does nothing: no update ran, the kept states are current.
 enum { EMB_FORWARD = 1, EMB_BACKWARD = 2 };
 struct EmbGradArgs {
     const int32_t* n_rows; int32_t start;                           // forward: the batch's rows (device, or nullptr) and the minibatch
@@ -437,7 +437,8 @@ struct EmbGradArgs {
 };
 
 // ramp_gnn_embed_grad_kernel's statements for job type m with the weight blob `w` (P's layout), by the whole CTA: shared with the
-// population's instances, which run one (weight set, job type) item after another
+// population's instances, which run one (weight set, job type) item after another.  The forward keeps round r's output at stride
+// D.zs in G.z and its module outputs in round r's slices of G.hn / G.he.
 template <int MODE>
 __device__ __forceinline__ void embed_grad_body(const PolicyDev& P, const float* w, const ModelDev* models, const GradModelDev* gms,
                                                 const EmbGradArgs& g, const int m) {
@@ -470,84 +471,14 @@ __device__ __forceinline__ void embed_grad_body(const PolicyDev& P, const float*
     float* buf = s_a[warp];
     float* dp = s_b[warp];
     auto zin_of = [&](int r) { return r == 0 ? M.nf : G.z + (size_t)(r - 1) * N * D.zs; };
-    // ---- forward: ramp_gnn_embed_kernel's rounds, every round's output and module outputs kept ----
-    for (int r = 0; r < c.num_rounds && MODE == EMB_FORWARD; ++r) {
-        const RoundW R = P.rounds[r];
-        const float* zin = zin_of(r);
-        const int zst = r == 0 ? c.in_features_node : D.zs;
-        float* zout = G.z + (size_t)r * N * D.zs;
-        float* hn = G.hn + (size_t)r * N * half;
-        float* he = G.he + (size_t)r * E * half;
-        for (int v = warp; v < N; v += n_warps) {
-            for (int k = lane; k < R.in; k += 32) buf[k] = zin[(size_t)v * zst + k];
-            __syncwarp();
-            warp_layer_norm(buf, R.in, w + R.nln_w, w + R.nln_b, lane);
-            for (int o = lane; o < half; o += 32) {
-                float a = w[R.nb + o];
-                const float* row = w + R.nW + (size_t)o * R.in;
-                for (int k = 0; k < R.in; ++k) a += row[k] * buf[k];
-                hn[(size_t)v * half + o] = act_fn(a, ak);
-            }
-            __syncwarp();
-        }
-        for (int e = warp; e < E; e += n_warps) {
-            for (int k = lane; k < ine; k += 32) buf[k] = M.ef[(size_t)e * ine + k];
-            __syncwarp();
-            warp_layer_norm(buf, ine, w + R.eln_w, w + R.eln_b, lane);
-            for (int o = lane; o < half; o += 32) {
-                float a = w[R.eb + o];
-                const float* row = w + R.eW + (size_t)o * ine;
-                for (int k = 0; k < ine; ++k) a += row[k] * buf[k];
-                he[(size_t)e * half + o] = act_fn(a, ak);
-            }
-            __syncwarp();
-        }
-        __syncthreads();
-        for (int v = warp; v < N; v += n_warps) {
-            const int e0 = M.in_ptr[v], e1 = M.in_ptr[v + 1];
-            float acc[POL_MAX_DIM / 32];
-#pragma unroll
-            for (int q = 0; q < POL_MAX_DIM / 32; ++q) acc[q] = 0.f;
-            if (e1 > e0) {
-                for (int mi = -1; mi < e1 - e0; ++mi) {
-                    const int src = mi < 0 ? v : M.in_src[e0 + mi];
-                    for (int k = lane; k < half; k += 32) {
-                        buf[k] = hn[(size_t)src * half + k];
-                        buf[half + k] = mi < 0 ? 0.f : he[(size_t)M.in_edge[e0 + mi] * half + k];
-                    }
-                    __syncwarp();
-                    warp_layer_norm(buf, msg, w + R.rln_w, w + R.rln_b, lane);
-#pragma unroll
-                    for (int q = 0; q < POL_MAX_DIM / 32; ++q) {
-                        const int o = lane + 32 * q;
-                        if (o < R.out) {
-                            float a = w[R.rb + o];
-                            const float* row = w + R.rW + (size_t)o * msg;
-                            for (int k = 0; k < msg; ++k) a += row[k] * buf[k];
-                            acc[q] += act_fn(a, ak);
-                        }
-                    }
-                    __syncwarp();
-                }
-            }
-            const float inv = 1.0f / (float)(e1 - e0 + 1);
-#pragma unroll
-            for (int q = 0; q < POL_MAX_DIM / 32; ++q) {
-                const int o = lane + 32 * q;
-                if (o < R.out) zout[(size_t)v * D.zs + o] = acc[q] * inv;
-            }
-        }
-        __syncthreads();
-    }
+    // ---- forward: the MeanPool rounds, every round's output and module outputs kept ----
     if (MODE == EMB_FORWARD) {
-        if (g.emb) {                                                // the mean over the job's nodes, as ramp_gnn_embed_kernel takes it
-            const float* zl = zin_of(c.num_rounds);
-            for (int o = threadIdx.x; o < on; o += blockDim.x) {
-                float s = 0.f;
-                for (int v = 0; v < N; ++v) s += zl[(size_t)v * D.zs + o];
-                g.emb[(size_t)m * on + o] = s / (float)N;
-            }
+        for (int r = 0; r < c.num_rounds; ++r) {
+            const RoundW R = P.rounds[r];
+            meanpool_round(P, w, R, M, zin_of(r), r == 0 ? c.in_features_node : D.zs, G.z + (size_t)r * N * D.zs, D.zs,
+                           G.hn + (size_t)r * N * half, G.he + (size_t)r * E * half, buf);
         }
+        if (g.emb) node_mean(zin_of(c.num_rounds), D.zs, N, on, g.emb + (size_t)m * on);
         return;
     }
     // ---- backward: d of the last round's output is d emb / n_nodes at every node (the node mean) ----

@@ -137,17 +137,8 @@ struct ramp_population {
     unsigned long long act_calls = 0;
     DeviceArray<unsigned long long> d_seeds, d_keys;
     std::vector<DeviceArray<unsigned char>> gallocs;     // every (set, job type)'s MeanPool states and backward scratch
-    DeviceArray<GradModelDev> d_gms;      // [K][n_models]
-    bool gms_ready = false;
-    // the learner: per set what ramp_policy keeps for one, stacked set-major
-    bool learner_ready = false;
-    int32_t parity = 0, lcap = 0, bcap = 0, boot_cap = 0;
-    DeviceArray<float> l_grad, l_m, l_v, l_gpart, l_rec, l_row_stats, l_boot, d_kl;
-    DeviceArray<int32_t> l_step, l_n_rows, l_row_model, l_boot_act;
-    DeviceArray<double> l_norm_part, l_stats, l_mb_stats;
-    std::map<int32_t, ramp_policy::SegTable> seg_tables;
-    DeviceArray<float> b_obs, b_logp, b_logp_old, b_adv, b_vt, b_old, b_value, b_lpx;
-    DeviceArray<int32_t> b_model, b_action, b_actx; DeviceArray<uint8_t> b_mask; DeviceArray<double> b_adv64;
+    LearnerBuffers L;                     // the learner: what ramp_policy keeps for one set, for K
+    DeviceArray<float> d_kl;              // [K][2]: kl_coeff, kl_target
     DeviceArray<GaeArgs> d_gae; DeviceArray<GradArgs> d_grad; DeviceArray<AdamArgs> d_adam;
 };
 
@@ -160,8 +151,8 @@ int pop_check_set(const ramp_population* q, int32_t set) {
 }
 
 // every (set, job type)'s forward states and backward scratch; the job types' out-edge CSR is the template's
-int pop_ensure_gms(ramp_population* q) {
-    if (q->gms_ready) return RAMP_OK;
+int pop_ensure_gms(ramp_population* q, cudaStream_t st) {
+    if (q->L.gmodels_ready) return RAMP_OK;
     ramp_policy* p = q->p;
     const int nm = p->P.c.n_models;
     std::vector<GradModelDev> h((size_t)q->K * nm);
@@ -176,10 +167,7 @@ int pop_ensure_gms(ramp_population* q) {
             if (rc != RAMP_OK) return rc;
         }
     }
-    CUDA_TRY(q->d_gms.alloc(h.size()));
-    CUDA_TRY(cudaMemcpy(q->d_gms.get(), h.data(), sizeof(GradModelDev) * h.size(), cudaMemcpyHostToDevice));
-    q->gms_ready = true;
-    return RAMP_OK;
+    return upload_gmodels(q->L, h, st);
 }
 
 int pop_launch_embed(ramp_population* q, cudaStream_t st, EmbGradArgs eg, bool forward) {
@@ -188,8 +176,8 @@ int pop_launch_embed(ramp_population* q, cudaStream_t st, EmbGradArgs eg, bool f
     pe.K = q->K; pe.n_weights = q->nw; pe.rec_stride = head_rec(p->P.c).stride;
     PolicyDev P = p->P;
     P.w = q->d_w.get();
-    if (forward) ramp_pop_embed_grad_kernel<EMB_FORWARD><<<q->embed_ctas, 256, 0, st>>>(P, p->d_models.get(), q->d_gms.get(), eg, pe);
-    else ramp_pop_embed_grad_kernel<EMB_BACKWARD><<<q->embed_ctas, 256, 0, st>>>(P, p->d_models.get(), q->d_gms.get(), eg, pe);
+    if (forward) ramp_pop_embed_grad_kernel<EMB_FORWARD><<<q->embed_ctas, 256, 0, st>>>(P, p->d_models.get(), q->L.gmodels.get(), eg, pe);
+    else ramp_pop_embed_grad_kernel<EMB_BACKWARD><<<q->embed_ctas, 256, 0, st>>>(P, p->d_models.get(), q->L.gmodels.get(), eg, pe);
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
 }
@@ -197,7 +185,7 @@ int pop_launch_embed(ramp_population* q, cudaStream_t st, EmbGradArgs eg, bool f
 // the embeddings of every set at its current weights (the single policy's act re-embeds the same way when they are stale)
 int pop_embed(ramp_population* q, cudaStream_t st) {
     int rc;
-    if ((rc = pop_ensure_gms(q)) != RAMP_OK) return rc;
+    if ((rc = pop_ensure_gms(q, st)) != RAMP_OK) return rc;
     EmbGradArgs eg{};
     eg.emb = q->d_emb.get();
     if ((rc = pop_launch_embed(q, st, eg, true)) != RAMP_OK) return rc;
@@ -220,65 +208,15 @@ int pop_launch_head(ramp_population* q, const HeadArgs& a, int32_t per, const un
     return RAMP_OK;
 }
 
+// the learner's buffers, and the per-set arguments of the population's kernels
 int pop_ensure_learner(ramp_population* q) {
-    if (q->learner_ready) return RAMP_OK;
-    ramp_policy* p = q->p;
-    const size_t n = (size_t)q->K * q->nw, K = q->K;
-    CUDA_TRY(alloc_each(n, q->l_grad, q->l_m, q->l_v));
-    CUDA_TRY(q->l_gpart.alloc(K * p->P.c.n_models * gnn_weight_count(p)));
-    CUDA_TRY(q->l_step.alloc(2 * K));
-    CUDA_TRY(q->l_n_rows.alloc(K));
-    CUDA_TRY(q->l_norm_part.alloc(K * LRN_GRID));
-    CUDA_TRY(q->l_stats.alloc(K * RAMP_PPO_STATS_LEN));
+    if (q->L.ready) return RAMP_OK;
+    const size_t K = q->K;
     CUDA_TRY(q->d_kl.alloc(2 * K));
     CUDA_TRY(q->d_gae.alloc(K));
     CUDA_TRY(q->d_grad.alloc(K));
     CUDA_TRY(q->d_adam.alloc(K));
-    CUDA_TRY(cudaMemset(q->l_m.get(), 0, sizeof(float) * n));
-    CUDA_TRY(cudaMemset(q->l_v.get(), 0, sizeof(float) * n));
-    CUDA_TRY(cudaMemset(q->l_step.get(), 0, sizeof(int32_t) * 2 * K));
-    q->parity = 0;
-    q->learner_ready = true;
-    return RAMP_OK;
-}
-
-// per-row scratch for K minibatches of mb rows, and the head segments of set 0's mb records
-int pop_ensure_rows(ramp_population* q, int32_t mb, cudaStream_t st, const ramp_policy::SegTable** segs) {
-    const ramp_policy_config_t& c = q->p->P.c;
-    const size_t n = (size_t)q->K * mb;
-    if (mb > q->lcap) {
-        q->lcap = 0;
-        q->seg_tables.clear();
-        CUDA_TRY(q->l_rec.alloc(n * head_rec(c).stride));
-        CUDA_TRY(q->l_row_stats.alloc(n * RS_N));
-        CUDA_TRY(q->l_row_model.alloc(n));
-        q->lcap = mb;
-    }
-    auto it = q->seg_tables.find(mb);
-    if (it == q->seg_tables.end()) {
-        Seg s[HEAD_SEGS];
-        ramp_policy::SegTable t;
-        t.count = head_segs(q->p->P, q->l_rec.get(), mb, s);
-        for (int k = 0; k < t.count; ++k) t.total += seg_size(s[k]);
-        CUDA_TRY(t.d.alloc(HEAD_SEGS));
-        CUDA_TRY(cudaMemcpyAsync(t.d.get(), s, sizeof(s), cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaStreamSynchronize(st));                              // `s` is pageable
-        it = q->seg_tables.emplace(mb, std::move(t)).first;
-    }
-    *segs = &it->second;
-    return RAMP_OK;
-}
-
-// the train batch for K groups of `rows` trajectory slots each
-int pop_ensure_batch(ramp_population* q, int32_t rows) {
-    if (rows <= q->bcap) return RAMP_OK;
-    const size_t n = (size_t)q->K * rows;
-    q->bcap = 0;
-    CUDA_TRY(alloc_each(n, q->b_logp, q->b_logp_old, q->b_adv, q->b_vt, q->b_value, q->b_lpx, q->b_model, q->b_action, q->b_actx, q->b_adv64));
-    CUDA_TRY(q->b_obs.alloc(n * 11));
-    CUDA_TRY(alloc_each(n * q->p->P.c.n_actions, q->b_mask, q->b_old));
-    q->bcap = rows;
-    return RAMP_OK;
+    return ensure_learner(q->L, q->p);
 }
 
 }  // namespace
@@ -291,7 +229,7 @@ int ramp_population_create(ramp_policy_t* p, int32_t n_sets, ramp_population_t**
     if (!p->weights_set) return set_error(RAMP_ERR_BAD_ARG, "policy: no weights (ramp_policy_set_weights)");
     CUDA_TRY(cudaSetDevice(p->device));
     std::unique_ptr<ramp_population> q(new ramp_population());
-    q->p = p; q->K = n_sets; q->nw = p->n_weights;
+    q->p = p; q->K = q->L.K = n_sets; q->nw = p->n_weights;
     const ramp_policy_config_t& c = p->P.c;
     int per_sm = 0;
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ramp_pop_embed_grad_kernel<EMB_BACKWARD>, 256, 0));
@@ -390,17 +328,11 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
     const int32_t B = eb.n_episodes, b = B / K, rows = n_steps * b, mb = cfgs[0].sgd_minibatch_size, n_mb = (rows + mb - 1) / mb;
     const int32_t n_pass = cfgs[0].num_sgd_iter, A = c.n_actions, on = c.out_features_node, nm = c.n_models;
     const size_t R = rows;
-    const ramp_policy::SegTable* segs = nullptr;
-    if ((rc = fence_in(p, st)) || (rc = pop_ensure_learner(q)) || (rc = pop_ensure_gms(q)) || (rc = pop_ensure_rows(q, mb, st, &segs)) ||
-        (rc = pop_ensure_batch(q, rows)))
+    if ((rc = fence_in(p, st)) || (rc = pop_ensure_learner(q)) || (rc = pop_ensure_gms(q, st)) || (rc = ensure_rows(q->L, p->P, mb, st)) ||
+        (rc = ensure_batch(q->L, c, rows)) || (rc = ensure_ppo(q->L, B, n_mb)))
         return rc;
     if (!q->emb_valid && (rc = pop_embed(q, st)) != RAMP_OK) return rc;
-    if (B > q->boot_cap) {
-        q->boot_cap = 0;
-        CUDA_TRY(alloc_each(B, q->l_boot, q->l_boot_act));
-        q->boot_cap = B;
-    }
-    if ((size_t)K * n_mb * RAMP_PPO_STATS_LEN > q->l_mb_stats.size()) CUDA_TRY(q->l_mb_stats.alloc((size_t)K * n_mb * RAMP_PPO_STATS_LEN));
+    const SegTable* segs = q->L.segs;
     if ((size_t)K * std::max(n_pass, 1) > q->d_keys.size()) CUDA_TRY(q->d_keys.alloc((size_t)K * std::max(n_pass, 1)));
     // every group's arguments: set s's slices of the trajectory's columns, the train batch, the scratch and the learner state
     const HeadRec HR = head_rec(c);
@@ -410,7 +342,7 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
     std::vector<float> kl(2 * K);
     std::vector<unsigned long long> keys((size_t)K * std::max(n_pass, 1));
     const float* boot = p->t_value.get() + (size_t)n_steps * B;
-    if (n_steps == p->traj_n) boot = q->l_boot.get();
+    if (n_steps == p->traj_n) boot = q->L.boot.get();
     for (int s = 0; s < K; ++s) {
         const ramp_ppo_config_t& cfg = cfgs[s];
         const size_t col = (size_t)s * b, r0 = (size_t)s * R, q0 = (size_t)s * mb;
@@ -420,22 +352,22 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
         ge.t_obs = p->t_obs.get() + col * 11; ge.t_model = p->t_model.get() + col; ge.t_mask = p->t_mask.get() + col * A;
         ge.t_action = p->t_action.get() + col; ge.t_logp = p->t_logp.get() + col; ge.t_value = p->t_value.get() + col;
         ge.t_reward = p->t_reward.get() + col; ge.t_done = p->t_done.get() + col;
-        ge.boot = boot + col; ge.adv64 = q->b_adv64.get() + col;
-        ge.obs = q->b_obs.get() + r0 * 11; ge.model = q->b_model.get() + r0; ge.mask = q->b_mask.get() + r0 * A; ge.action = q->b_action.get() + r0;
-        ge.logp = q->b_logp.get() + r0; ge.adv = q->b_adv.get() + r0; ge.vt = q->b_vt.get() + r0; ge.n_rows = q->l_n_rows.get() + s;
+        ge.boot = boot + col; ge.adv64 = q->L.b_adv64.get() + col;
+        ge.obs = q->L.b_obs.get() + r0 * 11; ge.model = q->L.b_model.get() + r0; ge.mask = q->L.b_mask.get() + r0 * A; ge.action = q->L.b_action.get() + r0;
+        ge.logp = q->L.b_logp.get() + r0; ge.adv = q->L.b_adv.get() + r0; ge.vt = q->L.b_vt.get() + r0; ge.n_rows = q->L.n_rows.get() + s;
         GradArgs& ga = grad[s];
-        ga.mb = mb; ga.n_rows = q->l_n_rows.get() + s; ga.shuffle = 1; ga.obs_dyn = q->b_obs.get() + r0 * 11; ga.model = q->b_model.get() + r0;
-        ga.mask = q->b_mask.get() + r0 * A; ga.action = q->b_action.get() + r0; ga.old_logits = q->b_old.get() + r0 * A;
-        ga.adv = q->b_adv.get() + r0; ga.vt = q->b_vt.get() + r0; ga.graph_static = p->d_gstatic.get(); ga.emb = q->d_emb.get() + (size_t)s * nm * on;
-        ga.rec = q->l_rec.get() + q0 * HR.stride; ga.row_model = q->l_row_model.get() + q0; ga.row_stats = q->l_row_stats.get() + q0 * RS_N;
-        ga.logp_old = q->b_logp_old.get() + r0;
+        ga.mb = mb; ga.n_rows = q->L.n_rows.get() + s; ga.shuffle = 1; ga.obs_dyn = q->L.b_obs.get() + r0 * 11; ga.model = q->L.b_model.get() + r0;
+        ga.mask = q->L.b_mask.get() + r0 * A; ga.action = q->L.b_action.get() + r0; ga.old_logits = q->L.b_old.get() + r0 * A;
+        ga.adv = q->L.b_adv.get() + r0; ga.vt = q->L.b_vt.get() + r0; ga.graph_static = p->d_gstatic.get(); ga.emb = q->d_emb.get() + (size_t)s * nm * on;
+        ga.rec = q->L.rec.get() + q0 * HR.stride; ga.row_model = q->L.row_model.get() + q0; ga.row_stats = q->L.row_stats.get() + q0 * RS_N;
+        ga.logp_old = q->L.b_logp_old.get() + r0;
         ppo_terms(ga, cfg);
         AdamArgs& aa = adam[s];
-        aa = adam_args(p, cfg, q->l_n_rows.get() + s, mb);
-        aa.step = q->l_step.get() + 2 * s; aa.m = q->l_m.get() + (size_t)s * q->nw; aa.v = q->l_v.get() + (size_t)s * q->nw;
-        aa.grad = q->l_grad.get() + (size_t)s * q->nw; aa.norm_part = q->l_norm_part.get() + (size_t)s * LRN_GRID; aa.w = q->d_w.get() + (size_t)s * q->nw;
+        aa = adam_args(p, cfg, q->L.n_rows.get() + s, mb);
+        aa.step = q->L.step.get() + 2 * s; aa.m = q->L.adam_m.get() + (size_t)s * q->nw; aa.v = q->L.adam_v.get() + (size_t)s * q->nw;
+        aa.grad = q->L.grad.get() + (size_t)s * q->nw; aa.norm_part = q->L.norm_part.get() + (size_t)s * LRN_GRID; aa.w = q->d_w.get() + (size_t)s * q->nw;
         aa.row_stats = ga.row_stats; aa.vf_coeff = ga.vf_coeff; aa.ent_coeff = ga.ent_coeff; aa.kl_coeff = ga.kl_coeff;
-        aa.stats = q->l_mb_stats.get() + (size_t)s * n_mb * RAMP_PPO_STATS_LEN;
+        aa.stats = q->L.mb_stats.get() + (size_t)s * n_mb * RAMP_PPO_STATS_LEN;
         kl[2 * s] = (float)cfg.kl_coeff; kl[2 * s + 1] = (float)cfg.kl_target;
         for (int pass = 0; pass < n_pass; ++pass) keys[(size_t)pass * K + s] = mix64(cfg.seed ^ mix64((uint64_t)pass + 1));
     }
@@ -452,7 +384,7 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
     if (n_steps == p->traj_n) {
         HeadArgs hb{};
         hb.obs_dyn = eb.obs_dynamic; hb.graph_static = p->d_gstatic.get(); hb.model = eb.queued_model; hb.done = eb.done;
-        hb.mask = eb.action_mask; hb.emb = q->d_emb.get(); hb.value = q->l_boot.get(); hb.actions = q->l_boot_act.get();
+        hb.mask = eb.action_mask; hb.emb = q->d_emb.get(); hb.value = q->L.boot.get(); hb.actions = q->L.boot_act.get();
         if ((rc = pop_launch_head(q, hb, b, nullptr, 0, st)) != RAMP_OK) return rc;
         ++launches;
     }
@@ -461,8 +393,8 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
     CUDA_TRY(cudaGetLastError());
     // 3. the collection weights' logits of every row
     HeadArgs ho{};
-    ho.obs_dyn = q->b_obs.get(); ho.graph_static = p->d_gstatic.get(); ho.model = q->b_model.get(); ho.mask = q->b_mask.get();
-    ho.emb = q->d_emb.get(); ho.logits = q->b_old.get(); ho.value = q->b_value.get(); ho.logp = q->b_lpx.get(); ho.actions = q->b_actx.get();
+    ho.obs_dyn = q->L.b_obs.get(); ho.graph_static = p->d_gstatic.get(); ho.model = q->L.b_model.get(); ho.mask = q->L.b_mask.get();
+    ho.emb = q->d_emb.get(); ho.logits = q->L.b_old.get(); ho.value = q->L.b_value.get(); ho.logp = q->L.b_lpx.get(); ho.actions = q->L.b_actx.get();
     if ((rc = pop_launch_head(q, ho, rows, nullptr, 0, st)) != RAMP_OK) return rc;
     // 4. minibatch j of every group in the same launches
     int64_t rgrid = (K * segs->total + 255) / 256;
@@ -471,30 +403,30 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
         for (int j = 0; j < n_mb; ++j) {
             const int32_t start = j * mb;
             EmbGradArgs ef{};
-            ef.n_rows = q->l_n_rows.get(); ef.start = start; ef.emb = pass || j ? q->d_emb.get() : nullptr;
+            ef.n_rows = q->L.n_rows.get(); ef.start = start; ef.emb = pass || j ? q->d_emb.get() : nullptr;
             if ((rc = pop_launch_embed(q, st, ef, true)) != RAMP_OK) return rc;
             ramp_pop_head_grad_kernel<<<(K * mb + LRN_WARPS - 1) / LRN_WARPS, LRN_WARPS * 32, 0, st>>>(
                 P, q->d_grad.get(), K, mb, start, q->d_keys.get() + (size_t)pass * K, pass == 0, q->nw);
             ramp_pop_head_reduce_kernel<<<(unsigned)rgrid, 256, 0, st>>>(P, segs->d.get(), segs->count, segs->total, K,
-                                                                         (int64_t)mb * HR.stride, q->nw, q->l_grad.get());
+                                                                         (int64_t)mb * HR.stride, q->nw, q->L.grad.get());
             EmbGradArgs eb2{};
-            eb2.rec = q->l_rec.get(); eb2.row_model = q->l_row_model.get(); eb2.rows = mb; eb2.gpart = q->l_gpart.get(); eb2.n_gnn = gnn_weight_count(p);
+            eb2.rec = q->L.rec.get(); eb2.row_model = q->L.row_model.get(); eb2.rows = mb; eb2.gpart = q->L.gpart.get(); eb2.n_gnn = gnn_weight_count(p);
             if ((rc = pop_launch_embed(q, st, eb2, false)) != RAMP_OK) return rc;
-            ramp_pop_finish_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->l_gpart.get(), nm, gnn_weight_count(p), q->nw, q->l_grad.get(),
-                                                                      q->l_norm_part.get());
-            ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_adam.get(), start, j, q->parity, q->nw);
-            q->parity ^= 1;
+            ramp_pop_finish_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->L.gpart.get(), nm, gnn_weight_count(p), q->nw, q->L.grad.get(),
+                                                                      q->L.norm_part.get());
+            ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_adam.get(), start, j, q->L.parity, q->nw);
+            q->L.parity ^= 1;
             CUDA_TRY(cudaGetLastError());
             launches += 6;
         }
     }
     if (n_pass > 0) q->emb_valid = false;
     // 5. every set's last-pass statistics and adapted KL coefficient: the call's one read-back
-    ramp_pop_learn_stats_kernel<<<(K + 127) / 128, 128, 0, st>>>(q->l_mb_stats.get(), n_mb, n_pass > 0 ? n_mb : 0, q->d_kl.get(),
-                                                                q->l_n_rows.get(), q->l_stats.get(), K);
+    ramp_pop_learn_stats_kernel<<<(K + 127) / 128, 128, 0, st>>>(q->L.mb_stats.get(), n_mb, n_pass > 0 ? n_mb : 0, q->d_kl.get(),
+                                                                q->L.n_rows.get(), q->L.stats.get(), K);
     CUDA_TRY(cudaGetLastError());
     ramp_internal_count_launches(eng, launches + 1);
-    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, q->l_stats.get(), sizeof(double) * K * RAMP_PPO_STATS_LEN, cudaMemcpyDeviceToHost, st));
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, q->L.stats.get(), sizeof(double) * K * RAMP_PPO_STATS_LEN, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     return fence_out(p, st);
 }
@@ -504,16 +436,16 @@ int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_
     if (rc != RAMP_OK) return rc;
     CUDA_TRY(cudaSetDevice(q->p->device));
     const size_t n = q->nw;
-    if (!q->learner_ready) {
+    if (!q->L.ready) {
         if (exp_avg_out) memset(exp_avg_out, 0, sizeof(float) * n);
         if (exp_avg_sq_out) memset(exp_avg_sq_out, 0, sizeof(float) * n);
         if (step_out) *step_out = 0;
         return RAMP_OK;
     }
     CUDA_TRY(cudaDeviceSynchronize());                                    // a learn call may still be updating them
-    if (exp_avg_out) CUDA_TRY(cudaMemcpy(exp_avg_out, q->l_m.get() + (size_t)set * n, sizeof(float) * n, cudaMemcpyDeviceToHost));
-    if (exp_avg_sq_out) CUDA_TRY(cudaMemcpy(exp_avg_sq_out, q->l_v.get() + (size_t)set * n, sizeof(float) * n, cudaMemcpyDeviceToHost));
-    if (step_out) CUDA_TRY(cudaMemcpy(step_out, q->l_step.get() + 2 * set + q->parity, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    if (exp_avg_out) CUDA_TRY(cudaMemcpy(exp_avg_out, q->L.adam_m.get() + (size_t)set * n, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    if (exp_avg_sq_out) CUDA_TRY(cudaMemcpy(exp_avg_sq_out, q->L.adam_v.get() + (size_t)set * n, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    if (step_out) CUDA_TRY(cudaMemcpy(step_out, q->L.step.get() + 2 * set + q->L.parity, sizeof(int32_t), cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
 
