@@ -494,6 +494,13 @@ struct LearnerBuffers {
     int32_t bcap = 0, boot_cap = 0;
     DeviceArray<float> b_obs, b_logp, b_logp_old, b_adv, b_vt, b_old, b_value, b_lpx, boot;
     DeviceArray<int32_t> b_model, b_action, b_actx, boot_act; DeviceArray<uint8_t> b_mask; DeviceArray<double> b_adv64;
+    // IMPALA (ramp_policy_learn_impala / ramp_impala_loss_grad / ramp_population_learn_impala): K groups of fragment rows ([icap]
+    // each, set s's i_rows rows at s i_rows, row f L + t) with their read-out at the current weights and V-trace values, the loss's
+    // job types (-1 outside it), the host batch's extra inputs; per set the row count, the statistics and each SGD step's
+    int32_t icap = 0, i_rows = 0, i_step_cap = 0;
+    DeviceArray<float> i_obs, i_blogp, i_tlogits, i_tvalue, i_tlogp, i_log_rho, i_vs, i_pg;
+    DeviceArray<int32_t> i_model, i_action, i_actx, i_lmodel, i_n_rows; DeviceArray<uint8_t> i_mask, i_done;
+    DeviceArray<double> i_reward, i_step_stats, i_stats;
 };
 
 struct ramp_policy {
@@ -531,12 +538,6 @@ struct ramp_policy {
     int32_t hcap = 0;
     DeviceArray<int32_t> h_model, h_action, h_n_rows; DeviceArray<float> h_gf, h_gl, h_gv, h_old, h_adv, h_vt; DeviceArray<uint8_t> h_mask;
     int32_t b_rows = 0;                   // the rows of the last train batch (ramp_policy_train_batch_read)
-    // IMPALA (ramp_policy_learn_impala / ramp_impala_loss_grad): the fragment rows ([icap], row f L + t) with their read-out at
-    // the current weights and V-trace values, the loss's job types (-1 outside it), the host batch's extra inputs, statistics
-    int32_t icap = 0, i_rows = 0, i_step_cap = 0;
-    DeviceArray<float> i_obs, i_blogp, i_tlogits, i_tvalue, i_tlogp, i_log_rho, i_vs, i_pg;
-    DeviceArray<int32_t> i_model, i_action, i_actx, i_lmodel, i_n_rows; DeviceArray<uint8_t> i_mask, i_done;
-    DeviceArray<double> i_reward, i_step_stats, i_stats;
 };
 
 namespace {
@@ -1017,25 +1018,25 @@ int host_batch_end(ramp_policy* p, float* grad_out, double* stats_out, const dou
     return RAMP_OK;
 }
 
-// IMPALA's per-row arrays for n fragment rows, and statistics for `steps` SGD steps
-int ensure_impala(ramp_policy* p, int32_t n, int32_t steps) {
-    const size_t A = p->P.c.n_actions;
-    if (n > p->icap) {
-        p->icap = 0;
-        CUDA_TRY(alloc_each(n, p->i_blogp, p->i_tvalue, p->i_tlogp, p->i_log_rho, p->i_vs, p->i_pg, p->i_model, p->i_action,
-                            p->i_actx, p->i_lmodel, p->i_done, p->i_reward));
-        CUDA_TRY(p->i_obs.alloc((size_t)n * 11));
-        CUDA_TRY(alloc_each((size_t)n * A, p->i_tlogits, p->i_mask));
-        p->icap = n;
+// IMPALA's per-row arrays for K groups of n fragment rows, and statistics for `steps` SGD steps of K sets
+int ensure_impala(LearnerBuffers& L, const ramp_policy_config_t& c, int32_t n, int32_t steps) {
+    const size_t K = L.K, A = c.n_actions;
+    if (n > L.icap) {
+        L.icap = 0;
+        CUDA_TRY(alloc_each(K * n, L.i_blogp, L.i_tvalue, L.i_tlogp, L.i_log_rho, L.i_vs, L.i_pg, L.i_model, L.i_action,
+                            L.i_actx, L.i_lmodel, L.i_done, L.i_reward));
+        CUDA_TRY(L.i_obs.alloc(K * n * 11));
+        CUDA_TRY(alloc_each(K * n * A, L.i_tlogits, L.i_mask));
+        L.icap = n;
     }
-    if (!p->i_n_rows.get()) {
-        CUDA_TRY(p->i_n_rows.alloc(1));
-        CUDA_TRY(p->i_stats.alloc(RAMP_IMPALA_STATS_LEN));
+    if (!L.i_n_rows.get()) {
+        CUDA_TRY(L.i_n_rows.alloc(K));
+        CUDA_TRY(L.i_stats.alloc(K * RAMP_IMPALA_STATS_LEN));
     }
-    if (steps > p->i_step_cap) {
-        p->i_step_cap = 0;
-        CUDA_TRY(p->i_step_stats.alloc((size_t)steps * RAMP_IMPALA_STATS_LEN));
-        p->i_step_cap = steps;
+    if (steps > L.i_step_cap) {
+        L.i_step_cap = 0;
+        CUDA_TRY(L.i_step_stats.alloc(K * steps * RAMP_IMPALA_STATS_LEN));
+        L.i_step_cap = steps;
     }
     return RAMP_OK;
 }
@@ -1054,21 +1055,21 @@ int impala_batch(ramp_policy* p, cudaStream_t st, const ramp_impala_config_t& cf
     h.n = n_frag * L; h.graph_features = graph_features ? graph_features + r0 * c.in_features_graph : nullptr;
     h.obs_dyn = obs_dyn ? obs_dyn + r0 * 11 : nullptr; h.graph_static = p->d_gstatic.get();
     h.model = model + r0; h.mask = mask + r0 * A; h.emb = p->d_emb.get();
-    h.logits = p->i_tlogits.get() + r0 * A; h.value = p->i_tvalue.get() + r0; h.actions = p->i_actx.get() + r0;
+    h.logits = p->L.i_tlogits.get() + r0 * A; h.value = p->L.i_tvalue.get() + r0; h.actions = p->L.i_actx.get() + r0;
     if ((rc = launch_head(p, h, st)) != RAMP_OK) return rc;
     VtraceArgs v{};
     v.L = L; v.n_frag = n_frag; v.row0 = row0; v.A = c.n_actions; v.n_models = c.n_models;
     v.gamma = cfg.gamma; v.clip_rho = cfg.vtrace_clip_rho_threshold; v.clip_pg_rho = cfg.vtrace_clip_pg_rho_threshold;
-    v.logits = p->i_tlogits.get(); v.value = p->i_tvalue.get();
+    v.logits = p->L.i_tlogits.get(); v.value = p->L.i_tvalue.get();
     v.model = model; v.action = action; v.blogp = blogp; v.reward = reward; v.done = done;
-    v.tlogp = p->i_tlogp.get(); v.log_rho = p->i_log_rho.get(); v.vs = p->i_vs.get(); v.pg_adv = p->i_pg.get(); v.lmodel = p->i_lmodel.get();
+    v.tlogp = p->L.i_tlogp.get(); v.log_rho = p->L.i_log_rho.get(); v.vs = p->L.i_vs.get(); v.pg_adv = p->L.i_pg.get(); v.lmodel = p->L.i_lmodel.get();
     ramp_vtrace_kernel<<<(unsigned)((n_frag + 7) / 8), 256, 0, st>>>(v);
     CUDA_TRY(cudaGetLastError());
-    ga.impala = 1; ga.shuffle = 0; ga.graph_features = graph_features; ga.obs_dyn = obs_dyn; ga.model = p->i_lmodel.get(); ga.mask = mask;
-    ga.action = action; ga.adv = p->i_pg.get(); ga.vt = p->i_vs.get();
+    ga.impala = 1; ga.shuffle = 0; ga.graph_features = graph_features; ga.obs_dyn = obs_dyn; ga.model = p->L.i_lmodel.get(); ga.mask = mask;
+    ga.action = action; ga.adv = p->L.i_pg.get(); ga.vt = p->L.i_vs.get();
     ga.vf_coeff = (float)cfg.vf_loss_coeff; ga.ent_coeff = (float)cfg.entropy_coeff;
     if ((rc = launch_grad(p, ga, st)) != RAMP_OK) return rc;
-    ramp_impala_step_stats_kernel<<<1, 1, 0, st>>>(p->L.row_stats.get(), p->L.row_model.get(), ga.mb, row0, p->i_log_rho.get(),
+    ramp_impala_step_stats_kernel<<<1, 1, 0, st>>>(p->L.row_stats.get(), p->L.row_model.get(), ga.mb, row0, p->L.i_log_rho.get(),
                                                    cfg.vf_loss_coeff, cfg.entropy_coeff, p->L.norm_part.get(), stats);
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
@@ -1531,23 +1532,23 @@ int ramp_impala_loss_grad(ramp_policy_t* p, const ramp_impala_config_t* cfg, int
         return set_error(RAMP_ERR_BAD_ARG, "impala: loss of %d fragments of %d rows", n_fragments, fragment_length);
     const int32_t n = n_fragments * fragment_length;
     CUDA_TRY(cudaSetDevice(p->device));
-    if ((rc = prepare_learner(p, 0, n)) || (rc = ensure_impala(p, n, 1)) ||
+    if ((rc = prepare_learner(p, 0, n)) || (rc = ensure_impala(p->L, p->P.c, n, 1)) ||
         (rc = upload_host_batch(p, n, model, graph_features, action_mask, nullptr, nullptr, action, nullptr, nullptr, nullptr)))
         return rc;
-    CUDA_TRY(cudaMemcpy(p->i_blogp.get(), behaviour_logp, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(p->i_reward.get(), reward, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(p->i_done.get(), done, (size_t)n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->L.i_blogp.get(), behaviour_logp, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->L.i_reward.get(), reward, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->L.i_done.get(), done, (size_t)n, cudaMemcpyHostToDevice));
     if ((rc = launch_states(p, 0, nullptr, 0, nullptr)) != RAMP_OK) return rc;
     GradArgs ga = host_batch_args(p, n);
     if ((rc = impala_batch(p, 0, *cfg, fragment_length, 0, n_fragments, nullptr, p->h_gf.get(), p->h_model.get(), p->h_mask.get(),
-                           p->h_action.get(), p->i_blogp.get(), p->i_reward.get(), p->i_done.get(), ga, p->i_stats.get())) != RAMP_OK)
+                           p->h_action.get(), p->L.i_blogp.get(), p->L.i_reward.get(), p->L.i_done.get(), ga, p->L.i_stats.get())) != RAMP_OK)
         return rc;
-    CUDA_TRY(cudaMemsetAsync(p->i_stats.get() + RAMP_IMPALA_SGD_STEPS, 0, sizeof(double), 0));
-    if ((rc = host_batch_end(p, grad_out, stats_out, p->i_stats.get(), RAMP_IMPALA_STATS_LEN)) != RAMP_OK) return rc;
-    p->i_rows = n;
-    if (vs_out) CUDA_TRY(cudaMemcpy(vs_out, p->i_vs.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
-    if (pg_adv_out) CUDA_TRY(cudaMemcpy(pg_adv_out, p->i_pg.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
-    if (log_rho_out) CUDA_TRY(cudaMemcpy(log_rho_out, p->i_log_rho.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemsetAsync(p->L.i_stats.get() + RAMP_IMPALA_SGD_STEPS, 0, sizeof(double), 0));
+    if ((rc = host_batch_end(p, grad_out, stats_out, p->L.i_stats.get(), RAMP_IMPALA_STATS_LEN)) != RAMP_OK) return rc;
+    p->L.i_rows = n;
+    if (vs_out) CUDA_TRY(cudaMemcpy(vs_out, p->L.i_vs.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    if (pg_adv_out) CUDA_TRY(cudaMemcpy(pg_adv_out, p->L.i_pg.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    if (log_rho_out) CUDA_TRY(cudaMemcpy(log_rho_out, p->L.i_log_rho.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
 
@@ -1563,40 +1564,40 @@ int ramp_policy_learn_impala(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_ste
     const ramp_policy_config_t& c = p->P.c;
     const int32_t B = eb.n_episodes, n_frag = (n_steps / L) * B, R = n_steps * B;
     const int32_t F = std::min(cfg->train_batch_size / L, n_frag), mb = F * L, n_sgd = (n_frag + F - 1) / F;
-    if ((rc = prepare_learner(p, st, mb)) || (rc = ensure_impala(p, R, n_sgd))) return rc;
+    if ((rc = prepare_learner(p, st, mb)) || (rc = ensure_impala(p->L, p->P.c, R, n_sgd))) return rc;
     // 1. the fragment rows, fragment-major
     ImpalaBatchArgs ba{};
     ba.T = n_steps; ba.B = B; ba.A = c.n_actions; ba.L = L; ba.n_models = c.n_models;
     ba.t_obs = p->t_obs.get(); ba.t_model = p->t_model.get(); ba.t_mask = p->t_mask.get(); ba.t_action = p->t_action.get();
     ba.t_logp = p->t_logp.get(); ba.t_reward = p->t_reward.get(); ba.t_done = p->t_done.get();
-    ba.obs = p->i_obs.get(); ba.model = p->i_model.get(); ba.mask = p->i_mask.get(); ba.action = p->i_action.get();
-    ba.blogp = p->i_blogp.get(); ba.reward = p->i_reward.get(); ba.done = p->i_done.get(); ba.n_rows = p->i_n_rows.get();
+    ba.obs = p->L.i_obs.get(); ba.model = p->L.i_model.get(); ba.mask = p->L.i_mask.get(); ba.action = p->L.i_action.get();
+    ba.blogp = p->L.i_blogp.get(); ba.reward = p->L.i_reward.get(); ba.done = p->L.i_done.get(); ba.n_rows = p->L.i_n_rows.get();
     ramp_impala_batch_kernel<<<(unsigned)((R + 255) / 256), 256, 0, st>>>(ba);
     CUDA_TRY(cudaGetLastError());
     // 2. one SGD step per train batch, in order
-    AdamArgs aa = adam_args(p, *cfg, p->i_n_rows.get(), mb);
-    aa.stats = p->i_stats.get();                                      // IMPALA's statistics: ramp_impala_step_stats_kernel
+    AdamArgs aa = adam_args(p, *cfg, p->L.i_n_rows.get(), mb);
+    aa.stats = p->L.i_stats.get();                                      // IMPALA's statistics: ramp_impala_step_stats_kernel
     for (int k = 0; k < n_sgd; ++k) {
         const int32_t start = k * mb, nf = std::min(F, n_frag - k * F);
         // the rounds at the current weights, kept for the backward; from the second step on also the embeddings, which the
         // previous update made stale (the first uses those the trajectory was collected with)
-        if ((rc = launch_states(p, st, p->i_n_rows.get(), start, k ? p->d_emb.get() : nullptr)) != RAMP_OK) return rc;
+        if ((rc = launch_states(p, st, p->L.i_n_rows.get(), start, k ? p->d_emb.get() : nullptr)) != RAMP_OK) return rc;
         GradArgs ga{};
-        ga.mb = mb; ga.start = start; ga.n_rows = p->i_n_rows.get();
-        if ((rc = impala_batch(p, st, *cfg, L, start, nf, p->i_obs.get(), nullptr, p->i_model.get(), p->i_mask.get(), p->i_action.get(),
-                               p->i_blogp.get(), p->i_reward.get(), p->i_done.get(), ga,
-                               p->i_step_stats.get() + (size_t)k * RAMP_IMPALA_STATS_LEN)) != RAMP_OK)
+        ga.mb = mb; ga.start = start; ga.n_rows = p->L.i_n_rows.get();
+        if ((rc = impala_batch(p, st, *cfg, L, start, nf, p->L.i_obs.get(), nullptr, p->L.i_model.get(), p->L.i_mask.get(), p->L.i_action.get(),
+                               p->L.i_blogp.get(), p->L.i_reward.get(), p->L.i_done.get(), ga,
+                               p->L.i_step_stats.get() + (size_t)k * RAMP_IMPALA_STATS_LEN)) != RAMP_OK)
             return rc;
         aa.start = start;
         if ((rc = launch_adam(p, aa, st)) != RAMP_OK) return rc;
     }
     p->emb_valid = false;
-    p->i_rows = R;
+    p->L.i_rows = R;
     // 3. the means over the steps: the call's one read-back
-    ramp_impala_learn_stats_kernel<<<1, 1, 0, st>>>(p->i_step_stats.get(), n_sgd, p->i_stats.get());
+    ramp_impala_learn_stats_kernel<<<1, 1, 0, st>>>(p->L.i_step_stats.get(), n_sgd, p->L.i_stats.get());
     CUDA_TRY(cudaGetLastError());
     ramp_internal_count_launches(eng, 2 + 9 * n_sgd);
-    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, p->i_stats.get(), sizeof(double) * RAMP_IMPALA_STATS_LEN, cudaMemcpyDeviceToHost, st));
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, p->L.i_stats.get(), sizeof(double) * RAMP_IMPALA_STATS_LEN, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     return RAMP_OK;
 }
@@ -1604,15 +1605,15 @@ int ramp_policy_learn_impala(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_ste
 int ramp_impala_vtrace_read(ramp_policy_t* p, int32_t* n_out, float* target_logp_out, float* log_rho_out, float* vs_out,
                             float* pg_adv_out) {
     if (!p || !n_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    if (p->i_rows < 1) return set_error(RAMP_ERR_BAD_ARG, "impala: no V-trace yet (ramp_policy_learn_impala / ramp_impala_loss_grad)");
+    if (p->L.i_rows < 1) return set_error(RAMP_ERR_BAD_ARG, "impala: no V-trace yet (ramp_policy_learn_impala / ramp_impala_loss_grad)");
     CUDA_TRY(cudaSetDevice(p->device));
     CUDA_TRY(cudaDeviceSynchronize());
-    const size_t n = (size_t)p->i_rows;
-    *n_out = p->i_rows;
-    if (target_logp_out) CUDA_TRY(cudaMemcpy(target_logp_out, p->i_tlogp.get(), 4 * n, cudaMemcpyDeviceToHost));
-    if (log_rho_out) CUDA_TRY(cudaMemcpy(log_rho_out, p->i_log_rho.get(), 4 * n, cudaMemcpyDeviceToHost));
-    if (vs_out) CUDA_TRY(cudaMemcpy(vs_out, p->i_vs.get(), 4 * n, cudaMemcpyDeviceToHost));
-    if (pg_adv_out) CUDA_TRY(cudaMemcpy(pg_adv_out, p->i_pg.get(), 4 * n, cudaMemcpyDeviceToHost));
+    const size_t n = (size_t)p->L.i_rows;
+    *n_out = p->L.i_rows;
+    if (target_logp_out) CUDA_TRY(cudaMemcpy(target_logp_out, p->L.i_tlogp.get(), 4 * n, cudaMemcpyDeviceToHost));
+    if (log_rho_out) CUDA_TRY(cudaMemcpy(log_rho_out, p->L.i_log_rho.get(), 4 * n, cudaMemcpyDeviceToHost));
+    if (vs_out) CUDA_TRY(cudaMemcpy(vs_out, p->L.i_vs.get(), 4 * n, cudaMemcpyDeviceToHost));
+    if (pg_adv_out) CUDA_TRY(cudaMemcpy(pg_adv_out, p->L.i_pg.get(), 4 * n, cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
 

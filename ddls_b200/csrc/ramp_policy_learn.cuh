@@ -22,6 +22,8 @@
 //   ramp_impala_*_stats_kernel      one SGD step's IMPALA statistics; the call's means over its steps
 //   ramp_pg_stats_kernel            PG's statistics
 //
+// Each kernel's statements are a __device__ __forceinline__ *_body that the population's kernels (ramp_population.cuh) call on
+// one weight set's slices; the kernels here are wrappers.
 // Every weight gradient is a sum in a fixed order with an f64 accumulator and no atomics: one call on one batch gives the same bits.
 #pragma once
 
@@ -834,19 +836,24 @@ struct ImpalaBatchArgs {
 
 // the first T slots of the trajectory as fragments of L rows, fragment f = (time block f / B, episode f % B), row r = f L + t.
 // A row whose episode had already finished, or had nothing queued (or a job type outside the policy's), gets model -1.
-__global__ void ramp_impala_batch_kernel(const ImpalaBatchArgs a) {
+// ramp_impala_batch_kernel's statements for row r over a.B episodes whose trajectory rows are ld apart (the population's groups
+// are column slices of one [T][K b] trajectory)
+__device__ __forceinline__ void impala_batch_body(const ImpalaBatchArgs& a, const int64_t r, const int ld) {
     const int64_t R = (int64_t)a.T * a.B;
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r == 0) *a.n_rows = (int32_t)R;
     if (r >= R) return;
     const int64_t f = r / a.L, t = r - f * a.L, j = f / a.B, b = f - j * a.B;
-    const size_t s = (size_t)(j * a.L + t), i = s * a.B + b;
-    const bool alive = s == 0 || !a.t_done[i - a.B];
+    const size_t s = (size_t)(j * a.L + t), i = s * ld + b;
+    const bool alive = s == 0 || !a.t_done[i - ld];
     const int32_t m = a.t_model[i];
     for (int k = 0; k < 11; ++k) a.obs[r * 11 + k] = a.t_obs[i * 11 + k];
     for (int k = 0; k < a.A; ++k) a.mask[r * a.A + k] = a.t_mask[i * a.A + k];
     a.model[r] = alive && m >= 0 && m < a.n_models ? m : -1;
     a.action[r] = a.t_action[i]; a.blogp[r] = a.t_logp[i]; a.reward[r] = a.t_reward[i]; a.done[r] = a.t_done[i];
+}
+
+__global__ void ramp_impala_batch_kernel(const ImpalaBatchArgs a) {
+    impala_batch_body(a, (int64_t)blockIdx.x * blockDim.x + threadIdx.x, a.B);
 }
 
 struct VtraceArgs {
@@ -861,10 +868,8 @@ struct VtraceArgs {
 // operation, so at the collection weights it is the collected value bit for bit -- then from_importance_weights (vtrace_torch.py)
 // scanning backwards in f64 with vtrace_drop_last_ts: rows 0 .. L-2 are the loss's, row L-1's value is the bootstrap and vs_{L-1}.
 // A row without a decision has log rho 0, V 0 (the head kernel's), its reward and done, and stays out of the loss (lmodel -1).
-__global__ void __launch_bounds__(256) ramp_vtrace_kernel(const VtraceArgs a) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int f = blockIdx.x * (blockDim.x >> 5) + warp;
-    if (f >= a.n_frag) return;
+// ramp_vtrace_kernel's statements for fragment f < a.n_frag, by the whole warp
+__device__ __forceinline__ void vtrace_body(const VtraceArgs& a, const int f, const int lane) {
     const int64_t r0 = (int64_t)a.row0 + (int64_t)f * a.L;
     for (int t = 0; t < a.L; ++t) {
         const int64_t r = r0 + t;
@@ -907,11 +912,18 @@ __global__ void __launch_bounds__(256) ramp_vtrace_kernel(const VtraceArgs a) {
     }
 }
 
+__global__ void __launch_bounds__(256) ramp_vtrace_kernel(const VtraceArgs a) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int f = blockIdx.x * (blockDim.x >> 5) + warp;
+    if (f >= a.n_frag) return;
+    vtrace_body(a, f, lane);
+}
+
 // one SGD step's statistics (RAMP_IMPALA_*): the loss's sums over the loss rows, their mean entropy and rho, the gradient's
 // global norm before clipping.  rows of the step: launch row i is batch row row0 + i.
-__global__ void ramp_impala_step_stats_kernel(const float* row_stats, const int32_t* row_model, int32_t rows, int32_t row0,
-                                              const float* log_rho, double vf_coeff, double ent_coeff, const double* norm_part,
-                                              double* out) {
+__device__ __forceinline__ void impala_step_stats_body(const float* row_stats, const int32_t* row_model, int32_t rows, int32_t row0,
+                                                       const float* log_rho, double vf_coeff, double ent_coeff, const double* norm_part,
+                                                       double* out) {
     double pi = 0.0, vf = 0.0, ent = 0.0, rho = 0.0;
     int n = 0;
     for (int i = 0; i < rows; ++i) {
@@ -927,8 +939,14 @@ __global__ void ramp_impala_step_stats_kernel(const float* row_stats, const int3
     out[RAMP_IMPALA_GRAD_NORM] = sum_norm_parts(norm_part); out[RAMP_IMPALA_ROWS] = n; out[RAMP_IMPALA_SGD_STEPS] = 1;
 }
 
+__global__ void ramp_impala_step_stats_kernel(const float* row_stats, const int32_t* row_model, int32_t rows, int32_t row0,
+                                              const float* log_rho, double vf_coeff, double ent_coeff, const double* norm_part,
+                                              double* out) {
+    impala_step_stats_body(row_stats, row_model, rows, row0, log_rho, vf_coeff, ent_coeff, norm_part, out);
+}
+
 // the means over the call's SGD steps, and their number
-__global__ void ramp_impala_learn_stats_kernel(const double* step_stats, int32_t n_steps, double* out) {
+__device__ __forceinline__ void impala_learn_stats_body(const double* step_stats, int32_t n_steps, double* out) {
     for (int j = 0; j < RAMP_IMPALA_STATS_LEN; ++j) {
         double s = 0.0;
         for (int i = 0; i < n_steps; ++i) s += step_stats[(size_t)i * RAMP_IMPALA_STATS_LEN + j];
@@ -937,13 +955,17 @@ __global__ void ramp_impala_learn_stats_kernel(const double* step_stats, int32_t
     out[RAMP_IMPALA_SGD_STEPS] = n_steps;
 }
 
+__global__ void ramp_impala_learn_stats_kernel(const double* step_stats, int32_t n_steps, double* out) {
+    impala_learn_stats_body(step_stats, n_steps, out);
+}
+
 // ---- PG (ramp_policy_learn_pg, ramp_pg_loss_grad) ----
 
 // PG's statistics (RAMP_PG_*) over the launch's first min(mb, *n_rows) rows (row i is batch row i: PG does not shuffle):
 // policy_loss = -sum(logp(a) adv) / rows, the rows the head-gradient kernel divides by; the mean entropy over the rows with a
 // decision
-__global__ void ramp_pg_stats_kernel(const float* row_stats, const int32_t* row_model, const float* adv, int32_t mb, const int32_t* n_rows,
-                                     const double* norm_part, double* out) {
+__device__ __forceinline__ void pg_stats_body(const float* row_stats, const int32_t* row_model, const float* adv, int32_t mb,
+                                              const int32_t* n_rows, const double* norm_part, double* out) {
     const int rows = max(0, min(mb, *n_rows));
     double pi = 0.0, ent = 0.0;
     int k = 0;
@@ -957,6 +979,11 @@ __global__ void ramp_pg_stats_kernel(const float* row_stats, const int32_t* row_
     out[RAMP_PG_ENTROPY] = k ? ent / k : 0.0;
     out[RAMP_PG_GRAD_NORM] = sum_norm_parts(norm_part);
     out[RAMP_PG_ROWS] = rows;
+}
+
+__global__ void ramp_pg_stats_kernel(const float* row_stats, const int32_t* row_model, const float* adv, int32_t mb, const int32_t* n_rows,
+                                     const double* norm_part, double* out) {
+    pg_stats_body(row_stats, row_model, adv, mb, n_rows, norm_part, out);
 }
 
 }  // namespace ramp

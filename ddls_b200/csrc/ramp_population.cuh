@@ -1,19 +1,23 @@
-// ramp_population.cuh -- K independent PPO trainings of the GNN policy in one environment batch (include/ramp_b200.h:
+// ramp_population.cuh -- K independent PPO, IMPALA or PG trainings of the GNN policy in one environment batch (include/ramp_b200.h:
 // ramp_population_*).  Included by ramp_policy.cu after the learner.
 //
 // The environment's B = K b episodes are K contiguous groups of b; group k acts with weight set k and learns only from its own
-// episodes with its own ramp_ppo_config_t.  Every kernel here runs the statements of the single policy's kernel (the shared
-// *_body functions of ramp_policy.cu / ramp_policy_learn.cuh) on one set's slice, with the set taken from the launch:
+// episodes with its own config.  Every kernel here runs the statements of the single policy's kernel (the shared *_body
+// functions of ramp_policy.cu / ramp_policy_learn.cuh) on one set's slice, with the set taken from the launch:
 //
 //   ramp_pop_embed_grad_kernel   persistent CTAs over (set, job type) items, grid-strided past the resident CTAs: the MeanPool
 //                                rounds (forward: states kept, embeddings [K][n_models][out_node]) or their backward
 //   ramp_pop_head_kernel         blockIdx.y = set: the read-out of the set's episodes / rows, its weights staged per CTA
-//   ramp_pop_gae_kernel          one 1,024-thread CTA per group: GAE over the group's columns of the [T][B] trajectory, its live
-//                                rows t-major into the group's slice of the train batch, standardised with the group's mean / std
-//   ramp_pop_head_grad_kernel    one warp per (set, minibatch row): the rows of every group's minibatch in one launch
+//   ramp_pop_gae_kernel          one 1,024-thread CTA per group: GAE (PG: discounted returns) over the group's columns of the
+//                                [T][B] trajectory, its live rows t-major into the group's slice of the train batch,
+//                                standardised with the group's mean / std when asked
+//   ramp_pop_head_grad_kernel    one warp per (set, launch row): the rows of every group's minibatch / SGD step in one launch
 //   ramp_pop_head_reduce_kernel  one thread per (set, read-out weight): the sum over the set's rows in row order
 //   ramp_pop_finish_kernel / ramp_pop_adam_kernel   blockIdx.y = set: the job types' sum, the norm partials, clip and Adam
 //   ramp_pop_learn_stats_kernel  one thread per set: the last pass's means and update_kl
+//   ramp_pop_impala_batch_kernel one thread per (set, fragment row): IMPALA's fragments of the group's columns
+//   ramp_pop_vtrace_kernel       one warp per (set, fragment): V-trace with the set's gamma and clip thresholds
+//   ramp_pop_impala_*_stats_kernel, ramp_pop_pg_stats_kernel   one thread per set: its statistics
 //
 // So group k computes what one policy with set k's weights computes on a b-episode environment with the same episode streams, bit
 // for bit: no float atomics, and every reduction in the single kernel's order.
@@ -23,6 +27,8 @@ namespace ramp {
 
 struct PopHead {
     int32_t per;                          // episodes / rows of one set
+    int32_t stride;                       // rows from one set's first to the next's (per, or a set's whole batch when the launch
+                                          // covers a slice of it)
     int64_t n_weights;
     const unsigned long long* seeds;      // [K] the sets' act seeds (sample), mixed with `mix` as ramp_policy_act mixes its call count
     unsigned long long mix;
@@ -30,7 +36,7 @@ struct PopHead {
 
 __global__ void __launch_bounds__(256, 3) ramp_pop_head_kernel(const PolicyDev P, const HeadArgs base, const PopHead ph) {
     const int s = blockIdx.y;
-    const size_t o = (size_t)s * ph.per, A = P.c.n_actions;
+    const size_t o = (size_t)s * ph.stride, A = P.c.n_actions;
     HeadArgs a = base;
     a.n = ph.per;
     a.model += o; a.mask += o * A; a.actions += o;
@@ -125,6 +131,59 @@ __global__ void ramp_pop_learn_stats_kernel(const double* mb_stats, int32_t n_mb
                      out + (size_t)s * RAMP_PPO_STATS_LEN);
 }
 
+// ---- IMPALA and PG: the single learner's bodies on one set's slices ----
+
+// IMPALA's fragment rows of every group, one thread per (set, row): a is set 0's (its a.B = b episodes per group), set s reads
+// the columns [s b, (s + 1) b) of the [T][K b] trajectory and writes its T b rows s T b rows further
+__global__ void ramp_pop_impala_batch_kernel(const ImpalaBatchArgs base, int32_t K) {
+    const int64_t R = (int64_t)base.T * base.B;
+    const int64_t gi = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gi >= K * R) return;
+    const int64_t s = gi / R;
+    const size_t col = (size_t)s * base.B, o = (size_t)s * R, A = base.A;
+    ImpalaBatchArgs a = base;
+    a.t_obs += col * 11; a.t_model += col; a.t_mask += col * A; a.t_action += col; a.t_logp += col; a.t_reward += col; a.t_done += col;
+    a.obs += o * 11; a.model += o; a.mask += o * A; a.action += o; a.blogp += o; a.reward += o; a.done += o; a.n_rows += s;
+    impala_batch_body(a, gi - s * R, K * base.B);
+}
+
+// one warp per (set, fragment): sets[k] is set k's VtraceArgs (its gamma, clip thresholds and row slices); the step's fragments
+// and first row are the launch's
+__global__ void __launch_bounds__(256) ramp_pop_vtrace_kernel(const VtraceArgs* sets, int32_t K, int32_t n_frag, int32_t row0) {
+    const int gi = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (gi >= K * n_frag) return;
+    const int s = gi / n_frag;
+    VtraceArgs a = sets[s];
+    a.n_frag = n_frag; a.row0 = row0;
+    vtrace_body(a, gi - s * n_frag, threadIdx.x & 31);
+}
+
+// one thread per set: SGD step k (of n_sgd) of every set, whose launch rows are mb apart and whose fragment rows R apart; coef:
+// [K][2] the sets' vf_loss_coeff and entropy_coeff
+__global__ void ramp_pop_impala_step_stats_kernel(const float* row_stats, const int32_t* row_model, int32_t mb, int32_t row0, const float* log_rho,
+                                                  int32_t R, const double* coef, const double* norm_part, double* step_stats, int32_t n_sgd,
+                                                  int32_t k, int32_t K) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= K) return;
+    impala_step_stats_body(row_stats + (size_t)s * mb * RS_N, row_model + (size_t)s * mb, mb, row0, log_rho + (size_t)s * R, coef[2 * s],
+                           coef[2 * s + 1], norm_part + (size_t)s * LRN_GRID, step_stats + ((size_t)s * n_sgd + k) * RAMP_IMPALA_STATS_LEN);
+}
+
+__global__ void ramp_pop_impala_learn_stats_kernel(const double* step_stats, int32_t n_sgd, double* out, int32_t K) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= K) return;
+    impala_learn_stats_body(step_stats + (size_t)s * n_sgd * RAMP_IMPALA_STATS_LEN, n_sgd, out + (size_t)s * RAMP_IMPALA_STATS_LEN);
+}
+
+// one thread per set: its statistics into its RAMP_PPO_STATS_LEN slice of `out`, where Adam wrote its row count
+__global__ void ramp_pop_pg_stats_kernel(const float* row_stats, const int32_t* row_model, const float* adv, int32_t rows, const int32_t* n_rows,
+                                         const double* norm_part, double* out, int32_t K) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= K) return;
+    pg_stats_body(row_stats + (size_t)s * rows * RS_N, row_model + (size_t)s * rows, adv + (size_t)s * rows, rows, n_rows + s,
+                  norm_part + (size_t)s * LRN_GRID, out + (size_t)s * RAMP_PPO_STATS_LEN);
+}
+
 }  // namespace ramp
 
 struct ramp_population {
@@ -140,6 +199,8 @@ struct ramp_population {
     LearnerBuffers L;                     // the learner: what ramp_policy keeps for one set, for K
     DeviceArray<float> d_kl;              // [K][2]: kl_coeff, kl_target
     DeviceArray<GaeArgs> d_gae; DeviceArray<GradArgs> d_grad; DeviceArray<AdamArgs> d_adam;
+    DeviceArray<VtraceArgs> d_vtrace;     // IMPALA: every set's V-trace arguments
+    DeviceArray<double> d_coef;           // IMPALA: [K][2] vf_loss_coeff, entropy_coeff
 };
 
 namespace {
@@ -193,7 +254,9 @@ int pop_embed(ramp_population* q, cudaStream_t st) {
     return RAMP_OK;
 }
 
-int pop_launch_head(ramp_population* q, const HeadArgs& a, int32_t per, const unsigned long long* seeds, unsigned long long mix, cudaStream_t st) {
+// the read-out of `per` rows per set, set s's starting `stride` rows after set s - 1's (0: per)
+int pop_launch_head(ramp_population* q, const HeadArgs& a, int32_t per, const unsigned long long* seeds, unsigned long long mix, cudaStream_t st,
+                    int32_t stride = 0) {
     ramp_policy* p = q->p;
     const int wpc = 8;
     int gx = (per + wpc - 1) / wpc;
@@ -202,7 +265,7 @@ int pop_launch_head(ramp_population* q, const HeadArgs& a, int32_t per, const un
     PolicyDev P = p->P;
     P.w = q->d_w.get();
     PopHead ph{};
-    ph.per = per; ph.n_weights = q->nw; ph.seeds = seeds; ph.mix = mix;
+    ph.per = per; ph.stride = stride ? stride : per; ph.n_weights = q->nw; ph.seeds = seeds; ph.mix = mix;
     ramp_pop_head_kernel<<<dim3(gx, q->K), wpc * 32, p->head_smem, st>>>(P, a, ph);
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
@@ -216,7 +279,93 @@ int pop_ensure_learner(ramp_population* q) {
     CUDA_TRY(q->d_gae.alloc(K));
     CUDA_TRY(q->d_grad.alloc(K));
     CUDA_TRY(q->d_adam.alloc(K));
+    CUDA_TRY(q->d_vtrace.alloc(K));
+    CUDA_TRY(q->d_coef.alloc(2 * K));
     return ensure_learner(q->L, q->p);
+}
+
+// set s's AdamArgs at cfg's settings on its slices of the gradient, moments, step counts, norm partials and weights
+template <class Cfg>
+AdamArgs pop_adam_args(ramp_population* q, const Cfg& cfg, int s, const int32_t* n_rows, int32_t mb) {
+    AdamArgs aa = adam_args(q->p, cfg, n_rows, mb);
+    aa.step = q->L.step.get() + 2 * s; aa.m = q->L.adam_m.get() + (size_t)s * q->nw; aa.v = q->L.adam_v.get() + (size_t)s * q->nw;
+    aa.grad = q->L.grad.get() + (size_t)s * q->nw; aa.norm_part = q->L.norm_part.get() + (size_t)s * LRN_GRID; aa.w = q->d_w.get() + (size_t)s * q->nw;
+    return aa;
+}
+
+// every set's configuration, each by its algorithm's own rules; the error names the set
+template <class Cfg>
+int pop_check_configs(const ramp_population* q, const Cfg* cfgs) {
+    if (!q || !cfgs) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    for (int s = 0; s < q->K; ++s)
+        if (check_learner_config(&cfgs[s]) != RAMP_OK) return set_error(RAMP_ERR_BAD_ARG, "population: set %d: %s", s, g_last_error.c_str());
+    return RAMP_OK;
+}
+
+// the opening of the population's learn calls after the configuration checks: learn_begin on the template with set 0's config, a
+// trajectory that splits into K groups, the learner's buffers and every (set, job type)'s states on `st`
+template <class Cfg>
+int pop_learn_begin(ramp_population* q, ramp_engine_t* eng, const Cfg* cfgs, int32_t n_steps, ramp_env_buffers_t* eb, cudaStream_t* st) {
+    int rc = learn_begin(q->p, eng, cfgs, n_steps, "population", eb, st);
+    if (rc != RAMP_OK) return rc;
+    if (eb->n_episodes % q->K)
+        return set_error(RAMP_ERR_BAD_ARG, "population: %d episodes do not split into %d groups of equal size", eb->n_episodes, q->K);
+    if ((rc = fence_in(q->p, *st)) || (rc = pop_ensure_learner(q)) || (rc = pop_ensure_gms(q, *st))) return rc;
+    if ((size_t)q->K > q->d_keys.size()) {                                // the head-gradient kernel reads a key per set (unused unshuffled)
+        CUDA_TRY(q->d_keys.alloc(q->K));
+        CUDA_TRY(cudaMemsetAsync(q->d_keys.get(), 0, sizeof(unsigned long long) * q->K, *st));
+    }
+    return RAMP_OK;
+}
+
+// head gradient (sets: q->d_grad) -> head reduce -> embedding backward -> finish over K launch rows of mb rows each: every set's
+// gradient and norm partials.  keys: the [K] shuffle keys (read, and unused, by an unshuffled launch); first_pass: logp_old is written
+int pop_launch_grad(ramp_population* q, cudaStream_t st, int32_t mb, int32_t start, const unsigned long long* keys, int first_pass) {
+    ramp_policy* p = q->p;
+    const int32_t K = q->K;
+    PolicyDev P = p->P;
+    P.w = q->d_w.get();
+    const SegTable* segs = q->L.segs;
+    int64_t rgrid = (K * segs->total + 255) / 256;
+    if (rgrid > 4 * p->sm_count) rgrid = 4 * p->sm_count;
+    ramp_pop_head_grad_kernel<<<(K * mb + LRN_WARPS - 1) / LRN_WARPS, LRN_WARPS * 32, 0, st>>>(P, q->d_grad.get(), K, mb, start, keys, first_pass, q->nw);
+    ramp_pop_head_reduce_kernel<<<(unsigned)rgrid, 256, 0, st>>>(P, segs->d.get(), segs->count, segs->total, K, (int64_t)mb * head_rec(P.c).stride,
+                                                                 q->nw, q->L.grad.get());
+    CUDA_TRY(cudaGetLastError());
+    EmbGradArgs eg{};
+    eg.rec = q->L.rec.get(); eg.row_model = q->L.row_model.get(); eg.rows = mb; eg.gpart = q->L.gpart.get(); eg.n_gnn = gnn_weight_count(p);
+    int rc = pop_launch_embed(q, st, eg, false);
+    if (rc != RAMP_OK) return rc;
+    ramp_pop_finish_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->L.gpart.get(), P.c.n_models, gnn_weight_count(p), q->nw, q->L.grad.get(),
+                                                              q->L.norm_part.get());
+    CUDA_TRY(cudaGetLastError());
+    return RAMP_OK;
+}
+
+// set s's GAE arguments: its group's b columns of the [T][K b] trajectory, its slice of the train batch; boot: the [K b] bootstrap
+// values, or nullptr: no critic (PG)
+GaeArgs pop_gae_args(ramp_population* q, int s, int32_t T, int32_t b, double gamma, double lambda, int32_t standardize, const float* boot) {
+    ramp_policy* p = q->p;
+    const size_t A = p->P.c.n_actions, col = (size_t)s * b, r0 = (size_t)s * T * b;
+    GaeArgs ge{};
+    ge.T = T; ge.B = b; ge.A = (int32_t)A; ge.n_models = p->P.c.n_models; ge.standardize = standardize; ge.gamma = gamma; ge.lambda = lambda;
+    ge.t_obs = p->t_obs.get() + col * 11; ge.t_model = p->t_model.get() + col; ge.t_mask = p->t_mask.get() + col * A;
+    ge.t_action = p->t_action.get() + col; ge.t_logp = p->t_logp.get() + col; ge.t_value = boot ? p->t_value.get() + col : nullptr;
+    ge.t_reward = p->t_reward.get() + col; ge.t_done = p->t_done.get() + col;
+    ge.boot = boot ? boot + col : nullptr; ge.adv64 = q->L.b_adv64.get() + col;
+    ge.obs = q->L.b_obs.get() + r0 * 11; ge.model = q->L.b_model.get() + r0; ge.mask = q->L.b_mask.get() + r0 * A; ge.action = q->L.b_action.get() + r0;
+    ge.logp = q->L.b_logp.get() + r0; ge.adv = q->L.b_adv.get() + r0; ge.vt = q->L.b_vt.get() + r0; ge.n_rows = q->L.n_rows.get() + s;
+    return ge;
+}
+
+// set s's head-gradient arguments for launch rows of mb rows: its slices of the per-row scratch and its embeddings
+GradArgs pop_grad_args(ramp_population* q, int s, int32_t mb) {
+    const ramp_policy_config_t& c = q->p->P.c;
+    const size_t q0 = (size_t)s * mb;
+    GradArgs ga{};
+    ga.mb = mb; ga.graph_static = q->p->d_gstatic.get(); ga.emb = q->d_emb.get() + (size_t)s * c.n_models * c.out_features_node;
+    ga.rec = q->L.rec.get() + q0 * head_rec(c).stride; ga.row_model = q->L.row_model.get() + q0; ga.row_stats = q->L.row_stats.get() + q0 * RS_N;
+    return ga;
 }
 
 }  // namespace
@@ -321,21 +470,16 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
     }
     ramp_env_buffers_t eb{};
     cudaStream_t st;
-    int rc = learn_begin(p, eng, cfgs, n_steps, "population", &eb, &st);
+    int rc = pop_learn_begin(q, eng, cfgs, n_steps, &eb, &st);
     if (rc != RAMP_OK) return rc;
-    if (eb.n_episodes % K) return set_error(RAMP_ERR_BAD_ARG, "population: %d episodes do not split into %d groups of equal size", eb.n_episodes, K);
     const ramp_policy_config_t& c = p->P.c;
     const int32_t B = eb.n_episodes, b = B / K, rows = n_steps * b, mb = cfgs[0].sgd_minibatch_size, n_mb = (rows + mb - 1) / mb;
-    const int32_t n_pass = cfgs[0].num_sgd_iter, A = c.n_actions, on = c.out_features_node, nm = c.n_models;
+    const int32_t n_pass = cfgs[0].num_sgd_iter, A = c.n_actions;
     const size_t R = rows;
-    if ((rc = fence_in(p, st)) || (rc = pop_ensure_learner(q)) || (rc = pop_ensure_gms(q, st)) || (rc = ensure_rows(q->L, p->P, mb, st)) ||
-        (rc = ensure_batch(q->L, c, rows)) || (rc = ensure_ppo(q->L, B, n_mb)))
-        return rc;
+    if ((rc = ensure_rows(q->L, p->P, mb, st)) || (rc = ensure_batch(q->L, c, rows)) || (rc = ensure_ppo(q->L, B, n_mb))) return rc;
     if (!q->emb_valid && (rc = pop_embed(q, st)) != RAMP_OK) return rc;
-    const SegTable* segs = q->L.segs;
     if ((size_t)K * std::max(n_pass, 1) > q->d_keys.size()) CUDA_TRY(q->d_keys.alloc((size_t)K * std::max(n_pass, 1)));
     // every group's arguments: set s's slices of the trajectory's columns, the train batch, the scratch and the learner state
-    const HeadRec HR = head_rec(c);
     std::vector<GaeArgs> gae(K);
     std::vector<GradArgs> grad(K);
     std::vector<AdamArgs> adam(K);
@@ -345,27 +489,16 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
     if (n_steps == p->traj_n) boot = q->L.boot.get();
     for (int s = 0; s < K; ++s) {
         const ramp_ppo_config_t& cfg = cfgs[s];
-        const size_t col = (size_t)s * b, r0 = (size_t)s * R, q0 = (size_t)s * mb;
-        GaeArgs& ge = gae[s];
-        ge.T = n_steps; ge.B = b; ge.A = A; ge.n_models = nm; ge.standardize = cfg.standardize_advantages;
-        ge.gamma = cfg.gamma; ge.lambda = cfg.lambda;
-        ge.t_obs = p->t_obs.get() + col * 11; ge.t_model = p->t_model.get() + col; ge.t_mask = p->t_mask.get() + col * A;
-        ge.t_action = p->t_action.get() + col; ge.t_logp = p->t_logp.get() + col; ge.t_value = p->t_value.get() + col;
-        ge.t_reward = p->t_reward.get() + col; ge.t_done = p->t_done.get() + col;
-        ge.boot = boot + col; ge.adv64 = q->L.b_adv64.get() + col;
-        ge.obs = q->L.b_obs.get() + r0 * 11; ge.model = q->L.b_model.get() + r0; ge.mask = q->L.b_mask.get() + r0 * A; ge.action = q->L.b_action.get() + r0;
-        ge.logp = q->L.b_logp.get() + r0; ge.adv = q->L.b_adv.get() + r0; ge.vt = q->L.b_vt.get() + r0; ge.n_rows = q->L.n_rows.get() + s;
+        const size_t r0 = (size_t)s * R;
+        gae[s] = pop_gae_args(q, s, n_steps, b, cfg.gamma, cfg.lambda, cfg.standardize_advantages, boot);
         GradArgs& ga = grad[s];
-        ga.mb = mb; ga.n_rows = q->L.n_rows.get() + s; ga.shuffle = 1; ga.obs_dyn = q->L.b_obs.get() + r0 * 11; ga.model = q->L.b_model.get() + r0;
+        ga = pop_grad_args(q, s, mb);
+        ga.n_rows = q->L.n_rows.get() + s; ga.shuffle = 1; ga.obs_dyn = q->L.b_obs.get() + r0 * 11; ga.model = q->L.b_model.get() + r0;
         ga.mask = q->L.b_mask.get() + r0 * A; ga.action = q->L.b_action.get() + r0; ga.old_logits = q->L.b_old.get() + r0 * A;
-        ga.adv = q->L.b_adv.get() + r0; ga.vt = q->L.b_vt.get() + r0; ga.graph_static = p->d_gstatic.get(); ga.emb = q->d_emb.get() + (size_t)s * nm * on;
-        ga.rec = q->L.rec.get() + q0 * HR.stride; ga.row_model = q->L.row_model.get() + q0; ga.row_stats = q->L.row_stats.get() + q0 * RS_N;
-        ga.logp_old = q->L.b_logp_old.get() + r0;
+        ga.adv = q->L.b_adv.get() + r0; ga.vt = q->L.b_vt.get() + r0; ga.logp_old = q->L.b_logp_old.get() + r0;
         ppo_terms(ga, cfg);
         AdamArgs& aa = adam[s];
-        aa = adam_args(p, cfg, q->L.n_rows.get() + s, mb);
-        aa.step = q->L.step.get() + 2 * s; aa.m = q->L.adam_m.get() + (size_t)s * q->nw; aa.v = q->L.adam_v.get() + (size_t)s * q->nw;
-        aa.grad = q->L.grad.get() + (size_t)s * q->nw; aa.norm_part = q->L.norm_part.get() + (size_t)s * LRN_GRID; aa.w = q->d_w.get() + (size_t)s * q->nw;
+        aa = pop_adam_args(q, cfg, s, q->L.n_rows.get() + s, mb);
         aa.row_stats = ga.row_stats; aa.vf_coeff = ga.vf_coeff; aa.ent_coeff = ga.ent_coeff; aa.kl_coeff = ga.kl_coeff;
         aa.stats = q->L.mb_stats.get() + (size_t)s * n_mb * RAMP_PPO_STATS_LEN;
         kl[2 * s] = (float)cfg.kl_coeff; kl[2 * s + 1] = (float)cfg.kl_target;
@@ -377,8 +510,6 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
     CUDA_TRY(cudaMemcpyAsync(q->d_kl.get(), kl.data(), sizeof(float) * 2 * K, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(q->d_keys.get(), keys.data(), sizeof(unsigned long long) * keys.size(), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaStreamSynchronize(st));                                  // the vectors are pageable
-    PolicyDev P = p->P;
-    P.w = q->d_w.get();
     int launches = 2;                                                     // GAE, old logits
     // 1. the value of the state after the last step, as ramp_policy_learn takes it
     if (n_steps == p->traj_n) {
@@ -397,23 +528,14 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
     ho.emb = q->d_emb.get(); ho.logits = q->L.b_old.get(); ho.value = q->L.b_value.get(); ho.logp = q->L.b_lpx.get(); ho.actions = q->L.b_actx.get();
     if ((rc = pop_launch_head(q, ho, rows, nullptr, 0, st)) != RAMP_OK) return rc;
     // 4. minibatch j of every group in the same launches
-    int64_t rgrid = (K * segs->total + 255) / 256;
-    if (rgrid > 4 * p->sm_count) rgrid = 4 * p->sm_count;
     for (int pass = 0; pass < n_pass; ++pass) {
         for (int j = 0; j < n_mb; ++j) {
             const int32_t start = j * mb;
             EmbGradArgs ef{};
             ef.n_rows = q->L.n_rows.get(); ef.start = start; ef.emb = pass || j ? q->d_emb.get() : nullptr;
-            if ((rc = pop_launch_embed(q, st, ef, true)) != RAMP_OK) return rc;
-            ramp_pop_head_grad_kernel<<<(K * mb + LRN_WARPS - 1) / LRN_WARPS, LRN_WARPS * 32, 0, st>>>(
-                P, q->d_grad.get(), K, mb, start, q->d_keys.get() + (size_t)pass * K, pass == 0, q->nw);
-            ramp_pop_head_reduce_kernel<<<(unsigned)rgrid, 256, 0, st>>>(P, segs->d.get(), segs->count, segs->total, K,
-                                                                         (int64_t)mb * HR.stride, q->nw, q->L.grad.get());
-            EmbGradArgs eb2{};
-            eb2.rec = q->L.rec.get(); eb2.row_model = q->L.row_model.get(); eb2.rows = mb; eb2.gpart = q->L.gpart.get(); eb2.n_gnn = gnn_weight_count(p);
-            if ((rc = pop_launch_embed(q, st, eb2, false)) != RAMP_OK) return rc;
-            ramp_pop_finish_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->L.gpart.get(), nm, gnn_weight_count(p), q->nw, q->L.grad.get(),
-                                                                      q->L.norm_part.get());
+            if ((rc = pop_launch_embed(q, st, ef, true)) != RAMP_OK ||
+                (rc = pop_launch_grad(q, st, mb, start, q->d_keys.get() + (size_t)pass * K, pass == 0)) != RAMP_OK)
+                return rc;
             ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_adam.get(), start, j, q->L.parity, q->nw);
             q->L.parity ^= 1;
             CUDA_TRY(cudaGetLastError());
@@ -429,6 +551,174 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
     if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, q->L.stats.get(), sizeof(double) * K * RAMP_PPO_STATS_LEN, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     return fence_out(p, st);
+}
+
+int ramp_population_learn_impala(ramp_population_t* q, ramp_engine_t* eng, int32_t n_steps, const ramp_impala_config_t* cfgs, double* stats_out) {
+    int rc = pop_check_configs(q, cfgs);
+    if (rc != RAMP_OK) return rc;
+    ramp_policy* p = q->p;
+    const int32_t K = q->K;
+    for (int s = 1; s < K; ++s) {
+        if (cfgs[s].rollout_fragment_length != cfgs[0].rollout_fragment_length)
+            return set_error(RAMP_ERR_BAD_ARG, "population: rollout_fragment_length of set %d (%d) differs from set 0's (%d)", s,
+                             cfgs[s].rollout_fragment_length, cfgs[0].rollout_fragment_length);
+        if (cfgs[s].train_batch_size != cfgs[0].train_batch_size)
+            return set_error(RAMP_ERR_BAD_ARG, "population: train_batch_size of set %d (%d) differs from set 0's (%d)", s,
+                             cfgs[s].train_batch_size, cfgs[0].train_batch_size);
+    }
+    ramp_env_buffers_t eb{};
+    cudaStream_t st;
+    if ((rc = pop_learn_begin(q, eng, cfgs, n_steps, &eb, &st)) != RAMP_OK) return rc;
+    const int32_t L = cfgs[0].rollout_fragment_length ? cfgs[0].rollout_fragment_length : n_steps;
+    if (n_steps % L) return set_error(RAMP_ERR_BAD_ARG, "impala: rollout_fragment_length %d does not divide %d steps", L, n_steps);
+    if (cfgs[0].train_batch_size < L)
+        return set_error(RAMP_ERR_BAD_ARG, "impala: train_batch_size %d is below rollout_fragment_length %d", cfgs[0].train_batch_size, L);
+    const ramp_policy_config_t& c = p->P.c;
+    const int32_t b = eb.n_episodes / K, n_frag = (n_steps / L) * b, R = n_steps * b, A = c.n_actions;
+    const int32_t F = std::min(cfgs[0].train_batch_size / L, n_frag), mb = F * L, n_sgd = (n_frag + F - 1) / F;
+    if ((rc = ensure_rows(q->L, p->P, mb, st)) || (rc = ensure_impala(q->L, c, R, n_sgd))) return rc;
+    if (!q->emb_valid && (rc = pop_embed(q, st)) != RAMP_OK) return rc;
+    LearnerBuffers& Lb = q->L;
+    // every set's arguments: its slices of the fragment rows, the per-row scratch and the learner state
+    std::vector<VtraceArgs> vt(K);
+    std::vector<GradArgs> grad(K);
+    std::vector<AdamArgs> adam(K);
+    std::vector<double> coef(2 * K);
+    for (int s = 0; s < K; ++s) {
+        const ramp_impala_config_t& cfg = cfgs[s];
+        const size_t r0 = (size_t)s * R;
+        VtraceArgs& v = vt[s];
+        v.L = L; v.A = A; v.n_models = c.n_models;
+        v.gamma = cfg.gamma; v.clip_rho = cfg.vtrace_clip_rho_threshold; v.clip_pg_rho = cfg.vtrace_clip_pg_rho_threshold;
+        v.logits = Lb.i_tlogits.get() + r0 * A; v.value = Lb.i_tvalue.get() + r0;
+        v.model = Lb.i_model.get() + r0; v.action = Lb.i_action.get() + r0; v.blogp = Lb.i_blogp.get() + r0; v.reward = Lb.i_reward.get() + r0;
+        v.done = Lb.i_done.get() + r0; v.tlogp = Lb.i_tlogp.get() + r0; v.log_rho = Lb.i_log_rho.get() + r0; v.vs = Lb.i_vs.get() + r0;
+        v.pg_adv = Lb.i_pg.get() + r0; v.lmodel = Lb.i_lmodel.get() + r0;
+        GradArgs& ga = grad[s];
+        ga = pop_grad_args(q, s, mb);
+        ga.n_rows = Lb.i_n_rows.get() + s; ga.impala = 1; ga.obs_dyn = Lb.i_obs.get() + r0 * 11; ga.model = Lb.i_lmodel.get() + r0;
+        ga.mask = Lb.i_mask.get() + r0 * A; ga.action = Lb.i_action.get() + r0; ga.adv = Lb.i_pg.get() + r0; ga.vt = Lb.i_vs.get() + r0;
+        ga.vf_coeff = (float)cfg.vf_loss_coeff; ga.ent_coeff = (float)cfg.entropy_coeff;
+        adam[s] = pop_adam_args(q, cfg, s, Lb.i_n_rows.get() + s, mb);
+        adam[s].stats = Lb.i_stats.get() + (size_t)s * RAMP_IMPALA_STATS_LEN;
+        coef[2 * s] = cfg.vf_loss_coeff; coef[2 * s + 1] = cfg.entropy_coeff;
+    }
+    CUDA_TRY(cudaMemcpyAsync(q->d_vtrace.get(), vt.data(), sizeof(VtraceArgs) * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(q->d_grad.get(), grad.data(), sizeof(GradArgs) * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(q->d_adam.get(), adam.data(), sizeof(AdamArgs) * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(q->d_coef.get(), coef.data(), sizeof(double) * 2 * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));                                  // the vectors are pageable
+    // 1. every group's fragment rows, fragment-major
+    ImpalaBatchArgs ba{};
+    ba.T = n_steps; ba.B = b; ba.A = A; ba.L = L; ba.n_models = c.n_models;
+    ba.t_obs = p->t_obs.get(); ba.t_model = p->t_model.get(); ba.t_mask = p->t_mask.get(); ba.t_action = p->t_action.get();
+    ba.t_logp = p->t_logp.get(); ba.t_reward = p->t_reward.get(); ba.t_done = p->t_done.get();
+    ba.obs = Lb.i_obs.get(); ba.model = Lb.i_model.get(); ba.mask = Lb.i_mask.get(); ba.action = Lb.i_action.get();
+    ba.blogp = Lb.i_blogp.get(); ba.reward = Lb.i_reward.get(); ba.done = Lb.i_done.get(); ba.n_rows = Lb.i_n_rows.get();
+    ramp_pop_impala_batch_kernel<<<(unsigned)(((int64_t)K * R + 255) / 256), 256, 0, st>>>(ba, K);
+    CUDA_TRY(cudaGetLastError());
+    // 2. SGD step k of every set in the same launches
+    for (int k = 0; k < n_sgd; ++k) {
+        const int32_t start = k * mb, nf = std::min(F, n_frag - k * F);
+        // the rounds at the current weights, kept for the backward; from the second step on also the embeddings
+        EmbGradArgs ef{};
+        ef.n_rows = Lb.i_n_rows.get(); ef.start = start; ef.emb = k ? q->d_emb.get() : nullptr;
+        if ((rc = pop_launch_embed(q, st, ef, true)) != RAMP_OK) return rc;
+        // the read-out of the step's fragment rows at the current weights: rows [s R + start, s R + start + nf L) of set s
+        HeadArgs h{};
+        h.obs_dyn = Lb.i_obs.get() + (size_t)start * 11; h.graph_static = p->d_gstatic.get(); h.model = Lb.i_model.get() + start;
+        h.mask = Lb.i_mask.get() + (size_t)start * A; h.emb = q->d_emb.get(); h.logits = Lb.i_tlogits.get() + (size_t)start * A;
+        h.value = Lb.i_tvalue.get() + start; h.actions = Lb.i_actx.get() + start;
+        if ((rc = pop_launch_head(q, h, nf * L, nullptr, 0, st, R)) != RAMP_OK) return rc;
+        ramp_pop_vtrace_kernel<<<(unsigned)((K * nf + 7) / 8), 256, 0, st>>>(q->d_vtrace.get(), K, nf, start);
+        CUDA_TRY(cudaGetLastError());
+        if ((rc = pop_launch_grad(q, st, mb, start, q->d_keys.get(), 1)) != RAMP_OK) return rc;
+        ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_adam.get(), start, 0, Lb.parity, q->nw);
+        Lb.parity ^= 1;
+        ramp_pop_impala_step_stats_kernel<<<(K + 127) / 128, 128, 0, st>>>(Lb.row_stats.get(), Lb.row_model.get(), mb, start, Lb.i_log_rho.get(), R,
+                                                                          q->d_coef.get(), Lb.norm_part.get(), Lb.i_step_stats.get(), n_sgd, k, K);
+        CUDA_TRY(cudaGetLastError());
+    }
+    q->emb_valid = false;
+    Lb.i_rows = R;
+    // 3. every set's means over its steps: the call's one read-back
+    ramp_pop_impala_learn_stats_kernel<<<(K + 127) / 128, 128, 0, st>>>(Lb.i_step_stats.get(), n_sgd, Lb.i_stats.get(), K);
+    CUDA_TRY(cudaGetLastError());
+    ramp_internal_count_launches(eng, 2 + 9 * n_sgd);
+    if (stats_out) CUDA_TRY(cudaMemcpyAsync(stats_out, Lb.i_stats.get(), sizeof(double) * K * RAMP_IMPALA_STATS_LEN, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return fence_out(p, st);
+}
+
+int ramp_population_learn_pg(ramp_population_t* q, ramp_engine_t* eng, int32_t n_steps, const ramp_pg_config_t* cfgs, double* stats_out) {
+    int rc = pop_check_configs(q, cfgs);
+    if (rc != RAMP_OK) return rc;
+    ramp_policy* p = q->p;
+    const int32_t K = q->K;
+    ramp_env_buffers_t eb{};
+    cudaStream_t st;
+    if ((rc = pop_learn_begin(q, eng, cfgs, n_steps, &eb, &st)) != RAMP_OK) return rc;
+    const ramp_policy_config_t& c = p->P.c;
+    const int32_t b = eb.n_episodes / K, rows = n_steps * b, A = c.n_actions;
+    if ((rc = ensure_rows(q->L, p->P, rows, st)) || (rc = ensure_batch(q->L, c, rows))) return rc;
+    if (!q->emb_valid && (rc = pop_embed(q, st)) != RAMP_OK) return rc;
+    LearnerBuffers& Lb = q->L;
+    std::vector<GaeArgs> gae(K);
+    std::vector<GradArgs> grad(K);
+    std::vector<AdamArgs> adam(K);
+    for (int s = 0; s < K; ++s) {
+        const ramp_pg_config_t& cfg = cfgs[s];
+        const size_t r0 = (size_t)s * rows;
+        gae[s] = pop_gae_args(q, s, n_steps, b, cfg.gamma, 1.0, 0, nullptr);
+        GradArgs& ga = grad[s];
+        ga = pop_grad_args(q, s, rows);
+        ga.n_rows = Lb.n_rows.get() + s; ga.pg = 1; ga.obs_dyn = Lb.b_obs.get() + r0 * 11; ga.model = Lb.b_model.get() + r0;
+        ga.mask = Lb.b_mask.get() + r0 * A; ga.action = Lb.b_action.get() + r0; ga.adv = Lb.b_adv.get() + r0; ga.logp_old = Lb.b_logp_old.get() + r0;
+        adam[s] = pop_adam_args(q, cfg, s, Lb.n_rows.get() + s, rows);
+        adam[s].stats = Lb.stats.get() + (size_t)s * RAMP_PPO_STATS_LEN;
+    }
+    CUDA_TRY(cudaMemcpyAsync(q->d_gae.get(), gae.data(), sizeof(GaeArgs) * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(q->d_grad.get(), grad.data(), sizeof(GradArgs) * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(q->d_adam.get(), adam.data(), sizeof(AdamArgs) * K, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));                                  // the vectors are pageable
+    // 1. every group's discounted returns, its live rows t-major into its slice of the train batch
+    ramp_pop_gae_kernel<<<K, 1024, 0, st>>>(q->d_gae.get(), eb.n_episodes);
+    CUDA_TRY(cudaGetLastError());
+    // 2. the loss's gradient over each group's whole batch at the collection weights
+    EmbGradArgs ef{};
+    ef.n_rows = Lb.n_rows.get();
+    if ((rc = pop_launch_embed(q, st, ef, true)) != RAMP_OK || (rc = pop_launch_grad(q, st, rows, 0, q->d_keys.get(), 1)) != RAMP_OK) return rc;
+    // 3. one Adam step per set; a set with no row makes none and keeps its step count
+    ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_adam.get(), 0, 0, Lb.parity, q->nw);
+    Lb.parity ^= 1;
+    // 4. the statistics: the call's one read-back
+    ramp_pop_pg_stats_kernel<<<(K + 127) / 128, 128, 0, st>>>(Lb.row_stats.get(), Lb.row_model.get(), Lb.b_adv.get(), rows, Lb.n_rows.get(),
+                                                              Lb.norm_part.get(), Lb.stats.get(), K);
+    CUDA_TRY(cudaGetLastError());
+    q->emb_valid = false;
+    ramp_internal_count_launches(eng, 8);
+    if (stats_out)
+        CUDA_TRY(cudaMemcpy2DAsync(stats_out, sizeof(double) * RAMP_PG_STATS_LEN, Lb.stats.get(), sizeof(double) * RAMP_PPO_STATS_LEN,
+                                   sizeof(double) * RAMP_PG_STATS_LEN, K, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return fence_out(p, st);
+}
+
+int ramp_population_vtrace_read(ramp_population_t* q, int32_t set, int32_t* n_out, float* target_logp_out, float* log_rho_out, float* vs_out,
+                                float* pg_adv_out) {
+    int rc = pop_check_set(q, set);
+    if (rc != RAMP_OK) return rc;
+    if (!n_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (q->L.i_rows < 1) return set_error(RAMP_ERR_BAD_ARG, "population: no V-trace yet (ramp_population_learn_impala)");
+    CUDA_TRY(cudaSetDevice(q->p->device));
+    CUDA_TRY(cudaDeviceSynchronize());
+    const size_t n = q->L.i_rows, o = (size_t)set * n;
+    *n_out = q->L.i_rows;
+    if (target_logp_out) CUDA_TRY(cudaMemcpy(target_logp_out, q->L.i_tlogp.get() + o, 4 * n, cudaMemcpyDeviceToHost));
+    if (log_rho_out) CUDA_TRY(cudaMemcpy(log_rho_out, q->L.i_log_rho.get() + o, 4 * n, cudaMemcpyDeviceToHost));
+    if (vs_out) CUDA_TRY(cudaMemcpy(vs_out, q->L.i_vs.get() + o, 4 * n, cudaMemcpyDeviceToHost));
+    if (pg_adv_out) CUDA_TRY(cudaMemcpy(pg_adv_out, q->L.i_pg.get() + o, 4 * n, cudaMemcpyDeviceToHost));
+    return RAMP_OK;
 }
 
 int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_avg_out, float* exp_avg_sq_out, int32_t* step_out) {

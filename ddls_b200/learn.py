@@ -130,7 +130,10 @@ def _bind(L):
                        ('ramp_es_state', [C.c_void_p] * 4),
                        ('ramp_es_reset', [C.c_void_p]),
                        ('ramp_population_learn', [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CConfig), C.c_void_p]),
-                       ('ramp_population_learner_state', [C.c_void_p, C.c_int32] + [C.c_void_p] * 3)):
+                       ('ramp_population_learner_state', [C.c_void_p, C.c_int32] + [C.c_void_p] * 3),
+                       ('ramp_population_learn_impala', [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CIMPALAConfig), C.c_void_p]),
+                       ('ramp_population_learn_pg', [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CPGConfig), C.c_void_p]),
+                       ('ramp_population_vtrace_read', [C.c_void_p, C.c_int32] + [C.c_void_p] * 5)):
         getattr(L, name).restype = C.c_int
         getattr(L, name).argtypes = args
     L.ramp_es_destroy.restype = None
@@ -225,24 +228,48 @@ class DevicePPOLearner(_GradientLearner):
         return _stats(STATS, out), grad
 
 
-class DevicePopulationPPOLearner:
-    """DevicePPOLearner for every set of a DeviceGNNPolicyPopulation at once: group k of the environment learns only from its own
-    episodes with configs[k], and ends each call with the weights, Adam state, statistics and kl_coeff a DevicePPOLearner with
-    configs[k] would reach on a group-sized environment with the same episode streams, bit for bit.  Every minibatch step runs
-    all K sets in the same launches.  sgd_minibatch_size and num_sgd_iter set that launch loop, so the K configs must agree on them."""
+class _PopulationLearner:
+    """What the population's PPO, IMPALA and PG learners share: one config per set, the fields every set must agree on (they set
+    the launch loop), each config's own checks before anything runs, and Adam's moments and step counts, which are the
+    population's -- one per set, whichever of the three learners made the step."""
+    _shared = ()                      # config fields every set must share
+    _checks = ()                      # (field, predicate, rule): each config's own rules, as the C learner checks them
 
     def __init__(self, population, configs):
         configs = [dataclasses.replace(c) for c in configs]
         if len(configs) != population.K:
             raise ValueError(f'{len(configs)} configs for a population of {population.K} sets')
-        for name in ('sgd_minibatch_size', 'num_sgd_iter'):
+        for name in self._shared:
             values = [getattr(c, name) for c in configs]
             if len(set(values)) > 1:
-                raise ValueError(f'{name} must be the same for every set (it sets the launch loop): {values}')
+                k = next(k for k, v in enumerate(values) if v != values[0])
+                raise ValueError(f'{name} must be the same for every set (it sets the launch loop): {values}; set {k} differs from set 0')
+        for k, c in enumerate(configs):
+            for name, ok, rule in self._checks:
+                if not ok(getattr(c, name)):
+                    raise ValueError(f'set {k}: {name} = {getattr(c, name)} (it must be {rule})')
         self.population, self.configs = population, configs
-        self._calls = 0
         self._L = population._L
         _bind(self._L)
+
+    def adam_state(self, k: int):
+        """set k's torch.optim.Adam state: exp_avg, exp_avg_sq (blob order) and the step count"""
+        n = self._L.ramp_policy_weight_count(C.byref(self.population.template._cfg))
+        m, v, step = np.zeros(n, np.float32), np.zeros(n, np.float32), C.c_int32()
+        _engine._check(self._L.ramp_population_learner_state(self.population._h, int(k), m.ctypes.data, v.ctypes.data, C.byref(step)))
+        return m, v, step.value
+
+
+class DevicePopulationPPOLearner(_PopulationLearner):
+    """DevicePPOLearner for every set of a DeviceGNNPolicyPopulation at once: group k of the environment learns only from its own
+    episodes with configs[k], and ends each call with the weights, Adam state, statistics and kl_coeff a DevicePPOLearner with
+    configs[k] would reach on a group-sized environment with the same episode streams, bit for bit.  Every minibatch step runs
+    all K sets in the same launches.  sgd_minibatch_size and num_sgd_iter set that launch loop, so the K configs must agree on them."""
+    _shared = ('sgd_minibatch_size', 'num_sgd_iter')
+
+    def __init__(self, population, configs):
+        super().__init__(population, configs)
+        self._calls = 0
 
     def learn(self, env, horizon: int):
         """One PPO learner step per set on the first ``horizon`` steps of the population's last collect(env, ...): a list of K stats
@@ -257,13 +284,6 @@ class DevicePopulationPPOLearner:
         for c, s in zip(self.configs, stats):
             c.kl_coeff = s['kl_coeff']
         return stats
-
-    def adam_state(self, k: int):
-        """set k's torch.optim.Adam state: exp_avg, exp_avg_sq (blob order) and the step count"""
-        n = self._L.ramp_policy_weight_count(C.byref(self.population.template._cfg))
-        m, v, step = np.zeros(n, np.float32), np.zeros(n, np.float32), C.c_int32()
-        _engine._check(self._L.ramp_population_learner_state(self.population._h, int(k), m.ctypes.data, v.ctypes.data, C.byref(step)))
-        return m, v, step.value
 
 
 class DeviceIMPALALearner(_GradientLearner):
@@ -362,6 +382,53 @@ class DevicePGLearner(_GradientLearner):
                                                  gf.ctypes.data, mask.ctypes.data, act.ctypes.data, adv.ctypes.data, grad.ctypes.data,
                                                  out.ctypes.data))
         return _stats(PG_STATS, out), grad
+
+
+class DevicePopulationIMPALALearner(_PopulationLearner):
+    """DeviceIMPALALearner for every set of a DeviceGNNPolicyPopulation at once: group k learns only from its own episodes with
+    configs[k], and ends each call with the weights, Adam state, statistics and V-trace values a DeviceIMPALALearner with configs[k]
+    would reach on a group-sized environment with the same episode streams, bit for bit.  SGD step j of every set runs in the same
+    launches.  rollout_fragment_length and train_batch_size fix the fragments and the SGD steps, so the K configs must agree on
+    them; gamma, the clip thresholds, the loss coefficients, grad_clip and Adam's settings are each set's own."""
+    _shared = ('rollout_fragment_length', 'train_batch_size')
+    _checks = (('vtrace_clip_rho_threshold', lambda v: v > 0, '> 0'), ('vtrace_clip_pg_rho_threshold', lambda v: v > 0, '> 0'),
+               ('lr', lambda v: v >= 0, '>= 0'), ('adam_eps', lambda v: v > 0, '> 0'),
+               ('rollout_fragment_length', lambda v: v >= 0, '>= 0'), ('train_batch_size', lambda v: v >= 1, '>= 1'))
+
+    def learn(self, env, horizon: int):
+        """One IMPALA learner step per set on the first ``horizon`` steps of the population's last collect(env, ...): a list of K
+        stats dicts (IMPALA_STATS), each the means over its set's SGD steps."""
+        pop = self.population
+        pop.group_size(env)
+        cfgs = (_CIMPALAConfig * pop.K)(*[_c_struct(_CIMPALAConfig, c) for c in self.configs])
+        out = np.zeros((pop.K, len(IMPALA_STATS)), dtype=np.float64)
+        _engine._check(self._L.ramp_population_learn_impala(pop._h, env.eng._h, int(horizon), cfgs, out.ctypes.data))
+        return [_stats(IMPALA_STATS, row) for row in out]
+
+    def vtrace(self, k: int) -> Dict[str, np.ndarray]:
+        """set k's per fragment row values of the last learn(), as DeviceIMPALALearner.vtrace() gives them for its group"""
+        n = C.c_int32()
+        _engine._check(self._L.ramp_population_vtrace_read(self.population._h, int(k), C.byref(n), None, None, None, None))
+        arrs = {key: np.zeros(n.value, np.float32) for key in ('target_logp', 'log_rho', 'vs', 'pg_advantages')}
+        _engine._check(self._L.ramp_population_vtrace_read(self.population._h, int(k), C.byref(n), *[a.ctypes.data for a in arrs.values()]))
+        return arrs
+
+
+class DevicePopulationPGLearner(_PopulationLearner):
+    """DevicePGLearner for every set of a DeviceGNNPolicyPopulation at once: group k learns only from its own episodes with
+    configs[k], and ends each call with the weights, Adam state and statistics a DevicePGLearner with configs[k] would reach on a
+    group-sized environment with the same episode streams, bit for bit.  Nothing has to agree across the configs."""
+    _checks = (('gamma', lambda v: v >= 0, '>= 0'), ('lr', lambda v: v >= 0, '>= 0'), ('adam_eps', lambda v: v > 0, '> 0'))
+
+    def learn(self, env, horizon: int):
+        """One PG learner step per set on the first ``horizon`` steps of the population's last collect(env, ...): a list of K stats
+        dicts (PG_STATS).  A group whose segment has no decision makes no update and keeps its step count."""
+        pop = self.population
+        pop.group_size(env)
+        cfgs = (_CPGConfig * pop.K)(*[_c_struct(_CPGConfig, c) for c in self.configs])
+        out = np.zeros((pop.K, len(PG_STATS)), dtype=np.float64)
+        _engine._check(self._L.ramp_population_learn_pg(pop._h, env.eng._h, int(horizon), cfgs, out.ctypes.data))
+        return [_stats(PG_STATS, row) for row in out]
 
 
 ES_STATS = ('episode_reward_mean', 'episode_len_mean', 'timesteps_this_iter', 'episodes_this_iter', 'weights_norm', 'grad_norm',

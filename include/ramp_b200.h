@@ -884,10 +884,10 @@ int ramp_es_act_read(ramp_es_t* es, ramp_engine_t* eng, float* logits_out, float
 int ramp_es_state(ramp_es_t* es, float* m_out, float* v_out, int32_t* t_out);
 int ramp_es_reset(ramp_es_t* es);
 
-/* ---- A population of K independent PPO trainings in one environment batch.  The environment's B = K b episodes are K contiguous
- * groups of b; group k acts with weight set k and learns only from its own episodes with its own ramp_ppo_config_t.  Group k
- * computes, bit for bit, what one policy holding set k's weights (ramp_policy_act, ramp_policy_learn with config k) computes on a
- * b-episode environment with the same episode streams.  The kernels run every group in the same launches: the MeanPool rounds
+/* ---- A population of K independent PPO, IMPALA or PG trainings in one environment batch.  The environment's B = K b episodes
+ * are K contiguous groups of b; group k acts with weight set k and learns only from its own episodes with its own config.  Group
+ * k computes, bit for bit, what one policy holding set k's weights (ramp_policy_act, ramp_policy_learn* with config k) computes
+ * on a b-episode environment with the same episode streams.  The kernels run every group in the same launches: the MeanPool rounds
  * and their backward on one CTA per (set, job type) item, grid-strided past the resident CTAs; no float atomics. */
 typedef struct ramp_population ramp_population_t;
 /* K = n_sets weight sets with p's configuration and job types, each a copy of p's current weights, and K Adam states at zero.  p
@@ -904,6 +904,20 @@ int ramp_population_act(ramp_population_t* q, ramp_engine_t* eng, int32_t sample
 /* ramp_policy_learn for every group on its columns of the template's trajectory, with cfgs[k] (HOST, [n_sets]); every config must
  * have the same sgd_minibatch_size and num_sgd_iter.  stats_out: [n_sets][RAMP_PPO_STATS_LEN] or NULL. */
 int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_steps, const ramp_ppo_config_t* cfgs, double* stats_out);
+/* ramp_policy_learn_impala for every group on its columns of the template's trajectory, with cfgs[k] (HOST, [n_sets]).  Group k's
+ * fragments are ordered as a b-episode environment's: time block by time block, then episode.  rollout_fragment_length and
+ * train_batch_size fix the SGD steps, so every config must have the same values; gamma, the clip thresholds, the loss
+ * coefficients, grad_clip and Adam's settings are the set's own.  SGD step k of every set runs in the same launches.  Adam's
+ * moments and step counts are the population's, the same state ramp_population_learn updates.  stats_out:
+ * [n_sets][RAMP_IMPALA_STATS_LEN] or NULL.  A configuration error names the set. */
+int ramp_population_learn_impala(ramp_population_t* q, ramp_engine_t* eng, int32_t n_steps, const ramp_impala_config_t* cfgs, double* stats_out);
+/* ramp_policy_learn_pg for every group on its columns of the template's trajectory, with cfgs[k] (HOST, [n_sets]); nothing has to
+ * agree across sets.  A group whose batch has no row makes no update and keeps its step count.  stats_out:
+ * [n_sets][RAMP_PG_STATS_LEN] or NULL.  A configuration error names the set. */
+int ramp_population_learn_pg(ramp_population_t* q, ramp_engine_t* eng, int32_t n_steps, const ramp_pg_config_t* cfgs, double* stats_out);
+/* ramp_impala_vtrace_read for set k after the last ramp_population_learn_impala: its group's n_out fragment rows */
+int ramp_population_vtrace_read(ramp_population_t* q, int32_t set, int32_t* n_out, float* target_logp_out, float* log_rho_out,
+                                float* vs_out, float* pg_adv_out);
 /* HOST copies of set k's Adam state, as ramp_policy_learner_state */
 int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_avg_out, float* exp_avg_sq_out, int32_t* step_out);
 /* the CTAs of the population's MeanPool launches: n_sets n_models items, at most the resident CTAs, each CTA runs items

@@ -1,13 +1,17 @@
-"""K PPO trainings in one batch on a config-3-like environment (64 workers, ResNet-50): learn-call and minibatch-step time of
-DevicePopulationPPOLearner against K sequential DevicePPOLearner calls, and every set's mean return per iteration.
+"""K PPO, IMPALA or PG trainings in one batch on a config-3-like environment (64 workers, ResNet-50): learn-call and
+minibatch-step time of DevicePopulation{PPO,IMPALA,PG}Learner against K sequential single-learner calls, and every set's mean
+return per iteration.
 
     python scripts/population_train.py --out profiles/h100_population_ppo_train.jsonl
+    python scripts/population_train.py --algo impala --out profiles/h100_population_impala_train.jsonl
+    python scripts/population_train.py --algo pg --out profiles/h100_population_pg_train.jsonl
 
-Timing rows ('kind': 'timing'): for each K, one collect on a K b-episode environment (b episodes per group) with ppo.yaml's
-settings except num_sgd_iter, then learn calls timed with a device synchronise around each, alternating with the single
-learner's call on a b-episode environment; the single call is timed once per repeat and multiplied by K (the K sequential calls
-would do the same work K times).  minibatch_step_ms is the call's time over its minibatch steps (num_sgd_iter x minibatches).
-Each measurement repeats `--repeats` times.  Return rows ('kind': 'returns'): a grid over lr x entropy_coeff, --iters iterations
+Timing rows ('kind': 'timing'): for each K, one collect on a K b-episode environment (b episodes per group) with the algorithm's
+settings (ppo.yaml's except num_sgd_iter; IMPALAConfig's, PGConfig's), then learn calls timed with a device synchronise around
+each, alternating with the single learner's call on a b-episode environment; the single call is timed once per repeat and
+multiplied by K (the K sequential calls would do the same work K times).  minibatch_step_ms is the call's time over its minibatch
+steps (PPO: num_sgd_iter x minibatches; IMPALA: its SGD steps; PG: its one step).  Each measurement repeats `--repeats` times.
+Return rows ('kind': 'returns'): a grid over lr x entropy_coeff (PG, which has no entropy term: lr x gamma), --iters iterations
 of collect + learn, each set's mean episode return (the group's summed rewards over its episodes).  The first row names the card,
 its power limit and max SM clock, read in the same process."""
 import argparse
@@ -45,69 +49,87 @@ def timed(fn, sync):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument('--algo', choices=('ppo', 'impala', 'pg'), default='ppo')
     ap.add_argument('--ks', default='1,8,32,128')
     ap.add_argument('--b', type=int, default=128, help='episodes per group')
     ap.add_argument('--horizon', type=int, default=4)
     ap.add_argument('--jobs', type=int, default=4)
-    ap.add_argument('--num-sgd-iter', type=int, default=1, help='ppo.yaml has 50; the timed calls run this many passes')
+    ap.add_argument('--num-sgd-iter', type=int, default=1, help='ppo: ppo.yaml has 50; the timed calls run this many passes')
     ap.add_argument('--repeats', type=int, default=3)
     ap.add_argument('--grid-k', type=int, default=8)
     ap.add_argument('--iters', type=int, default=5)
-    ap.add_argument('--out', default='profiles/h100_population_ppo_train.jsonl')
+    ap.add_argument('--out', default=None, help='default: profiles/h100_population_<algo>_train.jsonl')
     a = ap.parse_args()
     import torch
-    from ddls_b200 import policy as P, workload
-    from ddls_b200.learn import DevicePopulationPPOLearner, DevicePPOLearner, PPOConfig
+    from ddls_b200 import learn, policy as P, workload
     if not torch.cuda.is_available():
         raise SystemExit('population_train.py measures on the GPU; no CUDA device is visible')
     sync = torch.cuda.synchronize
     graphs = [workload.make_graph('resnet')]
     A = 17
-    cfg0 = P.algo_model_config('ppo', A)
-    base = PPOConfig(num_sgd_iter=a.num_sgd_iter)
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    out = open(a.out, 'w')
+    cfg0 = P.algo_model_config(a.algo, A)
+    Pop, Single, base = {'ppo': (learn.DevicePopulationPPOLearner, learn.DevicePPOLearner, learn.PPOConfig(num_sgd_iter=a.num_sgd_iter)),
+                         'impala': (learn.DevicePopulationIMPALALearner, learn.DeviceIMPALALearner, learn.IMPALAConfig()),
+                         'pg': (learn.DevicePopulationPGLearner, learn.DevicePGLearner, learn.PGConfig())}[a.algo]
+    seeded = (lambda c, k: dataclasses.replace(c, seed=k)) if a.algo == 'ppo' else (lambda c, k: c)
+    out_path = a.out or f'profiles/h100_population_{a.algo}_train.jsonl'
+    os.makedirs(os.path.dirname(os.path.abspath(out_path)), exist_ok=True)
+    out = open(out_path, 'w')
 
     def emit(row):                                               # written as measured: a cut-short run keeps what it measured
         print(json.dumps(row), flush=True)
         out.write(json.dumps(row) + '\n')
         out.flush()
 
-    emit(dict(kind='card', **card(), b=a.b, horizon=a.horizon, jobs=a.jobs, num_sgd_iter=a.num_sgd_iter,
-              sgd_minibatch_size=base.sgd_minibatch_size))
+    def steps(rows):
+        """the minibatch / SGD steps of one call on a group of `rows` rows"""
+        if a.algo == 'ppo':
+            return -(-rows // base.sgd_minibatch_size) * a.num_sgd_iter
+        if a.algo == 'impala':
+            L = base.rollout_fragment_length or a.horizon
+            n_frag = rows // L
+            return -(-n_frag // min(base.train_batch_size // L, n_frag))
+        return 1
+
+    head = dict(kind='card', **card(), **({} if a.algo == 'ppo' else dict(algo=a.algo)), b=a.b, horizon=a.horizon, jobs=a.jobs)
+    if a.algo == 'ppo':
+        head.update(num_sgd_iter=a.num_sgd_iter, sgd_minibatch_size=base.sgd_minibatch_size)
+    elif a.algo == 'impala':
+        head.update(rollout_fragment_length=base.rollout_fragment_length, train_batch_size=base.train_batch_size)
+    emit(head)
     # the single learner on a b-episode environment
     senv = env_of(graphs, a.b, a.jobs, seed=1)
     spol = P.DeviceGNNPolicy(graphs, A, cfg0, P.random_state_dict(cfg0, A, seed=0))
-    slrn = DevicePPOLearner(spol, base)
+    slrn = Single(spol, base)
     spol.collect(senv, a.horizon, seed=0)
     slrn.learn(senv, a.horizon)                                  # warm-up
     for K in [int(k) for k in a.ks.split(',')]:
         env = env_of(graphs, K * a.b, a.jobs, seed=1)
         pop = P.DeviceGNNPolicyPopulation(graphs, A, cfg0, [P.random_state_dict(cfg0, A, seed=k) for k in range(K)])
-        lrn = DevicePopulationPPOLearner(pop, [dataclasses.replace(base, seed=k) for k in range(K)])
+        lrn = Pop(pop, [seeded(base, k) for k in range(K)])
         pop.collect(env, a.horizon, seed=list(range(K)))
         lrn.learn(env, a.horizon)                                # warm-up: every buffer and launch shape
         for r in range(a.repeats):
             tp, stats = timed(lambda: lrn.learn(env, a.horizon), sync)
             ts, _ = timed(lambda: slrn.learn(senv, a.horizon), sync)
-            n_mb = -(-(a.horizon * a.b) // base.sgd_minibatch_size) * a.num_sgd_iter
+            n_mb = steps(a.horizon * a.b)
             emit(dict(kind='timing', K=K, repeat=r, population_learn_s=tp, population_minibatch_step_ms=1e3 * tp / n_mb,
                       single_learn_s=ts, single_x_K_learn_s=ts * K, single_minibatch_step_ms=1e3 * ts / n_mb,
                       embed_ctas=pop.embed_ctas(), train_rows=[int(s['rows']) for s in stats][:4]))
         pop.close()
         del env
-    # returns: a grid over lr x entropy_coeff
-    lrs, ents = [1e-4, 3e-4, 1e-3, 3e-3], [0.0, 0.01]
-    grid = [(lr, e) for lr in lrs for e in ents][:a.grid_k]
+    # returns: a grid over lr x entropy_coeff (PG: lr x gamma)
+    lrs, second = [1e-4, 3e-4, 1e-3, 3e-3], ('gamma', [0.99, 0.9]) if a.algo == 'pg' else ('entropy_coeff', [0.0, 0.01])
+    grid = [(lr, e) for lr in lrs for e in second[1]][:a.grid_k]
     K = len(grid)
     env = env_of(graphs, K * a.b, a.jobs, seed=2)
     pop = P.DeviceGNNPolicyPopulation(graphs, A, cfg0, [P.random_state_dict(cfg0, A, seed=0)] * K)
-    lrn = DevicePopulationPPOLearner(pop, [dataclasses.replace(base, lr=lr, entropy_coeff=e, seed=k) for k, (lr, e) in enumerate(grid)])
+    lrn = Pop(pop, [seeded(dataclasses.replace(base, lr=lr, **{second[0]: e}), k) for k, (lr, e) in enumerate(grid)])
     for it in range(a.iters):
         traj = pop.collect(env, a.jobs, seed=[100 * it + k for k in range(K)])
         ret = (traj['reward'] * traj['live']).sum(axis=0).reshape(K, a.b).mean(axis=1)
         lrn.learn(env, a.jobs)
-        emit(dict(kind='returns', iteration=it, sets=[dict(lr=lr, entropy_coeff=e, mean_return=float(x)) for (lr, e), x in zip(grid, ret)]))
+        emit(dict(kind='returns', iteration=it, sets=[{'lr': lr, second[0]: e, 'mean_return': float(x)} for (lr, e), x in zip(grid, ret)]))
     pop.close()
     out.close()
 
