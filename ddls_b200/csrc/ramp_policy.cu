@@ -686,12 +686,13 @@ uint64_t mix64(uint64_t x) {              // splitmix64, as the kernels' splitmi
 
 int64_t gnn_weight_count(const ramp_policy* p) { return p->P.gln_w; }     // the rounds come first in the blob
 
-// L's gradient, Adam state (zeroed), job-type partials, norm partials and statistics for the K sets of p's configuration
-int ensure_learner(LearnerBuffers& L, const ramp_policy* p) {
+// L's gradient, Adam state (zeroed), job-type partials, norm partials and statistics for K sets: n weights and n_gpart job-type
+// partials in all
+int ensure_learner(LearnerBuffers& L, size_t n, size_t n_gpart) {
     if (L.ready) return RAMP_OK;
-    const size_t K = L.K, n = K * (size_t)p->n_weights;
+    const size_t K = L.K;
     CUDA_TRY(alloc_each(n, L.grad, L.adam_m, L.adam_v));
-    CUDA_TRY(L.gpart.alloc(K * p->P.c.n_models * gnn_weight_count(p)));
+    CUDA_TRY(L.gpart.alloc(n_gpart));
     CUDA_TRY(L.n_rows.alloc(K));
     CUDA_TRY(L.step.alloc(2 * K));
     CUDA_TRY(L.norm_part.alloc(K * LRN_GRID));
@@ -806,7 +807,9 @@ int ensure_ppo(LearnerBuffers& L, int32_t B, int32_t n_mb) {
 // and per-row scratch for minibatches of `rows` rows
 int prepare_learner(ramp_policy* p, cudaStream_t st, int32_t rows) {
     int rc;
-    if ((rc = fence_in(p, st)) != RAMP_OK || (rc = ensure_learner(p->L, p)) != RAMP_OK || (rc = ensure_gmodels(p, st)) != RAMP_OK) return rc;
+    if ((rc = fence_in(p, st)) != RAMP_OK || (rc = ensure_learner(p->L, p->n_weights, (size_t)p->P.c.n_models * gnn_weight_count(p))) != RAMP_OK ||
+        (rc = ensure_gmodels(p, st)) != RAMP_OK)
+        return rc;
     if (!p->emb_valid && (rc = launch_embed(p, st)) != RAMP_OK) return rc;
     return ensure_rows(p->L, p->P, rows, st);
 }

@@ -2,8 +2,10 @@
 // ramp_population_*).  Included by ramp_policy.cu after the learner.
 //
 // The environment's B = K b episodes are K contiguous groups of b; group k acts with weight set k and learns only from its own
-// episodes with its own config.  Every kernel here runs the statements of the single policy's kernel (the shared *_body
-// functions of ramp_policy.cu / ramp_policy_learn.cuh) on one set's slice, with the set taken from the launch:
+// episodes with its own config.  The sets may differ in shape: set k has its own ramp_policy_config_t, and the kernels that depend
+// on it take set k's entry of the device table d_sets (PopSet: its PolicyDev with `w` at its weights, and its slices of the ragged
+// buffers).  Every kernel here runs the statements of the single policy's kernel (the shared *_body functions of ramp_policy.cu /
+// ramp_policy_learn.cuh) on one set's slice, with the set taken from the launch:
 //
 //   ramp_pop_embed_grad_kernel   persistent CTAs over (set, job type) items, grid-strided past the resident CTAs: the MeanPool
 //                                rounds (forward: states kept, embeddings [K][n_models][out_node]) or their backward
@@ -11,7 +13,8 @@
 //   ramp_pop_gae_kernel          one 1,024-thread CTA per group: GAE (PG: discounted returns) over the group's columns of the
 //                                [T][B] trajectory, its live rows t-major into the group's slice of the train batch,
 //                                standardised with the group's mean / std when asked
-//   ramp_pop_head_grad_kernel    one warp per (set, launch row): the rows of every group's minibatch / SGD step in one launch
+//   ramp_pop_head_grad_kernel    blockIdx.y = set, one warp per launch row: the rows of every group's minibatch / SGD step in one
+//                                launch
 //   ramp_pop_head_reduce_kernel  one thread per (set, read-out weight): the sum over the set's rows in row order
 //   ramp_pop_finish_kernel / ramp_pop_adam_kernel   blockIdx.y = set: the job types' sum, the norm partials, clip and Adam
 //   ramp_pop_learn_stats_kernel  one thread per set: the last pass's means and update_kl
@@ -25,55 +28,78 @@
 
 namespace ramp {
 
+// set s of a population: its configuration's layout with `w` at its own weights -- the PolicyDev the single policy's kernels take
+// -- and where its slices of the population's ragged buffers start.  Kernels serving one set per CTA stage the entry in shared
+// memory (pop_stage_set) and run the bodies on it.
+struct PopSet {
+    PolicyDev P;
+    int64_t n_w, w_off;                   // weights; their offset in every [sum n_w] buffer (weights, gradient, Adam's m / v)
+    int64_t n_gnn, gpart_off;             // the rounds' weights; set s's [n_models][n_gnn] job-type partials
+    int64_t emb_off;                      // set s's [n_models][out_node] embeddings
+};
+
+// sets[s] into shared `dst` by the whole CTA, word by word (the caller syncs before `dst` is rewritten)
+__device__ __forceinline__ void pop_stage_set(const PopSet* sets, int s, PopSet* dst) {
+    const int32_t* src = reinterpret_cast<const int32_t*>(sets + s);
+    int32_t* d = reinterpret_cast<int32_t*>(dst);
+    for (int i = threadIdx.x; i < (int)(sizeof(PopSet) / 4); i += blockDim.x) d[i] = src[i];
+    __syncthreads();
+}
+
 struct PopHead {
     int32_t per;                          // episodes / rows of one set
     int32_t stride;                       // rows from one set's first to the next's (per, or a set's whole batch when the launch
                                           // covers a slice of it)
-    int64_t n_weights;
     const unsigned long long* seeds;      // [K] the sets' act seeds (sample), mixed with `mix` as ramp_policy_act mixes its call count
     unsigned long long mix;
 };
 
-__global__ void __launch_bounds__(256, 3) ramp_pop_head_kernel(const PolicyDev P, const HeadArgs base, const PopHead ph) {
+// dynamic shared memory: the largest set's read-out staging.  The set's configuration is read from shared memory, not the constant
+// bank as in ramp_policy_head_kernel, and needs about 30 more registers: at 80 (three CTAs per SM) ptxas spills about 900 bytes
+__global__ void __launch_bounds__(256, 2) ramp_pop_head_kernel(const PopSet* sets, const HeadArgs base, const PopHead ph) {
+    __shared__ PopSet S;
     const int s = blockIdx.y;
-    const size_t o = (size_t)s * ph.stride, A = P.c.n_actions;
+    pop_stage_set(sets, s, &S);
+    const size_t o = (size_t)s * ph.stride, A = S.P.c.n_actions;
     HeadArgs a = base;
     a.n = ph.per;
     a.model += o; a.mask += o * A; a.actions += o;
     if (a.obs_dyn) a.obs_dyn += o * 11;
-    if (a.graph_features) a.graph_features += o * P.c.in_features_graph;
+    if (a.graph_features) a.graph_features += o * S.P.c.in_features_graph;
     if (a.done) a.done += o;
     if (a.logits) a.logits += o * A;
     if (a.value) a.value += o;
     if (a.logp) a.logp += o;
-    a.emb += (size_t)s * P.c.n_models * P.c.out_features_node;
+    a.emb += S.emb_off;
     if (a.sample) a.seed = ph.seeds[s] ^ ph.mix;
-    head_body(P, P.w + (size_t)s * ph.n_weights, a, blockIdx.x, gridDim.x);
+    head_body(S.P, S.P.w, a, blockIdx.x, gridDim.x);
 }
 
 struct PopEmbed {
-    int32_t K;
-    int64_t n_weights;
-    int32_t rec_stride;                   // backward: floats per head record
+    int32_t K, n_models;
+    int32_t rec_stride;                   // backward: floats per head record of the launch (the largest set's)
 };
 
 // item = set n_models + job type; the forward's n_rows / emb and the backward's records and partials are the set's slices
 template <int MODE>
-__global__ void __launch_bounds__(256, 1) ramp_pop_embed_grad_kernel(const PolicyDev P, const ModelDev* models, const GradModelDev* gms,
+__global__ void __launch_bounds__(256, 1) ramp_pop_embed_grad_kernel(const PopSet* sets, const ModelDev* models, const GradModelDev* gms,
                                                                      const EmbGradArgs g, const PopEmbed pe) {
-    const int nm = P.c.n_models;
+    __shared__ PopSet S;
+    const int nm = pe.n_models;
     for (int item = blockIdx.x; item < pe.K * nm; item += gridDim.x) {
         const int s = item / nm, m = item - s * nm;
+        pop_stage_set(sets, s, &S);
         EmbGradArgs e = g;
         if (MODE == EMB_FORWARD) {
             if (e.n_rows) e.n_rows += s;
-            if (e.emb) e.emb += (size_t)s * nm * P.c.out_features_node;
+            if (e.emb) e.emb += S.emb_off;
         } else {
             e.rec += (size_t)s * e.rows * pe.rec_stride;
             e.row_model += (size_t)s * e.rows;
-            e.gpart += (size_t)s * nm * e.n_gnn;
+            e.gpart += S.gpart_off;
+            e.n_gnn = S.n_gnn;
         }
-        embed_grad_body<MODE>(P, P.w + (size_t)s * pe.n_weights, models, gms + (size_t)s * nm, e, m);
+        embed_grad_body<MODE>(S.P, S.P.w, models, gms + (size_t)s * nm, e, m);
         __syncthreads();                  // the next item reuses the shared staging
     }
 }
@@ -83,43 +109,52 @@ __global__ void __launch_bounds__(1024) ramp_pop_gae_kernel(const GaeArgs* sets,
     gae_body(a, ld);
 }
 
-// sets[k]: group k's GradArgs for a minibatch starting at 0 (records, row model and statistics already at k mb); keys: the pass's [K]
-__global__ void __launch_bounds__(256) ramp_pop_head_grad_kernel(const PolicyDev P, const GradArgs* sets, int32_t K, int32_t mb, int32_t start,
-                                                                 const unsigned long long* keys, int32_t first_pass, int64_t n_weights) {
-    const int gi = blockIdx.x * LRN_WARPS + (threadIdx.x >> 5);
-    if (gi >= K * mb) return;
-    const int s = gi / mb;
-    GradArgs g = sets[s];
-    g.start = start; g.key = keys[s];
-    if (!first_pass) g.logp_old = nullptr;
-    head_grad_body(P, P.w + (size_t)s * n_weights, g, gi - s * mb);
+// blockIdx.y = set: args[k] is group k's GradArgs for a minibatch starting at 0 (records, row model and statistics already at k mb);
+// keys: the pass's [K]
+__global__ void __launch_bounds__(256) ramp_pop_head_grad_kernel(const PopSet* sets, const GradArgs* args, int32_t start,
+                                                                 const unsigned long long* keys, int32_t first_pass) {
+    __shared__ PopSet S;
+    __shared__ GradArgs g;                // in shared memory too: in registers beside the set's fields it spills
+    const int s = blockIdx.y;
+    if (threadIdx.x == 0) {
+        g = args[s];
+        g.start = start; g.key = keys[s];
+        if (!first_pass) g.logp_old = nullptr;
+    }
+    pop_stage_set(sets, s, &S);
+    head_grad_body(S.P, S.P.w, g, blockIdx.x * LRN_WARPS + (threadIdx.x >> 5));
 }
 
-// ramp_policy_head_reduce_kernel per set: segs hold set 0's records; set k's are k rec_shift floats further, its gradient and
-// weights k n_weights further
-__global__ void __launch_bounds__(256) ramp_pop_head_reduce_kernel(const PolicyDev P, const Seg* segs, int32_t n_segs, int64_t total, int32_t K,
-                                                                   int64_t rec_shift, int64_t n_weights, float* grad) {
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < K * total; e += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t s = e / total;
+// ramp_policy_head_reduce_kernel over every set: one thread per (set, read-out weight).  segs: [K][HEAD_SEGS] set s's segments on
+// its own records, their blob offsets into the population's weights `w`; n_segs: [K]; first: [K] set s's first thread
+__global__ void __launch_bounds__(256) ramp_pop_head_reduce_kernel(const Seg* segs, const int32_t* n_segs, const int64_t* first, int32_t K,
+                                                                   int64_t total, const float* w, float* grad) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+        int s = 0, hi = K - 1;
+        while (s < hi) {                                            // the last set starting at or before e
+            const int mid = (s + hi + 1) >> 1;
+            if (first[mid] <= e) s = mid; else hi = mid - 1;
+        }
+        const Seg* ss = segs + (size_t)s * HEAD_SEGS;
+        const int n = n_segs[s];
         int si = 0;
-        int64_t off = e - s * total;
-        while (si + 1 < n_segs && off >= seg_size(segs[si])) { off -= seg_size(segs[si]); ++si; }
-        Seg sg = segs[si];
-        sg.rec += s * rec_shift;
-        grad[s * n_weights + sg.w + off] = seg_element(sg, off, P.w + s * n_weights);
+        int64_t off = e - first[s];
+        while (si + 1 < n && off >= seg_size(ss[si])) { off -= seg_size(ss[si]); ++si; }
+        grad[ss[si].w + off] = seg_element(ss[si], off, w);
     }
 }
 
-__global__ void __launch_bounds__(256) ramp_pop_finish_kernel(const float* gpart, int32_t n_models, int64_t n_gnn, int64_t n_w, float* grad, double* norm_part) {
+__global__ void __launch_bounds__(256) ramp_pop_finish_kernel(const PopSet* sets, const float* gpart, int32_t n_models, float* grad, double* norm_part) {
     const size_t s = blockIdx.y;
-    grad_finish_body(gpart + s * n_models * n_gnn, n_models, n_gnn, n_w, grad + s * n_w, norm_part + s * LRN_GRID);
+    const PopSet& S = sets[s];
+    grad_finish_body(gpart + S.gpart_off, n_models, S.n_gnn, S.n_w, grad + S.w_off, norm_part + s * LRN_GRID);
 }
 
-// sets[k]: group k's AdamArgs for minibatch 0 of a pass; minibatch j starts at `start` and writes its statistics j rows further
-__global__ void __launch_bounds__(256) ramp_pop_adam_kernel(const AdamArgs* sets, int32_t start, int32_t j, int32_t parity, int64_t n_w) {
-    AdamArgs a = sets[blockIdx.y];
+// args[k]: group k's AdamArgs for minibatch 0 of a pass; minibatch j starts at `start` and writes its statistics j rows further
+__global__ void __launch_bounds__(256) ramp_pop_adam_kernel(const PopSet* sets, const AdamArgs* args, int32_t start, int32_t j, int32_t parity) {
+    AdamArgs a = args[blockIdx.y];
     a.start = start; a.parity = parity; a.stats += (size_t)j * RAMP_PPO_STATS_LEN;
-    adam_body(a, n_w);
+    adam_body(a, sets[blockIdx.y].n_w);
 }
 
 // kl: [K][2] the sets' kl_coeff and kl_target
@@ -186,17 +221,31 @@ __global__ void ramp_pop_pg_stats_kernel(const float* row_stats, const int32_t* 
 
 }  // namespace ramp
 
+// the head-reduce segments of every set for one launch row count
+struct PopSegs {
+    DeviceArray<Seg> segs; DeviceArray<int32_t> count; DeviceArray<int64_t> first;   // [K][HEAD_SEGS], [K], [K]
+    int64_t total = 0;
+};
+
 struct ramp_population {
-    ramp_policy* p = nullptr;             // the template: configuration, job types, act outputs and trajectory (not owned)
+    ramp_policy* p = nullptr;             // the template: job types, act outputs and trajectory (not owned)
     int32_t K = 0;
-    int64_t nw = 0;
+    std::vector<ramp_policy_config_t> cfgs;   // set s's configuration: the template's environment fields, the rest its own
+    std::vector<PopSet> sets;             // host copy of d_sets
+    std::vector<uint8_t> has_w;           // set s got weights (ramp_population_set_weights or the template's)
+    int64_t nw = 0, n_gpart = 0, n_emb = 0;   // sums over the sets: weights, job-type partials, embeddings
+    int32_t rec_stride = 0;               // the largest set's head record
+    size_t head_smem = 0;                 // the largest set's read-out staging
     int32_t embed_ctas = 0;               // CTAs of the embedding launches: at most the resident ones
-    DeviceArray<float> d_w, d_emb;        // [K][n_weights], [K][n_models][out_node]
+    DeviceArray<PopSet> d_sets;
+    DeviceArray<float> d_w, d_emb;        // ragged [K][n_w of the set], [K][n_models][out_node of the set]
     bool emb_valid = false;
     unsigned long long act_calls = 0;
     DeviceArray<unsigned long long> d_seeds, d_keys;
     std::vector<DeviceArray<unsigned char>> gallocs;     // every (set, job type)'s MeanPool states and backward scratch
-    LearnerBuffers L;                     // the learner: what ramp_policy keeps for one set, for K
+    LearnerBuffers L;                     // the learner: what ramp_policy keeps for one set, for K (its rec / segs unused: pop_ensure_rows)
+    std::map<int32_t, PopSegs> segs;      // every launch row count seen since L.rec was last allocated
+    const PopSegs* cur_segs = nullptr;
     DeviceArray<float> d_kl;              // [K][2]: kl_coeff, kl_target
     DeviceArray<GaeArgs> d_gae; DeviceArray<GradArgs> d_grad; DeviceArray<AdamArgs> d_adam;
     DeviceArray<VtraceArgs> d_vtrace;     // IMPALA: every set's V-trace arguments
@@ -211,7 +260,14 @@ int pop_check_set(const ramp_population* q, int32_t set) {
     return RAMP_OK;
 }
 
-// every (set, job type)'s forward states and backward scratch; the job types' out-edge CSR is the template's
+// act and learn read every set's weights
+int pop_check_weights(const ramp_population* q) {
+    for (int s = 0; s < q->K; ++s)
+        if (!q->has_w[s]) return set_error(RAMP_ERR_BAD_ARG, "population: set %d has no weights (ramp_population_set_weights)", s);
+    return RAMP_OK;
+}
+
+// every (set, job type)'s forward states and backward scratch at the set's configuration; the job types' out-edge CSR is the template's
 int pop_ensure_gms(ramp_population* q, cudaStream_t st) {
     if (q->L.gmodels_ready) return RAMP_OK;
     ramp_policy* p = q->p;
@@ -224,7 +280,7 @@ int pop_ensure_gms(ramp_population* q, cudaStream_t st) {
         for (int s = 0; s < q->K; ++s) {
             GradModelDev& g = h[(size_t)s * nm + m];
             g = hm.g;
-            const int rc = alloc_grad_scratch(p->P.c, hm.d.n_nodes, hm.d.n_edges, q->gallocs, g);
+            const int rc = alloc_grad_scratch(q->cfgs[s], hm.d.n_nodes, hm.d.n_edges, q->gallocs, g);
             if (rc != RAMP_OK) return rc;
         }
     }
@@ -234,11 +290,9 @@ int pop_ensure_gms(ramp_population* q, cudaStream_t st) {
 int pop_launch_embed(ramp_population* q, cudaStream_t st, EmbGradArgs eg, bool forward) {
     ramp_policy* p = q->p;
     PopEmbed pe{};
-    pe.K = q->K; pe.n_weights = q->nw; pe.rec_stride = head_rec(p->P.c).stride;
-    PolicyDev P = p->P;
-    P.w = q->d_w.get();
-    if (forward) ramp_pop_embed_grad_kernel<EMB_FORWARD><<<q->embed_ctas, 256, 0, st>>>(P, p->d_models.get(), q->L.gmodels.get(), eg, pe);
-    else ramp_pop_embed_grad_kernel<EMB_BACKWARD><<<q->embed_ctas, 256, 0, st>>>(P, p->d_models.get(), q->L.gmodels.get(), eg, pe);
+    pe.K = q->K; pe.n_models = p->P.c.n_models; pe.rec_stride = q->rec_stride;
+    if (forward) ramp_pop_embed_grad_kernel<EMB_FORWARD><<<q->embed_ctas, 256, 0, st>>>(q->d_sets.get(), p->d_models.get(), q->L.gmodels.get(), eg, pe);
+    else ramp_pop_embed_grad_kernel<EMB_BACKWARD><<<q->embed_ctas, 256, 0, st>>>(q->d_sets.get(), p->d_models.get(), q->L.gmodels.get(), eg, pe);
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
 }
@@ -262,11 +316,9 @@ int pop_launch_head(ramp_population* q, const HeadArgs& a, int32_t per, const un
     int gx = (per + wpc - 1) / wpc;
     const int cap = std::max(1, (2 * p->sm_count + q->K - 1) / q->K);      // about the single launch's 2 CTAs per SM in all
     gx = std::max(1, std::min(gx, cap));
-    PolicyDev P = p->P;
-    P.w = q->d_w.get();
     PopHead ph{};
-    ph.per = per; ph.stride = stride ? stride : per; ph.n_weights = q->nw; ph.seeds = seeds; ph.mix = mix;
-    ramp_pop_head_kernel<<<dim3(gx, q->K), wpc * 32, p->head_smem, st>>>(P, a, ph);
+    ph.per = per; ph.stride = stride ? stride : per; ph.seeds = seeds; ph.mix = mix;
+    ramp_pop_head_kernel<<<dim3(gx, q->K), wpc * 32, q->head_smem, st>>>(q->d_sets.get(), a, ph);
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
 }
@@ -281,15 +333,60 @@ int pop_ensure_learner(ramp_population* q) {
     CUDA_TRY(q->d_adam.alloc(K));
     CUDA_TRY(q->d_vtrace.alloc(K));
     CUDA_TRY(q->d_coef.alloc(2 * K));
-    return ensure_learner(q->L, q->p);
+    return ensure_learner(q->L, q->nw, q->n_gpart);
+}
+
+// ensure_rows for the population: per-row scratch for K launch rows of n rows, set s's at s n rec_stride floats, and every set's
+// head segments summing exactly n of its rows, uploaded on `st` the first time n is seen
+int pop_ensure_rows(ramp_population* q, int32_t n, cudaStream_t st) {
+    LearnerBuffers& L = q->L;
+    const size_t K = q->K;
+    if (n > L.lcap) {
+        const size_t rows = K * n;
+        L.lcap = 0;
+        q->cur_segs = nullptr;
+        q->segs.clear();
+        CUDA_TRY(L.rec.alloc(rows * q->rec_stride));
+        CUDA_TRY(L.row_stats.alloc(rows * RS_N));
+        CUDA_TRY(L.row_model.alloc(rows));
+        L.lcap = n;
+    }
+    auto it = q->segs.find(n);
+    if (it == q->segs.end()) {
+        std::vector<Seg> h(K * HEAD_SEGS);
+        std::vector<int32_t> count(K);
+        std::vector<int64_t> first(K);
+        PopSegs t;
+        for (size_t s = 0; s < K; ++s) {
+            Seg* ss = h.data() + s * HEAD_SEGS;
+            count[s] = head_segs(q->sets[s].P, L.rec.get() + s * n * q->rec_stride, n, ss);
+            first[s] = t.total;
+            for (int k = 0; k < count[s]; ++k) {
+                const int64_t o = q->sets[s].w_off;
+                ss[k].w += o; ss[k].lnw += o; ss[k].lnb += o;
+                t.total += seg_size(ss[k]);
+            }
+        }
+        CUDA_TRY(t.segs.alloc(h.size()));
+        CUDA_TRY(t.count.alloc(K));
+        CUDA_TRY(t.first.alloc(K));
+        CUDA_TRY(cudaMemcpyAsync(t.segs.get(), h.data(), sizeof(Seg) * h.size(), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(t.count.get(), count.data(), sizeof(int32_t) * K, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(t.first.get(), first.data(), sizeof(int64_t) * K, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaStreamSynchronize(st));                              // the vectors are pageable
+        it = q->segs.emplace(n, std::move(t)).first;
+    }
+    q->cur_segs = &it->second;
+    return RAMP_OK;
 }
 
 // set s's AdamArgs at cfg's settings on its slices of the gradient, moments, step counts, norm partials and weights
 template <class Cfg>
 AdamArgs pop_adam_args(ramp_population* q, const Cfg& cfg, int s, const int32_t* n_rows, int32_t mb) {
     AdamArgs aa = adam_args(q->p, cfg, n_rows, mb);
-    aa.step = q->L.step.get() + 2 * s; aa.m = q->L.adam_m.get() + (size_t)s * q->nw; aa.v = q->L.adam_v.get() + (size_t)s * q->nw;
-    aa.grad = q->L.grad.get() + (size_t)s * q->nw; aa.norm_part = q->L.norm_part.get() + (size_t)s * LRN_GRID; aa.w = q->d_w.get() + (size_t)s * q->nw;
+    const size_t o = q->sets[s].w_off;
+    aa.step = q->L.step.get() + 2 * s; aa.m = q->L.adam_m.get() + o; aa.v = q->L.adam_v.get() + o;
+    aa.grad = q->L.grad.get() + o; aa.norm_part = q->L.norm_part.get() + (size_t)s * LRN_GRID; aa.w = q->d_w.get() + o;
     return aa;
 }
 
@@ -307,7 +404,7 @@ int pop_check_configs(const ramp_population* q, const Cfg* cfgs) {
 template <class Cfg>
 int pop_learn_begin(ramp_population* q, ramp_engine_t* eng, const Cfg* cfgs, int32_t n_steps, ramp_env_buffers_t* eb, cudaStream_t* st) {
     int rc = learn_begin(q->p, eng, cfgs, n_steps, "population", eb, st);
-    if (rc != RAMP_OK) return rc;
+    if (rc != RAMP_OK || (rc = pop_check_weights(q)) != RAMP_OK) return rc;
     if (eb->n_episodes % q->K)
         return set_error(RAMP_ERR_BAD_ARG, "population: %d episodes do not split into %d groups of equal size", eb->n_episodes, q->K);
     if ((rc = fence_in(q->p, *st)) || (rc = pop_ensure_learner(q)) || (rc = pop_ensure_gms(q, *st))) return rc;
@@ -318,26 +415,24 @@ int pop_learn_begin(ramp_population* q, ramp_engine_t* eng, const Cfg* cfgs, int
     return RAMP_OK;
 }
 
-// head gradient (sets: q->d_grad) -> head reduce -> embedding backward -> finish over K launch rows of mb rows each: every set's
+// head gradient (args: q->d_grad) -> head reduce -> embedding backward -> finish over K launch rows of mb rows each: every set's
 // gradient and norm partials.  keys: the [K] shuffle keys (read, and unused, by an unshuffled launch); first_pass: logp_old is written
 int pop_launch_grad(ramp_population* q, cudaStream_t st, int32_t mb, int32_t start, const unsigned long long* keys, int first_pass) {
     ramp_policy* p = q->p;
     const int32_t K = q->K;
-    PolicyDev P = p->P;
-    P.w = q->d_w.get();
-    const SegTable* segs = q->L.segs;
-    int64_t rgrid = (K * segs->total + 255) / 256;
+    const PopSegs* segs = q->cur_segs;
+    int64_t rgrid = (segs->total + 255) / 256;
     if (rgrid > 4 * p->sm_count) rgrid = 4 * p->sm_count;
-    ramp_pop_head_grad_kernel<<<(K * mb + LRN_WARPS - 1) / LRN_WARPS, LRN_WARPS * 32, 0, st>>>(P, q->d_grad.get(), K, mb, start, keys, first_pass, q->nw);
-    ramp_pop_head_reduce_kernel<<<(unsigned)rgrid, 256, 0, st>>>(P, segs->d.get(), segs->count, segs->total, K, (int64_t)mb * head_rec(P.c).stride,
-                                                                 q->nw, q->L.grad.get());
+    ramp_pop_head_grad_kernel<<<dim3((mb + LRN_WARPS - 1) / LRN_WARPS, K), LRN_WARPS * 32, 0, st>>>(q->d_sets.get(), q->d_grad.get(), start, keys,
+                                                                                                   first_pass);
+    ramp_pop_head_reduce_kernel<<<(unsigned)rgrid, 256, 0, st>>>(segs->segs.get(), segs->count.get(), segs->first.get(), K, segs->total,
+                                                                 q->d_w.get(), q->L.grad.get());
     CUDA_TRY(cudaGetLastError());
     EmbGradArgs eg{};
-    eg.rec = q->L.rec.get(); eg.row_model = q->L.row_model.get(); eg.rows = mb; eg.gpart = q->L.gpart.get(); eg.n_gnn = gnn_weight_count(p);
+    eg.rec = q->L.rec.get(); eg.row_model = q->L.row_model.get(); eg.rows = mb; eg.gpart = q->L.gpart.get();
     int rc = pop_launch_embed(q, st, eg, false);
     if (rc != RAMP_OK) return rc;
-    ramp_pop_finish_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->L.gpart.get(), P.c.n_models, gnn_weight_count(p), q->nw, q->L.grad.get(),
-                                                              q->L.norm_part.get());
+    ramp_pop_finish_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_sets.get(), q->L.gpart.get(), p->P.c.n_models, q->L.grad.get(), q->L.norm_part.get());
     CUDA_TRY(cudaGetLastError());
     return RAMP_OK;
 }
@@ -360,36 +455,88 @@ GaeArgs pop_gae_args(ramp_population* q, int s, int32_t T, int32_t b, double gam
 
 // set s's head-gradient arguments for launch rows of mb rows: its slices of the per-row scratch and its embeddings
 GradArgs pop_grad_args(ramp_population* q, int s, int32_t mb) {
-    const ramp_policy_config_t& c = q->p->P.c;
     const size_t q0 = (size_t)s * mb;
     GradArgs ga{};
-    ga.mb = mb; ga.graph_static = q->p->d_gstatic.get(); ga.emb = q->d_emb.get() + (size_t)s * c.n_models * c.out_features_node;
-    ga.rec = q->L.rec.get() + q0 * head_rec(c).stride; ga.row_model = q->L.row_model.get() + q0; ga.row_stats = q->L.row_stats.get() + q0 * RS_N;
+    ga.mb = mb; ga.graph_static = q->p->d_gstatic.get(); ga.emb = q->d_emb.get() + q->sets[s].emb_off;
+    ga.rec = q->L.rec.get() + q0 * q->rec_stride; ga.row_model = q->L.row_model.get() + q0; ga.row_stats = q->L.row_stats.get() + q0 * RS_N;
     return ga;
+}
+
+// ramp_population_create_configs' work: the sets' checks, layouts and buffers, no weights yet
+int pop_create(ramp_policy* p, int32_t n_sets, const ramp_policy_config_t* cfgs, std::unique_ptr<ramp_population>& out) {
+    const ramp_policy_config_t& t = p->P.c;
+    std::vector<int64_t> n_w(n_sets);
+    int64_t nw = 0;
+    size_t smem = 0;
+    for (int s = 0; s < n_sets; ++s) {
+        const ramp_policy_config_t& c = cfgs[s];
+        if (check_config(c) != RAMP_OK) return set_error(RAMP_ERR_BAD_ARG, "population: set %d: %s", s, g_last_error.c_str());
+        const char* field = c.in_features_node != t.in_features_node ? "in_features_node" : c.in_features_edge != t.in_features_edge ? "in_features_edge"
+                          : c.in_features_graph != t.in_features_graph ? "in_features_graph" : c.n_actions != t.n_actions ? "n_actions"
+                          : c.n_models != t.n_models ? "n_models" : nullptr;
+        if (field)
+            return set_error(RAMP_ERR_BAD_ARG, "population: set %d: %s differs from the template's (the environment and its job types fix it)", s, field);
+        const size_t hs = head_smem_floats(c, 8) * sizeof(float);
+        if (hs > 200 * 1024) return set_error(RAMP_ERR_CAPACITY, "population: set %d: the read-out needs %zu B of shared memory (max 200 KiB)", s, hs);
+        smem = std::max(smem, hs);
+        n_w[s] = layout(c, nullptr);
+        nw += n_w[s];
+    }
+    CUDA_TRY(cudaSetDevice(p->device));
+    std::unique_ptr<ramp_population> q(new ramp_population());
+    q->p = p; q->K = q->L.K = n_sets; q->nw = nw; q->head_smem = smem;
+    int per_sm = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ramp_pop_embed_grad_kernel<EMB_BACKWARD>, 256, 0));
+    q->embed_ctas = std::max(1, std::min(n_sets * t.n_models, std::max(1, per_sm) * p->sm_count));
+    CUDA_TRY(reserve_dynamic_smem((const void*)ramp_pop_head_kernel, smem));
+    CUDA_TRY(q->d_w.alloc((size_t)nw));
+    q->cfgs.assign(cfgs, cfgs + n_sets);
+    q->sets.resize(n_sets);
+    for (int s = 0; s < n_sets; ++s) {
+        PopSet& S = q->sets[s];
+        S.P.c = cfgs[s];
+        layout(cfgs[s], &S.P);
+        S.n_w = n_w[s]; S.w_off = s ? q->sets[s - 1].w_off + n_w[s - 1] : 0; S.P.w = q->d_w.get() + S.w_off;
+        S.n_gnn = S.P.gln_w;                                              // the rounds come first in the blob
+        S.gpart_off = q->n_gpart; q->n_gpart += (int64_t)t.n_models * S.n_gnn;
+        S.emb_off = q->n_emb; q->n_emb += (int64_t)t.n_models * cfgs[s].out_features_node;
+        q->rec_stride = std::max(q->rec_stride, head_rec(cfgs[s]).stride);
+    }
+    q->has_w.assign(n_sets, 0);
+    CUDA_TRY(q->d_emb.alloc((size_t)q->n_emb));
+    CUDA_TRY(q->d_seeds.alloc(n_sets));
+    CUDA_TRY(q->d_sets.alloc(n_sets));
+    CUDA_TRY(cudaMemcpy(q->d_sets.get(), q->sets.data(), sizeof(PopSet) * n_sets, cudaMemcpyHostToDevice));
+    out = std::move(q);
+    return RAMP_OK;
 }
 
 }  // namespace
 
 extern "C" {
 
+int ramp_population_create_configs(ramp_policy_t* p, int32_t n_sets, const ramp_policy_config_t* cfgs, ramp_population_t** out) {
+    if (!p || !cfgs || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (n_sets < 1) return set_error(RAMP_ERR_BAD_ARG, "population: %d weight sets", n_sets);
+    std::unique_ptr<ramp_population> q;
+    const int rc = pop_create(p, n_sets, cfgs, q);
+    if (rc != RAMP_OK) return rc;
+    *out = q.release();
+    return RAMP_OK;
+}
+
 int ramp_population_create(ramp_policy_t* p, int32_t n_sets, ramp_population_t** out) {
     if (!p || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     if (n_sets < 1) return set_error(RAMP_ERR_BAD_ARG, "population: %d weight sets", n_sets);
     if (!p->weights_set) return set_error(RAMP_ERR_BAD_ARG, "policy: no weights (ramp_policy_set_weights)");
-    CUDA_TRY(cudaSetDevice(p->device));
-    std::unique_ptr<ramp_population> q(new ramp_population());
-    q->p = p; q->K = q->L.K = n_sets; q->nw = p->n_weights;
-    const ramp_policy_config_t& c = p->P.c;
-    int per_sm = 0;
-    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ramp_pop_embed_grad_kernel<EMB_BACKWARD>, 256, 0));
-    q->embed_ctas = std::max(1, std::min(n_sets * c.n_models, std::max(1, per_sm) * p->sm_count));
-    CUDA_TRY(reserve_dynamic_smem((const void*)ramp_pop_head_kernel, p->head_smem));
-    CUDA_TRY(q->d_w.alloc((size_t)n_sets * q->nw));
-    CUDA_TRY(q->d_emb.alloc((size_t)n_sets * c.n_models * c.out_features_node));
-    CUDA_TRY(q->d_seeds.alloc(n_sets));
+    const std::vector<ramp_policy_config_t> cfgs(n_sets, p->P.c);
+    std::unique_ptr<ramp_population> q;
+    const int rc = pop_create(p, n_sets, cfgs.data(), q);
+    if (rc != RAMP_OK) return rc;
     CUDA_TRY(cudaDeviceSynchronize());                                    // a running call may still update the template's weights
     for (int s = 0; s < n_sets; ++s)
-        CUDA_TRY(cudaMemcpy(q->d_w.get() + (size_t)s * q->nw, p->d_w.get(), sizeof(float) * q->nw, cudaMemcpyDeviceToDevice));
+        CUDA_TRY(cudaMemcpy(q->d_w.get() + q->sets[s].w_off, p->d_w.get(), sizeof(float) * p->n_weights, cudaMemcpyDeviceToDevice));
+    q->has_w.assign(n_sets, 1);
     *out = q.release();
     return RAMP_OK;
 }
@@ -404,10 +551,13 @@ int ramp_population_set_weights(ramp_population_t* q, int32_t set, const float* 
     int rc = pop_check_set(q, set);
     if (rc != RAMP_OK) return rc;
     if (!weights) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    if (n != q->nw) return set_error(RAMP_ERR_BAD_ARG, "population: %lld weights given for set %d, the configuration has %lld", (long long)n, set, (long long)q->nw);
+    const PopSet& S = q->sets[set];
+    if (n != S.n_w)
+        return set_error(RAMP_ERR_BAD_ARG, "population: %lld weights given for set %d, its configuration has %lld", (long long)n, set, (long long)S.n_w);
     CUDA_TRY(cudaSetDevice(q->p->device));
     CUDA_TRY(cudaDeviceSynchronize());                                    // a running rollout may still read the old set
-    CUDA_TRY(cudaMemcpy(q->d_w.get() + (size_t)set * q->nw, weights, sizeof(float) * n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(q->d_w.get() + S.w_off, weights, sizeof(float) * n, cudaMemcpyHostToDevice));
+    q->has_w[set] = 1;
     q->emb_valid = false;
     return RAMP_OK;
 }
@@ -416,9 +566,10 @@ int ramp_population_get_weights(ramp_population_t* q, int32_t set, float* out) {
     int rc = pop_check_set(q, set);
     if (rc != RAMP_OK) return rc;
     if (!out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    const PopSet& S = q->sets[set];
     CUDA_TRY(cudaSetDevice(q->p->device));
     CUDA_TRY(cudaDeviceSynchronize());                                    // a learn call may still be updating them
-    CUDA_TRY(cudaMemcpy(out, q->d_w.get() + (size_t)set * q->nw, sizeof(float) * q->nw, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(out, q->d_w.get() + S.w_off, sizeof(float) * S.n_w, cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }
 
@@ -435,6 +586,7 @@ int ramp_population_act(ramp_population_t* q, ramp_engine_t* eng, int32_t sample
     if (eb.n_models > c.n_models) return set_error(RAMP_ERR_BAD_ARG, "the environment has %d job types, the policy %d", eb.n_models, c.n_models);
     if (eb.n_episodes % q->K)
         return set_error(RAMP_ERR_BAD_ARG, "population: %d episodes do not split into %d groups of equal size", eb.n_episodes, q->K);
+    if ((rc = pop_check_weights(q)) != RAMP_OK) return rc;
     CUDA_TRY(cudaSetDevice(p->device));
     cudaStream_t st = ramp_internal_stream(eng);
     int launches = 1;
@@ -476,7 +628,7 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
     const int32_t B = eb.n_episodes, b = B / K, rows = n_steps * b, mb = cfgs[0].sgd_minibatch_size, n_mb = (rows + mb - 1) / mb;
     const int32_t n_pass = cfgs[0].num_sgd_iter, A = c.n_actions;
     const size_t R = rows;
-    if ((rc = ensure_rows(q->L, p->P, mb, st)) || (rc = ensure_batch(q->L, c, rows)) || (rc = ensure_ppo(q->L, B, n_mb))) return rc;
+    if ((rc = pop_ensure_rows(q, mb, st)) || (rc = ensure_batch(q->L, c, rows)) || (rc = ensure_ppo(q->L, B, n_mb))) return rc;
     if (!q->emb_valid && (rc = pop_embed(q, st)) != RAMP_OK) return rc;
     if ((size_t)K * std::max(n_pass, 1) > q->d_keys.size()) CUDA_TRY(q->d_keys.alloc((size_t)K * std::max(n_pass, 1)));
     // every group's arguments: set s's slices of the trajectory's columns, the train batch, the scratch and the learner state
@@ -536,7 +688,7 @@ int ramp_population_learn(ramp_population_t* q, ramp_engine_t* eng, int32_t n_st
             if ((rc = pop_launch_embed(q, st, ef, true)) != RAMP_OK ||
                 (rc = pop_launch_grad(q, st, mb, start, q->d_keys.get() + (size_t)pass * K, pass == 0)) != RAMP_OK)
                 return rc;
-            ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_adam.get(), start, j, q->L.parity, q->nw);
+            ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_sets.get(), q->d_adam.get(), start, j, q->L.parity);
             q->L.parity ^= 1;
             CUDA_TRY(cudaGetLastError());
             launches += 6;
@@ -576,7 +728,7 @@ int ramp_population_learn_impala(ramp_population_t* q, ramp_engine_t* eng, int32
     const ramp_policy_config_t& c = p->P.c;
     const int32_t b = eb.n_episodes / K, n_frag = (n_steps / L) * b, R = n_steps * b, A = c.n_actions;
     const int32_t F = std::min(cfgs[0].train_batch_size / L, n_frag), mb = F * L, n_sgd = (n_frag + F - 1) / F;
-    if ((rc = ensure_rows(q->L, p->P, mb, st)) || (rc = ensure_impala(q->L, c, R, n_sgd))) return rc;
+    if ((rc = pop_ensure_rows(q, mb, st)) || (rc = ensure_impala(q->L, c, R, n_sgd))) return rc;
     if (!q->emb_valid && (rc = pop_embed(q, st)) != RAMP_OK) return rc;
     LearnerBuffers& Lb = q->L;
     // every set's arguments: its slices of the fragment rows, the per-row scratch and the learner state
@@ -633,7 +785,7 @@ int ramp_population_learn_impala(ramp_population_t* q, ramp_engine_t* eng, int32
         ramp_pop_vtrace_kernel<<<(unsigned)((K * nf + 7) / 8), 256, 0, st>>>(q->d_vtrace.get(), K, nf, start);
         CUDA_TRY(cudaGetLastError());
         if ((rc = pop_launch_grad(q, st, mb, start, q->d_keys.get(), 1)) != RAMP_OK) return rc;
-        ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_adam.get(), start, 0, Lb.parity, q->nw);
+        ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_sets.get(), q->d_adam.get(), start, 0, Lb.parity);
         Lb.parity ^= 1;
         ramp_pop_impala_step_stats_kernel<<<(K + 127) / 128, 128, 0, st>>>(Lb.row_stats.get(), Lb.row_model.get(), mb, start, Lb.i_log_rho.get(), R,
                                                                           q->d_coef.get(), Lb.norm_part.get(), Lb.i_step_stats.get(), n_sgd, k, K);
@@ -660,7 +812,7 @@ int ramp_population_learn_pg(ramp_population_t* q, ramp_engine_t* eng, int32_t n
     if ((rc = pop_learn_begin(q, eng, cfgs, n_steps, &eb, &st)) != RAMP_OK) return rc;
     const ramp_policy_config_t& c = p->P.c;
     const int32_t b = eb.n_episodes / K, rows = n_steps * b, A = c.n_actions;
-    if ((rc = ensure_rows(q->L, p->P, rows, st)) || (rc = ensure_batch(q->L, c, rows))) return rc;
+    if ((rc = pop_ensure_rows(q, rows, st)) || (rc = ensure_batch(q->L, c, rows))) return rc;
     if (!q->emb_valid && (rc = pop_embed(q, st)) != RAMP_OK) return rc;
     LearnerBuffers& Lb = q->L;
     std::vector<GaeArgs> gae(K);
@@ -689,7 +841,7 @@ int ramp_population_learn_pg(ramp_population_t* q, ramp_engine_t* eng, int32_t n
     ef.n_rows = Lb.n_rows.get();
     if ((rc = pop_launch_embed(q, st, ef, true)) != RAMP_OK || (rc = pop_launch_grad(q, st, rows, 0, q->d_keys.get(), 1)) != RAMP_OK) return rc;
     // 3. one Adam step per set; a set with no row makes none and keeps its step count
-    ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_adam.get(), 0, 0, Lb.parity, q->nw);
+    ramp_pop_adam_kernel<<<dim3(LRN_GRID, K), 256, 0, st>>>(q->d_sets.get(), q->d_adam.get(), 0, 0, Lb.parity);
     Lb.parity ^= 1;
     // 4. the statistics: the call's one read-back
     ramp_pop_pg_stats_kernel<<<(K + 127) / 128, 128, 0, st>>>(Lb.row_stats.get(), Lb.row_model.get(), Lb.b_adv.get(), rows, Lb.n_rows.get(),
@@ -725,7 +877,7 @@ int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_
     int rc = pop_check_set(q, set);
     if (rc != RAMP_OK) return rc;
     CUDA_TRY(cudaSetDevice(q->p->device));
-    const size_t n = q->nw;
+    const size_t n = q->sets[set].n_w, o = q->sets[set].w_off;
     if (!q->L.ready) {
         if (exp_avg_out) memset(exp_avg_out, 0, sizeof(float) * n);
         if (exp_avg_sq_out) memset(exp_avg_sq_out, 0, sizeof(float) * n);
@@ -733,8 +885,8 @@ int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_
         return RAMP_OK;
     }
     CUDA_TRY(cudaDeviceSynchronize());                                    // a learn call may still be updating them
-    if (exp_avg_out) CUDA_TRY(cudaMemcpy(exp_avg_out, q->L.adam_m.get() + (size_t)set * n, sizeof(float) * n, cudaMemcpyDeviceToHost));
-    if (exp_avg_sq_out) CUDA_TRY(cudaMemcpy(exp_avg_sq_out, q->L.adam_v.get() + (size_t)set * n, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    if (exp_avg_out) CUDA_TRY(cudaMemcpy(exp_avg_out, q->L.adam_m.get() + o, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    if (exp_avg_sq_out) CUDA_TRY(cudaMemcpy(exp_avg_sq_out, q->L.adam_v.get() + o, sizeof(float) * n, cudaMemcpyDeviceToHost));
     if (step_out) CUDA_TRY(cudaMemcpy(step_out, q->L.step.get() + 2 * set + q->L.parity, sizeof(int32_t), cudaMemcpyDeviceToHost));
     return RAMP_OK;
 }

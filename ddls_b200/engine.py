@@ -179,7 +179,8 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_policy_set_weights_device', 'ramp_policy_forward_device', 'ramp_policy_backward_device',
                     'ramp_population_create', 'ramp_population_destroy', 'ramp_population_set_weights', 'ramp_population_get_weights',
                     'ramp_population_act', 'ramp_population_learn', 'ramp_population_learner_state', 'ramp_population_embed_ctas',
-                    'ramp_population_learn_impala', 'ramp_population_learn_pg', 'ramp_population_vtrace_read']
+                    'ramp_population_learn_impala', 'ramp_population_learn_pg', 'ramp_population_vtrace_read',
+                    'ramp_population_create_configs']
 
 
 def device_bytes():

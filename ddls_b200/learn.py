@@ -254,7 +254,7 @@ class _PopulationLearner:
 
     def adam_state(self, k: int):
         """set k's torch.optim.Adam state: exp_avg, exp_avg_sq (blob order) and the step count"""
-        n = self._L.ramp_policy_weight_count(C.byref(self.population.template._cfg))
+        n = self.population.weight_count(k)
         m, v, step = np.zeros(n, np.float32), np.zeros(n, np.float32), C.c_int32()
         _engine._check(self._L.ramp_population_learner_state(self.population._h, int(k), m.ctypes.data, v.ctypes.data, C.byref(step)))
         return m, v, step.value

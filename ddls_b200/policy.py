@@ -152,6 +152,11 @@ def weight_shapes(config: Dict, n_actions: int) -> Dict[str, tuple]:
     return shapes
 
 
+def weight_count(config: Dict, n_actions: int) -> int:
+    """the weights of a configuration (ramp_policy_weight_count)"""
+    return sum(int(np.prod(v)) for v in weight_shapes(config, n_actions).values())
+
+
 def pack_weights(state_dict: Dict, config: Dict, n_actions: int) -> np.ndarray:
     """Flat fp32 blob from a GNNPolicy state_dict (torch tensors or arrays); shapes are checked against the configuration, and a
     value branch the configuration's vf_share_layers does not have is refused."""
@@ -408,6 +413,7 @@ def _bind_population(L):
     if getattr(L, '_population_bound', False):
         return
     for name, args in (('ramp_population_create', [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]),
+                       ('ramp_population_create_configs', [C.c_void_p, C.c_int32, C.POINTER(_Config), C.POINTER(C.c_void_p)]),
                        ('ramp_population_set_weights', [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]),
                        ('ramp_population_get_weights', [C.c_void_p, C.c_int32, C.c_void_p]),
                        ('ramp_population_act', [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
@@ -419,39 +425,69 @@ def _bind_population(L):
     L._population_bound = True
 
 
-class DeviceGNNPolicyPopulation:
-    """K weight sets of one configuration acting on one DeviceRampJobPartitioningEnvironment: its B = K b episodes are K contiguous
-    groups of b, group k decided by set k.  Group k's decisions are, bit for bit, those a DeviceGNNPolicy holding set k's weights
-    makes on a b-episode environment with the same episode streams (include/ramp_b200.h: ramp_population_*).
-    DevicePopulationPPOLearner trains the K sets, each with its own PPOConfig."""
+# the ramp_policy_config_t fields the environment and its job types fix: every set of a population shares them
+ENV_FIELDS = ('in_features_node', 'in_features_edge', 'in_features_graph', 'n_actions', 'n_models')
 
-    def __init__(self, graphs, n_actions: int, config: Optional[Dict] = None, state_dicts: Sequence = (), device: int = 0):
-        """graphs, n_actions, config: as DeviceGNNPolicy's; state_dicts: one GNNPolicy state_dict (or blob) per set, K = their number."""
+
+class DeviceGNNPolicyPopulation:
+    """K weight sets acting on one DeviceRampJobPartitioningEnvironment: its B = K b episodes are K contiguous groups of b, group k
+    decided by set k.  Group k's decisions are, bit for bit, those a DeviceGNNPolicy holding set k's weights makes on a b-episode
+    environment with the same episode streams (include/ramp_b200.h: ramp_population_*).  The sets may differ in shape: each has
+    its own configuration (widths, rounds, read-out, activations), all of them in the same launches.
+    DevicePopulationPPOLearner, DevicePopulationIMPALALearner and DevicePopulationPGLearner train the K sets."""
+
+    def __init__(self, graphs, n_actions: int, config=None, state_dicts: Sequence = (), device: int = 0):
+        """graphs, n_actions: as DeviceGNNPolicy's; config: one configuration for every set (a dict, as DeviceGNNPolicy's), or a
+        sequence of K, set k's completed from DEFAULT_CONFIG; state_dicts: one GNNPolicy state_dict (or blob) per set, of its
+        set's shape, K = their number."""
         state_dicts = list(state_dicts)
         if not state_dicts:
             raise ValueError('a population needs at least one state_dict')
-        cfg = dict(DEFAULT_CONFIG)
-        cfg.update(config or {})
+        K, n_actions, n_models = len(state_dicts), int(n_actions), len(graphs)
+        per_set = config is not None and not isinstance(config, dict)
+        configs = list(config) if per_set else [config] * K
+        if len(configs) != K:
+            raise ValueError(f'{len(configs)} configs for {K} state_dicts')
+        configs = [dict(DEFAULT_CONFIG, **(c or {})) for c in configs]
+        ccfgs = []
+        for k, c in enumerate(configs):               # every set's configuration and shapes are checked before anything is allocated
+            if len(tuple(c['fcnet_hiddens'])) != 1:
+                raise ValueError(f'configs[{k}]: the device read-out has one hidden layer (gnn.yaml: fcnet_hiddens [256])')
+            if c.get('module_depth', 1) != 1:
+                raise ValueError(f'configs[{k}]: module_depth must be 1 (gnn.yaml)')
+            ccfgs.append(c_config(c, n_actions, n_models))
+            for f in ENV_FIELDS:
+                if getattr(ccfgs[k], f) != getattr(ccfgs[0], f):
+                    raise ValueError(f'configs[{k}]: {f} = {getattr(ccfgs[k], f)}, set 0 has {getattr(ccfgs[0], f)} '
+                                     '(the environment fixes it for every set)')
         blobs = []
-        for k, sd in enumerate(state_dicts):          # every set's shapes are checked before anything is allocated
+        for k, sd in enumerate(state_dicts):
             try:
-                blob = sd if isinstance(sd, np.ndarray) else pack_weights(sd, cfg, int(n_actions))
+                blob = sd if isinstance(sd, np.ndarray) else pack_weights(sd, configs[k], n_actions)
             except (KeyError, ValueError) as e:
                 raise ValueError(f'state_dicts[{k}]: {e}') from None
             blob = np.ascontiguousarray(blob, dtype=np.float32)
-            n = sum(int(np.prod(v)) for v in weight_shapes(cfg, int(n_actions)).values())
+            n = weight_count(configs[k], n_actions)
             if blob.shape != (n,):
-                raise ValueError(f'state_dicts[{k}]: a blob of shape {blob.shape}, the configuration has {n} weights')
+                raise ValueError(f'state_dicts[{k}]: a blob of shape {blob.shape}, set {k}\'s configuration has {n} weights')
             blobs.append(blob)
-        self.K, self.graphs, self.device = len(blobs), list(graphs), device
-        self.template = DeviceGNNPolicy(graphs, n_actions, cfg, state_dict=blobs[0], device=device)
+        self.K, self.graphs, self.device = K, list(graphs), device
+        self.configs = configs
+        self.template = DeviceGNNPolicy(graphs, n_actions, configs[0], state_dict=blobs[0], device=device)
         self.config, self.n_actions, self.n_models = self.template.config, self.template.n_actions, self.template.n_models
+        self._ccfgs = ccfgs
         self._L = self.template._L
         _bind_population(self._L)
         self._h = C.c_void_p()
-        _engine._check(self._L.ramp_population_create(self.template._h, self.K, C.byref(self._h)))
-        for k, blob in enumerate(blobs[1:], 1):
-            self.set_weights(k, blob)
+        if per_set:
+            arr = (_Config * K)(*ccfgs)
+            _engine._check(self._L.ramp_population_create_configs(self.template._h, K, arr, C.byref(self._h)))
+            first = 0
+        else:
+            _engine._check(self._L.ramp_population_create(self.template._h, K, C.byref(self._h)))
+            first = 1                                   # set 0 holds the template's weights
+        for k in range(first, K):
+            self.set_weights(k, blobs[k])
 
     def close(self):
         if getattr(self, '_h', None):
@@ -466,23 +502,35 @@ class DeviceGNNPolicyPopulation:
         except Exception:
             pass
 
+    def _set(self, k) -> int:
+        k = int(k)
+        if not 0 <= k < self.K:
+            raise IndexError(f'set {k} outside [0, {self.K})')
+        return k
+
+    def weight_count(self, k: int) -> int:
+        """the weights of set k's configuration"""
+        return int(self._L.ramp_policy_weight_count(C.byref(self._ccfgs[self._set(k)])))
+
     def set_weights(self, k: int, state_dict):
-        blob = state_dict if isinstance(state_dict, np.ndarray) else pack_weights(state_dict, self.config, self.n_actions)
+        """set k's weights: a state_dict of its configuration's shapes, or a blob"""
+        k = self._set(k)
+        blob = state_dict if isinstance(state_dict, np.ndarray) else pack_weights(state_dict, self.configs[k], self.n_actions)
         blob = np.ascontiguousarray(blob, dtype=np.float32)
-        _engine._check(self._L.ramp_population_set_weights(self._h, int(k), blob.ctypes.data, len(blob)))
+        _engine._check(self._L.ramp_population_set_weights(self._h, k, blob.ctypes.data, len(blob)))
 
     def get_weights(self, k: int) -> np.ndarray:
-        out = np.zeros(self._L.ramp_policy_weight_count(C.byref(self.template._cfg)), dtype=np.float32)
+        out = np.zeros(self.weight_count(k), dtype=np.float32)
         _engine._check(self._L.ramp_population_get_weights(self._h, int(k), out.ctypes.data))
         return out
 
     def gnn_state_dict(self, k: int) -> Dict[str, np.ndarray]:
-        """set k's weights under the reference's GNNPolicy key names and shapes"""
-        return unpack_weights(self.get_weights(k), self.config, self.n_actions)
+        """set k's weights under the reference's GNNPolicy key names and its configuration's shapes"""
+        return unpack_weights(self.get_weights(k), self.configs[self._set(k)], self.n_actions)
 
     def policy(self, k: int) -> DeviceGNNPolicy:
-        """a standalone DeviceGNNPolicy holding set k's current weights (e.g. for agents.evaluate)"""
-        return DeviceGNNPolicy(self.graphs, self.n_actions, self.config, state_dict=self.get_weights(k), device=self.device)
+        """a standalone DeviceGNNPolicy with set k's configuration and current weights (e.g. for agents.evaluate)"""
+        return DeviceGNNPolicy(self.graphs, self.n_actions, self.configs[self._set(k)], state_dict=self.get_weights(k), device=self.device)
 
     def group_size(self, env) -> int:
         """b, the episodes of one group; ValueError unless K divides the environment's B"""

@@ -894,8 +894,16 @@ typedef struct ramp_population ramp_population_t;
  * stays the population's template: its job types must not change, and it must outlive the population.  The population's act
  * writes p's act outputs, so ramp_policy_read and ramp_policy_trajectory_* on p record the population's decisions. */
 int ramp_population_create(ramp_policy_t* p, int32_t n_sets, ramp_population_t** out);
+/* K = n_sets weight sets whose shapes may differ: set k has configuration cfgs[k] (HOST, [n_sets]), K Adam states at zero and no
+ * weights yet -- act and learn refuse to run, naming the set, until ramp_population_set_weights gave every set its blob.  Each
+ * cfgs[k] must be a valid configuration with the template's in_features_node / _edge / _graph, n_actions and n_models (the
+ * environment and its job types fix them); widths, rounds, fcnet_hidden, the activations and vf_share_layers are the set's own.
+ * Errors name the set.  p is the template as for ramp_population_create; its weights are not used.  Every set runs in the same
+ * launches as a population of one shape; the read-out launches reserve the largest set's shared memory.
+ * ramp_population_create(p, K) is this call with K copies of p's configuration, followed by a copy of p's weights into every set. */
+int ramp_population_create_configs(ramp_policy_t* p, int32_t n_sets, const ramp_policy_config_t* cfgs, ramp_population_t** out);
 void ramp_population_destroy(ramp_population_t* q);
-/* set k's weights from / to a HOST blob of ramp_policy_weight_count floats */
+/* set k's weights from / to a HOST blob of ramp_policy_weight_count(cfgs[k]) floats: set_weights refuses any other n */
 int ramp_population_set_weights(ramp_population_t* q, int32_t set, const float* weights, int64_t n);
 int ramp_population_get_weights(ramp_population_t* q, int32_t set, float* out);
 /* ramp_policy_act for every group: episode k b + i draws as episode i of a policy whose ramp_policy_act got seeds[k] (HOST,
@@ -918,7 +926,7 @@ int ramp_population_learn_pg(ramp_population_t* q, ramp_engine_t* eng, int32_t n
 /* ramp_impala_vtrace_read for set k after the last ramp_population_learn_impala: its group's n_out fragment rows */
 int ramp_population_vtrace_read(ramp_population_t* q, int32_t set, int32_t* n_out, float* target_logp_out, float* log_rho_out,
                                 float* vs_out, float* pg_adv_out);
-/* HOST copies of set k's Adam state, as ramp_policy_learner_state */
+/* HOST copies of set k's Adam state, as ramp_policy_learner_state: ramp_policy_weight_count(cfgs[k]) floats each */
 int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_avg_out, float* exp_avg_sq_out, int32_t* step_out);
 /* the CTAs of the population's MeanPool launches: n_sets n_models items, at most the resident CTAs, each CTA runs items
  * c, c + ctas, ... */

@@ -13,7 +13,15 @@ multiplied by K (the K sequential calls would do the same work K times).  miniba
 steps (PPO: num_sgd_iter x minibatches; IMPALA: its SGD steps; PG: its one step).  Each measurement repeats `--repeats` times.
 Return rows ('kind': 'returns'): a grid over lr x entropy_coeff (PG, which has no entropy term: lr x gamma), --iters iterations
 of collect + learn, each set's mean episode return (the group's summed rewards over its episodes).  The first row names the card,
-its power limit and max SM clock, read in the same process."""
+its power limit and max SM clock, read in the same process.
+
+    python scripts/population_train.py --shapes sweep --algo {ppo,impala,pg}
+
+writes profiles/h100_population_shapes_<algo>_train.jsonl instead: scripts/wandb_sweep_config.yaml's PHASE 3 grid (out_features_msg,
+_hidden, _node over {8, 16, 32, 64}, num_rounds over {2, 4}: 128 shapes at gnn.yaml's other settings), one shape per set.  Rows
+'mixed' time the 128-shape population's learn call, rows 'same' homogeneous K = 128 populations at gnn.yaml's shape and at the
+grid's largest, --repeats each, alternating; the row 'sequential' sums 128 single learners' calls, one per shape, each on its own
+b-episode environment and timed once after a warm-up call."""
 import argparse
 import dataclasses
 import json
@@ -58,7 +66,9 @@ def main():
     ap.add_argument('--repeats', type=int, default=3)
     ap.add_argument('--grid-k', type=int, default=8)
     ap.add_argument('--iters', type=int, default=5)
-    ap.add_argument('--out', default=None, help='default: profiles/h100_population_<algo>_train.jsonl')
+    ap.add_argument('--shapes', choices=('same', 'sweep'), default='same', help='sweep: one PHASE 3 shape per set')
+    ap.add_argument('--out', default=None, help='default: profiles/h100_population_<algo>_train.jsonl (--shapes sweep: '
+                    'profiles/h100_population_shapes_<algo>_train.jsonl)')
     a = ap.parse_args()
     import torch
     from ddls_b200 import learn, policy as P, workload
@@ -72,7 +82,7 @@ def main():
                          'impala': (learn.DevicePopulationIMPALALearner, learn.DeviceIMPALALearner, learn.IMPALAConfig()),
                          'pg': (learn.DevicePopulationPGLearner, learn.DevicePGLearner, learn.PGConfig())}[a.algo]
     seeded = (lambda c, k: dataclasses.replace(c, seed=k)) if a.algo == 'ppo' else (lambda c, k: c)
-    out_path = a.out or f'profiles/h100_population_{a.algo}_train.jsonl'
+    out_path = a.out or f'profiles/h100_population_{"shapes_" if a.shapes == "sweep" else ""}{a.algo}_train.jsonl'
     os.makedirs(os.path.dirname(os.path.abspath(out_path)), exist_ok=True)
     out = open(out_path, 'w')
 
@@ -97,6 +107,10 @@ def main():
     elif a.algo == 'impala':
         head.update(rollout_fragment_length=base.rollout_fragment_length, train_batch_size=base.train_batch_size)
     emit(head)
+    if a.shapes == 'sweep':
+        sweep(a, graphs, A, Pop, Single, base, seeded, steps, emit, sync)
+        out.close()
+        return
     # the single learner on a b-episode environment
     senv = env_of(graphs, a.b, a.jobs, seed=1)
     spol = P.DeviceGNNPolicy(graphs, A, cfg0, P.random_state_dict(cfg0, A, seed=0))
@@ -132,6 +146,52 @@ def main():
         emit(dict(kind='returns', iteration=it, sets=[{'lr': lr, second[0]: e, 'mean_return': float(x)} for (lr, e), x in zip(grid, ret)]))
     pop.close()
     out.close()
+
+
+def phase3_grid():
+    """scripts/wandb_sweep_config.yaml's PHASE 3: out_features_msg, _hidden, _node over {8, 16, 32, 64}, num_rounds over {2, 4}"""
+    return [dict(out_features_msg=m, out_features_hidden=h, out_features_node=n, num_rounds=r)
+            for m in (8, 16, 32, 64) for h in (8, 16, 32, 64) for n in (8, 16, 32, 64) for r in (2, 4)]
+
+
+def sweep(a, graphs, A, Pop, Single, base, seeded, steps, emit, sync):
+    """the 128-shape population's learn call against homogeneous K = 128 populations and 128 sequential single learners"""
+    from ddls_b200 import policy as P
+    shapes = [dict(P.DEFAULT_CONFIG, **s) for s in phase3_grid()]
+    K = len(shapes)
+    n_mb = steps(a.horizon * a.b)
+    largest = dict(P.DEFAULT_CONFIG, **max(phase3_grid(), key=lambda s: P.weight_count(dict(P.DEFAULT_CONFIG, **s), A)))
+    runs = {'mixed': shapes, 'gnn_yaml': [dict(P.DEFAULT_CONFIG)] * K, 'largest': [largest] * K}
+    emit(dict(kind='shapes', K=K, weights=[P.weight_count(c, A) for c in shapes], largest=largest))
+    live = {}
+    for name, cfgs in runs.items():
+        env = env_of(graphs, K * a.b, a.jobs, seed=1)
+        pop = P.DeviceGNNPolicyPopulation(graphs, A, cfgs, [P.random_state_dict(c, A, seed=k) for k, c in enumerate(cfgs)])
+        lrn = Pop(pop, [seeded(base, k) for k in range(K)])
+        pop.collect(env, a.horizon, seed=list(range(K)))
+        lrn.learn(env, a.horizon)                                # warm-up: every buffer and launch shape
+        live[name] = (env, pop, lrn)
+    for r in range(a.repeats):
+        for name, (env, pop, lrn) in live.items():
+            t, _ = timed(lambda: lrn.learn(env, a.horizon), sync)
+            emit(dict(kind='mixed' if name == 'mixed' else 'same', shape=name, K=K, repeat=r, population_learn_s=t,
+                      population_minibatch_step_ms=1e3 * t / n_mb, embed_ctas=pop.embed_ctas()))
+    for env, pop, lrn in live.values():
+        pop.close()
+    live.clear()
+    # 128 single learners, one per shape, each timed once
+    times = []
+    senv = env_of(graphs, a.b, a.jobs, seed=1)
+    for k, c in enumerate(shapes):
+        spol = P.DeviceGNNPolicy(graphs, A, c, P.random_state_dict(c, A, seed=k))
+        slrn = Single(spol, seeded(base, k))
+        spol.collect(senv, a.horizon, seed=k)
+        slrn.learn(senv, a.horizon)                              # warm-up
+        t, _ = timed(lambda: slrn.learn(senv, a.horizon), sync)
+        times.append(t)
+        spol.close()
+    emit(dict(kind='sequential', K=K, single_learn_s_sum=sum(times), single_learn_s_min=min(times), single_learn_s_max=max(times),
+              single_learn_s=times))
 
 
 if __name__ == '__main__':
