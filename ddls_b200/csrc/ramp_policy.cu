@@ -158,12 +158,14 @@ __device__ __forceinline__ void meanpool_round(const PolicyDev& P, const float* 
     __syncthreads();
 }
 
-// the mean over the job's n_nodes node states (rows `stride` apart) into emb_out[od] (gnn_policy.py:262-268), by the whole CTA
+// the mean over the job's n_nodes node states (rows `stride` apart) into emb_out[od] (gnn_policy.py:262-268), by the whole CTA.
+// The sum runs in double: an fp32 running sum of thousands of like-signed states drifts by ~n ulp (5.6e-5 relative on a 4,097-node
+// out-star of single-unit states)
 __device__ __forceinline__ void node_mean(const float* z, int stride, int n_nodes, int od, float* emb_out) {
     for (int o = threadIdx.x; o < od; o += blockDim.x) {
-        float s = 0.f;
-        for (int v = 0; v < n_nodes; ++v) s += z[(size_t)v * stride + o];
-        emb_out[o] = s / (float)n_nodes;
+        double s = 0.0;
+        for (int v = 0; v < n_nodes; ++v) s += (double)z[(size_t)v * stride + o];
+        emb_out[o] = (float)(s / (double)n_nodes);
     }
 }
 

@@ -19,27 +19,33 @@ import pytest
 import torch
 
 from test_gpu_policy_learn import _Static, _env, host_batch, tensor_errors
-from tie_reference import TAU, deltas, explain, flips, grad64, near_ties
+from tie_reference import GNN_MODULES, TAU, deltas, explain, flips, grad64, near_ties
 
 pytestmark = pytest.mark.gpu
 
 
-def check_explained(pol, tag, grad, model, gf, mask, loss_fn, params=None):
+def check_explained(pol, tag, grad, model, gf, mask, loss_fn, params=None, graphs=None, max_candidates=None):
     """the kernel's gradient `grad` (blob) of loss_fn(logits, value) over the rows (model, gf, mask) at the policy's weights (or
-    `params`, name -> array) against float64 through explain(); returns (S as Flip, residuals, the float64 gradient)"""
+    `params`, name -> array) against float64 through explain(); returns (S as Flip, residuals, the float64 gradient).  graphs:
+    per job type, objects with nf, ef, src, dst (default: the policy's own job types).  Only ReLU / leaky-ReLU sites are
+    candidates: tanh has no branch to flip; max_candidates keeps the closest ones (each costs an autograd run)"""
     from ddls_b200 import policy as P
     c, A = pol.config, pol.n_actions
     params = P.unpack_weights(pol.get_weights(), c, A) if params is None else params
-    graphs = [_Static(st) for st in pol.static]
+    graphs = [_Static(st) for st in pol.static] if graphs is None else graphs
     g64, gl, gv = grad64(params, c, graphs, model, gf, mask, loss_fn)
     g32 = grad64(params, c, graphs, model, gf, mask, loss_fn, dtype=torch.float32)[0]
     e32 = tensor_errors(P.pack_weights(g32, c, A), g64, c, A)
     gk = {k: v.astype(np.float64) for k, v in P.unpack_weights(grad, c, A).items()}
-    ties = near_ties(params, c, graphs, model, gf, mask, TAU)
+    ties = [t for t in near_ties(params, c, graphs, model, gf, mask, TAU)
+            if c['aggregator_activation' if t.site[0] in GNN_MODULES else 'fcnet_activation'] != 'tanh']
     errs = tensor_errors(grad, g64, c, A)
     if all(e <= max(1e-4, 10 * e32[k]) for k, e in errs.items()):
         S, resid = [], errs                                             # nothing to explain: no flip needed
     else:
+        ties = ties[:max_candidates]
+        bad = {k: f'{e:.2e} (torch fp32 {e32[k]:.2e})' for k, e in errs.items() if e > max(1e-4, 10 * e32[k])}
+        print(f'{tag}: explaining {bad} by the closest {len(ties)} near-ties', flush=True)
         cands, ds = flips(ties, deltas(params, c, graphs, model, gf, mask, gl.numpy(), gv.numpy(), ties))
         S, resid = explain(gk, g64, ds, e32, cands)
         S = [cands[i] for i in S]
@@ -98,24 +104,29 @@ ENVS = {'cfg3': ('cfg3', 64, 6), 'mix128': ('mix128', 64, 6), 'bench_types': ('b
 @pytest.mark.parametrize('wseed', [2, 4, 6, 21])
 @pytest.mark.parametrize('eid', list(ENVS))
 def test_learner_gradients_on_recorded_batches(eid, wseed):
+    kind, B, J = ENVS[eid]
+    env, graphs = _make_env(kind, B, J)
+    learner_gradients_on_a_recorded_batch(env, graphs, J, wseed, f'{eid} seed {wseed}', min_rows=3000 if B > 1000 else 100)
+
+
+def learner_gradients_on_a_recorded_batch(env, graphs, J, wseed, tag, min_rows):
+    """a J-step segment of env recorded by a DeviceGNNPolicy on graphs at weight seed wseed; the PPO, IMPALA and PG gradients on
+    the batches each learner forms from it, explained against float64.  Closes env."""
     from ddls_b200 import policy as P
     from ddls_b200.learn import DeviceIMPALALearner, DevicePGLearner, DevicePPOLearner, IMPALAConfig, PGConfig, PPOConfig
     from impala_reference import fragments
     from pg_reference import train_rows
-    kind, B, J = ENVS[eid]
-    env, graphs = _make_env(kind, B, J)
     A = env.max_partitions_per_op + 1
     pol = P.DeviceGNNPolicy(graphs, A, None, P.random_state_dict(P.DEFAULT_CONFIG, A, seed=wseed))
     try:
         traj = {k: np.array(v) for k, v in pol.collect(env, J, sample=True, seed=3).items()}
         assert traj['done'][-1].all()
-        tag = f'{eid} seed {wseed}'
         # PPO: the train batch learn() builds (GAE, standardised advantages), old logits at the collection weights
         cfg = PPOConfig(num_sgd_iter=0)
         probe = DevicePPOLearner(pol, cfg)
         probe.learn(env, J)
         b = host_batch(pol, traj, probe.train_batch(env))
-        assert len(b['model']) > (3000 if B > 1000 else 100)
+        assert len(b['model']) > min_rows
         _, g = DevicePPOLearner(pol, PPOConfig()).loss_and_grad(b)
         check_explained(pol, f'ppo {tag}', g, b['model'], b['graph_features'], b['action_mask'], ppo_loss(b, PPOConfig()))
         # IMPALA: every fragment of the segment (one per episode) in one batch

@@ -197,10 +197,15 @@ def host_batch(pol, traj, tb):
 
 
 def test_first_pass_recomputes_the_collected_log_probabilities_bit_for_bit():
-    from ddls_b200.learn import DevicePPOLearner, PPOConfig
     J = 8
     env, graphs = _env(J=J)
-    pol = _policy(graphs)
+    first_pass_recomputes_the_collected_log_probabilities(env, _policy(graphs), J)
+
+
+def first_pass_recomputes_the_collected_log_probabilities(env, pol, J):
+    """a J-step segment collected by pol, then one PPO pass over all of it: the pass's log-probabilities are the collected ones,
+    bit for bit (EMB_FORWARD's embeddings are the embed kernel's).  Closes env and pol."""
+    from ddls_b200.learn import DevicePPOLearner, PPOConfig
     try:
         traj = pol.collect(env, J, sample=True, seed=3)
         lrn = DevicePPOLearner(pol, PPOConfig(num_sgd_iter=1, sgd_minibatch_size=J * env.B))

@@ -76,14 +76,15 @@ def _learners(algo):
             'pg': (learn.DevicePopulationPGLearner, learn.DevicePGLearner)}[algo]
 
 
-def _twin_run(algos, configs, b=3, H=8, J=6, kinds=('resnet',), compare=None, iters=3):
+def _twin_run(algos, configs, b=3, H=8, J=6, kinds=('resnet',), compare=None, iters=3, graphs=None):
     """iters collect -> learn iterations of a population with one configuration per set and of its twins, the population's
-    learner of iteration i being algos[i % len(algos)]; every comparison is asserted here.  Returns the population's embedding
-    CTAs and, per compared set, its weight count."""
+    learner of iteration i being algos[i % len(algos)]; every comparison is asserted here.  The job types are `graphs`
+    (synth.ForwardGraph) or else the workload graphs `kinds`.  Returns the population's embedding CTAs and, per compared set, its
+    weight count."""
     from ddls_b200 import workload
     from ddls_b200 import policy as P
     K = len(configs)
-    graphs = [workload.make_graph(k) for k in kinds]
+    graphs = graphs or [workload.make_graph(k) for k in kinds]
     script = _script(K * b, J, len(graphs), seed=11)
     sds = [P.random_state_dict(dict(P.DEFAULT_CONFIG, **c), A, seed=30 + k) for k, c in enumerate(configs)]
     compare = list(range(K)) if compare is None else compare

@@ -438,21 +438,27 @@ def test_module_gradients_on_recorded_batches_are_held_to_float64(eid, wseed):
     """tests/test_gpu_learn_grad_recorded.py's rule for the module: PPO's and PG's gradients on the batches those learners form
     from a recorded segment, each tensor within max(1e-4, 10 e32) of float64 once tie_reference.explain() has accounted for the
     flips of named near-tied units"""
+    from test_gpu_learn_grad_recorded import ENVS, _make_env
+    kind, B, J = ENVS[eid]
+    env, graphs = _make_env(kind, B, J)
+    module_gradients_on_a_recorded_batch(env, graphs, J, wseed, f'module {eid} seed {wseed}')
+
+
+def module_gradients_on_a_recorded_batch(env, graphs, J, wseed, tag):
+    """TorchGNNPolicy's PPO and PG gradients on a J-step segment of env recorded at weight seed wseed, explained against float64.
+    Closes env."""
     from ddls_b200 import policy as P
     from ddls_b200.learn import DevicePPOLearner, PGConfig, PPOConfig
     from ddls_b200.torch_policy import TorchGNNPolicy
     from pg_reference import train_rows
-    from test_gpu_learn_grad_recorded import ENVS, _make_env, check_explained, pg_loss, ppo_loss
+    from test_gpu_learn_grad_recorded import check_explained, pg_loss, ppo_loss
     from test_gpu_policy_learn import host_batch
-    kind, B, J = ENVS[eid]
-    env, graphs = _make_env(kind, B, J)
     A = env.max_partitions_per_op + 1
     sd = P.random_state_dict(P.DEFAULT_CONFIG, A, seed=wseed)
     pol = P.DeviceGNNPolicy(graphs, A, None, sd)
     mod = TorchGNNPolicy(pol.static, A, state_dict=sd)
     try:
         traj = {k: np.array(v) for k, v in pol.collect(env, J, sample=True, seed=3).items()}
-        tag = f'module {eid} seed {wseed}'
         probe = DevicePPOLearner(pol, PPOConfig(num_sgd_iter=0))
         probe.learn(env, J)
         b = host_batch(pol, traj, probe.train_batch(env))
