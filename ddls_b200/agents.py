@@ -59,19 +59,22 @@ class DeviceHeuristicAgents:
 def evaluate(env, actor, seed: int = 0, sample: bool = False, step_stats: bool = False):
     """EvalLoop.run (loops/eval_loop.py:26-134) for every episode of a DeviceRampJobPartitioningEnvironment at once: reset, then
     ``jobs_per_episode`` rounds of actor -> ``env.step_device()`` (an env-step consumes the one queued job, so no episode takes
-    more), then ``env.episode_stats()``.  actor: a DeviceHeuristicAgents, or a DeviceGNNPolicy (greedy unless ``sample``).  The
-    loop does not synchronise when ``prewarm()`` lets the device decide every placement.  Raises if an episode is not done.
+    more), then ``env.episode_stats()``.  actor: a DeviceHeuristicAgents, a DeviceGNNPolicy (greedy unless ``sample``), or a
+    DeviceGNNPolicyPopulation, set k deciding group k of the episodes.  A greedy population decides each group as that set's
+    policy(k) would on the group alone; under ``sample`` every set acts with seed + t at env-step t, and its draws are keyed by
+    the population's own act count, not a standalone policy's.  The loop does not synchronise when ``prewarm()`` lets the device
+    decide every placement.  Raises if an episode is not done.
 
     step_stats=False returns ``env.episode_stats()``.  step_stats=True returns EvalLoop.run's ``{'step_stats': ...,
     'episode_stats': ...}``: the device records every env-step's action, reward and reduced steps_log row while the loop runs
     (``env.record_steps``), still without synchronising, and ``step_stats`` is ``env.recorded_steps()`` -- per key a list of B
     arrays, one entry per env-step of the episode."""
-    from .policy import DeviceGNNPolicy
+    from .policy import DeviceGNNPolicy, DeviceGNNPolicyPopulation
     env.reset()
     if step_stats:
         env.record_steps(env.J)
     for t in range(env.J):
-        if isinstance(actor, DeviceGNNPolicy):
+        if isinstance(actor, (DeviceGNNPolicy, DeviceGNNPolicyPopulation)):
             actor.act(env, sample=sample, seed=seed + t)
         else:
             actor.act(seed)                                # Random's draws are keyed by the episode's decision count

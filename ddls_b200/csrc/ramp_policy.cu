@@ -1676,5 +1676,5 @@ int ramp_policy_learn_pg(ramp_policy_t* p, ramp_engine_t* eng, int32_t n_steps, 
 
 }  // extern "C"
 
-#include "ramp_es.cuh"
 #include "ramp_population.cuh"
+#include "ramp_es.cuh"

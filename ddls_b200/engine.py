@@ -180,7 +180,10 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_population_create', 'ramp_population_destroy', 'ramp_population_set_weights', 'ramp_population_get_weights',
                     'ramp_population_act', 'ramp_population_learn', 'ramp_population_learner_state', 'ramp_population_embed_ctas',
                     'ramp_population_learn_impala', 'ramp_population_learn_pg', 'ramp_population_vtrace_read',
-                    'ramp_population_create_configs']
+                    'ramp_population_create_configs', 'ramp_population_es_create', 'ramp_population_es_destroy',
+                    'ramp_population_es_round_begin', 'ramp_population_es_act', 'ramp_population_es_round_end',
+                    'ramp_population_es_step', 'ramp_population_es_update', 'ramp_population_es_read', 'ramp_population_es_act_read',
+                    'ramp_population_es_state', 'ramp_population_es_reset', 'ramp_population_es_embed_ctas']
 
 
 def device_bytes():

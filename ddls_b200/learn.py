@@ -133,11 +133,23 @@ def _bind(L):
                        ('ramp_population_learner_state', [C.c_void_p, C.c_int32] + [C.c_void_p] * 3),
                        ('ramp_population_learn_impala', [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CIMPALAConfig), C.c_void_p]),
                        ('ramp_population_learn_pg', [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_CPGConfig), C.c_void_p]),
-                       ('ramp_population_vtrace_read', [C.c_void_p, C.c_int32] + [C.c_void_p] * 5)):
+                       ('ramp_population_vtrace_read', [C.c_void_p, C.c_int32] + [C.c_void_p] * 5),
+                       ('ramp_population_es_create', [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+                       ('ramp_population_es_round_begin', [C.c_void_p, C.c_void_p, C.POINTER(_CESConfig), C.c_int32]),
+                       ('ramp_population_es_act', [C.c_void_p, C.c_void_p, C.c_int32]),
+                       ('ramp_population_es_round_end', [C.c_void_p, C.c_void_p, C.c_void_p]),
+                       ('ramp_population_es_step', [C.c_void_p, C.POINTER(_CESConfig), C.c_void_p]),
+                       ('ramp_population_es_update', [C.c_void_p, C.POINTER(_CESConfig)] + [C.c_void_p] * 4),
+                       ('ramp_population_es_read', [C.c_void_p, C.c_int32] + [C.c_void_p] * 11),
+                       ('ramp_population_es_act_read', [C.c_void_p] * 5),
+                       ('ramp_population_es_state', [C.c_void_p, C.c_int32] + [C.c_void_p] * 3),
+                       ('ramp_population_es_reset', [C.c_void_p]),
+                       ('ramp_population_es_embed_ctas', [C.c_void_p] * 3)):
         getattr(L, name).restype = C.c_int
         getattr(L, name).argtypes = args
-    L.ramp_es_destroy.restype = None
-    L.ramp_es_destroy.argtypes = [C.c_void_p]
+    for name in ('ramp_es_destroy', 'ramp_population_es_destroy'):
+        getattr(L, name).restype = None
+        getattr(L, name).argtypes = [C.c_void_p]
     L._learn_bound = True
 
 
@@ -464,6 +476,50 @@ class _CESConfig(C.Structure):
         (n, C.c_int32) for n in ('episodes_per_batch', 'train_batch_size', 'n_eval', 'report_length')]
 
 
+def es_n_eval(config: ESConfig, B: int) -> int:
+    """eval episodes per round of a B-episode environment (a population's: of one group): config.n_eval, else RLlib's expected
+    share of eval episodes B eval_prob / (2 - eval_prob), at least 1, plus one when B - E would be odd"""
+    if config.n_eval is not None:
+        return int(config.n_eval)
+    p = config.eval_prob
+    E = max(1, int(round(B * p / (2.0 - p))))
+    return E + ((B - E) & 1)
+
+
+def _es_learn(self, env, timing: bool = False):
+    """One ES training step: rounds until end_round() says no more are needed, then step().  Each round resets env and runs
+    env.J env-steps, so every episode ends in it; the round synchronises once, at its end.  timing=True also synchronises after
+    the embeddings and adds the wall time (seconds) of the embeddings (embed_s), of the rollouts (rollout_s) and of the update
+    (update_s)."""
+    B = env.B
+    times = dict(embed_s=0.0, rollout_s=0.0)
+    rnd, more = 0, True
+    while more:
+        env.reset()
+        t0 = time.perf_counter()
+        self.begin_round(env, rnd)
+        if timing:
+            env.eng.sync()
+        t1 = time.perf_counter()
+        for t in range(env.J):
+            self.act(env, t)
+            env.step_device()
+        more = self.end_round(env)
+        _, _, done = env.read()                        # raises what a step would have raised
+        if not done.all():
+            raise Exception(f'{int((~done).sum())} of {B} episodes are not done after {env.J} env-steps')
+        t2 = time.perf_counter()
+        times['embed_s'] += t1 - t0
+        times['rollout_s'] += t2 - t1
+        rnd += 1
+    t3 = time.perf_counter()
+    stats = self.step()
+    if timing:
+        for s in (stats if isinstance(stats, list) else [stats]):
+            s.update(times, update_s=time.perf_counter() - t3)
+    return stats
+
+
 def shared_noise_table(size: int) -> np.ndarray:
     """RLlib's shared noise table (es.py create_shared_noise), bit for bit.  At the default size it takes seconds and 1 GB as
     float32 (2 GB more while numpy draws it in float64)."""
@@ -505,13 +561,8 @@ class DeviceESLearner:
             pass
 
     def n_eval(self, B: int) -> int:
-        """eval episodes per round of a B-episode environment: config.n_eval, else RLlib's expected share of eval episodes
-        B eval_prob / (2 - eval_prob), at least 1, plus one when B - E would be odd"""
-        if self.config.n_eval is not None:
-            return int(self.config.n_eval)
-        p = self.config.eval_prob
-        E = max(1, int(round(B * p / (2.0 - p))))
-        return E + ((B - E) & 1)
+        """eval episodes per round of a B-episode environment (es_n_eval)"""
+        return es_n_eval(self.config, B)
 
     def _c(self, B: int) -> _CESConfig:
         return _c_struct(_CESConfig, self.config, n_eval=self.n_eval(B))
@@ -540,35 +591,8 @@ class DeviceESLearner:
         return _stats(ES_STATS, out)
 
     def learn(self, env, timing: bool = False) -> Dict[str, float]:
-        """One ES training step (ES_STATS).  Each round resets env and runs env.J env-steps, so every episode ends in it; the
-        round synchronises once, at its end.  timing=True also synchronises after the embeddings and adds the wall time (seconds)
-        of the embeddings (embed_s), of the rollouts (rollout_s) and of the update (update_s)."""
-        B = env.B
-        times = dict(embed_s=0.0, rollout_s=0.0)
-        rnd, more = 0, True
-        while more:
-            env.reset()
-            t0 = time.perf_counter()
-            self.begin_round(env, rnd)
-            if timing:
-                env.eng.sync()
-            t1 = time.perf_counter()
-            for t in range(env.J):
-                self.act(env, t)
-                env.step_device()
-            more = self.end_round(env)
-            _, _, done = env.read()                        # raises what a step would have raised
-            if not done.all():
-                raise Exception(f'{int((~done).sum())} of {B} episodes are not done after {env.J} env-steps')
-            t2 = time.perf_counter()
-            times['embed_s'] += t1 - t0
-            times['rollout_s'] += t2 - t1
-            rnd += 1
-        t3 = time.perf_counter()
-        stats = self.step()
-        if timing:
-            stats.update(times, update_s=time.perf_counter() - t3)
-        return stats
+        """One ES training step (ES_STATS); see _es_learn."""
+        return _es_learn(self, env, timing)
 
     def update(self, noise_index, returns):
         """the update on host inputs: noise_index [n], returns [n, 2] (R+, R-) -> (ES_STATS, ranks [n, 2], g [n_weights]); theta
@@ -612,3 +636,156 @@ class DeviceESLearner:
     def reset(self):
         """zero the ES Adam state"""
         _engine._check(self._L.ramp_es_reset(self._h))
+
+
+class DevicePopulationESLearner(_PopulationLearner):
+    """DeviceESLearner for every set of a DeviceGNNPolicyPopulation at once (include/ramp_b200.h: ramp_population_es_*): group k
+    of the environment's B = K b episodes is set k's ES population, N_k = (b - E_k) / 2 antithetic pairs and E_k eval episodes
+    with configs[k], and ends each step where a DeviceESLearner(population.policy(k), configs[k]) ends on a b-episode environment
+    with the same episode streams, bit for bit: the step record, the statistics, the weights and the ES Adam state.  A group stops
+    collecting after the round its twin would stop after (rounds_k of them); the population runs rounds until every group has
+    stopped, and in the later rounds a stopped group's episodes all run its unperturbed weights and count for nothing.  The
+    population's torch-Adam state (DevicePopulationPPOLearner's) is not touched; the ES Adam state is this learner's own.  One
+    shared noise table serves every set, so noise_size must be the same in every config."""
+    _checks = (('noise_stdev', lambda v: v >= 0, '>= 0'), ('stepsize', lambda v: v >= 0, '>= 0'), ('adam_eps', lambda v: v > 0, '> 0'),
+               ('adam_beta1', lambda v: 0 <= v < 1, 'in [0, 1)'), ('adam_beta2', lambda v: 0 <= v < 1, 'in [0, 1)'),
+               ('episodes_per_batch', lambda v: v >= 0, '>= 0'), ('train_batch_size', lambda v: v >= 0, '>= 0'),
+               ('report_length', lambda v: v >= 1, '>= 1'), ('observation_filter', lambda v: v == 'NoFilter',
+                                                              "'NoFilter' (MeanStdFilter would standardise the padded edge indices and "
+                                                              'the action mask the GNN reads back from the observation)'),
+               ('n_eval', lambda v: v is None or v >= 0, 'None or >= 0'))
+
+    def __init__(self, population, configs, noise: np.ndarray = None):
+        """population: a DeviceGNNPolicyPopulation, whose sets the learner updates in place; configs: one ESConfig per set.  noise:
+        the shared noise table (float32); None draws shared_noise_table(noise_size)."""
+        super().__init__(population, configs)
+        sizes = [c.noise_size for c in self.configs]
+        if len(set(sizes)) > 1:
+            k = next(k for k, v in enumerate(sizes) if v != sizes[0])
+            raise ValueError(f'noise_size must be the same for every set (one noise table serves them all): {sizes}; set {k} differs '
+                             'from set 0')
+        noise = shared_noise_table(sizes[0]) if noise is None else np.ascontiguousarray(noise, dtype=np.float32).ravel()
+        self.noise_size = len(noise)
+        for k in range(population.K):
+            if population.weight_count(k) > self.noise_size:
+                raise ValueError(f'set {k}: a noise table of {self.noise_size} floats is smaller than its {population.weight_count(k)} weights')
+        self._h = C.c_void_p()
+        _engine._check(self._L.ramp_population_es_create(population._h, noise.ctypes.data, self.noise_size, C.byref(self._h)))
+        self._B = 0
+
+    def close(self):
+        if getattr(self, '_h', None):
+            self._L.ramp_population_es_destroy(self._h)
+            self._h = None
+
+    def _handle(self):
+        """the learner's handle; every call but close() reads the population's sets, so both must still be open"""
+        if not getattr(self, '_h', None):
+            raise RuntimeError('the ES learner is closed')
+        if not self.population._h:
+            raise RuntimeError('the population was closed before its ES learner')
+        return self._h
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def n_eval(self, b: int):
+        """each group's eval episodes per round when a group has b episodes (es_n_eval)"""
+        return [es_n_eval(c, b) for c in self.configs]
+
+    def _c(self, B: int):
+        b = B // self.population.K
+        cfgs = [_c_struct(_CESConfig, c, n_eval=E) for c, E in zip(self.configs, self.n_eval(b))]
+        return (_CESConfig * self.population.K)(*cfgs)
+
+    def _check_groups(self, b: int):
+        for k, E in enumerate(self.n_eval(b)):
+            if b - E < 2 or (b - E) & 1:
+                raise ValueError(f'set {k}: {b} episodes per group less {E} eval episodes leave {b - E}, which must be even and >= 2')
+
+    def begin_round(self, env, rnd: int):
+        """after env.reset(): round rnd's noise indices, weight sets and embeddings of every group still collecting (round 0 starts
+        a new step)"""
+        self._check_groups(self.population.group_size(env))
+        self._B = env.B
+        _engine._check(self._L.ramp_population_es_round_begin(self._handle(), env.eng._h, self._c(env.B), int(rnd)))
+
+    def act(self, env, t: int):
+        """env-step t of the round: every episode's sampled action from its own weight set"""
+        _engine._check(self._L.ramp_population_es_act(self._handle(), env.eng._h, int(t)))
+
+    def end_round(self, env) -> bool:
+        """the round's returns and env-steps into the records of the groups that ran pairs; True while any group needs more"""
+        more = C.c_int32()
+        _engine._check(self._L.ramp_population_es_round_end(self._handle(), env.eng._h, C.byref(more)))
+        return bool(more.value)
+
+    def step(self):
+        """every set's update on its step record: a list of K ES_STATS dicts; stats[k]['rounds'] is group k's rounds"""
+        out = np.zeros((self.population.K, len(ES_STATS)), dtype=np.float64)
+        _engine._check(self._L.ramp_population_es_step(self._handle(), self._c(self._B), out.ctypes.data))
+        return [_stats(ES_STATS, row) for row in out]
+
+    learn = _es_learn
+
+    def update(self, noise_index, returns):
+        """the update on host inputs, per set: noise_index[k] [n_k], returns[k] [n_k, 2] -> a list of K (ES_STATS, ranks [n_k, 2],
+        g), as DeviceESLearner.update gives them for set k"""
+        K = self.population.K
+        if len(noise_index) != K or len(returns) != K:
+            raise ValueError(f'{len(noise_index)} noise index lists and {len(returns)} return lists for {K} sets')
+        idx = [np.ascontiguousarray(i, dtype=np.int32).ravel() for i in noise_index]
+        ret = [np.ascontiguousarray(r, dtype=np.float32).reshape(len(i), 2) for i, r in zip(idx, returns)]
+        n = np.array([len(i) for i in idx], np.int32)
+        for k in range(K):
+            if n[k] < 1:
+                raise ValueError(f'set {k}: an update needs at least one pair')
+        flat_i, flat_r = np.concatenate(idx), np.ascontiguousarray(np.concatenate(ret))
+        out = np.zeros((K, len(ES_STATS)), dtype=np.float64)
+        _engine._check(self._L.ramp_population_es_update(self._handle(), self._c(K * (2 * int(n.max()) + 1)), n.ctypes.data, flat_i.ctypes.data,
+                                                         flat_r.ctypes.data, out.ctypes.data))
+        res = []
+        for k in range(K):
+            rec = self.last_step(k)
+            res.append((_stats(ES_STATS, out[k]), rec['ranks'], rec['g']))
+        return res
+
+    def last_step(self, k: int) -> Dict[str, np.ndarray]:
+        """set k's last step record, as DeviceESLearner.last_step gives its own"""
+        k = self.population._set(k)
+        n, ne, ns = C.c_int32(), C.c_int32(), C.c_int32()
+        _engine._check(self._L.ramp_population_es_read(self._handle(), k, C.byref(n), C.byref(ne), C.byref(ns), *([None] * 9)))
+        n, ne, ns = n.value, ne.value, ns.value
+        out = dict(noise_index=np.zeros(n, np.int32), returns=np.zeros((n, 2), np.float32), lengths=np.zeros((n, 2), np.int32),
+                   seeds=np.zeros(ns, np.uint64), ranks=np.zeros((n, 2), np.float32), g=np.zeros(self.population.weight_count(k), np.float32),
+                   eval_returns=np.zeros(ne, np.float32), eval_lengths=np.zeros(ne, np.int32))
+        _engine._check(self._L.ramp_population_es_read(self._handle(), k, None, None, None, *[a.ctypes.data for a in out.values()]))
+        return out
+
+    def act_read(self, env):
+        """the last act's logits [B, |A|], log-probabilities [B] and actions [B]"""
+        B, A = env.B, self.population.n_actions
+        logits, logp, actions = np.zeros((B, A), np.float32), np.zeros(B, np.float32), np.zeros(B, np.int32)
+        _engine._check(self._L.ramp_population_es_act_read(self._handle(), env.eng._h, logits.ctypes.data, logp.ctypes.data, actions.ctypes.data))
+        return logits, logp, actions
+
+    def adam_state(self, k: int):
+        """set k's optimizers.Adam m, v (blob order) and t"""
+        k = self.population._set(k)
+        n = self.population.weight_count(k)
+        m, v, t = np.zeros(n, np.float32), np.zeros(n, np.float32), C.c_int32()
+        _engine._check(self._L.ramp_population_es_state(self._handle(), k, m.ctypes.data, v.ctypes.data, C.byref(t)))
+        return m, v, t.value
+
+    def reset(self):
+        """zero every set's ES Adam state"""
+        _engine._check(self._L.ramp_population_es_reset(self._handle()))
+
+    def embed_ctas(self):
+        """the last round's embedding launch: (CTAs, (ES weight set, job type) items); each CTA runs items c, c + ctas, ..."""
+        ctas, items = C.c_int32(), C.c_int32()
+        _engine._check(self._L.ramp_population_es_embed_ctas(self._handle(), C.byref(ctas), C.byref(items)))
+        return ctas.value, items.value

@@ -932,6 +932,45 @@ int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_
  * c, c + ctas, ... */
 int ramp_population_embed_ctas(ramp_population_t* q, int32_t* ctas_out);
 
+/* ---- ES for every set of a population: group k of the environment's B = K b episodes is the ES population of weight set k
+ * with cfgs[k] (HOST, [K]): 2 N_k = b - n_eval_k noisy episodes, then n_eval_k eval episodes at theta_k.  Group k ends each step
+ * where ramp_es_* on a policy holding set k's weights (and that set's configuration) ends on a b-episode environment with the same
+ * episode streams, bit for bit: its step record, statistics, theta_k and ES Adam state.  Noise indices and act seeds are keyed by
+ * (cfgs[k].seed, iteration, round, .) with the group's own pair and episode indices; the iteration count is the learner's.
+ * theta_k is the population's set k, updated in place; the ES Adam state (m, v, t per set) belongs to the learner, and the
+ * population's torch-Adam state (ramp_population_learner_state) is not touched.  Every configuration error names the set. */
+typedef struct ramp_population_es ramp_population_es_t;
+/* uploads noise[noise_size] (RLlib's shared noise table, HOST float32), which must cover the largest set's weights */
+int ramp_population_es_create(ramp_population_t* q, const float* noise, int64_t noise_size, ramp_population_es_t** out);
+void ramp_population_es_destroy(ramp_population_es_t* es);
+/* ramp_es_round_begin for every group (the same checks per set; n_sets must divide B).  A group's twin stops after the round at
+ * whose end its record holds episodes_per_batch noisy episodes and train_batch_size noisy env-steps; in every later round of the
+ * step the group has no pairs: all its episodes run theta_k and nothing of theirs is recorded.  A round after every group
+ * stopped is refused. */
+int ramp_population_es_round_begin(ramp_population_es_t* es, ramp_engine_t* eng, const ramp_es_config_t* cfgs, int32_t round);
+/* ramp_es_act for every group: episode k b + i is episode i of group k's twin, with group k's act seed */
+int ramp_population_es_act(ramp_population_es_t* es, ramp_engine_t* eng, int32_t t);
+/* ramp_es_round_end for every group that ran pairs in the round; *more_out = 1 while any group's twin would run another round */
+int ramp_population_es_round_end(ramp_population_es_t* es, ramp_engine_t* eng, int32_t* more_out);
+/* ramp_es_step for every set, each on its own record with cfgs[k]: ranks over its own pairs, g, Adam and the norms in the single
+ * update's partition and order.  stats_out [n_sets][RAMP_ES_STATS_LEN] or NULL. */
+int ramp_population_es_step(ramp_population_es_t* es, const ramp_es_config_t* cfgs, double* stats_out);
+/* ramp_es_update for every set on HOST inputs: set k's n_pairs[k] pairs follow set k - 1's in noise_index [sum n_pairs] and
+ * returns [sum n_pairs][2].  Its ranks and g are read back by ramp_population_es_read.  stats_out [n_sets][RAMP_ES_STATS_LEN] or NULL. */
+int ramp_population_es_update(ramp_population_es_t* es, const ramp_es_config_t* cfgs, const int32_t* n_pairs, const int32_t* noise_index,
+                              const float* returns, double* stats_out);
+/* ramp_es_read of set k's last step record; grad_out has set k's weight count */
+int ramp_population_es_read(ramp_population_es_t* es, int32_t set, int32_t* n_pairs_out, int32_t* n_eval_out, int32_t* n_seeds_out,
+                            int32_t* noise_index_out, float* returns_out, int32_t* lengths_out, uint64_t* seeds_out, float* ranks_out,
+                            float* grad_out, float* eval_returns_out, int32_t* eval_lengths_out);
+/* HOST copies of the last ramp_population_es_act's logits [B][n_actions], log-probabilities [B] and actions [B] (any may be NULL) */
+int ramp_population_es_act_read(ramp_population_es_t* es, ramp_engine_t* eng, float* logits_out, float* logp_out, int32_t* actions_out);
+/* set k's ES Adam state, as ramp_es_state; ramp_population_es_reset zeroes every set's */
+int ramp_population_es_state(ramp_population_es_t* es, int32_t set, float* m_out, float* v_out, int32_t* t_out);
+int ramp_population_es_reset(ramp_population_es_t* es);
+/* the last round's embedding launch: its CTAs and its (ES weight set, job type) items; each CTA runs items c, c + ctas, ... */
+int ramp_population_es_embed_ctas(ramp_population_es_t* es, int32_t* ctas_out, int32_t* items_out);
+
 #ifdef __cplusplus
 }
 #endif

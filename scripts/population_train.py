@@ -21,7 +21,15 @@ writes profiles/h100_population_shapes_<algo>_train.jsonl instead: scripts/wandb
 _hidden, _node over {8, 16, 32, 64}, num_rounds over {2, 4}: 128 shapes at gnn.yaml's other settings), one shape per set.  Rows
 'mixed' time the 128-shape population's learn call, rows 'same' homogeneous K = 128 populations at gnn.yaml's shape and at the
 grid's largest, --repeats each, alternating; the row 'sequential' sums 128 single learners' calls, one per shape, each on its own
-b-episode environment and timed once after a warm-up call."""
+b-episode environment and timed once after a warm-up call.
+
+    python scripts/population_train.py --algo es [--shapes sweep]
+
+writes profiles/h100_population_es_train.jsonl: for each K, one learn() step of DevicePopulationESLearner on a K b-episode
+environment (ESConfig's es.yaml defaults: about 8 rounds of --jobs env-steps at b = 128) with timing=True's embed / rollout /
+update split, alternating with K sequential DeviceESLearner steps on a b-episode environment, one per set, with the same split
+summed over the K steps (--shapes sweep: set k has PHASE 3 shape k mod 128; otherwise gnn.yaml's shape).  Each measurement
+repeats `--repeats` times after a warm-up step."""
 import argparse
 import dataclasses
 import json
@@ -57,7 +65,7 @@ def timed(fn, sync):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument('--algo', choices=('ppo', 'impala', 'pg'), default='ppo')
+    ap.add_argument('--algo', choices=('ppo', 'impala', 'pg', 'es'), default='ppo')
     ap.add_argument('--ks', default='1,8,32,128')
     ap.add_argument('--b', type=int, default=128, help='episodes per group')
     ap.add_argument('--horizon', type=int, default=4)
@@ -77,6 +85,9 @@ def main():
     sync = torch.cuda.synchronize
     graphs = [workload.make_graph('resnet')]
     A = 17
+    if a.algo == 'es':
+        es_timing(a, graphs, A, sync)
+        return
     cfg0 = P.algo_model_config(a.algo, A)
     Pop, Single, base = {'ppo': (learn.DevicePopulationPPOLearner, learn.DevicePPOLearner, learn.PPOConfig(num_sgd_iter=a.num_sgd_iter)),
                          'impala': (learn.DevicePopulationIMPALALearner, learn.DeviceIMPALALearner, learn.IMPALAConfig()),
@@ -145,6 +156,60 @@ def main():
         lrn.learn(env, a.jobs)
         emit(dict(kind='returns', iteration=it, sets=[{'lr': lr, second[0]: e, 'mean_return': float(x)} for (lr, e), x in zip(grid, ret)]))
     pop.close()
+    out.close()
+
+
+def es_timing(a, graphs, A, sync):
+    """the population's ES step against K sequential single ES steps, alternating; see the module docstring"""
+    import numpy as np
+    from ddls_b200 import learn, policy as P
+    out_path = a.out or 'profiles/h100_population_es_train.jsonl'
+    os.makedirs(os.path.dirname(os.path.abspath(out_path)), exist_ok=True)
+    out = open(out_path, 'w')
+
+    def emit(row):
+        print(json.dumps(row), flush=True)
+        out.write(json.dumps(row) + '\n')
+        out.flush()
+
+    ks = [int(k) for k in a.ks.split(',')]
+    shapes = [dict(P.DEFAULT_CONFIG, **s) for s in phase3_grid()] if a.shapes == 'sweep' else [dict(P.DEFAULT_CONFIG)]
+    base = learn.ESConfig(noise_size=1 << 25)
+    noise = np.random.default_rng(0).standard_normal(base.noise_size, dtype=np.float32)   # its values do not change the work
+    emit(dict(kind='card', **card(), algo='es', shapes=a.shapes, b=a.b, jobs=a.jobs, episodes_per_batch=base.episodes_per_batch,
+              train_batch_size=base.train_batch_size, eval_prob=base.eval_prob))
+    senv = env_of(graphs, a.b, a.jobs, seed=1)
+    singles = []                                                 # a policy and an ES learner per shape, each warmed up once
+    for k, c in enumerate(shapes[:max(ks)]):
+        spol = P.DeviceGNNPolicy(graphs, A, c, P.random_state_dict(c, A, seed=k))
+        slrn = learn.DeviceESLearner(spol, dataclasses.replace(base, seed=k), noise=noise)
+        slrn.learn(senv)
+        singles.append((spol, slrn))
+    for K in ks:
+        env = env_of(graphs, K * a.b, a.jobs, seed=1)
+        cfgs = [shapes[k % len(shapes)] for k in range(K)]
+        pop = P.DeviceGNNPolicyPopulation(graphs, A, cfgs, [P.random_state_dict(c, A, seed=k) for k, c in enumerate(cfgs)])
+        lrn = learn.DevicePopulationESLearner(pop, [dataclasses.replace(base, seed=k) for k in range(K)], noise=noise)
+        lrn.learn(env)                                           # warm-up: every buffer and launch shape
+        for r in range(a.repeats):
+            tp, stats = timed(lambda: lrn.learn(env, timing=True), sync)
+            ts, split = [], dict(embed_s=0.0, rollout_s=0.0, update_s=0.0)
+            for k in range(K):
+                t, st = timed(lambda: singles[k % len(singles)][1].learn(senv, timing=True), sync)
+                ts.append(t)
+                for key in split:
+                    split[key] += st[key]
+            ctas, items = lrn.embed_ctas()
+            emit(dict(kind='timing', K=K, repeat=r, population_step_s=tp, embed_s=stats[0]['embed_s'], rollout_s=stats[0]['rollout_s'],
+                      update_s=stats[0]['update_s'], rounds=max(int(s['rounds']) for s in stats), single_steps_s=sum(ts),
+                      single_step_s_min=min(ts), single_step_s_max=max(ts), single_embed_s=split['embed_s'],
+                      single_rollout_s=split['rollout_s'], single_update_s=split['update_s'], last_embed_ctas=ctas, last_embed_items=items))
+        lrn.close()
+        pop.close()
+        del env
+    for spol, slrn in singles:
+        slrn.close()
+        spol.close()
     out.close()
 
 
