@@ -347,6 +347,22 @@ void es_read_record(const EsRecord& r, int32_t* n_pairs_out, int32_t* n_eval_out
     if (eval_lengths_out) memcpy(eval_lengths_out, r.eval_len.data(), sizeof(int32_t) * r.eval_len.size());
 }
 
+// what the next steps read besides the Adam state: the iteration count (it keys the noise indices and the act seeds) and the
+// record's eval means so far (episode_reward_mean's window); rewards_out may be NULL to learn n_rewards first
+void es_get_progress(int64_t iteration, const EsRecord& r, int64_t* iteration_out, int32_t* n_rewards_out, double* rewards_out) {
+    if (iteration_out) *iteration_out = iteration;
+    if (n_rewards_out) *n_rewards_out = (int32_t)r.reward_list.size();
+    if (rewards_out) memcpy(rewards_out, r.reward_list.data(), sizeof(double) * r.reward_list.size());
+}
+
+int es_set_progress(int64_t* iteration, EsRecord& r, int64_t it, int32_t n_rewards, const double* rewards) {
+    if (it < 0 || n_rewards < 0 || (n_rewards > 0 && !rewards))
+        return set_error(RAMP_ERR_BAD_ARG, "es: iteration %lld and %d eval means (both must be >= 0)", (long long)it, n_rewards);
+    *iteration = it;
+    r.reward_list.assign(rewards, rewards + n_rewards);
+    return RAMP_OK;
+}
+
 // the population buffers for B episodes (2 n_pairs + 1 sets)
 int es_population(ramp_es* es, int32_t B) {
     if (B <= es->cap) return RAMP_OK;
@@ -606,6 +622,29 @@ int ramp_es_reset(ramp_es_t* es) {
     CUDA_TRY(cudaMemset(es->v.get(), 0, sizeof(float) * (size_t)es->n));
     es->t = 0;
     return RAMP_OK;
+}
+
+int ramp_es_set_state(ramp_es_t* es, const float* m, const float* v, int64_t n, int32_t t) {
+    if (!es || !m || !v) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (n != es->n) return set_error(RAMP_ERR_BAD_ARG, "es: an Adam state of %lld weights given, the policy has %lld", (long long)n, (long long)es->n);
+    if (t < 0) return set_error(RAMP_ERR_BAD_ARG, "es: Adam step count %d < 0", t);
+    CUDA_TRY(cudaSetDevice(es->p->device));
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemcpy(es->m.get(), m, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(es->v.get(), v, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
+    es->t = t;
+    return RAMP_OK;
+}
+
+int ramp_es_get_progress(ramp_es_t* es, int64_t* iteration_out, int32_t* n_rewards_out, double* rewards_out) {
+    if (!es) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    es_get_progress(es->iteration, es->rec, iteration_out, n_rewards_out, rewards_out);
+    return RAMP_OK;
+}
+
+int ramp_es_set_progress(ramp_es_t* es, int64_t iteration, int32_t n_rewards, const double* rewards) {
+    if (!es) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    return es_set_progress(&es->iteration, es->rec, iteration, n_rewards, rewards);
 }
 
 }  // extern "C"
@@ -921,6 +960,7 @@ int ramp_population_es_round_begin(ramp_population_es_t* es, ramp_engine_t* eng,
                          (long long)n_sets, ES_MAX_SETS);
     CUDA_TRY(cudaSetDevice(p->device));
     cudaStream_t st = ramp_internal_stream(eng);
+    if ((rc = fence_in(p, st)) != RAMP_OK) return rc;                    // a ramp_population_copy_sets may still write the weights
     if (round == 0) {
         for (EsRecord& r : es->rec) r.begin();
         es->n_eval.resize(K);
@@ -1132,6 +1172,49 @@ int ramp_population_es_reset(ramp_population_es_t* es) {
     CUDA_TRY(cudaMemset(es->m.get(), 0, sizeof(float) * (size_t)es->q->nw));
     CUDA_TRY(cudaMemset(es->v.get(), 0, sizeof(float) * (size_t)es->q->nw));
     es->t.assign(es->K, 0);
+    return RAMP_OK;
+}
+
+int ramp_population_set_es_state(ramp_population_es_t* es, int32_t set, const float* m, const float* v, int64_t n, int32_t t) {
+    if (!es || !m || !v) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = pop_check_set(es->q, set);
+    if (rc != RAMP_OK) return rc;
+    const PopSet& S = es->q->sets[set];
+    if (n != S.n_w)
+        return set_error(RAMP_ERR_BAD_ARG, "population: es: an Adam state of %lld weights given for set %d, its configuration has %lld", (long long)n, set,
+                         (long long)S.n_w);
+    if (t < 0) return set_error(RAMP_ERR_BAD_ARG, "population: set %d: es: Adam step count %d < 0", set, t);
+    CUDA_TRY(cudaSetDevice(es->q->p->device));
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemcpy(es->m.get() + S.w_off, m, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(es->v.get() + S.w_off, v, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
+    es->t[set] = t;
+    return RAMP_OK;
+}
+
+int ramp_population_get_es_progress(ramp_population_es_t* es, int32_t set, int64_t* iteration_out, int32_t* n_rewards_out, double* rewards_out) {
+    if (!es) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = pop_check_set(es->q, set);
+    if (rc != RAMP_OK) return rc;
+    es_get_progress(es->iteration, es->rec[set], iteration_out, n_rewards_out, rewards_out);
+    return RAMP_OK;
+}
+
+int ramp_population_set_es_progress(ramp_population_es_t* es, int32_t set, int64_t iteration, int32_t n_rewards, const double* rewards) {
+    if (!es) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = pop_check_set(es->q, set);
+    if (rc != RAMP_OK) return rc;
+    return es_set_progress(&es->iteration, es->rec[set], iteration, n_rewards, rewards);
+}
+
+int ramp_population_copy_es_sets(ramp_population_es_t* es, int32_t n_pairs, const int32_t* dst, const int32_t* src) {
+    if (!es) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    int rc = pop_check_pairs(es->q, n_pairs, dst, src);
+    if (rc != RAMP_OK || (rc = pop_copy_sets(es->q, n_pairs, dst, src, es->m.get(), es->v.get(), nullptr, nullptr)) != RAMP_OK) return rc;
+    for (int i = 0; i < n_pairs; ++i) {
+        es->t[dst[i]] = es->t[src[i]];
+        es->rec[dst[i]].reward_list = es->rec[src[i]].reward_list;
+    }
     return RAMP_OK;
 }
 

@@ -1525,6 +1525,34 @@ int ramp_policy_learner_reset(ramp_policy_t* p) {
     return RAMP_OK;
 }
 
+int ramp_policy_set_learner_state(ramp_policy_t* p, const float* exp_avg, const float* exp_avg_sq, int64_t n, int32_t step) {
+    if (!p || !exp_avg || !exp_avg_sq) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (n != p->n_weights)
+        return set_error(RAMP_ERR_BAD_ARG, "policy: a learner state of %lld weights given, the configuration has %lld", (long long)n, (long long)p->n_weights);
+    if (step < 0) return set_error(RAMP_ERR_BAD_ARG, "policy: Adam step count %d < 0", step);
+    CUDA_TRY(cudaSetDevice(p->device));
+    int rc = ensure_learner(p->L, p->n_weights, (size_t)p->P.c.n_models * gnn_weight_count(p));
+    if (rc != RAMP_OK) return rc;
+    CUDA_TRY(cudaDeviceSynchronize());                                    // a learn call may still be updating them
+    CUDA_TRY(cudaMemcpy(p->L.adam_m.get(), exp_avg, sizeof(float) * n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->L.adam_v.get(), exp_avg_sq, sizeof(float) * n, cudaMemcpyHostToDevice));
+    const int32_t steps[2] = {step, step};                              // whichever parity the next step reads
+    CUDA_TRY(cudaMemcpy(p->L.step.get(), steps, sizeof(steps), cudaMemcpyHostToDevice));
+    return RAMP_OK;
+}
+
+int ramp_policy_get_act_count(ramp_policy_t* p, uint64_t* out) {
+    if (!p || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    *out = p->act_calls;
+    return RAMP_OK;
+}
+
+int ramp_policy_set_act_count(ramp_policy_t* p, uint64_t n) {
+    if (!p) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    p->act_calls = n;
+    return RAMP_OK;
+}
+
 int ramp_impala_loss_grad(ramp_policy_t* p, const ramp_impala_config_t* cfg, int32_t n_fragments, int32_t fragment_length,
                           const int32_t* model, const float* graph_features, const uint8_t* action_mask, const int32_t* action,
                           const float* behaviour_logp, const double* reward, const uint8_t* done, float* grad_out,

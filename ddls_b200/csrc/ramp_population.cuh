@@ -219,6 +219,32 @@ __global__ void ramp_pop_pg_stats_kernel(const float* row_stats, const int32_t* 
                   norm_part + (size_t)s * LRN_GRID, out + (size_t)s * RAMP_PPO_STATS_LEN);
 }
 
+// ---- population-based training's exploit: one set's training state onto another ----
+
+struct CopySetsArgs {
+    const PopSet* sets;
+    const int32_t* pairs;                 // [n_pairs][2]: destination set, source set (equal shapes, checked on the host)
+    float* buf[3];                        // [sum n_w] buffers in the population's layout (PopSet::w_off); nullptr: none
+    int32_t* step;                        // [K][2] Adam's step counts (both parities), or nullptr
+};
+
+// pair `pair`'s source slices onto its destination's, elements chunk blockDim.x + threadIdx.x, grid-strided over n_chunks CTAs
+__device__ __forceinline__ void copy_sets_body(const CopySetsArgs& a, int pair, int chunk, int n_chunks) {
+    const int d = a.pairs[2 * pair], s = a.pairs[2 * pair + 1];
+    const int64_t n = a.sets[d].n_w, od = a.sets[d].w_off, os = a.sets[s].w_off;
+    for (int64_t i = (int64_t)chunk * blockDim.x + threadIdx.x; i < n; i += (int64_t)n_chunks * blockDim.x) {
+#pragma unroll
+        for (int b = 0; b < 3; ++b)
+            if (a.buf[b]) a.buf[b][od + i] = a.buf[b][os + i];
+    }
+    if (a.step && chunk == 0 && threadIdx.x < 2) a.step[2 * d + threadIdx.x] = a.step[2 * s + threadIdx.x];
+}
+
+// blockIdx.y = pair, blockIdx.x = chunk: ramp_population_copy_sets and ramp_population_copy_es_sets
+__global__ void __launch_bounds__(256) ramp_pop_copy_sets_kernel(const CopySetsArgs a) {
+    copy_sets_body(a, blockIdx.y, blockIdx.x, gridDim.x);
+}
+
 }  // namespace ramp
 
 // the head-reduce segments of every set for one launch row count
@@ -250,6 +276,10 @@ struct ramp_population {
     DeviceArray<GaeArgs> d_gae; DeviceArray<GradArgs> d_grad; DeviceArray<AdamArgs> d_adam;
     DeviceArray<VtraceArgs> d_vtrace;     // IMPALA: every set's V-trace arguments
     DeviceArray<double> d_coef;           // IMPALA: [K][2] vf_loss_coeff, entropy_coeff
+    // the copies' (destination, source) pairs: page-locked staging, its device copy, and the end of the last upload from it
+    PinnedArray<int32_t> h_pairs;
+    DeviceArray<int32_t> d_pairs;
+    Event ev_pairs;
 };
 
 namespace {
@@ -509,6 +539,69 @@ int pop_create(ramp_policy* p, int32_t n_sets, const ramp_policy_config_t* cfgs,
     CUDA_TRY(cudaMemcpy(q->d_sets.get(), q->sets.data(), sizeof(PopSet) * n_sets, cudaMemcpyHostToDevice));
     out = std::move(q);
     return RAMP_OK;
+}
+
+// the copies' pairs: sets in [0, K) of equal shape, the source with weights, no set the destination twice, and no set both a source
+// and a destination (so the result does not depend on the order the pairs run in).  Errors name the pair.
+int pop_check_pairs(const ramp_population* q, int32_t n_pairs, const int32_t* dst, const int32_t* src) {
+    if (!q || n_pairs < 0 || (n_pairs > 0 && (!dst || !src))) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    if (n_pairs > 65535) return set_error(RAMP_ERR_BAD_ARG, "population: %d pairs in one copy (max 65535)", n_pairs);
+    std::vector<int32_t> as_dst(q->K, -1), as_src(q->K, -1);
+    for (int i = 0; i < n_pairs; ++i) {
+        const int32_t d = dst[i], s = src[i];
+        if (d < 0 || d >= q->K || s < 0 || s >= q->K)
+            return set_error(RAMP_ERR_BAD_ARG, "population: pair %d (set %d <- set %d): a set outside [0, %d)", i, d, s, q->K);
+        if (memcmp(&q->cfgs[d], &q->cfgs[s], sizeof(ramp_policy_config_t)) != 0)
+            return set_error(RAMP_ERR_BAD_ARG, "population: pair %d (set %d <- set %d): the sets differ in shape (ramp_policy_config_t)", i, d, s);
+        if (as_dst[d] >= 0)
+            return set_error(RAMP_ERR_BAD_ARG, "population: pair %d (set %d <- set %d): set %d is already the destination of pair %d", i, d, s, d,
+                             as_dst[d]);
+        as_dst[d] = i;
+        if (as_src[s] < 0) as_src[s] = i;
+        if (!q->has_w[s]) return set_error(RAMP_ERR_BAD_ARG, "population: pair %d (set %d <- set %d): set %d has no weights", i, d, s, s);
+    }
+    for (int i = 0; i < n_pairs; ++i) {
+        const int32_t d = dst[i], s = src[i];
+        if (as_src[d] >= 0 || as_dst[s] >= 0)
+            return set_error(RAMP_ERR_BAD_ARG, "population: pair %d (set %d <- set %d): set %d is both a source and a destination", i, d, s,
+                             as_src[d] >= 0 ? d : s);
+    }
+    return RAMP_OK;
+}
+
+// every pair's source slices of b0..b2 (each [sum n_w] in the population's layout, or nullptr) and, when step is given, its Adam
+// step counts onto its destination's: one launch on the default stream, after the template's last fenced call and fenced itself,
+// with no host synchronisation.  The pairs were checked (pop_check_pairs).
+int pop_copy_sets(ramp_population* q, int32_t n_pairs, const int32_t* dst, const int32_t* src, float* b0, float* b1, float* b2, int32_t* step) {
+    if (n_pairs == 0) return RAMP_OK;
+    ramp_policy* p = q->p;
+    CUDA_TRY(cudaSetDevice(p->device));
+    if (!p->ev_done) {                                                    // until now every call kept its own synchronisation
+        CUDA_TRY(cudaDeviceSynchronize());
+        CUDA_TRY(create(p->ev_done, cudaEventDisableTiming));
+    }
+    if (!q->ev_pairs) CUDA_TRY(create(q->ev_pairs, cudaEventDisableTiming));
+    if (q->h_pairs.size() < 2 * (size_t)q->K) {
+        CUDA_TRY(q->h_pairs.alloc(2 * (size_t)q->K));
+        CUDA_TRY(q->d_pairs.alloc(2 * (size_t)q->K));
+    }
+    CUDA_TRY(cudaEventSynchronize(q->ev_pairs.get()));                    // the last copy's upload has read the staging
+    int64_t n_max = 0;
+    for (int i = 0; i < n_pairs; ++i) {
+        q->h_pairs.get()[2 * i] = dst[i];
+        q->h_pairs.get()[2 * i + 1] = src[i];
+        n_max = std::max(n_max, q->sets[dst[i]].n_w);
+    }
+    int rc;
+    if ((rc = fence_in(p, 0)) != RAMP_OK) return rc;
+    CUDA_TRY(cudaMemcpyAsync(q->d_pairs.get(), q->h_pairs.get(), sizeof(int32_t) * 2 * n_pairs, cudaMemcpyHostToDevice, 0));
+    CUDA_TRY(cudaEventRecord(q->ev_pairs.get(), 0));
+    CopySetsArgs a{};
+    a.sets = q->d_sets.get(); a.pairs = q->d_pairs.get(); a.buf[0] = b0; a.buf[1] = b1; a.buf[2] = b2; a.step = step;
+    const int chunks = (int)std::max<int64_t>(1, std::min<int64_t>((n_max + 255) / 256, (2 * p->sm_count + n_pairs - 1) / n_pairs));
+    ramp_pop_copy_sets_kernel<<<dim3(chunks, n_pairs), 256, 0, 0>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    return fence_out(p, 0);
 }
 
 }  // namespace
@@ -888,6 +981,49 @@ int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_
     if (exp_avg_out) CUDA_TRY(cudaMemcpy(exp_avg_out, q->L.adam_m.get() + o, sizeof(float) * n, cudaMemcpyDeviceToHost));
     if (exp_avg_sq_out) CUDA_TRY(cudaMemcpy(exp_avg_sq_out, q->L.adam_v.get() + o, sizeof(float) * n, cudaMemcpyDeviceToHost));
     if (step_out) CUDA_TRY(cudaMemcpy(step_out, q->L.step.get() + 2 * set + q->L.parity, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return RAMP_OK;
+}
+
+int ramp_population_set_learner_state(ramp_population_t* q, int32_t set, const float* exp_avg, const float* exp_avg_sq, int64_t n, int32_t step) {
+    int rc = pop_check_set(q, set);
+    if (rc != RAMP_OK) return rc;
+    if (!exp_avg || !exp_avg_sq) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    const PopSet& S = q->sets[set];
+    if (n != S.n_w)
+        return set_error(RAMP_ERR_BAD_ARG, "population: a learner state of %lld weights given for set %d, its configuration has %lld", (long long)n, set,
+                         (long long)S.n_w);
+    if (step < 0) return set_error(RAMP_ERR_BAD_ARG, "population: set %d: Adam step count %d < 0", set, step);
+    CUDA_TRY(cudaSetDevice(q->p->device));
+    if ((rc = pop_ensure_learner(q)) != RAMP_OK) return rc;
+    CUDA_TRY(cudaDeviceSynchronize());                                    // a learn call may still be updating them
+    CUDA_TRY(cudaMemcpy(q->L.adam_m.get() + S.w_off, exp_avg, sizeof(float) * n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(q->L.adam_v.get() + S.w_off, exp_avg_sq, sizeof(float) * n, cudaMemcpyHostToDevice));
+    const int32_t steps[2] = {step, step};
+    CUDA_TRY(cudaMemcpy(q->L.step.get() + 2 * set, steps, sizeof(steps), cudaMemcpyHostToDevice));
+    return RAMP_OK;
+}
+
+int ramp_population_copy_sets(ramp_population_t* q, int32_t n_pairs, const int32_t* dst, const int32_t* src) {
+    int rc = pop_check_pairs(q, n_pairs, dst, src);
+    if (rc != RAMP_OK) return rc;
+    LearnerBuffers& L = q->L;                                             // before the first learn call every Adam state is zero
+    if ((rc = pop_copy_sets(q, n_pairs, dst, src, q->d_w.get(), L.ready ? L.adam_m.get() : nullptr, L.ready ? L.adam_v.get() : nullptr,
+                            L.ready ? L.step.get() : nullptr)) != RAMP_OK)
+        return rc;
+    for (int i = 0; i < n_pairs; ++i) q->has_w[dst[i]] = 1;
+    if (n_pairs > 0) q->emb_valid = false;
+    return RAMP_OK;
+}
+
+int ramp_population_get_act_count(ramp_population_t* q, uint64_t* out) {
+    if (!q || !out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    *out = q->act_calls;
+    return RAMP_OK;
+}
+
+int ramp_population_set_act_count(ramp_population_t* q, uint64_t n) {
+    if (!q) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    q->act_calls = n;
     return RAMP_OK;
 }
 

@@ -183,7 +183,11 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_population_create_configs', 'ramp_population_es_create', 'ramp_population_es_destroy',
                     'ramp_population_es_round_begin', 'ramp_population_es_act', 'ramp_population_es_round_end',
                     'ramp_population_es_step', 'ramp_population_es_update', 'ramp_population_es_read', 'ramp_population_es_act_read',
-                    'ramp_population_es_state', 'ramp_population_es_reset', 'ramp_population_es_embed_ctas']
+                    'ramp_population_es_state', 'ramp_population_es_reset', 'ramp_population_es_embed_ctas',
+                    'ramp_policy_set_learner_state', 'ramp_policy_get_act_count', 'ramp_policy_set_act_count', 'ramp_es_set_state',
+                    'ramp_es_get_progress', 'ramp_es_set_progress', 'ramp_population_set_learner_state', 'ramp_population_copy_sets',
+                    'ramp_population_get_act_count', 'ramp_population_set_act_count', 'ramp_population_set_es_state',
+                    'ramp_population_get_es_progress', 'ramp_population_set_es_progress', 'ramp_population_copy_es_sets']
 
 
 def device_bytes():

@@ -144,7 +144,16 @@ def _bind(L):
                        ('ramp_population_es_act_read', [C.c_void_p] * 5),
                        ('ramp_population_es_state', [C.c_void_p, C.c_int32] + [C.c_void_p] * 3),
                        ('ramp_population_es_reset', [C.c_void_p]),
-                       ('ramp_population_es_embed_ctas', [C.c_void_p] * 3)):
+                       ('ramp_population_es_embed_ctas', [C.c_void_p] * 3),
+                       ('ramp_policy_set_learner_state', [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32]),
+                       ('ramp_population_set_learner_state', [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32]),
+                       ('ramp_es_set_state', [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32]),
+                       ('ramp_es_get_progress', [C.c_void_p] * 4),
+                       ('ramp_es_set_progress', [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]),
+                       ('ramp_population_set_es_state', [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32]),
+                       ('ramp_population_get_es_progress', [C.c_void_p, C.c_int32] + [C.c_void_p] * 3),
+                       ('ramp_population_set_es_progress', [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_void_p]),
+                       ('ramp_population_copy_es_sets', [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p])):
         getattr(L, name).restype = C.c_int
         getattr(L, name).argtypes = args
     for name in ('ramp_es_destroy', 'ramp_population_es_destroy'):
@@ -155,6 +164,23 @@ def _bind(L):
 
 def _stats(keys, out) -> Dict[str, float]:
     return {k: float(v) for k, v in zip(keys, out)}
+
+
+def _state_array(state, key: str, n: int) -> np.ndarray:
+    """state[key] as the n float32 values the library reads through a raw pointer, refusing any other count"""
+    a = np.ascontiguousarray(state[key], dtype=np.float32).ravel()
+    if a.shape != (n,):
+        raise ValueError(f'training state: {key} has {a.size} values, the set has {n} weights')
+    return a
+
+
+def _es_progress(fn, *args):
+    """(iteration, eval means [n]) from ramp_es_get_progress / ramp_population_get_es_progress"""
+    it, n = C.c_int64(), C.c_int32()
+    _engine._check(fn(*args, C.byref(it), C.byref(n), None))
+    means = np.zeros(n.value, np.float64)
+    _engine._check(fn(*args, None, None, means.ctypes.data))
+    return it.value, means
 
 
 class _GradientLearner:
@@ -189,6 +215,21 @@ class _GradientLearner:
         """zero Adam's moments and step count"""
         _engine._check(self._L.ramp_policy_learner_reset(self.policy._h))
 
+    def training_state(self) -> Dict:
+        """everything the next collect -> learn call depends on besides the config: the weights, Adam's moments and step count,
+        and the policy's act count (its draws mix it in).  np.savez of the dict is a checkpoint."""
+        m, v, step = self.adam_state()
+        return dict(weights=self.policy.get_weights(), exp_avg=m, exp_avg_sq=v, step=step, act_count=self.policy.act_count())
+
+    def load_training_state(self, state):
+        """resume from a training_state() (or np.load of its np.savez): this learner, made with the config the saving one had,
+        then computes what the saving one would have, bit for bit"""
+        n = self._L.ramp_policy_weight_count(C.byref(self.policy._cfg))
+        w, m, v = (_state_array(state, key, n) for key in ('weights', 'exp_avg', 'exp_avg_sq'))
+        self.policy.set_weights(w)
+        _engine._check(self._L.ramp_policy_set_learner_state(self.policy._h, m.ctypes.data, v.ctypes.data, n, int(state['step'])))
+        self.policy.set_act_count(int(state['act_count']))
+
 
 def _train_batch(self, env) -> Dict[str, np.ndarray]:
     """the last learn()'s train batch: per live row, t-major, the job type, action, collected log-probability, the one the gradient
@@ -220,6 +261,16 @@ class DevicePPOLearner(_GradientLearner):
         stats = _stats(STATS, out)
         self.config.kl_coeff = stats['kl_coeff']
         return stats
+
+    def training_state(self) -> Dict:
+        """_GradientLearner.training_state, plus the adapted kl_coeff and the call count (the next call shuffles with
+        config.seed + calls)"""
+        return dict(super().training_state(), kl_coeff=self.config.kl_coeff, calls=self._calls)
+
+    def load_training_state(self, state):
+        super().load_training_state(state)
+        self.config.kl_coeff = float(state['kl_coeff'])
+        self._calls = int(state['calls'])
 
     def loss_and_grad(self, batch: Dict[str, np.ndarray]):
         """PPO's loss statistics (STATS) and gradient (blob order) on one minibatch of host arrays, with no update: model [n],
@@ -271,6 +322,23 @@ class _PopulationLearner:
         _engine._check(self._L.ramp_population_learner_state(self.population._h, int(k), m.ctypes.data, v.ctypes.data, C.byref(step)))
         return m, v, step.value
 
+    def training_state(self, k: int) -> Dict:
+        """set k's training state, as the single learner's training_state(): its weights, Adam state, and the population's act
+        count, which every group's draws mix in"""
+        k = self.population._set(k)
+        m, v, step = self.adam_state(k)
+        return dict(weights=self.population.get_weights(k), exp_avg=m, exp_avg_sq=v, step=step, act_count=self.population.act_count())
+
+    def load_training_state(self, k: int, state):
+        """set k resumes from a training_state (a population's set or a single learner's of the same shape).  The act count is one
+        for every set: loading it through any set sets it for all."""
+        k = self.population._set(k)
+        n = self.population.weight_count(k)
+        w, m, v = (_state_array(state, key, n) for key in ('weights', 'exp_avg', 'exp_avg_sq'))
+        self.population.set_weights(k, w)
+        _engine._check(self._L.ramp_population_set_learner_state(self.population._h, k, m.ctypes.data, v.ctypes.data, n, int(state['step'])))
+        self.population.set_act_count(int(state['act_count']))
+
 
 class DevicePopulationPPOLearner(_PopulationLearner):
     """DevicePPOLearner for every set of a DeviceGNNPolicyPopulation at once: group k of the environment learns only from its own
@@ -296,6 +364,15 @@ class DevicePopulationPPOLearner(_PopulationLearner):
         for c, s in zip(self.configs, stats):
             c.kl_coeff = s['kl_coeff']
         return stats
+
+    def training_state(self, k: int) -> Dict:
+        """_PopulationLearner.training_state, plus configs[k]'s adapted kl_coeff and the call count (one for every set)"""
+        return dict(super().training_state(k), kl_coeff=self.configs[k].kl_coeff, calls=self._calls)
+
+    def load_training_state(self, k: int, state):
+        super().load_training_state(k, state)
+        self.configs[k].kl_coeff = float(state['kl_coeff'])
+        self._calls = int(state['calls'])
 
 
 class DeviceIMPALALearner(_GradientLearner):
@@ -637,6 +714,23 @@ class DeviceESLearner:
         """zero the ES Adam state"""
         _engine._check(self._L.ramp_es_reset(self._h))
 
+    def training_state(self) -> Dict:
+        """everything the next step depends on besides the config and the noise table: theta, the ES Adam state (m, v, t), the
+        iteration count (it keys the noise indices and act seeds) and the steps' mean eval returns (episode_reward_mean's
+        window).  np.savez of the dict is a checkpoint."""
+        m, v, t = self.adam_state()
+        it, means = _es_progress(self._L.ramp_es_get_progress, self._h)
+        return dict(weights=self.policy.get_weights(), m=m, v=v, t=t, iteration=it, eval_means=means)
+
+    def load_training_state(self, state):
+        """resume from a training_state(): this learner, made with the saving one's config and noise table, then steps as it would"""
+        n = self._L.ramp_policy_weight_count(C.byref(self.policy._cfg))
+        w, m, v = (_state_array(state, key, n) for key in ('weights', 'm', 'v'))
+        means = np.ascontiguousarray(state['eval_means'], dtype=np.float64).ravel()
+        self.policy.set_weights(w)
+        _engine._check(self._L.ramp_es_set_state(self._h, m.ctypes.data, v.ctypes.data, n, int(state['t'])))
+        _engine._check(self._L.ramp_es_set_progress(self._h, int(state['iteration']), len(means), means.ctypes.data))
+
 
 class DevicePopulationESLearner(_PopulationLearner):
     """DeviceESLearner for every set of a DeviceGNNPolicyPopulation at once (include/ramp_b200.h: ramp_population_es_*): group k
@@ -783,6 +877,33 @@ class DevicePopulationESLearner(_PopulationLearner):
     def reset(self):
         """zero every set's ES Adam state"""
         _engine._check(self._L.ramp_population_es_reset(self._handle()))
+
+    def training_state(self, k: int) -> Dict:
+        """set k's training state, as DeviceESLearner.training_state(); the iteration count is the learner's, one for every set"""
+        k = self.population._set(k)
+        m, v, t = self.adam_state(k)
+        it, means = _es_progress(self._L.ramp_population_get_es_progress, self._handle(), k)
+        return dict(weights=self.population.get_weights(k), m=m, v=v, t=t, iteration=it, eval_means=means)
+
+    def load_training_state(self, k: int, state):
+        """set k resumes from a training_state (a population's set or a DeviceESLearner's of the same shape).  The iteration
+        count is one for every set: loading it through any set sets it for all."""
+        k = self.population._set(k)
+        n = self.population.weight_count(k)
+        w, m, v = (_state_array(state, key, n) for key in ('weights', 'm', 'v'))
+        means = np.ascontiguousarray(state['eval_means'], dtype=np.float64).ravel()
+        self.population.set_weights(k, w)
+        _engine._check(self._L.ramp_population_set_es_state(self._handle(), k, m.ctypes.data, v.ctypes.data, n, int(state['t'])))
+        _engine._check(self._L.ramp_population_set_es_progress(self._handle(), k, int(state['iteration']), len(means), means.ctypes.data))
+
+    def copy_sets(self, dst, src):
+        """population.copy_sets' exploit for this learner's own state: set src[i]'s ES Adam state and mean eval returns onto set
+        dst[i], with the same checks.  The weights are the population's: population.copy_sets copies them."""
+        d = np.ascontiguousarray(dst, dtype=np.int32).ravel()
+        s = np.ascontiguousarray(src, dtype=np.int32).ravel()
+        if len(d) != len(s):
+            raise ValueError(f'{len(d)} destinations for {len(s)} sources')
+        _engine._check(self._L.ramp_population_copy_es_sets(self._handle(), len(d), d.ctypes.data, s.ctypes.data))
 
     def embed_ctas(self):
         """the last round's embedding launch: (CTAs, (ES weight set, job type) items); each CTA runs items c, c + ctas, ..."""

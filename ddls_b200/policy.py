@@ -102,6 +102,10 @@ def _bind(L):
     L.ramp_policy_get_weights.argtypes = [C.c_void_p, C.c_void_p]
     L.ramp_policy_backward.restype = C.c_int
     L.ramp_policy_backward.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 6
+    L.ramp_policy_get_act_count.restype = C.c_int
+    L.ramp_policy_get_act_count.argtypes = [C.c_void_p, C.c_void_p]
+    L.ramp_policy_set_act_count.restype = C.c_int
+    L.ramp_policy_set_act_count.argtypes = [C.c_void_p, C.c_uint64]
     L._policy_bound = True
 
 
@@ -317,6 +321,16 @@ class DeviceGNNPolicy:
         mask = _shaped('action_mask', np.ascontiguousarray(action_mask, dtype=np.uint8), (n, self.n_actions))
         return model, gf, mask
 
+    def act_count(self) -> int:
+        """act calls so far, which the draws mix in (act_draw_key's `calls`)"""
+        n = C.c_uint64()
+        _engine._check(self._L.ramp_policy_get_act_count(self._h, C.byref(n)))
+        return n.value
+
+    def set_act_count(self, n: int):
+        """resume the draws after n act calls"""
+        _engine._check(self._L.ramp_policy_set_act_count(self._h, int(n) & _M64))
+
     def act(self, env, sample: bool = False, seed: int = 0):
         """One decision per episode of a DeviceRampJobPartitioningEnvironment, written into its device action buffer; follow with
         ``env.step(None)``.  Nothing is copied to the host."""
@@ -417,7 +431,10 @@ def _bind_population(L):
                        ('ramp_population_set_weights', [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]),
                        ('ramp_population_get_weights', [C.c_void_p, C.c_int32, C.c_void_p]),
                        ('ramp_population_act', [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
-                       ('ramp_population_embed_ctas', [C.c_void_p, C.c_void_p])):
+                       ('ramp_population_embed_ctas', [C.c_void_p, C.c_void_p]),
+                       ('ramp_population_copy_sets', [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+                       ('ramp_population_get_act_count', [C.c_void_p, C.c_void_p]),
+                       ('ramp_population_set_act_count', [C.c_void_p, C.c_uint64])):
         getattr(L, name).restype = C.c_int
         getattr(L, name).argtypes = args
     L.ramp_population_destroy.restype = None
@@ -559,6 +576,26 @@ class DeviceGNNPolicyPopulation:
 
     def read(self, env):
         return self.template.read(env)
+
+    def copy_sets(self, dst: Sequence[int], src: Sequence[int]):
+        """set src[i]'s weights and torch-Adam state (DevicePopulation{PPO,IMPALA,PG}Learner's) onto set dst[i], every pair in one
+        device launch with no host synchronisation; the destinations' embeddings are recomputed by the next act or learn call.
+        Refused, naming the pair: a set outside [0, K), two sets of different configurations, a set that is the destination of two
+        pairs, a set that is both a source and a destination."""
+        d = np.ascontiguousarray(dst, dtype=np.int32).ravel()
+        s = np.ascontiguousarray(src, dtype=np.int32).ravel()
+        if len(d) != len(s):
+            raise ValueError(f'{len(d)} destinations for {len(s)} sources')
+        _engine._check(self._L.ramp_population_copy_sets(self._h, len(d), d.ctypes.data, s.ctypes.data))
+
+    def act_count(self) -> int:
+        """act calls so far, one count for every group (DeviceGNNPolicy.act_count)"""
+        n = C.c_uint64()
+        _engine._check(self._L.ramp_population_get_act_count(self._h, C.byref(n)))
+        return n.value
+
+    def set_act_count(self, n: int):
+        _engine._check(self._L.ramp_population_set_act_count(self._h, int(n) & _M64))
 
     def embed_ctas(self) -> int:
         """CTAs of the MeanPool launches; each runs the (set, job type) items c, c + ctas, ..."""

@@ -718,6 +718,13 @@ int ramp_policy_train_batch_read(ramp_policy_t* p, ramp_engine_t* eng, int32_t* 
 int ramp_policy_learner_state(ramp_policy_t* p, float* exp_avg_out, float* exp_avg_sq_out, int32_t* step_out);
 /* zeroes Adam's moments and step count */
 int ramp_policy_learner_reset(ramp_policy_t* p);
+/* loads Adam's state from HOST arrays exp_avg, exp_avg_sq [n] and the step count (checkpoint and resume): n must be
+ * ramp_policy_weight_count, step >= 0.  Allocates the learner's buffers when no learn call has yet. */
+int ramp_policy_set_learner_state(ramp_policy_t* p, const float* exp_avg, const float* exp_avg_sq, int64_t n, int32_t step);
+/* ramp_policy_act's call count, which its draws mix in (seed ^ 0x9E3779B97F4A7C15 * count); setting it makes a resumed policy
+ * draw what the uninterrupted one would */
+int ramp_policy_get_act_count(ramp_policy_t* p, uint64_t* out);
+int ramp_policy_set_act_count(ramp_policy_t* p, uint64_t n);
 
 /* ---- RLlib's IMPALA learner step on the device (ray 3.0.0.dev0, as the reference pins it): ray/rllib/algorithms/impala/
  * impala_torch_policy.py (VTraceLoss, ImpalaTorchPolicy.loss with _make_time_major and vtrace_drop_last_ts) and
@@ -883,6 +890,13 @@ int ramp_es_act_read(ramp_es_t* es, ramp_engine_t* eng, float* logits_out, float
 /* HOST copies of the ES Adam state (any may be NULL): m, v [ramp_policy_weight_count] and t; ramp_es_reset zeroes them */
 int ramp_es_state(ramp_es_t* es, float* m_out, float* v_out, int32_t* t_out);
 int ramp_es_reset(ramp_es_t* es);
+/* loads the ES Adam state from HOST arrays m, v [n] and t: n must be ramp_policy_weight_count, t >= 0 (checkpoint and resume) */
+int ramp_es_set_state(ramp_es_t* es, const float* m, const float* v, int64_t n, int32_t t);
+/* What the next steps read besides theta and the Adam state: the iteration count (ramp_es_step calls so far, unless set: it keys
+ * the noise indices and the act seeds) and every step's mean eval return so far (episode_reward_mean's report_length window).
+ * get: any pointer may be NULL (rewards_out NULL to learn *n_rewards_out first); set: iteration >= 0, rewards [n_rewards] HOST. */
+int ramp_es_get_progress(ramp_es_t* es, int64_t* iteration_out, int32_t* n_rewards_out, double* rewards_out);
+int ramp_es_set_progress(ramp_es_t* es, int64_t iteration, int32_t n_rewards, const double* rewards);
 
 /* ---- A population of K independent PPO, IMPALA or PG trainings in one environment batch.  The environment's B = K b episodes
  * are K contiguous groups of b; group k acts with weight set k and learns only from its own episodes with its own config.  Group
@@ -928,6 +942,19 @@ int ramp_population_vtrace_read(ramp_population_t* q, int32_t set, int32_t* n_ou
                                 float* vs_out, float* pg_adv_out);
 /* HOST copies of set k's Adam state, as ramp_policy_learner_state: ramp_policy_weight_count(cfgs[k]) floats each */
 int ramp_population_learner_state(ramp_population_t* q, int32_t set, float* exp_avg_out, float* exp_avg_sq_out, int32_t* step_out);
+/* loads set k's Adam state, as ramp_policy_set_learner_state: n must be ramp_policy_weight_count(cfgs[k]) */
+int ramp_population_set_learner_state(ramp_population_t* q, int32_t set, const float* exp_avg, const float* exp_avg_sq, int64_t n, int32_t step);
+/* Population-based training's exploit: for every i < n_pairs, set src[i]'s weights, Adam exp_avg / exp_avg_sq and step count onto
+ * set dst[i] (HOST [n_pairs] each), in one kernel launch (one CTA row per pair, grid-strided over the slice) on the default
+ * stream, ordered after the population's last call and before its next by the template's completion event; no host
+ * synchronisation.  Every population cache of a destination is stale afterwards: its MeanPool embeddings are recomputed by the
+ * next act or learn call.  Refused, naming the pair: a set outside [0, n_sets), two sets of different ramp_policy_config_t, a set
+ * that is the destination of two pairs, a set that is both a source and a destination (so the result does not depend on the
+ * order the pairs run in), a source without weights. */
+int ramp_population_copy_sets(ramp_population_t* q, int32_t n_pairs, const int32_t* dst, const int32_t* src);
+/* the population's act call count, which every group's draws mix in (ramp_policy_get_act_count) */
+int ramp_population_get_act_count(ramp_population_t* q, uint64_t* out);
+int ramp_population_set_act_count(ramp_population_t* q, uint64_t n);
 /* the CTAs of the population's MeanPool launches: n_sets n_models items, at most the resident CTAs, each CTA runs items
  * c, c + ctas, ... */
 int ramp_population_embed_ctas(ramp_population_t* q, int32_t* ctas_out);
@@ -968,6 +995,16 @@ int ramp_population_es_act_read(ramp_population_es_t* es, ramp_engine_t* eng, fl
 /* set k's ES Adam state, as ramp_es_state; ramp_population_es_reset zeroes every set's */
 int ramp_population_es_state(ramp_population_es_t* es, int32_t set, float* m_out, float* v_out, int32_t* t_out);
 int ramp_population_es_reset(ramp_population_es_t* es);
+/* loads set k's ES Adam state, as ramp_es_set_state: n must be ramp_policy_weight_count(cfgs[k]) */
+int ramp_population_set_es_state(ramp_population_es_t* es, int32_t set, const float* m, const float* v, int64_t n, int32_t t);
+/* ramp_es_get_progress / _set_progress for set k: the iteration count is the learner's, one for every set (setting it through
+ * any set sets it for all); the eval means are set k's own */
+int ramp_population_get_es_progress(ramp_population_es_t* es, int32_t set, int64_t* iteration_out, int32_t* n_rewards_out, double* rewards_out);
+int ramp_population_set_es_progress(ramp_population_es_t* es, int32_t set, int64_t iteration, int32_t n_rewards, const double* rewards);
+/* ramp_population_copy_sets' exploit for the ES learner's state: set src[i]'s ES Adam m and v onto set dst[i]'s in one launch of
+ * the same kernel, its t and its eval means (episode_reward_mean's window) on the host; the same checks, naming the pair.  The
+ * weights are the population's: copy them with ramp_population_copy_sets. */
+int ramp_population_copy_es_sets(ramp_population_es_t* es, int32_t n_pairs, const int32_t* dst, const int32_t* src);
 /* the last round's embedding launch: its CTAs and its (ES weight set, job type) items; each CTA runs items c, c + ctas, ... */
 int ramp_population_es_embed_ctas(ramp_population_es_t* es, int32_t* ctas_out, int32_t* items_out);
 
