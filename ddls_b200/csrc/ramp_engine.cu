@@ -187,8 +187,11 @@ struct ramp_engine {
     DeviceArray<unsigned long long> env_range_err;        // [1] ramp_env_ingest_kernel's sticky word
     DeviceArray<long long> env_range_val;                 // [B] the out-of-set action recorded with it
     Event env_ev_to_caller, env_ev_to_engine;             // the caller's stream waits for the engine's / the engine's for the caller's
-    uint32_t env_ingest_seq = 0;                          // ingest calls since the word was last cleared
+    DeviceArray<uint32_t> env_ingest_seq;                 // [2] ramp_env_ingest_kernel's call number and CTA count (EnvIngestArgs)
     bool env_range_armed = false;                         // a ramp_env_ingest ran since the word was last looked at
+    // CUDA-graph capture of the torch steps (ramp_env_ingest on a capturing stream, DESIGN.md §7 g)
+    bool env_captured = false;           // a whole step was captured: its replays leave their errors unannounced to the host
+    int64_t sized_templates = -1;        // the template count the last eager ramp_step_device sized the scratch for (-1: none)
     // standalone lookahead buffers
     DeviceArray<WorkItem> sa_chunk_items;
     DeviceArray<ChunkDesc> sa_chunks;
@@ -542,13 +545,29 @@ int env_fence(cudaEvent_t ev, cudaStream_t from, cudaStream_t to) {
     return RAMP_OK;
 }
 
+// A step captured into a CUDA graph must need nothing from the host: a replay runs no host code, so the launch shapes and buffers
+// the step uses must already be fixed by eager steps (DESIGN.md §7 g).  Checked before a captured step enqueues anything.
+int capture_refusal(ramp_engine* e) {
+    if (e->n_nonresident > 0)
+        return set_error(RAMP_ERR_BAD_ARG, "CUDA-graph capture refused: %d template(s) run on the CTA kernel, whose launch shape needs "
+                         "the step's work count on the host", e->n_nonresident);
+    if (e->sized_templates < 0)
+        return set_error(RAMP_ERR_BAD_ARG, "CUDA-graph capture refused: no eager step has run yet to size the engine's buffers");
+    if (e->sized_templates != (int64_t)e->templates.size())
+        return set_error(RAMP_ERR_BAD_ARG, "CUDA-graph capture refused: %lld template(s) were registered since the last eager step, "
+                         "so the lookahead scratch may have to grow", (long long)e->templates.size() - (long long)e->sized_templates);
+    return RAMP_OK;
+}
+
 // the range word and the events of ramp_env_ingest / ramp_env_export, made by the first of them; the word is cleared on the
 // engine stream, which both calls fence their kernels behind
 int env_io_ready(ramp_engine* e) {
     if (e->env_ev_to_engine) return RAMP_OK;
     CUDA_TRY(e->env_range_err.alloc(1));
     CUDA_TRY(e->env_range_val.alloc((size_t)e->env.B));
+    CUDA_TRY(e->env_ingest_seq.alloc(2));
     CUDA_TRY(cudaMemsetAsync(e->env_range_err.get(), 0xFF, sizeof(unsigned long long), e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(e->env_ingest_seq.get(), 0, 2 * sizeof(uint32_t), e->stream.get()));
     CUDA_TRY(create(e->env_ev_to_caller, cudaEventDisableTiming));
     CUDA_TRY(create(e->env_ev_to_engine, cudaEventDisableTiming));
     return RAMP_OK;
@@ -572,8 +591,8 @@ int env_range_raise(ramp_engine* e) {
     CUDA_TRY(cudaMemcpy(&a, e->env_range_val.get() + b, sizeof(long long), cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemsetAsync(e->env_range_err.get(), 0xFF, sizeof(unsigned long long), e->stream.get()));
     CUDA_TRY(cudaMemsetAsync(e->env.err, 0, sizeof(int32_t), e->stream.get()));
+    CUDA_TRY(cudaMemsetAsync(e->env_ingest_seq.get(), 0, sizeof(uint32_t), e->stream.get()));
     CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
-    e->env_ingest_seq = 0;
     std::string set;
     for (int k = 0; k <= e->env.max_degree; ++k) set += (k ? ", " : "") + std::to_string(k);
     return set_error(RAMP_ERR_BAD_ARG, "episode %d: Action %lld not in action set [%s]. (RJPE:314-316)", b, a, set.c_str());
@@ -840,6 +859,10 @@ int ramp_template_count(ramp_engine_t* e) { return e ? (int)e->templates.size() 
 
 int ramp_register_template(ramp_engine_t* e, const ramp_lowered_job_t* j, int32_t* id_out) {
     if (!e || !j || !id_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    // a captured step's graph holds the template count and the lookahead scratch that registering a template may change
+    if (e->env_captured)
+        return set_error(RAMP_ERR_BAD_ARG, "no template can be registered once a step was captured into a CUDA graph: the graph keeps "
+                         "the template count and the lookahead scratch a new template may regrow");
     if ((int)e->templates.size() >= e->cfg.max_templates)
         return set_error(RAMP_ERR_CAPACITY, "max_templates (%d) reached", e->cfg.max_templates);
     const int32_t N = j->n_ops, E = j->n_deps, W = j->n_workers, C = j->n_channels;
@@ -1057,14 +1080,24 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
     if (!e || !d_actions) return set_error(RAMP_ERR_BAD_ARG, "null argument");
     if (e->ep.n_jobs < 1) return set_error(RAMP_ERR_BAD_ARG, "ramp_reset must be called before ramp_step");
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    if (e->n_nonresident > 0) { int rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
-    if (e->n_resident > 0) { int rc = ensure_thread_scratch(e); if (rc != RAMP_OK) return rc; }
+    cudaStream_t st = e->stream.get();
+    // under capture (the engine stream forked into a caller's capture) the buffers are those the last eager step sized, and the
+    // step neither times itself nor reads anything back
+    bool capturing = false;
+    int rc0 = capture_status(st, &capturing);
+    if (rc0 == RAMP_OK && capturing) rc0 = capture_refusal(e);
+    if (rc0 != RAMP_OK) return rc0;
+    if (!capturing) {
+        if (e->n_nonresident > 0) { int rc = ensure_scratch(e); if (rc != RAMP_OK) return rc; }
+        if (e->n_resident > 0) { int rc = ensure_thread_scratch(e); if (rc != RAMP_OK) return rc; }
+        e->sized_templates = (int64_t)e->templates.size();
+    }
     // the overlapped path covers per-episode memo keys on resident templates; steps with engine-written actions, a template
-    // on the CTA kernel (its launch shape needs the work count on the host) or another memo mode run in order
-    if (e->overlap && e->cfg.memo_mode == RAMP_MEMO_REFERENCE && e->n_nonresident == 0 && e->n_resident > 0 && !engine_owned(e, d_actions))
+    // on the CTA kernel (its launch shape needs the work count on the host), another memo mode or a capture run in order
+    if (e->overlap && e->cfg.memo_mode == RAMP_MEMO_REFERENCE && e->n_nonresident == 0 && e->n_resident > 0 && !engine_owned(e, d_actions) &&
+        !capturing)
         return step_overlapped(e, d_actions, fuse, d_stats_out, d_ncs_out);
     const int B = e->cfg.n_episodes;
-    cudaStream_t st = e->stream.get();
     CUDA_TRY(cudaMemsetAsync(e->d_counters.get(), 0, 2 * sizeof(int32_t), st));   // n_work and work_cursor
     PlanArgs p{};
     p.actions = d_actions; p.templates = e->d_templates.get(); p.n_templates = (int32_t)e->templates.size();
@@ -1075,8 +1108,10 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
     ramp_plan_kernel<<<(B + 127) / 128, 128, 0, st>>>(p);
     e->launches++;
     if (!e->templates.empty()) {
-        if (e->ev_pending >= MAX_EVENT_PAIRS) { CUDA_TRY(cudaStreamSynchronize(st)); int rc = resolve_events(e); if (rc) return rc; }
-        CUDA_TRY(cudaEventRecord(e->ev_a[e->ev_pending].get(), st));
+        if (!capturing) {                // a replay would record the pair again with no host to resolve it
+            if (e->ev_pending >= MAX_EVENT_PAIRS) { CUDA_TRY(cudaStreamSynchronize(st)); int rc = resolve_events(e); if (rc) return rc; }
+            CUDA_TRY(cudaEventRecord(e->ev_a[e->ev_pending].get(), st));
+        }
         // memo misses on resident templates: one THREAD per lookahead, grouped on the device.  Their count stays there: idle
         // CTAs find the chunk cursor exhausted and exit.
         if (e->n_resident > 0) bucket_resident(e, e->d_items_res.get(), e->d_counters.get(), e->d_chunk_items.get(), e->d_chunks.get(), e->d_rank.get(),
@@ -1092,8 +1127,10 @@ int ramp_step_device(ramp_engine_t* e, const ramp_action_t* d_actions, int32_t f
         int rc = launch_lookaheads(e, e->d_chunks.get(), e->d_chunk_items.get(), e->n_resident > 0 ? e->res_grid : 0, e->d_items.get(), n_nonres,
                                    e->d_counters.get(), e->res.view(), e->pool.view(), e->d_stats.get(), st);
         if (rc != RAMP_OK) return rc;
-        CUDA_TRY(cudaEventRecord(e->ev_b[e->ev_pending].get(), st));
-        e->ev_pending++;
+        if (!capturing) {
+            CUDA_TRY(cudaEventRecord(e->ev_b[e->ev_pending].get(), st));
+            e->ev_pending++;
+        }
     }
     launch_step_kernel(e, d_actions, fuse, d_stats_out, d_ncs_out);
     CUDA_TRY(cudaGetLastError());
@@ -1572,7 +1609,7 @@ int ramp_env_reset(ramp_engine_t* e, const int32_t* model_of, const double* frac
     CUDA_TRY(cudaMemsetAsync(v.err, 0, sizeof(int32_t), e->stream.get()));
     if (e->env_range_err.get()) {
         CUDA_TRY(cudaMemsetAsync(e->env_range_err.get(), 0xFF, sizeof(unsigned long long), e->stream.get()));
-        e->env_ingest_seq = 0;
+        CUDA_TRY(cudaMemsetAsync(e->env_ingest_seq.get(), 0, sizeof(uint32_t), e->stream.get()));
         e->env_range_armed = false;
     }
     int rc = ramp_reset(e, arrivals, v.J);
@@ -1616,6 +1653,14 @@ int ramp_env_decide(ramp_engine_t* e, const int32_t* actions, int32_t* n_need_ho
     EnvDev& v = e->env;
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     cudaStream_t st = e->stream.get();
+    if (n_need_host_out || actions) {
+        bool capturing = false;
+        int rc = capture_status(st, &capturing);
+        if (rc != RAMP_OK) return rc;
+        if (capturing)
+            return set_error(RAMP_ERR_BAD_ARG, "CUDA-graph capture refused: a captured decision can neither take host actions nor "
+                             "hand episodes to the host's placer");
+    }
     if (actions) CUDA_TRY(cudaMemcpyAsync(v.actions, actions, sizeof(int32_t) * v.B, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemsetAsync(v.n_need_host, 0, sizeof(int32_t), st));
     ramp_env_decide_kernel<<<(v.B + 127) / 128, 128, 0, st>>>(v, e->ep, e->d_actions.get());
@@ -1635,7 +1680,7 @@ int ramp_env_decide(ramp_engine_t* e, const int32_t* actions, int32_t* n_need_ho
     if (n_need_host_out) {
         CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get(), host_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 1, v.err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        const bool range = e->env_range_armed;
+        const bool range = e->env_range_armed || e->env_captured;
         if (range) { int rc = env_range_fetch(e); if (rc != RAMP_OK) return rc; }
         CUDA_TRY(cudaStreamSynchronize(st));
         if (range) { int rc = env_range_raise(e); if (rc != RAMP_OK) return rc; }
@@ -1699,13 +1744,14 @@ int ramp_env_read(ramp_engine_t* e, double* reward, uint8_t* done, int32_t* queu
     if (obs_dynamic) CUDA_TRY(cudaMemcpyAsync(obs_dynamic, v.obs_dyn, sizeof(float) * 11 * v.B, cudaMemcpyDeviceToHost, st));
     if (action_mask) CUDA_TRY(cudaMemcpyAsync(action_mask, v.action_mask, (size_t)v.B * (v.max_degree + 1), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 4, &e->d_counters.get()->err_episode, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    if (e->env_unchecked_decide) {
-        // decisions taken without the host looking (a device-resident policy): an invalid action under apply_action_mask is sticky
-        // in `err`; episodes the tables could not decide were left unplaced, which only the LAST decide's count can show
+    if (e->env_unchecked_decide || e->env_captured) {
+        // decisions taken without the host looking (a device-resident policy, a replayed CUDA graph): an invalid action under
+        // apply_action_mask is sticky in `err`; episodes the tables could not decide were left unplaced, which only the LAST
+        // decide's count can show
         CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 2, e->has_placer ? e->place.n_host : v.n_need_host, sizeof(int32_t),
                                  cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(e->env_h_need.get() + 3, v.err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        const bool range = e->env_range_armed;
+        const bool range = e->env_range_armed || e->env_captured;
         int rc = range ? env_range_fetch(e) : RAMP_OK;
         if (rc != RAMP_OK) return rc;
         rc = ramp_sync(e);
@@ -1721,7 +1767,7 @@ int ramp_env_read(ramp_engine_t* e, double* reward, uint8_t* done, int32_t* queu
         return e->env_h_need.get()[4] != 0 ? ramp_check_status(e, nullptr, nullptr) : RAMP_OK;
     }
     {
-        const bool range = e->env_range_armed;
+        const bool range = e->env_range_armed || e->env_captured;
         int rc = range ? env_range_fetch(e) : RAMP_OK;
         if (rc != RAMP_OK) return rc;
         rc = ramp_sync(e);
@@ -1748,20 +1794,44 @@ int ramp_env_ingest(ramp_engine_t* e, const void* actions, int32_t dtype, void* 
     if (dtype != RAMP_ACTIONS_INT32 && dtype != RAMP_ACTIONS_INT64)
         return set_error(RAMP_ERR_BAD_ARG, "actions dtype %d is neither RAMP_ACTIONS_INT32 nor RAMP_ACTIONS_INT64", dtype);
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    int rc = env_io_ready(e);
-    if (rc != RAMP_OK) return rc;
     EnvDev& v = e->env;
     cudaStream_t cs = (cudaStream_t)stream, st = e->stream.get();
-    // the last ramp_env_advance wrote `done` and read `actions` (its env-step record), both on the engine stream
-    if ((rc = env_fence(e->env_ev_to_caller.get(), st, cs)) != RAMP_OK) return rc;
+    bool capturing = false;
+    int rc = capture_status(cs, &capturing);
+    if (rc != RAMP_OK) return rc;
+    if (capturing) {
+        // the step's first call: every refusal of a captured step is decided here, before anything is enqueued
+        if (!e->env_ev_to_engine)
+            return set_error(RAMP_ERR_BAD_ARG, "CUDA-graph capture refused: no eager step has run yet to make the environment's i/o buffers");
+        if ((rc = capture_refusal(e)) != RAMP_OK) return rc;
+    } else {
+        if ((rc = env_io_ready(e)) != RAMP_OK) return rc;
+        // the last ramp_env_advance wrote `done` and read `actions` (its env-step record), both on the engine stream.  A capture
+        // does not wait here: the graph's replays queue behind the caller's stream, which every eager call leaves behind the engine
+        if ((rc = env_fence(e->env_ev_to_caller.get(), st, cs)) != RAMP_OK) return rc;
+    }
     EnvIngestArgs a{};
-    a.actions = actions; a.is64 = dtype == RAMP_ACTIONS_INT64; a.B = v.B; a.max_degree = v.max_degree; a.seq = e->env_ingest_seq++;
+    a.actions = actions; a.is64 = dtype == RAMP_ACTIONS_INT64; a.B = v.B; a.max_degree = v.max_degree; a.seq = e->env_ingest_seq.get();
     a.done = v.done; a.out = v.actions; a.range_err = e->env_range_err.get(); a.range_val = e->env_range_val.get();
     ramp_env_ingest_kernel<<<(v.B + 127) / 128, 128, 0, cs>>>(a);
     e->launches++;
     CUDA_TRY(cudaGetLastError());
     e->env_range_armed = true;
-    return env_fence(e->env_ev_to_engine.get(), cs, st);       // ramp_env_decide reads what the kernel wrote
+    // ramp_env_decide reads what the kernel wrote; under capture this forks the engine stream into the caller's capture, and
+    // ramp_env_export joins it back
+    return env_fence(e->env_ev_to_engine.get(), cs, st);
+}
+
+int ramp_env_join(ramp_engine_t* e, void* stream) {
+    if (!e || !e->has_env) return set_error(RAMP_ERR_BAD_ARG, "no environment");
+    CUDA_TRY(cudaSetDevice(e->cfg.device));
+    cudaStream_t cs = (cudaStream_t)stream;
+    bool capturing = false;
+    int rc = capture_status(cs, &capturing);
+    if (rc != RAMP_OK) return rc;
+    if (capturing) return set_error(RAMP_ERR_BAD_ARG, "ramp_env_join: the stream is capturing a CUDA graph; join after the replay");
+    if ((rc = env_io_ready(e)) != RAMP_OK) return rc;
+    return env_fence(e->env_ev_to_engine.get(), cs, e->stream.get());
 }
 
 // RampJobPartitioningObservation (ramp_job_partitioning_observation.py:275, observation.py:80-131, 358-498), reward and done of the
@@ -1771,11 +1841,16 @@ int ramp_env_export(ramp_engine_t* e, void* stream, const ramp_env_export_t* out
     if (out->graph_features && !e->env_graph_static.get())
         return set_error(RAMP_ERR_BAD_ARG, "graph_features needs the per-graph statistics: call ramp_env_set_graph_static first");
     CUDA_TRY(cudaSetDevice(e->cfg.device));
-    int rc = env_io_ready(e);
-    if (rc != RAMP_OK) return rc;
     const EnvDev& v = e->env;
     cudaStream_t cs = (cudaStream_t)stream, st = e->stream.get();
-    if ((rc = env_fence(e->env_ev_to_caller.get(), st, cs)) != RAMP_OK) return rc;     // ramp_env_update_kernel's outputs
+    bool capturing = false;
+    int rc = capture_status(cs, &capturing);
+    if (rc != RAMP_OK) return rc;
+    if (capturing && !e->env_ev_to_engine)
+        return set_error(RAMP_ERR_BAD_ARG, "CUDA-graph capture refused: no eager step has run yet to make the environment's i/o buffers");
+    if (!capturing && (rc = env_io_ready(e)) != RAMP_OK) return rc;
+    // ramp_env_update_kernel's outputs; under capture this joins the engine stream back into the caller's capture
+    if ((rc = env_fence(e->env_ev_to_caller.get(), st, cs)) != RAMP_OK) return rc;
     EnvExportArgs a{};
     a.B = v.B; a.A = v.max_degree + 1; a.n_models = v.n_models;
     a.queued_model = v.queued_model; a.obs_dyn = v.obs_dyn; a.mask = v.action_mask; a.reward = v.reward; a.done = v.done;
@@ -1786,12 +1861,21 @@ int ramp_env_export(ramp_engine_t* e, void* stream, const ramp_env_export_t* out
     ramp_env_export_kernel<<<(unsigned)((n + 255) / 256), 256, 0, cs>>>(a);
     e->launches++;
     CUDA_TRY(cudaGetLastError());
+    if (capturing) {
+        // no fork is left open: the next captured step's ingest orders the engine stream again, and after a replay the engine
+        // stream's next work waits for the caller's stream through ramp_env_join or the next ingest
+        e->env_captured = true;
+        return RAMP_OK;
+    }
     return env_fence(e->env_ev_to_engine.get(), cs, st);       // the next step's kernels overwrite what the kernel reads
 }
 
 
 int ramp_enable_tick_lists(ramp_engine_t* e, int32_t cap) {
     if (!e || cap < 1) return set_error(RAMP_ERR_BAD_ARG, "ramp_enable_tick_lists: cap must be >= 1");
+    if (e->env_captured)
+        return set_error(RAMP_ERR_BAD_ARG, "ramp_enable_tick_lists: a step was captured into a CUDA graph, whose step kernels keep the "
+                         "lists' addresses");
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     CUDA_TRY(cudaStreamSynchronize(e->stream.get()));
     e->ep.tick_util = nullptr; e->ep.tick_util_n = nullptr;     // no lists until both arrays are there
@@ -1863,6 +1947,18 @@ int ramp_env_steplog_begin(ramp_engine_t* e, int32_t horizon) {
     EnvDev& v = e->env;
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     CUDA_TRY(cudaStreamSynchronize(e->stream.get()));      // no queued ramp_env_advance still writes the old record
+    if (e->env_captured && horizon != v.log_horizon)
+        return set_error(RAMP_ERR_BAD_ARG, "the env-step record of horizon %d is written by captured CUDA-graph steps; it can only be "
+                         "cleared (horizon %d), not replaced by one of horizon %d", v.log_horizon, v.log_horizon, horizon);
+    if (e->env_captured) {                                 // the same buffers, cleared: a graph's kernels keep their addresses
+        const size_t n = (size_t)horizon * v.B;
+        if (n) {
+            CUDA_TRY(cudaMemset(v.log_stats, 0, sizeof(double) * n * RAMP_ENV_STEP_STATS_LEN));
+            CUDA_TRY(cudaMemset(v.log_rewards, 0, sizeof(double) * n));
+            CUDA_TRY(cudaMemset(v.log_actions, 0, sizeof(int32_t) * n));
+        }
+        return RAMP_OK;
+    }
     v.log_horizon = 0; v.log_stats = nullptr; v.log_actions = nullptr; v.log_rewards = nullptr;
     e->steplog_stats = {}; e->steplog_actions = {}; e->steplog_rewards = {};
     if (horizon == 0) return RAMP_OK;

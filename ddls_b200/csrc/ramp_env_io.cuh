@@ -5,7 +5,8 @@
 //   ramp_env_ingest_kernel  one thread per episode: an int32 or int64 action -> the environment's int32 `actions`.  A value outside
 //                           the action set [0, max_degree] never reaches ramp_env_decide_kernel: it is written as 0 and the first
 //                           such live episode is recorded (RJPE:314-316 raises "Action a not in action set", whatever
-//                           apply_action_mask says)
+//                           apply_action_mask says).  The call number that keys the record is on the device and advanced by the
+//                           kernel, so a CUDA graph's replays number their calls as eager calls do
 //   ramp_env_export_kernel  one thread per (episode, graph_features column): RampJobPartitioningObservation's graph_features row
 //                           (ramp_job_partitioning_observation.py:275: the nine job features, the queued model's six per-graph
 //                           statistics, mounted workers and running jobs, then the action mask as 0.0 / 1.0), plus model, mask,
@@ -22,7 +23,9 @@ constexpr unsigned long long ENV_NO_RANGE_ERR = ~0ull;
 struct EnvIngestArgs {
     const void* actions;               // caller's [B] int32 (is64 = 0) or int64 (is64 = 1)
     int32_t is64, B, max_degree;
-    uint32_t seq;                      // ingest call number since the error word was last cleared
+    uint32_t* seq;                     // [2]: the ingest call number since the error word was last cleared, and the CTAs of this
+                                       // call that are done with it; the call's last CTA advances the number (a replayed CUDA
+                                       // graph runs no host code, so the number lives here)
     const uint8_t* done;               // [B] EnvDev::done
     int32_t* out;                      // [B] EnvDev::actions
     unsigned long long* range_err;     // (seq << 32) | episode of the first out-of-set action, ENV_NO_RANGE_ERR when none
@@ -31,17 +34,30 @@ struct EnvIngestArgs {
 
 __global__ void ramp_env_ingest_kernel(const EnvIngestArgs a) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= a.B) return;
-    const long long x = a.is64 ? static_cast<const long long*>(a.actions)[b] : (long long)static_cast<const int32_t*>(a.actions)[b];
-    const bool in_set = x >= 0 && x <= a.max_degree;
-    a.out[b] = in_set ? (int32_t)x : 0;
-    if (in_set || a.done[b]) return;                                                 // RJPE:314-316 looks at the live episodes
-    // the word is sticky: an error of an earlier call (stream order makes its key visible here) stays the one reported.  Within
-    // one call the lowest episode wins, and only thread b writes range_val[b]
-    const unsigned long long cur = *(volatile unsigned long long*)a.range_err;
-    if (cur != ENV_NO_RANGE_ERR && (uint32_t)(cur >> 32) != a.seq) return;
-    a.range_val[b] = x;
-    atomicMin(a.range_err, ((unsigned long long)a.seq << 32) | (unsigned)b);
+    if (b < a.B) {
+        const long long x = a.is64 ? static_cast<const long long*>(a.actions)[b] : (long long)static_cast<const int32_t*>(a.actions)[b];
+        const bool in_set = x >= 0 && x <= a.max_degree;
+        a.out[b] = in_set ? (int32_t)x : 0;
+        if (!in_set && !a.done[b]) {                                                 // RJPE:314-316 looks at the live episodes
+            // the word is sticky: an error of an earlier call (stream order makes its key visible here) stays the one reported.
+            // Within one call the lowest episode wins, and only thread b writes range_val[b]
+            const uint32_t seq = a.seq[0];
+            const unsigned long long cur = *(volatile unsigned long long*)a.range_err;
+            if (cur == ENV_NO_RANGE_ERR || (uint32_t)(cur >> 32) == seq) {
+                a.range_val[b] = x;
+                atomicMin(a.range_err, ((unsigned long long)seq << 32) | (unsigned)b);
+            }
+        }
+    }
+    // every thread of the CTA has read the number; the last CTA to get here advances it for the next call
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        if (atomicAdd(a.seq + 1, 1u) == gridDim.x - 1) {
+            a.seq[1] = 0;
+            a.seq[0] += 1;
+        }
+    }
 }
 
 struct EnvExportArgs {

@@ -35,6 +35,15 @@ inline int set_error(int code, const char* fmt, ...) {
             return set_error(RAMP_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
     } while (0)
 
+// *on := `st` is capturing a CUDA graph.  A capture that CUDA has already invalidated is an error: nothing may be enqueued into it.
+inline int capture_status(cudaStream_t st, bool* on) {
+    cudaStreamCaptureStatus s = cudaStreamCaptureStatusNone;
+    CUDA_TRY(cudaStreamIsCapturing(st, &s));
+    if (s == cudaStreamCaptureStatusInvalidated) return set_error(RAMP_ERR_CUDA, "the stream's CUDA-graph capture was invalidated");
+    *on = s == cudaStreamCaptureStatusActive;
+    return RAMP_OK;
+}
+
 // raises a kernel's cudaFuncAttributeMaxDynamicSharedMemorySize to at least `bytes`, never lowers it (ramp_engine.cu)
 cudaError_t reserve_dynamic_smem(const void* kern, size_t bytes);
 

@@ -523,6 +523,10 @@ struct ramp_policy {
     // inputs and outputs of ramp_policy_forward / ramp_policy_decide, apart from act's
     int32_t fcap = 0;
     DeviceArray<int32_t> f_model, f_actions; DeviceArray<float> f_gf, f_logits, f_value, f_logp; DeviceArray<uint8_t> f_mask;
+    // a forward captured into a CUDA graph (ramp_policy_forward_device) holds the f_* addresses for the graph's life, which the
+    // policy cannot see end: once one was captured, staging that grows is kept here until the policy is destroyed, not freed
+    bool fwd_captured = false;
+    std::vector<DeviceArray<int32_t>> kept_i32; std::vector<DeviceArray<float>> kept_f32; std::vector<DeviceArray<uint8_t>> kept_u8;
     unsigned long long act_calls = 0;
     // trajectory of a rollout segment (ramp_policy_trajectory_*): [horizon][B] per field, on the device until read
     int32_t traj_h = 0, traj_b = 0, traj_a = 0;
@@ -626,6 +630,11 @@ int stage_forward(ramp_policy* p, int32_t n) {
     if (n <= p->fcap) return RAMP_OK;
     const ramp_policy_config_t& c = p->P.c;
     p->fcap = 0;                          // until every buffer has the new size
+    if (p->fwd_captured) {
+        for (DeviceArray<int32_t>* a : {&p->f_model, &p->f_actions}) p->kept_i32.push_back(std::move(*a));
+        for (DeviceArray<float>* a : {&p->f_gf, &p->f_logits, &p->f_value, &p->f_logp}) p->kept_f32.push_back(std::move(*a));
+        p->kept_u8.push_back(std::move(p->f_mask));
+    }
     CUDA_TRY(alloc_each(n, p->f_model, p->f_actions, p->f_value, p->f_logp));
     CUDA_TRY(p->f_gf.alloc((size_t)n * c.in_features_graph));
     CUDA_TRY(alloc_each((size_t)n * c.n_actions, p->f_mask, p->f_logits));
@@ -1362,23 +1371,60 @@ int ramp_policy_set_weights_device(ramp_policy_t* p, const float* weights, int64
     return fence_out(p, st);
 }
 
+// the embeddings remade into d_emb on `st` when stale.  Once a backward has set up the learner, they are remade by the gradient
+// kernel's forward instance: the same bits, and its kept states spare the next backward a second pass over the MeanPool rounds
+// (the fused learners do the same)
+int refresh_embeddings(ramp_policy* p, cudaStream_t st) {
+    if (p->emb_valid) return RAMP_OK;
+    if (p->L.ready && p->L.gmodels_ready) {
+        int rc = launch_states(p, st, nullptr, 0, p->d_emb.get());
+        if (rc != RAMP_OK) return rc;
+        p->emb_valid = true;
+        return RAMP_OK;
+    }
+    return launch_embed(p, st);
+}
+
 int ramp_policy_forward_device(ramp_policy_t* p, void* stream, int32_t n, const void* model, int32_t model_dtype,
                                const float* graph_features, int64_t graph_features_stride, const uint8_t* action_mask,
                                float* logits_out, float* value_out) {
     if (!p || !logits_out || !value_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    int rc = device_call_ready(p, n, model, model_dtype, graph_features, graph_features_stride, action_mask);
-    if (rc != RAMP_OK || n == 0) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = stage_forward(p, n)) != RAMP_OK || (rc = fence_in(p, st)) != RAMP_OK ||
-        (rc = launch_ingest(p, st, n, model, model_dtype, graph_features, graph_features_stride, action_mask, nullptr, nullptr)) != RAMP_OK)
-        return rc;
-    // once a backward has set up the learner, stale embeddings are remade by the gradient kernel's forward instance: the same
-    // bits, and its kept states spare the next backward a second pass over the MeanPool rounds (the fused learners do the same)
-    if (!p->emb_valid && p->L.ready && p->L.gmodels_ready) {
-        if ((rc = launch_states(p, st, nullptr, 0, p->d_emb.get())) != RAMP_OK) return rc;
-        p->emb_valid = true;
+    bool capturing = false;
+    int rc = capture_status(st, &capturing);
+    if (rc != RAMP_OK) return rc;
+    if (capturing) {
+        // a replay runs no host code: the weights, embeddings and staging are what eager calls left, and the graph reads them
+        // at their addresses.  The fencing event is not used: the graph's replays are ordered on the capturing stream's successor
+        if (!p->emb_valid || !p->ev_done)
+            return set_error(RAMP_ERR_BAD_ARG, "CUDA-graph capture refused: the policy's embeddings are stale and would be remade "
+                             "inside the graph; call refresh() (ramp_policy_refresh_device) or an eager forward first");
+        if (n > p->fcap)
+            return set_error(RAMP_ERR_BAD_ARG, "CUDA-graph capture refused: %d rows are more than any eager forward staged (%d); the "
+                             "staging would have to grow", n, p->fcap);
     }
+    rc = device_call_ready(p, n, model, model_dtype, graph_features, graph_features_stride, action_mask);
+    if (rc != RAMP_OK || n == 0) return rc;
+    if ((rc = stage_forward(p, n)) != RAMP_OK || (!capturing && (rc = fence_in(p, st)) != RAMP_OK) ||
+        (rc = launch_ingest(p, st, n, model, model_dtype, graph_features, graph_features_stride, action_mask, nullptr, nullptr)) != RAMP_OK ||
+        (rc = refresh_embeddings(p, st)) != RAMP_OK)
+        return rc;
     if ((rc = launch_forward(p, st, n, 0, 0, logits_out, value_out, nullptr)) != RAMP_OK) return rc;
+    if (capturing) p->fwd_captured = true;
+    return capturing ? RAMP_OK : fence_out(p, st);
+}
+
+int ramp_policy_refresh_device(ramp_policy_t* p, void* stream) {
+    if (!p) return set_error(RAMP_ERR_BAD_ARG, "null argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    bool capturing = false;
+    int rc = capture_status(st, &capturing);
+    if (rc != RAMP_OK) return rc;
+    if (capturing) return set_error(RAMP_ERR_BAD_ARG, "ramp_policy_refresh_device cannot be captured: it runs before a replay, eagerly");
+    CUDA_TRY(cudaSetDevice(p->device));
+    if (p->emb_valid) return RAMP_OK;
+    if (!p->ev_done) CUDA_TRY(create(p->ev_done, cudaEventDisableTiming));
+    if ((rc = fence_in(p, st)) != RAMP_OK || (rc = refresh_embeddings(p, st)) != RAMP_OK) return rc;
     return fence_out(p, st);
 }
 
@@ -1386,10 +1432,14 @@ int ramp_policy_backward_device(ramp_policy_t* p, void* stream, int32_t n, const
                                 const float* graph_features, int64_t graph_features_stride, const uint8_t* action_mask,
                                 const float* grad_logits, const float* grad_value, float* grad_weights_out) {
     if (!p || !grad_logits || !grad_value || !grad_weights_out) return set_error(RAMP_ERR_BAD_ARG, "null argument");
-    int rc = device_call_ready(p, n, model, model_dtype, graph_features, graph_features_stride, action_mask);
+    cudaStream_t st = (cudaStream_t)stream;
+    bool capturing = false;
+    int rc = capture_status(st, &capturing);
+    if (rc != RAMP_OK) return rc;
+    if (capturing) return set_error(RAMP_ERR_BAD_ARG, "CUDA-graph capture refused: the policy's backward is not capturable");
+    rc = device_call_ready(p, n, model, model_dtype, graph_features, graph_features_stride, action_mask);
     if (rc != RAMP_OK) return rc;
     if (n < 1) return set_error(RAMP_ERR_BAD_ARG, "policy: backward of %d rows", n);
-    cudaStream_t st = (cudaStream_t)stream;
     if ((rc = prepare_learner(p, st, n)) != RAMP_OK || (rc = stage_host_batch(p, n)) != RAMP_OK ||
         (rc = launch_ingest(p, st, n, model, model_dtype, graph_features, graph_features_stride, action_mask, grad_logits, grad_value)) != RAMP_OK ||
         (rc = launch_backward(p, st, n, true)) != RAMP_OK)

@@ -187,7 +187,8 @@ EXPORTED_SYMBOLS = ['ramp_last_error', 'ramp_engine_create', 'ramp_engine_destro
                     'ramp_policy_set_learner_state', 'ramp_policy_get_act_count', 'ramp_policy_set_act_count', 'ramp_es_set_state',
                     'ramp_es_get_progress', 'ramp_es_set_progress', 'ramp_population_set_learner_state', 'ramp_population_copy_sets',
                     'ramp_population_get_act_count', 'ramp_population_set_act_count', 'ramp_population_set_es_state',
-                    'ramp_population_get_es_progress', 'ramp_population_set_es_progress', 'ramp_population_copy_es_sets']
+                    'ramp_population_get_es_progress', 'ramp_population_set_es_progress', 'ramp_population_copy_es_sets',
+                    'ramp_env_join', 'ramp_policy_refresh_device']
 
 
 def device_bytes():

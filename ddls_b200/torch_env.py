@@ -7,7 +7,15 @@ Every kernel that touches a tensor runs on ``torch.cuda.current_stream()`` (incl
 so a torch policy feeds the environment and reads it back at device speed, and the caching allocator never needs ``record_stream``.
 What the policy observes of a job type whatever the cluster holds -- node and edge features, edge endpoints, the six per-graph
 statistics -- is ``static``, uploaded once per job type.  With ``torch_policy`` it is one of the two modules of the package that
-import torch."""
+import torch.
+
+``step`` can be captured with ``torch.cuda.graph`` and replayed (DESIGN.md §7 g): a replay gives the bits an eager step gives.  Each
+replayed step reads its actions from the tensor captured (copy the next actions into it before ``g.replay()``) and writes the
+outputs captured (``out=`` tensors, or the graph pool's tensors the captured call returned).  A capture needs the device tables to
+decide every placement (``prewarm=True``, no model that splits its ops unevenly), every template on the thread kernel, and an
+eager step since the last template was registered; otherwise ``step`` refuses it before anything is enqueued.  ``reset()`` and
+``record_steps()`` stay eager, and a graph replays correctly after any number of resets.  Replay on the stream the environment's
+other calls then run on (torch's current stream): those calls order the engine behind it."""
 from __future__ import annotations
 
 import ctypes as C
@@ -35,6 +43,8 @@ def _bind(L):
     L.ramp_env_set_graph_static.argtypes = [C.c_void_p, C.c_void_p]
     L.ramp_env_ingest.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     L.ramp_env_export.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_Export)]
+    L.ramp_env_join.restype = C.c_int
+    L.ramp_env_join.argtypes = [C.c_void_p, C.c_void_p]
 
 
 def static_tensors(graphs, device='cpu'):
@@ -72,33 +82,54 @@ class TorchRampJobPartitioningEnvironment:
                 eng.close()
             raise
 
-    # ---- pass-throughs ------------------------------------------------------------------------------------------------
+    # ---- pass-throughs (each first orders the engine stream behind the caller's, so it sees replayed steps) ------------------
     def episode_stats(self):
+        self._join()
         return self.env.episode_stats()
 
     def decisions(self):
+        """[B] env-steps every episode has taken since reset(): the device's count, replayed steps included."""
+        self._join()
         return self.env.decisions()
 
     def record_steps(self, horizon: int):
+        """Eager only.  Once a step has been captured, the record keeps its buffers: only its own horizon is accepted (the record
+        is cleared), as captured steps write it at its address."""
+        self._join()
         self.env.record_steps(horizon)
 
     def recorded_steps(self):
+        self._join()
         return self.env.recorded_steps()
 
     def close(self):
         env = getattr(self, 'env', None)
         if env is not None:
-            env.close()
-            self.env = None
+            try:
+                self._join()                           # a replay still queued on the caller's stream ends before the free
+            finally:
+                self.env = None
+                env.close()
+
+    def _join(self):
+        _engine._check(self._L.ramp_env_join(self._h, torch.cuda.current_stream(self.device).cuda_stream))
 
     # ---- the environment -----------------------------------------------------------------------------------------------
     def check(self):
         """Synchronises and raises what the steps since the last check deferred: an action outside the action set, an action
-        the mask forbids (apply_action_mask=True), a simulation error."""
+        the mask forbids (apply_action_mask=True), a simulation error -- replayed steps' included, with an eager step's episode and
+        message.  Inside a capture it does nothing: call it after the replays."""
+        if torch.cuda.is_current_stream_capturing():
+            return
+        self._join()
         _engine._check(self._L.ramp_env_read(self._h, None, None, None, None, None))
 
     def reset(self):
-        """RampJobPartitioningEnvironment.reset for every episode; the first observation: {model, graph_features, action_mask}."""
+        """RampJobPartitioningEnvironment.reset for every episode; the first observation: {model, graph_features, action_mask}.
+        Eager only: it draws the arrival streams on the host."""
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError('CUDA-graph capture refused: reset() draws the arrival streams on the host and stays eager')
+        self._join()
         self.env.reset()
         obs = self._export(None)
         return {k: obs[k] for k in ('model', 'graph_features', 'action_mask')}
@@ -108,7 +139,10 @@ class TorchRampJobPartitioningEnvironment:
         (obs, reward, done, info): fresh tensors, or the tensors of ``out`` (a dict keyed by 'model', 'graph_features',
         'action_mask', 'reward', 'done'; any subset) written in place.  Does not synchronise when the device tables decide every
         placement (``prewarm=True``, no model splits its ops unevenly); errors then surface at ``check()`` or the next synchronising
-        call.  Otherwise the host's placer decides the rest, as ``step_device()`` does."""
+        call.  Otherwise the host's placer decides the rest, as ``step_device()`` does.
+
+        Inside ``torch.cuda.graph`` the call is captured; see the module's docstring for what a capture needs.  ``step_counter`` is
+        a host counter: it counts the captured call once and replays do not advance it (``decisions()`` is the device's count)."""
         if not isinstance(actions, torch.Tensor):
             raise TypeError(f'actions must be a torch.Tensor, not {type(actions).__name__}')
         if actions.dtype not in (torch.int32, torch.int64):
@@ -117,6 +151,9 @@ class TorchRampJobPartitioningEnvironment:
             raise ValueError(f'actions are on {actions.device}, the environment on {self.device}')
         if tuple(actions.shape) != (self.B,):
             raise ValueError(f'actions have shape {tuple(actions.shape)}, expected ({self.B},)')
+        if torch.cuda.is_current_stream_capturing() and not self.env._device_decides_everything:
+            raise RuntimeError('CUDA-graph capture refused: the device tables do not decide every placement (the environment is '
+                               "not prewarmed, or a model splits its ops unevenly), so a step may need the host's placer")
         actions = actions.contiguous()
         stream = torch.cuda.current_stream(self.device).cuda_stream
         dtype = ACTIONS_INT64 if actions.dtype == torch.int64 else ACTIONS_INT32

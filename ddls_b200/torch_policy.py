@@ -9,7 +9,15 @@ Checkpoints in the reference's GNNPolicy key set go through ``gnn_state_dict()``
 The weights are copied to the library on the device when ``(weight.data_ptr(), weight._version)`` changes, which re-embeds the
 job types; forwards at fixed weights (a rollout under ``torch.no_grad()``) run the read-out kernel alone.  A row whose model is
 outside [0, n_models) -- a finished episode's -1 -- gets logits 0 and value 0 and passes no gradient, as the head kernel rules.
-With ``torch_env`` this is one of the two modules of the package that import torch."""
+With ``torch_env`` this is one of the two modules of the package that import torch.
+
+A forward under ``torch.no_grad()`` can be captured with ``torch.cuda.graph`` (DESIGN.md §7 g): the graph gathers the rows and runs
+the read-out, reading the embeddings from a buffer the module holds for its whole life.  A replay runs no host code, so it cannot
+see a weight change: after an optimiser step (or any change to ``weight``), call ``refresh()`` -- or any eager forward -- before the
+next replay.  A capture refuses, before anything is enqueued, a forward that would upload weights or re-embed inside the graph,
+or that has more rows than an eager forward has staged; backward is not capturable.  A replay is ordered only by the stream it
+runs on: replay on the stream the module's eager calls use (torch's current stream).  Staging that a later, larger eager forward
+outgrows is kept, not freed, until ``close()``, so a captured forward's buffers stay valid for the graph's life."""
 from __future__ import annotations
 
 import ctypes as C
@@ -28,9 +36,11 @@ MODEL_INT32, MODEL_INT64 = 0, 1               # include/ramp_b200.h RAMP_MODEL_*
 
 def _bind(L):
     _policy._bind(L)
-    for name in ('ramp_policy_set_weights_device', 'ramp_policy_forward_device', 'ramp_policy_backward_device'):
+    for name in ('ramp_policy_set_weights_device', 'ramp_policy_forward_device', 'ramp_policy_backward_device',
+                 'ramp_policy_refresh_device'):
         getattr(L, name).restype = C.c_int
     L.ramp_policy_set_weights_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+    L.ramp_policy_refresh_device.argtypes = [C.c_void_p, C.c_void_p]
     L.ramp_policy_forward_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64,
                                              C.c_void_p, C.c_void_p, C.c_void_p]
     L.ramp_policy_backward_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64,
@@ -175,6 +185,18 @@ class TorchGNNPolicy(torch.nn.Module):
         logits, value = _PolicyFunction.apply(self.weight, model, gf, mask, self)
         return logits.reshape(lead + (A,)), value.reshape(lead)
 
+    def refresh(self):
+        """Eagerly, on the current stream: uploads ``weight`` and re-embeds the job types, into the buffer a captured forward reads,
+        when the weights changed since the last upload; otherwise does nothing.  Call it after an optimiser step and before the next
+        replay of a graph that captured the forward (an eager forward does the same)."""
+        if not self._h:
+            raise RuntimeError('the policy is closed')
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError('TorchGNNPolicy.refresh() runs eagerly, before a replay; it cannot be captured')
+        stream = self._stream()
+        self._upload(self.weight, stream)
+        _engine._check(self._L.ramp_policy_refresh_device(self._h, stream))
+
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
 
@@ -182,6 +204,10 @@ class TorchGNNPolicy(torch.nn.Module):
         """the library's weights := `weight` when they are not already (re-embeds on the next call)"""
         key = (weight.data_ptr(), weight._version)
         if key != self._key:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError('CUDA-graph capture refused: the weights changed since they were last uploaded (or never were), '
+                                   'so the forward would upload and re-embed inside the graph; call refresh() or an eager forward '
+                                   'before capturing')
             w = weight.detach()
             if not w.is_contiguous() or w.dtype != torch.float32 or w.device != self.device:
                 raise ValueError(f'weight must be a contiguous float32 tensor on {self.device}')
@@ -209,6 +235,8 @@ class TorchGNNPolicy(torch.nn.Module):
     def _backward_rows(self, weight, model, gf, mask, grad_logits, grad_value):
         if not self._h:
             raise RuntimeError('the policy is closed')
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError('CUDA-graph capture refused: the backward of TorchGNNPolicy is not capturable')
         n, A = model.shape[0], self.n_actions
         grad = torch.empty(weight.shape, dtype=torch.float32, device=self.device)
         if not n:

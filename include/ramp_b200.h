@@ -545,6 +545,25 @@ int ramp_env_set_graph_static(ramp_engine_t* eng, const float* graph_static);
 int ramp_env_ingest(ramp_engine_t* eng, const void* actions, int32_t dtype, void* stream);
 int ramp_env_export(ramp_engine_t* eng, void* stream, const ramp_env_export_t* out);
 
+/* ---- CUDA-graph capture of a step (DESIGN.md §7 g).  ramp_env_ingest, ramp_env_decide(eng, NULL, NULL, NULL), ramp_env_advance
+ * and ramp_env_export may be captured into a CUDA graph on `stream` (e.g. inside torch.cuda.graph): each call asks
+ * cudaStreamIsCapturing of the stream it runs on, and there is no flag to set.  Under capture a step records no timing event, never
+ * synchronises, allocates nothing and reads nothing back; the ingest's fence forks the engine stream into the capture and the
+ * export's joins it back, and the export leaves no fork open.  ramp_env_ingest refuses to start a captured step (RAMP_ERR_BAD_ARG,
+ * nothing enqueued) when a replay would need the host: a template on the CTA kernel (its launch shape needs a work count on the
+ * host), no eager step yet (the i/o buffers and lookahead scratch are sized by eager steps), or a template registered since the
+ * last eager step (the scratch may have to grow).  ramp_env_decide refuses host actions and need_host_out under capture.  The
+ * caller refuses a capture when the device tables do not decide every placement.  Replays advance the ingest call number on
+ * the device, so their errors are those of eager steps: the next ramp_env_read raises them.  Once a step was captured, the
+ * env-step record (ramp_env_steplog_begin) keeps its buffers: it can be cleared at its horizon, not replaced; and
+ * ramp_register_template and ramp_enable_tick_lists are refused, as the graph keeps the template count, the lookahead scratch
+ * and the lists' addresses.  Host-set values a
+ * captured launch carries (ramp_set_limits, the record's horizon) are those of the capture.
+ * ramp_env_join makes the engine stream wait for the work queued on `stream` so far, without a synchronisation: after a replay
+ * on `stream`, call it before engine-stream calls (ramp_env_read, ramp_env_reset, the statistics) so they see the replay.
+ * Refused while `stream` captures. */
+int ramp_env_join(ramp_engine_t* eng, void* stream);
+
 
 /* ---- the GNN policy forward on the device (SURVEY.md 8f-3): GNNPolicy.forward (ml_models/policies/gnn_policy.py:137-296) =
  * num_rounds MeanPool message-passing rounds over the queued job's graph (ml_models/models/mean_pool.py:107-150, gnn.py:84-92),
@@ -662,6 +681,16 @@ int ramp_policy_forward_device(ramp_policy_t* p, void* stream, int32_t n, const 
 int ramp_policy_backward_device(ramp_policy_t* p, void* stream, int32_t n, const void* model, int32_t model_dtype,
                                 const float* graph_features, int64_t graph_features_stride, const uint8_t* action_mask,
                                 const float* grad_logits, const float* grad_value, float* grad_weights_out);
+/* CUDA-graph capture: ramp_policy_forward_device may be captured on `stream` (detected with cudaStreamIsCapturing).  Under capture
+ * it launches the row gather and the read-out only, reading the embeddings from the buffer the policy holds for its whole life,
+ * and does not use the fencing event: replays are ordered by the stream they run on.  It refuses (RAMP_ERR_BAD_ARG, nothing
+ * enqueued) when the embeddings are stale, which would put a re-embed inside the graph, and when n is more rows than an eager call
+ * has staged.  ramp_policy_backward_device refuses any capture.  A replay cannot see new weights:
+ * ramp_policy_refresh_device re-embeds, eagerly on `stream` and into the same buffer, when the embeddings are stale (after
+ * ramp_policy_set_weights_device), and does nothing otherwise; call it before the next replay.  Once a forward was captured,
+ * staging that a later, larger call outgrows is kept until ramp_policy_destroy instead of being freed, so the graph's addresses
+ * stay valid. */
+int ramp_policy_refresh_device(ramp_policy_t* p, void* stream);
 
 /* PPO's settings (RLlib PPOConfig names; scripts/ramp_job_partitioning_configs/algo/ppo.yaml holds the reference's values) */
 typedef struct {
